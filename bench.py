@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — fwd+bwd views/sec of the rasterizer hot path (BASELINE.json metric) on N B200s.
+"""bench.py — fwd+bwd views/sec of the rasterizer hot path (BASELINE.json metric) on N H100s.
 
   python bench.py --gpus 1 --steps 50 --warmup 10                      # our kernels
   python bench.py --impl reference --gpus 1 --steps 20 --warmup 3      # reference CUDA kernels
@@ -10,15 +10,16 @@ A "step" is one full forward + backward of the differentiable rasterizer for one
 (1M Gaussians, 800x800, S=5 feature channels, SH degree 3, seeded synthetic `shell-v1` scene,
 8-camera ring, fixed random cotangents); with N GPUs the views of a step are sharded one per GPU
 and a single NCCL all-reduce of the per-Gaussian parameter gradients follows backward (weak
-scaling).  Prints ONE JSON line on rank 0.
+scaling).  Prints ONE JSON line on rank 0.  `--steps K` is the number of timed steps of every timed
+loop; `--dump-outputs DIR` writes what the last timed step computed (rank 0) as DIR/<name>.npy.
 
 Keys: `value` = whole-job views/s with inputs resident in HBM (C-ABI level operator calls);
 `e2e` = the same step through the reference-facing public API (GaussianRasterizer module +
 autograd) including, every step, the host->device copy of that step's inputs from pinned memory
 (camera + ground-truth image) and the device->host read of the loss; `roofline` = dominant kernel
-vs the measured HBM peak (MEASURED_PEAKS.json); `cpu_baseline` = the CPU oracle port timed on a
+vs the HBM peak (MEASURED_PEAKS.json if present, else the H100 SXM data-sheet figure); `cpu_baseline` = the CPU oracle port timed on a
 bounded sample (rank 0, N=1 only).  `--impl reference` times the UNMODIFIED reference CUDA kernels
-(oracle/_ref, built from /root/reference by oracle/build_ref.sh) on the same GPU; when that build
+(oracle/_ref, built from the reference sources by oracle/build_ref.sh) on the same GPU; when that build
 is absent it falls back to the CPU oracle port.
 """
 import argparse
@@ -38,14 +39,12 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 HEADLINE = dict(P=1_000_000, W=800, H=800, S=5, views=8, recipe="shell-v1", seed=0)
-# DRAM bytes per launch of the compositors at the headline config, from ncu --set full (profiles/)
-NCU_TRAFFIC = {"composite_bwd": 63854848 + 1705728, "composite_fwd": 48878592 + 4990208}
 STAGES = ["project", "depth_sort", "bin_count", "bin_offsets", "bin_scatter", "composite_fwd",   # bin_scatter includes tile_order + block_mask
           "surface_normal", "composite_bwd", "project_bwd"]
 
 
 class ClockSampler:
-    """nvidia-smi sampler running DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler running DURING the timed region: SM clock and throttle reasons."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -115,7 +114,7 @@ def workload_config(cfg, num_rendered):
     return {"workload": f"rasterizer fwd+bwd, {cfg['recipe']} seed {cfg['seed']}, P={cfg['P']}, {cfg['W']}x{cfg['H']}, S={cfg['S']}, SH deg 3, "
                         f"{cfg['views']}-camera ring, one view per GPU per step, fixed random cotangents",
             "P": cfg["P"], "W": cfg["W"], "H": cfg["H"], "S": cfg["S"], "num_rendered": num_rendered,
-            "l2": "inputs larger than L2 (236 MB Gaussian parameters + ~190 MB binning per step vs 126 MB L2)"}
+            "l2": "inputs larger than L2 (236 MB Gaussian parameters + ~190 MB binning per step vs 50 MB L2)"}
 
 
 def measured_peak():
@@ -125,7 +124,35 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
+
+
+DUMP_ROWS = 32768                  # per-Gaussian rows written by --dump-outputs
+DUMP_IMAGE_BYTES = 48 << 20        # images above this are written at a fixed sample of pixels
+
+
+def dump_outputs(outdir, out, grads, P):
+    """--dump-outputs: what the last timed step returned to its caller, as float32 .npy files (num_rendered as
+    float64).  Images [C, H*W] in full up to DUMP_IMAGE_BYTES, else at a fixed, seeded pixel sample (pixels.npy);
+    per-Gaussian arrays (weights, radii, gradients) at a fixed, seeded sample of DUMP_ROWS rows (rows.npy)."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    arrays = {"num_rendered": np.array([int(out[0])], np.float64)}
+    images = dict(zip(("n_contrib", "color", "opacity", "depth", "feature", "normal", "surface_xyz"), out[1:8]))
+    images = {n: t.reshape(-1 if t.dim() == 2 else t.shape[0], t.shape[-2] * t.shape[-1]) for n, t in images.items()}
+    hw = images["color"].shape[1]
+    if sum(t.numel() for t in images.values()) * 4 > DUMP_IMAGE_BYTES:
+        pix = np.sort(np.random.default_rng(1).choice(hw, DUMP_IMAGE_BYTES // (4 * sum(t.shape[0] for t in images.values())), replace=False))
+        arrays["pixels"] = pix.astype(np.float64)
+        images = {n: t[:, torch.from_numpy(pix).to(t.device)] for n, t in images.items()}
+    rows = np.sort(np.random.default_rng(0).choice(P, min(P, DUMP_ROWS), replace=False))
+    arrays["rows"] = rows.astype(np.float64)
+    ri = torch.from_numpy(rows)
+    per_gaussian = {"weights": out[8], "radii": out[9], **{"grad_" + n: t for n, t in grads.items()}}
+    for n, t in {**images, **{n: t[ri.to(t.device)] for n, t in per_gaussian.items()}}.items():
+        arrays[n] = t.detach().float().cpu().numpy()
+    for n, a in arrays.items():
+        np.save(os.path.join(outdir, n + ".npy"), a)
 
 
 def make_inputs(cfg, device):
@@ -184,7 +211,7 @@ def bench_ours(args, cfg, rank, local, world):
         c = cam["c"]
         out = C.rasterize_gaussians(bg, means3D, feats, E, opac, scales, rots, 1.0, E, cam["view"], cam["proj"],
                                     c.tanfovx, c.tanfovy, c.cx, c.cy, H, W, shs, 3, cam["pos"], False, True, False)
-        stats["R"] = out[0]; stats["radii"] = out[9]
+        stats["R"] = out[0]; stats["radii"] = out[9]; stats["out"] = out
         C.rasterize_gaussians_backward(bg, means3D, feats, out[9], E, scales, rots, 1.0, E, cam["view"], cam["proj"],
                                        c.tanfovx, c.tanfovy, dcot["color"], dcot["opacity"], dcot["depth"],
                                        dcot["feature"], shs, 3, cam["pos"], out[10], out[0], out[11], out[12],
@@ -245,6 +272,10 @@ def bench_ours(args, cfg, rank, local, world):
     blocks = stats["blocks"]
     clocks = sampler.stop() if sampler else None
     value = world * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        # what the step hands its caller: the exchanged gradients (the averaged SH gradient, not the per-view factor)
+        dump_outputs(args.dump_outputs, stats["out"], getattr(bucket, "grads", bucket.views), P)
+    stats.pop("out")
 
     # ---- e2e: public API (module + autograd), per-step host inputs from pinned memory -------
     params = [t.clone().requires_grad_(True) for t in (means3D, opac, shs, scales, rots, feats)]
@@ -307,7 +338,7 @@ def bench_ours(args, cfg, rank, local, world):
         loss_host[i % 64:i % 64 + 1].copy_(loss.detach().reshape(1), non_blocking=True)
 
     leaf_bucket = rdist.LeafGradBucket([params[k] for k in (0, 1, 3, 4, 5)], dev, symmetric=exchange_kind == "p2p") if factored else None
-    e_steps = max(50, args.steps)
+    e_steps = args.steps
     # (1) the path an UNCHANGED caller of the reference surface gets: synchronous instance count (one host wait per forward,
     #     like the reference's own cudaMemcpy at rasterizer_impl.cu:291).  Its warm-up also teaches the deferred path the counts.
     set_deferred_count(False)
@@ -331,7 +362,7 @@ def bench_ours(args, cfg, rank, local, world):
         achieved = ab[dom] / (stage[dom] * 1e-3) / 1e9
         step_alg = sum(ab.values())
         res = {
-            "metric": "fwd+bwd views/sec at 1M Gaussians 800x800, 1/2/4/8 B200; HBM GB/s vs peak" if cfg == HEADLINE else "fwd+bwd views/sec (non-headline config)",
+            "metric": "fwd+bwd views/sec at 1M Gaussians 800x800, 1/2/4/8 H100; HBM GB/s vs peak" if cfg == HEADLINE else "fwd+bwd views/sec (non-headline config)",
             "value": value, "unit": "views/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "ms_per_step_block_median": statistics.median(blocks),
             "ms_per_step_blocks": blocks, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -356,9 +387,7 @@ def bench_ours(args, cfg, rank, local, world):
             "clocks": clocks,
             "stage_ms": stage,
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": NCU_TRAFFIC.get(dom) if cfg == HEADLINE else None,
-                         "traffic_source": "dram__bytes_read.sum + dram__bytes_write.sum of one ncu --set full capture per launch (profiles/r02_ncu_composite_*_final.md)",
-                         "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "alg_bytes_per_launch": ab[dom],
                          "step_alg_bytes": step_alg, "step_frac_of_peak": step_alg / (ms / args.steps * 1e-3) / 1e9 / peak},
         }
@@ -398,7 +427,7 @@ def bench_reference(args, cfg, rank, local, world):
     if rank != 0:
         return None
     from oracle import ref_gpu
-    base = {"impl": "reference", "metric": "fwd+bwd views/sec at 1M Gaussians 800x800, 1/2/4/8 B200; HBM GB/s vs peak" if cfg == HEADLINE else "fwd+bwd views/sec (non-headline config)",
+    base = {"impl": "reference", "metric": "fwd+bwd views/sec at 1M Gaussians 800x800, 1/2/4/8 H100; HBM GB/s vs peak" if cfg == HEADLINE else "fwd+bwd views/sec (non-headline config)",
             "unit": "views/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic"}
     P, S, W, H = cfg["P"], cfg["S"], cfg["W"], cfg["H"]
@@ -456,9 +485,9 @@ def bench_reference(args, cfg, rank, local, world):
         v = args.steps / (ms / 1e3)
         base.update({"value": v, "ms_per_step": ms / args.steps, "clocks": clocks,
                      "config": workload_config(cfg, int(o["num_rendered"])),
-                     "arm": {"impl": f"{kind}; sm_100 build of /root/reference, same scene / cameras / cotangents"},
+                     "arm": {"impl": f"{kind}; sm_90 build of the reference, same scene / cameras / cotangents"},
                      "cpu_baseline": {"value": v, "unit": "views/s", "cores": os.cpu_count(), "kind": "reference",
-                                      "sample": "not a CPU run: the reference has no CPU rasterizer; this is its own CUDA build timed on the same B200 (north_star), full workload, 8-camera ring"},
+                                      "sample": "not a CPU run: the reference has no CPU rasterizer; this is its own CUDA build timed on the same GPU (north_star), full workload, 8-camera ring"},
                      "e2e": {"value": v, "unit": "views/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}})
         return base
     # fallback: CPU oracle port on a bounded sample
@@ -480,7 +509,7 @@ def main():
 
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 200; 30 for --workload stage2)")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--P", type=int, default=None)
@@ -493,9 +522,13 @@ def main():
                          "configs #4 (1 GPU: 1.5M / 1600x1200) / #5 (N GPUs: 2M / 1920x1080), printed with \"workload\": \"stage2\"")
     ap.add_argument("--ref-shim", action="store_true", help="reference arm: force the raw-pointer shim instead of the stock wrapper + pybind module")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (images, sampled per-Gaussian rows and gradients) as DIR/<name>.npy")
     ap.add_argument("--exchange", default="auto", choices=["auto", "p2p", "factored", "dense"],
                     help="N > 1: gradient exchange per step (DESIGN.md section 5)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "headline" or args.impl != "ours"):
+        ap.error("--dump-outputs writes the outputs of this project's headline step: it needs --workload headline --impl ours")
     args.warmup = max(args.warmup, 3)
     cfg = dict(HEADLINE)
     for k in ("P", "W", "H", "S"):
@@ -509,7 +542,7 @@ def main():
         for k in ("P", "W", "H", "N"):
             if getattr(args, k) is not None:
                 cfg2[k] = getattr(args, k)
-        if args.steps == 200:
+        if args.steps is None:
             args.steps = 30                     # a stage-2 step is ~10x a headline step
         if args.impl == "reference":
             if rank == 0:
@@ -529,6 +562,8 @@ def main():
             tdist.barrier()
             tdist.destroy_process_group()
         return
+    if args.steps is None:
+        args.steps = 200
     if args.impl == "reference":
         if rank == 0:
             emit(bench_reference(args, cfg, rank, local, world))

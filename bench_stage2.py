@@ -12,7 +12,7 @@ per GPU on N GPUs), assembled exactly like the reference assembles it:
                                          run once before the loop and reported beside the step
 
 Two arms over the SAME seeded model, cameras and targets:
-  * ours       — fused shading kernels, B200 rasterizer through the GaussianRasterizer mirror (deferred
+  * ours       — fused shading kernels, this project's rasterizer through the GaussianRasterizer mirror (deferred
                  count), FusedAdam, LBVH bake with in-kernel direction sampling;
   * reference  — the reference's PyTorch rendering_equation formulation (oracle/oracle_shading.py, pinned
                  to the reference's own function bodies), its own rasterizer (stock wrapper + pybind module
@@ -386,6 +386,6 @@ def run_reference(args, cfg, rank, local, world):
             "phase_ms_median": phases,
             "bake": {"seconds": bake_s, "rays": P * N, "mrays_per_s": P * N / bake_s / 1e6, "what": bake_kind},
             "cpu_baseline": {"value": v, "unit": "views/s", "cores": os.cpu_count(), "kind": "reference",
-                             "sample": "not a CPU run: the reference has no CPU path for this step; its own CUDA kernels + PyTorch on the same B200"},
+                             "sample": "not a CPU run: the reference has no CPU path for this step; its own CUDA kernels + PyTorch on the same GPU"},
             "e2e": {"value": v, "unit": "views/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "peak_mem_GB": torch.cuda.max_memory_allocated(dev) / 1e9}

@@ -1,5 +1,5 @@
 /*
- * r3dg_b200 — C ABI of the B200-native (sm_100a) relightable-Gaussian rasterizer hot path.
+ * r3dg_b200 — C ABI of the H100-native (sm_90a) relightable-Gaussian rasterizer hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b): plain pointers and sizes, no torch types, an
  * explicit CUDA stream, caller-allocated memory, no hidden allocation, errors returned as
@@ -384,16 +384,16 @@ int r3dg_prof_end(float* stage_ms /* [9] */, int* fwd_calls, int* bwd_calls);
  *                     2 warp-private tagged copies, 1 shared-memory atomics (default),
  *                     0 global atomics; larger textures fall back to the lower modes
  *   "composite_bulk"  1 = per-lane cp.async.bulk record staging in the forward compositor
- *                     (measured slower, profiles/r02_composite_bulk_staging.md), 0 (default)
+ *                     (an experiment; the register prefetch is the default), 0 (default)
  *   "composite_fwd_ctas" / "composite_bwd_ctas"  resident CTAs per SM of the two compositors,
  *                     enforced with dynamic shared memory; 0 (default) = whatever fits
- *                     (profiles/r02_warp_timing.md: every lower setting is slower)
+ *                     (lower settings trade occupancy for faster heaviest warps)
  * Initial values can also be given by the environment (R3DG_SHADE_GROUP, R3DG_SHADE_ENV_MODE,
  * R3DG_SHADE_FWD_VARIANT, R3DG_SHADE_BWD_VARIANT, R3DG_COMPOSITE_BULK, R3DG_FWD_CTAS,
  * R3DG_BWD_CTAS). */
 int r3dg_tune(const char* key, int value, int* previous);
 
-/* Library identification: returns a static string such as "r3dg_b200 0.1 sm_100a". */
+/* Library identification: returns a static string such as "r3dg_b200 0.1 sm_90a". */
 const char* r3dg_version(void);
 
 #ifdef __cplusplus

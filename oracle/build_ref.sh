@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# TEST INFRASTRUCTURE.  Builds the UNMODIFIED reference CUDA kernels for sm_100 into
+# TEST INFRASTRUCTURE.  Builds the UNMODIFIED reference CUDA kernels for sm_90 into
 # oracle/_ref/ (git-ignored; travels to the GPU box with gpurun).  Sources are compiled
 # where they lie under /root/reference; nothing is copied into the repo.  Only the BVH
 # builder needs a one-line patched copy (SURVEY.md §8c-addendum), generated into
@@ -11,7 +11,7 @@ OUT="$HERE/_ref"
 [ -d "$REF" ] || { echo "[build_ref] $REF absent — skipping (prebuilt oracle/_ref is used if present)"; exit 0; }
 mkdir -p "$OUT"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-ARCH="-gencode arch=compute_100,code=sm_100"
+ARCH="-gencode arch=compute_90,code=sm_90"
 # Flags = the reference's own (r3dg-rasterization/setup.py:30-33: -O3 + glm include) plus
 # what torch's BuildExtension always adds, plus the two header papering pre-includes.
 TORCHISH="-D__CUDA_NO_HALF_OPERATORS__ -D__CUDA_NO_HALF_CONVERSIONS__ -D__CUDA_NO_BFLOAT16_CONVERSIONS__ -D__CUDA_NO_HALF2_OPERATORS__ --expt-relaxed-constexpr -std=c++17"

@@ -2,7 +2,7 @@
 # TEST INFRASTRUCTURE.  Builds the reference's OWN torch extensions — `r3dg_rasterization._C`
 # (r3dg-rasterization/setup.py:21-33: rasterizer_impl.cu forward.cu backward.cu rasterize_points.cu
 # ext.cpp) and `bvh_tracing._C` (bvh/setup.py:12-26: bvh.cu trace.cu construct.cu bindings.cpp) —
-# for sm_100 with the reference's flags, from the sources where they lie under /root/reference, into
+# for sm_90 with the reference's flags, from the sources where they lie under /root/reference, into
 # oracle/_ref/ext/ (git-ignored; travels to the GPU box with gpurun), and drops the reference's two
 # Python wrapper files (+ the two utils modules they import) into oracle/_ref/py/.
 #
@@ -33,7 +33,7 @@ print(" ".join("-I" + p for p in c.include_paths("cuda")) + " -I" + sysconfig.ge
 EOF
 )
 TORCH_LIB=$($PY -c "import os, torch; print(os.path.join(os.path.dirname(torch.__file__), 'lib'))" 2>/dev/null)
-ARCH="-gencode arch=compute_100,code=sm_100"
+ARCH="-gencode arch=compute_90,code=sm_90"
 # what torch's BuildExtension adds to every nvcc line
 TORCHISH="-D__CUDA_NO_HALF_OPERATORS__ -D__CUDA_NO_HALF_CONVERSIONS__ -D__CUDA_NO_BFLOAT16_CONVERSIONS__ -D__CUDA_NO_HALF2_OPERATORS__ --expt-relaxed-constexpr -std=c++17 -DTORCH_API_INCLUDE_EXTENSION_H -D_GLIBCXX_USE_CXX11_ABI=1"
 RAS="$REF/r3dg-rasterization"
@@ -54,7 +54,7 @@ if [ ! -f "$OUT/ext/r3dg_rasterization/_C.so" ]; then
 fi
 
 if [ ! -f "$OUT/ext/bvh_tracing/_C.so" ]; then
-  echo "[build_ref_ext] bvh_tracing._C (construct.cu: the one-line `-> aabb_type` patched copy, SURVEY §8c-addendum)"
+  echo "[build_ref_ext] bvh_tracing._C (construct.cu: the one-line '-> aabb_type' patched copy, SURVEY §8c-addendum)"
   sed '166s/rhs)[[:space:]]*{/rhs) -> aabb_type {/' "$BVH/src/construct.cu" > "$OUT/construct_patched.cu"
   diff "$BVH/src/construct.cu" "$OUT/construct_patched.cu" || true
   $NVCC $ARCH -O3 $TORCHISH -DTORCH_EXTENSION_NAME=_C --expt-extended-lambda -I"$BVH/include" $TORCH_INC -Xcompiler -fPIC \

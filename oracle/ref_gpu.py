@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — not product code.
 
 ctypes driver for oracle/_ref/libref_raster.so: the UNMODIFIED reference rasterizer kernels
-(/root/reference/r3dg-rasterization/cuda_rasterizer/*.cu) compiled for sm_100 by
+(/root/reference/r3dg-rasterization/cuda_rasterizer/*.cu) compiled for sm_90 by
 oracle/build_ref.sh behind the raw-pointer shim oracle/ref_shim_raster.cu.  It is the parity
 oracle on the GPU box (bit-exact checks of radii / point_list / ranges / n_contrib, tolerance
 checks of images and gradients) and the timed `--impl reference` arm of bench.py.
@@ -216,7 +216,7 @@ def ref_bvh_trace_opacity(nodes, aabbs, rays_o, rays_d, means3D, covs3D, opaciti
 # The STOCK code path: the reference's own Python wrappers (git-ignored copies under oracle/_ref/py,
 # made by oracle/build_ref_ext.sh) over either the reference's own pybind modules (oracle/_ref/ext)
 # or this repo's drop-in packages (dropin/) — the latter is how tests/test_dropin_gpu.py proves that
-# the reference's files run unmodified on the B200 kernels.
+# the reference's files run unmodified on this project's kernels.
 # ----------------------------------------------------------------------------------------------
 import importlib.util
 import sys
@@ -314,7 +314,7 @@ def reference_rasterizer():
             return dict(num_rendered=num_rendered, num_contrib=num_contrib, color=color, opacity=opac, depth=depth, feature=feature,
                         radii=radii, means2D=means2D)
         return raster, ("the reference's own rasterizer, stock code path: gaussian_renderer/r3dg_rasterization.py -> r3dg_rasterization._C "
-                        "(rasterize_points.cu + cuda_rasterizer/*.cu built for sm_100 by oracle/build_ref_ext.sh)")
+                        "(rasterize_points.cu + cuda_rasterizer/*.cu built for sm_90 by oracle/build_ref_ext.sh)")
     ref = RefRasterizer()
 
     def raster(cam, cd, bg, xyz, opacity, shs, scales, rotations, features):
@@ -335,7 +335,7 @@ def reference_update_visibility(xyz, scaling, rotation, icov, opacity, normal, s
     if ext_available("bvh"):
         mod = load_reference_wrapper("bvh", "ref")
         rt = mod.RayTracer(xyz, scaling, rotation)
-        kind = "reference RayTracer (bvh/__init__.py) + bvh_tracing._C built for sm_100, PyTorch direction sampling, the reference's chunk loop"
+        kind = "reference RayTracer (bvh/__init__.py) + bvh_tracing._C built for sm_90, PyTorch direction sampling, the reference's chunk loop"
         trace = lambda o, d: rt.trace_visibility(o, d, xyz, icov, opacity, normal)["visibility"]
     else:
         nodes, aabbs, _ = ref_bvh_create(xyz, scaling, rotation)

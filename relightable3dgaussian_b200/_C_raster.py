@@ -47,7 +47,7 @@ class DeferredCount:
     """`num_rendered` of a forward whose read-back has not been waited for yet (opt-in, see
     rasterizer.set_deferred_count).  int() / resolve() waits for the forward's event.  The binning
     buffer of a deferred forward is sized _HEADROOM x the largest count any view of this shape has
-    produced (HBM is plentiful on B200: 6 B per instance); should a view still overflow it, nothing
+    produced (HBM is plentiful on an 80 GB H100: 6 B per instance); should a view still overflow it, nothing
     out of bounds was written, `overflowed` is set and the autograd backward re-runs the forward
     with the exact size before differentiating (rasterizer._RasterizeGaussians.backward)."""
 

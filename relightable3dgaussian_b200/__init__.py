@@ -1,4 +1,4 @@
-"""r3dg-b200: the Relightable3DGaussian renderer hot path on B200 (sm_100a).
+"""r3dg-b200: the Relightable3DGaussian renderer hot path on H100 (sm_90a).
 
 Host mirrors of the reference's operator surface over one C-ABI CUDA library (include/r3dg_b200.h):
 rasterizer (GaussianRasterizer), shading (rendering_equation), raytracer (RayTracer / visibility bake), optim

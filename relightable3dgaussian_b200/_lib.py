@@ -1,7 +1,7 @@
 """ctypes binding of libr3dg_b200.so (C ABI: include/r3dg_b200.h).
 
 There is NO fallback: if the CUDA library is missing or does not export a declared symbol this
-module raises at import time, so a GPU run can never silently use anything but the sm_100a
+module raises at import time, so a GPU run can never silently use anything but the sm_90a
 kernels.
 """
 import ctypes

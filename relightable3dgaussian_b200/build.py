@@ -1,4 +1,4 @@
-"""In-tree build of libr3dg_b200.so with nvcc for sm_100a (no torch headers, so a full rebuild is
+"""In-tree build of libr3dg_b200.so with nvcc for sm_90a (no torch headers, so a full rebuild is
 about a minute; nvcc cross-compiles without a GPU).  `python -m relightable3dgaussian_b200.build`."""
 import os
 import subprocess
@@ -10,7 +10,8 @@ CSRC = os.path.join(HERE, "csrc")
 ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "libr3dg_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC] + os.environ.get("R3DG_NVCC_DEFS", "").split()
 
 
@@ -18,10 +19,8 @@ FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std
 # without FMA contraction the fused kernel reproduces that rounding instead of a differently
 # (if slightly better) rounded result of an ill-conditioned GGX denominator.
 # adam.cu: flush-to-zero arithmetic.  Real gradients span the whole fp32 range (g^2 of a barely visible Gaussian is a
-# denormal); IEEE sqrt / division take a slow subroutine for denormal operands, and one such lane stalls its warp:
-# measured 1.33 ms inside the stage-2 step vs 0.70 ms on well-scaled data (profiles/r02_launches_stage2.csv vs
-# r02_stage3_bvh2.jsonl).  With -ftz the results are unchanged for every normal number (torch's own CUDA kernels are
-# compiled the same way).
+# denormal); IEEE sqrt / division take a slow subroutine for denormal operands, and one such lane stalls its warp.
+# With -ftz the results are unchanged for every normal number (torch's own CUDA kernels are compiled the same way).
 PER_FILE_FLAGS = {"shading.cu": ["-fmad=false"], "adam.cu": ["-ftz=true"]}
 if os.environ.get("R3DG_SHADING_FMAD") == "1":      # experiment knob (tools/): let nvcc contract mul+add in shading.cu
     PER_FILE_FLAGS["shading.cu"] = []
@@ -61,7 +60,7 @@ def build(force=False, verbose=False):
                 if r.returncode != 0:
                     raise RuntimeError("nvcc failed for " + cmd[-3])
     if jobs or not os.path.exists(LIB):
-        subprocess.check_call([NVCC, "-shared", "-o", LIB] + objs + ["-lcudart"])
+        subprocess.check_call([NVCC] + ARCH + ["-shared", "-o", LIB] + objs + ["-lcudart"])
     return LIB
 
 

@@ -7,7 +7,7 @@
 // Here ONE launch updates every group: 28 B per element (read p, g, m, v; write p, m, v), the
 // HBM floor for Adam with fp32 state.
 //
-// B200 design notes
+// Design notes
 //  * the descriptor table (<= 16 tensors) travels in the kernel parameter space; blocks are dealt
 //    over the concatenation of all tensors in units of 4096 elements, a block finds its tensor
 //    with a <= 16-step scan of the block prefix;
@@ -53,8 +53,7 @@ __device__ __forceinline__ void adam_update(const AdamTensor& t, float& p, float
     // CUDA functors contract mul+add into FMA).  The quotient only scales the UPDATE, so it
     // uses the one-MUFU forms (sqrt.approx, division by reciprocal: <= 2 ulp of the update, ~1e-7 of a step that is itself
     // ~lr): IEEE div / sqrt branch to a slow subroutine whenever an operand is zero or denormal, real gradients are
-    // full of exact zeros (Gaussians a view does not see), and one such lane stalls its warp — the kernel ran at 3.6 TB/s
-    // inside the stage-2 step against 6.7 TB/s on dense synthetic gradients (profiles/r02_launches_stage2.csv).
+    // full of exact zeros (Gaussians a view does not see), and one such lane stalls its warp.
     float sq;
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(sq) : "f"(v));                      // exact 0 for v == 0, no slow path
     const float denom = __fadd_rn(__fmul_rn(sq, t.inv_bc2_sqrt), t.eps);

@@ -13,10 +13,10 @@ namespace {
 int g_num_sms[64] = {0};            // per device (the caller may drive several GPUs from one process)
 int num_sms() {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;   // B200
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;   // H100 SXM
     if (g_num_sms[dev] == 0) {
         int n = 0;
-        g_num_sms[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 148;
+        g_num_sms[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
     }
     return g_num_sms[dev];
 }
@@ -40,7 +40,7 @@ inline void prof_mark(bool fwd, int i, cudaStream_t s) {
 
 extern "C" {
 
-const char* r3dg_version(void) { return "r3dg_b200 0.1 sm_100a"; }
+const char* r3dg_version(void) { return "r3dg_b200 0.1 sm_90a"; }
 
 size_t r3dg_raster_geom_bytes(int P, int S) { return GeomLayout(P < 1 ? 1 : P, S).total; }
 size_t r3dg_raster_img_bytes(int W, int H) { return ImgLayout(W, H).total; }

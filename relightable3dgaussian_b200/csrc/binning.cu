@@ -60,8 +60,8 @@ __global__ void __launch_bounds__(256) bin_count_kernel(int P, int T, int gx, in
 }
 
 // bin_scatter: one CTA per chunk.  Writing every instance straight to its slot costs one 4-byte
-// L2 write transaction per instance (~8M scattered sector writes = 130 us, whatever the ranking
-// logic).  Instead the chunk's instances are first gathered in shared memory grouped by tile:
+// L2 write transaction per instance (~8M scattered sector writes at the headline config, whatever
+// the ranking logic).  Instead the chunk's instances are first gathered in shared memory grouped by tile:
 //   1. recount the chunk per tile (as bin_count), exclusive scan -> local CSR offsets;
 //   2. unordered append: one thread per Gaussian, slot = shared atomicAdd on the tile's cursor,
 //      entry = {Gaussian id, tile << 16 | position in the chunk};

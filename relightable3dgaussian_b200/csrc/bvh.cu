@@ -2,7 +2,7 @@
 // bakes per-Gaussian visibility (reference bvh/: __init__.py:29-71, src/construct.cu:147-266,
 // src/trace.cu:196-287, include/utility.cuh:35-111; kernels K17-K22 of SURVEY.md §2.3).
 //
-// B200 design notes
+// Design notes
 //  * build: no thrust temporaries or host round trips — scene bounds by ordered-int atomics, Morton
 //    keys sorted with the library's own one-sweep radix sort (stable => the reference's
 //    (morton, index) order), Karras internal nodes, bottom-up refit with fenced flags.  Every

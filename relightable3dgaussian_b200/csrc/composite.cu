@@ -1,7 +1,7 @@
 // Stage 2 forward: per-tile front-to-back alpha compositing (reference K7, forward.cu:263-395)
 // and the surface-xyz / pseudo-normal pass (K8+K9, forward.cu:398-491, fused into one kernel).
 //
-// B200 design notes
+// Design notes
 //  * each warp owns a compact 8x4 pixel block of a 16x16 tile and walks the tile's sorted list
 //    AUTONOMOUSLY: no CTA barrier, per-warp early termination (the reference's CTA-wide
 //    fetch/compute lock-step spent ~half of its stall samples at the barrier);
@@ -11,7 +11,7 @@
 //    queued entries (id -> packed record prefetched one batch ahead, staged in a warp-private
 //    shared-memory slab, exact ellipse / block test once per entry by the lane that staged it);
 //  * the kernel is bound by per-warp latency and by its heaviest warps, not by issue slots
-//    (profiles/r02_warp_timing.md): entries are composited in rounds of U whose alpha evaluations
+//    (tools/warp_timing.py): entries are composited in rounds of U whose alpha evaluations
 //    are in flight together, the sequential part is branch-free (predicated FMAs);
 //  * accumulators live in registers (template on the number of float4 channel groups) — the
 //    reference's runtime-indexed F[33] spills to local memory;
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(256) block_mask_kernel(int gx, const uint2* __
 // BULK = true : the TMA-unit experiment north_star asks for — every lane issues ONE 1-D bulk copy (cp.async.bulk, SASS
 //   UBLKCP) of its entry's record (recf * 4 bytes, 16-byte aligned) straight into a double-buffered AoS slab; the
 //   warp's mbarrier counts the transaction bytes.  No prefetch registers (12-28 fewer live registers), no staging
-//   stores.  Selected with r3dg_tune("composite_bulk", 1); measured result in profiles/r02_composite_bulk_staging.md.
+//   stores.  Selected with r3dg_tune("composite_bulk", 1); the register prefetch is the default.
 template <int NG, int NW, int MINB, bool BULK>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const CompositeFwdParams p) {
     constexpr int RG = 2 + NG;                       // float4 groups per record
@@ -222,9 +222,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = r[g];
         }
         // second, exact filter — each lane applies round 1's exact-conservative ellipse / rectangle test to ITS OWN staged
-        // entry (one evaluation per entry): the block rectangle lets through 3.26 M (warp, entry) pairs at the headline
-        // config, the exact test 2.28 M (profiles/r02_ncu_composite_fwd_final.md vs _v2_), and every pair dropped here
-        // saves the ~41-instruction alpha evaluation of the loop below
+        // entry (one evaluation per entry): the block rectangle is conservative, the exact test drops the (warp, entry)
+        // pairs whose ellipse misses the block, and every pair dropped here saves the alpha evaluation of the loop below
         uint32_t word;
         if (BULK) word = n == 32 ? 0xffffffffu : ((1u << n) - 1u);       // (records are not in registers in this variant)
         else word = __ballot_sync(0xffffffffu, lane < n && touch_block(r[0], r[1], (float)bx0, (float)by0));
@@ -250,8 +249,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
         // work) depend neither on one another nor on the pixel's state, so all U are issued back to back: U dependency
         // chains in flight per warp instead of one.  Only the short transmittance recurrence that follows is sequential,
         // in list order, with exactly the reference's arithmetic.  This is what bounds the kernel: the heaviest pixel
-        // blocks composite ~1000 entries one after the other, and while the light tiles drain the machine those few
-        // warps decide the makespan (tools/warp_timing.py, profiles/r02_warp_timing.md).  A round with fewer than U
+        // blocks composite many entries one after the other, and while the light tiles drain the machine those few
+        // warps decide the makespan (tools/warp_timing.py).  A round with fewer than U
         // entries left re-evaluates the last one, masked out.
         constexpr int U = NG <= 2 ? R3DG_FWD_ILP : R3DG_FWD_ILP_WIDE;
         while (word) {

@@ -1,6 +1,6 @@
 // Stage 2 backward: per-tile back-to-front re-traversal (reference K10, backward.cu:401-614).
 //
-// B200 design notes
+// Design notes
 //  * the reference issues 10+S global atomicAdds per contributing (pixel, Gaussian) pair.  Here a
 //    warp (8x4 pixels) first reduces its 32 per-pixel gradient rows with transposed butterflies
 //    ("reduce-scatter": ~V shuffles for V values instead of 5V), after which every lane holds one
@@ -14,7 +14,7 @@
 //    deepest last contributor — no culling test, no record fetch, no exp() for anything else;
 //  * CTAs are launched in the order of the work the forward pass measured (cta_order_kernel), and
 //    the walk is laid out in rounds of U entries for instruction-level parallelism: the kernel is
-//    bound by per-warp latency and its heaviest warps (profiles/r02_warp_timing.md);
+//    bound by per-warp latency and its heaviest warps (tools/warp_timing.py measures both);
 //  * per-pixel state is register resident (template on channel groups); the reference keeps three
 //    float[24] arrays in local memory and 36 KB of shared memory per CTA;
 //  * gradients differ from the reference only by fp32 summation order (the reference's own
@@ -311,8 +311,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll
             for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
-        // Rounds of U entries.  The kernel is latency-bound, not issue-bound (fewer resident CTAs make it slower at every
-        // setting, profiles/r02_warp_timing.md), and the heaviest pixel blocks walk ~500 contributors one after the other,
+        // Rounds of U entries.  The kernel is latency-bound, not issue-bound (fewer resident CTAs make it slower), and the
+        // heaviest pixel blocks walk hundreds of contributors one after the other,
         // so the round is laid out for instruction-level parallelism inside the warp: (1) everything that depends only on
         // the entry — record fetch, exp(), alpha, 1/(1-alpha), the entry's own cotangent dot D — for all U entries; (2) the
         // two short recurrences T and A in list order; (3) gradient rows and butterflies of the U entries, advanced level

@@ -67,8 +67,8 @@ int composite_bwd_tune(const char* key, int value, int* previous);
 
 // Dynamic shared memory to request so that at most `ctas` CTAs of `kernel` are resident per SM (0 when ctas <= 0 or
 // the kernel's own footprint already allows no more).  The compositors are bound by their heaviest warps (a pixel
-// block that composites ~1000 entries one after the other): fewer co-resident warps let those run faster while the
-// total throughput stays issue-bound — see the residency sweep in profiles/r02_warp_timing.md.
+// block that composites its entries one after the other): fewer co-resident warps let those run faster while the
+// total throughput stays issue-bound (tools/residency_sweep.py sweeps the setting).
 template <typename K>
 inline size_t residency_pad(K kernel, int ctas) {
     if (ctas <= 0) return 0;

@@ -3,12 +3,12 @@
 // (K4, rasterizer_impl.cu:70-111), tile ranges (K6, rasterizer_impl.cu:116-138) and
 // markVisible (K13).  The radix sort (K5) lives in radix_sort.cu.
 //
-// B200 design notes
+// Design notes
 //  * one packed 16B-aligned record per Gaussian (common.cuh) is produced here so the compositors
 //    gather one row instead of five arrays;
 //  * the floating-point association of everything that feeds radii / tile rectangles / depth keys
 //    is pinned with explicit round-to-nearest intrinsics to the association of the reference's
-//    sm_100 binary, which makes point_list / ranges / n_contrib bit-identical;
+//    compiled binary, which makes point_list / ranges / n_contrib bit-identical;
 //  * the instance count R never travels to the host inside the pipeline: kernels read it from
 //    the geometry header, grids are sized from the SM count, and the binning buffer is
 //    capacity-checked on the device.
@@ -308,8 +308,8 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
     }
     // ---- packed record row: staged in shared memory (the SH slab is dead by now), written back by ONE TMA bulk store ---
     // A thread writing its own 64-112 B row straight to global memory issues 4-7 STG.128 whose 32 lanes are 64-112 B
-    // apart: every instruction touches 32 half-used sectors and the kernel was bound by the L1/TEX pipeline (78-87 % of
-    // its peak, profiles/r02_ncu_project_kernel_bulk.md), not by HBM.  The CTA's rows are one contiguous slab; rows of
+    // apart: every instruction touches 32 half-used sectors and the kernel was bound by the L1/TEX pipeline, not by
+    // HBM.  The CTA's rows are one contiguous slab; rows of
     // culled Gaussians are written as zeros (nothing ever reads them: they are in no tile list).
     const int rec4n = p.recf >> 2;
     float4* srow = reinterpret_cast<float4*>(sSH) + (size_t)threadIdx.x * rec4n;
@@ -426,7 +426,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(int P, const uint32_
 
 // Longest-processing-time-first order of the tiles for the compositors: the CTAs of the heavy
 // tiles (longest sorted lists) are launched first so that the grid's tail consists of light tiles
-// (with row-major order the last heavy CTAs left 20% of the SM-cycles idle).  Coarse counting sort
+// (with row-major order the last heavy CTAs leave SMs idle at the end of the grid).  Coarse counting sort
 // by list length (64 buckets), one CTA.
 __global__ void __launch_bounds__(1024) tile_order_kernel(int T, const uint2* __restrict__ ranges, uint32_t* __restrict__ order,
                                                           uint32_t* __restrict__ bwd_work) {
@@ -456,8 +456,8 @@ __global__ void __launch_bounds__(1024) tile_order_kernel(int T, const uint2* __
 
 // The same coarse LPT order for the backward compositor's CTAs, by what the forward pass measured: keys[c] = entries the
 // busiest warp of half-tile CTA c composited = exactly the iterations its backward twin will run.  List length is a poor
-// predictor there (a dense tile saturates after a fraction of its list): ordered by it, heavy backward CTAs started at
-// 40 % of the kernel and finished last (profiles/r02_warp_timing.md).
+// predictor there (a dense tile saturates after a fraction of its list): ordered by it, heavy backward CTAs started
+// late and finished last (tools/warp_timing.py shows the per-warp start and end times).
 __global__ void __launch_bounds__(1024) cta_order_kernel(int n, const uint32_t* __restrict__ keys, uint32_t* __restrict__ order) {
     __shared__ uint32_t s_max, s_cnt[64], s_cur[64];
     const int tid = threadIdx.x;

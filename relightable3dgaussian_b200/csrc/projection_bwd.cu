@@ -2,7 +2,7 @@
 // backward (K12, backward.cu:348-398, SH backward :20-139, cov3D backward :280-343) fused into a
 // single per-Gaussian kernel.
 //
-// B200 design notes
+// Design notes
 //  * one pass over the Gaussians instead of two kernels + ten zero-fill memsets: every output row
 //    (including the rows of culled Gaussians) is written here exactly once, so the caller hands
 //    in uninitialised memory (the reference zero-fills 320 MB at P=1M, rasterize_points.cu:183-192);

@@ -2,7 +2,7 @@
 // by view depth once (P pairs) instead of the reference's cub::DeviceRadixSort::SortPairs over
 // all R ~ 8 P (tile, depth) instances (rasterizer_impl.cu:313-318); the per-tile lists are then
 // produced by the order-preserving binning in binning.cu.  The BVH and kNN builders sort their
-// 30-bit Morton codes with it (bvh.cu, knn.cu).  Hand-written for sm_100a:
+// 30-bit Morton codes with it (bvh.cu, knn.cu).  Hand-written for sm_90a:
 //
 //   sort_histogram_kernel : per-tile digit counts of the first pass;
 //   per pass:
@@ -17,8 +17,7 @@
 //
 // An earlier version chained the tiles with a decoupled look-back (one kernel per pass).  The sorts
 // here are small (P ~ 1M pairs = ~500 tiles, all resident at once), so every tile had to poll
-// hundreds of predecessors' descriptors: ~3000 instructions per warp and 27 us per pass, most of
-// it polling.  Counting ahead removes every inter-CTA wait: nothing spins, nothing can deadlock.
+// hundreds of predecessors' descriptors, and most of each pass was spent polling.  Counting ahead removes every inter-CTA wait: nothing spins, nothing can deadlock.
 //
 // Which key bits need sorting is decided on the device (sort_plan in common.cuh): no host sync.
 #include <algorithm>
@@ -147,8 +146,8 @@ __global__ void __launch_bounds__(R3DG_SORT_THREADS, 4) sort_scatter_kernel(
         }
 #pragma unroll
         for (int i = 0; i < R3DG_SORT_ITEMS; ++i) {
-            // peers with the same digit, from w ballots: a match.any over ~32 distinct values costs
-            // ~400 cycles on sm_100, eight ballots ~140 (profiles/r01_ubench_warp_primitives.jsonl)
+            // peers with the same digit, from w ballots rather than one match.any over ~32 distinct values
+            // (tools/ubench.cu measures both)
             uint32_t peers = 0xffffffffu;
 #pragma unroll
             for (int b = 0; b < 8; ++b) {

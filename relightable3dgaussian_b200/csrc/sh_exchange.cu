@@ -9,7 +9,7 @@
 // and summing the outer products locally replaces 2*(N-1)/N * 192 B of all-reduce traffic per
 // Gaussian and GPU by (N-1) * 12 B, and the projection backward no longer writes the dense tensor.
 //
-// B200 design notes: HBM-bound (reads 12 B + N*12 B, writes 192 B per Gaussian); one thread per
+// Design notes: HBM-bound (reads 12 B + N*12 B, writes 192 B per Gaussian); one thread per
 // Gaussian accumulates its 3*M values in a transposed shared slab column (conflict-free), the CTA
 // writes the [128][3M] slab back with coalesced 16-byte stores — the same slab scheme as
 // projection_bwd.cu.  The basis is evaluated with the expressions of projection_bwd.cu so a

@@ -4,7 +4,7 @@
 // :71-128) — ~40 elementwise PyTorch kernels over [P,N,3] tensors in the reference, whose autograd
 // graph keeps >= 15 such tensors alive (SURVEY.md §3.4) — as ONE forward and ONE backward kernel.
 //
-// B200 design notes
+// Design notes
 //  * a group of 8 lanes per Gaussian (4 Gaussians per warp), lanes stride the N incident samples:
 //    the baked [P,N,*] tensors (direction 12 B + visibility 4 B + area 4 B per sample — the only
 //    per-sample HBM traffic) are read once per direction, rows of neighbouring Gaussians are
@@ -126,8 +126,8 @@ __device__ __forceinline__ void stage_incidents(const ShadeArgs& a, int g, float
 }
 
 // 1/x with one MUFU (<= 1 ulp), for the BACKWARD kernel only: its recomputed forward quantities and its gradient
-// arithmetic tolerate a last-bit difference (tests: 1e-4 relative), while the ~19 IEEE divisions per sample cost ~230 of
-// its ~1500 instructions (FCHK + slow-path branch each; profiles/r02_ncu_shade_bwd.md).  The forward kernel keeps the
+// arithmetic tolerate a last-bit difference (tests: 1e-4 relative), while each of its IEEE divisions per sample costs an
+// FCHK and a slow-path branch.  The forward kernel keeps the
 // IEEE divisions of the PyTorch expression.
 __device__ __forceinline__ float fast_rcp(float x) {
     float r;
@@ -308,8 +308,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? 6 : 1) shade_fwd_ker
 }
 
 // ---- environment-map gradient (grid_sample backward: a scatter-add of P*N*4 taps) ----------------
-// There is no native fp32 shared-memory atomic add on sm_100: `atomicAdd(float*)` on shared memory
-// compiles to an LDS / FADD / ATOMS.CAST.SPIN loop that occupies the LSU for ~64 cycles per warp
+// There is no native fp32 shared-memory atomic add on sm_90: `atomicAdd(float*)` on shared memory
+// compiles to an LDS / FADD / ATOMS.CAST.SPIN loop that occupies the LSU for many cycles per warp
 // instruction, and 12 of them per sample bounded the whole backward kernel.  ENV_TAG mode gives
 // every warp a PRIVATE float4 {r,g,b,-} copy of the texture gradient and resolves the (rare)
 // intra-warp collisions with a one-byte tag per texel: every pending lane stores its lane id, the
@@ -528,9 +528,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
 struct ShadeKnob { const char* key; const char* env; int lo, hi, dflt, value; };
 static ShadeKnob g_knobs[] = {
     {"shade_group", "R3DG_SHADE_GROUP", 8, 32, 8, -1},            // lanes per Gaussian: 8, 16 or 32
-    // defaults = the fastest measured combination (profiles/r01_stage3_shading_variants.jsonl, 300k x 64 backward:
-    // variant 0 + tag 1.92 ms, variant 1 + tag 1.42, variant 2 + tag 1.51 (3 CTAs/SM by shared memory),
-    // variant 2 + shared atomics 1.20 (5 CTAs/SM); forward variant 0 0.57 ms, variant 1 0.47)
+    // defaults = the fastest combination measured during development (tools/bench_stage3.py times the variants;
+    // variant 2 with shared atomics fits more CTAs per SM than with tagged copies)
     {"shade_env_mode", "R3DG_SHADE_ENV_MODE", 0, 2, ENV_CAS, -1}, // highest env-gradient mode allowed
     {"shade_fwd_variant", "R3DG_SHADE_FWD_VARIANT", 0, 1, 1, -1}, // 1: incident SH coefficients in shared memory
     {"shade_bwd_variant", "R3DG_SHADE_BWD_VARIANT", 0, 2, 2, -1}, // 1: as forward; 2: + gradient accumulators in shared memory
@@ -629,7 +628,7 @@ extern "C" {
 
 static int shade_num_sms() {
     static int n = 0;
-    if (n == 0) { int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148; }
+    if (n == 0) { int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132; }
     return n;
 }
 

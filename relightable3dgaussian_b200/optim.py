@@ -1,6 +1,6 @@
 """Host-side mirror of the optimiser the reference trains with: `torch.optim.Adam(l, lr=0.0,
 eps=1e-15)` over 7-13 per-Gaussian parameter groups (scene/gaussian_model.py:465-497), backed by
-ONE fused sm_100a launch for all groups (r3dg_adam_step, csrc/adam.cu) instead of ~8 elementwise
+ONE fused sm_90a launch for all groups (r3dg_adam_step, csrc/adam.cu) instead of ~8 elementwise
 kernels per group.
 
 `FusedAdam` keeps torch.optim.Adam's observable behaviour for the configuration the reference

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's operator surface for the rasterizer
 (gaussian_renderer/r3dg_rasterization.py:32-262): `GaussianRasterizationSettings`,
 `GaussianRasterizer`, `rasterize_gaussians`, with the same field names, argument meaning, return
-tuple and error behaviour, on top of the B200 kernels (through `_C_raster`, our stand-in for
+tuple and error behaviour, on top of this project's CUDA kernels (through `_C_raster`, our stand-in for
 `r3dg_rasterization._C`).
 """
 from typing import NamedTuple

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's BVH operator surface — `RayTracer` (bvh/__init__.py:28-71),
 `sample_incident_rays` / `fibonacci_sphere_sampling` (scene/gaussian_model.py:20-28,
 utils/graphics_utils.py:9-37, utils/sh_utils.py:36-68) and the visibility bake `update_visibility`
-(scene/gaussian_model.py:312-342) — as thin marshalling over the B200 kernels.  No sampling or
+(scene/gaussian_model.py:312-342) — as thin marshalling over this project's CUDA kernels.  No sampling or
 tracing arithmetic lives in this file: directions come from `r3dg_sample_incident_dirs`, the bake
 from `r3dg_bvh_bake_visibility` (directions generated inside the trace kernel, written once).
 

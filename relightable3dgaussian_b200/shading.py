@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's shading step: `rendering_equation(...)` with the signature,
 return value (pbr, extra_results dict) and light-object duck typing of
-gaussian_renderer/neilf.py:339-371, backed by the fused sm_100a kernels
+gaussian_renderer/neilf.py:339-371, backed by the fused sm_90a kernels
 (r3dg_render_equation_forward / _backward).
 
 The reference function lives inside gaussian_renderer/neilf.py (pure PyTorch), so there is no

@@ -54,6 +54,43 @@ def max_rel_above_floor(a, b, floor=1e-6):
     return float((np.abs(a - b)[m] / np.abs(b)[m]).max())
 
 
+def digest(t):
+    """sha256 of an integer array's values (as int64): bit-exact comparison against a stored fixture."""
+    import hashlib
+    a = t.detach().cpu().long().numpy() if isinstance(t, torch.Tensor) else np.asarray(t).astype(np.int64)
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def sketch(t, k=32):
+    """k random +-1 projections of a float array (a Johnson-Lindenstrauss sketch, float64).  The rows are a
+    fixed integer hash of (row, element index), identical on every device, so the sketches of two arrays
+    estimate their relative L2 difference over ALL elements: rel_l2_sketch(sketch(a), sketch(b))."""
+    x = t.detach().reshape(-1).double()
+    j = torch.arange(x.numel(), dtype=torch.int64, device=x.device)
+    out = np.empty(k)
+    for i in range(k):
+        h = (j + ((i + 1) * 0x9E3779B1 & 0xFFFFFFFF)) & 0xFFFFFFFF
+        h = (((h >> 16) ^ h) * 0x45D9F3B) & 0xFFFFFFFF
+        h = (((h >> 16) ^ h) * 0x45D9F3B) & 0xFFFFFFFF
+        h = (h >> 16) ^ h
+        out[i] = float((x * ((h & 1).double() * 2 - 1)).sum())
+    return out
+
+
+def rel_l2_sketch(a, b):
+    return float(np.linalg.norm(np.asarray(a) - np.asarray(b)) / (np.linalg.norm(b) + 1e-30))
+
+
+def raster_key(P, W, H, S, view, shift, bwd, deg=3, M=16, boost=1.0):
+    """Name of a rasterizer parity case in tests/golden/live_raster.npz."""
+    return f"P{P}_{W}x{H}_S{S}_v{view}_c{int(shift)}_b{int(bwd)}_d{deg}_M{M}_x{boost:g}"
+
+
+def fixed_sample(n, k, seed):
+    """Seeded sorted sample of min(n, k) indices out of n."""
+    return np.sort(np.random.default_rng(seed).choice(n, min(n, k), replace=False))
+
+
 def inverse_covariance(scales, rotations):
     """scene/gaussian_model.py:257-260 + utils/general_utils.py:151-160 (strip_symmetric of
     L L^T with L = R diag(1/s)); torch ops, device of the inputs."""

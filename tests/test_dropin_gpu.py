@@ -1,28 +1,38 @@
-"""The drop-in boundary, executed for real (SURVEY.md §8b): the reference's OWN wrapper files
-(gaussian_renderer/r3dg_rasterization.py, bvh/__init__.py — git-ignored copies under oracle/_ref/py made
-by oracle/build_ref_ext.sh) are loaded by path twice: once over the reference's own pybind modules
-(oracle/_ref/ext: rasterize_points.cu / bvh.cu glue + its kernels, built for sm_100) and once over this
-repo's `dropin/` packages.  Same inputs, same wrapper code, two back ends: outputs and gradients must agree
-to the north_star tolerances.  Also: the full visibility bake (own tree + in-kernel sampling + own trace)
-against the reference's bake (its tree + PyTorch sampling + its trace), and the sampling kernel against the
-reference's own `fibonacci_sphere_sampling`."""
+"""The drop-in boundary (SURVEY.md §8b): this repo's `dropin/` packages (`r3dg_rasterization`, `bvh_tracing`) against
+what the reference's OWN code path computed on the same seeded inputs — its wrapper files
+(gaussian_renderer/r3dg_rasterization.py, bvh/__init__.py) over its own pybind modules (rasterize_points.cu / bvh.cu
+glue + its kernels).  Those results are stored in tests/golden/live_dropin.npz (tests/golden/make_golden_live.py):
+integer outputs as sha256 digests, images at a seeded pixel sample and as random-sign sketches, gradients as sketches, visibility at
+a seeded ray sample.  Outputs and gradients must agree to the north_star tolerances.  Also: the full visibility bake
+(own tree + in-kernel sampling + own trace) against the reference's bake (its tree + PyTorch sampling + its trace),
+and the sampling kernel against the reference's own `fibonacci_sphere_sampling`."""
+import importlib
+import os
+import sys
+
 import numpy as np
 import pytest
 import torch
 
-from helpers import case_inputs, npy, rel_l2
+from helpers import GOLDEN, ROOT, case_inputs, digest, fixed_sample, npy, rel_l2_sketch, sketch
 
 pytestmark = pytest.mark.gpu
+DROPIN_CASES = [(60_000, 400, 304, 16), (300_000, 800, 800, 5)]
+BAKE_CASES = [(100_000, 32), (40_000, 64)]
 
 
-def _need(which):
-    from oracle import ref_gpu
-    if not ref_gpu.ext_available(which):
-        pytest.skip(f"oracle/_ref/ext ({which}) not built — run oracle/build_ref_ext.sh in the build container")
-    return ref_gpu
+@pytest.fixture(scope="module")
+def golden():
+    return np.load(os.path.join(GOLDEN, "live_dropin.npz"))
 
 
-def _render_through_wrapper(mod, sc, cam, S, bg, cots):
+def dropin(pkg):
+    if os.path.join(ROOT, "dropin") not in sys.path:
+        sys.path.insert(0, os.path.join(ROOT, "dropin"))
+    return importlib.import_module(pkg)
+
+
+def render_through_wrapper(mod, sc, cam, S, bg, cots):
     d = lambda t: t.cuda()
     leaves = [d(t).requires_grad_(True) for t in (sc.means3D, sc.opacities, sc.shs, sc.scales, sc.rotations, sc.features)]
     xyz, opac, shs, scales, rots, feats = leaves
@@ -49,108 +59,102 @@ def _render_through_wrapper(mod, sc, cam, S, bg, cots):
     return res, grads
 
 
-@pytest.mark.parametrize("P,W,H,S", [(60_000, 400, 304, 16), (300_000, 800, 800, 5)], ids=["60k-S16", "300k-S5"])
-def test_reference_wrapper_runs_unmodified_over_dropin(P, W, H, S):
-    ref_gpu = _need("raster")
-    ours = ref_gpu.load_reference_wrapper("raster", "dropin")
-    theirs = ref_gpu.load_reference_wrapper("raster", "ref")
-    assert "relightable3dgaussian_b200" in ours._C_origin and "oracle/_ref/ext" in theirs._C_origin
+@pytest.mark.parametrize("P,W,H,S", DROPIN_CASES, ids=["60k-S16", "300k-S5"])
+def test_dropin_rasterizer_matches_reference_wrapper_golden(golden, P, W, H, S):
+    mod = dropin("r3dg_rasterization")
+    assert os.path.realpath(mod._C.__file__).startswith(os.path.join(os.path.realpath(ROOT), "relightable3dgaussian_b200"))
+    key = f"raster_P{P}_S{S}__"
     sc, cam = case_inputs(P, W, H, S, view=4, center_shift=True)
-    bg = torch.tensor([0.3, 0.1, 0.7])
     g = torch.Generator().manual_seed(3)
     cots = [torch.randn(c, H, W, generator=g) for c in (3, 1, 1, S)]
-    ro, rg = _render_through_wrapper(theirs, sc, cam, S, bg, cots)
-    oo, og = _render_through_wrapper(ours, sc, cam, S, bg, cots)
-    assert oo["num_rendered"] == ro["num_rendered"]
-    assert torch.equal(oo["radii"], ro["radii"]) and torch.equal(oo["num_contrib"], ro["num_contrib"].to(oo["num_contrib"].dtype))
-    assert torch.equal(oo["visible"], ro["visible"])
+    oo, og = render_through_wrapper(mod, sc, cam, S, torch.tensor([0.3, 0.1, 0.7]), cots)
+    assert oo["num_rendered"] == int(golden[key + "num_rendered"])
+    for n in ("radii", "num_contrib", "visible"):
+        assert digest(oo[n]) == str(golden[key + "dig_" + n]), n
+    pix = torch.from_numpy(golden[key + "pix"].astype(np.int64)).cuda()
     for n in ("color", "opacity", "depth", "feature", "normal", "surface_xyz"):
-        assert (oo[n] - ro[n]).abs().max().item() <= 1e-4, n
+        t = oo[n]
+        assert np.abs(npy(t.reshape(t.shape[0], -1)[:, pix]) - golden[key + "img_" + n]).max() <= 1e-4, n
+        assert rel_l2_sketch(sketch(t), golden[key + "sk_img_" + n]) < 1e-4, n
     for n in og:
-        assert og[n] is not None and rg[n] is not None, n
-        assert rel_l2(npy(og[n]), npy(rg[n])) < 1e-3, n
+        assert og[n] is not None, n
+        assert rel_l2_sketch(sketch(og[n]), golden[key + "sk_" + n]) < 1e-3, n
 
 
-def _bvh_scene(P):
+def bvh_scene(P):
     sc, _ = case_inputs(P, 64, 64, 0)
     d = lambda t: t.cuda()
     return d(sc.means3D), d(sc.scales), d(sc.rotations), d(sc.opacities[:, 0].contiguous()), d(sc.normals)
 
 
-def test_reference_raytracer_runs_unmodified_over_dropin():
-    ref_gpu = _need("bvh")
+def test_dropin_raytracer_matches_reference_golden(golden):
     from oracle import oracle_sampling
-    ours = ref_gpu.load_reference_wrapper("bvh", "dropin")
-    theirs = ref_gpu.load_reference_wrapper("bvh", "ref")
-    xyz, s, r, op, nrm = _bvh_scene(30_000)
+    ours = dropin("bvh_tracing")
+    xyz, s, r, op, nrm = bvh_scene(30_000)
     icov = oracle_sampling.inverse_covariance(s, r)
-    a, b = ours.RayTracer(xyz, s, r), theirs.RayTracer(xyz, s, r)
+    a = ours.RayTracer(xyz, s, r)
     for name in ("tree", "morton"):                                   # topology + Morton codes bit-exact
-        ta, tb = getattr(a, name, None), getattr(b, name, None)
-        if ta is not None and tb is not None:
-            assert torch.equal(ta, tb), name
+        if "tracer__dig_" + name in golden.files:
+            assert digest(getattr(a, name)) == str(golden["tracer__dig_" + name]), name
     dirs, _ = oracle_sampling.sample_incident_rays(nrm, False, 24)
     ro = xyz[:, None].expand_as(dirs)
-    va = a.trace_visibility(ro, dirs, xyz, icov, op, nrm)
-    vb = b.trace_visibility(ro, dirs, xyz, icov, op, nrm)
-    flips = ((va["visibility"] == 0) != (vb["visibility"] == 0)).float().mean().item()
-    same = (va["visibility"] == 0) == (vb["visibility"] == 0)
+    va = npy(a.trace_visibility(ro, dirs, xyz, icov, op, nrm)["visibility"]).reshape(-1)[golden["tracer__ray_idx"]]
+    vb = golden["tracer__visibility"]
+    flips = ((va == 0) != (vb == 0)).mean()
+    same = (va == 0) == (vb == 0)
     assert flips <= 1e-3, flips
-    assert (va["visibility"] - vb["visibility"])[same].abs().max().item() <= 1e-4
+    assert np.abs(va - vb)[same].max() <= 1e-4
 
 
-def test_sampling_kernel_vs_reference_function():
-    """r3dg_sample_incident_dirs vs the reference's own fibonacci_sphere_sampling (utils/graphics_utils.py:9-37, loaded
-    from the git-ignored copy) on this GPU, deterministic and random-rotate variants."""
-    ref_gpu = _need("bvh")
-    import importlib.util
-    import os
-    import sys
-    from relightable3dgaussian_b200 import raytracer
-    py = os.path.join(os.path.dirname(ref_gpu.__file__), "_ref", "py")
-    sys.path.insert(0, py)
-    try:
-        saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k == "utils" or k.startswith("utils.")}
-        from utils.graphics_utils import fibonacci_sphere_sampling as ref_fib
-    finally:
-        sys.path.remove(py)
-        for k in [k for k in sys.modules if k == "utils" or k.startswith("utils.")]:
-            del sys.modules[k]
-        sys.modules.update(saved)
+def sampling_normals():
     g = torch.Generator().manual_seed(1)
     nrm = torch.nn.functional.normalize(torch.randn(50_000, 3, generator=g), dim=-1).cuda()
     nrm[0] = torch.tensor([0.0, 0.0, -1.0]); nrm[1] = torch.tensor([0.0, 0.0, 1.0])      # the -I fallback and the identity
+    return nrm
+
+
+def sampling_pairs(P, N):
+    """Flat (normal, direction) indices: every direction of the two special normals + a seeded sample of the rest."""
+    return np.concatenate([np.arange(2 * N), fixed_sample(P * N - 2 * N, 2048, N) + 2 * N])
+
+
+def test_sampling_kernel_vs_reference_function(golden):
+    """r3dg_sample_incident_dirs vs the reference's own fibonacci_sphere_sampling (utils/graphics_utils.py:9-37),
+    deterministic and random-rotate variants."""
+    from relightable3dgaussian_b200 import raytracer
+    nrm = sampling_normals()
     for N in (24, 32, 384):
-        d_ref, a_ref = ref_fib(nrm, N, random_rotate=False)
         d, a = raytracer.sample_incident_rays(nrm, False, N)
-        assert d.shape == d_ref.shape and a.shape == a_ref.shape and torch.equal(a, a_ref)
-        assert (d - d_ref).abs().max().item() <= 5e-7, N                                      # unit vectors: a few ulp at most
-        print(f"[sampling] N={N}: bit-equal fraction {(d == d_ref).float().mean().item():.6f}")
+        assert tuple(d.shape) == tuple(golden[f"sampling__shape_{N}"]) and a.shape == d.shape[:-1] + (1,)
+        assert digest(a.contiguous().view(torch.int32)) == str(golden[f"sampling__dig_areas_{N}"])
+        dd = npy(d).reshape(-1, 3)[golden[f"sampling__idx_{N}"]]
+        assert np.abs(dd - golden[f"sampling__dirs_{N}"]).max() <= 5e-7, N                    # unit vectors: a few ulp at most
+        print(f"[sampling] N={N}: bit-equal fraction {(dd == golden[f'sampling__dirs_{N}']).mean():.6f}")
     # random rotation: same phase numbers through both
     torch.manual_seed(5)
-    d_ref, _ = ref_fib(nrm, 32, random_rotate=True)
-    torch.manual_seed(5)
     d, _ = raytracer.fibonacci_sphere_sampling(nrm, 32, random_rotate=True)
-    assert (d - d_ref).abs().max().item() <= 5e-6
+    assert np.abs(npy(d).reshape(-1, 3)[sampling_pairs(nrm.shape[0], 32)] - golden["sampling__dirs_rot32"]).max() <= 5e-6
 
 
-@pytest.mark.parametrize("P,N", [(100_000, 32), (40_000, 64)])
-def test_full_bake_parity_own_tree_vs_reference_tree(P, N):
+@pytest.mark.parametrize("P,N", BAKE_CASES)
+def test_full_bake_parity_own_tree_vs_reference_tree(golden, P, N):
     """update_visibility end to end: OUR tree (exact refit) + in-kernel sampling + our trace, against the REFERENCE's
     bake (its racy-refit tree, PyTorch sampling, its trace kernel, its chunk loop).  Visibility is a step function of T
     at 0.9, so the flip rate across that cliff is the meaningful figure (north_star)."""
-    ref_gpu = _need("bvh")
     from oracle import oracle_sampling
     from relightable3dgaussian_b200 import raytracer
-    xyz, s, r, op, nrm = _bvh_scene(P)
+    key = f"bake_P{P}_N{N}__"
+    xyz, s, r, op, nrm = bvh_scene(P)
     icov = oracle_sampling.inverse_covariance(s, r)
     assert (raytracer.inverse_covariance(s, r) - icov).abs().max().item() <= 1e-3 * icov.abs().max().item()
     vis, dirs, areas = raytracer.update_visibility(xyz, s, r, icov, op, nrm, N)
-    rvis, rdirs, rareas, _ = ref_gpu.reference_update_visibility(xyz, s, r, icov, op, nrm, N)
-    assert vis.shape == rvis.shape == (P, N, 1) and dirs.shape == rdirs.shape and torch.equal(areas, rareas)
-    assert (dirs - rdirs).abs().max().item() <= 5e-7
-    flip = ((vis == 0) != (rvis == 0)).float().mean().item()
-    same = (vis == 0) == (rvis == 0)
-    print(f"[bake] P={P} N={N}: blocked {float((rvis == 0).float().mean()):.3f}, flip rate {flip:.2e}, max-abs on agreeing rays {(vis - rvis)[same].abs().max().item():.2e}")
+    assert vis.shape == (P, N, 1) and dirs.shape == (P, N, 3)
+    assert digest(areas.contiguous().view(torch.int32)) == str(golden[key + "dig_areas"])
+    idx = golden[key + "ray_idx"]
+    assert np.abs(npy(dirs).reshape(-1, 3)[idx] - golden[key + "dirs"]).max() <= 5e-7
+    v, rv = npy(vis).reshape(-1)[idx], golden[key + "visibility"]
+    flip = ((v == 0) != (rv == 0)).mean()
+    same = (v == 0) == (rv == 0)
+    print(f"[bake] P={P} N={N}: blocked {float(golden[key + 'blocked']):.3f}, flip rate {flip:.2e}, max-abs on agreeing rays {np.abs(v - rv)[same].max():.2e}")
     assert flip <= 1e-3
-    assert (vis - rvis)[same].abs().max().item() <= 1e-4
+    assert np.abs(v - rv)[same].max() <= 1e-4

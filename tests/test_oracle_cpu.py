@@ -1,7 +1,7 @@
 """The CPU oracle pinned against reference-owned data (no GPU needed):
   * eval_sh restatement vs outputs of the Python reference (config #1, tests/golden/sh_eval.npz);
   * the C rasterizer restatement vs outputs of the unmodified reference CUDA kernels
-    (tests/golden/raster_*.npz, generated on the B200 box by tests/golden/make_golden.py);
+    (tests/golden/raster_*.npz, generated on a GPU by tests/golden/make_golden.py);
   * internal invariants of the binning (sortedness, ranges partition, stability)."""
 import glob
 import os

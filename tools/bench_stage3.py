@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Stage-3 measurements on one B200 (development / evidence, not the headline bench):
+"""Stage-3 measurements on one H100 (development / evidence, not the headline bench):
   * BVH build + visibility bake (update_visibility) vs the unmodified reference kernels
     (oracle/_ref/libref_bvh.so driven like bvh/__init__.py + scene/gaussian_model.py:312-342);
   * fused rendering_equation fwd+bwd vs the reference's PyTorch formulation (oracle_shading on GPU).

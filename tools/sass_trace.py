@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Symbolic tracer for straight-line fp32 SASS (sm_100).
+"""Symbolic tracer for straight-line fp32 SASS (sm_90).
 
 Purpose: derive the exact FMA association the reference kernels were compiled to (nvcc fuses in
 NVVM *and* again in ptxas, so neither the C source nor the PTX is authoritative) so that the

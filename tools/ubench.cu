@@ -1,6 +1,5 @@
-// Micro-benchmarks of the warp primitives the sort / binning kernels lean on (development aid;
-// results are recorded in profiles/).  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3
-// -o tools/ubench tools/ubench.cu ; run on the GPU box.
+// Micro-benchmarks of the warp primitives the sort / binning kernels lean on (development aid).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench tools/ubench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -66,20 +65,20 @@ void run_lat(const char* name, int K, long long* d_cyc, uint32_t* d_sink, uint32
     cudaMemcpy(&c, d_cyc, 8, cudaMemcpyDeviceToHost);
     // throughput flavour: 16 warps on one SM
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    lat_kernel<OP><<<148, 512>>>(K, 0, d_cyc, d_sink, gbuf);
+    lat_kernel<OP><<<132, 512>>>(K, 0, d_cyc, d_sink, gbuf);
     cudaEventRecord(e0);
-    lat_kernel<OP><<<148, 512>>>(K, 0, d_cyc, d_sink, gbuf);
+    lat_kernel<OP><<<132, 512>>>(K, 0, d_cyc, d_sink, gbuf);
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
     long long c16 = 0;
     cudaMemcpy(&c16, d_cyc, 8, cudaMemcpyDeviceToHost);
-    printf("{\"op\": \"%s\", \"K\": %d, \"cyc_per_iter_1warp\": %.1f, \"cyc_per_iter_16warps_per_SM\": %.1f, \"ms_148x16warps\": %.4f}\n", name, K,
+    printf("{\"op\": \"%s\", \"K\": %d, \"cyc_per_iter_1warp\": %.1f, \"cyc_per_iter_16warps_per_SM\": %.1f, \"ms_132x16warps\": %.4f}\n", name, K,
            (double)c / ITERS, (double)c16 / ITERS, ms);
 }
 
 int main() {
     long long* d_cyc; uint32_t* d_sink; uint32_t* gbuf;
-    cudaMalloc(&d_cyc, 8); cudaMalloc(&d_sink, 148 * 512 * 4); cudaMalloc(&gbuf, 1024 * 32 * 4);
+    cudaMalloc(&d_cyc, 8); cudaMalloc(&d_sink, 132 * 512 * 4); cudaMalloc(&gbuf, 1024 * 32 * 4);
     cudaMemset(gbuf, 0, 1024 * 32 * 4);
     for (int K : {1, 4, 16, 32}) run_lat<0>("match_any", K, d_cyc, d_sink, gbuf);
     for (int K : {1, 32}) run_lat<1>("ballot_match_8bit", K, d_cyc, d_sink, gbuf);
@@ -101,12 +100,12 @@ int main() {
     for (int scattered = 0; scattered <= 1; ++scattered) {
         cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
         const int reps = 64;
-        store_kernel<<<148 * 8, 256>>>(big, words, scattered, reps);
+        store_kernel<<<132 * 8, 256>>>(big, words, scattered, reps);
         cudaEventRecord(e0);
-        store_kernel<<<148 * 8, 256>>>(big, words, scattered, reps);
+        store_kernel<<<132 * 8, 256>>>(big, words, scattered, reps);
         cudaEventRecord(e1); cudaEventSynchronize(e1);
         float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
-        const double n = (double)148 * 8 * 8 * 32 * reps;
+        const double n = (double)132 * 8 * 8 * 32 * reps;
         printf("{\"op\": \"store_%s\", \"stores\": %.0f, \"ms\": %.4f, \"Gstores_per_s\": %.2f}\n", scattered ? "scattered_sector_per_lane" : "coalesced", n, ms, n / ms / 1e6);
     }
     cudaError_t e = cudaDeviceSynchronize();

@@ -1,7 +1,7 @@
 """Load-balance study of the two compositors (diagnostic build only).
 
 Build the library with  R3DG_NVCC_DEFS=-DR3DG_WARP_TIMING python -m relightable3dgaussian_b200.build --force , run this
-on a B200: one fwd+bwd of the headline view with every compositor warp recording (start, end, entries composited, SM);
+on an H100: one fwd+bwd of the headline view with every compositor warp recording (start, end, entries composited, SM);
 prints the makespan against the per-SM busy time and the heaviest warps, and stores the raw table in gpurun_out/."""
 import ctypes
 import json
