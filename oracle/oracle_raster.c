@@ -18,6 +18,7 @@
  * not (CUDA's expf is ~2 ulp, MUFU.EX2 based), so composited images agree to ~1e-6 and
  * n_contrib can differ at measure-zero threshold pixels.
  */
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -58,15 +59,25 @@ static inline float xform_row(const float* m, int r, float x, float y, float z) 
     return dot3(x, m[r], y, m[4 + r], z, m[8 + r]) + m[12 + r];
 }
 
+/* float -> int as a CUDA (int) cast compiles (cvt.rzi.s32.f32): truncation, saturating at the int range, NaN -> 0.
+ * A C cast is undefined there (x86 gives INT_MIN); the reference reaches NaN for the radius of a Gaussian whose 2D
+ * covariance is negative definite (sqrt of a negative eigenvalue, forward.cu:231-233) and gets radius 0. */
+static inline int f2i_rz(float v) {
+    if (v != v) return 0;
+    if (v >= 2147483648.0f) return INT_MAX;
+    if (v <= -2147483648.0f) return INT_MIN;
+    return (int)v;
+}
+
 /* getRect: auxiliary.h:46-56.  Division by BLOCK_X=16 is compiled to an exact *0.0625f. */
 static inline void get_rect(float px, float py, int radius, int gx, int gy, int* x0, int* y0,
                             int* x1, int* y1) {
     float r = (float)radius;
     int a;
-    a = (int)((px - r) * 0.0625f);                    *x0 = a < 0 ? 0 : (a > gx ? gx : a);
-    a = (int)((py - r) * 0.0625f);                    *y0 = a < 0 ? 0 : (a > gy ? gy : a);
-    a = (int)((((px + r) + 16.0f) + -1.0f) * 0.0625f); *x1 = a < 0 ? 0 : (a > gx ? gx : a);
-    a = (int)((((py + r) + 16.0f) + -1.0f) * 0.0625f); *y1 = a < 0 ? 0 : (a > gy ? gy : a);
+    a = f2i_rz((px - r) * 0.0625f);                    *x0 = a < 0 ? 0 : (a > gx ? gx : a);
+    a = f2i_rz((py - r) * 0.0625f);                    *y0 = a < 0 ? 0 : (a > gy ? gy : a);
+    a = f2i_rz((((px + r) + 16.0f) + -1.0f) * 0.0625f); *x1 = a < 0 ? 0 : (a > gx ? gx : a);
+    a = f2i_rz((((py + r) + 16.0f) + -1.0f) * 0.0625f); *y1 = a < 0 ? 0 : (a > gy ? gy : a);
 }
 
 /* computeCov3D: forward.cu:119-153 (M = S*R in glm column-major, Sigma = M^T M; quaternion is
@@ -217,7 +228,7 @@ void oracle_preprocess(int P, int D, int M, const float* means3D, const float* s
         const float mid = (cov_a + cov_c) * 0.5f;
         const float disc = sqrtf(fmaxf(fmaf(mid, mid, -det), 0.1f));
         const float lam = fmaxf(mid + disc, mid - disc);
-        const int my_radius = (int)ceilf(sqrtf(lam) * 3.0f);
+        const int my_radius = f2i_rz(ceilf(sqrtf(lam) * 3.0f));
         const float pix_x = (float)(fma((double)projx + 1.0, (double)W, -1.0) * 0.5);
         const float pix_y = (float)(fma((double)projy + 1.0, (double)H, -1.0) * 0.5);
         int x0, y0, x1, y1;

@@ -338,6 +338,9 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                 alpha[u] = fminf(0.99f, mul_(b.y, G[u]));
                 // the same three tests as the forward pass (identical arithmetic) + "not behind this pixel's last contributor"
                 valid[u] = j0 + u < n && k < last_contributor && !(power > 0.0f) && !(alpha[u] < 1.0f / 255.0f);
+                // a skipped entry of a non-positive-definite conic can have power > 88: expf = inf, and the gated
+                // products below (0 * inf) would be NaN.  Composited entries have power <= 0, so G <= 1 is unchanged.
+                G[u] = valid[u] ? G[u] : 0.0f;
                 asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv[u]) : "f"(1.0f - alpha[u]));   // 1 - alpha in [0.01, 1]: one MUFU
                 float d = fmaf(b.z, dpix_d, dpix_o);                        // depth * dL_ddepth + 1 * dL_dopacity
 #pragma unroll

@@ -105,3 +105,16 @@ def make_camera(k: int, W: int, H: int, radius: float = 4.0311, elevation_deg: f
     campos = view.inverse()[3, :3].contiguous()
     return Camera(H, W, math.tan(fovx / 2.0), math.tan(fovy / 2.0), float(cx), float(cy), view, full,
                   campos)
+
+
+def make_axis_camera(W: int, H: int, fovx: float = 0.6911112070083618) -> Camera:
+    """Camera at the origin looking down +z: identity view rotation, zero translation.  The view-space
+    depth of a point is then its z coordinate, bit for bit, so a scene can place depths exactly (sort
+    keys, the z = 0.2 cull plane)."""
+    view = torch.eye(4)
+    znear, zfar = 0.01, 100.0
+    fovy = 2.0 * math.atan(math.tan(fovx / 2.0) * H / W)
+    t, r = math.tan(fovy / 2.0) * znear, math.tan(fovx / 2.0) * znear
+    full = _projection(znear, zfar, -r, r, t, -t).t().contiguous()
+    return Camera(H, W, math.tan(fovx / 2.0), math.tan(fovy / 2.0), W / 2.0, H / 2.0, view, full,
+                  torch.zeros(3))

@@ -4,6 +4,8 @@
 reference's own pybind modules and Python wrappers):
 
     python tests/golden/make_golden_live.py <outdir>      # then copy <outdir>/live_*.npz into tests/golden/
+    python tests/golden/make_golden_live.py --only edge <outdir>   # live_raster_edge.npz alone (needs only
+                                                                   # oracle/_ref/libref_raster.so)
 
 The inputs are not stored: every case is regenerated from its seed by relightable3dgaussian_b200.synth.
 What the parity tests compared against the live reference is stored compactly:
@@ -14,6 +16,10 @@ What the parity tests compared against the live reference is stored compactly:
   * gradients: a 32-row random-sign sketch (tests/helpers.py:sketch) of every gradient tensor, which
     estimates the relative L2 error over all elements;
   * visibility and sampled directions: a fixed, seeded sample of rays.
+The `edge` group (tests/helpers.py EDGE_CASES) also stores final_T bit-exact (sha256 of its int32 view), the bits
+of depths / means2D / conic_opacity of the visible Gaussians, and noise_<grad>: the largest relative L2 gap between
+the first of four backward runs of the reference and the others, i.e. its own atomic-order noise on these
+ill-conditioned cases.
 """
 import os
 import sys
@@ -24,7 +30,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
-from helpers import bvh_case, case_inputs, digest, fixed_sample, npy, oracle_kwargs, raster_key, sketch  # noqa: E402
+from helpers import EDGE_CASES, bvh_case, case_inputs, digest, edge_case, fixed_sample, npy, oracle_kwargs, raster_key, rel_l2, sketch  # noqa: E402
 from oracle import ref_gpu  # noqa: E402
 
 IMAGES = ("color", "opacity", "depth", "feature", "normal", "surface_xyz")
@@ -84,6 +90,44 @@ def raster_live(rec):
                 if rg[n].numel() and float(rg[n].abs().max()) > 0:
                     rec[key + "sk_" + n] = sketch(rg[n])
         print(f"[golden] raster {key[:-2]}: R={ro['num_rendered']}", flush=True)
+        del ref
+        torch.cuda.empty_cache()
+
+
+def edge_live(rec):
+    dev = lambda t: t if t is None else torch.as_tensor(t).cuda()
+    for name in EDGE_CASES:
+        key = name + "__"
+        kw, cots = edge_case(name)
+        P, W, H = kw["means3D"].shape[0], kw["W"], kw["H"]
+        tk = {k: (dev(v) if isinstance(v, np.ndarray) else v) for k, v in kw.items() if v is not None}
+        ref = ref_gpu.RefRasterizer()
+        ro = ref.forward(**tk)
+        rec[key + "num_rendered"] = ro["num_rendered"]
+        rec[key + "dig_radii"] = digest(ro["radii"])
+        for n in ("tiles_touched", "point_list", "point_list_keys", "ranges", "n_contrib"):
+            rec[key + "dig_" + n] = digest(ref.intermediate(n))
+        rec[key + "dig_final_T"] = digest(ref.intermediate("final_T").view(torch.int32))
+        vis = ro["radii"] > 0
+        for n in ("depths", "means2D", "conic_opacity"):
+            rec[key + "dig_" + n] = digest(ref.intermediate(n)[vis].contiguous().view(torch.int32))
+        image_samples(ro, H, W, P + 7, key, rec)
+        gi = fixed_sample(P, N_PIX, P + 1)
+        rec[key + "weights_idx"] = gi
+        rec[key + "weights"] = npy(ro["weights"])[gi]
+        rec[key + "weights_absmax"] = float(ro["weights"].abs().max())
+        rec[key + "sk_weights"] = sketch(ro["weights"])
+        bk = {k: v for k, v in tk.items() if k in ("means3D", "viewmatrix", "projmatrix", "campos", "bg", "tan_fovx", "tan_fovy",
+                                                    "shs", "colors_precomp", "scales", "rotations", "cov3D_precomp", "features",
+                                                    "sh_degree", "scale_modifier")}
+        cd = [dev(c) for c in cots]
+        runs = [ref.backward(ro, dL_dcolor=cd[0], dL_dopacity=cd[1], dL_ddepth=cd[2], dL_dfeature=cd[3], **bk) for _ in range(4)]
+        for n in GRADS:
+            a = runs[0][n]
+            if a.numel() and float(a.abs().max()) > 0:
+                rec[key + "sk_" + n] = sketch(a)
+                rec[key + "noise_" + n] = max(rel_l2(npy(r[n]), npy(a)) for r in runs[1:])
+        print(f"[golden] edge {name}: R={ro['num_rendered']}", flush=True)
         del ref
         torch.cuda.empty_cache()
 
@@ -167,10 +211,16 @@ def bvh_live(rec):
     print("[golden] bvh cube20k", flush=True)
 
 
-def main(outdir):
+GROUPS = {"bvh": ("live_bvh", bvh_live), "dropin": ("live_dropin", dropin_live), "raster": ("live_raster", raster_live),
+          "edge": ("live_raster_edge", edge_live)}
+
+
+def main(outdir, only=None):
     os.makedirs(outdir, exist_ok=True)
-    assert ref_gpu.available() and ref_gpu.bvh_available() and ref_gpu.ext_available("raster") and ref_gpu.ext_available("bvh")
-    for name, fn in (("live_bvh", bvh_live), ("live_dropin", dropin_live), ("live_raster", raster_live)):
+    assert ref_gpu.available()
+    if only is None:
+        assert ref_gpu.bvh_available() and ref_gpu.ext_available("raster") and ref_gpu.ext_available("bvh")
+    for name, fn in [GROUPS[g] for g in (only or GROUPS)]:
         rec = {}
         fn(rec)
         path = os.path.join(outdir, name + ".npz")
@@ -180,4 +230,9 @@ def main(outdir):
 
 
 if __name__ == "__main__":
-    main(sys.argv[1] if len(sys.argv) > 1 else HERE)
+    import argparse
+    ap = argparse.ArgumentParser()
+    ap.add_argument("outdir", nargs="?", default=HERE)
+    ap.add_argument("--only", action="append", choices=sorted(GROUPS), help="generate only these groups (repeatable)")
+    a = ap.parse_args()
+    main(a.outdir, a.only)

@@ -1,4 +1,5 @@
 """Shared test utilities: seeded cases, conversions, comparison helpers."""
+import math
 import os
 import sys
 
@@ -84,6 +85,189 @@ def rel_l2_sketch(a, b):
 def raster_key(P, W, H, S, view, shift, bwd, deg=3, M=16, boost=1.0):
     """Name of a rasterizer parity case in tests/golden/live_raster.npz."""
     return f"P{P}_{W}x{H}_S{S}_v{view}_c{int(shift)}_b{int(bwd)}_d{deg}_M{M}_x{boost:g}"
+
+
+def _axis_points(n, g, W, H, tanfovx, z, margin=0.9):
+    """n points at depths z (tensor [n]) whose projections fall inside the image of make_axis_camera."""
+    tanfovy = tanfovx * H / W
+    u = (torch.rand(n, 2, generator=g) * 2 - 1) * margin
+    return torch.stack([u[:, 0] * tanfovx * z, u[:, 1] * tanfovy * z, z], dim=1)
+
+
+def _edge_scene(name):
+    """-> (Scene-like dict of torch inputs, Camera, S).  See EDGE_CASES."""
+    family, _, arg = name.partition("-")
+    g = torch.Generator().manual_seed(sum(map(ord, name)))
+    if family == "inside":                                  # camera inside a cube of random Gaussians
+        sc = synth.make_scene(30_000, "cube-v1", 4, 5)
+        cam = synth.make_camera(3, 320, 240, radius=0.3, fovx=1.8)
+        return dict(means3D=sc.means3D, opacities=sc.opacities, shs=sc.shs, scales=sc.scales * 3.0, rotations=sc.rotations,
+                    features=sc.features, scale_modifier=float(arg[1:])), cam, 5
+    if family == "needles":                                 # per-axis scale ratios up to ~1e4 : 1
+        P = 2_500
+        sc = synth.make_scene(P, "shell-v1", 6, 0)
+        stretch = torch.exp((torch.rand(P, 3, generator=g) * 2 - 1) * math.log(100.0))
+        scales = sc.scales * stretch * torch.tensor([3.0, 1.0, 0.3])
+        opac = 1.0 - torch.rand(P, 1, generator=g)          # (0, 1]
+        return dict(means3D=sc.means3D, opacities=opac, shs=sc.shs, scales=scales, rotations=sc.rotations,
+                    features=None), synth.make_camera(2, 320, 232), 0
+    if family == "opaque":                                  # stacks of near-coincident, nearly opaque Gaussians
+        S = int(arg[1:])
+        k = torch.randint(8, 65, (260,), generator=g)
+        centre = torch.repeat_interleave(synth.make_scene(260, "shell-v1", 7, 0).means3D, k, dim=0)
+        P = centre.shape[0]
+        sc = synth.make_scene(P, "shell-v1", 8, S)
+        means = centre + 2e-3 * torch.randn(P, 3, generator=g)
+        scales = 0.02 + 0.04 * torch.rand(P, 3, generator=g)
+        opac = 0.97 + 0.03 * torch.rand(P, 1, generator=g)
+        return dict(means3D=means, opacities=opac, shs=sc.shs, scales=scales, rotations=sc.rotations,
+                    features=sc.features), synth.make_camera(1, 208, 144), S
+    if family == "depth":                                   # depth-key bit patterns of every radix-sort plan
+        P, W, H = 6_500, 128, 96
+        cam = synth.make_axis_camera(W, H)
+        z = {"equal": torch.full((P,), 2.0),
+             "adjacent": torch.where(torch.rand(P, generator=g) < 0.5, torch.tensor(2.0),
+                                     torch.nextafter(torch.tensor(2.0), torch.tensor(3.0))),
+             "narrow": 1.0 + torch.randint(0, 2 ** 15, (P,), generator=g).float() * 2.0 ** -23,
+             "w7": 1.0 + torch.randint(0, 2 ** 20, (P,), generator=g).float() * 2.0 ** -23,
+             "3to5": 3.0 + 2.0 * torch.rand(P, generator=g),
+             "wide": torch.exp(math.log(0.25) + math.log(240.0) * torch.rand(P, generator=g))}[arg].float()
+        # exact ties: a third of the Gaussians copy the depth of another one
+        tie = torch.rand(P, generator=g) < 0.33
+        z = torch.where(tie, z[torch.randint(0, P, (P,), generator=g)], z)
+        means = _axis_points(P, g, W, H, cam.tanfovx, z)
+        scales = z[:, None] * torch.exp(torch.rand(P, 3, generator=g) * 2.3 - 5.0)
+        sc = synth.make_scene(P, "shell-v1", 9, 3)
+        return dict(means3D=means, opacities=sc.opacities, shs=sc.shs, scales=scales, rotations=sc.rotations,
+                    features=sc.features), cam, 3
+    if family == "thresholds":                              # the z = 0.2 cull plane and the alpha = 1/255 threshold
+        W, H = 65, 49                                       # odd: the principal point is a pixel centre
+        cam = synth.make_axis_camera(W, H)
+        z02 = torch.tensor(0.2, dtype=torch.float32)
+        zs = torch.stack([torch.nextafter(z02, torch.tensor(0.0)), z02, torch.nextafter(z02, torch.tensor(1.0)),
+                          torch.tensor(0.5), torch.tensor(1.5)])
+        a = torch.tensor(1.0 / 255.0, dtype=torch.float32)
+        ops = torch.stack([torch.nextafter(a, torch.tensor(0.0)), a, torch.nextafter(a, torch.tensor(1.0)),
+                           torch.tensor(0.99), torch.tensor(1.0)])
+        zz, oo = torch.meshgrid(zs, ops, indexing="ij")
+        zz, oo = zz.reshape(-1).repeat(12), oo.reshape(-1).repeat(12)
+        P = zz.numel()
+        means = _axis_points(P, g, W, H, cam.tanfovx, zz)
+        means[:25, :2] = 0.0                                 # centred on the principal point: alpha == opacity there
+        scales = zz[:, None] * torch.exp(torch.rand(P, 3, generator=g) * 1.5 - 4.5)
+        sc = synth.make_scene(P, "shell-v1", 10, 2)
+        return dict(means3D=means, opacities=oo[:, None].contiguous(), shs=sc.shs, scales=scales,
+                    rotations=sc.rotations, features=sc.features), cam, 2
+    if family == "strip":                                   # degenerate image shapes
+        W, H = map(int, arg.split("x"))
+        sc = synth.make_scene(3_000, "shell-v1", 11, 1)
+        return dict(means3D=sc.means3D, opacities=sc.opacities, shs=sc.shs, scales=sc.scales * 2.0,
+                    rotations=sc.rotations, features=sc.features), synth.make_camera(4, W, H), 1
+    if family == "precomp":                                 # colours + covariances given, some indefinite / singular
+        P, W, H = 4_000, 160, 120
+        sc = synth.make_scene(P, "shell-v1", 12, 0)
+        cam = synth.make_axis_camera(W, H)
+        means = _axis_points(P, g, W, H, cam.tanfovx, 1.0 + 3.0 * torch.rand(P, generator=g))
+        A = torch.randn(P, 3, 3, generator=g) * 0.03
+        cov = A @ A.transpose(1, 2)
+        kind = torch.arange(P) % 5
+        ev = torch.randn(P, 3, generator=g).abs() * 1e-3
+        ev = torch.where((kind == 1)[:, None], ev * torch.tensor([1.0, -1.0, 1.0]), ev)        # indefinite
+        ev = torch.where((kind == 2)[:, None], ev * torch.tensor([1.0, 1e-7, 1e-7]), ev)       # nearly rank 1
+        ev = torch.where((kind == 3)[:, None], ev * torch.tensor([1.0, 1.0, 1e-7]), ev)        # nearly rank 2
+        # (no negative-definite covariances: their 2D radius is NaN -> 0 while they still touch a tile, and the
+        # reference then leaves those list entries unwritten, rasterizer_impl.cu:85)
+        Q = torch.linalg.qr(torch.randn(P, 3, 3, generator=g))[0]
+        cov = torch.where((kind == 0)[:, None, None], cov, Q @ torch.diag_embed(ev) @ Q.transpose(1, 2))
+        c6 = torch.stack([cov[:, 0, 0], cov[:, 0, 1], cov[:, 0, 2], cov[:, 1, 1], cov[:, 1, 2], cov[:, 2, 2]], 1)
+        # det(cov2D) == 0 exactly: a centred Gaussian whose projected x variance cancels the +0.3 low-pass term
+        fx = W / (2.0 * cam.tanfovx)
+        means[:8] = torch.tensor([0.0, 0.0, 1.0])
+        c6[:8] = torch.tensor([-0.3 / fx ** 2, 0.0, 0.0, 1e-3, 0.0, 1e-3])
+        colors = torch.rand(P, 3, generator=g)
+        return dict(means3D=means, opacities=sc.opacities, colors_precomp=colors, cov3D_precomp=c6.float(),
+                    features=None), cam, 0
+    raise KeyError(name)
+
+
+# Adversarial rasterizer cases (tests/test_raster_gpu.py, tests/golden/make_golden_live.py --only edge).  Small enough
+# for the CPU oracle; every one asserts that it reaches the path it is named for (edge_coverage).
+EDGE_CASES = (["inside-x1", "inside-x0.6", "inside-x1.8", "needles", "opaque-S0", "opaque-S5", "opaque-S16"] +
+              [f"depth-{k}" for k in ("equal", "adjacent", "narrow", "w7", "3to5", "wide")] +
+              ["thresholds"] +
+              [f"strip-{s}" for s in ("1x1", "1x37", "37x1", "7x5", "9x4", "17x33", "4100x16", "16x2050")] +
+              ["precomp"])
+
+
+def edge_case(name):
+    """Seeded inputs of one EDGE_CASES entry as numpy arrays: (oracle / run_ours keyword arguments, cotangents)."""
+    d, cam, S = _edge_scene(name)
+    bg = torch.tensor([0.0, 0.5, 1.0])
+    kw = dict(means3D=d["means3D"], opacities=d["opacities"], viewmatrix=cam.viewmatrix, projmatrix=cam.projmatrix,
+              campos=cam.campos, bg=bg, W=cam.image_width, H=cam.image_height, tan_fovx=cam.tanfovx,
+              tan_fovy=cam.tanfovy, cx=cam.cx, cy=cam.cy, features=d["features"],
+              scale_modifier=d.get("scale_modifier", 1.0))
+    for k in ("shs", "scales", "rotations", "colors_precomp", "cov3D_precomp"):
+        if k in d:
+            kw[k] = d[k]
+    kw = {k: (np.ascontiguousarray(npy(v.float())) if isinstance(v, torch.Tensor) else v) for k, v in kw.items()}
+    gen = torch.Generator().manual_seed(2)
+    H, W = cam.image_height, cam.image_width
+    cots = [npy(torch.randn(c, H, W, generator=gen)) for c in (3, 1, 1, S)]
+    return kw, cots
+
+
+def edge_stats(kw, radii, depths, conic_opacity, n_contrib, final_T, ranges):
+    """What an edge case reaches, from a rasterizer's intermediates (ours or the oracle's): the radix-sort plan of the
+    visible depth keys (common.cuh sort_plan), the fraction of visible Gaussians whose x / y view direction is clamped
+    to 1.3 tan(fov), the trace^2 / det range of the visible conics, and how many pixels stop early."""
+    vis = np.asarray(radii) > 0
+    bits = np.asarray(depths, np.float32).view(np.uint32)[vis]
+    diff = (int(np.bitwise_or.reduce(bits)) & int(np.bitwise_or.reduce(~bits))) if bits.size else 0
+    nb = diff.bit_length()
+    passes = (nb + 7) // 8
+    w = -(-nb // passes) if passes else 0
+    V = np.asarray(kw["viewmatrix"], np.float64)
+    t = np.c_[np.asarray(kw["means3D"], np.float64), np.ones(len(vis))] @ V
+    t = t[vis]
+    cx = np.abs(t[:, 0] / t[:, 2]) > 1.3 * kw["tan_fovx"]
+    cy = np.abs(t[:, 1] / t[:, 2]) > 1.3 * kw["tan_fovy"]
+    co = np.asarray(conic_opacity, np.float64)[vis]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        cond = (co[:, 0] + co[:, 2]) ** 2 / (co[:, 0] * co[:, 2] - co[:, 1] ** 2)
+    pd = (co[:, 0] > 0) & (co[:, 2] > 0) & np.isfinite(cond) & (cond > 0)
+    W, H = kw["W"], kw["H"]
+    gx = (W + 15) // 16
+    rg = np.asarray(ranges, np.int64).reshape(-1, 2)
+    lens = rg[:, 1] - rg[:, 0]
+    tile = (np.arange(H)[:, None] // 16) * gx + np.arange(W)[None, :] // 16
+    nc = np.asarray(n_contrib, np.int64).reshape(H, W)
+    fT = np.asarray(final_T, np.float32).reshape(H, W)
+    early = nc < lens[tile]
+    sat = early & (fT < 1e-2)
+    return dict(P=len(vis), visible=int(vis.sum()), passes=passes, w=w, clamp_x=float(cx.mean()) if vis.any() else 0.0,
+                clamp_y=float(cy.mean()) if vis.any() else 0.0, near=int((t[:, 2] < 0.3).sum()),
+                cond_min=float(cond[pd].min()) if pd.any() else 0.0, cond_max=float(cond[pd].max()) if pd.any() else 0.0,
+                cond_over=int((cond[pd] > 6000).sum()), cond_under=int((cond[pd] <= 6000).sum()), not_pd=int((~pd).sum()),
+                max_radius=int(np.asarray(radii).max()) if len(vis) else 0, early=int(early.sum()), saturated=int(sat.sum()),
+                sat_stop_residues=sorted(set((nc[sat] % 4).tolist())), sat_min_contrib=int(nc[sat].min()) if sat.any() else -1)
+
+
+def edge_coverage(name, s):
+    """Assert that edge case `name` still reaches the path it exists for (stats from edge_stats)."""
+    family, _, arg = name.partition("-")
+    assert s["visible"] > 0, s
+    if family == "inside":
+        assert s["passes"] == 4 and s["clamp_x"] > 0.004 and s["clamp_y"] > 0.004 and s["near"] > 100, s
+    elif family == "needles":
+        assert s["cond_over"] > 50 and s["cond_under"] > 50 and s["max_radius"] > 200, s
+    elif family == "opaque":
+        assert s["saturated"] > 1000 and s["sat_stop_residues"] == [0, 1, 2, 3] and s["sat_min_contrib"] <= 3, s
+    elif family == "depth":
+        assert (s["passes"], s["w"]) == {"equal": (0, 0), "adjacent": (1, 1), "narrow": (2, 8), "w7": (3, 7),
+                                         "3to5": (3, 8), "wide": (4, 8)}[arg], s
+    elif family == "precomp":
+        assert s["not_pd"] > 100, s
 
 
 def fixed_sample(n, k, seed):

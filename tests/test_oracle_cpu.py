@@ -11,7 +11,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import GOLDEN, case_inputs, max_rel_above_floor, npy, oracle_kwargs, rel_l2, sh_case
+from helpers import EDGE_CASES, GOLDEN, case_inputs, digest, edge_case, edge_coverage, edge_stats, max_rel_above_floor, npy, oracle_kwargs, rel_l2, sh_case
 from oracle import oracle
 
 RASTER_CASES = sorted(glob.glob(os.path.join(GOLDEN, "raster_*.npz")))
@@ -276,3 +276,30 @@ def test_sampling_oracle_pinned_to_reference_functions():
     cov = R @ torch.diag_embed(s * s) @ R.transpose(1, 2)
     full = torch.stack([ic[:, 0], ic[:, 1], ic[:, 2], ic[:, 1], ic[:, 3], ic[:, 4], ic[:, 2], ic[:, 4], ic[:, 5]], -1).view(-1, 3, 3)
     assert torch.allclose(full @ cov, torch.eye(3).expand(50, 3, 3), atol=1e-4)
+
+
+EDGE = os.path.join(GOLDEN, "live_raster_edge.npz")
+
+
+@pytest.mark.parametrize("name", EDGE_CASES)
+def test_oracle_matches_reference_on_edge_cases(name):
+    """Pins the CPU oracle's preprocess and binning on the adversarial geometry of tests/helpers.py EDGE_CASES against
+    the unmodified reference kernels (tests/golden/live_raster_edge.npz, make_golden_live.py --only edge): radii,
+    tiles_touched, the sorted keys and point list, the tile ranges, and the visible depths / means2D / conics bit-exact.
+    Also asserts, from the oracle's own intermediates, that each case reaches the path it is named for."""
+    g = np.load(EDGE)
+    key = name + "__"
+    kw, _ = edge_case(name)
+    f = oracle.rasterize_forward(**kw)
+    pre, b, img = f["pre"], f["binned"], f["img"]
+    assert b["num_rendered"] == int(g[key + "num_rendered"])
+    assert digest(pre["radii"]) == str(g[key + "dig_radii"])
+    assert digest(pre["tiles_touched"]) == str(g[key + "dig_tiles_touched"])
+    assert digest(b["point_list"]) == str(g[key + "dig_point_list"])
+    assert digest(b["keys"].view(np.int64)) == str(g[key + "dig_point_list_keys"])
+    assert digest(b["ranges"]) == str(g[key + "dig_ranges"])
+    vis = pre["radii"] > 0
+    for n in ("depths", "means2D", "conic_opacity"):
+        assert digest(np.ascontiguousarray(pre[n][vis]).view(np.int32)) == str(g[key + "dig_" + n]), n
+    edge_coverage(name, edge_stats(kw, pre["radii"], pre["depths"], pre["conic_opacity"], img["n_contrib"], img["final_T"],
+                                   b["ranges"]))
