@@ -345,6 +345,28 @@ int r3dg_knn_dist2(int P, const float* points /* [P,3] */, float* mean_dist2 /* 
                    size_t tmp_bytes, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Fused D-SSIM loss term.  Replaces `ssim(img1, img2, window_size=11, size_average)` of
+ * utils/loss_utils.py:32-63 (11x11 Gaussian window, sigma 1.5, zero padding 5, C1 = 0.01^2,
+ * C2 = 0.03^2), called every step by gaussian_renderer/render.py:150 and twice by
+ * gaussian_renderer/neilf.py:227,234, and as a metric by eval_nvs.py:72 and
+ * eval_relighting_syn4.py:191,195.  Computed in IEEE fp32 (the reference's cuDNN convolutions
+ * run in TF32 under torch's defaults); deterministic, and exactly 1 for identical images.
+ * img1 / img2 / dL_dimg1 are [N,C,H,W] contiguous.
+ *   r3dg_ssim_tmp_bytes : size of `tmp` for the forward (0 for an invalid shape);
+ *   r3dg_ssim_forward   : out = mean of the SSIM map, [1] over everything when size_average,
+ *                         else [N] per image (ssim_map.mean(1).mean(1).mean(1));
+ *   r3dg_ssim_backward  : dL_dimg1 from dL_dout ([1] or [N], read on the device).  dL/dimg2 is
+ *                         the same call with img1 and img2 swapped.
+ * R3DG_ERR_BAD_ARG for N, C, H or W <= 0, a NULL pointer or too small a tmp;
+ * R3DG_ERR_UNSUPPORTED for N*C > 65535, H*W >= 2^31 or H > 1048560.  Nothing is launched then.
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_ssim_tmp_bytes(int N, int C, int H, int W);
+int r3dg_ssim_forward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average,
+                      float* out, void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+int r3dg_ssim_backward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average,
+                       const float* dL_dout, float* dL_dimg1, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optimiser step (SURVEY.md §8f next #3).  Replaces, for all parameter groups at once, the
  * per-group `torch.optim.Adam(l, lr=0.0, eps=1e-15).step()` of scene/gaussian_model.py:489,495-497
  * (torch 1.12.1 torch/optim/adam.py:_single_tensor_adam: no weight decay, no amsgrad, no

@@ -111,6 +111,9 @@ SYMBOLS = [
     ("r3dg_compact_rows", c_int, [c_int, c_int, ctypes.POINTER(CompactTensor), c_void_p, c_void_p, c_void_p]),
     ("r3dg_knn_tmp_bytes", c_size_t, [c_int]),
     ("r3dg_knn_dist2", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_ssim_tmp_bytes", c_size_t, [c_int, c_int, c_int, c_int]),
+    ("r3dg_ssim_forward", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_ssim_backward", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     ("r3dg_adam_step", c_int, [c_int, ctypes.POINTER(AdamTensor), c_void_p]),
     ("r3dg_launch_count", ctypes.c_ulonglong, []),
     ("r3dg_tune", c_int, [ctypes.c_char_p, c_int, ctypes.POINTER(c_int)]),

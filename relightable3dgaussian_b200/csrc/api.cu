@@ -266,6 +266,21 @@ int r3dg_knn_dist2(int P, const float* points, float* mean_dist2, void* tmp, siz
     return launch_knn(P, points, mean_dist2, tmp, tmp_bytes, num_sms(), (cudaStream_t)stream);
 }
 
+// ---- utils.loss_utils.ssim ----------------------------------------------------------------------
+size_t r3dg_ssim_tmp_bytes(int N, int C, int H, int W) { return ssim_tmp_bytes(N, C, H, W); }
+int r3dg_ssim_forward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average, float* out,
+                      void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_ssim_forward(N, C, H, W, img1, img2, size_average, out, tmp, tmp_bytes, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 2;        // tiles, reduction
+    return rc;
+}
+int r3dg_ssim_backward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average,
+                       const float* dL_dout, float* dL_dimg1, r3dg_stream_t stream) {
+    const int rc = launch_ssim_backward(N, C, H, W, img1, img2, size_average, dL_dout, dL_dimg1, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 1;
+    return rc;
+}
+
 namespace {
 __global__ void unpack_rec_kernel(int P, int recf, int what, const float* __restrict__ rec,
                                   const uint32_t* __restrict__ tiles, float* __restrict__ dst) {

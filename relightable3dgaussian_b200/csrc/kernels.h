@@ -97,4 +97,11 @@ int launch_compact_rows(int P, int num, const r3dg_compact_tensor* tensors, cons
 size_t knn_tmp_bytes(int P);
 int launch_knn(int P, const float* points, float* out, void* tmp, size_t tmp_bytes, int num_sms, cudaStream_t stream);
 
+// ssim.cu: fused SSIM loss; both launchers validate every argument before launching anything
+size_t ssim_tmp_bytes(int N, int C, int H, int W);
+int launch_ssim_forward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average, float* out,
+                        void* tmp, size_t tmp_bytes, cudaStream_t stream);
+int launch_ssim_backward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average,
+                         const float* dL_dout, float* dL_dimg1, cudaStream_t stream);
+
 }  // namespace r3dg
