@@ -367,6 +367,39 @@ int r3dg_ssim_backward(int N, int C, int H, int W, const float* img1, const floa
                        const float* dL_dout, float* dL_dimg1, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Fused smoothness regularisers of utils/loss_utils.py, computed in IEEE fp32 (the reference's
+ * kornia convolutions run in TF32 under torch's defaults), deterministic, no float atomics.
+ *
+ * first_order_edge_aware_loss(data, img) (:104-105; gaussian_renderer/render.py:170,
+ * gaussian_renderer/neilf.py:284,291,299):
+ *   out[0] = 1/(C H W) sum_{c,y,x} sum_{d in x,y} |S_d(data_c)| * exp(-|S_d(img_c)|),
+ * S_d the Sobel response divided by 8 with replicate padding of 1 (kornia spatial_gradient,
+ * normalized).  data is [Cd,H,W], img [Ci,H,W], both contiguous; Cd and Ci are each 1 or
+ * C = max(Cd, Ci), a 1-channel input being broadcast (torch broadcasting).
+ *   r3dg_edge_aware_tmp_bytes : size of `tmp` for the forward (0 for an invalid shape);
+ *   r3dg_edge_aware_backward  : dL_ddata [Cd,H,W] and / or dL_dimg [Ci,H,W] (either may be NULL,
+ *                               not both) from dL_dout ([1], read on the device); a 1-channel
+ *                               input's gradient is summed over the C channels.
+ * R3DG_ERR_BAD_ARG for Cd, Ci, H or W <= 0, channel counts that do not broadcast, a NULL pointer
+ * or too small a tmp; R3DG_ERR_UNSUPPORTED for C > 65535, H*W >= 2^31 or H > 1048560.
+ *
+ * tv_loss(x) (:113-117; gaussian_renderer/neilf.py:306,312), x [B,H,W] contiguous:
+ *   out[0] = mean((x[:,1:,:] - x[:,:-1,:])^2) + mean((x[:,:,1:] - x[:,:,:-1])^2).
+ * R3DG_ERR_BAD_ARG for B <= 0, H or W < 2 (the reference returns NaN there), a NULL pointer or
+ * too small a tmp; R3DG_ERR_UNSUPPORTED for B > 65535 or H*W >= 2^31.
+ *
+ * The forwards launch 2 kernels, the backwards 1.  Nothing is launched on an error.
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_edge_aware_tmp_bytes(int Cd, int Ci, int H, int W);
+int r3dg_edge_aware_forward(int Cd, int Ci, int H, int W, const float* data, const float* img, float* out, void* tmp,
+                            size_t tmp_bytes, r3dg_stream_t stream);
+int r3dg_edge_aware_backward(int Cd, int Ci, int H, int W, const float* data, const float* img, const float* dL_dout,
+                             float* dL_ddata, float* dL_dimg, r3dg_stream_t stream);
+size_t r3dg_tv_tmp_bytes(int B, int H, int W);
+int r3dg_tv_forward(int B, int H, int W, const float* x, float* out, void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+int r3dg_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, float* dL_dx, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optimiser step (SURVEY.md §8f next #3).  Replaces, for all parameter groups at once, the
  * per-group `torch.optim.Adam(l, lr=0.0, eps=1e-15).step()` of scene/gaussian_model.py:489,495-497
  * (torch 1.12.1 torch/optim/adam.py:_single_tensor_adam: no weight decay, no amsgrad, no

@@ -114,6 +114,12 @@ SYMBOLS = [
     ("r3dg_ssim_tmp_bytes", c_size_t, [c_int, c_int, c_int, c_int]),
     ("r3dg_ssim_forward", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("r3dg_ssim_backward", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    ("r3dg_edge_aware_tmp_bytes", c_size_t, [c_int, c_int, c_int, c_int]),
+    ("r3dg_edge_aware_forward", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_edge_aware_backward", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    ("r3dg_tv_tmp_bytes", c_size_t, [c_int, c_int, c_int]),
+    ("r3dg_tv_forward", c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_tv_backward", c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_adam_step", c_int, [c_int, ctypes.POINTER(AdamTensor), c_void_p]),
     ("r3dg_launch_count", ctypes.c_ulonglong, []),
     ("r3dg_tune", c_int, [ctypes.c_char_p, c_int, ctypes.POINTER(c_int)]),

@@ -281,6 +281,32 @@ int r3dg_ssim_backward(int N, int C, int H, int W, const float* img1, const floa
     return rc;
 }
 
+// ---- utils.loss_utils.first_order_edge_aware_loss / tv_loss ---------------------------------------
+size_t r3dg_edge_aware_tmp_bytes(int Cd, int Ci, int H, int W) { return edge_aware_tmp_bytes(Cd, Ci, H, W); }
+int r3dg_edge_aware_forward(int Cd, int Ci, int H, int W, const float* data, const float* img, float* out, void* tmp,
+                            size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_edge_aware_forward(Cd, Ci, H, W, data, img, out, tmp, tmp_bytes, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 2;        // tiles, reduction
+    return rc;
+}
+int r3dg_edge_aware_backward(int Cd, int Ci, int H, int W, const float* data, const float* img, const float* dL_dout,
+                             float* dL_ddata, float* dL_dimg, r3dg_stream_t stream) {
+    const int rc = launch_edge_aware_backward(Cd, Ci, H, W, data, img, dL_dout, dL_ddata, dL_dimg, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 1;
+    return rc;
+}
+size_t r3dg_tv_tmp_bytes(int B, int H, int W) { return tv_tmp_bytes(B, H, W); }
+int r3dg_tv_forward(int B, int H, int W, const float* x, float* out, void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_tv_forward(B, H, W, x, out, tmp, tmp_bytes, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 2;        // blocks, reduction
+    return rc;
+}
+int r3dg_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, float* dL_dx, r3dg_stream_t stream) {
+    const int rc = launch_tv_backward(B, H, W, x, dL_dout, dL_dx, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 1;
+    return rc;
+}
+
 namespace {
 __global__ void unpack_rec_kernel(int P, int recf, int what, const float* __restrict__ rec,
                                   const uint32_t* __restrict__ tiles, float* __restrict__ dst) {

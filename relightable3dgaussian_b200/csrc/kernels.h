@@ -104,4 +104,14 @@ int launch_ssim_forward(int N, int C, int H, int W, const float* img1, const flo
 int launch_ssim_backward(int N, int C, int H, int W, const float* img1, const float* img2, int size_average,
                          const float* dL_dout, float* dL_dimg1, cudaStream_t stream);
 
+// smooth.cu: edge-aware smoothness and TV losses; every launcher validates its arguments before launching anything
+size_t edge_aware_tmp_bytes(int Cd, int Ci, int H, int W);
+int launch_edge_aware_forward(int Cd, int Ci, int H, int W, const float* data, const float* img, float* out, void* tmp,
+                              size_t tmp_bytes, cudaStream_t stream);
+int launch_edge_aware_backward(int Cd, int Ci, int H, int W, const float* data, const float* img, const float* dL_dout,
+                               float* dL_ddata, float* dL_dimg, cudaStream_t stream);
+size_t tv_tmp_bytes(int B, int H, int W);
+int launch_tv_forward(int B, int H, int W, const float* x, float* out, void* tmp, size_t tmp_bytes, cudaStream_t stream);
+int launch_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, float* dL_dx, cudaStream_t stream);
+
 }  // namespace r3dg

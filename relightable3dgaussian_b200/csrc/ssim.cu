@@ -11,6 +11,7 @@
 // contract it into FMAs: every op is rounded on its own, as in the reference's chain of PyTorch kernels.
 #include "common.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace r3dg {
 namespace {
@@ -109,7 +110,6 @@ __global__ void __launch_bounds__(NT) ssim_fwd_kernel(int H, int W, const float*
     constexpr int SR = TH + 2 * R, SC = TW + 2 * R;
     __shared__ float sx[SR * SC], sy[SR * SC];
     __shared__ float h[5 * SR * TW];
-    __shared__ double warp_sum[NT / 32];
     const size_t plane = (size_t)blockIdx.z * H * W;
     const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
     stage(x + plane, y + plane, H, W, y0 - R, x0 - R, SR, SC, sx, sy);
@@ -125,32 +125,7 @@ __global__ void __launch_bounds__(NT) ssim_fwd_kernel(int H, int W, const float*
             acc += (double)ssim_map(q).m;
         }
     }
-    // fixed-order CTA sum: butterfly within each warp, then the warps in index order
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int w = 0; w < NT / 32; ++w) s += warp_sum[w];
-        partial[((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = s;
-    }
-}
-
-// out[b] = sum(partial[b * per .. (b+1) * per)) / count, one CTA per output, fixed summation order
-__global__ void __launch_bounds__(NT) ssim_reduce_kernel(const double* __restrict__ partial, long long per, double count,
-                                                         float* __restrict__ out) {
-    __shared__ double s[NT];
-    const double* p = partial + (size_t)blockIdx.x * per;
-    double acc = 0.0;
-    for (long long i = threadIdx.x; i < per; i += NT) acc += p[i];
-    s[threadIdx.x] = acc;
-    __syncthreads();
-    for (int o = NT / 2; o > 0; o >>= 1) {
-        if (threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) out[blockIdx.x] = (float)(s[0] / count);
+    cta_partial<NT>(acc, partial + ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
 }
 
 // dL/dx = s * (G*alpha + 2x (G*beta) + y (G*gamma)) over in-image pixels, with the map terms
@@ -252,7 +227,7 @@ int launch_ssim_forward(int N, int C, int H, int W, const float* img1, const flo
     const long long per_image = (long long)gr.x * gr.y * C;
     const int outs = size_average ? 1 : N;
     const double count = (double)C * H * W * (size_average ? N : 1);
-    ssim_reduce_kernel<<<outs, NT, 0, stream>>>(partial, per_image * N / outs, count, out);
+    reduce_partials_kernel<<<outs, kReduceNT, 0, stream>>>(partial, per_image * N / outs, count, out);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }
