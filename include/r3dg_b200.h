@@ -291,6 +291,64 @@ int r3dg_compact_rows(int P, int num_tensors, const r3dg_compact_tensor* tensors
                       const void* tmp, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Stage-1 densification: `GaussianModel.add_densification_stats` and `densify_and_prune`
+ * (scene/gaussian_model.py:890-937); the host side is relightable3dgaussian_b200/densify.py.
+ *
+ * r3dg_densify_stats: in place, for all P rows, weights_accum += weights and, where
+ *   update_filter[i] != 0, xyz_gradient_accum += |viewspace_grad[i, 0:2]|, normal_gradient_accum +=
+ *   |normal_grad[i]|, denom += 1, and (radii != NULL) max_radii2D = max(max_radii2D, radii).
+ *   viewspace_grad rows are grad_stride floats apart (>= 2); radii and max_radii2D are both NULL or
+ *   both given.  One launch, no host synchronisation.
+ *
+ * r3dg_densify_classify: per row, the clone / split sets and which of the row's output rows survive
+ *   the final prune (the thresholds are the reference's Python floats rounded to fp32; see
+ *   densify.py for their derivation), then a scan of the four output segments.  Copies 7 ints to
+ *   the pinned host array `totals_host` (may be NULL) asynchronously on `stream`:
+ *     [0] kept originals (segment A)  [1] kept clones (B)  [2] split rows whose copies are kept (C)
+ *     [3] |S|  [4] |C|  [5] originals whose normal gradient passes the normal threshold
+ *     [6] unsplit originals with weights_accum < weights_threshold
+ *   The final row count is [0] + [1] + 2 [2].  3 launches (1 for P = 0).
+ *
+ * r3dg_densify_apply: writes every output tensor in one launch from the classify results in `tmp`
+ *   and `totals` (the host copy of the 7 totals).  Output rows: kept originals, kept clones, split
+ *   copy 1, split copy 2, each in row order; split copy c of the k-th split row uses
+ *   samples[c |S| + k] ([2|S|,3] standard normals).  Kinds: COPY (every new row a copy), MOMENT (new
+ *   rows zero), XYZ (split copies: R(q) (z * exp(s)) + x, from `rotation` [P,4] and `scaling` [P,3]),
+ *   SCALING (split copies: log(exp(s) * split_recip)), ZERO (dst only: all final rows zero).
+ *   At most R3DG_DENSIFY_MAX tensors; row_bytes a multiple of 4 (12 for XYZ / SCALING).
+ * Bad arguments return R3DG_ERR_BAD_ARG before anything is launched.
+ * ------------------------------------------------------------------------------------------ */
+#define R3DG_DENSIFY_MAX 48
+enum { R3DG_DENSIFY_COPY = 0, R3DG_DENSIFY_MOMENT = 1, R3DG_DENSIFY_XYZ = 2, R3DG_DENSIFY_SCALING = 3, R3DG_DENSIFY_ZERO = 4 };
+typedef struct r3dg_densify_tensor {
+    const void* src;               /* [P, row_bytes] (unused for ZERO) */
+    void* dst;                     /* [P', row_bytes] */
+    long long row_bytes;
+    int kind;
+} r3dg_densify_tensor;
+typedef struct r3dg_densify_thresholds {
+    float max_grad, max_grad_normal;   /* gradient thresholds of clone and split */
+    float dense_scale;                 /* percent_dense * extent: clone if max scale <=, split if > */
+    float min_opacity, weights_threshold;
+    float max_screen_size;             /* used when check_size != 0 */
+    float big_scale;                   /* 0.1 * extent, used when check_size != 0 */
+    float split_recip;                 /* fp32 reciprocal of 0.8 * 2: split copies' scale factor */
+    int check_size;
+} r3dg_densify_thresholds;
+int r3dg_densify_stats(int P, const float* viewspace_grad, int grad_stride, const float* normal_grad,
+                       const uint8_t* update_filter, const float* weights, const int32_t* radii,
+                       float* weights_accum, float* xyz_gradient_accum, float* normal_gradient_accum,
+                       float* denom, float* max_radii2D, r3dg_stream_t stream);
+size_t r3dg_densify_tmp_bytes(int P);
+int r3dg_densify_classify(int P, const float* xyz_gradient_accum, const float* normal_gradient_accum,
+                          const float* denom, const float* weights_accum, const float* scaling,
+                          const float* opacity, const r3dg_densify_thresholds* thresholds, void* tmp,
+                          size_t tmp_bytes, int* totals_host, r3dg_stream_t stream);
+int r3dg_densify_apply(int P, const int* totals, int num_tensors, const r3dg_densify_tensor* tensors,
+                       const float* rotation, const float* scaling, const float* samples, float split_recip,
+                       const void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * BRDF shading: fused `rendering_equation` (gaussian_renderer/neilf.py:339-371) + `GGX_specular`
  * (:374-406) + lat-long environment lookup (scene/direct_light_map.py:70-83) + SH incident light.
  * The reference has no extension boundary here (pure PyTorch; its render_equation.cu is dead,

@@ -72,6 +72,16 @@ class CompactTensor(ctypes.Structure):
     _fields_ = [("src", c_void_p), ("dst", c_void_p), ("row_bytes", c_ll)]
 
 
+class DensifyTensor(ctypes.Structure):
+    _fields_ = [("src", c_void_p), ("dst", c_void_p), ("row_bytes", c_ll), ("kind", c_int)]
+
+
+class DensifyThresholds(ctypes.Structure):
+    _fields_ = ([(n, c_float) for n in ("max_grad", "max_grad_normal", "dense_scale", "min_opacity", "weights_threshold",
+                                        "max_screen_size", "big_scale", "split_recip")] +
+                [("check_size", c_int)])
+
+
 class AdamTensor(ctypes.Structure):
     _fields_ = ([(n, c_void_p) for n in ("param", "grad", "exp_avg", "exp_avg_sq")] +
                 [("n", c_ll), ("step", c_ll)] +
@@ -109,6 +119,13 @@ SYMBOLS = [
     ("r3dg_compact_tmp_bytes", c_size_t, [c_int]),
     ("r3dg_compact_scan", c_int, [c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     ("r3dg_compact_rows", c_int, [c_int, c_int, ctypes.POINTER(CompactTensor), c_void_p, c_void_p, c_void_p]),
+    ("r3dg_densify_stats", c_int, [c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p, c_void_p, c_void_p]),
+    ("r3dg_densify_tmp_bytes", c_size_t, [c_int]),
+    ("r3dg_densify_classify", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      ctypes.POINTER(DensifyThresholds), c_void_p, c_size_t, c_void_p, c_void_p]),
+    ("r3dg_densify_apply", c_int, [c_int, ctypes.POINTER(c_int), c_int, ctypes.POINTER(DensifyTensor), c_void_p, c_void_p,
+                                   c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
     ("r3dg_knn_tmp_bytes", c_size_t, [c_int]),
     ("r3dg_knn_dist2", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("r3dg_ssim_tmp_bytes", c_size_t, [c_int, c_int, c_int, c_int]),

@@ -258,6 +258,36 @@ int r3dg_compact_rows(int P, int num_tensors, const r3dg_compact_tensor* tensors
     return launch_compact_rows(P, num_tensors, tensors, keep, tmp, num_sms(), (cudaStream_t)stream);
 }
 
+// ---- GaussianModel.add_densification_stats / densify_and_prune ------------------------------------
+int r3dg_densify_stats(int P, const float* viewspace_grad, int grad_stride, const float* normal_grad,
+                       const uint8_t* update_filter, const float* weights, const int32_t* radii, float* weights_accum,
+                       float* xyz_gradient_accum, float* normal_gradient_accum, float* denom, float* max_radii2D,
+                       r3dg_stream_t stream) {
+    const int rc = launch_densify_stats(P, viewspace_grad, grad_stride, normal_grad, update_filter, weights, radii, weights_accum,
+                                        xyz_gradient_accum, normal_gradient_accum, denom, max_radii2D, (cudaStream_t)stream);
+    if (rc == 0 && P > 0) g_launches += 1;
+    return rc;
+}
+size_t r3dg_densify_tmp_bytes(int P) { return densify_tmp_bytes(P < 0 ? 0 : P); }
+int r3dg_densify_classify(int P, const float* xyz_gradient_accum, const float* normal_gradient_accum, const float* denom,
+                          const float* weights_accum, const float* scaling, const float* opacity,
+                          const r3dg_densify_thresholds* thresholds, void* tmp, size_t tmp_bytes, int* totals_host,
+                          r3dg_stream_t stream) {
+    if (!thresholds) return R3DG_ERR_BAD_ARG;
+    const int rc = launch_densify_classify(P, xyz_gradient_accum, normal_gradient_accum, denom, weights_accum, scaling, opacity,
+                                           *thresholds, tmp, tmp_bytes, totals_host, (cudaStream_t)stream);
+    if (rc == 0) g_launches += P > 0 ? 3 : 1;     // classify, scan, offsets
+    return rc;
+}
+int r3dg_densify_apply(int P, const int* totals, int num_tensors, const r3dg_densify_tensor* tensors, const float* rotation,
+                       const float* scaling, const float* samples, float split_recip, const void* tmp, size_t tmp_bytes,
+                       r3dg_stream_t stream) {
+    const int rc = launch_densify_apply(P, totals, num_tensors, tensors, rotation, scaling, samples, split_recip, tmp, tmp_bytes,
+                                        num_sms(), (cudaStream_t)stream);
+    if (rc == 0 && P > 0 && num_tensors > 0) g_launches += 1;
+    return rc;
+}
+
 // ---- simple_knn._C.distCUDA2 ----------------------------------------------------------------
 size_t r3dg_knn_tmp_bytes(int P) { return knn_tmp_bytes(P); }
 int r3dg_knn_dist2(int P, const float* points, float* mean_dist2, void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {

@@ -6,6 +6,7 @@
 // bytes once.  Row order is preserved (stable), exactly what boolean indexing gives.
 #include "common.cuh"
 #include "kernels.h"
+#include "scan.cuh"
 
 namespace r3dg {
 
@@ -44,38 +45,6 @@ __global__ void __launch_bounds__(CMP_THREADS) compact_block_sums_kernel(int P, 
         for (int w = 0; w < CMP_THREADS / 32; ++w) t += s_warp[w];
         block_sums[blockIdx.x] = t;
     }
-}
-
-// single CTA: exclusive scan of the block sums in place, total at the end
-__global__ void __launch_bounds__(1024) compact_scan_sums_kernel(long long n, uint32_t* __restrict__ block_sums,
-                                                                 uint32_t* __restrict__ total, int* count_host) {
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_carry;
-    if (threadIdx.x == 0) s_carry = 0;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (long long base = 0; base < n; base += 1024) {
-        const long long i = base + threadIdx.x;
-        const uint32_t v = i < n ? block_sums[i] : 0u;
-        uint32_t inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-        if (lane == 31) s_warp[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t w = s_warp[lane], winc = w;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += t; }
-            s_warp[lane] = winc - w;                       // exclusive prefix of the warp totals
-        }
-        __syncthreads();
-        const uint32_t excl = s_carry + s_warp[warp] + inc - v;
-        if (i < n) block_sums[i] = excl;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) { *total = s_carry; if (count_host) *count_host = (int)s_carry; }
 }
 
 __global__ void __launch_bounds__(CMP_THREADS) compact_offsets_kernel(int P, const uint8_t* __restrict__ keep,
@@ -130,7 +99,7 @@ int launch_compact_scan(int P, const uint8_t* keep, void* tmp_, size_t tmp_bytes
     uint32_t* sums = (uint32_t*)(tmp + t.block_sums);
     uint32_t* total = (uint32_t*)(tmp + t.total_off);
     if (P > 0) compact_block_sums_kernel<<<(unsigned)t.nblocks, CMP_THREADS, 0, stream>>>(P, keep, sums);
-    compact_scan_sums_kernel<<<1, 1024, 0, stream>>>(P > 0 ? t.nblocks : 0, sums, total, nullptr);
+    block_sums_scan_kernel<1><<<1, 1024, 0, stream>>>(P > 0 ? t.nblocks : 0, 0, sums, total);
     if (P > 0) compact_offsets_kernel<<<(unsigned)t.nblocks, CMP_THREADS, 0, stream>>>(P, keep, sums, (uint32_t*)(tmp + t.offsets));
     if (count_host) R3DG_CUDA_TRY(cudaMemcpyAsync(count_host, total, sizeof(int), cudaMemcpyDeviceToHost, stream));
     R3DG_CUDA_TRY(cudaGetLastError());

@@ -94,6 +94,19 @@ int launch_compact_scan(int P, const uint8_t* keep, void* tmp, size_t tmp_bytes,
 int launch_compact_rows(int P, int num, const r3dg_compact_tensor* tensors, const uint8_t* keep, const void* tmp,
                         int num_sms, cudaStream_t stream);
 
+// densify.cu: stage-1 densification statistics and densify-and-prune; launchers validate before launching
+size_t densify_tmp_bytes(int P);
+int launch_densify_stats(int P, const float* vgrad, int stride, const float* ngrad, const uint8_t* filter, const float* weights,
+                         const int32_t* radii, float* weights_accum, float* xyz_accum, float* normal_accum, float* denom,
+                         float* max_radii2D, cudaStream_t stream);
+int launch_densify_classify(int P, const float* xyz_accum, const float* normal_accum, const float* denom,
+                            const float* weights_accum, const float* scaling, const float* opacity,
+                            const r3dg_densify_thresholds& th, void* tmp, size_t tmp_bytes, int* totals_host,
+                            cudaStream_t stream);
+int launch_densify_apply(int P, const int* totals, int num, const r3dg_densify_tensor* tensors, const float* rotation,
+                         const float* scaling, const float* samples, float split_recip, const void* tmp, size_t tmp_bytes,
+                         int num_sms, cudaStream_t stream);
+
 size_t knn_tmp_bytes(int P);
 int launch_knn(int P, const float* points, float* out, void* tmp, size_t tmp_bytes, int num_sms, cudaStream_t stream);
 
