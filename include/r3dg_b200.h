@@ -71,11 +71,12 @@ typedef struct r3dg_raster_fwd_args {
     void* geom;   size_t geom_bytes;
     void* img;    size_t img_bytes;
     void* binning; size_t binning_bytes;
-    /* Pinned HOST int receiving num_rendered via an async copy on `stream` (may be NULL).
+    /* Pinned HOST int receiving num_rendered (may be NULL): page-locked memory is written directly by the
+     * binning kernel that computes the count, other host memory by an async copy on `stream`.
      * num_rendered > capacity means the binning buffer was too small: outputs are invalid and
      * the call must be repeated with a larger buffer (nothing out of bounds is ever written). */
     int* num_rendered_host;
-    /* optional cudaEvent_t: recorded on `stream` right after the copy into num_rendered_host has been enqueued, which
+    /* optional cudaEvent_t: recorded on `stream` right after the write into num_rendered_host has been enqueued, which
      * happens as soon as the instance count exists on the device (after the binning offsets, ~1/4 into the forward) —
      * a host that waits on this event instead of the stream gets the count while the compositor is still running and
      * can already enqueue what follows the forward.  NULL: not used. */
@@ -177,6 +178,11 @@ int r3dg_mark_visible(int P, const float* means3D, const float* viewmatrix,
  *      10 point_list_keys u64[R] | 13 final_T f32[HW] | 14 n_contrib i32[HW] | 15 ranges u32[2T]
  *      (ours only) 16 bwd_work u32[2T]: entries composited by the busiest warp of each half-tile
  *      CTA | 17 bwd_order u32[2T]: the backward compositor's launch order (valid after a backward)
+ *      | 18 bmask u8[R]: per list entry, bit b = 8x4 pixel block b of the entry's tile (row b >> 1,
+ *      column b & 1) meets the Gaussian's block rectangle | 19 cmask u8[R]: per list entry, bit b =
+ *      block b composited the entry in the forward | 20 brects u32[2P]: per Gaussian the inclusive
+ *      block rectangle {bx0 | bx1 << 16, by0 | by1 << 16} (empty when bx0 > bx1)
+ *      (9, 18, 19: the copy stops at max_bytes, pass R entries' worth)
  * Returns bytes written or a negative error. */
 long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom,
                                  const void* img, const void* binning, size_t binning_bytes,

@@ -63,7 +63,6 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     char* geom = (char*)a->geom;
     char* img = (char*)a->img;
     char* bin = (char*)a->binning;
-    const int tiles = ((a->W + R3DG_TILE - 1) / R3DG_TILE) * ((a->H + R3DG_TILE - 1) / R3DG_TILE);
     R3DG_CUDA_TRY(cudaMemsetAsync(geom + gl.header, 0, sizeof(GeomHeader), stream));
     int rc = 0;
     auto mark = [](int i, cudaStream_t s) { prof_mark(true, i, s); };
@@ -73,19 +72,18 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
         prof_mark(true, 1, stream);
         if ((rc = launch_binning(a->P, a->W, a->H, geom, gl, img, il, bin, bl, num_sms(), stream, mark, a->num_rendered_host,
                                  a->count_ready_event)) != 0) return rc;
-        g_launches += 1 + (1 + R3DG_SORT_MAX_PASSES) + 5;   // project; histogram + radix passes; count, colsum, starts, apply, scatter
+        g_launches += 1 + (1 + R3DG_SORT_MAX_PASSES) + 4;   // project; histogram + radix passes; count, colsum + starts, apply, scatter
     } else {
-        R3DG_CUDA_TRY(cudaMemsetAsync(img + il.ranges, 0, (size_t)tiles * 8, stream));
+        if ((rc = launch_empty_binning(a->W, a->H, geom, gl, img, il, stream)) != 0) return rc;
         for (int i = 1; i <= 4; ++i) prof_mark(true, i, stream);
+        g_launches += 1;                                    // starts (empty ranges, tile order)
     }
-    if ((rc = launch_tile_order(img + il.ranges, (uint32_t*)(img + il.tile_order), (uint32_t*)(img + il.bwd_work), tiles, stream)) != 0) return rc;
-    if (a->P > 0 && (rc = launch_block_masks(a->W, a->H, gl, il, geom, img, bin, bl, stream)) != 0) return rc;
     prof_mark(true, 5, stream);
     if ((rc = launch_composite_forward(*a, gl, il, bin, bl, stream, mark)) != 0) return rc;
     prof_mark(true, 7, stream);
-    g_launches += 2 + (a->P > 0 ? 1 : 0) + (a->computer_pseudo_normal ? 1 : 0);   // tile order, block masks, composite, normals
+    g_launches += 1 + (a->computer_pseudo_normal ? 1 : 0);   // composite, normals
     if (g_prof.on) g_prof.fwd_calls++;
-    if (a->P == 0) {      // (P > 0: the count was copied, and the event recorded, as soon as the binning offsets existed)
+    if (a->P == 0) {      // (P > 0: the count was written, and the event recorded, as soon as the binning offsets existed)
         if (a->num_rendered_host) R3DG_CUDA_TRY(cudaMemcpyAsync(a->num_rendered_host, geom + gl.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
         if (a->count_ready_event) R3DG_CUDA_TRY(cudaEventRecord((cudaEvent_t)a->count_ready_event, stream));
     }
@@ -403,12 +401,15 @@ long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void*
         case 15: return copy(img + il.ranges, 8 * (size_t)tiles);
         case 16: return copy(img + il.bwd_work, 8 * (size_t)tiles);
         case 17: return copy(img + il.bwd_order, 8 * (size_t)tiles);
-        case 9: case 10: {
+        case 20: return copy(geom + gl.brects, 8 * (size_t)P);
+        case 9: case 10: case 18: case 19: {
             const long long capacity = bin_capacity_for_bytes(binning_bytes);
             if (capacity < 1) return -1;
             const BinLayout bl(capacity);
             // caller limits the copy to R entries through max_bytes
             if (id == 9) return copy(bin + bl.point_list, std::min((size_t)max_bytes, (size_t)capacity * 4));
+            if (id == 18) return copy(bin + bl.bmask, std::min((size_t)max_bytes, (size_t)capacity));
+            if (id == 19) return copy(bin + bl.cmask, std::min((size_t)max_bytes, (size_t)capacity));
             // reference binningState.point_list_keys (sorted): rebuilt from the lists
             const long long limit = std::min(max_bytes / 8, capacity);
             if (launch_rebuild_keys(tiles, img + il.ranges, (const uint32_t*)(bin + bl.point_list), rec, gl.recf, limit,

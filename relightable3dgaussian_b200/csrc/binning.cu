@@ -11,11 +11,14 @@
 // passes over the depth-sorted sequence cut into chunks (one CTA per chunk, per-tile tables in
 // shared memory):
 //   bin_count                  : M[chunk][tile] = number of instances the chunk adds to the tile;
-//   bin_colsum/starts/apply    : exclusive scan of every column of M (per tile over the chunks),
-//                                exclusive scan of the tile totals -> ranges[tile], R; M becomes the
-//                                absolute first slot of (chunk, tile);
-//   bin_scatter                : every chunk re-walks its Gaussians and writes each instance to
-//                                M[chunk][tile] + (rank inside the chunk, in sequence order).
+//   bin_colsum(+starts)/apply  : exclusive scan of every column of M (per tile over the chunks),
+//                                exclusive scan of the tile totals -> ranges[tile], R, and the
+//                                compositors' tile order; M becomes the absolute first slot of
+//                                (chunk, tile), row M[chunks] the end of every tile's list;
+//   bin_scatter                : every chunk takes its per-tile counts from two rows of M, re-walks its
+//                                Gaussians and writes each instance to M[chunk][tile] + (rank inside
+//                                the chunk, in sequence order), with its block mask and a zeroed
+//                                contributor mask.
 // Equal (tile, depth) keys end up in Gaussian-index order, exactly as the reference's stable sort
 // leaves them, so point_list and ranges are bit-identical.
 #include <algorithm>
@@ -28,7 +31,8 @@ namespace r3dg {
 // bin_count: one CTA per chunk, one thread per Gaussian walking its own rectangle; counting
 // needs no order, so the lanes work on different Gaussians in parallel with fire-and-forget
 // shared atomics on the CTA's table.
-__global__ void __launch_bounds__(256) bin_count_kernel(int P, int T, int gx, int CH,
+#define BIN_COUNT_THREADS 512       // the grid is one CTA per chunk, fewer than 4 per SM at the headline
+__global__ void __launch_bounds__(BIN_COUNT_THREADS) bin_count_kernel(int P, int T, int gx, int CH,
                                                         const GeomHeader* __restrict__ header,
                                                         const uint32_t* __restrict__ vals_a,
                                                         const uint32_t* __restrict__ vals_b,
@@ -62,27 +66,42 @@ __global__ void __launch_bounds__(256) bin_count_kernel(int P, int T, int gx, in
 // bin_scatter: one CTA per chunk.  Writing every instance straight to its slot costs one 4-byte
 // L2 write transaction per instance (~8M scattered sector writes at the headline config, whatever
 // the ranking logic).  Instead the chunk's instances are first gathered in shared memory grouped by tile:
-//   1. recount the chunk per tile (as bin_count), exclusive scan -> local CSR offsets;
+//   1. per-tile counts of the chunk = M[chunk + 1][tile] - M[chunk][tile] (bin_apply left the absolute
+//      first slots there, and the list ends in the row after the last chunk), exclusive scan -> local
+//      CSR offsets;
 //   2. unordered append: one thread per Gaussian, slot = shared atomicAdd on the tile's cursor,
-//      entry = {Gaussian id, tile << 16 | position in the chunk};
+//      entry = tile << 16 | position in the chunk (4 bytes); the Gaussian's id and block rectangle
+//      are staged once per position;
 //   3. one thread per staged entry: rank = number of entries of its run (same tile) that come
 //      earlier in the sequence; global slot = M[chunk][tile] + rank.  A warp's lanes hold
 //      consecutive staged entries, i.e. whole runs, whose global slots are contiguous: the
-//      stores coalesce into a few sectors per run instead of one transaction per entry.
+//      stores (id, block mask byte, zeroed contributor mask byte) coalesce into a few sectors per
+//      run instead of one transaction per entry.
 // A chunk whose instances exceed the staging area is handled in several windows of tiles.
 #define BIN_SCATTER_THREADS 1024
 #define BIN_LONG_RUN 24            // runs longer than this are ranked through the bitmap
 #define BIN_MAX_LONG 2048          // >= staging capacity / BIN_LONG_RUN
 
+// t / gx for t, gx < 2^16 as a multiply-high: gx_inv = 2^32 / gx + 1 (exact, the error stays below 2^-16 < 1 / gx)
+__device__ __forceinline__ uint32_t tile_row(int t, unsigned long long gx_inv) {
+    return (uint32_t)(((unsigned long long)(uint32_t)t * gx_inv) >> 32);
+}
+
 __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
-    int P, int T, int gx, int CH, int cap, const GeomHeader* __restrict__ header, const uint32_t* __restrict__ vals_a,
-    const uint32_t* __restrict__ vals_b, const uint2* __restrict__ rects, const uint32_t* __restrict__ M,
-    uint32_t* __restrict__ point_list, long long capacity) {
+    int P, int T, int gx, unsigned long long gx_inv, int CH, int cap, const GeomHeader* __restrict__ header,
+    const uint32_t* __restrict__ vals_a,
+    const uint32_t* __restrict__ vals_b, const uint2* __restrict__ rects, const uint2* __restrict__ brects,
+    const uint32_t* __restrict__ M, uint32_t* __restrict__ point_list, uint8_t* __restrict__ bmask,
+    uint8_t* __restrict__ cmask, long long capacity, int starts_in_smem) {
     extern __shared__ __align__(16) uint32_t bin_smem[];
+    const size_t T4 = ((size_t)T + 3) & ~(size_t)3;
     uint32_t* a = bin_smem;                               // [T] counts -> exclusive offsets -> cursors
+    uint32_t* s_start = bin_smem + T4;                    // [T] (if it fits) copy of the chunk's row of M
     const int words = (CH + 31) >> 5;                     // bitmap over the chunk positions, per warp
-    uint32_t* bitmaps = bin_smem + (((size_t)T + 3) & ~(size_t)3);
-    uint2* stage = reinterpret_cast<uint2*>(bitmaps + (size_t)(BIN_SCATTER_THREADS / 32) * 2 * words);
+    uint32_t* bitmaps = s_start + (starts_in_smem ? T4 : 0);
+    uint32_t* s_id = bitmaps + (size_t)(BIN_SCATTER_THREADS / 32) * 2 * words;     // [CH] Gaussian id per position
+    uint2* s_br = reinterpret_cast<uint2*>(s_id + CH);                             // [CH] its block rectangle
+    uint32_t* stage = reinterpret_cast<uint32_t*>(s_br + CH);                      // [cap] tile << 16 | position
     __shared__ uint32_t s_warp[BIN_SCATTER_THREADS / 32];
     __shared__ int s_hi;
     __shared__ uint32_t s_total, s_nlong;
@@ -92,23 +111,14 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
     const int c = blockIdx.x;
     const int j0 = c * CH, j1 = min(P, j0 + CH);
     const uint32_t* __restrict__ row = M + (size_t)c * T;
-    for (int t = tid; t < T; t += BIN_SCATTER_THREADS) a[t] = 0u;
-    __syncthreads();
     // ---- 1. per-tile counts of the chunk, exclusive scan over the tiles --------------------------
-    for (int j = j0 + tid; j < j1; j += BIN_SCATTER_THREADS) {
-        const uint2 r = rects[order[j]];
-        const uint32_t w = r.y & 0xffffu, h = r.y >> 16;
-        // one flat loop over the w*h tiles (lanes have different rectangles: nested loops would
-        // serialise max(h) * max(w) trips per warp instead of max(w*h))
-        uint32_t tile = (r.x >> 16) * (uint32_t)gx + (r.x & 0xffffu), x = 0;
-        const uint32_t n = w * h, skip = (uint32_t)gx - w;
-#pragma unroll 1
-        for (uint32_t k = 0; k < n; ++k) {
-            atomicAdd(&a[tile], 1u);
-            ++tile;
-            if (++x == w) { x = 0; tile += skip; }
-        }
+    for (int t = tid; t < T; t += BIN_SCATTER_THREADS) {
+        const uint32_t s = row[t];
+        a[t] = row[T + t] - s;
+        if (starts_in_smem) s_start[t] = s;
     }
+    // the first global slot of (chunk, tile) for step 3: from shared memory when the table fits, else from L2
+    const uint32_t* start = starts_in_smem ? s_start : row;
     __syncthreads();
     const int per = (T + BIN_SCATTER_THREADS - 1) / BIN_SCATTER_THREADS;
     const int t0 = min(T, tid * per), t1 = min(T, t0 + per);
@@ -155,17 +165,26 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
         __syncthreads();
         // ---- 2. unordered append of the window's instances --------------------------------------
         for (int j = j0 + tid; j < j1; j += BIN_SCATTER_THREADS) {
-            const uint32_t g = order[j];
+            const uint32_t seq = (uint32_t)(j - j0);
+            uint32_t g;
+            if (lo == 0) {
+                g = order[j];
+                s_id[seq] = g;
+                s_br[seq] = brects[g];
+            } else {
+                g = s_id[seq];
+            }
             const uint2 r = rects[g];
+            // one flat loop over the w*h tiles (lanes have different rectangles: nested loops would
+            // serialise max(h) * max(w) trips per warp instead of max(w*h))
             const uint32_t w = r.y & 0xffffu, h = r.y >> 16;
             uint32_t tile = (r.x >> 16) * (uint32_t)gx + (r.x & 0xffffu), x = 0;
             const uint32_t n = w * h, skip = (uint32_t)gx - w;
-            const uint32_t seq = (uint32_t)(j - j0);
 #pragma unroll 1
             for (uint32_t k = 0; k < n; ++k) {
                 if ((int)tile >= lo && (int)tile < hi) {
                     const uint32_t slot = atomicAdd(&a[tile], 1u) - first;
-                    stage[slot] = make_uint2(g, (tile << 16) | seq);
+                    stage[slot] = (tile << 16) | seq;
                 }
                 ++tile;
                 if (++x == w) { x = 0; tile += skip; }
@@ -183,16 +202,22 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
         // ---- 3. rank inside the run, coalesced copy-out -------------------------------------------
         // 3a. short runs: one thread per staged entry, all-pairs rank
         for (uint32_t i = tid; i < n_stage; i += BIN_SCATTER_THREADS) {
-            const uint2 e = stage[i];
-            const int t = (int)(e.y >> 16);
-            const uint32_t seq = e.y & 0xffffu;
+            const uint32_t e = stage[i];
+            const int t = (int)(e >> 16);
             const uint32_t rb = (t > lo ? a[t - 1] : first) - first, re = a[t] - first;
             if (re - rb > BIN_LONG_RUN) continue;
-            uint32_t rank = 0;
+            const uint32_t base = start[t];               // issued before the rank loop, which hides its latency
+            uint32_t rank = 0;                            // the run shares the tile: compare whole entries
 #pragma unroll 2
-            for (uint32_t k = rb; k < re; ++k) rank += ((stage[k].y & 0xffffu) < seq) ? 1u : 0u;
-            const long long pos = (long long)row[t] + rank;
-            if (pos < capacity) point_list[pos] = e.x;
+            for (uint32_t k = rb; k < re; ++k) rank += (stage[k] < e) ? 1u : 0u;
+            const long long pos = (long long)base + rank;
+            if (pos < capacity) {
+                const uint32_t seq = e & 0xffffu;
+                point_list[pos] = s_id[seq];
+                const uint32_t ty = tile_row(t, gx_inv);
+                bmask[pos] = (uint8_t)block_mask_of_rect(s_br[seq], 2u * ((uint32_t)t - ty * (uint32_t)gx), 4u * ty);
+                cmask[pos] = 0;
+            }
         }
         // 3b. long runs (depth slices that pile up on few tiles): one warp per run; a bitmap over the
         //     chunk positions turns the rank into a prefix population count
@@ -205,7 +230,7 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
                 for (int k = lane; k < words; k += 32) bm[k] = 0u;
                 __syncwarp();
 #pragma unroll 1
-                for (uint32_t k = rb + lane; k < re; k += 32) { const uint32_t sq = stage[k].y & 0xffffu; atomicOr(&bm[sq >> 5], 1u << (sq & 31u)); }
+                for (uint32_t k = rb + lane; k < re; k += 32) { const uint32_t sq = stage[k] & 0xffffu; atomicOr(&bm[sq >> 5], 1u << (sq & 31u)); }
                 __syncwarp();
                 uint32_t carry = 0;
 #pragma unroll 1
@@ -218,14 +243,19 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
                     carry += __shfl_sync(0xffffffffu, inc, 31);
                 }
                 __syncwarp();
-                const uint32_t base = row[t];
+                const uint32_t base = start[t];
+                const uint32_t ty = tile_row(t, gx_inv);
+                const uint32_t c0 = 2u * ((uint32_t)t - ty * (uint32_t)gx), r0 = 4u * ty;
 #pragma unroll 1
                 for (uint32_t k = rb + lane; k < re; k += 32) {
-                    const uint2 e = stage[k];
-                    const uint32_t sq = e.y & 0xffffu;
+                    const uint32_t sq = stage[k] & 0xffffu;
                     const uint32_t rank = bp[sq >> 5] + (uint32_t)__popc(bm[sq >> 5] & ((1u << (sq & 31u)) - 1u));
                     const long long pos = (long long)base + rank;
-                    if (pos < capacity) point_list[pos] = e.x;
+                    if (pos < capacity) {
+                        point_list[pos] = s_id[sq];
+                        bmask[pos] = (uint8_t)block_mask_of_rect(s_br[sq], c0, r0);
+                        cmask[pos] = 0;
+                    }
                 }
                 __syncwarp();
             }
@@ -238,17 +268,26 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
 // ---- column scan of M ------------------------------------------------------------------------
 // CTA = 32 tiles x 32 groups of BIN_G consecutive chunks (a "slab" of 32*BIN_G chunks);
 // grid = (tiles / 32, slabs).
-//   bin_colsum  : slab_sum[slab][tile] = sum of the slab's rows;
-//   bin_starts  : one CTA; exclusive scan of the tile totals -> ranges, R; per slab and tile the
-//                 absolute first slot (tile start + earlier slabs) -> slab_sum in place;
+//   bin_colsum  : slab_sum[slab][tile] = sum of the slab's rows; the CTA that finishes last then runs
+//   bin_starts  : exclusive scan of the tile totals -> ranges, R; per slab and tile the absolute first
+//                 slot (tile start + earlier slabs) -> slab_sum in place; then the compositors' tile
+//                 order from the ranges it has just written;
 //   bin_apply   : every thread keeps its BIN_G counts in registers, the CTA scans the 32 group sums
-//                 through shared memory and M is rewritten as ABSOLUTE first slots.
+//                 through shared memory and M is rewritten as ABSOLUTE first slots; row M[chunks]
+//                 receives the end of every tile's list (not clamped to the capacity).
 #define BIN_G 16
 #define BIN_SLAB (32 * BIN_G)
 
-__global__ void __launch_bounds__(1024) bin_colsum_kernel(int T, int chunks, const uint32_t* __restrict__ M,
-                                                          uint32_t* __restrict__ slab_sum) {
+__device__ __forceinline__ void bin_starts_cta(int T, int slabs, uint32_t* __restrict__ slab_sum, uint2* ranges,
+                                               GeomHeader* header, long long capacity, uint32_t* __restrict__ tile_order,
+                                               uint32_t* __restrict__ bwd_work, volatile int* count_host);
+
+__global__ void __launch_bounds__(1024) bin_colsum_kernel(int T, int chunks, int slabs, const uint32_t* __restrict__ M,
+                                                          uint32_t* __restrict__ slab_sum, uint2* ranges, GeomHeader* header,
+                                                          long long capacity, uint32_t* __restrict__ tile_order,
+                                                          uint32_t* __restrict__ bwd_work, volatile int* count_host) {
     __shared__ uint32_t s[32][33];
+    __shared__ bool s_last;
     const int tx = threadIdx.x, gy = threadIdx.y;
     const int t = blockIdx.x * 32 + tx;
     const int c0 = blockIdx.y * BIN_SLAB + gy * BIN_G;
@@ -265,19 +304,68 @@ __global__ void __launch_bounds__(1024) bin_colsum_kernel(int T, int chunks, con
         for (int g = 0; g < 32; ++g) acc += s[g][tx];
         if (t < T) slab_sum[(size_t)blockIdx.y * T + t] = acc;
     }
+    // the CTA that finishes last runs bin_starts (threadfence-reduction pattern: publish, then take a ticket)
+    __threadfence();
+    __syncthreads();
+    if (tx == 0 && gy == 0) s_last = atomicAdd(&header->bin_ticket, 1u) == gridDim.x * gridDim.y - 1;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    bin_starts_cta(T, slabs, slab_sum, ranges, header, capacity, tile_order, bwd_work, count_host);
 }
 
-// Empty tiles stay (0,0) like the reference's zero-initialised imgState.ranges.
-__global__ void __launch_bounds__(1024) bin_starts_kernel(int T, int slabs, uint32_t* __restrict__ slab_sum,
-                                                          uint2* __restrict__ ranges, GeomHeader* header,
-                                                          long long capacity) {
+// Longest-processing-time-first order of the tiles for the compositors: the CTAs of the heavy
+// tiles (longest sorted lists) are launched first so that the grid's tail consists of light tiles
+// (with row-major order the last heavy CTAs leave SMs idle at the end of the grid).  Coarse counting sort
+// by list length (64 buckets), by one CTA of 1024 threads once `ranges` is complete and visible to it.
+// Also zeroes bwd_work, which the forward compositor atomicMax-es into.
+__device__ __forceinline__ void tile_order_cta(int T, const uint2* ranges, uint32_t* __restrict__ order,
+                                               uint32_t* __restrict__ bwd_work) {
+    __shared__ uint32_t s_max, s_cnt[64], s_cur[64];
+    const int tid = threadIdx.x + blockDim.x * threadIdx.y;
+    for (int i = tid; i < 2 * T; i += 1024) bwd_work[i] = 0u;
+    if (tid == 0) s_max = 0;
+    if (tid < 64) s_cnt[tid] = 0;
+    __syncthreads();
+    uint32_t m = 0;
+    for (int t = tid; t < T; t += 1024) { const uint2 r = ranges[t]; m = max(m, r.y - r.x); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((tid & 31) == 0) atomicMax(&s_max, m);
+    __syncthreads();
+    const uint32_t mx = s_max;
+    const int shift = mx < 64 ? 0 : (32 - __clz(mx)) - 6;            // bucket = len >> shift in [0, 63]
+    for (int t = tid; t < T; t += 1024) { const uint2 r = ranges[t]; atomicAdd(&s_cnt[min(63u, (r.y - r.x) >> shift)], 1u); }
+    __syncthreads();
+    if (tid < 32) {                                       // descending bucket starts: lane l owns buckets 63-2l, 62-2l
+        const uint32_t c0 = s_cnt[63 - 2 * tid], c1 = s_cnt[62 - 2 * tid];
+        uint32_t inc = c0 + c1;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o); if (tid >= o) inc += v; }
+        s_cur[63 - 2 * tid] = inc - c0 - c1;
+        s_cur[62 - 2 * tid] = inc - c1;
+    }
+    __syncthreads();
+    for (int t = tid; t < T; t += 1024) {
+        const uint2 r = ranges[t];
+        order[atomicAdd(&s_cur[min(63u, (r.y - r.x) >> shift)], 1u)] = (uint32_t)t;
+    }
+}
+
+// Empty tiles stay (0,0) like the reference's zero-initialised imgState.ranges.  With slabs == 0 (P == 0) every
+// list is empty: ranges (0,0), R = 0, and the tile order of all-empty tiles.  count_host: the caller's page-locked
+// host word for R, written straight from here (no copy in the stream between here and the scatter), or null.
+// One CTA of 1024 threads (1-D or 32 x 32); slab_sum is read through L2 (other CTAs wrote it).
+__device__ __forceinline__ void bin_starts_cta(int T, int slabs, uint32_t* __restrict__ slab_sum, uint2* ranges,
+                                               GeomHeader* header, long long capacity, uint32_t* __restrict__ tile_order,
+                                               uint32_t* __restrict__ bwd_work, volatile int* count_host) {
     __shared__ uint32_t s_warp[32];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x + blockDim.x * threadIdx.y, lane = tid & 31, warp = tid >> 5;
     const int per = (T + 1023) / 1024;
     const int t0 = min(T, tid * per), t1 = min(T, t0 + per);
     uint32_t sum = 0;
     for (int t = t0; t < t1; ++t)
-        for (int k = 0; k < slabs; ++k) sum += slab_sum[(size_t)k * T + t];
+        for (int k = 0; k < slabs; ++k) sum += __ldcg(slab_sum + (size_t)k * T + t);
     uint32_t inc = sum;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
@@ -289,18 +377,31 @@ __global__ void __launch_bounds__(1024) bin_starts_kernel(int T, int slabs, uint
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= o) wi += v; }
         s_warp[lane] = wi - wv;
-        if (lane == 31) header->num_rendered = wi;
+        if (lane == 31) {
+            header->num_rendered = wi;
+            if (count_host) *count_host = (int)wi;        // fenced after the ranges, by this thread
+        }
     }
     __syncthreads();
     uint32_t run = s_warp[warp] + inc - sum;
     for (int t = t0; t < t1; ++t) {
         uint32_t n = 0;
-        for (int k = 0; k < slabs; ++k) { const uint32_t v = slab_sum[(size_t)k * T + t]; slab_sum[(size_t)k * T + t] = run + n; n += v; }
+        for (int k = 0; k < slabs; ++k) { const uint32_t v = __ldcg(slab_sum + (size_t)k * T + t); slab_sum[(size_t)k * T + t] = run + n; n += v; }
         // on overflow (R > capacity: the host grows the buffer and re-runs) keep every range inside the buffer
         ranges[t] = n ? make_uint2((uint32_t)min((long long)run, capacity), (uint32_t)min((long long)run + n, capacity))
                       : make_uint2(0u, 0u);
         run += n;
     }
+    // R reaches the host before the kernel counts as complete (by now the store has mostly travelled)
+    if (count_host && tid == 31) __threadfence_system();
+    __syncthreads();                                      // every range written above is visible to the whole CTA
+    tile_order_cta(T, ranges, tile_order, bwd_work);
+}
+
+// P == 0: every list empty (ranges (0,0), R = 0) and the tile order of all-empty tiles, by the same routine.
+__global__ void __launch_bounds__(1024) bin_starts_kernel(int T, uint2* ranges, GeomHeader* header,
+                                                          uint32_t* __restrict__ tile_order, uint32_t* __restrict__ bwd_work) {
+    bin_starts_cta(T, 0, nullptr, ranges, header, 0, tile_order, bwd_work, nullptr);
 }
 
 __global__ void __launch_bounds__(1024) bin_apply_kernel(int T, int chunks, uint32_t* __restrict__ M,
@@ -330,6 +431,7 @@ __global__ void __launch_bounds__(1024) bin_apply_kernel(int T, int chunks, uint
             if (c0 + i < chunks) M[(size_t)(c0 + i) * T + t] = run;
             run += v[i];
         }
+        if (c0 < chunks && chunks <= c0 + BIN_G) M[(size_t)chunks * T + t] = run;   // the group holding the last chunk
     }
 }
 
@@ -358,13 +460,20 @@ int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* 
     const int T = gx * gy;
     const int CH = bin_chunk_len(P, (size_t)T);
     const int chunks = (P + CH - 1) / CH;
-    // shared memory of bin_scatter: the per-tile array + as large a staging area as fits (>= CH entries,
-    // since one tile can receive every Gaussian of the chunk)
+    // shared memory of bin_scatter: the per-tile array, the per-warp bitmaps, the per-position ids and block
+    // rectangles + a staging area of up to 12 entries per Gaussian, as far as it fits (>= CH entries, since one tile
+    // can receive every Gaussian of the chunk); a copy of the chunk's first slots per tile where that still leaves the
+    // full staging area (up to 1080p tile counts), otherwise step 3 reads them from M.  A larger staging area is
+    // slower at the headline: it spares the few heaviest chunks a second window but leaves less of the SM's
+    // L1 / shared-memory split to L1.
     const size_t smem_max = 220 * 1024;                   // + ~5 KB static
-    const size_t tbl_bytes = (((size_t)T + 3) & ~(size_t)3) * 4 +
-                             (size_t)(BIN_SCATTER_THREADS / 32) * 2 * ((CH + 31) / 32) * 4;      // per-tile array + per-warp bitmaps
-    if (gx > 65535 || gy > 65535 || T > 65535 || tbl_bytes + (size_t)CH * 8 > smem_max) return R3DG_ERR_UNSUPPORTED;
-    int cap = (int)std::min<size_t>(std::min<size_t>((smem_max - tbl_bytes) / 8, (size_t)CH * 12), (size_t)BIN_MAX_LONG * BIN_LONG_RUN);
+    const size_t tile_bytes = (((size_t)T + 3) & ~(size_t)3) * 4;
+    size_t tbl_bytes = tile_bytes + (size_t)(BIN_SCATTER_THREADS / 32) * 2 * ((CH + 31) / 32) * 4 + (size_t)CH * 12;
+    if (gx > 65535 || gy > 65535 || T > 65535 || CH > 65536 || tbl_bytes + (size_t)CH * 4 > smem_max) return R3DG_ERR_UNSUPPORTED;
+    const size_t full_stage = std::min<size_t>((size_t)CH * 12, (size_t)BIN_MAX_LONG * BIN_LONG_RUN);
+    const int starts_in_smem = tbl_bytes + tile_bytes + full_stage * 4 <= smem_max ? 1 : 0;
+    if (starts_in_smem) tbl_bytes += tile_bytes;
+    int cap = (int)std::min<size_t>((smem_max - tbl_bytes) / 4, full_stage);
     if (const char* e = getenv("R3DG_BIN_STAGE_CAP")) cap = std::max(CH, std::min(cap, atoi(e)));   // tests: force the multi-window path
     GeomHeader* header = (GeomHeader*)(geom + gl.header);
     const SortLayout sl(P);
@@ -373,7 +482,7 @@ int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* 
     if (rc != 0) return rc;
     mark(2, stream);
     const size_t smem_count = (size_t)T * 4;
-    const size_t smem_scatter = tbl_bytes + (size_t)cap * 8;
+    const size_t smem_scatter = tbl_bytes + (size_t)cap * 4;
     static size_t attr_smem[2] = {0, 0};
     if (smem_count > attr_smem[0]) {
         R3DG_CUDA_TRY(cudaFuncSetAttribute(bin_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_count));
@@ -392,17 +501,39 @@ int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* 
     uint32_t* point_list = (uint32_t*)(bin + bl.point_list);
     const int slabs = (chunks + BIN_SLAB - 1) / BIN_SLAB;
     const dim3 sgrid((T + 31) / 32, slabs), sblock(32, 32);
-    bin_count_kernel<<<chunks, 256, smem_count, stream>>>(P, T, gx, CH, header, va, vb, rects, M);
+    bin_count_kernel<<<chunks, BIN_COUNT_THREADS, smem_count, stream>>>(P, T, gx, CH, header, va, vb, rects, M);
     mark(3, stream);
-    bin_colsum_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, M, slab_sum);
-    bin_starts_kernel<<<1, 1024, 0, stream>>>(T, slabs, slab_sum, ranges, header, bl.capacity);
-    // the instance count exists now: hand it to the host early (the scatter and the compositor are still to run)
-    if (num_rendered_host) R3DG_CUDA_TRY(cudaMemcpyAsync(num_rendered_host, header, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    // the instance count exists after bin_starts: hand it to the host early (the scatter and the compositor are still
+    // to run).  Page-locked host memory is mapped into the device's address space: bin_starts stores the count there
+    // itself, which spares the stream a device-to-host copy between two kernels.  Pageable memory takes the copy.
+    int* count_host = nullptr;
+    if (num_rendered_host) {
+        cudaPointerAttributes pa;
+        if (cudaPointerGetAttributes(&pa, num_rendered_host) == cudaSuccess && pa.type == cudaMemoryTypeHost &&
+            pa.devicePointer && pa.hostPointer)
+            count_host = (int*)((char*)pa.devicePointer + ((char*)num_rendered_host - (char*)pa.hostPointer));
+        else
+            cudaGetLastError();                           // clear the query's error state
+    }
+    bin_colsum_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, slabs, M, slab_sum, ranges, header, bl.capacity,
+                                                    (uint32_t*)(img + il.tile_order), (uint32_t*)(img + il.bwd_work), count_host);
+    if (num_rendered_host && !count_host)
+        R3DG_CUDA_TRY(cudaMemcpyAsync(num_rendered_host, header, sizeof(int), cudaMemcpyDeviceToHost, stream));
     if (count_ready_event) R3DG_CUDA_TRY(cudaEventRecord((cudaEvent_t)count_ready_event, stream));
     bin_apply_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, M, slab_sum);
     mark(4, stream);
-    bin_scatter_kernel<<<chunks, BIN_SCATTER_THREADS, smem_scatter, stream>>>(P, T, gx, CH, cap, header, va, vb, rects, M,
-                                                                               point_list, bl.capacity);
+    bin_scatter_kernel<<<chunks, BIN_SCATTER_THREADS, smem_scatter, stream>>>(
+        P, T, gx, (1ull << 32) / (unsigned long long)gx + 1ull, CH, cap, header, va, vb, rects, (const uint2*)(geom + gl.brects), M, point_list,
+        (uint8_t*)(bin + bl.bmask), (uint8_t*)(bin + bl.cmask), bl.capacity, starts_in_smem);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int launch_empty_binning(int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
+                         cudaStream_t stream) {
+    const int T = ((W + R3DG_TILE - 1) / R3DG_TILE) * ((H + R3DG_TILE - 1) / R3DG_TILE);
+    bin_starts_kernel<<<1, 1024, 0, stream>>>(T, (uint2*)(img + il.ranges), (GeomHeader*)(geom + gl.header),
+                                              (uint32_t*)(img + il.tile_order), (uint32_t*)(img + il.bwd_work));
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -35,7 +35,8 @@ struct GeomHeader {               // first 256 bytes of the geometry buffer
     uint32_t depth_or;            // OR of the sort keys (visible depth bit patterns)
     uint32_t depth_nor;           // OR of their complements: bit varies across keys iff set in both
     uint32_t sort_exec;           // number of radix passes actually executed (parity = result buffer)
-    uint32_t pad[51];
+    uint32_t bin_ticket;          // CTAs of bin_colsum done (the last one scans the tile totals)
+    uint32_t pad[50];
 };
 static_assert(sizeof(GeomHeader) == 256, "header size");
 
@@ -111,7 +112,7 @@ struct GeomLayout {
 // ---- depth-ordered tile binning (binning.cu) -------------------------------------------------
 // The depth-sorted Gaussians are cut into `chunks` runs of CH; M[chunk][tile] first counts the
 // instances a chunk adds to a tile, then (scanned down the columns) is the chunk's first slot
-// inside the tile's list.
+// inside the tile's list, and row M[chunks] holds the (unclamped) end of every list.
 #define R3DG_BIN_MAX_CHUNKS 1024
 __host__ __device__ inline int bin_max_chunks(size_t T) {
 #ifndef __CUDA_ARCH__
@@ -143,15 +144,15 @@ struct ImgLayout {
         bwd_work = off;  off = align_up(off + 2 * T * 4, 256);    // per half-tile CTA: entries its busiest warp composited (forward)
         bwd_order = off; off = align_up(off + 2 * T * 4, 256);    // half-tile CTAs by descending bwd_work (backward launch order)
         slab_sum = off;  off = align_up(off + T * 4 * ((R3DG_BIN_MAX_CHUNKS + 511) / 512), 256);   // per 512-chunk slab
-        bin_matrix = off; off = align_up(off + (size_t)bin_max_chunks(T) * T * 4, 256);
+        bin_matrix = off; off = align_up(off + ((size_t)bin_max_chunks(T) + 1) * T * 4, 256);   // + the row of list ends
         total = off;
     }
 };
 
 // Binning buffer (capacity-sized, speculative): the per-tile depth-sorted Gaussian lists (reference
 // binningState.point_list) plus one byte per instance for each of
-//   bmask: bit b = 8x4 pixel block b of the instance's tile may be touched by the Gaussian (block_mask_kernel,
-//          the exact-conservative ellipse/rectangle test evaluated ONCE per instance instead of by 8 warps);
+//   bmask: bit b = 8x4 pixel block b of the instance's tile may be touched by the Gaussian (written by bin_scatter
+//          with block_mask_of_rect: the conservative block-rectangle test evaluated ONCE per instance instead of by 8 warps);
 //   cmask: bit b = block b actually composited the instance in the forward pass (some pixel accepted it).  The
 //          backward compositor visits exactly the cmask entries of its block, nothing else.
 // 6 B per instance instead of the reference's 24 B + sort temp.
@@ -341,8 +342,8 @@ __device__ __forceinline__ bool touch_block(const float4 A, const float4 B, floa
 // absorbs the fp32 evaluation error of the per-pixel quadratic for conics with trace^2/det <= 6000 (error <=
 // 2.4e-7 * 1.5 * trace^2/det * q); worse-conditioned, non-positive-definite or NaN conics get the full range.
 // Packed {bx0 | bx1 << 16, by0 | by1 << 16}, inclusive block column / row indices; empty (bx0 > bx1) when the
-// opacity is below 1/255.  This is only a PRE-filter (block_mask_kernel): the compositor still applies the exact
-// ellipse / rectangle test to what passes, and the exact per-pixel tests to what passes that.
+// opacity is below 1/255.  This is only a PRE-filter (block_mask_of_rect, written by bin_scatter): the compositor
+// still applies the exact ellipse / rectangle test to what passes, and the exact per-pixel tests to what passes that.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint2 block_rect(float gx, float gy, float ca, float cb, float cc, float op) {
     if (op < 1.0f / 255.0f) return make_uint2(1u, 0u);                       // bx0 = 1 > bx1 = 0: touches nothing
@@ -355,6 +356,22 @@ __device__ __forceinline__ uint2 block_rect(float gx, float gy, float ca, float 
     // a box entirely left of / above the image maps to an empty range (pixels have coordinates >= 0)
     if (gx + hx < 0.0f || gy + hy < 0.0f) return make_uint2(1u, 0u);
     return make_uint2(blk(gx - hx, 0.125f) | (blk(gx + hx, 0.125f) << 16), blk(gy - hy, 0.25f) | (blk(gy + hy, 0.25f) << 16));
+}
+
+// The 8-bit block pre-filter mask of one (tile, Gaussian) instance: bit b = block b of the tile intersects the
+// Gaussian's block rectangle.  c0 / r0 = first block column / row of the tile.
+__device__ __forceinline__ uint32_t block_mask_of_rect(uint2 br, uint32_t c0, uint32_t r0) {
+    const uint32_t bx0 = br.x & 0xffffu, bx1 = br.x >> 16, by0 = br.y & 0xffffu, by1 = br.y >> 16;
+    // block rows r0 + [rlo, rhi] and columns c0 + [clo, chi] lie inside the rectangle: contiguous bit runs
+    const int rlo = max((int)by0 - (int)r0, 0), rhi = min((int)by1 - (int)r0, 3);
+    const int clo = max((int)bx0 - (int)c0, 0), chi = min((int)bx1 - (int)c0, 1);
+    const uint32_t rows = rlo <= rhi ? (2u << rhi) - (1u << rlo) : 0u;
+    const uint32_t cols = clo <= chi ? (2u << chi) - (1u << clo) : 0u;
+    // block b = (row b >> 1, column b & 1): spread the row bits to even positions; times cols (0..3) places them in
+    // column 0, column 1 or both (the spread bits are two apart, so the product has no carries)
+    uint32_t spread = (rows | (rows << 2)) & 0x33u;
+    spread = (spread | (spread << 1)) & 0x55u;
+    return spread * cols;
 }
 
 // The same test for all 8 blocks of a tile at once (block b: x offset 8 * (b & 1), y offset 4 * (b >> 1)), with

@@ -5,7 +5,7 @@
 //  * each warp owns a compact 8x4 pixel block of a 16x16 tile and walks the tile's sorted list
 //    AUTONOMOUSLY: no CTA barrier, per-warp early termination (the reference's CTA-wide
 //    fetch/compute lock-step spent ~half of its stall samples at the barrier);
-//  * stream compaction instead of per-warp culling: block_mask_kernel leaves one pre-filter byte
+//  * stream compaction instead of per-warp culling: the binning scatter leaves one pre-filter byte
 //    per (tile, Gaussian) instance; a warp streams the bytes 128 instances per step, compacts the
 //    positions whose bit for ITS block is set into a circular queue and composites batches of 32
 //    queued entries (id -> packed record prefetched one batch ahead, staged in a warp-private
@@ -41,8 +41,8 @@ struct CompositeFwdParams {
     int W, H, gx, S, recf;
     const uint2* ranges;
     const uint32_t* point_list;  // per-tile depth-sorted Gaussian ids (binning.cu)
-    const uint32_t* bmask32;     // per-instance block-touch masks (block_mask_kernel), viewed as words of 4 instances
-    uint32_t* cmask32;           // per-instance contributor masks (zeroed by block_mask_kernel, set here)
+    const uint32_t* bmask32;     // per-instance block-touch masks (bin_scatter), viewed as words of 4 instances
+    uint32_t* cmask32;           // per-instance contributor masks (zeroed by bin_scatter, set here)
     const GeomHeader* header;
     const uint32_t* tile_order;  // CTA -> tile, heaviest tiles first
     uint32_t* bwd_work;          // [2 tiles] entries composited by the busiest warp of each half-tile CTA (backward launch order)
@@ -57,54 +57,6 @@ struct CompositeFwdParams {
 __device__ WarpTiming g_wt_fwd[R3DG_WT_MAX];
 extern "C" int r3dg_debug_wt_fwd(void* dst, size_t bytes) { return (int)cudaMemcpyFromSymbol(dst, g_wt_fwd, bytes); }
 #endif
-
-// The 8-bit block pre-filter mask of one (tile, Gaussian) instance: bit b = block b of the tile intersects the
-// Gaussian's conservative block rectangle (projection.cu / block_rect()).
-__device__ __forceinline__ uint32_t block_mask_of_rect(uint2 br, uint32_t c0, uint32_t r0) {
-    const uint32_t bx0 = br.x & 0xffffu, bx1 = br.x >> 16, by0 = br.y & 0xffffu, by1 = br.y >> 16;
-    uint32_t cols = 0u, rows = 0u;
-    if (bx0 <= c0 && c0 <= bx1) cols |= 1u;
-    if (bx0 <= c0 + 1u && c0 + 1u <= bx1) cols |= 2u;
-#pragma unroll
-    for (uint32_t k = 0; k < 4; ++k)
-        if (by0 <= r0 + k && r0 + k <= by1) rows |= 1u << k;
-    // block b = (row b >> 1, column b & 1): spread the row bits to even positions, combine with the column bits
-    const uint32_t spread = (rows & 1u) | ((rows & 2u) << 1) | ((rows & 4u) << 2) | ((rows & 8u) << 3);
-    return ((cols & 1u) ? spread : 0u) | ((cols & 2u) ? (spread << 1) : 0u);
-}
-
-// Pre-filter mask byte + zeroed contributor byte for every instance.  CTA per tile (heaviest first).  A thread takes
-// FOUR consecutive instances of the tile's list: one 16-byte load of the ids, four independent 8-byte gathers of the
-// block rectangles (the latency this kernel is bound by), one 4-byte store per mask array.  The ragged ends of the
-// tile's range (it starts and ends anywhere inside a word shared with the neighbouring tiles) are written bytewise.
-__global__ void __launch_bounds__(256) block_mask_kernel(int gx, const uint2* __restrict__ ranges,
-                                                         const uint32_t* __restrict__ tile_order,
-                                                         const uint32_t* __restrict__ point_list,
-                                                         const uint2* __restrict__ brects, uint8_t* __restrict__ bmask,
-                                                         uint8_t* __restrict__ cmask) {
-    const int tile = (int)tile_order[blockIdx.x];
-    const uint2 range = ranges[tile];
-    const uint32_t c0 = 2u * (uint32_t)(tile % gx), r0 = 4u * (uint32_t)(tile / gx);   // first block column / row of the tile
-    const uint32_t a0 = min((range.x + 3u) & ~3u, range.y), a1 = max(range.y & ~3u, a0);  // [a0, a1): whole words
-    if (threadIdx.x < 8) {                                                                // <= 3 head + <= 3 tail bytes
-        const uint32_t i = threadIdx.x < 4 ? range.x + threadIdx.x : a1 + (threadIdx.x - 4);
-        const bool mine = threadIdx.x < 4 ? i < a0 : i < range.y;
-        if (mine) {
-            bmask[i] = (uint8_t)block_mask_of_rect(brects[point_list[i]], c0, r0);
-            cmask[i] = 0;
-        }
-    }
-    const uint4* __restrict__ ids4 = reinterpret_cast<const uint4*>(point_list);
-    uint32_t* __restrict__ bmask32 = reinterpret_cast<uint32_t*>(bmask);
-    uint32_t* __restrict__ cmask32 = reinterpret_cast<uint32_t*>(cmask);
-    for (uint32_t w = (a0 >> 2) + threadIdx.x; w < (a1 >> 2); w += 256) {
-        const uint4 id = ids4[w];
-        const uint2 b0 = brects[id.x], b1 = brects[id.y], b2 = brects[id.z], b3 = brects[id.w];
-        bmask32[w] = block_mask_of_rect(b0, c0, r0) | (block_mask_of_rect(b1, c0, r0) << 8) |
-                     (block_mask_of_rect(b2, c0, r0) << 16) | (block_mask_of_rect(b3, c0, r0) << 24);
-        cmask32[w] = 0u;
-    }
-}
 
 // NW = warps per CTA (4: two CTAs per tile).  Warps are autonomous: no
 // CTA-wide barrier anywhere; the CTA only exists so that the warps of a tile share L1 lines.
@@ -433,16 +385,6 @@ static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, cudaStream_t s
     composite_env();
     if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel(composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true>, p, tiles, stream);
     else launch_fwd_kernel(composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false>, p, tiles, stream);
-}
-
-int launch_block_masks(int W, int H, const GeomLayout& gl, const ImgLayout& il, char* geom, char* img, char* bin,
-                       const BinLayout& bl, cudaStream_t stream) {
-    const int gx = (W + R3DG_TILE - 1) / R3DG_TILE, gy = (H + R3DG_TILE - 1) / R3DG_TILE;
-    block_mask_kernel<<<gx * gy, 256, 0, stream>>>(gx, (const uint2*)(img + il.ranges), (const uint32_t*)(img + il.tile_order),
-                                                   (const uint32_t*)(bin + bl.point_list), (const uint2*)(geom + gl.brects),
-                                                   (uint8_t*)(bin + bl.bmask), (uint8_t*)(bin + bl.cmask));
-    R3DG_CUDA_TRY(cudaGetLastError());
-    return 0;
 }
 
 int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl, const ImgLayout& il,

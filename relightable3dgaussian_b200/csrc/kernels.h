@@ -10,21 +10,21 @@ typedef void (*stage_mark_fn)(int, cudaStream_t);
 int launch_projection(const r3dg_raster_fwd_args& a, const GeomLayout& gl, cudaStream_t stream);
 int launch_point_offsets(int P, const uint32_t* tiles_touched, uint32_t* out, uint32_t* state,
                          GeomHeader* ticket_header, cudaStream_t stream);
-int launch_tile_order(const void* ranges, uint32_t* tile_order, uint32_t* bwd_work, int num_tiles, cudaStream_t stream);
 int launch_cta_order(const uint32_t* work, uint32_t* order, int n, cudaStream_t stream);
 int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,
                         cudaStream_t stream);
 // radix_sort.cu: stable sort of n (u32 key, u32 value) pairs laid out by SortLayout in `buf`
 int launch_sort(void* geom_header, char* buf, const SortLayout& sl, long long n, int num_sms,
                 cudaStream_t stream);
-// binning.cu: depth sort + order-preserving tile binning -> point_list, ranges, num_rendered
+// binning.cu: depth sort + order-preserving tile binning -> point_list, bmask, zeroed cmask, ranges, num_rendered,
+// tile_order, zeroed bwd_work.  launch_empty_binning: the same per-tile outputs for P == 0 (all lists empty).
 int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
                    char* bin, const BinLayout& bl, int num_sms, cudaStream_t stream, stage_mark_fn mark,
                    int* num_rendered_host, void* count_ready_event);
+int launch_empty_binning(int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
+                         cudaStream_t stream);
 int launch_rebuild_keys(int T, const void* ranges, const uint32_t* point_list, const float* rec, int recf,
                         long long limit, uint64_t* keys, cudaStream_t stream);
-int launch_block_masks(int W, int H, const GeomLayout& gl, const ImgLayout& il, char* geom, char* img, char* bin,
-                       const BinLayout& bl, cudaStream_t stream);
 int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl,
                              const ImgLayout& il, char* bin, const BinLayout& bl,
                              cudaStream_t stream, stage_mark_fn mark);

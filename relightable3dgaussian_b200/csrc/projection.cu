@@ -424,37 +424,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(int P, const uint32_
     }
 }
 
-// Longest-processing-time-first order of the tiles for the compositors: the CTAs of the heavy
-// tiles (longest sorted lists) are launched first so that the grid's tail consists of light tiles
-// (with row-major order the last heavy CTAs leave SMs idle at the end of the grid).  Coarse counting sort
-// by list length (64 buckets), one CTA.
-__global__ void __launch_bounds__(1024) tile_order_kernel(int T, const uint2* __restrict__ ranges, uint32_t* __restrict__ order,
-                                                          uint32_t* __restrict__ bwd_work) {
-    __shared__ uint32_t s_max, s_cnt[64], s_cur[64];
-    const int tid = threadIdx.x;
-    for (int i = tid; i < 2 * T; i += 1024) bwd_work[i] = 0u;          // the forward compositor atomicMax-es into it
-    if (tid == 0) s_max = 0;
-    if (tid < 64) s_cnt[tid] = 0;
-    __syncthreads();
-    uint32_t m = 0;
-    for (int t = tid; t < T; t += 1024) { const uint2 r = ranges[t]; m = max(m, r.y - r.x); }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((tid & 31) == 0) atomicMax(&s_max, m);
-    __syncthreads();
-    const uint32_t mx = s_max;
-    const int shift = mx < 64 ? 0 : (32 - __clz(mx)) - 6;            // bucket = len >> shift in [0, 63]
-    for (int t = tid; t < T; t += 1024) { const uint2 r = ranges[t]; atomicAdd(&s_cnt[min(63u, (r.y - r.x) >> shift)], 1u); }
-    __syncthreads();
-    if (tid == 0) { uint32_t acc = 0; for (int b = 63; b >= 0; --b) { s_cur[b] = acc; acc += s_cnt[b]; } }   // descending
-    __syncthreads();
-    for (int t = tid; t < T; t += 1024) {
-        const uint2 r = ranges[t];
-        order[atomicAdd(&s_cur[min(63u, (r.y - r.x) >> shift)], 1u)] = (uint32_t)t;
-    }
-}
-
-// The same coarse LPT order for the backward compositor's CTAs, by what the forward pass measured: keys[c] = entries the
+// The same coarse LPT order as the tile order (binning.cu, bin_starts) for the backward compositor's CTAs, by what the forward pass measured: keys[c] = entries the
 // busiest warp of half-tile CTA c composited = exactly the iterations its backward twin will run.  List length is a poor
 // predictor there (a dense tile saturates after a fraction of its list): ordered by it, heavy backward CTAs started
 // late and finished last (tools/warp_timing.py shows the per-warp start and end times).
@@ -526,12 +496,6 @@ int launch_point_offsets(int P, const uint32_t* tiles_touched, uint32_t* out, ui
     R3DG_CUDA_TRY(cudaMemsetAsync(state, 0, (size_t)(nscan + 1) * 4, stream));
     R3DG_CUDA_TRY(cudaMemsetAsync(ticket_header, 0, sizeof(GeomHeader), stream));
     scan_kernel<<<nscan, SCAN_THREADS, 0, stream>>>(P, tiles_touched, out, (volatile uint32_t*)state, ticket_header);
-    R3DG_CUDA_TRY(cudaGetLastError());
-    return 0;
-}
-
-int launch_tile_order(const void* ranges, uint32_t* tile_order, uint32_t* bwd_work, int num_tiles, cudaStream_t stream) {
-    tile_order_kernel<<<1, 1024, 0, stream>>>(num_tiles, (const uint2*)ranges, tile_order, bwd_work);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }
