@@ -153,8 +153,10 @@ __device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOp
     // ---- environment + local SH light --------------------------------------------------------
     float ex = dx, ey = dy, ez = dz;
     if (a.transform) {                                     // dirs @ transform.T  (scene/envmap.py:39-42)
+        // the sums start from +0 like a BLAS product: a row of -0 terms gives +0 (not -0), which decides the env
+        // column at the seam (atan2(+0, x < 0) = +pi -> column 0, atan2(-0, x < 0) = -pi -> column We-1)
         const float* T = a.transform;
-        ex = dx * T[0] + dy * T[1] + dz * T[2]; ey = dx * T[3] + dy * T[4] + dz * T[5]; ez = dx * T[6] + dy * T[7] + dz * T[8];
+        ex = 0.f + dx * T[0] + dy * T[1] + dz * T[2]; ey = 0.f + dx * T[3] + dy * T[4] + dz * T[5]; ez = 0.f + dx * T[6] + dy * T[7] + dz * T[8];
     }
     e.taps = env_taps(ex, ey, ez, a.He, a.We);
 #pragma unroll

@@ -308,6 +308,15 @@ def bvh_case(recipe, P, n_src, N, boost, seed=3):
                 normals=normals, inv_cov=inverse_covariance(scales, sc.rotations), rays_o=rays_o, rays_d=dirs.contiguous())
 
 
+# every shading kernel variant r3dg_tune can select: lanes per Gaussian, env-gradient accumulation mode, SH operands /
+# gradient accumulators in shared memory (csrc/shading.cu g_knobs)
+SHADE_KNOBS = [dict(shade_group=16), dict(shade_group=32), dict(shade_env_mode=1), dict(shade_env_mode=0),
+               dict(shade_group=32, shade_env_mode=1), dict(shade_fwd_variant=1, shade_bwd_variant=1),
+               dict(shade_fwd_variant=1, shade_bwd_variant=2), dict(shade_bwd_variant=2, shade_env_mode=1),
+               dict(shade_fwd_variant=0, shade_bwd_variant=0, shade_env_mode=2), dict(shade_bwd_variant=1, shade_env_mode=2),
+               dict(shade_bwd_variant=2, shade_env_mode=2)]
+
+
 def shading_case(P, N, He, seed):
     """Seeded inputs of `rendering_equation` (neilf.py:339): activated material parameters, SH
     incident light, raw env map (softplus applied by the light object), baked visibility / dirs."""

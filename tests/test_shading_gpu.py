@@ -9,7 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import GOLDEN, npy, rel_l2, shading_case
+from helpers import GOLDEN, SHADE_KNOBS, npy, rel_l2, shading_case
 
 pytestmark = pytest.mark.gpu
 CASES = sorted(glob.glob(os.path.join(GOLDEN, "shading_*.npz")))
@@ -66,12 +66,7 @@ def test_matches_pytorch_oracle(P, N, He, fixed):
     _check_against_oracle(P, N, He, fixed)
 
 
-@pytest.mark.parametrize("knobs", [dict(shade_group=16), dict(shade_group=32), dict(shade_env_mode=1), dict(shade_env_mode=0),
-                                   dict(shade_group=32, shade_env_mode=1), dict(shade_fwd_variant=1, shade_bwd_variant=1),
-                                   dict(shade_fwd_variant=1, shade_bwd_variant=2), dict(shade_bwd_variant=2, shade_env_mode=1),
-                                   dict(shade_fwd_variant=0, shade_bwd_variant=0, shade_env_mode=2), dict(shade_bwd_variant=1, shade_env_mode=2),
-                                   dict(shade_bwd_variant=2, shade_env_mode=2)],
-                         ids=lambda k: ",".join(f"{a[6:]}={b}" for a, b in k.items()))
+@pytest.mark.parametrize("knobs", SHADE_KNOBS, ids=lambda k: ",".join(f"{a[6:]}={b}" for a, b in k.items()))
 def test_kernel_variants_match_oracle(knobs):
     """Every kernel variant selectable through r3dg_tune: lanes per Gaussian, env-gradient
     accumulation mode, SH operands / gradient accumulators in shared memory."""
