@@ -81,6 +81,11 @@ typedef struct r3dg_raster_fwd_args {
      * a host that waits on this event instead of the stream gets the count while the compositor is still running and
      * can already enqueue what follows the forward.  NULL: not used. */
     void* count_ready_event;
+    /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
+     * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
+     * det_work: device workspace of at least r3dg_raster_fwd_det_bytes(P) bytes, zeroed by the call.  0 = the default path (det_work unused). */
+    int deterministic;
+    void* det_work; size_t det_work_bytes;
 } r3dg_raster_fwd_args;
 
 /* Replaces CudaRasterizer::Rasterizer::forward (rasterizer.h:34-65, rasterizer_impl.cu:199-380)
@@ -123,6 +128,11 @@ typedef struct r3dg_raster_bwd_args {
     void* geom;   size_t geom_bytes;
     void* img;    size_t img_bytes;
     void* binning; size_t binning_bytes;
+    /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
+     * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
+     * det_work: device workspace of at least r3dg_raster_bwd_det_bytes(P, S) bytes, zeroed by the call.  0 = the default path (det_work unused). */
+    int deterministic;
+    void* det_work; size_t det_work_bytes;
 } r3dg_raster_bwd_args;
 
 /* Replaces CudaRasterizer::Rasterizer::backward (rasterizer.h:67-100, rasterizer_impl.cu:384-491)
@@ -396,10 +406,39 @@ typedef struct r3dg_shade_args {
     float* dL_dviewdirs;               /* [P,3] */
     float* dL_dincidents;              /* [P,16,3] */
     float* dL_denv;                    /* [env_h,env_w,3] (zeroed, then accumulated) */
+    /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero (backward only) = sums that float atomics would make
+     * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
+     * det_work: device workspace of at least r3dg_shade_det_bytes(env_h, env_w) bytes, zeroed by the call.  0 = the default path (det_work unused). */
+    int deterministic;
+    void* det_work; size_t det_work_bytes;
 } r3dg_shade_args;
 
 int r3dg_render_equation_forward(const r3dg_shade_args* args, r3dg_stream_t stream);
 int r3dg_render_equation_backward(const r3dg_shade_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * DETERMINISTIC MODE.  With `deterministic` set in r3dg_raster_fwd_args, r3dg_raster_bwd_args or
+ * r3dg_shade_args, the three sums that float atomics make depend on the order in which warps finish
+ * are accumulated in fixed point instead (csrc/detacc.cuh): out_weights of the forward, the
+ * per-Gaussian gradient rows of the backward (hence all nine rasterizer gradients) and dL_denv of the
+ * shading backward.  Results are then bitwise reproducible for the same inputs on the same device,
+ * whatever the scheduling (r3dg_tune knobs included).  Everything else these calls compute is already
+ * order-independent and unchanged.  Each term is rounded to a multiple of 2^-48 (|term| < 2^47;
+ * larger finite terms saturate to +-Inf, NaN / +-Inf propagate as in IEEE addition); each total is
+ * rounded to fp32 once.  out_weights is exact (integer units of 2^-24 per pixel).
+ * The workspace is the caller's, separate from `geom` (default memory use is unchanged); missing or
+ * too small a workspace returns R3DG_ERR_BAD_ARG before anything is launched.
+ *   r3dg_raster_fwd_det_bytes : 8 B per Gaussian;
+ *   r3dg_raster_bwd_det_bytes : ~24 B per gradient-row float (8 + 4 ceil((3 + S) / 4) floats per
+ *                               Gaussian): 384 MB at P = 1M, S = 5;
+ *   r3dg_shade_det_bytes      : ~24 B per env-texel channel.
+ * r3dg_det_sum_host: the accumulation primitive's host build (tests): *out = the sum of the n
+ * host floats `terms` as the deterministic mode computes it.
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_raster_fwd_det_bytes(int P);
+size_t r3dg_raster_bwd_det_bytes(int P, int S);
+size_t r3dg_shade_det_bytes(int env_h, int env_w);
+int r3dg_det_sum_host(long long n, const float* terms, float* out);
 
 /* Replaces `simple_knn._C.distCUDA2` (submodules/simple-knn/spatial.cu:15-26, simple_knn.cu:185-221):
  * mean_dist2[i] = mean of the 3 smallest squared distances from point i to the other points.

@@ -13,6 +13,10 @@ Differences that are not observable through the reference's Python wrapper
     read back once, after everything has been enqueued — the pipeline itself never synchronises;
     a missed speculation re-runs the forward (synchronous path: immediately; deferred path: in the
     autograd backward, before differentiating).
+
+Under torch.use_deterministic_algorithms(True), read at call time, both calls run the library's
+deterministic mode: out_weights and the nine gradients are then bitwise reproducible (the reference's
+float atomics make them run-to-run nondeterministic).  Its workspace comes from the torch allocator.
 """
 import ctypes
 
@@ -82,6 +86,18 @@ def _ptr(t):
     return t.data_ptr()
 
 
+def _det_workspace(nbytes, dev):
+    """Workspace of the deterministic mode when torch.are_deterministic_algorithms_enabled(), else None."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return None
+    return torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+
+
+def _set_det(a, ws):
+    if ws is not None:
+        a.deterministic, a.det_work, a.det_work_bytes = 1, ws.data_ptr(), ws.numel()
+
+
 def _prep(t, name):
     if t is None or t.numel() == 0:
         return t
@@ -147,6 +163,7 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     else:
         capacity = max(st["capacity"], 4 * P + 4096)
     stream = torch.cuda.current_stream(dev)
+    det_ws = _det_workspace(lib.r3dg_raster_fwd_det_bytes(P), dev)
     slot = st["next"]
     st["next"] = (slot + 1) % _SLOTS
     pinned = st["pinned"][slot:slot + 1]
@@ -176,6 +193,7 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
             ev = torch.cuda.Event()
             ev.record(stream)             # (creates the underlying cudaEvent_t; re-recorded inside the call)
             a.count_ready_event = ev.cuda_event
+            _set_det(a, det_ws)
             _lib.check(lib.r3dg_raster_forward(ctypes.byref(a), stream.cuda_stream), "rasterize_gaussians")
             if _defer:                    # opt-in: let the host run ahead; the count is resolved later
                 rendered = DeferredCount(ev, pinned, capacity, st, P)
@@ -271,6 +289,8 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
         a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
+        det_ws = _det_workspace(lib.r3dg_raster_bwd_det_bytes(P, S), dev)
+        _set_det(a, det_ws)
         stream = torch.cuda.current_stream(dev)
         with torch.cuda.device(dev):
             _lib.check(lib.r3dg_raster_backward(ctypes.byref(a), stream.cuda_stream),

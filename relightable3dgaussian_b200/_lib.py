@@ -27,7 +27,8 @@ class RasterFwdArgs(ctypes.Structure):
                                  "out_normal", "out_surface_xyz", "out_weights", "radii",
                                  "n_contrib")] +
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
-         ("binning", c_void_p), ("binning_bytes", c_size_t), ("num_rendered_host", c_void_p), ("count_ready_event", c_void_p)])
+         ("binning", c_void_p), ("binning_bytes", c_size_t), ("num_rendered_host", c_void_p), ("count_ready_event", c_void_p),
+         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class RasterBwdArgs(ctypes.Structure):
@@ -43,7 +44,8 @@ class RasterBwdArgs(ctypes.Structure):
                                  "dL_dmeans3D", "dL_dfeatures", "dL_dcov3D", "dL_dsh",
                                  "dL_dscales", "dL_drotations", "dL_dsh_factor")] +
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
-         ("binning", c_void_p), ("binning_bytes", c_size_t)])
+         ("binning", c_void_p), ("binning_bytes", c_size_t),
+         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class ShadeArgs(ctypes.Structure):
@@ -55,7 +57,8 @@ class ShadeArgs(ctypes.Structure):
                                  "mean_local_lights", "mean_global_lights", "mean_visibility",
                                  "incident_lights", "local_incident_lights", "global_incident_lights",
                                  "dL_dpbr", "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color",
-                                 "dL_droughness", "dL_dviewdirs", "dL_dincidents", "dL_denv")])
+                                 "dL_droughness", "dL_dviewdirs", "dL_dincidents", "dL_denv")] +
+        [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class ExchangeArgs(ctypes.Structure):
@@ -126,6 +129,10 @@ SYMBOLS = [
                                       ctypes.POINTER(DensifyThresholds), c_void_p, c_size_t, c_void_p, c_void_p]),
     ("r3dg_densify_apply", c_int, [c_int, ctypes.POINTER(c_int), c_int, ctypes.POINTER(DensifyTensor), c_void_p, c_void_p,
                                    c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_raster_fwd_det_bytes", c_size_t, [c_int]),
+    ("r3dg_raster_bwd_det_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_shade_det_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_det_sum_host", c_int, [c_ll, c_void_p, c_void_p]),
     ("r3dg_knn_tmp_bytes", c_size_t, [c_int]),
     ("r3dg_knn_dist2", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("r3dg_ssim_tmp_bytes", c_size_t, [c_int, c_int, c_int, c_int]),

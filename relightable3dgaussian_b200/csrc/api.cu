@@ -5,6 +5,7 @@
 #include <cstring>
 #include <vector>
 #include "common.cuh"
+#include "detacc.cuh"
 #include "kernels.h"
 
 using namespace r3dg;
@@ -46,6 +47,20 @@ size_t r3dg_raster_geom_bytes(int P, int S) { return GeomLayout(P < 1 ? 1 : P, S
 size_t r3dg_raster_img_bytes(int W, int H) { return ImgLayout(W, H).total; }
 size_t r3dg_raster_binning_bytes(long long capacity) { return bin_bytes_for_capacity(capacity < 1 ? 1 : capacity); }
 size_t r3dg_raster_img_n_contrib_offset(int W, int H) { return ImgLayout(W, H).n_contrib; }
+size_t r3dg_raster_fwd_det_bytes(int P) { return align_up((size_t)(P < 1 ? 1 : P) * 8, 256); }
+size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S)); }
+
+int r3dg_det_sum_host(long long n, const float* terms, float* out) {
+    if (n < 0 || (n > 0 && !terms) || !out) return R3DG_ERR_BAD_ARG;
+    uint64_t lo = 0, mid = 0, hi = 0;
+    uint32_t flag = 0;
+    for (long long i = 0; i < n; ++i) {
+        const DetTerm t = det_term(terms[i]);
+        lo += t.lo; mid += t.mid; hi += t.hi; flag |= t.flag;
+    }
+    *out = det_value(lo, mid, hi, flag);
+    return 0;
+}
 
 int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -57,6 +72,7 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     const GeomLayout gl(a->P < 1 ? 1 : a->P, a->S);
     const ImgLayout il(a->W, a->H);
     if (a->geom_bytes < gl.total || a->img_bytes < il.total) return R3DG_ERR_BAD_ARG;
+    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(a->P))) return R3DG_ERR_BAD_ARG;
     const long long capacity = bin_capacity_for_bytes(a->binning_bytes);
     if (capacity < 1) return R3DG_ERR_BAD_ARG;
     const BinLayout bl(capacity);
@@ -81,7 +97,7 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     prof_mark(true, 5, stream);
     if ((rc = launch_composite_forward(*a, gl, il, bin, bl, stream, mark)) != 0) return rc;
     prof_mark(true, 7, stream);
-    g_launches += 1 + (a->computer_pseudo_normal ? 1 : 0);   // composite, normals
+    g_launches += 1 + (a->computer_pseudo_normal ? 1 : 0) + (a->deterministic && a->P > 0 ? 1 : 0);   // composite, normals, weights
     if (g_prof.on) g_prof.fwd_calls++;
     if (a->P == 0) {      // (P > 0: the count was written, and the event recorded, as soon as the binning offsets existed)
         if (a->num_rendered_host) R3DG_CUDA_TRY(cudaMemcpyAsync(a->num_rendered_host, geom + gl.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
@@ -98,6 +114,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!a || a->P < 0 || a->W <= 0 || a->H <= 0 || a->S < 0) return R3DG_ERR_BAD_ARG;
     if (a->S > R3DG_MAX_S_BWD) return R3DG_ERR_UNSUPPORTED;
+    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(a->P, a->S))) return R3DG_ERR_BAD_ARG;
     if (a->P == 0) return 0;
     const GeomLayout gl(a->P, a->S);
     const ImgLayout il(a->W, a->H);

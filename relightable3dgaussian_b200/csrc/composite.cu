@@ -24,6 +24,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "common.cuh"
+#include "detacc.cuh"
 #include "kernels.h"
 
 #ifndef R3DG_FWD_CTAS          // default resident CTAs per SM of the forward compositor (0 = whatever fits)
@@ -51,6 +52,7 @@ struct CompositeFwdParams {
     float* final_T;
     int* n_contrib;
     float *out_color, *out_opacity, *out_depth, *out_feature, *out_weights;
+    uint64_t* det_weights;             // DET: [P] out_weights in exact 2^-24 units (zeroed), converted by det_weights_kernel
 };
 
 #ifdef R3DG_WARP_TIMING
@@ -71,7 +73,9 @@ extern "C" int r3dg_debug_wt_fwd(void* dst, size_t bytes) { return (int)cudaMemc
 //   UBLKCP) of its entry's record (recf * 4 bytes, 16-byte aligned) straight into a double-buffered AoS slab; the
 //   warp's mbarrier counts the transaction bytes.  No prefetch registers (12-28 fewer live registers), no staging
 //   stores.  Selected with r3dg_tune("composite_bulk", 1); the register prefetch is the default.
-template <int NG, int NW, int MINB, bool BULK>
+// DET (deterministic mode): the per-warp integer weight sums go to a u64 per Gaussian instead of a float atomic, so
+//   out_weights does not depend on the order in which warps finish.  Everything else is the same code.
+template <int NG, int NW, int MINB, bool BULK, bool DET = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const CompositeFwdParams p) {
     constexpr int RG = 2 + NG;                       // float4 groups per record
     __shared__ __align__(16) float4 sRec[BULK ? 1 : NW][BULK ? 1 : RG][BULK ? 1 : 32];   // this warp's current 32-entry batch, SoA
@@ -262,7 +266,11 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             if (__all_sync(0xffffffffu, done)) { all_done = true; break; }      // once per round: entries after the last
         }                                                                        // pixel finished change nothing (valid needs !done)
         if (last_j >= 0) last_contributor = q[(h0 + last_j) & (R3DG_QCAP - 1)] + 1u;     // 1-based position in the tile list
-        if (my_wsum != 0) atomicAdd(&p.out_weights[sId[warp][lane]], (float)my_wsum * (1.0f / 16777216.0f));
+        if constexpr (DET) {
+            if (my_wsum != 0) det_red_u64(p.det_weights + sId[warp][lane], (uint64_t)(uint32_t)my_wsum);   // my_wsum > 0
+        } else {
+            if (my_wsum != 0) atomicAdd(&p.out_weights[sId[warp][lane]], (float)my_wsum * (1.0f / 16777216.0f));
+        }
         stage ^= 1;
         composited += (uint32_t)__popc(cw);
         // contributor bits for the backward pass: one fire-and-forget atomic per composited entry
@@ -287,6 +295,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
 #ifdef R3DG_WARP_TIMING
     if (lane == 0 && blockIdx.x * NW + warp < R3DG_WT_MAX) g_wt_fwd[blockIdx.x * NW + warp] = WarpTiming{wt_t0, wt_now(), wt_iters, wt_smid()};
 #endif
+}
+
+// Deterministic mode: out_weights = the exact integer total in 2^-24 units, rounded to fp32 once.
+__global__ void __launch_bounds__(256) det_weights_kernel(int P, const uint64_t* __restrict__ acc, float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < P) out[i] = __fmul_rn(__ull2float_rn(acc[i]), 1.0f / 16777216.0f);
 }
 
 // renderSurfaceXYZCUDA + renderPseudoNormalCUDA fused: neighbours' surface points are recomputed
@@ -383,6 +397,11 @@ static void launch_fwd_kernel(K kernel, const CompositeFwdParams& p, int tiles, 
 template <int NG>
 static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, cudaStream_t stream) {
     composite_env();
+    if (p.det_weights) {
+        if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel(composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true, true>, p, tiles, stream);
+        else launch_fwd_kernel(composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false, true>, p, tiles, stream);
+        return;
+    }
     if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel(composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true>, p, tiles, stream);
     else launch_fwd_kernel(composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false>, p, tiles, stream);
 }
@@ -406,6 +425,8 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl
     p.n_contrib = (int*)(img + il.n_contrib);
     p.out_color = a.out_color; p.out_opacity = a.out_opacity; p.out_depth = a.out_depth;
     p.out_feature = a.out_feature; p.out_weights = a.out_weights;
+    p.det_weights = a.deterministic ? (uint64_t*)a.det_work : nullptr;
+    if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, (size_t)a.P * 8, stream));
     const int tiles = p.gx * gy;
     switch (num_groups(a.S)) {
         case 1: launch_fwd_ng<1>(p, tiles, stream); break;
@@ -419,6 +440,7 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl
         case 9: launch_fwd_ng<9>(p, tiles, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;
     }
+    if (p.det_weights && a.P > 0) det_weights_kernel<<<(a.P + 255) / 256, 256, 0, stream>>>(a.P, p.det_weights, a.out_weights);
     const size_t HW = (size_t)a.H * a.W;
     mark(6, stream);
     if (a.computer_pseudo_normal) {

@@ -22,6 +22,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "common.cuh"
+#include "detacc.cuh"
 #include "kernels.h"
 
 #ifndef R3DG_BWD_CTAS          // default resident CTAs per SM of the backward compositor (0 = whatever fits)
@@ -51,6 +52,7 @@ struct CompositeBwdParams {
     const int* n_contrib;
     const float *dL_dpix, *dL_dpix_o, *dL_dpix_d, *dL_dpix_f;
     float* grad;     // [P][recf], zero-initialised
+    DetAcc det;      // DET: the same rows as fixed-point accumulators (detacc.cuh), [P * recf], zero-initialised
 };
 
 // Sum v[i] over the 32 lanes for every i in [0,N) (N power of two, 4 <= N <= 32) with a
@@ -152,7 +154,9 @@ __device__ __forceinline__ void reduce_scatter_permuted_multi(float (&x)[U][W], 
 // its tile's contributor bytes BACK TO FRONT, 128 instances per step, compacts the positions whose bit is set into a
 // circular queue (warp scan) and processes batches of 32 of them: every staged entry is one that some pixel of the
 // block composited in the forward pass — no culling test, no record fetch and no exp() for anything else.
-template <int NG, int NW, int MINB>
+// DET (deterministic mode): each finished row component is added through the order-independent fixed-point primitive
+// (detacc.cuh) into p.det instead of by a float atomic into p.grad.  Everything else is the same code.
+template <int NG, int NW, int MINB, bool DET = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const CompositeBwdParams p) {
     constexpr int NC = 4 * NG;              // padded channel count {r,g,b,f...}; gradient row = 8 geometry slots + NC
     // the NC channel components are reduced in power-of-two chunks of 16 / 8 / 4 (select-free butterflies)
@@ -417,11 +421,19 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 if (j0 + u < n) {                                           // (warp-uniform)
-                    float* grow = p.grad + sId[warp][ju[u]];
-                    if constexpr (C4_SECOND) {
-                        if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) atomicAdd(grow + 8 + B4 + (lane >> 3), t4[u]);
+                    if constexpr (DET) {
+                        const size_t row = sId[warp][ju[u]];
+                        if constexpr (C4_SECOND) {
+                            if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) det_add(p.det, row + 8 + B4 + (lane >> 3), t4[u]);
+                        }
+                        if (my_sel >= 0) det_add(p.det, row + my_off, mine[u]);
+                    } else {
+                        float* grow = p.grad + sId[warp][ju[u]];
+                        if constexpr (C4_SECOND) {
+                            if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) atomicAdd(grow + 8 + B4 + (lane >> 3), t4[u]);
+                        }
+                        if (my_sel >= 0) atomicAdd(grow + my_off, mine[u]);
                     }
-                    if (my_sel >= 0) atomicAdd(grow + my_off, mine[u]);
                 }
             }
         }
@@ -450,10 +462,10 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
     g_bwd_ctas = value;
     return 0;
 }
-template <int NG>
+template <int NG, bool DET>
 static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
     composite_bwd_env();
-    auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v>;
+    auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET>;
     static int pad_for = -1, pad_dev = -1;
     static size_t pad = 0;
     int dev = 0;
@@ -481,18 +493,21 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const GeomLayout& g
     p.dL_dpix_f = a.dL_dout_feature;
     p.grad = (float*)(geom + gl.grad);
     p.n_contrib = (const int*)(img + il.n_contrib);
-    R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)a.P * gl.recf * 4, stream));
+    const bool det = a.deterministic != 0;
+    p.det = det_acc(a.det_work, (size_t)a.P * gl.recf);
+    if (det) R3DG_CUDA_TRY(cudaMemsetAsync(a.det_work, 0, det_bytes(p.det.n), stream));
+    else R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)a.P * gl.recf * 4, stream));
     const int tiles = p.gx * gy;
     int rc = launch_cta_order((const uint32_t*)(img + il.bwd_work), (uint32_t*)(img + il.bwd_order), 2 * tiles, stream);
     if (rc != 0) return rc;
     switch (num_groups(a.S)) {
-        case 1: launch_bwd_ng<1>(p, tiles, stream); break;
-        case 2: launch_bwd_ng<2>(p, tiles, stream); break;
-        case 3: launch_bwd_ng<3>(p, tiles, stream); break;
-        case 4: launch_bwd_ng<4>(p, tiles, stream); break;
-        case 5: launch_bwd_ng<5>(p, tiles, stream); break;
-        case 6: launch_bwd_ng<6>(p, tiles, stream); break;
-        case 7: launch_bwd_ng<7>(p, tiles, stream); break;
+        case 1: det ? launch_bwd_ng<1, true>(p, tiles, stream) : launch_bwd_ng<1, false>(p, tiles, stream); break;
+        case 2: det ? launch_bwd_ng<2, true>(p, tiles, stream) : launch_bwd_ng<2, false>(p, tiles, stream); break;
+        case 3: det ? launch_bwd_ng<3, true>(p, tiles, stream) : launch_bwd_ng<3, false>(p, tiles, stream); break;
+        case 4: det ? launch_bwd_ng<4, true>(p, tiles, stream) : launch_bwd_ng<4, false>(p, tiles, stream); break;
+        case 5: det ? launch_bwd_ng<5, true>(p, tiles, stream) : launch_bwd_ng<5, false>(p, tiles, stream); break;
+        case 6: det ? launch_bwd_ng<6, true>(p, tiles, stream) : launch_bwd_ng<6, false>(p, tiles, stream); break;
+        case 7: det ? launch_bwd_ng<7, true>(p, tiles, stream) : launch_bwd_ng<7, false>(p, tiles, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;   // S > 24: reference backward limit (backward.cu:449)
     }
     R3DG_CUDA_TRY(cudaGetLastError());

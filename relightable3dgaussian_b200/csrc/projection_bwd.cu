@@ -9,6 +9,7 @@
 //  * the input gradient is one packed [RECF] row per Gaussian produced by the compositor;
 //  * cov3D is recomputed from scale/rotation instead of being stored and re-read.
 #include "common.cuh"
+#include "detacc.cuh"
 #include "kernels.h"
 
 namespace r3dg {
@@ -25,6 +26,7 @@ struct ProjBwdParams {
     float *dL_dmeans2D, *dL_dcolors, *dL_dopacity, *dL_dmeans3D, *dL_dfeatures, *dL_dcov3D, *dL_dsh,
         *dL_dscales, *dL_drotations;
     float* dL_dsh_factor;       // [P,3] gated dL_dRGB (multi-GPU exchange, sh_exchange.cu); dL_dsh may then be NULL
+    DetAcc det;                 // DET: the gradient rows as fixed-point accumulators (composite_bwd.cu), read instead of grad
 };
 
 __device__ __forceinline__ void cov3d_plain(const float* s3, float mod, const float* q, float* c6,
@@ -51,6 +53,8 @@ __device__ __forceinline__ void cov3d_plain(const float* s3, float mod, const fl
 
 #define PROJ_THREADS 128
 #define SLAB_LD (PROJ_THREADS + 1)
+// DET (deterministic mode): the packed gradient row is read from the fixed-point accumulators and converted on load.
+template <bool DET = false>
 __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const ProjBwdParams p) {
     // SH rows (192 B at M=16) travel through shared memory: the CTA's [128][3M] slab of shs is ONE contiguous
     // 24 KB block, fetched by a single TMA-unit bulk copy (cp.async.bulk, mbarrier-signalled) into a row-major
@@ -82,7 +86,14 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     float m3[3] = {0, 0, 0}, s3[3] = {0, 0, 0};
     unsigned cl = 0;
     if (visible) {
-        gA = g4[0]; gB = g4[1]; gC = g4[2];
+        if constexpr (DET) {
+            const size_t r0 = (size_t)idx * p.recf;
+            gA = make_float4(det_load(p.det, r0), det_load(p.det, r0 + 1), det_load(p.det, r0 + 2), det_load(p.det, r0 + 3));
+            gB = make_float4(det_load(p.det, r0 + 4), det_load(p.det, r0 + 5), det_load(p.det, r0 + 6), 0.0f);
+            gC = make_float4(det_load(p.det, r0 + 8), det_load(p.det, r0 + 9), det_load(p.det, r0 + 10), 0.0f);
+        } else {
+            gA = g4[0]; gB = g4[1]; gC = g4[2];
+        }
         m3[0] = p.means3D[3 * (size_t)idx]; m3[1] = p.means3D[3 * (size_t)idx + 1]; m3[2] = p.means3D[3 * (size_t)idx + 2];
         if (!p.cov3D_precomp) {
             q4 = *reinterpret_cast<const float4*>(p.rotations + 4 * (size_t)idx);
@@ -108,7 +119,10 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     // feature gradients: straight copy-out of the packed row
     if (p.S > 0 && in_range) {
         float* df = p.dL_dfeatures + (size_t)idx * p.S;
-        for (int c = 0; c < p.S; ++c) df[c] = visible ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f;
+        for (int c = 0; c < p.S; ++c) {
+            if constexpr (DET) df[c] = visible ? det_load(p.det, (size_t)idx * p.recf + 11 + c) : 0.0f;
+            else df[c] = visible ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f;
+        }
     }
     if (visible) {
         dmean2[0] = gA.x; dmean2[1] = gA.y; dmean2[2] = gA.z; dop = gA.w;
@@ -403,8 +417,11 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const GeomLayout& 
     p.dL_dmeans3D = a.dL_dmeans3D; p.dL_dfeatures = a.dL_dfeatures; p.dL_dcov3D = a.dL_dcov3D;
     p.dL_dsh = a.dL_dsh; p.dL_dscales = a.dL_dscales; p.dL_drotations = a.dL_drotations;
     p.dL_dsh_factor = a.dL_dsh_factor;
+    p.det = det_acc(a.det_work, (size_t)a.P * gl.recf);
     const size_t sh_smem = a.shs ? (size_t)3 * a.M * SLAB_LD * sizeof(float) : 0;
-    projection_bwd_kernel<<<(a.P + PROJ_THREADS - 1) / PROJ_THREADS, PROJ_THREADS, sh_smem, stream>>>(p);
+    const int blocks = (a.P + PROJ_THREADS - 1) / PROJ_THREADS;
+    if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    else projection_bwd_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -21,6 +21,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "common.cuh"
+#include "detacc.cuh"
 #include "kernels.h"
 
 namespace r3dg {
@@ -39,6 +40,7 @@ struct ShadeArgs {
     // backward
     const float *g_pbr, *g_diffuse, *g_specular;
     float *d_base, *d_rough, *d_view, *d_incidents, *d_env;
+    DetAcc det;                                  // deterministic mode: dL/denv accumulators [He * We * 3] (detacc.cuh)
 };
 
 __device__ __forceinline__ void sh_basis3(float x, float y, float z, float* w) {
@@ -317,7 +319,10 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? 6 : 1) shade_fwd_ker
 // intra-warp collisions with a one-byte tag per texel: every pending lane stores its lane id, the
 // id that survives owns the texel this round and does a plain 128-bit read-modify-write, the losers
 // retry.  The copies are summed and flushed once per CTA.
-enum { ENV_GLOBAL = 0, ENV_CAS = 1, ENV_TAG = 2 };
+// The deterministic mode accumulates every tap through the fixed-point primitive (detacc.cuh): ENV_DET_SMEM into
+// per-CTA integer accumulators in shared memory whose words are added to the global ones once per CTA (integer sums,
+// so the flush order does not matter either), ENV_DET_GLOBAL straight into the global accumulators (larger textures).
+enum { ENV_GLOBAL = 0, ENV_CAS = 1, ENV_TAG = 2, ENV_DET_SMEM = 3, ENV_DET_GLOBAL = 4 };
 
 __device__ __forceinline__ void warp_private_add(float4* wg, volatile unsigned char* tag, int texel, float x, float y, float z, int lane) {
     bool pending = texel >= 0;
@@ -336,11 +341,12 @@ __device__ __forceinline__ void warp_private_add(float4* wg, volatile unsigned c
 }
 
 // resident CTAs the register allocation is pinned to: variant 1 -> 3 (<= 168 registers); variant 2 ->
-// 3 with the warp-private env copies (67 KB of shared memory per CTA), 5 otherwise (<= 102 registers)
+// 3 with the warp-private env copies (67 KB of shared memory per CTA) or the deterministic modes (their fixed-point
+// conversion spills at 102 registers), 5 otherwise (<= 102 registers)
 template <int ENV_MODE, int G, int VAR>
-__global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (ENV_MODE == 2 ? 3 : 5)) shade_bwd_kernel(const ShadeArgs a) {
+__global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (ENV_MODE <= 1 ? 5 : 3)) shade_bwd_kernel(const ShadeArgs a) {
     extern __shared__ __align__(16) float s_bwd[];    // [incident slots (VAR >= 1)][gradient accumulators (VAR 2)][env ...]
-    constexpr bool SMEM_ENV = ENV_MODE != ENV_GLOBAL;
+    constexpr bool SMEM_ENV = ENV_MODE != ENV_GLOBAL && ENV_MODE != ENV_DET_GLOBAL;
     constexpr int GPW = 32 / G;
     constexpr int INC_FLOATS = VAR >= 1 ? SHADE_WARPS * GPW * SHADE_INC_STRIDE : 0;
     constexpr int DINC_FLOATS = VAR == 2 ? 48 * SHADE_THREADS : 0;
@@ -358,10 +364,18 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
     float4* wgrad_all = reinterpret_cast<float4*>(s_mem + ne4);
     float4* wgrad = wgrad_all + (size_t)warp * nt;
     volatile unsigned char* wtag = reinterpret_cast<unsigned char*>(wgrad_all + (size_t)SHADE_WARPS * nt) + (size_t)warp * ntp;
+    // ENV_DET_SMEM: [env ne (padded to 2)][accumulator words 3 ne][flag words (ne + 15) / 16]
+    uint64_t* s_dwords = reinterpret_cast<uint64_t*>(s_mem + ((ne + 1) & ~1));
+    uint32_t* s_dflags = reinterpret_cast<uint32_t*>(s_dwords + 3 * (size_t)ne);
+    const int nflag = (ne + 15) >> 4;
     if (SMEM_ENV) {
         for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_env[i] = a.env[i];
         if (ENV_MODE == ENV_CAS) for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_genv[i] = 0.f;
         if (ENV_MODE == ENV_TAG) for (int i = threadIdx.x; i < SHADE_WARPS * nt; i += SHADE_THREADS) wgrad_all[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (ENV_MODE == ENV_DET_SMEM) {
+            for (int i = threadIdx.x; i < 3 * ne; i += SHADE_THREADS) s_dwords[i] = 0u;
+            for (int i = threadIdx.x; i < nflag; i += SHADE_THREADS) s_dflags[i] = 0u;
+        }
         __syncthreads();
     }
     const float* env = SMEM_ENV ? s_env : a.env;
@@ -437,6 +451,17 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
                     const int texel = (any && e.taps.idx[t] >= 0) ? e.taps.idx[t] / 3 : -1;
                     warp_private_add(wgrad, wtag, texel, dG[0] * e.taps.w[t], dG[1] * e.taps.w[t], dG[2] * e.taps.w[t], lane);
                 }
+            } else if (ENV_MODE == ENV_DET_SMEM || ENV_MODE == ENV_DET_GLOBAL) {
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                    if (dG[c] != 0.f) {
+#pragma unroll
+                        for (int t = 0; t < 4; ++t)
+                            if (e.taps.idx[t] >= 0) {
+                                if (ENV_MODE == ENV_DET_SMEM) det_add(s_dwords, s_dflags, ne, e.taps.idx[t] + c, dG[c] * e.taps.w[t], true);
+                                else det_add(a.det, e.taps.idx[t] + c, dG[c] * e.taps.w[t]);
+                            }
+                    }
             } else {
 #pragma unroll
                 for (int c = 0; c < 3; ++c)
@@ -522,6 +547,20 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
             if (s.z != 0.f) atomicAdd(a.d_env + 3 * t + 2, s.z);
         }
     }
+    if (ENV_MODE == ENV_DET_SMEM) {
+        __syncthreads();
+        for (int i = threadIdx.x; i < 3 * ne; i += SHADE_THREADS) {
+            const uint64_t v = s_dwords[i];
+            if (v) det_red_u64(a.det.words + (size_t)(i / ne) * a.det.n + (i % ne), v);
+        }
+        for (int i = threadIdx.x; i < nflag; i += SHADE_THREADS) { const uint32_t f = s_dflags[i]; if (f) atomicOr(a.det.flags + i, f); }
+    }
+}
+
+// deterministic mode: dL/denv from its accumulators, every element written
+__global__ void __launch_bounds__(256) det_env_kernel(const DetAcc acc, float* __restrict__ out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < acc.n) out[i] = det_load(acc, i);
 }
 
 // ---- launch ---------------------------------------------------------------------------------------
@@ -608,8 +647,24 @@ static int launch_bwd(const ShadeArgs& a, int num_sms, size_t env_smem, cudaStre
     return shade_launch(shade_bwd_kernel<MODE, 32, 0>, a, units, num_sms, smem, stream);
 }
 
+// shared memory of ENV_DET_SMEM (env, accumulator words, flag words); larger textures use ENV_DET_GLOBAL
+static size_t det_smem_bytes(size_t ne) { return ((ne + 1) & ~(size_t)1) * sizeof(float) + 3 * ne * 8 + (ne + 15) / 16 * 4; }
+
 int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
     const size_t nt = (size_t)a.He * a.We, env_bytes = nt * 3 * sizeof(float);
+    if (a.det.words) {
+        R3DG_CUDA_TRY(cudaMemsetAsync(a.det.words, 0, det_bytes(a.det.n), stream));
+        int rc = 0;
+        if (a.P > 0) {
+            const size_t smem = det_smem_bytes(a.det.n);
+            a.env_in_smem = smem <= 64 * 1024;
+            rc = a.env_in_smem ? launch_bwd<ENV_DET_SMEM>(a, num_sms, smem, stream) : launch_bwd<ENV_DET_GLOBAL>(a, num_sms, 0, stream);
+        }
+        if (rc) return rc;
+        det_env_kernel<<<(unsigned)((a.det.n + 255) / 256), 256, 0, stream>>>(a.det, a.d_env);
+        R3DG_CUDA_TRY(cudaGetLastError());
+        return 0;
+    }
     R3DG_CUDA_TRY(cudaMemsetAsync(a.d_env, 0, env_bytes, stream));
     if (a.P <= 0) return 0;
     // shared-memory cost of the env-gradient modes (kept within the 48 KB that need no opt-in on their own)
@@ -648,6 +703,7 @@ static int fill_args(const r3dg_shade_args* s, ShadeArgs& a) {
     a.g_pbr = s->dL_dpbr; a.g_diffuse = s->dL_ddiffuse_light; a.g_specular = s->dL_dspecular;
     a.d_base = s->dL_dbase_color; a.d_rough = s->dL_droughness; a.d_view = s->dL_dviewdirs; a.d_incidents = s->dL_dincidents;
     a.d_env = s->dL_denv;
+    a.det = DetAcc{nullptr, nullptr, 0};
     return 0;
 }
 
@@ -666,7 +722,16 @@ int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream
     int rc = fill_args(s, a);
     if (rc) return rc;
     if (!a.g_pbr || !a.d_base || !a.d_rough || !a.d_view || !a.d_incidents || !a.d_env) return R3DG_ERR_BAD_ARG;
+    if (s->deterministic) {
+        const size_t n = (size_t)a.He * a.We * 3;
+        if (!s->det_work || s->det_work_bytes < det_bytes(n)) return R3DG_ERR_BAD_ARG;
+        a.det = det_acc(s->det_work, n);
+    }
     return launch_shade_backward(a, shade_num_sms(), (cudaStream_t)stream);
+}
+
+size_t r3dg_shade_det_bytes(int env_h, int env_w) {
+    return env_h > 0 && env_w > 0 ? det_bytes((size_t)env_h * env_w * 3) : 0;
 }
 
 }  // extern "C"

@@ -9,7 +9,9 @@ extension module to replace; `install()` rebinds `gaussian_renderer.neilf.render
 
 Gradients: base_color, roughness, viewdirs, incidents and the light's environment map (through
 `light.get_env`, i.e. softplus, in PyTorch); normals and the baked tensors receive none, exactly as
-in the reference call (neilf.py:92-96).  The per-sample entries of extra_results
+in the reference call (neilf.py:92-96).  Under torch.use_deterministic_algorithms(True), read at call
+time, the backward accumulates the environment-map gradient in fixed point, so every gradient is
+bitwise reproducible (the reference's grid_sample backward raises under that flag).  The per-sample entries of extra_results
 (`incident_lights`, `local_incident_lights`, `global_incident_lights`) are materialised lazily on
 first access (eval only) and carry no gradient.
 """
@@ -88,6 +90,9 @@ class _RenderEquation(torch.autograd.Function):
         a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = [t.data_ptr() for t in g]
         a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = d_base.data_ptr(), d_rough.data_ptr(), d_view.data_ptr()
         a.dL_dincidents, a.dL_denv = d_inc.data_ptr(), d_env.data_ptr()
+        if torch.are_deterministic_algorithms_enabled():
+            ws = torch.empty((lib.r3dg_shade_det_bytes(env.shape[0], env.shape[1]),), dtype=torch.uint8, device=dev)
+            a.deterministic, a.det_work, a.det_work_bytes = 1, ws.data_ptr(), ws.numel()
         with torch.cuda.device(dev):
             _lib.check(lib.r3dg_render_equation_backward(ctypes.byref(a), torch.cuda.current_stream(dev).cuda_stream),
                        "rendering_equation backward")
