@@ -7,31 +7,21 @@ import torch
 from . import _lib
 
 
-def _c(t, dtype=torch.float32):
-    if t.dtype != dtype:
-        t = t.to(dtype)
-    return t.contiguous()
-
-
 def create_bvh(means3D, scales, rotations, nodes, aabbs):
     """== create_bvh (bvh/src/bvh.cu:8-27).  `nodes` i32[2P-1,5] / `aabbs` f32[2P-1,6] are pre-filled
     by the caller (bvh/__init__.py:32-57) and completed IN PLACE; returns (nodes, aabbs, morton i64[P]).
     means3D / scales / rotations are unused by the reference's construct_bvh too."""
-    lib = _lib.load()
     P = means3D.size(0)
     assert nodes.is_cuda and nodes.dtype == torch.int32 and nodes.is_contiguous() and nodes.shape == (2 * P - 1, 5)
     assert aabbs.is_cuda and aabbs.dtype == torch.float32 and aabbs.is_contiguous() and aabbs.shape == (2 * P - 1, 6)
     morton = torch.zeros((P,), dtype=torch.int64, device=means3D.device)
-    tmp = torch.empty((lib.r3dg_bvh_build_tmp_bytes(P),), dtype=torch.uint8, device=means3D.device)
-    stream = torch.cuda.current_stream(means3D.device)
-    with torch.cuda.device(means3D.device):
-        _lib.check(lib.r3dg_bvh_build(P, nodes.data_ptr(), aabbs.data_ptr(), morton.data_ptr(), tmp.data_ptr(),
-                                      tmp.numel(), stream.cuda_stream), "create_bvh")
+    tmp = _lib.scratch(_lib.load().r3dg_bvh_build_tmp_bytes(P), means3D.device)
+    _lib.call("r3dg_bvh_build", means3D.device, P, nodes.data_ptr(), aabbs.data_ptr(), morton.data_ptr(), tmp.data_ptr(),
+              tmp.numel(), what="create_bvh")
     return nodes, aabbs, morton
 
 
 def _trace(nodes, aabbs, rays_o, rays_per_origin, origin_offset, rays_d, means3D, covs3D, opacities, normals):
-    lib = _lib.load()
     P = means3D.size(0)
     dev = rays_d.device
     out_shape = rays_d.shape[:-1]
@@ -40,18 +30,14 @@ def _trace(nodes, aabbs, rays_o, rays_per_origin, origin_offset, rays_d, means3D
     rendered_opacity = torch.empty(out_shape, dtype=torch.float32, device=dev)
     if num_rays == 0:
         return num_contributes, rendered_opacity
-    nodes, aabbs = _c(nodes, torch.int32), _c(aabbs)
-    rays_o, rays_d = _c(rays_o), _c(rays_d)
-    means3D, covs3D, opacities, normals = _c(means3D), _c(covs3D), _c(opacities), _c(normals)
-    tmp = torch.empty((lib.r3dg_bvh_trace_tmp_bytes(P),), dtype=torch.uint8, device=dev)
-    stream = torch.cuda.current_stream(dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.r3dg_bvh_trace_opacity(P, num_rays, nodes.data_ptr(), aabbs.data_ptr(), rays_o.data_ptr(),
-                                              int(rays_per_origin), float(origin_offset), rays_d.data_ptr(),
-                                              means3D.data_ptr(), covs3D.data_ptr(), opacities.data_ptr(),
-                                              normals.data_ptr(), num_contributes.data_ptr(),
-                                              rendered_opacity.data_ptr(), tmp.data_ptr(), tmp.numel(),
-                                              stream.cuda_stream), "trace_bvh_opacity")
+    nodes = nodes.to(torch.int32).contiguous()
+    aabbs, rays_o, rays_d = _lib.f32(aabbs), _lib.f32(rays_o), _lib.f32(rays_d)
+    means3D, covs3D, opacities, normals = _lib.f32(means3D), _lib.f32(covs3D), _lib.f32(opacities), _lib.f32(normals)
+    tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_tmp_bytes(P), dev)
+    _lib.call("r3dg_bvh_trace_opacity", dev, P, num_rays, nodes.data_ptr(), aabbs.data_ptr(), rays_o.data_ptr(),
+              int(rays_per_origin), float(origin_offset), rays_d.data_ptr(), means3D.data_ptr(), covs3D.data_ptr(),
+              opacities.data_ptr(), normals.data_ptr(), num_contributes.data_ptr(), rendered_opacity.data_ptr(),
+              tmp.data_ptr(), tmp.numel(), what="trace_bvh_opacity")
     return num_contributes, rendered_opacity
 
 

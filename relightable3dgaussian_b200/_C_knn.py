@@ -6,13 +6,11 @@ from . import _lib
 
 def distCUDA2(points):
     """== distCUDA2 (spatial.cu:15-26): f32[P] mean squared distance to the 3 nearest neighbours."""
-    lib = _lib.load()
     P = points.size(0)
-    pts = points.detach().float().contiguous()
+    pts = _lib.f32(points)
     out = torch.full((P,), 0.0, dtype=torch.float32, device=points.device)
     if P > 0:
-        tmp = torch.empty((lib.r3dg_knn_tmp_bytes(P),), dtype=torch.uint8, device=points.device)
-        with torch.cuda.device(points.device):
-            _lib.check(lib.r3dg_knn_dist2(P, pts.data_ptr(), out.data_ptr(), tmp.data_ptr(), tmp.numel(),
-                                          torch.cuda.current_stream(points.device).cuda_stream), "distCUDA2")
+        tmp = _lib.scratch(_lib.load().r3dg_knn_tmp_bytes(P), points.device)
+        _lib.call("r3dg_knn_dist2", points.device, P, pts.data_ptr(), out.data_ptr(), tmp.data_ptr(), tmp.numel(),
+                  what="distCUDA2")
     return out

@@ -19,6 +19,7 @@ deterministic mode: out_weights and the nine gradients are then bitwise reproduc
 float atomics make them run-to-run nondeterministic).  Its workspace comes from the torch allocator.
 """
 import ctypes
+import warnings
 
 import torch
 
@@ -78,26 +79,6 @@ class DeferredCount:
         return f"DeferredCount({self._value if self._value is not None else 'pending'})"
 
 
-def _ptr(t):
-    """Device pointer of an optional tensor; empty tensors mean "absent" (NULL), like the
-    reference (forward.cu:206,242)."""
-    if t is None or t.numel() == 0:
-        return None
-    return t.data_ptr()
-
-
-def _det_workspace(nbytes, dev):
-    """Workspace of the deterministic mode when torch.are_deterministic_algorithms_enabled(), else None."""
-    if not torch.are_deterministic_algorithms_enabled():
-        return None
-    return torch.empty((nbytes,), dtype=torch.uint8, device=dev)
-
-
-def _set_det(a, ws):
-    if ws is not None:
-        a.deterministic, a.det_work, a.det_work_bytes = 1, ws.data_ptr(), ws.numel()
-
-
 def _prep(t, name):
     if t is None or t.numel() == 0:
         return t
@@ -151,7 +132,6 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     if prev is not None:                 # a deferred forward whose backward never ran: account for it now
         prev.resolve()
         if prev.overflowed:
-            import warnings
             warnings.warn("a deferred-count forward overflowed its binning buffer and was never differentiated; "
                           "its images were truncated (use the synchronous path for forwards without backward)")
     if st["seen"] < _LEARN:
@@ -162,52 +142,50 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
         capacity = max(int(st["rmax"] * _HEADROOM) + 4096, 4 * P + 4096)
     else:
         capacity = max(st["capacity"], 4 * P + 4096)
-    stream = torch.cuda.current_stream(dev)
-    det_ws = _det_workspace(lib.r3dg_raster_fwd_det_bytes(P), dev)
+    a = _lib.RasterFwdArgs()
+    a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
+    a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
+    a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.opacities = _lib.ptr(opacity)
+    a.scales = _lib.ptr(scales); a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
+    a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
+    a.scale_modifier = float(scale_modifier); a.tan_fovx = float(tan_fovx)
+    a.tan_fovy = float(tan_fovy); a.cx = float(cx); a.cy = float(cy)
+    a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
+    a.debug = int(bool(debug))
+    a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
+    a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
+    a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
+    a.out_weights = _lib.ptr(out_weights); a.radii = _lib.ptr(radii); a.n_contrib = None
+    a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
+    a.img = imgBuffer.data_ptr(); a.img_bytes = imgBuffer.numel()
+    det_ws = _lib.det_workspace(a, lib.r3dg_raster_fwd_det_bytes(P), dev)
     slot = st["next"]
     st["next"] = (slot + 1) % _SLOTS
     pinned = st["pinned"][slot:slot + 1]
-    with torch.cuda.device(dev):
-        while True:
-            binningBuffer = torch.empty((lib.r3dg_raster_binning_bytes(capacity),), dtype=torch.uint8,
-                                        device=dev)
-            a = _lib.RasterFwdArgs()
-            a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
-            a.background = _ptr(background); a.means3D = _ptr(means3D); a.shs = _ptr(sh)
-            a.colors_precomp = _ptr(colors); a.features = _ptr(features); a.opacities = _ptr(opacity)
-            a.scales = _ptr(scales); a.rotations = _ptr(rotations); a.cov3D_precomp = _ptr(cov3D_precomp)
-            a.viewmatrix = _ptr(viewmatrix); a.projmatrix = _ptr(projmatrix); a.campos = _ptr(campos)
-            a.scale_modifier = float(scale_modifier); a.tan_fovx = float(tan_fovx)
-            a.tan_fovy = float(tan_fovy); a.cx = float(cx); a.cy = float(cy)
-            a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
-            a.debug = int(bool(debug))
-            a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
-            a.out_depth = out_depth.data_ptr(); a.out_feature = _ptr(out_feature)
-            a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
-            a.out_weights = _ptr(out_weights); a.radii = _ptr(radii); a.n_contrib = None
-            a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
-            a.img = imgBuffer.data_ptr(); a.img_bytes = imgBuffer.numel()
-            a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-            a.num_rendered_host = pinned.data_ptr()
-            # recorded by the library right after the count's D2H copy — a quarter into the forward, not at its end
-            ev = torch.cuda.Event()
-            ev.record(stream)             # (creates the underlying cudaEvent_t; re-recorded inside the call)
-            a.count_ready_event = ev.cuda_event
-            _set_det(a, det_ws)
-            _lib.check(lib.r3dg_raster_forward(ctypes.byref(a), stream.cuda_stream), "rasterize_gaussians")
-            if _defer:                    # opt-in: let the host run ahead; the count is resolved later
-                rendered = DeferredCount(ev, pinned, capacity, st, P)
-                st["pending"] = rendered
-                break
-            if debug:
-                stream.synchronize()
-            else:
-                ev.synchronize()          # the one readback: num_rendered is part of the return tuple.  The host resumes
+    a.num_rendered_host = pinned.data_ptr()
+    stream = torch.cuda.current_stream(dev)
+    while True:
+        # this module's torch.empty, not _lib.scratch: tests substitute it to hand the forward a reused binning buffer
+        binningBuffer = torch.empty((lib.r3dg_raster_binning_bytes(capacity),), dtype=torch.uint8, device=dev)
+        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
+        # recorded by the library right after the count's D2H copy — a quarter into the forward, not at its end
+        ev = torch.cuda.Event()
+        ev.record(stream)                 # (creates the underlying cudaEvent_t; re-recorded inside the call)
+        a.count_ready_event = ev.cuda_event
+        _lib.call("r3dg_raster_forward", dev, ctypes.byref(a), what="rasterize_gaussians")
+        if _defer:                        # opt-in: let the host run ahead; the count is resolved later
+            rendered = DeferredCount(ev, pinned, capacity, st, P)
+            st["pending"] = rendered
+            break
+        if debug:
+            stream.synchronize()
+        else:
+            ev.synchronize()              # the one readback: num_rendered is part of the return tuple.  The host resumes
                                           # while the compositor still runs and can enqueue the loss / backward behind it
-            rendered = int(pinned.item())
-            if rendered <= capacity:
-                break
-            capacity = int(rendered * 1.25) + 4096      # speculation missed: rerun with room to spare
+        rendered = int(pinned.item())
+        if rendered <= capacity:
+            break
+        capacity = int(rendered * 1.25) + 4096          # speculation missed: rerun with room to spare
     if not _defer:
         _observe(st, rendered, P)
     off = lib.r3dg_raster_img_n_contrib_offset(W, H)
@@ -273,45 +251,37 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     if P != 0:
         a = _lib.RasterBwdArgs()
         a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
-        a.background = _ptr(background); a.means3D = _ptr(means3D); a.shs = _ptr(sh)
-        a.colors_precomp = _ptr(colors); a.features = _ptr(features); a.scales = _ptr(scales)
-        a.rotations = _ptr(rotations); a.cov3D_precomp = _ptr(cov3D_precomp)
-        a.viewmatrix = _ptr(viewmatrix); a.projmatrix = _ptr(projmatrix); a.campos = _ptr(campos)
+        a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
+        a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.scales = _lib.ptr(scales)
+        a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
+        a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
         a.scale_modifier = float(scale_modifier); a.tan_fovx = float(tan_fovx); a.tan_fovy = float(tan_fovy)
         a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
-        a.dL_dout_color = _ptr(dL_dout_color); a.dL_dout_opacity = _ptr(dL_dout_opacity)
-        a.dL_dout_depth = _ptr(dL_dout_depth); a.dL_dout_feature = _ptr(dL_dout_feature)
-        a.dL_dmeans2D = _ptr(dL_dmeans2D); a.dL_dcolors = _ptr(dL_dcolors)
-        a.dL_dopacity = _ptr(dL_dopacity); a.dL_dmeans3D = _ptr(dL_dmeans3D)
-        a.dL_dfeatures = _ptr(dL_dfeatures); a.dL_dcov3D = _ptr(dL_dcov3D); a.dL_dsh = _ptr(dL_dsh)
-        a.dL_dscales = _ptr(dL_dscales); a.dL_drotations = _ptr(dL_drotations)
-        a.dL_dsh_factor = _ptr(sh_factor)
+        a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
+        a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
+        a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
+        a.dL_dopacity = _lib.ptr(dL_dopacity); a.dL_dmeans3D = _lib.ptr(dL_dmeans3D)
+        a.dL_dfeatures = _lib.ptr(dL_dfeatures); a.dL_dcov3D = _lib.ptr(dL_dcov3D); a.dL_dsh = _lib.ptr(dL_dsh)
+        a.dL_dscales = _lib.ptr(dL_dscales); a.dL_drotations = _lib.ptr(dL_drotations)
+        a.dL_dsh_factor = _lib.ptr(sh_factor)
         a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-        det_ws = _det_workspace(lib.r3dg_raster_bwd_det_bytes(P, S), dev)
-        _set_det(a, det_ws)
-        stream = torch.cuda.current_stream(dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_raster_backward(ctypes.byref(a), stream.cuda_stream),
-                       "rasterize_gaussians_backward")
+        det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(P, S), dev)
+        _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_gaussians_backward")
     return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
             dL_dscales, dL_drotations)
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):
     """== markVisible (rasterize_points.cu:237-256): bool[P] = view-space z > 0.2."""
-    lib = _lib.load()
     P = means3D.size(0)
     present = torch.zeros((P,), dtype=torch.bool, device=means3D.device)
     if P != 0:
         means3D = _prep(means3D, "means3D"); viewmatrix = _prep(viewmatrix, "viewmatrix")
         projmatrix = _prep(projmatrix, "projmatrix")
-        stream = torch.cuda.current_stream(means3D.device)
-        with torch.cuda.device(means3D.device):
-            _lib.check(lib.r3dg_mark_visible(P, means3D.data_ptr(), viewmatrix.data_ptr(),
-                                             projmatrix.data_ptr(), present.data_ptr(),
-                                             stream.cuda_stream), "mark_visible")
+        _lib.call("r3dg_mark_visible", means3D.device, P, means3D.data_ptr(), viewmatrix.data_ptr(),
+                  projmatrix.data_ptr(), present.data_ptr(), what="mark_visible")
     return present
 
 

@@ -7,6 +7,8 @@ kernels.
 import ctypes
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # R3DG_LIB_PATH: developer knob to A/B kernel builds (tools/variant_sweep.sh); unset = the in-tree library
 LIB_PATH = os.environ.get("R3DG_LIB_PATH") or os.path.join(_HERE, "libr3dg_b200.so")
@@ -186,3 +188,39 @@ def check(rc, what):
         if rc in (-10001, -10002):
             raise RuntimeError(f"{what}: {'bad argument' if rc == -10001 else 'unsupported configuration'} ({rc})")
         raise RuntimeError(f"{what}: CUDA error {-rc}")
+
+
+def call(name, device, *args, what=None):
+    """Run the launching entry point `name` on `device`, enqueued on torch's current stream of that device (every
+    launching entry point takes the stream last); a non-zero status raises through check() with `what`."""
+    with torch.cuda.device(device):
+        check(getattr(load(), name)(*args, torch.cuda.current_stream(device).cuda_stream), what or name)
+
+
+def scratch(nbytes, device):
+    """Uninitialised device workspace of `nbytes` bytes."""
+    return torch.empty((nbytes,), dtype=torch.uint8, device=device)
+
+
+def ptr(t):
+    """Device pointer of an optional tensor; empty tensors mean "absent" (NULL), like the
+    reference (forward.cu:206,242)."""
+    if t is None or t.numel() == 0:
+        return None
+    return t.data_ptr()
+
+
+def f32(t):
+    """`t` detached from autograd as a contiguous float32 tensor (the same storage when it already is one)."""
+    return t.detach().float().contiguous()
+
+
+def det_workspace(args, nbytes, device):
+    """Under torch.are_deterministic_algorithms_enabled(), read at call time: a workspace of `nbytes` for the
+    library's deterministic mode, entered into the argument struct `args` (deterministic, det_work, det_work_bytes).
+    Otherwise None, and `args` keeps the default mode.  The caller holds the workspace until the call is enqueued."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return None
+    ws = scratch(nbytes, device)
+    args.deterministic, args.det_work, args.det_work_bytes = 1, ws.data_ptr(), ws.numel()
+    return ws

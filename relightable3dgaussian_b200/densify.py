@@ -97,13 +97,10 @@ def add_densification_stats(model, viewspace_point_tensor, update_filter, weight
     devs = {grad.device, ngrad.device, weights.device, update_filter.device}
     if len(devs) != 1:
         raise RuntimeError("add_densification_stats: all tensors must live on one device")
-    dev = grad.device
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().r3dg_densify_stats(
-            P, grad.data_ptr(), grad.shape[1], ngrad.data_ptr(), update_filter.view(torch.uint8).data_ptr(), weights.data_ptr(),
-            radii.data_ptr() if radii is not None else None, model.weights_accum.data_ptr(), model.xyz_gradient_accum.data_ptr(),
-            model.normal_gradient_accum.data_ptr(), model.denom.data_ptr(), mr.data_ptr() if mr is not None else None,
-            torch.cuda.current_stream(dev).cuda_stream), "densify_stats")
+    _lib.call("r3dg_densify_stats", grad.device, P, grad.data_ptr(), grad.shape[1], ngrad.data_ptr(),
+              update_filter.view(torch.uint8).data_ptr(), weights.data_ptr(), radii.data_ptr() if radii is not None else None,
+              model.weights_accum.data_ptr(), model.xyz_gradient_accum.data_ptr(), model.normal_gradient_accum.data_ptr(),
+              model.denom.data_ptr(), mr.data_ptr() if mr is not None else None, what="densify_stats")
 
 
 def _groups(model, P):
@@ -156,57 +153,52 @@ def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, max
     th.max_screen_size = _f32(max_screen_size) if max_screen_size else 0.0
     th.big_scale = _f32(0.1 * extent)
     th.split_recip = split_recip
-    lib = _lib.load()
-    stream = torch.cuda.current_stream(dev)
     key = dev.index
     if key not in _pinned:
         _pinned[key] = torch.zeros(8, dtype=torch.int32).pin_memory()
     totals_h = _pinned[key]
-    with torch.cuda.device(dev):
-        tmp = torch.empty((lib.r3dg_densify_tmp_bytes(P),), dtype=torch.uint8, device=dev)
-        _lib.check(lib.r3dg_densify_classify(
-            P, model.xyz_gradient_accum.data_ptr(), model.normal_gradient_accum.data_ptr(), model.denom.data_ptr(),
-            model.weights_accum.data_ptr(), byname["scaling"].data_ptr(), byname["opacity"].data_ptr(), ctypes.byref(th),
-            tmp.data_ptr(), tmp.numel(), totals_h.data_ptr(), stream.cuda_stream), "densify_classify")
-        stream.synchronize()                                            # the one read-back
-        tot = [int(v) for v in totals_h.tolist()]
-        keep_a, keep_b, keep_c, n_split, n_clone, normal_sel, light = tot[:7]
-        P1 = P + n_clone
-        # clones enter the split test with a padded gradient of 0, and clones and split copies carry weights_accum = 1
-        zero_f, one_f, thn, wt = np.float32(0), np.float32(1), np.float32(max_grad_normal), np.float32(weights_threshold)
-        print("densify_and_split_normal:", normal_sel + (n_clone if zero_f >= thn else 0), "/", P1)
-        print("weights_accum:", light + (n_clone + 2 * n_split if one_f < wt else 0), "/", P1 + n_split)
-        z = _sampler((2 * n_split, 3), dev)
-        if z.shape != (2 * n_split, 3):
-            raise ValueError(f"densify_and_prune: sampler returned shape {tuple(z.shape)}, expected {(2 * n_split, 3)}")
-        z = _check(z, "normal samples")
-        Pn = keep_a + keep_b + 2 * keep_c
-        descs, hold, new = [], [], []
-        for g, name, p, st in groups:
-            kind = {"xyz": "xyz", "scaling": "scaling"}.get(name, "copy")
-            row_bytes = p[0].numel() * 4 if P > 0 else 4 * max(1, int(np.prod(p.shape[1:])))
-            np_ = torch.empty((Pn,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
-            work = [(p, np_, kind)]
-            moms = None
-            if st is not None:
-                moms = (torch.empty_like(np_), torch.empty_like(np_))
-                work += [(st["exp_avg"], moms[0], "moment"), (st["exp_avg_sq"], moms[1], "moment")]
-            for src, dst, k in work:
-                d = _lib.DensifyTensor()
-                d.src, d.dst, d.row_bytes, d.kind = src.data_ptr(), dst.data_ptr(), row_bytes, KIND[k]
-                descs.append(d)
-            new.append((g, name, p, st, np_, moms))
-        stats = {n: torch.empty((Pn, 1), dtype=torch.float32, device=dev) for n in STATS}
-        stats["max_radii2D"] = torch.empty((Pn,), dtype=torch.float32, device=dev)
-        for t in stats.values():
+    tmp = _lib.scratch(_lib.load().r3dg_densify_tmp_bytes(P), dev)
+    _lib.call("r3dg_densify_classify", dev, P, model.xyz_gradient_accum.data_ptr(), model.normal_gradient_accum.data_ptr(),
+              model.denom.data_ptr(), model.weights_accum.data_ptr(), byname["scaling"].data_ptr(), byname["opacity"].data_ptr(),
+              ctypes.byref(th), tmp.data_ptr(), tmp.numel(), totals_h.data_ptr(), what="densify_classify")
+    torch.cuda.current_stream(dev).synchronize()                    # the one read-back
+    tot = [int(v) for v in totals_h.tolist()]
+    keep_a, keep_b, keep_c, n_split, n_clone, normal_sel, light = tot[:7]
+    P1 = P + n_clone
+    # clones enter the split test with a padded gradient of 0, and clones and split copies carry weights_accum = 1
+    zero_f, one_f, thn, wt = np.float32(0), np.float32(1), np.float32(max_grad_normal), np.float32(weights_threshold)
+    print("densify_and_split_normal:", normal_sel + (n_clone if zero_f >= thn else 0), "/", P1)
+    print("weights_accum:", light + (n_clone + 2 * n_split if one_f < wt else 0), "/", P1 + n_split)
+    z = _sampler((2 * n_split, 3), dev)
+    if z.shape != (2 * n_split, 3):
+        raise ValueError(f"densify_and_prune: sampler returned shape {tuple(z.shape)}, expected {(2 * n_split, 3)}")
+    z = _check(z, "normal samples")
+    Pn = keep_a + keep_b + 2 * keep_c
+    descs, hold, new = [], [], []
+    for g, name, p, st in groups:
+        kind = {"xyz": "xyz", "scaling": "scaling"}.get(name, "copy")
+        row_bytes = p[0].numel() * 4 if P > 0 else 4 * max(1, int(np.prod(p.shape[1:])))
+        np_ = torch.empty((Pn,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
+        work = [(p, np_, kind)]
+        moms = None
+        if st is not None:
+            moms = (torch.empty_like(np_), torch.empty_like(np_))
+            work += [(st["exp_avg"], moms[0], "moment"), (st["exp_avg_sq"], moms[1], "moment")]
+        for src, dst, k in work:
             d = _lib.DensifyTensor()
-            d.src, d.dst, d.row_bytes, d.kind = None, t.data_ptr(), 4, KIND["zero"]
+            d.src, d.dst, d.row_bytes, d.kind = src.data_ptr(), dst.data_ptr(), row_bytes, KIND[k]
             descs.append(d)
-        arr = (_lib.DensifyTensor * len(descs))(*descs)
-        tot_c = (ctypes.c_int * 7)(*tot[:7])
-        _lib.check(lib.r3dg_densify_apply(P, tot_c, len(descs), arr, byname["rotation"].data_ptr(), byname["scaling"].data_ptr(),
-                                          z.data_ptr(), split_recip, tmp.data_ptr(), tmp.numel(), stream.cuda_stream),
-                   "densify_apply")
+        new.append((g, name, p, st, np_, moms))
+    stats = {n: torch.empty((Pn, 1), dtype=torch.float32, device=dev) for n in STATS}
+    stats["max_radii2D"] = torch.empty((Pn,), dtype=torch.float32, device=dev)
+    for t in stats.values():
+        d = _lib.DensifyTensor()
+        d.src, d.dst, d.row_bytes, d.kind = None, t.data_ptr(), 4, KIND["zero"]
+        descs.append(d)
+    arr = (_lib.DensifyTensor * len(descs))(*descs)
+    tot_c = (ctypes.c_int * 7)(*tot[:7])
+    _lib.call("r3dg_densify_apply", dev, P, tot_c, len(descs), arr, byname["rotation"].data_ptr(), byname["scaling"].data_ptr(),
+              z.data_ptr(), split_recip, tmp.data_ptr(), tmp.numel(), what="densify_apply")
     opt = model.optimizer
     for g, name, p, st, np_, moms in new:
         newp = torch.nn.Parameter(np_.requires_grad_(True))

@@ -11,10 +11,13 @@ logic is tested without a GPU); on the GPU box it is backed by NCCL over NVLink 
 kernels write directly into its views (`_C_raster.rasterize_gaussians_backward(_out=...)`), so
 no packing copy precedes the collective.
 """
+import ctypes
 from collections import OrderedDict
 
 import torch
 import torch.distributed as dist
+
+from . import _lib
 
 # per-Gaussian parameter gradients that are summed across views (means2D / colors / cov3D are
 # per-view by-products: means2D feeds per-view densification statistics, SURVEY.md §8e)
@@ -96,17 +99,12 @@ class FactoredGradExchange:
 
     def rebuild_sh(self, means3D, campos_all, degree):
         """dL_dsh = (1/world) * sum_v basis(dir(means3D, campos_all[v])) x gathered[v]  (CUDA kernel)."""
-        from . import _lib
-        lib = _lib.load()
         assert campos_all.shape == (self.world, 3) and campos_all.is_contiguous() and campos_all.dtype == torch.float32
         assert means3D.is_contiguous() and means3D.dtype == torch.float32 and means3D.shape == (self.P, 3)
         if not means3D.is_cuda:
             raise RuntimeError("FactoredGradExchange.rebuild_sh runs on the GPU only (no CPU path)")
-        dev = means3D.device
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_sh_grad_from_factors(self.P, int(degree), self.M, self.world, means3D.data_ptr(), campos_all.data_ptr(),
-                                                     self.gathered.data_ptr(), 1.0 / self.world, self.sh.data_ptr(),
-                                                     torch.cuda.current_stream(dev).cuda_stream), "sh_grad_from_factors")
+        _lib.call("r3dg_sh_grad_from_factors", means3D.device, self.P, int(degree), self.M, self.world, means3D.data_ptr(),
+                  campos_all.data_ptr(), self.gathered.data_ptr(), 1.0 / self.world, self.sh.data_ptr(), what="sh_grad_from_factors")
         return self.sh
 
     def exchange(self, means3D, campos_all, degree, group=None):
@@ -158,23 +156,15 @@ class P2PGradExchange:
         return (self.n_dense + self.P * 3) * 4
 
     def exchange(self, means3D, campos_all, degree, dense=True):
-        from . import _lib
-        import ctypes
-        lib = _lib.load()
         assert campos_all.shape == (self.world, 3) and campos_all.is_contiguous() and campos_all.dtype == torch.float32
         assert means3D.is_contiguous() and means3D.dtype == torch.float32 and means3D.shape == (self.P, 3)
-        dev = means3D.device
-        a = _lib.ExchangeArgs()
-        a.P, a.D, a.M, a.world, a.rank = self.P, int(degree), self.M, self.world, self.rank
+        a = _exchange_args(self.world, self.rank, self.peer_ptrs, self.n_dense if dense else 0, self.multicast)
+        a.P, a.D, a.M = self.P, int(degree), self.M
         a.means3D, a.campos, a.dL_dsh = means3D.data_ptr(), campos_all.data_ptr(), self.sh.data_ptr()
         for v in range(self.world):
             a.factors[v] = self.peer_ptrs[v] + 4 * self.factor_off
-            a.dense[v] = self.peer_ptrs[v]
-        a.n_dense = self.n_dense if dense else 0
-        a.dense_multicast = self.multicast if self.multicast else None
         self.hdl.barrier(channel=0)                    # every rank's backward has written its factors / dense rows
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_exchange_p2p(ctypes.byref(a), torch.cuda.current_stream(dev).cuda_stream), "exchange_p2p")
+        _lib.call("r3dg_exchange_p2p", means3D.device, ctypes.byref(a), what="exchange_p2p")
         self.hdl.barrier(channel=1)                    # every rank is done reading / writing everyone's buffers
         return self.sh
 
@@ -186,21 +176,24 @@ class P2PGradExchange:
         return self.exchange(means3D, campos_all, degree, dense=False)
 
 
+def _exchange_args(world, rank, peer_ptrs, n_dense, multicast):
+    """ExchangeArgs of the dense job: the first n_dense floats of every rank's symmetric buffer (peer_ptrs[v]) are
+    replaced by their mean over the ranks, through the multicast address when there is one (0: none)."""
+    a = _lib.ExchangeArgs()
+    a.world, a.rank, a.n_dense = world, rank, n_dense
+    for v in range(world):
+        a.dense[v] = peer_ptrs[v]
+    a.dense_multicast = multicast if multicast else None
+    return a
+
+
 def _nvls_mean_inplace(flat, hdl, world, rank, multicast, peer_ptrs):
     """In-place mean over the ranks of a symmetric flat fp32 buffer: barrier, one r3dg_exchange_p2p launch (dense job
     only), barrier."""
-    from . import _lib
-    import ctypes
-    a = _lib.ExchangeArgs()
-    a.P, a.D, a.M, a.world, a.rank = 0, 0, 1, world, rank
-    n = flat.numel() // 4 * 4
-    for v in range(world):
-        a.dense[v] = peer_ptrs[v]
-    a.n_dense = n
-    a.dense_multicast = multicast if multicast else None
+    a = _exchange_args(world, rank, peer_ptrs, flat.numel() // 4 * 4, multicast)
+    a.M = 1
     hdl.barrier(channel=0)
-    with torch.cuda.device(flat.device):
-        _lib.check(_lib.load().r3dg_exchange_p2p(ctypes.byref(a), torch.cuda.current_stream(flat.device).cuda_stream), "nvls mean")
+    _lib.call("r3dg_exchange_p2p", flat.device, ctypes.byref(a), what="nvls mean")
     hdl.barrier(channel=1)
 
 

@@ -28,23 +28,24 @@ DEFAULT_MODULES = ("utils.loss_utils", "gaussian_renderer.render", "gaussian_ren
 _saved = []            # (module, name, previous value) of every rebinding made by install()
 
 
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
+def _check_cuda_f32(fn, name, t):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise ValueError(f"{fn}: {name} must be a CUDA tensor")
+    if t.dtype != torch.float32:
+        raise TypeError(f"{fn}: {name} must be float32 (got {t.dtype})")
 
 
 class _SSIM(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img1, img2, size_average):
-        lib = _lib.load()
-        x, y = img1.detach().contiguous(), img2.detach().contiguous()
+        x, y = _lib.f32(img1), _lib.f32(img2)
         N = 1 if x.dim() == 3 else x.shape[0]
         C, H, W = x.shape[-3:]
         dev = x.device
         out = torch.empty(() if size_average else (N,), dtype=torch.float32, device=dev)
-        tmp = torch.empty(max(lib.r3dg_ssim_tmp_bytes(N, C, H, W), 1), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_ssim_forward(N, C, H, W, x.data_ptr(), y.data_ptr(), int(size_average), out.data_ptr(),
-                                             tmp.data_ptr(), tmp.numel(), _stream(dev)), "ssim")
+        tmp = _lib.scratch(max(_lib.load().r3dg_ssim_tmp_bytes(N, C, H, W), 1), dev)
+        _lib.call("r3dg_ssim_forward", dev, N, C, H, W, x.data_ptr(), y.data_ptr(), int(size_average), out.data_ptr(),
+                  tmp.data_ptr(), tmp.numel(), what="ssim")
         ctx.save_for_backward(x, y)
         ctx.size_average = size_average
         return out
@@ -52,20 +53,17 @@ class _SSIM(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        lib = _lib.load()
         x, y = ctx.saved_tensors
         N = 1 if x.dim() == 3 else x.shape[0]
         C, H, W = x.shape[-3:]
-        dev = x.device
-        g = g.float().contiguous()
+        g = _lib.f32(g)
         grads = []
         for need, a, b in ((ctx.needs_input_grad[0], x, y), (ctx.needs_input_grad[1], y, x)):   # dL/dimg2: img1 <-> img2
             d = None
             if need:
                 d = torch.empty_like(a)
-                with torch.cuda.device(dev):
-                    _lib.check(lib.r3dg_ssim_backward(N, C, H, W, a.data_ptr(), b.data_ptr(), int(ctx.size_average),
-                                                      g.data_ptr(), d.data_ptr(), _stream(dev)), "ssim backward")
+                _lib.call("r3dg_ssim_backward", x.device, N, C, H, W, a.data_ptr(), b.data_ptr(), int(ctx.size_average),
+                          g.data_ptr(), d.data_ptr(), what="ssim backward")
             grads.append(d)
         return grads[0], grads[1], None
 
@@ -76,10 +74,7 @@ def ssim(img1, img2, window_size=11, size_average=True):
     if window_size != 11:
         raise ValueError(f"ssim: only window_size=11 is supported (got {window_size})")
     for name, t in (("img1", img1), ("img2", img2)):
-        if not isinstance(t, torch.Tensor) or not t.is_cuda:
-            raise ValueError(f"ssim: {name} must be a CUDA tensor")
-        if t.dtype != torch.float32:
-            raise TypeError(f"ssim: {name} must be float32 (got {t.dtype})")
+        _check_cuda_f32("ssim", name, t)
         if t.dim() not in (3, 4):
             raise ValueError(f"ssim: {name} must be [C,H,W] or [N,C,H,W] (got {tuple(t.shape)})")
     if img1.shape != img2.shape:
@@ -92,43 +87,29 @@ def ssim(img1, img2, window_size=11, size_average=True):
     return _SSIM.apply(img1, img2, bool(size_average))
 
 
-def _check_cuda_f32(fn, name, t):
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise ValueError(f"{fn}: {name} must be a CUDA tensor")
-    if t.dtype != torch.float32:
-        raise TypeError(f"{fn}: {name} must be float32 (got {t.dtype})")
-
-
 class _EdgeAware(torch.autograd.Function):
     @staticmethod
     def forward(ctx, data, img):
-        lib = _lib.load()
-        d, i = data.detach().contiguous(), img.detach().contiguous()
+        d, i = _lib.f32(data), _lib.f32(img)
         (Cd, H, W), Ci = d.shape, i.shape[0]
         dev = d.device
         out = torch.empty((), dtype=torch.float32, device=dev)
-        tmp = torch.empty(max(lib.r3dg_edge_aware_tmp_bytes(Cd, Ci, H, W), 1), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_edge_aware_forward(Cd, Ci, H, W, d.data_ptr(), i.data_ptr(), out.data_ptr(),
-                                                   tmp.data_ptr(), tmp.numel(), _stream(dev)), "first_order_edge_aware_loss")
+        tmp = _lib.scratch(max(_lib.load().r3dg_edge_aware_tmp_bytes(Cd, Ci, H, W), 1), dev)
+        _lib.call("r3dg_edge_aware_forward", dev, Cd, Ci, H, W, d.data_ptr(), i.data_ptr(), out.data_ptr(),
+                  tmp.data_ptr(), tmp.numel(), what="first_order_edge_aware_loss")
         ctx.save_for_backward(d, i)
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        lib = _lib.load()
         d, i = ctx.saved_tensors
         (Cd, H, W), Ci = d.shape, i.shape[0]
-        dev = d.device
-        g = g.float().contiguous()
+        g = _lib.f32(g)
         dd = torch.empty_like(d) if ctx.needs_input_grad[0] else None
         di = torch.empty_like(i) if ctx.needs_input_grad[1] else None
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_edge_aware_backward(Cd, Ci, H, W, d.data_ptr(), i.data_ptr(), g.data_ptr(),
-                                                    dd.data_ptr() if dd is not None else None,
-                                                    di.data_ptr() if di is not None else None, _stream(dev)),
-                       "first_order_edge_aware_loss backward")
+        _lib.call("r3dg_edge_aware_backward", d.device, Cd, Ci, H, W, d.data_ptr(), i.data_ptr(), g.data_ptr(),
+                  _lib.ptr(dd), _lib.ptr(di), what="first_order_edge_aware_loss backward")
         return dd, di
 
 
@@ -155,32 +136,26 @@ def first_order_edge_aware_loss(data, img):
 class _TV(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x):
-        lib = _lib.load()
-        xc = x.detach().contiguous()
+        xc = _lib.f32(x)
         H, W = xc.shape[-2:]
         B = xc.numel() // (H * W)
         dev = xc.device
         out = torch.empty((), dtype=torch.float32, device=dev)
-        tmp = torch.empty(max(lib.r3dg_tv_tmp_bytes(B, H, W), 1), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_tv_forward(B, H, W, xc.data_ptr(), out.data_ptr(), tmp.data_ptr(), tmp.numel(),
-                                           _stream(dev)), "tv_loss")
+        tmp = _lib.scratch(max(_lib.load().r3dg_tv_tmp_bytes(B, H, W), 1), dev)
+        _lib.call("r3dg_tv_forward", dev, B, H, W, xc.data_ptr(), out.data_ptr(), tmp.data_ptr(), tmp.numel(),
+                  what="tv_loss")
         ctx.save_for_backward(xc)
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        lib = _lib.load()
         (xc,) = ctx.saved_tensors
         H, W = xc.shape[-2:]
         B = xc.numel() // (H * W)
-        dev = xc.device
-        g = g.float().contiguous()
+        g = _lib.f32(g)
         dx = torch.empty_like(xc)
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_tv_backward(B, H, W, xc.data_ptr(), g.data_ptr(), dx.data_ptr(), _stream(dev)),
-                       "tv_loss backward")
+        _lib.call("r3dg_tv_backward", xc.device, B, H, W, xc.data_ptr(), g.data_ptr(), dx.data_ptr(), what="tv_loss backward")
         return dx
 
 

@@ -12,8 +12,6 @@ checkpoints store `optimizer.state_dict()` (:129), so state dicts are interchang
 torch.optim.Adam in both directions.  weight_decay / amsgrad / maximize are not used by the
 reference and are rejected.  There is no CPU path: parameters must be CUDA float32.
 """
-import ctypes
-
 import torch
 
 from . import _lib
@@ -80,9 +78,7 @@ class FusedAdam(torch.optim.Optimizer):
                 entries.append(e)
         if entries:
             arr = (_lib.AdamTensor * len(entries))(*entries)
-            with torch.cuda.device(device):
-                _lib.check(_lib.load().r3dg_adam_step(len(entries), arr, torch.cuda.current_stream(device).cuda_stream),
-                           "FusedAdam.step")
+            _lib.call("r3dg_adam_step", device, len(entries), arr, what="FusedAdam.step")
         return loss
 
 
@@ -119,9 +115,7 @@ def compact_rows(tensors, keep):
     """[t[keep] for t in tensors] for tensors that share dim 0 (fp32 / int32 / any dtype whose row is a
     multiple of 4 bytes; other rows fall back to boolean indexing).  One host read-back of the kept
     count — boolean indexing has the same one."""
-    import ctypes
     global _compact_pinned
-    lib = _lib.load()
     keep = keep.reshape(-1)
     P = keep.shape[0]
     dev = keep.device
@@ -130,32 +124,30 @@ def compact_rows(tensors, keep):
     k8 = keep.to(torch.uint8).contiguous() if keep.dtype != torch.uint8 else keep.contiguous()
     if keep.dtype == torch.bool:
         k8 = keep.contiguous().view(torch.uint8)
-    tmp = torch.empty((lib.r3dg_compact_tmp_bytes(P),), dtype=torch.uint8, device=dev)
+    tmp = _lib.scratch(_lib.load().r3dg_compact_tmp_bytes(P), dev)
     if _compact_pinned is None:
         _compact_pinned = torch.zeros(1, dtype=torch.int32).pin_memory()
-    stream = torch.cuda.current_stream(dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.r3dg_compact_scan(P, k8.data_ptr(), tmp.data_ptr(), tmp.numel(), _compact_pinned.data_ptr(), stream.cuda_stream),
-                   "compact_scan")
-        stream.synchronize()
-        count = int(_compact_pinned.item())
-        outs, descs, hold = [], [], []
-        for t in tensors:
-            assert t.shape[0] == P, "all tensors must share dim 0 with the mask"
-            row_bytes = (t.numel() // max(P, 1)) * t.element_size() if P > 0 else 0
-            if P == 0 or row_bytes % 4 != 0 or not t.is_cuda:
-                outs.append(t[keep.bool()])
-                continue
-            src = t.detach().contiguous()
-            dst = torch.empty((count,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
-            hold.append(src)
-            d = _lib.CompactTensor()
-            d.src, d.dst, d.row_bytes = src.data_ptr(), dst.data_ptr(), row_bytes
-            descs.append(d)
-            outs.append(dst)
-        if descs and count > 0:
-            arr = (_lib.CompactTensor * len(descs))(*descs)
-            _lib.check(lib.r3dg_compact_rows(P, len(descs), arr, k8.data_ptr(), tmp.data_ptr(), stream.cuda_stream), "compact_rows")
+    _lib.call("r3dg_compact_scan", dev, P, k8.data_ptr(), tmp.data_ptr(), tmp.numel(), _compact_pinned.data_ptr(),
+              what="compact_scan")
+    torch.cuda.current_stream(dev).synchronize()
+    count = int(_compact_pinned.item())
+    outs, descs, hold = [], [], []
+    for t in tensors:
+        assert t.shape[0] == P, "all tensors must share dim 0 with the mask"
+        row_bytes = (t.numel() // max(P, 1)) * t.element_size() if P > 0 else 0
+        if P == 0 or row_bytes % 4 != 0 or not t.is_cuda:
+            outs.append(t[keep.bool()])
+            continue
+        src = t.detach().contiguous()
+        dst = torch.empty((count,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+        hold.append(src)
+        d = _lib.CompactTensor()
+        d.src, d.dst, d.row_bytes = src.data_ptr(), dst.data_ptr(), row_bytes
+        descs.append(d)
+        outs.append(dst)
+    if descs and count > 0:
+        arr = (_lib.CompactTensor * len(descs))(*descs)
+        _lib.call("r3dg_compact_rows", dev, P, len(descs), arr, k8.data_ptr(), tmp.data_ptr(), what="compact_rows")
     return outs
 
 

@@ -4,12 +4,14 @@
 tuple and error behaviour, on top of this project's CUDA kernels (through `_C_raster`, our stand-in for
 `r3dg_rasterization._C`).
 """
+import warnings
 from typing import NamedTuple
 
 import torch
 import torch.nn as nn
 
 from . import _C_raster as _C
+from . import _lib
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -155,7 +157,6 @@ class _RasterizeGaussians(torch.autograd.Function):
         if isinstance(ctx.num_rendered, _C.DeferredCount):
             ctx.num_rendered.resolve()          # after the backward kernels are in flight
             if ctx.num_rendered.overflowed:     # rare: re-run the forward with the exact size, differentiate that
-                import warnings
                 warnings.warn(f"deferred rasterization overflowed its binning buffer ({int(ctx.num_rendered)} instances); "
                               "forward re-run inside backward (cotangents come from the truncated first attempt)")
                 out = _C.rasterize_gaussians(rs.bg, means3D, features, colors_precomp, opacities, scales, rotations,
@@ -219,31 +220,24 @@ class GaussianRasterizer(nn.Module):
 class _Unpremultiply(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feature, opacity, num_contrib):
-        from . import _lib
-        lib = _lib.load()
         S, HW = feature.shape[0], feature.shape[1] * feature.shape[2]
-        f, o = feature.detach().float().contiguous(), opacity.detach().float().contiguous()
+        f, o = _lib.f32(feature), _lib.f32(opacity)
         n = num_contrib.detach().to(torch.int32).contiguous()
         out = torch.empty_like(f)
         if S > 0 and HW > 0:
-            with torch.cuda.device(f.device):
-                _lib.check(lib.r3dg_unpremultiply_forward(S, HW, f.data_ptr(), o.data_ptr(), n.data_ptr(), out.data_ptr(),
-                                                          torch.cuda.current_stream(f.device).cuda_stream), "unpremultiply")
+            _lib.call("r3dg_unpremultiply_forward", f.device, S, HW, f.data_ptr(), o.data_ptr(), n.data_ptr(), out.data_ptr(),
+                      what="unpremultiply")
         ctx.save_for_backward(f, o, n)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        from . import _lib
-        lib = _lib.load()
         f, o, n = ctx.saved_tensors
         S, HW = f.shape[0], f.shape[1] * f.shape[2]
-        g = g.float().contiguous()
+        g = _lib.f32(g)
         d_f, d_o = torch.empty_like(f), torch.empty_like(o)
-        with torch.cuda.device(f.device):
-            _lib.check(lib.r3dg_unpremultiply_backward(S, HW, f.data_ptr(), o.data_ptr(), n.data_ptr(), g.data_ptr(), d_f.data_ptr(),
-                                                       d_o.data_ptr(), torch.cuda.current_stream(f.device).cuda_stream),
-                       "unpremultiply backward")
+        _lib.call("r3dg_unpremultiply_backward", f.device, S, HW, f.data_ptr(), o.data_ptr(), n.data_ptr(), g.data_ptr(),
+                  d_f.data_ptr(), d_o.data_ptr(), what="unpremultiply backward")
         return d_f, d_o, None
 
 
@@ -259,37 +253,30 @@ def unpremultiply(rendered_feature, rendered_opacity, num_contrib):
 class _PackFeatures(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, viewmatrix, *tensors):
-        import ctypes
-        from . import _lib
-        lib = _lib.load()
         P = tensors[0].shape[0] if tensors else means3D.shape[0]
         dev = (tensors[0] if tensors else means3D).device
-        srcs = [t.detach().float().contiguous().view(P, -1) for t in tensors]
+        srcs = [_lib.f32(t).view(P, -1) for t in tensors]
         depth = means3D is not None
         S = (2 if depth else 0) + sum(t.shape[1] for t in srcs)
         out = torch.empty((P, S), dtype=torch.float32, device=dev)
-        m = means3D.detach().float().contiguous() if depth else None
-        v = viewmatrix.detach().float().contiguous() if depth else None
+        m = _lib.f32(means3D) if depth else None
+        v = _lib.f32(viewmatrix) if depth else None
         arr = (_lib.PackSrc * max(len(srcs), 1))()
         for k, t in enumerate(srcs):
             arr[k].ptr, arr[k].width = t.data_ptr(), t.shape[1]
         if P > 0:
-            with torch.cuda.device(dev):
-                _lib.check(lib.r3dg_pack_features_forward(P, S, m.data_ptr() if depth else None, v.data_ptr() if depth else None, len(srcs), arr,
-                                                          out.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), "pack_features")
+            _lib.call("r3dg_pack_features_forward", dev, P, S, _lib.ptr(m), _lib.ptr(v), len(srcs), arr, out.data_ptr(),
+                      what="pack_features")
         ctx.meta = (P, S, [tuple(t.shape) for t in tensors], [t.shape[1] for t in srcs], depth)
         ctx.save_for_backward(*([m, v] if depth else []))
         return out
 
     @staticmethod
     def backward(ctx, g):
-        import ctypes
-        from . import _lib
-        lib = _lib.load()
         P, S, shapes, widths, depth = ctx.meta
         m, v = ctx.saved_tensors if depth else (None, None)
         dev = g.device
-        g = g.float().contiguous()
+        g = _lib.f32(g)
         need = ctx.needs_input_grad
         outs = [torch.empty((P, w), dtype=torch.float32, device=dev) if need[2 + k] else None for k, w in enumerate(widths)]
         d_m = torch.empty((P, 3), dtype=torch.float32, device=dev) if depth and need[0] else None
@@ -297,10 +284,8 @@ class _PackFeatures(torch.autograd.Function):
         for k, w in enumerate(widths):
             arr[k].ptr, arr[k].width = (outs[k].data_ptr() if outs[k] is not None else None), w
         if P > 0:
-            with torch.cuda.device(dev):
-                _lib.check(lib.r3dg_pack_features_backward(P, S, m.data_ptr() if depth else None, v.data_ptr() if depth else None, g.data_ptr(),
-                                                           len(widths), arr, d_m.data_ptr() if d_m is not None else None,
-                                                           torch.cuda.current_stream(dev).cuda_stream), "pack_features backward")
+            _lib.call("r3dg_pack_features_backward", dev, P, S, _lib.ptr(m), _lib.ptr(v), g.data_ptr(), len(widths), arr,
+                      _lib.ptr(d_m), what="pack_features backward")
         return (d_m, None) + tuple(o.view(s) if o is not None else None for o, s in zip(outs, shapes))
 
 

@@ -18,17 +18,12 @@ from . import _C_bvh as _C
 from . import _lib
 
 
-def _f32(t):
-    return t.detach().float().contiguous()
-
-
 def fibonacci_sphere_sampling(normals, sample_num, random_rotate=True):
     """utils/graphics_utils.py:9-37: (incident_dirs [...,N,3], incident_areas [...,N,1]).  With
     random_rotate the per-Gaussian phase is drawn here with torch.rand (as the reference does) and
     applied in the kernel."""
-    lib = _lib.load()
     pre_shape = normals.shape[:-1]
-    n = _f32(normals).reshape(-1, 3)
+    n = _lib.f32(normals).reshape(-1, 3)
     P, N = n.shape[0], int(sample_num)
     if not n.is_cuda:
         raise RuntimeError("fibonacci_sphere_sampling runs on the GPU only (no CPU path)")
@@ -36,10 +31,8 @@ def fibonacci_sphere_sampling(normals, sample_num, random_rotate=True):
     areas = torch.empty((P, N, 1), dtype=torch.float32, device=n.device)
     phase = torch.rand(P, device=n.device) if random_rotate else None
     if P > 0 and N > 0:
-        with torch.cuda.device(n.device):
-            _lib.check(lib.r3dg_sample_incident_dirs(P, N, n.data_ptr(), None if phase is None else phase.data_ptr(),
-                                                     dirs.data_ptr(), areas.data_ptr(),
-                                                     torch.cuda.current_stream(n.device).cuda_stream), "sample_incident_dirs")
+        _lib.call("r3dg_sample_incident_dirs", n.device, P, N, n.data_ptr(), _lib.ptr(phase), dirs.data_ptr(),
+                  areas.data_ptr(), what="sample_incident_dirs")
     return dirs.reshape(*pre_shape, N, 3), areas.reshape(*pre_shape, N, 1)
 
 
@@ -66,16 +59,13 @@ class RayTracer:
     """bvh/__init__.py:28-71: builds the LBVH in __init__, `trace_visibility` bakes T in {0} U [0.9,1]."""
 
     def __init__(self, means3D, scales, rotations):
-        lib = _lib.load()
         P = means3D.shape[0]
         dev = means3D.device
         nodes = torch.empty((2 * P - 1, 5), dtype=torch.int32, device=dev)
         aabbs = torch.empty((2 * P - 1, 6), dtype=torch.float32, device=dev)
-        m, s, r = _f32(means3D), _f32(scales), _f32(rotations)
-        stream = torch.cuda.current_stream(dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_bvh_leaf_aabbs(P, m.data_ptr(), s.data_ptr(), r.data_ptr(), nodes.data_ptr(),
-                                               aabbs.data_ptr(), stream.cuda_stream), "RayTracer leaf boxes")
+        m, s, r = _lib.f32(means3D), _lib.f32(scales), _lib.f32(rotations)
+        _lib.call("r3dg_bvh_leaf_aabbs", dev, P, m.data_ptr(), s.data_ptr(), r.data_ptr(), nodes.data_ptr(), aabbs.data_ptr(),
+                  what="RayTracer leaf boxes")
         self.tree, self.aabb, self.morton = _C.create_bvh(m, s, r, nodes, aabbs)
 
     @torch.no_grad()
@@ -95,7 +85,6 @@ class RayTracer:
         launch (r3dg_bvh_bake_visibility).  Returns dict(visibility [P,N,1], incident_dirs [P,N,3],
         incident_areas [P,N,1][, contribute]); rows of Gaussians outside the slot range keep the content of
         `out` (zero-initialised when not given) — that is what the sharded bake sums over the ranks."""
-        lib = _lib.load()
         P, N = means3D.shape[0], int(sample_num)
         dev = means3D.device
         count = P - first_slot if count is None else count
@@ -108,17 +97,13 @@ class RayTracer:
                 out.update(incident_dirs=mk((P, N, 3), **f), incident_areas=mk((P, N, 1), **f))
             if want_contribute:
                 out["contribute"] = mk((P, N, 1), dtype=torch.int32, device=dev)
-        m, ci, op, nr = _f32(means3D), _f32(symm_inv), _f32(opacity), _f32(normals)
-        tmp = torch.empty((lib.r3dg_bvh_trace_tmp_bytes(P),), dtype=torch.uint8, device=dev)
-        contrib = out.get("contribute")
+        m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(normals)
+        tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_tmp_bytes(P), dev)
         if P > 0 and N > 0 and count > 0:
-            with torch.cuda.device(dev):
-                _lib.check(lib.r3dg_bvh_bake_visibility(
-                    P, int(first_slot), int(count), N, self.tree.data_ptr(), self.aabb.data_ptr(), m.data_ptr(), ci.data_ptr(),
-                    op.data_ptr(), nr.data_ptr(), 0.05, None if contrib is None else contrib.data_ptr(),
-                    out["visibility"].data_ptr(), out["incident_dirs"].data_ptr() if "incident_dirs" in out else None,
-                    out["incident_areas"].data_ptr() if "incident_areas" in out else None,
-                    tmp.data_ptr(), tmp.numel(), torch.cuda.current_stream(dev).cuda_stream), "bake_visibility")
+            _lib.call("r3dg_bvh_bake_visibility", dev, P, int(first_slot), int(count), N, self.tree.data_ptr(),
+                      self.aabb.data_ptr(), m.data_ptr(), ci.data_ptr(), op.data_ptr(), nr.data_ptr(), 0.05,
+                      _lib.ptr(out.get("contribute")), out["visibility"].data_ptr(), _lib.ptr(out.get("incident_dirs")),
+                      _lib.ptr(out.get("incident_areas")), tmp.data_ptr(), tmp.numel(), what="bake_visibility")
         return out
 
 

@@ -38,33 +38,34 @@ def _args(P, N, He, We):
     return a
 
 
-def _c(t):
-    return t.detach().float().contiguous()
+def _shade_args(inputs, transform):
+    """ShadeArgs for the nine inputs (base_color, roughness, normals, viewdirs, incidents, env, visibility,
+    incident_dirs, incident_areas) and the optional [3,3] env transform, all as contiguous float32.  Returns the
+    struct and the converted inputs and transform, which must outlive the launch."""
+    ts = [_lib.f32(t) for t in inputs]
+    tr = None if transform is None else _lib.f32(transform)
+    env, dirs = ts[5], ts[7]
+    a = _args(dirs.shape[0], dirs.shape[1], env.shape[0], env.shape[1])
+    (a.base_color, a.roughness, a.normals, a.viewdirs, a.incidents, a.env, a.visibility, a.incident_dirs,
+     a.incident_areas) = [t.data_ptr() for t in ts]
+    a.env_transform = None if tr is None else tr.data_ptr()
+    return a, ts, tr
 
 
 class _RenderEquation(torch.autograd.Function):
     @staticmethod
     def forward(ctx, base_color, roughness, viewdirs, incidents, env, normals, visibility, dirs, areas, transform, want_means):
-        lib = _lib.load()
-        P, N = dirs.shape[0], dirs.shape[1]
-        dev = dirs.device
-        ts = [_c(t) for t in (base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas)]
-        tr = None if transform is None else _c(transform)
-        f = dict(dtype=torch.float32, device=dev)
+        P = dirs.shape[0]
+        f = dict(dtype=torch.float32, device=dirs.device)
+        a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas), transform)
         pbr, diffuse, specular = (torch.empty((P, 3), **f) for _ in range(3))
-        a = _args(P, N, env.shape[0], env.shape[1])
-        (a.base_color, a.roughness, a.normals, a.viewdirs, a.incidents, a.env, a.visibility, a.incident_dirs,
-         a.incident_areas) = [t.data_ptr() for t in ts]
-        a.env_transform = None if tr is None else tr.data_ptr()
         a.pbr, a.diffuse_light, a.specular = pbr.data_ptr(), diffuse.data_ptr(), specular.data_ptr()
         means = None
         if want_means:
             means = [torch.empty((P, 3), **f) for _ in range(3)] + [torch.empty((P, 1), **f)]
             a.mean_incident_lights, a.mean_local_lights, a.mean_global_lights, a.mean_visibility = [m.data_ptr() for m in means]
         if P > 0:
-            with torch.cuda.device(dev):
-                _lib.check(lib.r3dg_render_equation_forward(ctypes.byref(a), torch.cuda.current_stream(dev).cuda_stream),
-                           "rendering_equation")
+            _lib.call("r3dg_render_equation_forward", dirs.device, ctypes.byref(a), what="rendering_equation")
         ctx.save_for_backward(*ts)
         ctx.transform = tr
         ctx.mark_non_differentiable(*(means or []))
@@ -72,30 +73,22 @@ class _RenderEquation(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_pbr, g_diffuse, g_specular, *_):
-        lib = _lib.load()
-        base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas = ctx.saved_tensors
-        P, N = dirs.shape[0], dirs.shape[1]
+        a, ts, _ = _shade_args(ctx.saved_tensors, ctx.transform)
+        env, dirs = ts[5], ts[7]
+        P = dirs.shape[0]
         dev = dirs.device
         f = dict(dtype=torch.float32, device=dev)
         d_base, d_view = torch.empty((P, 3), **f), torch.empty((P, 3), **f)
         d_rough = torch.empty((P, 1), **f)
         d_inc = torch.empty((P, 16, 3), **f)
         d_env = torch.empty(env.shape, **f)
-        a = _args(P, N, env.shape[0], env.shape[1])
-        (a.base_color, a.roughness, a.normals, a.viewdirs, a.incidents, a.env, a.visibility, a.incident_dirs,
-         a.incident_areas) = [t.data_ptr() for t in (base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas)]
-        a.env_transform = None if ctx.transform is None else ctx.transform.data_ptr()
         gz = torch.zeros((P, 3), **f)
-        g = [gz if t is None else _c(t) for t in (g_pbr, g_diffuse, g_specular)]
+        g = [gz if t is None else _lib.f32(t) for t in (g_pbr, g_diffuse, g_specular)]
         a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = [t.data_ptr() for t in g]
         a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = d_base.data_ptr(), d_rough.data_ptr(), d_view.data_ptr()
         a.dL_dincidents, a.dL_denv = d_inc.data_ptr(), d_env.data_ptr()
-        if torch.are_deterministic_algorithms_enabled():
-            ws = torch.empty((lib.r3dg_shade_det_bytes(env.shape[0], env.shape[1]),), dtype=torch.uint8, device=dev)
-            a.deterministic, a.det_work, a.det_work_bytes = 1, ws.data_ptr(), ws.numel()
-        with torch.cuda.device(dev):
-            _lib.check(lib.r3dg_render_equation_backward(ctypes.byref(a), torch.cuda.current_stream(dev).cuda_stream),
-                       "rendering_equation backward")
+        det_ws = _lib.det_workspace(a, _lib.load().r3dg_shade_det_bytes(env.shape[0], env.shape[1]), dev)
+        _lib.call("r3dg_render_equation_backward", dev, ctypes.byref(a), what="rendering_equation backward")
         return d_base, d_rough, d_view, d_inc, d_env, None, None, None, None, None, None
 
 
@@ -144,23 +137,15 @@ def rendering_equation(base_color, roughness, normals, viewdirs, incidents, dire
                                                    areas, transform, False)
 
     def per_sample():
-        lib = _lib.load()
+        a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, vis, dirs, areas), transform)
         P, N = dirs.shape[0], dirs.shape[1]
         f = dict(dtype=torch.float32, device=dirs.device)
         outs = [torch.empty((P, N, 3), **f) for _ in range(3)]
         scratch = [torch.empty((P, 3), **f) for _ in range(3)]
-        ts = [_c(t) for t in (base_color, roughness, normals, viewdirs, incidents, env, vis, dirs, areas)]
-        tr = None if transform is None else _c(transform)
-        a = _args(P, N, env.shape[0], env.shape[1])
-        (a.base_color, a.roughness, a.normals, a.viewdirs, a.incidents, a.env, a.visibility, a.incident_dirs,
-         a.incident_areas) = [t.data_ptr() for t in ts]
-        a.env_transform = None if tr is None else tr.data_ptr()
         a.pbr, a.diffuse_light, a.specular = [t.data_ptr() for t in scratch]
         a.incident_lights, a.local_incident_lights, a.global_incident_lights = [t.data_ptr() for t in outs]
         if P > 0:
-            with torch.cuda.device(dirs.device):
-                _lib.check(lib.r3dg_render_equation_forward(ctypes.byref(a), torch.cuda.current_stream(dirs.device).cuda_stream),
-                           "rendering_equation (per-sample lights)")
+            _lib.call("r3dg_render_equation_forward", dirs.device, ctypes.byref(a), what="rendering_equation (per-sample lights)")
         return dict(zip(_LazyExtras._LAZY, outs))
 
     extra = _LazyExtras({"incident_dirs": dirs, "incident_visibility": vis, "diffuse_light": diffuse, "specular": specular},

@@ -1,5 +1,6 @@
-"""C-ABI surface: the shared library loads and exports every symbol include/r3dg_b200.h declares,
-struct layouts agree with the header, sizing functions are sane.  No GPU compute is issued."""
+"""C-ABI surface: the shared library loads and exports every symbol include/r3dg_b200.h declares, the ctypes
+bindings (struct layouts and function signatures) agree with the header, sizing functions are sane.  No GPU compute
+is issued."""
 import ctypes
 import os
 import re
@@ -10,39 +11,111 @@ from helpers import ROOT
 from relightable3dgaussian_b200 import _lib
 
 
-def _declared_functions():
-    hdr = open(os.path.join(ROOT, "include", "r3dg_b200.h")).read()
-    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
-    names = re.findall(r"\b(r3dg_[a-z0-9_]+)\s*\(", hdr)
-    return sorted(set(n for n in names if not n.endswith("_t")))
+C = ctypes
+# header struct -> its ctypes class
+STRUCTS = {"r3dg_raster_fwd_args": _lib.RasterFwdArgs, "r3dg_raster_bwd_args": _lib.RasterBwdArgs,
+           "r3dg_exchange_args": _lib.ExchangeArgs, "r3dg_pack_src": _lib.PackSrc,
+           "r3dg_compact_tensor": _lib.CompactTensor, "r3dg_densify_tensor": _lib.DensifyTensor,
+           "r3dg_densify_thresholds": _lib.DensifyThresholds, "r3dg_shade_args": _lib.ShadeArgs,
+           "r3dg_adam_tensor": _lib.AdamTensor}
+SCALARS = {"int": C.c_int, "long long": C.c_longlong, "unsigned long long": C.c_ulonglong, "size_t": C.c_size_t,
+           "float": C.c_float, "double": C.c_double, "uint8_t": C.c_uint8, "int32_t": C.c_int32, "uint64_t": C.c_uint64}
+
+
+def _ctype_name(t):
+    if isinstance(t, type) and issubclass(t, C.Array):
+        return f"{_ctype_name(t._type_)}[{t._length_}]"
+    if isinstance(t, type) and issubclass(t, C._Pointer):
+        return f"POINTER({_ctype_name(t._type_)})"
+    return getattr(t, "__name__", repr(t))
+
+
+def _type(decl):
+    """C type of a declaration without its name, normalised: no `const`, single spaces, `*` attached."""
+    t = " ".join(decl.replace("const ", " ").replace("*", " * ").split())
+    return t.replace(" *", "*")
+
+
+def parse_header():
+    """({struct: [(field, C type, array length or None)]}, {function: (return type, [parameter types])}) of
+    include/r3dg_b200.h, comments stripped."""
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "r3dg_b200.h")).read(), flags=re.S)
+    structs = {}
+    for name, body, alias in re.findall(r"typedef struct (\w+) \{(.*?)\} (\w+);", src, re.S):
+        assert name == alias, name
+        fields = []
+        for decl in filter(None, (d.strip() for d in body.split(";"))):
+            base, names = re.fullmatch(r"((?:const\s+)?(?:unsigned\s+)?(?:long\s+long|\w+))\s*(.*)", decl, re.S).groups()
+            for n in names.split(","):
+                stars, field, length = re.fullmatch(r"\s*(\**)\s*(\w+)\s*(?:\[(\d+)\])?\s*", n).groups()
+                fields.append((field, _type(base + stars), int(length) if length else None))
+        structs[name] = fields
+    src = re.sub(r"^[ \t]*#.*$", ";", re.sub(r"typedef struct \w+ \{.*?\} \w+;", ";", src, flags=re.S), flags=re.M)
+    protos = {}
+    for ret, name, params in re.findall(r"([A-Za-z_][\w\s*]*?)\b(r3dg_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", src):
+        params = [p.strip() for p in params.split(",")]
+        protos[name] = (_type(ret), [] if params == ["void"] else [_type(re.fullmatch(r"(.*?)\w+", p, re.S).group(1))
+                                                                   for p in params])
+    return structs, protos
+
+
+def _expected_field(ctype, length):
+    t = C.c_void_p if ctype.endswith("*") else SCALARS[ctype]
+    return t * length if length else t
+
+
+def _param_ok(ctype, bound):
+    """Scalars exactly; a header struct by POINTER(its class); `const char*` as c_char_p; any other pointer and the
+    stream as c_void_p or POINTER of the matching scalar."""
+    if ctype in SCALARS:
+        return bound is SCALARS[ctype]
+    if ctype.endswith("*") and ctype[:-1] in STRUCTS:
+        return bound is C.POINTER(STRUCTS[ctype[:-1]])
+    if ctype == "char*":
+        return bound is C.c_char_p
+    if ctype.endswith("*") and ctype[:-1] in SCALARS and bound is C.POINTER(SCALARS[ctype[:-1]]):
+        return True
+    return bound is C.c_void_p and (ctype.endswith("*") or ctype == "r3dg_stream_t")
 
 
 def test_library_exports_every_declared_symbol():
     lib = _lib.load()
-    declared = _declared_functions()
-    assert len(declared) >= 10
+    _, protos = parse_header()
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "r3dg_b200.h")).read(), flags=re.S)
+    assert set(protos) == {n for n in re.findall(r"\b(r3dg_[a-z0-9_]+)\s*\(", hdr) if not n.endswith("_t")}
+    assert len(protos) >= 10
     bound = {n for n, _, _ in _lib.SYMBOLS}
-    for name in declared:
+    for name in sorted(protos):
         assert hasattr(lib, name), f"{name} declared in include/r3dg_b200.h but not exported"
         assert name in bound, f"{name} is exported but not bound in _lib.SYMBOLS"
     assert b"sm_90a" in lib.r3dg_version()
 
 
 def test_struct_field_order_matches_header():
-    hdr = open(os.path.join(ROOT, "include", "r3dg_b200.h")).read()
-    for cname, cls in (("r3dg_raster_fwd_args", _lib.RasterFwdArgs), ("r3dg_raster_bwd_args", _lib.RasterBwdArgs),
-                       ("r3dg_shade_args", _lib.ShadeArgs), ("r3dg_adam_tensor", _lib.AdamTensor)):
-        body = re.search(r"typedef struct " + cname + r" \{(.*?)\} " + cname + ";", hdr, re.S).group(1)
-        body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-        fields = []
-        for decl in body.split(";"):
-            decl = decl.strip()
-            if not decl:
-                continue
-            names = re.sub(r"^(const\s+)?(float|int|void|size_t|long long|double)\s*\**", "", decl)
-            for n in names.split(","):
-                fields.append(n.replace("*", "").strip())
-        assert fields == [f[0] for f in cls._fields_], cname
+    """Every struct of the header has a ctypes class whose fields match it in order, name, type and array length."""
+    structs, _ = parse_header()
+    assert sorted(structs) == sorted(STRUCTS)
+    for cname, fields in structs.items():
+        cls = STRUCTS[cname]
+        assert [f[0] for f in cls._fields_] == [f[0] for f in fields], cname
+        for (field, ctype, length), (_, bound) in zip(fields, cls._fields_):
+            want = _expected_field(ctype, length)
+            assert bound is want, f"{cname}.{field}: header {ctype}{f'[{length}]' if length else ''}, bound as " \
+                                  f"{_ctype_name(bound)} (expected {_ctype_name(want)})"
+    for cls in (_lib.RasterFwdArgs, _lib.RasterBwdArgs, _lib.ShadeArgs):
+        assert [f[0] for f in cls._fields_[-3:]] == ["deterministic", "det_work", "det_work_bytes"]
+
+
+def test_symbols_match_prototypes():
+    """Every _lib.SYMBOLS binding has its prototype's return type and the number and types of its parameters."""
+    _, protos = parse_header()
+    for name, restype, argtypes in _lib.SYMBOLS:
+        assert name in protos, f"{name} is bound but not declared in include/r3dg_b200.h"
+        ret, params = protos[name]
+        assert _param_ok(ret, restype), f"{name} returns {ret}, bound as {_ctype_name(restype)}"
+        assert len(argtypes) == len(params), f"{name} takes {len(params)} arguments ({params}), bound with {len(argtypes)}"
+        for k, (ctype, bound) in enumerate(zip(params, argtypes)):
+            assert _param_ok(ctype, bound), f"{name} argument {k}: header {ctype}, bound as {_ctype_name(bound)}"
 
 
 def test_sizing_functions_monotone_and_aligned():

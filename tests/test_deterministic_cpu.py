@@ -151,7 +151,6 @@ def test_zero_filled_structs_mean_the_default_mode():
     for cls in (_lib.RasterFwdArgs, _lib.RasterBwdArgs, _lib.ShadeArgs):
         a = cls()
         assert a.deterministic == 0 and not a.det_work and a.det_work_bytes == 0
-        assert [f[0] for f in cls._fields_[-3:]] == ["deterministic", "det_work", "det_work_bytes"]
 
 
 FAKE = 0x10000      # never dereferenced: every call below is refused before anything is launched

@@ -90,6 +90,7 @@ def shade_kernels(P, N):
     kernel variant (r3dg_tune): lanes per Gaussian x env-gradient mode."""
     import ctypes
     from relightable3dgaussian_b200 import _lib
+    from relightable3dgaussian_b200.shading import _shade_args
     lib = _lib.load()
     c = {k: v.cuda() for k, v in shading_case(P, N, 16, seed=2).items()}
     env = F.softplus(c["env_raw"])[0].contiguous()
@@ -97,11 +98,8 @@ def shade_kernels(P, N):
     outs = [torch.empty((P, 3), **f) for _ in range(3)]
     grads = dict(d_base=torch.empty((P, 3), **f), d_rough=torch.empty((P, 1), **f), d_view=torch.empty((P, 3), **f),
                  d_inc=torch.empty((P, 16, 3), **f), d_env=torch.empty(env.shape, **f))
-    a = _lib.ShadeArgs()
-    a.P, a.N, a.sh_coeffs, a.env_h, a.env_w = P, N, 16, env.shape[0], env.shape[1]
-    (a.base_color, a.roughness, a.normals, a.viewdirs, a.incidents, a.env, a.visibility, a.incident_dirs, a.incident_areas) = [
-        c[k].contiguous().data_ptr() for k in ("base_color", "roughness", "normals", "viewdirs", "incidents")] + [env.data_ptr()] + [
-        c[k].contiguous().data_ptr() for k in ("visibility", "incident_dirs", "incident_areas")]
+    a, _, _ = _shade_args([c[k] for k in ("base_color", "roughness", "normals", "viewdirs", "incidents")] + [env] +
+                          [c[k] for k in ("visibility", "incident_dirs", "incident_areas")], None)
     a.pbr, a.diffuse_light, a.specular = [t.data_ptr() for t in outs]
     a.dL_dpbr, a.dL_ddiffuse_light = c["cot_pbr"].data_ptr(), c["cot_diffuse"].data_ptr()
     a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = grads["d_base"].data_ptr(), grads["d_rough"].data_ptr(), grads["d_view"].data_ptr()
