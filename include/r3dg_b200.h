@@ -545,10 +545,7 @@ int r3dg_prof_end(float* stage_ms /* [9] */, int* fwd_calls, int* bwd_calls);
  *                     (an experiment; the register prefetch is the default), 0 (default)
  *   "composite_fwd_ctas" / "composite_bwd_ctas"  resident CTAs per SM of the two compositors,
  *                     enforced with dynamic shared memory; 0 (default) = whatever fits
- *                     (lower settings trade occupancy for faster heaviest warps)
- * Initial values can also be given by the environment (R3DG_SHADE_GROUP, R3DG_SHADE_ENV_MODE,
- * R3DG_SHADE_FWD_VARIANT, R3DG_SHADE_BWD_VARIANT, R3DG_COMPOSITE_BULK, R3DG_FWD_CTAS,
- * R3DG_BWD_CTAS). */
+ *                     (lower settings trade occupancy for faster heaviest warps) */
 int r3dg_tune(const char* key, int value, int* previous);
 
 /* Library identification: returns a static string such as "r3dg_b200 0.1 sm_90a". */

@@ -10,7 +10,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# R3DG_LIB_PATH: developer knob to A/B kernel builds (tools/variant_sweep.sh); unset = the in-tree library
+# R3DG_LIB_PATH: developer knob to load another build of the library (e.g. to A/B two builds); unset = the in-tree library
 LIB_PATH = os.environ.get("R3DG_LIB_PATH") or os.path.join(_HERE, "libr3dg_b200.so")
 
 c_void_p, c_int, c_float, c_size_t, c_ll = (ctypes.c_void_p, ctypes.c_int, ctypes.c_float,

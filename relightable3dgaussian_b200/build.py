@@ -12,7 +12,7 @@ LIB = os.path.join(HERE, "libr3dg_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC] + os.environ.get("R3DG_NVCC_DEFS", "").split()
+         "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 
 # shading.cu mirrors a chain of separate PyTorch elementwise kernels (each op rounded on its own);
@@ -22,8 +22,6 @@ FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
 # denormal); IEEE sqrt / division take a slow subroutine for denormal operands, and one such lane stalls its warp.
 # With -ftz the results are unchanged for every normal number (torch's own CUDA kernels are compiled the same way).
 PER_FILE_FLAGS = {"shading.cu": ["-fmad=false"], "adam.cu": ["-ftz=true"]}
-if os.environ.get("R3DG_SHADING_FMAD") == "1":      # experiment knob (tools/): let nvcc contract mul+add in shading.cu
-    PER_FILE_FLAGS["shading.cu"] = []
 
 
 def sources():

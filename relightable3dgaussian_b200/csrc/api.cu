@@ -10,17 +10,18 @@
 
 using namespace r3dg;
 
-namespace {
-int g_num_sms[64] = {0};            // per device (the caller may drive several GPUs from one process)
-int num_sms() {
+int r3dg::num_sms() {
+    static int per_device[kMaxDevices] = {0};      // the caller may drive several GPUs from one process
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;   // H100 SXM
-    if (g_num_sms[dev] == 0) {
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return 132;   // H100 SXM
+    if (per_device[dev] == 0) {
         int n = 0;
-        g_num_sms[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
+        per_device[dev] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;
     }
-    return g_num_sms[dev];
+    return per_device[dev];
 }
+
+namespace {
 // ---- optional stage profiler: CUDA events recorded on the launching stream between stages ----
 enum { ST_PROJECT = 0, ST_DEPTH_SORT, ST_BIN_COUNT, ST_BIN_OFFSETS, ST_BIN_SCATTER, ST_COMPOSITE, ST_NORMAL, ST_COMPOSITE_BWD,
        ST_PROJECT_BWD, ST_COUNT };

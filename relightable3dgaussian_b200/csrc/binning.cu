@@ -483,15 +483,8 @@ int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* 
     mark(2, stream);
     const size_t smem_count = (size_t)T * 4;
     const size_t smem_scatter = tbl_bytes + (size_t)cap * 4;
-    static size_t attr_smem[2] = {0, 0};
-    if (smem_count > attr_smem[0]) {
-        R3DG_CUDA_TRY(cudaFuncSetAttribute(bin_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_count));
-        attr_smem[0] = smem_count;
-    }
-    if (smem_scatter > attr_smem[1]) {
-        R3DG_CUDA_TRY(cudaFuncSetAttribute(bin_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_scatter));
-        attr_smem[1] = smem_scatter;
-    }
+    R3DG_CUDA_TRY(allow_dyn_smem<bin_count_kernel>(smem_count));
+    R3DG_CUDA_TRY(allow_dyn_smem<bin_scatter_kernel>(smem_scatter));
     const uint32_t* va = (const uint32_t*)(sbuf + sl.vals_a);
     const uint32_t* vb = (const uint32_t*)(sbuf + sl.vals_b);
     const uint2* rects = (const uint2*)(geom + gl.rects);

@@ -78,17 +78,6 @@ __device__ __forceinline__ void sort_plan(uint32_t diff, int& passes, int& w) {
     w = passes ? (nb + passes - 1) / passes : 0;
 }
 
-// Tuning knob (tools/pad_sweep.py): extra bytes in front of the gradient rows, read from the
-// environment on the host.  Used to probe address-mapping effects between rec[] and grad[].
-inline __host__ size_t geom_grad_pad() {
-#ifndef __CUDA_ARCH__
-    const char* e = getenv("R3DG_PAD_GRAD");
-    return e ? align_up((size_t)atoll(e), 256) : 0;
-#else
-    return 0;
-#endif
-}
-
 struct GeomLayout {
     size_t header, rec, tiles_touched, rects, brects, clamped, scan_state, sort, grad, total;
     int P, S, recf;
@@ -103,7 +92,6 @@ struct GeomLayout {
         clamped = off;       off = align_up(off + (size_t)P_, 256);
         scan_state = off;    off = align_up(off + ((size_t)P_ / R3DG_SCAN_ITEMS + 2) * 4, 256);
         sort = off;          off = align_up(off + SortLayout(P_).total, 256);   // depth sort of the Gaussians
-        off += geom_grad_pad();
         grad = off;          off = align_up(off + (size_t)P_ * recf * 4, 256);   // backward scratch
         total = off;
     }
@@ -171,17 +159,6 @@ struct BinLayout {
 inline __host__ long long bin_capacity_for_bytes(size_t bytes) { return bytes < 768 + 384 ? 0 : (long long)((bytes - 768) / 6 / 64 * 64); }
 inline __host__ size_t bin_bytes_for_capacity(long long cap) { return (size_t)((cap + 63) / 64 * 64) * 6 + 768; }
 
-// getHigherMsb (reference rasterizer_impl.cu:35-50): bits needed for tile ids.
-inline __host__ uint32_t higher_msb(uint32_t n) {
-    uint32_t msb = sizeof(n) * 4, step = msb;
-    while (step > 1) {
-        step /= 2;
-        if (n >> msb) msb += step; else msb -= step;
-    }
-    if (n >> msb) msb++;
-    return msb;
-}
-
 // Relaxed GPU-scope accesses for the look-back descriptors (flag and value share one word, so no
 // further ordering is needed); `volatile` asm so that polling loops really re-load.
 // ---- asynchronous global -> shared copies (LDGSTS): no register staging, overlap with math -----
@@ -191,15 +168,6 @@ __device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) 
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
-
-#ifdef R3DG_WARP_TIMING
-// Diagnostic build only (tools/warp_timing.py): every compositor warp records its start / end time, the entries it
-// composited and its SM, to study the load balance of the tile-ordered launch.
-struct WarpTiming { unsigned long long t0, t1; unsigned iters, smid; };
-constexpr int R3DG_WT_MAX = 1 << 17;
-__device__ __forceinline__ unsigned long long wt_now() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-__device__ __forceinline__ unsigned wt_smid() { unsigned v; asm volatile("mov.u32 %0, %%smid;" : "=r"(v)); return v; }
-#endif
 
 // ---- TMA-unit bulk copies (cp.async.bulk, SASS UBLKCP) completing on an mbarrier (SYNCS) -------------------
 // One instruction moves a contiguous, 16-byte aligned slab global -> shared with no register staging and no
@@ -372,41 +340,6 @@ __device__ __forceinline__ uint32_t block_mask_of_rect(uint2 br, uint32_t c0, ui
     uint32_t spread = (rows | (rows << 2)) & 0x33u;
     spread = (spread | (spread << 1)) & 0x55u;
     return spread * cols;
-}
-
-// The same test for all 8 blocks of a tile at once (block b: x offset 8 * (b & 1), y offset 4 * (b >> 1)), with
-// the per-Gaussian part (validity, tau, the two edge slopes) evaluated once.  Bit b of the result == touch_block()
-// of block b: identical arithmetic per block, so the compositors stay exactly as conservative as before.
-__device__ __forceinline__ uint32_t touch_mask8(const float4 A, const float4 B, float TX0, float TY0) {
-    const float gx = A.x, gy = A.y, ca = A.z, cb = A.w, cc = B.x, op = B.y;
-    if (op < 1.0f / 255.0f) return 0u;
-    if (!(ca > 0.0f && cc > 0.0f && ca * cc - cb * cb > 0.0f)) return 0xffu;
-    const float tau = 2.0f * __logf(255.0f * op);
-    if (!(tau >= 0.0f)) return 0xffu;
-    const float rc = __fdividef(-cb, cc), ra = __fdividef(-cb, ca);
-    uint32_t m = 0u;
-#pragma unroll
-    for (int b = 0; b < 8; ++b) {
-        const float X0 = TX0 + 8.0f * (float)(b & 1), Y0 = TY0 + 4.0f * (float)(b >> 1);
-        const float u0 = gx - (X0 + 7.0f), u1 = gx - X0, v0 = gy - (Y0 + 3.0f), v1 = gy - Y0;
-        bool touch = (u0 <= 0.0f && u1 >= 0.0f && v0 <= 0.0f && v1 >= 0.0f);
-        if (!touch) {
-            auto edge_u = [&](float U) {
-                const float v = fminf(fmaxf(rc * U, v0), v1);
-                return ca * U * U + 2.0f * cb * U * v + cc * v * v;
-            };
-            auto edge_v = [&](float V) {
-                const float u = fminf(fmaxf(ra * V, u0), u1);
-                return ca * u * u + 2.0f * cb * u * V + cc * V * V;
-            };
-            const float qmin = fminf(fminf(edge_u(u0), edge_u(u1)), fminf(edge_v(v0), edge_v(v1)));
-            const float um = fmaxf(fabsf(u0), fabsf(u1)), vm = fmaxf(fabsf(v0), fabsf(v1));
-            const float slack = 1.0f + 1e-5f * (ca * um * um + cc * vm * vm + 2.0f * fabsf(cb) * um * vm);
-            touch = !(qmin > tau + slack);
-        }
-        m |= (touch ? 1u : 0u) << b;
-    }
-    return m;
 }
 
 // ---- warp-level stream compaction over per-instance mask bytes (compositors) ---------------------

@@ -11,7 +11,7 @@
 //    queued entries (id -> packed record prefetched one batch ahead, staged in a warp-private
 //    shared-memory slab, exact ellipse / block test once per entry by the lane that staged it);
 //  * the kernel is bound by per-warp latency and by its heaviest warps, not by issue slots
-//    (tools/warp_timing.py): entries are composited in rounds of U whose alpha evaluations
+//    (DESIGN.md §4.2): entries are composited in rounds of U whose alpha evaluations
 //    are in flight together, the sequential part is branch-free (predicated FMAs);
 //  * accumulators live in registers (template on the number of float4 channel groups) — the
 //    reference's runtime-indexed F[33] spills to local memory;
@@ -21,21 +21,11 @@
 //    half-tile CTA, the number of entries its busiest warp composited (the backward launch order);
 //  * per-pixel arithmetic keeps the association of the reference binary, so n_contrib and the
 //    images are bit-identical to it for identical lists.
-#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "detacc.cuh"
 #include "kernels.h"
 
-#ifndef R3DG_FWD_CTAS          // default resident CTAs per SM of the forward compositor (0 = whatever fits)
-#define R3DG_FWD_CTAS 0
-#endif
-#ifndef R3DG_FWD_ILP           // staged entries whose alpha evaluation is in flight together (composite_fwd_kernel), S <= 5
-#define R3DG_FWD_ILP 4
-#endif
-#ifndef R3DG_FWD_ILP_WIDE      // the same for S > 5 (more accumulators per pixel: registers)
-#define R3DG_FWD_ILP_WIDE 2
-#endif
 namespace r3dg {
 
 struct CompositeFwdParams {
@@ -54,11 +44,6 @@ struct CompositeFwdParams {
     float *out_color, *out_opacity, *out_depth, *out_feature, *out_weights;
     uint64_t* det_weights;             // DET: [P] out_weights in exact 2^-24 units (zeroed), converted by det_weights_kernel
 };
-
-#ifdef R3DG_WARP_TIMING
-__device__ WarpTiming g_wt_fwd[R3DG_WT_MAX];
-extern "C" int r3dg_debug_wt_fwd(void* dst, size_t bytes) { return (int)cudaMemcpyFromSymbol(dst, g_wt_fwd, bytes); }
-#endif
 
 // NW = warps per CTA (4: two CTAs per tile).  Warps are autonomous: no
 // CTA-wide barrier anywhere; the CTA only exists so that the warps of a tile share L1 lines.
@@ -99,10 +84,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
     const uint32_t* __restrict__ plist = p.point_list + lo;
     uint32_t* q = sQ[warp];
 
-#ifdef R3DG_WARP_TIMING
-    const unsigned long long wt_t0 = wt_now();
-    unsigned wt_iters = 0;
-#endif
     float T = 1.0f, Dp = 0.0f, Op = 0.0f;
     float C[4 * NG];
 #pragma unroll
@@ -206,9 +187,10 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
         // chains in flight per warp instead of one.  Only the short transmittance recurrence that follows is sequential,
         // in list order, with exactly the reference's arithmetic.  This is what bounds the kernel: the heaviest pixel
         // blocks composite many entries one after the other, and while the light tiles drain the machine those few
-        // warps decide the makespan (tools/warp_timing.py).  A round with fewer than U
-        // entries left re-evaluates the last one, masked out.
-        constexpr int U = NG <= 2 ? R3DG_FWD_ILP : R3DG_FWD_ILP_WIDE;
+        // warps decide the makespan (DESIGN.md §4.2).  A round with fewer than U
+        // entries left re-evaluates the last one, masked out.  U = 4 for S <= 5, 2 for S > 5 (more accumulators per
+        // pixel: registers).
+        constexpr int U = NG <= 2 ? 4 : 2;
         while (word) {
             int jj[U];
             bool pv[U];
@@ -218,9 +200,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
                 const bool have = word != 0u;
                 jj[u] = have ? __ffs(word) - 1 : jj[u ? u - 1 : 0];
                 word &= word - 1u;
-#ifdef R3DG_WARP_TIMING
-                wt_iters += have ? 1u : 0u;
-#endif
                 const float4 a = BULK ? sRecB[warp][stage][jj[u]][0] : sRec[warp][0][jj[u]];
                 const float4 b = BULK ? sRecB[warp][stage][jj[u]][1] : sRec[warp][1][jj[u]];
                 const float dx = sub_(a.x, pxf), dy = sub_(a.y, pyf);
@@ -292,9 +271,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
         p.out_depth[pix] = Dp;
         p.out_opacity[pix] = Op;
     }
-#ifdef R3DG_WARP_TIMING
-    if (lane == 0 && blockIdx.x * NW + warp < R3DG_WT_MAX) g_wt_fwd[blockIdx.x * NW + warp] = WarpTiming{wt_t0, wt_now(), wt_iters, wt_smid()};
-#endif
 }
 
 // Deterministic mode: out_weights = the exact integer total in 2^-24 units, rounded to fp32 once.
@@ -354,23 +330,13 @@ __global__ void __launch_bounds__(256) surface_normal_kernel(int W, int H, const
 }
 
 // resident CTAs per SM the register allocation is pinned to (ptxas otherwise drifts a few registers above the
-// count that fits one more CTA): by channel groups NG, for the 4-warp CTA (the 8-warp variant is left to ptxas)
-#ifndef R3DG_FWD_OCC2          // resident CTAs per SM the kernels are compiled for, by channel groups (tools/occ_sweep.sh)
-#define R3DG_FWD_OCC2 7
-#endif
-#ifndef R3DG_FWD_OCC5
-#define R3DG_FWD_OCC5 5
-#endif
-template <int NG> struct FwdOcc { static constexpr int v = NG <= 2 ? R3DG_FWD_OCC2 : (NG <= 3 ? 6 : (NG <= 5 ? R3DG_FWD_OCC5 : (NG <= 6 ? 4 : 3))); };
+// count that fits one more CTA): by channel groups NG, for the 4-warp CTA (the 8-warp variant is left to ptxas).
+// The values are those of the occupancy sweep in DESIGN.md §4.2.
+template <int NG> struct FwdOcc { static constexpr int v = NG <= 2 ? 7 : (NG <= 3 ? 6 : (NG <= 5 ? 5 : (NG <= 6 ? 4 : 3))); };
 
-int g_composite_bulk = -1;      // r3dg_tune("composite_bulk"): 1 = TMA bulk-copy record staging in the forward compositor
-int g_fwd_ctas = -1;            // r3dg_tune("composite_fwd_ctas"): resident CTAs per SM (0 = whatever fits)
-static void composite_env() {
-    if (g_composite_bulk < 0) { const char* e = getenv("R3DG_COMPOSITE_BULK"); g_composite_bulk = (e && atoi(e) == 1) ? 1 : 0; }
-    if (g_fwd_ctas < 0) { const char* e = getenv("R3DG_FWD_CTAS"); g_fwd_ctas = e ? atoi(e) : R3DG_FWD_CTAS; if (g_fwd_ctas < 0) g_fwd_ctas = 0; }
-}
+int g_composite_bulk = 0;       // r3dg_tune("composite_bulk"): 1 = TMA bulk-copy record staging in the forward compositor
+int g_fwd_ctas = 0;             // r3dg_tune("composite_fwd_ctas"): resident CTAs per SM (0 = whatever fits)
 int composite_tune(const char* key, int value, int* previous) {
-    composite_env();
     if (strcmp(key, "composite_bulk") == 0) {
         if (previous) *previous = g_composite_bulk;
         if (value != 0 && value != 1) return R3DG_ERR_BAD_ARG;
@@ -385,25 +351,19 @@ int composite_tune(const char* key, int value, int* previous) {
     }
     return R3DG_ERR_UNSUPPORTED;
 }
-template <typename K>
-static void launch_fwd_kernel(K kernel, const CompositeFwdParams& p, int tiles, cudaStream_t stream) {
-    static int pad_for = -1, pad_dev = -1;
-    static size_t pad = 0;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (pad_for != g_fwd_ctas || pad_dev != dev) { pad = residency_pad(kernel, g_fwd_ctas); pad_for = g_fwd_ctas; pad_dev = dev; }
-    kernel<<<tiles * 2, 128, pad, stream>>>(p);                          // two 4-warp CTAs per tile
+template <auto K>
+static void launch_fwd_kernel(const CompositeFwdParams& p, int tiles, cudaStream_t stream) {
+    K<<<tiles * 2, 128, residency_pad<K>(g_fwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
 static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, cudaStream_t stream) {
-    composite_env();
     if (p.det_weights) {
-        if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel(composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true, true>, p, tiles, stream);
-        else launch_fwd_kernel(composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false, true>, p, tiles, stream);
+        if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel<composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true, true>>(p, tiles, stream);
+        else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false, true>>(p, tiles, stream);
         return;
     }
-    if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel(composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true>, p, tiles, stream);
-    else launch_fwd_kernel(composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false>, p, tiles, stream);
+    if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel<composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true>>(p, tiles, stream);
+    else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false>>(p, tiles, stream);
 }
 
 int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl, const ImgLayout& il,

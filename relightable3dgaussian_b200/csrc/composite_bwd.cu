@@ -14,30 +14,21 @@
 //    deepest last contributor — no culling test, no record fetch, no exp() for anything else;
 //  * CTAs are launched in the order of the work the forward pass measured (cta_order_kernel), and
 //    the walk is laid out in rounds of U entries for instruction-level parallelism: the kernel is
-//    bound by per-warp latency and its heaviest warps (tools/warp_timing.py measures both);
+//    bound by per-warp latency and its heaviest warps (DESIGN.md §4.2);
 //  * per-pixel state is register resident (template on channel groups); the reference keeps three
 //    float[24] arrays in local memory and 36 KB of shared memory per CTA;
 //  * gradients differ from the reference only by fp32 summation order (the reference's own
 //    atomics make it run-to-run nondeterministic), tolerance 1e-3 relative.
-#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "detacc.cuh"
 #include "kernels.h"
 
-#ifndef R3DG_BWD_CTAS          // default resident CTAs per SM of the backward compositor (0 = whatever fits)
-#define R3DG_BWD_CTAS 0
-#endif
-#ifndef R3DG_BWD_ILP           // entries per round of the backward walk (composite_bwd_kernel), S <= 5
-#define R3DG_BWD_ILP 2
-#endif
-#ifndef R3DG_BWD_ILP_WIDE      // the same for S > 5 (twice the accumulators: registers)
-#define R3DG_BWD_ILP_WIDE 1
-#endif
-
 namespace r3dg {
 
-template <int NG> struct BwdIlp { static constexpr int v = NG <= 2 ? R3DG_BWD_ILP : R3DG_BWD_ILP_WIDE; };
+// entries per round of the backward walk (composite_bwd_kernel): 2 for S <= 5, 1 for S > 5 (twice the accumulators:
+// registers)
+template <int NG> struct BwdIlp { static constexpr int v = NG <= 2 ? 2 : 1; };
 
 struct CompositeBwdParams {
     int W, H, gx, S, recf, backward_geometry;
@@ -124,11 +115,6 @@ __device__ __forceinline__ float reduce_scatter_permuted(float (&x)[W]) {
     return r;
 }
 
-#ifdef R3DG_WARP_TIMING
-__device__ WarpTiming g_wt_bwd[R3DG_WT_MAX];
-extern "C" int r3dg_debug_wt_bwd(void* dst, size_t bytes) { return (int)cudaMemcpyFromSymbol(dst, g_wt_bwd, bytes); }
-#endif
-
 template <int U, int W>
 __device__ __forceinline__ void reduce_scatter_permuted_multi(float (&x)[U][W], float (&r)[U]) {
     int m = 16;
@@ -188,13 +174,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     const uint32_t* __restrict__ plist = p.point_list + lo;
     uint32_t* q = sQ[warp];
 
-#ifdef R3DG_WARP_TIMING
-    const unsigned long long wt_t0 = wt_now();
-    unsigned wt_iters = 0;
-    auto wt_done = [&]() {
-        if (lane == 0 && blockIdx.x * NW + warp < R3DG_WT_MAX) g_wt_bwd[blockIdx.x * NW + warp] = WarpTiming{wt_t0, wt_now(), wt_iters, wt_smid()};
-    };
-#endif
     const float T_final = inside ? p.final_T[pix] : 0.0f;
     float T = T_final;
     const int last_contributor = inside ? p.n_contrib[pix] : 0;
@@ -203,9 +182,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) total = max(total, __shfl_xor_sync(0xffffffffu, total, o));
     total = min(total, (int)(range.y - range.x));
-#ifdef R3DG_WARP_TIMING
-    if (total == 0) wt_done();
-#endif
     if (total == 0) return;
 
     auto load_dpix = [&](int c) -> float {                   // cotangent of channel c of {r,g,b,f0..} at this lane's pixel
@@ -330,9 +306,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
             for (int u = 0; u < U; ++u) {                                   // (1)
                 ju[u] = min(j0 + u, n - 1);
                 const int k = (int)sK[warp][ju[u]];
-#ifdef R3DG_WARP_TIMING
-                wt_iters += j0 + u < n ? 1u : 0u;
-#endif
                 const float4 a = sRec[warp][0][ju[u]];
                 const float4 b = sRec[warp][1][ju[u]];
                 dx[u] = sub_(a.x, pxf); dy[u] = sub_(a.y, pyf);
@@ -438,24 +411,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
             }
         }
     }
-#ifdef R3DG_WARP_TIMING
-    wt_done();
-#endif
 }
 
-#ifndef R3DG_BWD_OCC2
-#define R3DG_BWD_OCC2 5
-#endif
-#ifndef R3DG_BWD_OCC5
-#define R3DG_BWD_OCC5 4
-#endif
-template <int NG> struct BwdOcc { static constexpr int v = NG <= 2 ? R3DG_BWD_OCC2 : (NG <= 3 ? 5 : (NG <= 5 ? R3DG_BWD_OCC5 : 3)); };
-int g_bwd_ctas = -1;            // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
-static void composite_bwd_env() {
-    if (g_bwd_ctas < 0) { const char* e = getenv("R3DG_BWD_CTAS"); g_bwd_ctas = e ? atoi(e) : R3DG_BWD_CTAS; if (g_bwd_ctas < 0) g_bwd_ctas = 0; }
-}
+// resident CTAs per SM the register allocation is pinned to, by channel groups NG (the occupancy sweep in DESIGN.md §4.2)
+template <int NG> struct BwdOcc { static constexpr int v = NG <= 3 ? 5 : (NG <= 5 ? 4 : 3); };
+int g_bwd_ctas = 0;             // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
 int composite_bwd_tune(const char* key, int value, int* previous) {
-    composite_bwd_env();
     if (strcmp(key, "composite_bwd_ctas") != 0) return R3DG_ERR_UNSUPPORTED;
     if (previous) *previous = g_bwd_ctas;
     if (value < 0 || value > 32) return R3DG_ERR_BAD_ARG;
@@ -464,14 +425,8 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
 }
 template <int NG, bool DET>
 static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
-    composite_bwd_env();
-    auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET>;
-    static int pad_for = -1, pad_dev = -1;
-    static size_t pad = 0;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (pad_for != g_bwd_ctas || pad_dev != dev) { pad = residency_pad(kernel, g_bwd_ctas); pad_for = g_bwd_ctas; pad_dev = dev; }
-    kernel<<<tiles * 2, 128, pad, stream>>>(p);                          // two 4-warp CTAs per tile
+    constexpr auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET>;
+    kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 
 int launch_composite_backward(const r3dg_raster_bwd_args& a, const GeomLayout& gl, const ImgLayout& il,

@@ -65,16 +65,36 @@ int shade_tune(const char* key, int value, int* previous);
 int composite_tune(const char* key, int value, int* previous);
 int composite_bwd_tune(const char* key, int value, int* previous);
 
-// Dynamic shared memory to request so that at most `ctas` CTAs of `kernel` are resident per SM (0 when ctas <= 0 or
+// api.cu: SMs of the current device, cached per device (132, the H100 SXM count, if the query fails)
+int num_sms();
+
+// Lets kernel K launch with up to `bytes` of dynamic shared memory on the current device.  Function attributes belong
+// to the device's context and a caller may drive several GPUs from one process, so the attribute is raised once per
+// (kernel, device) and only when a launch needs more than an earlier one did.
+constexpr int kMaxDevices = 64;
+template <auto K>
+inline cudaError_t allow_dyn_smem(size_t bytes) {
+    static size_t allowed[kMaxDevices] = {};
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    const bool cached = dev >= 0 && dev < kMaxDevices;
+    if (cached && bytes <= allowed[dev]) return cudaSuccess;
+    e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess && cached) allowed[dev] = bytes;
+    return e;
+}
+
+// Dynamic shared memory to request so that at most `ctas` CTAs of kernel K are resident per SM (0 when ctas <= 0 or
 // the kernel's own footprint already allows no more).  The compositors are bound by their heaviest warps (a pixel
 // block that composites its entries one after the other): fewer co-resident warps let those run faster while the
 // total throughput stays issue-bound (tools/residency_sweep.py sweeps the setting).
-template <typename K>
-inline size_t residency_pad(K kernel, int ctas) {
+template <auto K>
+inline size_t residency_pad(int ctas) {
     if (ctas <= 0) return 0;
     cudaFuncAttributes fa;
     int dev = 0, smem_sm = 0, smem_blk = 0;
-    if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess || cudaGetDevice(&dev) != cudaSuccess) return 0;
+    if (cudaFuncGetAttributes(&fa, K) != cudaSuccess || cudaGetDevice(&dev) != cudaSuccess) return 0;
     cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
     cudaDeviceGetAttribute(&smem_blk, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     const size_t fixed = fa.sharedSizeBytes + 1024;                       // static + the per-CTA system reservation
@@ -82,7 +102,7 @@ inline size_t residency_pad(K kernel, int ctas) {
     if (per <= fixed) return 0;
     size_t dyn = per - fixed;
     if (fa.sharedSizeBytes + dyn > (size_t)smem_blk) dyn = (size_t)smem_blk - fa.sharedSizeBytes;
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn) != cudaSuccess) { cudaGetLastError(); return 0; }
+    if (allow_dyn_smem<K>(dyn) != cudaSuccess) { cudaGetLastError(); return 0; }
     return dyn;
 }
 

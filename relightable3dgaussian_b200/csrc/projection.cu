@@ -427,7 +427,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(int P, const uint32_
 // The same coarse LPT order as the tile order (binning.cu, bin_starts) for the backward compositor's CTAs, by what the forward pass measured: keys[c] = entries the
 // busiest warp of half-tile CTA c composited = exactly the iterations its backward twin will run.  List length is a poor
 // predictor there (a dense tile saturates after a fraction of its list): ordered by it, heavy backward CTAs started
-// late and finished last (tools/warp_timing.py shows the per-warp start and end times).
+// late and finished last (the per-warp timing study of commit 072299e, DESIGN.md §4.2).
 __global__ void __launch_bounds__(1024) cta_order_kernel(int n, const uint32_t* __restrict__ keys, uint32_t* __restrict__ order) {
     __shared__ uint32_t s_max, s_cnt[64], s_cur[64];
     const int tid = threadIdx.x;

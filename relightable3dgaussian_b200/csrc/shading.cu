@@ -18,7 +18,6 @@
 //    grid_sample's scatter-add of P*N*4 taps — is accumulated in warp-private shared-memory copies
 //    without atomics (see "environment-map gradient" below), summed and flushed once per CTA;
 //  * the backward recomputes the forward per sample instead of saving [P,N,*] activations.
-#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "detacc.cuh"
@@ -146,10 +145,8 @@ struct SampleEval {       // forward quantities of one (Gaussian, direction) pai
     float H[3], hn, NoL, NoV, NoH, VoH, NoL_r, NoV_r, NoH_r, VoH_r, p2, frac0, nom0, nom1, nom2, nom_r, nom;
 };
 
-#ifndef R3DG_SHADE_FWD_FAST        // experiment knob: one-MUFU reciprocals in the FORWARD kernel too (default: IEEE divisions)
-#define R3DG_SHADE_FWD_FAST false
-#endif
-template <bool SMEM_ENV, bool INC_SMEM, bool FAST = R3DG_SHADE_FWD_FAST>
+// FAST: one-MUFU reciprocals (the backward kernel); the forward keeps IEEE divisions
+template <bool SMEM_ENV, bool INC_SMEM, bool FAST = false>
 __device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOperands& o, const float* __restrict__ env,
                                             const float* __restrict__ sinc, float dx, float dy, float dz, float vis, SampleEval& e) {
     // ---- environment + local SH light --------------------------------------------------------
@@ -564,30 +561,22 @@ __global__ void __launch_bounds__(256) det_env_kernel(const DetAcc acc, float* _
 }
 
 // ---- launch ---------------------------------------------------------------------------------------
-// tuning knobs (A/B measurements and tests of the non-default paths): initial value from the
-// environment, changed at run time through r3dg_tune (include/r3dg_b200.h)
-struct ShadeKnob { const char* key; const char* env; int lo, hi, dflt, value; };
+// tuning knobs (A/B measurements and tests of the non-default paths), changed at run time through r3dg_tune
+// (include/r3dg_b200.h); each starts at its default
+struct ShadeKnob { const char* key; int lo, hi, value; };
 static ShadeKnob g_knobs[] = {
-    {"shade_group", "R3DG_SHADE_GROUP", 8, 32, 8, -1},            // lanes per Gaussian: 8, 16 or 32
+    {"shade_group", 8, 32, 8},            // lanes per Gaussian: 8, 16 or 32
     // defaults = the fastest combination measured during development (tools/bench_stage3.py times the variants;
     // variant 2 with shared atomics fits more CTAs per SM than with tagged copies)
-    {"shade_env_mode", "R3DG_SHADE_ENV_MODE", 0, 2, ENV_CAS, -1}, // highest env-gradient mode allowed
-    {"shade_fwd_variant", "R3DG_SHADE_FWD_VARIANT", 0, 1, 1, -1}, // 1: incident SH coefficients in shared memory
-    {"shade_bwd_variant", "R3DG_SHADE_BWD_VARIANT", 0, 2, 2, -1}, // 1: as forward; 2: + gradient accumulators in shared memory
+    {"shade_env_mode", 0, 2, ENV_CAS},    // highest env-gradient mode allowed
+    {"shade_fwd_variant", 0, 1, 1},       // 1: incident SH coefficients in shared memory
+    {"shade_bwd_variant", 0, 2, 2},       // 1: as forward; 2: + gradient accumulators in shared memory
 };
 static bool knob_ok(const ShadeKnob& k, int v) {
     if (v < k.lo || v > k.hi) return false;
     return strcmp(k.key, "shade_group") != 0 || v == 8 || v == 16 || v == 32;
 }
-static int knob(int i) {
-    ShadeKnob& k = g_knobs[i];
-    if (k.value < 0) {
-        const char* e = getenv(k.env);
-        const int v = e ? atoi(e) : k.dflt;
-        k.value = knob_ok(k, v) ? v : k.dflt;
-    }
-    return k.value;
-}
+static int knob(int i) { return g_knobs[i].value; }
 int shade_tune(const char* key, int value, int* previous) {
     for (int i = 0; i < (int)(sizeof(g_knobs) / sizeof(g_knobs[0])); ++i) {
         if (strcmp(key, g_knobs[i].key)) continue;
@@ -683,12 +672,6 @@ int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
 using namespace r3dg;
 extern "C" {
 
-static int shade_num_sms() {
-    static int n = 0;
-    if (n == 0) { int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132; }
-    return n;
-}
-
 static int fill_args(const r3dg_shade_args* s, ShadeArgs& a) {
     if (!s || s->P < 0 || s->N <= 0 || s->env_h <= 0 || s->env_w <= 0) return R3DG_ERR_BAD_ARG;
     if (s->sh_coeffs != 16) return R3DG_ERR_UNSUPPORTED;          // incidents are degree-3 SH ([P,16,3]) in the reference
@@ -714,7 +697,7 @@ int r3dg_render_equation_forward(const r3dg_shade_args* s, r3dg_stream_t stream)
     if (a.P > 0 && (!a.pbr || !a.diffuse || !a.specular)) return R3DG_ERR_BAD_ARG;
     if ((a.mean_lights != nullptr) != (a.mean_local != nullptr) || (a.mean_lights != nullptr) != (a.mean_global != nullptr)) return R3DG_ERR_BAD_ARG;
     if ((a.s_lights != nullptr) != (a.s_local != nullptr) || (a.s_lights != nullptr) != (a.s_global != nullptr)) return R3DG_ERR_BAD_ARG;
-    return launch_shade_forward(a, shade_num_sms(), (cudaStream_t)stream);
+    return launch_shade_forward(a, num_sms(), (cudaStream_t)stream);
 }
 
 int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream) {
@@ -727,7 +710,7 @@ int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream
         if (!s->det_work || s->det_work_bytes < det_bytes(n)) return R3DG_ERR_BAD_ARG;
         a.det = det_acc(s->det_work, n);
     }
-    return launch_shade_backward(a, shade_num_sms(), (cudaStream_t)stream);
+    return launch_shade_backward(a, num_sms(), (cudaStream_t)stream);
 }
 
 size_t r3dg_shade_det_bytes(int env_h, int env_w) {

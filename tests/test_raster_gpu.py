@@ -515,6 +515,72 @@ def test_bulk_copy_record_staging_variant_is_bit_identical(C):
         assert torch.equal(a[n], b[n]), n
 
 
+IMAGES = ("color", "opacity", "depth", "feature", "normal", "surface_xyz", "n_contrib")
+
+
+def _assert_bits_equal(a, b, names):
+    bits = lambda t: t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
+    for n in names:
+        assert a[n].shape == b[n].shape and torch.equal(bits(a[n]), bits(b[n])), n
+
+
+def _shell_case(P, W, H, S, view):
+    sc, cam = case_inputs(P, W, H, S, view=view)
+    kw = oracle_kwargs(sc, cam, torch.tensor([0.0, 0.5, 1.0]))
+    kw.update(shs=npy(sc.shs), scales=npy(sc.scales), rotations=npy(sc.rotations), features=npy(sc.features) if S else None)
+    gen = torch.Generator().manual_seed(2)
+    return kw, [torch.randn(c, H, W, generator=gen) for c in (3, 1, 1, S)]
+
+
+def test_residency_knobs_held_across_kernel_instantiations(C):
+    """composite_fwd_ctas = composite_bwd_ctas = 2 set once, then forward + backward with several compositor
+    instantiations in a row (channel-group counts, deterministic mode).  The residency padding (~100 KB of dynamic
+    shared memory per CTA at 2 CTAs/SM) is computed and allowed for each instantiation on its own, and changes only
+    residency: images and n_contrib, and in deterministic mode out_weights and the gradients, are bitwise those of
+    the same call at the default residency."""
+    from relightable3dgaussian_b200 import _lib
+    cases = [(5, False), (5, True), (16, False), (24, True)]          # (S, deterministic mode)
+    inputs = {S: _shell_case(200_000, 640, 480, S, view=4) for S in (5, 16, 24)}
+    prev_det = torch.are_deterministic_algorithms_enabled()
+
+    def run(S, det):
+        kw, cots = inputs[S]
+        torch.use_deterministic_algorithms(det)
+        try:
+            o = run_ours(C, cots=cots, **kw)
+        finally:
+            torch.use_deterministic_algorithms(prev_det)
+        return {**{n: o[n] for n in IMAGES + ("weights",)}, **o["grads"]}
+
+    refs = [run(S, det) for S, det in cases]
+    prev = {k: _lib.tune(k, 2) for k in ("composite_fwd_ctas", "composite_bwd_ctas")}
+    try:
+        outs = [run(S, det) for S, det in cases]
+    finally:
+        for k, v in prev.items():
+            _lib.tune(k, v)
+    for (S, det), ref, out in zip(cases, refs, outs):
+        names = IMAGES + (("weights",) + tuple(n for n in GRADS if ref[n].numel()) if det else ())
+        _assert_bits_equal(ref, out, names)
+
+
+def test_second_device_renders_bitwise_like_the_first(C):
+    """One process renders the headline view on cuda:0 and then on cuda:1: the kernels whose launch attributes are
+    cached (the binning scatter asks for far more than 48 KB of dynamic shared memory here) get them on each device,
+    and the two renders are bitwise equal."""
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs >= 2 GPUs")
+    kw, _ = _shell_case(1_000_000, 800, 800, 5, view=0)
+    outs = []
+    for d in (0, 1):
+        with torch.cuda.device(d):
+            o = run_ours(C, **kw)
+        assert o["color"].device == torch.device("cuda", d)
+        outs.append({n: o[n].cpu() for n in IMAGES + ("radii",)} | {"num_rendered": o["num_rendered"]})
+    assert outs[0]["num_rendered"] == outs[1]["num_rendered"]
+    _assert_bits_equal(outs[0], outs[1], IMAGES + ("radii",))
+
+
 def _our_edge_stats(o, kw):
     return edge_stats(kw, npy(o["radii"]), npy(o["mid"]("depths")), npy(o["mid"]("conic_opacity")), npy(o["n_contrib"]),
                       npy(o["mid"]("final_T")), npy(o["mid"]("ranges")))

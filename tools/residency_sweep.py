@@ -1,5 +1,5 @@
-"""Sweep the compositors' resident-CTAs-per-SM knobs (r3dg_tune composite_fwd_ctas / composite_bwd_ctas) for one
-library build (R3DG_LIB_PATH selects it): per setting, mean stage times of the raster fwd+bwd over a few views.
+"""Sweep the compositors' resident-CTAs-per-SM knobs (r3dg_tune composite_fwd_ctas / composite_bwd_ctas): per
+setting, mean stage times of the raster fwd+bwd over a few views.  TAG labels the output lines.
 usage: python tools/residency_sweep.py TAG P W H S "f,b f,b ..." """
 import ctypes
 import json
