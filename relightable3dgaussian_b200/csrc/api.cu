@@ -38,6 +38,95 @@ inline void prof_mark(bool fwd, int i, cudaStream_t s) {
     if (call >= g_prof.max_calls) return;
     cudaEventRecord(g_prof.at(call, i), s);
 }
+
+// ---- the rasterizer's work buffers: regions in this order, each 256-byte aligned ---------------------------------
+struct GeomLayout {
+    size_t header, rec, tiles_touched, rects, brects, clamped, scan_state, sort, grad, total;
+    int recf;
+    SortLayout sl;
+    GeomLayout(int P, int S) : recf(rec_floats(S)), sl(P) {
+        size_t off = 0;
+        header = off;        off = align_up(off + sizeof(GeomHeader), 256);
+        rec = off;           off = align_up(off + (size_t)P * recf * 4, 256);
+        tiles_touched = off; off = align_up(off + (size_t)P * 4, 256);
+        rects = off;         off = align_up(off + (size_t)P * 8, 256);         // packed tile rectangles
+        brects = off;        off = align_up(off + (size_t)P * 8, 256);         // packed block rectangles (block_rect())
+        clamped = off;       off = align_up(off + (size_t)P, 256);
+        scan_state = off;    off = align_up(off + ((size_t)P / R3DG_SCAN_ITEMS + 2) * 4, 256);
+        sort = off;          off = align_up(off + sl.total, 256);               // depth sort of the Gaussians
+        grad = off;          off = align_up(off + (size_t)P * recf * 4, 256);   // backward scratch
+        total = off;
+    }
+};
+
+struct ImgLayout {
+    size_t final_T, n_contrib, ranges, tile_order, bwd_work, bwd_order, slab_sum, bin_matrix, total;
+    int gx, gy, max_chunks;
+    ImgLayout(int W, int H) : gx((W + R3DG_TILE - 1) / R3DG_TILE), gy((H + R3DG_TILE - 1) / R3DG_TILE) {
+        const size_t HW = (size_t)W * H, T = (size_t)gx * gy;
+        max_chunks = bin_max_chunks(T);
+        size_t off = 0;
+        final_T = off;   off = align_up(off + HW * 4, 256);
+        n_contrib = off; off = align_up(off + HW * 4, 256);
+        ranges = off;    off = align_up(off + T * 8, 256);
+        tile_order = off; off = align_up(off + T * 4, 256);      // tiles by descending list length
+        bwd_work = off;  off = align_up(off + 2 * T * 4, 256);    // per half-tile CTA: entries its busiest warp composited (forward)
+        bwd_order = off; off = align_up(off + 2 * T * 4, 256);    // half-tile CTAs by descending bwd_work (backward launch order)
+        slab_sum = off;  off = align_up(off + T * 4 * ((R3DG_BIN_MAX_CHUNKS + 511) / 512), 256);   // per 512-chunk slab
+        bin_matrix = off; off = align_up(off + ((size_t)max_chunks + 1) * T * 4, 256);   // + the row of list ends
+        total = off;
+    }
+};
+
+// Binning buffer (capacity-sized, speculative): the per-tile depth-sorted Gaussian lists (reference
+// binningState.point_list) plus one byte per instance for each of
+//   bmask: bit b = 8x4 pixel block b of the instance's tile may be touched by the Gaussian (written by bin_scatter
+//          with block_mask_of_rect: the conservative block-rectangle test evaluated ONCE per instance instead of by 8 warps);
+//   cmask: bit b = block b actually composited the instance in the forward pass (some pixel accepted it).  The
+//          backward compositor visits exactly the cmask entries of its block, nothing else.
+// 6 B per instance instead of the reference's 24 B + sort temp.
+struct BinLayout {
+    size_t point_list, bmask, cmask, total;
+    long long capacity;
+    BinLayout(long long cap) : capacity(cap) {
+        size_t off = 0;
+        point_list = off; off = align_up(off + (size_t)cap * 4, 256);
+        bmask = off;      off = align_up(off + (size_t)cap, 256);
+        cmask = off;      off = align_up(off + (size_t)cap, 256);
+        total = off;
+    }
+};
+// largest capacity (a multiple of 64 instances) whose layout fits in `bytes`; r3dg_raster_binning_bytes is its inverse
+long long bin_capacity_for_bytes(size_t bytes) { return bytes < 768 + 384 ? 0 : (long long)((bytes - 768) / 6 / 64 * 64); }
+size_t bin_bytes_for_capacity(long long cap) { return (size_t)((cap + 63) / 64 * 64) * 6 + 768; }
+
+// Fills `b` for one call; P = 0 is laid out as P = 1, as r3dg_raster_geom_bytes sizes it.  Returns R3DG_ERR_BAD_ARG
+// when a buffer is smaller than its layout or the binning buffer holds no instance, and fills `b` either way
+// (r3dg_raster_debug_copy passes SIZE_MAX for the sizes it is not given, and needs the binning only for some ids).
+int raster_buffers(int P, int S, int W, int H, void* geom_, size_t geom_bytes, void* img_, size_t img_bytes,
+                   void* bin_, size_t bin_bytes, RasterBuffers& b) {
+    const GeomLayout gl(P < 1 ? 1 : P, S);
+    const ImgLayout il(W, H);
+    const BinLayout bl(bin_capacity_for_bytes(bin_bytes));
+    char *geom = (char*)geom_, *img = (char*)img_, *bin = (char*)bin_;
+    b.header = (GeomHeader*)(geom + gl.header);
+    b.rec = (float*)(geom + gl.rec); b.grad = (float*)(geom + gl.grad);
+    b.tiles_touched = (uint32_t*)(geom + gl.tiles_touched);
+    b.rects = (uint2*)(geom + gl.rects); b.brects = (uint2*)(geom + gl.brects);
+    b.clamped = (uint8_t*)(geom + gl.clamped);
+    b.sort = geom + gl.sort; b.sort_layout = gl.sl;
+    b.final_T = (float*)(img + il.final_T); b.n_contrib = (int*)(img + il.n_contrib);
+    b.ranges = (uint2*)(img + il.ranges); b.tile_order = (uint32_t*)(img + il.tile_order);
+    b.bwd_work = (uint32_t*)(img + il.bwd_work); b.bwd_order = (uint32_t*)(img + il.bwd_order);
+    b.slab_sum = (uint32_t*)(img + il.slab_sum); b.bin_matrix = (uint32_t*)(img + il.bin_matrix);
+    b.point_list = (uint32_t*)(bin + bl.point_list);
+    b.bmask = (uint8_t*)(bin + bl.bmask); b.cmask = (uint8_t*)(bin + bl.cmask);
+    b.capacity = bl.capacity;
+    b.recf = gl.recf; b.gx = il.gx; b.gy = il.gy; b.tiles = il.gx * il.gy;
+    b.chunk_len = bin_chunk_len(P, il.max_chunks);          // one read of R3DG_BIN_MAX_CHUNKS sizes M and the chunks
+    b.chunks = (P + b.chunk_len - 1) / b.chunk_len;
+    return geom_bytes < gl.total || img_bytes < il.total || bl.capacity < 1 ? R3DG_ERR_BAD_ARG : 0;
+}
 }  // namespace
 
 extern "C" {
@@ -70,38 +159,31 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     if (a->P > 0 && ((a->shs == nullptr) == (a->colors_precomp == nullptr))) return R3DG_ERR_BAD_ARG;
     if (a->P > 0 && (a->cov3D_precomp == nullptr) && (a->scales == nullptr || a->rotations == nullptr)) return R3DG_ERR_BAD_ARG;
     if (a->shs && a->M > 16) return R3DG_ERR_UNSUPPORTED;
-    const GeomLayout gl(a->P < 1 ? 1 : a->P, a->S);
-    const ImgLayout il(a->W, a->H);
-    if (a->geom_bytes < gl.total || a->img_bytes < il.total) return R3DG_ERR_BAD_ARG;
+    RasterBuffers b;
+    int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
+                            a->binning_bytes, b);
+    if (rc != 0) return rc;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(a->P))) return R3DG_ERR_BAD_ARG;
-    const long long capacity = bin_capacity_for_bytes(a->binning_bytes);
-    if (capacity < 1) return R3DG_ERR_BAD_ARG;
-    const BinLayout bl(capacity);
-    char* geom = (char*)a->geom;
-    char* img = (char*)a->img;
-    char* bin = (char*)a->binning;
-    R3DG_CUDA_TRY(cudaMemsetAsync(geom + gl.header, 0, sizeof(GeomHeader), stream));
-    int rc = 0;
+    R3DG_CUDA_TRY(cudaMemsetAsync(b.header, 0, sizeof(GeomHeader), stream));
     auto mark = [](int i, cudaStream_t s) { prof_mark(true, i, s); };
     prof_mark(true, 0, stream);
     if (a->P > 0) {
-        if ((rc = launch_projection(*a, gl, stream)) != 0) return rc;
+        if ((rc = launch_projection(*a, b, stream)) != 0) return rc;
         prof_mark(true, 1, stream);
-        if ((rc = launch_binning(a->P, a->W, a->H, geom, gl, img, il, bin, bl, num_sms(), stream, mark, a->num_rendered_host,
-                                 a->count_ready_event)) != 0) return rc;
+        if ((rc = launch_binning(a->P, b, num_sms(), stream, mark, a->num_rendered_host, a->count_ready_event)) != 0) return rc;
         g_launches += 1 + (1 + R3DG_SORT_MAX_PASSES) + 4;   // project; histogram + radix passes; count, colsum + starts, apply, scatter
     } else {
-        if ((rc = launch_empty_binning(a->W, a->H, geom, gl, img, il, stream)) != 0) return rc;
+        if ((rc = launch_empty_binning(b, stream)) != 0) return rc;
         for (int i = 1; i <= 4; ++i) prof_mark(true, i, stream);
         g_launches += 1;                                    // starts (empty ranges, tile order)
     }
     prof_mark(true, 5, stream);
-    if ((rc = launch_composite_forward(*a, gl, il, bin, bl, stream, mark)) != 0) return rc;
+    if ((rc = launch_composite_forward(*a, b, stream, mark)) != 0) return rc;
     prof_mark(true, 7, stream);
     g_launches += 1 + (a->computer_pseudo_normal ? 1 : 0) + (a->deterministic && a->P > 0 ? 1 : 0);   // composite, normals, weights
     if (g_prof.on) g_prof.fwd_calls++;
     if (a->P == 0) {      // (P > 0: the count was written, and the event recorded, as soon as the binning offsets existed)
-        if (a->num_rendered_host) R3DG_CUDA_TRY(cudaMemcpyAsync(a->num_rendered_host, geom + gl.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        if (a->num_rendered_host) R3DG_CUDA_TRY(cudaMemcpyAsync(a->num_rendered_host, b.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
         if (a->count_ready_event) R3DG_CUDA_TRY(cudaEventRecord((cudaEvent_t)a->count_ready_event, stream));
     }
     if (a->debug) {   // reference CHECK_CUDA semantics (auxiliary.h:166-173): sync and report
@@ -117,18 +199,14 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (a->S > R3DG_MAX_S_BWD) return R3DG_ERR_UNSUPPORTED;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(a->P, a->S))) return R3DG_ERR_BAD_ARG;
     if (a->P == 0) return 0;
-    const GeomLayout gl(a->P, a->S);
-    const ImgLayout il(a->W, a->H);
-    if (a->geom_bytes < gl.total || a->img_bytes < il.total) return R3DG_ERR_BAD_ARG;
-    const long long capacity = bin_capacity_for_bytes(a->binning_bytes);
-    if (capacity < 1) return R3DG_ERR_BAD_ARG;
-    const BinLayout bl(capacity);
-    char* bin = (char*)a->binning;
-    int rc = 0;
+    RasterBuffers b;
+    int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
+                            a->binning_bytes, b);
+    if (rc != 0) return rc;
     prof_mark(false, 8, stream);
-    if ((rc = launch_composite_backward(*a, gl, il, bin, bl, stream)) != 0) return rc;
+    if ((rc = launch_composite_backward(*a, b, stream)) != 0) return rc;
     prof_mark(false, 9, stream);
-    if ((rc = launch_projection_backward(*a, gl, stream)) != 0) return rc;
+    if ((rc = launch_projection_backward(*a, b, stream)) != 0) return rc;
     prof_mark(false, 10, stream);
     g_launches += 3;   // CTA order, composite, projection
     if (g_prof.on) g_prof.bwd_calls++;
@@ -381,15 +459,12 @@ long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void*
                                  const void* bin_, size_t binning_bytes, void* dst, long long max_bytes,
                                  r3dg_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    const GeomLayout gl(P < 1 ? 1 : P, S);
-    const ImgLayout il(W, H);
-    const char* geom = (const char*)geom_;
-    const char* img = (const char*)img_;
-    const char* bin = (const char*)bin_;
+    RasterBuffers b;       // the geom and img sizes are not given: only the binning buffer's is checked
+    const bool binned = raster_buffers(P, S, W, H, const_cast<void*>(geom_), SIZE_MAX, const_cast<void*>(img_), SIZE_MAX,
+                                       const_cast<void*>(bin_), binning_bytes, b) == 0;
     const size_t HW = (size_t)W * H;
-    const int tiles = ((W + R3DG_TILE - 1) / R3DG_TILE) * ((H + R3DG_TILE - 1) / R3DG_TILE);
-    const float* rec = (const float*)(geom + gl.rec);
-    const uint32_t* tt = (const uint32_t*)(geom + gl.tiles_touched);
+    const float* rec = b.rec;
+    const uint32_t* tt = b.tiles_touched;
     const int nb = (P + 255) / 256;
     auto copy = [&](const void* src, size_t n) -> long long {
         if ((long long)n > max_bytes) n = (size_t)max_bytes;
@@ -397,12 +472,12 @@ long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void*
         return (long long)n;
     };
     switch (id) {
-        case 0: if (max_bytes < 4LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, gl.recf, 0, rec, tt, (float*)dst); return 4LL * P;
-        case 1: if (max_bytes < 3LL * P) return -1; if (P) unpack_clamped_kernel<<<nb, 256, 0, stream>>>(P, (const uint8_t*)(geom + gl.clamped), tt, (uint8_t*)dst); return 3LL * P;
-        case 3: if (max_bytes < 8LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, gl.recf, 3, rec, tt, (float*)dst); return 8LL * P;
-        case 5: if (max_bytes < 16LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, gl.recf, 5, rec, tt, (float*)dst); return 16LL * P;
-        case 6: if (max_bytes < 12LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, gl.recf, 6, rec, tt, (float*)dst); return 12LL * P;
-        case 7: return copy(geom + gl.tiles_touched, 4 * (size_t)P);
+        case 0: if (max_bytes < 4LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, b.recf, 0, rec, tt, (float*)dst); return 4LL * P;
+        case 1: if (max_bytes < 3LL * P) return -1; if (P) unpack_clamped_kernel<<<nb, 256, 0, stream>>>(P, b.clamped, tt, (uint8_t*)dst); return 3LL * P;
+        case 3: if (max_bytes < 8LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, b.recf, 3, rec, tt, (float*)dst); return 8LL * P;
+        case 5: if (max_bytes < 16LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, b.recf, 5, rec, tt, (float*)dst); return 16LL * P;
+        case 6: if (max_bytes < 12LL * P) return -1; if (P) unpack_rec_kernel<<<nb, 256, 0, stream>>>(P, b.recf, 6, rec, tt, (float*)dst); return 12LL * P;
+        case 7: return copy(tt, 4 * (size_t)P);
         case 8: {   // reference geomState.point_offsets: rebuilt on demand (not needed by the hot path)
             if (max_bytes < 4LL * P) return -1;
             if (P == 0) return 0;
@@ -414,24 +489,21 @@ long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void*
             cudaFree(tmp);
             return rc == 0 ? 4LL * P : -2;
         }
-        case 13: return copy(img + il.final_T, 4 * HW);
-        case 14: return copy(img + il.n_contrib, 4 * HW);
-        case 15: return copy(img + il.ranges, 8 * (size_t)tiles);
-        case 16: return copy(img + il.bwd_work, 8 * (size_t)tiles);
-        case 17: return copy(img + il.bwd_order, 8 * (size_t)tiles);
-        case 20: return copy(geom + gl.brects, 8 * (size_t)P);
+        case 13: return copy(b.final_T, 4 * HW);
+        case 14: return copy(b.n_contrib, 4 * HW);
+        case 15: return copy(b.ranges, 8 * (size_t)b.tiles);
+        case 16: return copy(b.bwd_work, 8 * (size_t)b.tiles);
+        case 17: return copy(b.bwd_order, 8 * (size_t)b.tiles);
+        case 20: return copy(b.brects, 8 * (size_t)P);
         case 9: case 10: case 18: case 19: {
-            const long long capacity = bin_capacity_for_bytes(binning_bytes);
-            if (capacity < 1) return -1;
-            const BinLayout bl(capacity);
+            if (!binned) return -1;
             // caller limits the copy to R entries through max_bytes
-            if (id == 9) return copy(bin + bl.point_list, std::min((size_t)max_bytes, (size_t)capacity * 4));
-            if (id == 18) return copy(bin + bl.bmask, std::min((size_t)max_bytes, (size_t)capacity));
-            if (id == 19) return copy(bin + bl.cmask, std::min((size_t)max_bytes, (size_t)capacity));
+            if (id == 9) return copy(b.point_list, std::min((size_t)max_bytes, (size_t)b.capacity * 4));
+            if (id == 18) return copy(b.bmask, std::min((size_t)max_bytes, (size_t)b.capacity));
+            if (id == 19) return copy(b.cmask, std::min((size_t)max_bytes, (size_t)b.capacity));
             // reference binningState.point_list_keys (sorted): rebuilt from the lists
-            const long long limit = std::min(max_bytes / 8, capacity);
-            if (launch_rebuild_keys(tiles, img + il.ranges, (const uint32_t*)(bin + bl.point_list), rec, gl.recf, limit,
-                                    (uint64_t*)dst, stream) != 0) return -2;
+            const long long limit = std::min(max_bytes / 8, b.capacity);
+            if (launch_rebuild_keys(b.tiles, b.ranges, b.point_list, rec, b.recf, limit, (uint64_t*)dst, stream) != 0) return -2;
             return limit * 8;
         }
     }

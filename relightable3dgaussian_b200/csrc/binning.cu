@@ -453,13 +453,9 @@ int launch_rebuild_keys(int T, const void* ranges, const uint32_t* point_list, c
     return 0;
 }
 
-int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
-                   char* bin, const BinLayout& bl, int num_sms, cudaStream_t stream, stage_mark_fn mark,
+int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stream, stage_mark_fn mark,
                    int* num_rendered_host, void* count_ready_event) {
-    const int gx = (W + R3DG_TILE - 1) / R3DG_TILE, gy = (H + R3DG_TILE - 1) / R3DG_TILE;
-    const int T = gx * gy;
-    const int CH = bin_chunk_len(P, (size_t)T);
-    const int chunks = (P + CH - 1) / CH;
+    const int gx = b.gx, gy = b.gy, T = b.tiles, CH = b.chunk_len, chunks = b.chunks;
     // shared memory of bin_scatter: the per-tile array, the per-warp bitmaps, the per-position ids and block
     // rectangles + a staging area of up to 12 entries per Gaussian, as far as it fits (>= CH entries, since one tile
     // can receive every Gaussian of the chunk); a copy of the chunk's first slots per tile where that still leaves the
@@ -475,26 +471,19 @@ int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* 
     if (starts_in_smem) tbl_bytes += tile_bytes;
     int cap = (int)std::min<size_t>((smem_max - tbl_bytes) / 4, full_stage);
     if (const char* e = getenv("R3DG_BIN_STAGE_CAP")) cap = std::max(CH, std::min(cap, atoi(e)));   // tests: force the multi-window path
-    GeomHeader* header = (GeomHeader*)(geom + gl.header);
-    const SortLayout sl(P);
-    char* sbuf = geom + gl.sort;
-    int rc = launch_sort(header, sbuf, sl, P, num_sms, stream);
+    int rc = launch_sort(b.header, b.sort, b.sort_layout, P, num_sms, stream);
     if (rc != 0) return rc;
     mark(2, stream);
     const size_t smem_count = (size_t)T * 4;
     const size_t smem_scatter = tbl_bytes + (size_t)cap * 4;
     R3DG_CUDA_TRY(allow_dyn_smem<bin_count_kernel>(smem_count));
     R3DG_CUDA_TRY(allow_dyn_smem<bin_scatter_kernel>(smem_scatter));
-    const uint32_t* va = (const uint32_t*)(sbuf + sl.vals_a);
-    const uint32_t* vb = (const uint32_t*)(sbuf + sl.vals_b);
-    const uint2* rects = (const uint2*)(geom + gl.rects);
-    uint32_t* M = (uint32_t*)(img + il.bin_matrix);
-    uint2* ranges = (uint2*)(img + il.ranges);
-    uint32_t* slab_sum = (uint32_t*)(img + il.slab_sum);
-    uint32_t* point_list = (uint32_t*)(bin + bl.point_list);
+    const uint32_t* va = (const uint32_t*)(b.sort + b.sort_layout.vals_a);
+    const uint32_t* vb = (const uint32_t*)(b.sort + b.sort_layout.vals_b);
+    uint32_t* M = b.bin_matrix;
     const int slabs = (chunks + BIN_SLAB - 1) / BIN_SLAB;
     const dim3 sgrid((T + 31) / 32, slabs), sblock(32, 32);
-    bin_count_kernel<<<chunks, BIN_COUNT_THREADS, smem_count, stream>>>(P, T, gx, CH, header, va, vb, rects, M);
+    bin_count_kernel<<<chunks, BIN_COUNT_THREADS, smem_count, stream>>>(P, T, gx, CH, b.header, va, vb, b.rects, M);
     mark(3, stream);
     // the instance count exists after bin_starts: hand it to the host early (the scatter and the compositor are still
     // to run).  Page-locked host memory is mapped into the device's address space: bin_starts stores the count there
@@ -508,25 +497,22 @@ int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* 
         else
             cudaGetLastError();                           // clear the query's error state
     }
-    bin_colsum_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, slabs, M, slab_sum, ranges, header, bl.capacity,
-                                                    (uint32_t*)(img + il.tile_order), (uint32_t*)(img + il.bwd_work), count_host);
+    bin_colsum_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, slabs, M, b.slab_sum, b.ranges, b.header, b.capacity,
+                                                    b.tile_order, b.bwd_work, count_host);
     if (num_rendered_host && !count_host)
-        R3DG_CUDA_TRY(cudaMemcpyAsync(num_rendered_host, header, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        R3DG_CUDA_TRY(cudaMemcpyAsync(num_rendered_host, b.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
     if (count_ready_event) R3DG_CUDA_TRY(cudaEventRecord((cudaEvent_t)count_ready_event, stream));
-    bin_apply_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, M, slab_sum);
+    bin_apply_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, M, b.slab_sum);
     mark(4, stream);
     bin_scatter_kernel<<<chunks, BIN_SCATTER_THREADS, smem_scatter, stream>>>(
-        P, T, gx, (1ull << 32) / (unsigned long long)gx + 1ull, CH, cap, header, va, vb, rects, (const uint2*)(geom + gl.brects), M, point_list,
-        (uint8_t*)(bin + bl.bmask), (uint8_t*)(bin + bl.cmask), bl.capacity, starts_in_smem);
+        P, T, gx, (1ull << 32) / (unsigned long long)gx + 1ull, CH, cap, b.header, va, vb, b.rects, b.brects, M, b.point_list,
+        b.bmask, b.cmask, b.capacity, starts_in_smem);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
-int launch_empty_binning(int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
-                         cudaStream_t stream) {
-    const int T = ((W + R3DG_TILE - 1) / R3DG_TILE) * ((H + R3DG_TILE - 1) / R3DG_TILE);
-    bin_starts_kernel<<<1, 1024, 0, stream>>>(T, (uint2*)(img + il.ranges), (GeomHeader*)(geom + gl.header),
-                                              (uint32_t*)(img + il.tile_order), (uint32_t*)(img + il.bwd_work));
+int launch_empty_binning(const RasterBuffers& b, cudaStream_t stream) {
+    bin_starts_kernel<<<1, 1024, 0, stream>>>(b.tiles, b.ranges, b.header, b.tile_order, b.bwd_work);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -1,5 +1,6 @@
-// Shared device-side definitions: work-buffer layouts, the packed per-Gaussian record and
-// small helpers.  Nothing here is visible through the C ABI (include/r3dg_b200.h).
+// Shared device-side definitions: the packed per-Gaussian record, the radix-sort layout and
+// small helpers.  Nothing here is visible through the C ABI (include/r3dg_b200.h); the layout
+// of the rasterizer's work buffers belongs to api.cu.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -78,86 +79,24 @@ __device__ __forceinline__ void sort_plan(uint32_t diff, int& passes, int& w) {
     w = passes ? (nb + passes - 1) / passes : 0;
 }
 
-struct GeomLayout {
-    size_t header, rec, tiles_touched, rects, brects, clamped, scan_state, sort, grad, total;
-    int P, S, recf;
-    __host__ GeomLayout(int P_, int S_) : P(P_), S(S_) {
-        recf = rec_floats(S_);
-        size_t off = 0;
-        header = off;        off = align_up(off + sizeof(GeomHeader), 256);
-        rec = off;           off = align_up(off + (size_t)P_ * recf * 4, 256);
-        tiles_touched = off; off = align_up(off + (size_t)P_ * 4, 256);
-        rects = off;         off = align_up(off + (size_t)P_ * 8, 256);         // packed tile rectangles
-        brects = off;        off = align_up(off + (size_t)P_ * 8, 256);         // packed block rectangles (block_rect())
-        clamped = off;       off = align_up(off + (size_t)P_, 256);
-        scan_state = off;    off = align_up(off + ((size_t)P_ / R3DG_SCAN_ITEMS + 2) * 4, 256);
-        sort = off;          off = align_up(off + SortLayout(P_).total, 256);   // depth sort of the Gaussians
-        grad = off;          off = align_up(off + (size_t)P_ * recf * 4, 256);   // backward scratch
-        total = off;
-    }
-};
-
 // ---- depth-ordered tile binning (binning.cu) -------------------------------------------------
 // The depth-sorted Gaussians are cut into `chunks` runs of CH; M[chunk][tile] first counts the
 // instances a chunk adds to a tile, then (scanned down the columns) is the chunk's first slot
 // inside the tile's list, and row M[chunks] holds the (unclamped) end of every list.
 #define R3DG_BIN_MAX_CHUNKS 1024
-__host__ __device__ inline int bin_max_chunks(size_t T) {
-#ifndef __CUDA_ARCH__
+inline int bin_max_chunks(size_t T) {                                 // the most chunks M holds for T tiles
     if (const char* e = getenv("R3DG_BIN_MAX_CHUNKS")) { const int v = atoi(e); if (v >= 1 && v <= R3DG_BIN_MAX_CHUNKS) return v; }   // tests: long chunks
-#endif
     size_t c = ((size_t)1 << 26) / (T ? T : 1);
     return (int)(c < 296 ? 296 : (c > R3DG_BIN_MAX_CHUNKS ? R3DG_BIN_MAX_CHUNKS : c));
 }
-__host__ __device__ inline int bin_chunk_len(int P, size_t T) {     // Gaussians per chunk, multiple of 256
+inline int bin_chunk_len(int P, int max_chunks) {                     // Gaussians per chunk, multiple of 256
     // ~3 chunks per SM for load balance, 512..2048 Gaussians (longer per-tile runs coalesce better,
     // the staging area of bin_scatter bounds it), and never more chunks than M has rows
     int ch = ((P + 443) / 444 + 255) / 256 * 256;
     ch = ch < 512 ? 512 : (ch > 2048 ? 2048 : ch);
-    const int mc = bin_max_chunks(T);
-    const int need = ((P + mc - 1) / mc + 255) / 256 * 256;
+    const int need = ((P + max_chunks - 1) / max_chunks + 255) / 256 * 256;
     return ch > need ? ch : need;
 }
-
-struct ImgLayout {
-    size_t final_T, n_contrib, ranges, tile_order, bwd_work, bwd_order, slab_sum, bin_matrix, total;
-    __host__ __device__ ImgLayout(int W, int H) {
-        size_t HW = (size_t)W * H;
-        size_t T = (size_t)((W + R3DG_TILE - 1) / R3DG_TILE) * ((H + R3DG_TILE - 1) / R3DG_TILE);
-        size_t off = 0;
-        final_T = off;   off = align_up(off + HW * 4, 256);
-        n_contrib = off; off = align_up(off + HW * 4, 256);
-        ranges = off;    off = align_up(off + T * 8, 256);
-        tile_order = off; off = align_up(off + T * 4, 256);      // tiles by descending list length
-        bwd_work = off;  off = align_up(off + 2 * T * 4, 256);    // per half-tile CTA: entries its busiest warp composited (forward)
-        bwd_order = off; off = align_up(off + 2 * T * 4, 256);    // half-tile CTAs by descending bwd_work (backward launch order)
-        slab_sum = off;  off = align_up(off + T * 4 * ((R3DG_BIN_MAX_CHUNKS + 511) / 512), 256);   // per 512-chunk slab
-        bin_matrix = off; off = align_up(off + ((size_t)bin_max_chunks(T) + 1) * T * 4, 256);   // + the row of list ends
-        total = off;
-    }
-};
-
-// Binning buffer (capacity-sized, speculative): the per-tile depth-sorted Gaussian lists (reference
-// binningState.point_list) plus one byte per instance for each of
-//   bmask: bit b = 8x4 pixel block b of the instance's tile may be touched by the Gaussian (written by bin_scatter
-//          with block_mask_of_rect: the conservative block-rectangle test evaluated ONCE per instance instead of by 8 warps);
-//   cmask: bit b = block b actually composited the instance in the forward pass (some pixel accepted it).  The
-//          backward compositor visits exactly the cmask entries of its block, nothing else.
-// 6 B per instance instead of the reference's 24 B + sort temp.
-struct BinLayout {
-    size_t point_list, bmask, cmask, total;
-    long long capacity;
-    __host__ __device__ BinLayout(long long cap) : capacity(cap) {
-        size_t off = 0;
-        point_list = off; off = align_up(off + (size_t)cap * 4, 256);
-        bmask = off;      off = align_up(off + (size_t)cap, 256);
-        cmask = off;      off = align_up(off + (size_t)cap, 256);
-        total = off;
-    }
-};
-// largest capacity (a multiple of 64 instances) whose layout fits in `bytes`; r3dg_raster_binning_bytes is its inverse
-inline __host__ long long bin_capacity_for_bytes(size_t bytes) { return bytes < 768 + 384 ? 0 : (long long)((bytes - 768) / 6 / 64 * 64); }
-inline __host__ size_t bin_bytes_for_capacity(long long cap) { return (size_t)((cap + 63) / 64 * 64) * 6 + 768; }
 
 // Relaxed GPU-scope accesses for the look-back descriptors (flag and value share one word, so no
 // further ordering is needed); `volatile` asm so that polling loops really re-load.

@@ -366,28 +366,25 @@ static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, cudaStream_t s
     else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false>>(p, tiles, stream);
 }
 
-int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl, const ImgLayout& il,
-                             char* bin, const BinLayout& bl, cudaStream_t stream, stage_mark_fn mark) {
-    char* geom = (char*)a.geom;
-    char* img = (char*)a.img;
+int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream,
+                             stage_mark_fn mark) {
     CompositeFwdParams p;
-    p.W = a.W; p.H = a.H; p.gx = (a.W + R3DG_TILE - 1) / R3DG_TILE; p.S = a.S; p.recf = gl.recf;
-    const int gy = (a.H + R3DG_TILE - 1) / R3DG_TILE;
-    p.ranges = (const uint2*)(img + il.ranges);
-    p.point_list = (const uint32_t*)(bin + bl.point_list);
-    p.bmask32 = (const uint32_t*)(bin + bl.bmask); p.cmask32 = (uint32_t*)(bin + bl.cmask);
-    p.header = (const GeomHeader*)(geom + gl.header);
-    p.tile_order = (const uint32_t*)(img + il.tile_order);
-    p.bwd_work = (uint32_t*)(img + il.bwd_work);
-    p.rec = (const float*)(geom + gl.rec);
+    p.W = a.W; p.H = a.H; p.gx = b.gx; p.S = a.S; p.recf = b.recf;
+    p.ranges = b.ranges;
+    p.point_list = b.point_list;
+    p.bmask32 = (const uint32_t*)b.bmask; p.cmask32 = (uint32_t*)b.cmask;
+    p.header = b.header;
+    p.tile_order = b.tile_order;
+    p.bwd_work = b.bwd_work;
+    p.rec = b.rec;
     p.bg = a.background;
-    p.final_T = (float*)(img + il.final_T);
-    p.n_contrib = (int*)(img + il.n_contrib);
+    p.final_T = b.final_T;
+    p.n_contrib = b.n_contrib;
     p.out_color = a.out_color; p.out_opacity = a.out_opacity; p.out_depth = a.out_depth;
     p.out_feature = a.out_feature; p.out_weights = a.out_weights;
     p.det_weights = a.deterministic ? (uint64_t*)a.det_work : nullptr;
     if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, (size_t)a.P * 8, stream));
-    const int tiles = p.gx * gy;
+    const int tiles = b.tiles;
     switch (num_groups(a.S)) {
         case 1: launch_fwd_ng<1>(p, tiles, stream); break;
         case 2: launch_fwd_ng<2>(p, tiles, stream); break;
@@ -413,7 +410,7 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl
         R3DG_CUDA_TRY(cudaMemsetAsync(a.out_surface_xyz, 0, 3 * HW * 4, stream));
     }
     if (a.n_contrib)   // the reference returns n_contrib as a view of imgBuffer (rasterize_points.cu:136-139)
-        R3DG_CUDA_TRY(cudaMemcpyAsync(a.n_contrib, img + il.n_contrib, HW * 4, cudaMemcpyDeviceToDevice, stream));
+        R3DG_CUDA_TRY(cudaMemcpyAsync(a.n_contrib, b.n_contrib, HW * 4, cudaMemcpyDeviceToDevice, stream));
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

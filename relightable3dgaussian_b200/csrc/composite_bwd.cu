@@ -429,31 +429,27 @@ static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, cudaStream_t s
     kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 
-int launch_composite_backward(const r3dg_raster_bwd_args& a, const GeomLayout& gl, const ImgLayout& il,
-                              char* bin, const BinLayout& bl, cudaStream_t stream) {
-    char* geom = (char*)a.geom;
-    char* img = (char*)a.img;
+int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
     CompositeBwdParams p;
-    p.W = a.W; p.H = a.H; p.gx = (a.W + R3DG_TILE - 1) / R3DG_TILE; p.S = a.S; p.recf = gl.recf;
+    p.W = a.W; p.H = a.H; p.gx = b.gx; p.S = a.S; p.recf = b.recf;
     p.backward_geometry = a.backward_geometry;
-    const int gy = (a.H + R3DG_TILE - 1) / R3DG_TILE;
-    p.ranges = (const uint2*)(img + il.ranges);
-    p.point_list = (const uint32_t*)(bin + bl.point_list); p.cmask32 = (const uint32_t*)(bin + bl.cmask);
-    p.header = (const GeomHeader*)(geom + gl.header);
-    p.cta_order = (const uint32_t*)(img + il.bwd_order);
-    p.rec = (const float*)(geom + gl.rec);
+    p.ranges = b.ranges;
+    p.point_list = b.point_list; p.cmask32 = (const uint32_t*)b.cmask;
+    p.header = b.header;
+    p.cta_order = b.bwd_order;
+    p.rec = b.rec;
     p.bg = a.background;
-    p.final_T = (const float*)(img + il.final_T);
+    p.final_T = b.final_T;
     p.dL_dpix = a.dL_dout_color; p.dL_dpix_o = a.dL_dout_opacity; p.dL_dpix_d = a.dL_dout_depth;
     p.dL_dpix_f = a.dL_dout_feature;
-    p.grad = (float*)(geom + gl.grad);
-    p.n_contrib = (const int*)(img + il.n_contrib);
+    p.grad = b.grad;
+    p.n_contrib = b.n_contrib;
     const bool det = a.deterministic != 0;
-    p.det = det_acc(a.det_work, (size_t)a.P * gl.recf);
+    p.det = det_acc(a.det_work, (size_t)a.P * b.recf);
     if (det) R3DG_CUDA_TRY(cudaMemsetAsync(a.det_work, 0, det_bytes(p.det.n), stream));
-    else R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)a.P * gl.recf * 4, stream));
-    const int tiles = p.gx * gy;
-    int rc = launch_cta_order((const uint32_t*)(img + il.bwd_work), (uint32_t*)(img + il.bwd_order), 2 * tiles, stream);
+    else R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)a.P * b.recf * 4, stream));
+    const int tiles = b.tiles;
+    int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;
     switch (num_groups(a.S)) {
         case 1: det ? launch_bwd_ng<1, true>(p, tiles, stream) : launch_bwd_ng<1, false>(p, tiles, stream); break;

@@ -6,8 +6,29 @@
 
 namespace r3dg {
 
+// Typed views of the rasterizer's three caller-owned work buffers (regions described in api.cu, which alone knows
+// their byte layout and fills and size-checks this once per call) and the values derived from the call's shapes.
+struct RasterBuffers {
+    GeomHeader* header;                                                            // geom: per Gaussian
+    float *rec, *grad;
+    uint32_t* tiles_touched;
+    uint2 *rects, *brects;
+    uint8_t* clamped;
+    char* sort;                                                                    // laid out by sort_layout
+    SortLayout sort_layout{0};
+    float* final_T;                                                                // img: per pixel and per tile
+    int* n_contrib;
+    uint2* ranges;
+    uint32_t *tile_order, *bwd_work, *bwd_order, *slab_sum, *bin_matrix;
+    uint32_t* point_list;                                                          // binning: per instance
+    uint8_t *bmask, *cmask;
+    long long capacity;                                                            // instances the binning holds
+    int recf, gx, gy, tiles;
+    int chunk_len, chunks;                                                         // binning: depth-sorted runs
+};
+
 typedef void (*stage_mark_fn)(int, cudaStream_t);
-int launch_projection(const r3dg_raster_fwd_args& a, const GeomLayout& gl, cudaStream_t stream);
+int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream);
 int launch_point_offsets(int P, const uint32_t* tiles_touched, uint32_t* out, uint32_t* state,
                          GeomHeader* ticket_header, cudaStream_t stream);
 int launch_cta_order(const uint32_t* work, uint32_t* order, int n, cudaStream_t stream);
@@ -18,21 +39,15 @@ int launch_sort(void* geom_header, char* buf, const SortLayout& sl, long long n,
                 cudaStream_t stream);
 // binning.cu: depth sort + order-preserving tile binning -> point_list, bmask, zeroed cmask, ranges, num_rendered,
 // tile_order, zeroed bwd_work.  launch_empty_binning: the same per-tile outputs for P == 0 (all lists empty).
-int launch_binning(int P, int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
-                   char* bin, const BinLayout& bl, int num_sms, cudaStream_t stream, stage_mark_fn mark,
+int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stream, stage_mark_fn mark,
                    int* num_rendered_host, void* count_ready_event);
-int launch_empty_binning(int W, int H, char* geom, const GeomLayout& gl, char* img, const ImgLayout& il,
-                         cudaStream_t stream);
+int launch_empty_binning(const RasterBuffers& b, cudaStream_t stream);
 int launch_rebuild_keys(int T, const void* ranges, const uint32_t* point_list, const float* rec, int recf,
                         long long limit, uint64_t* keys, cudaStream_t stream);
-int launch_composite_forward(const r3dg_raster_fwd_args& a, const GeomLayout& gl,
-                             const ImgLayout& il, char* bin, const BinLayout& bl,
-                             cudaStream_t stream, stage_mark_fn mark);
-int launch_composite_backward(const r3dg_raster_bwd_args& a, const GeomLayout& gl,
-                              const ImgLayout& il, char* bin, const BinLayout& bl,
-                              cudaStream_t stream);
-int launch_projection_backward(const r3dg_raster_bwd_args& a, const GeomLayout& gl,
-                               cudaStream_t stream);
+int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream,
+                             stage_mark_fn mark);
+int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
+int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
 
 size_t bvh_build_tmp_bytes(int P);
 size_t bvh_packets_bytes(int P);

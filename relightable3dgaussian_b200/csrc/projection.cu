@@ -458,12 +458,11 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 }
 
 // ---- host launchers -----------------------------------------------------------------------
-int launch_projection(const r3dg_raster_fwd_args& a, const GeomLayout& gl, cudaStream_t stream) {
-    char* geom = (char*)a.geom;
+int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
     ProjParams p;
     p.P = a.P; p.S = a.S; p.D = a.D; p.M = a.M; p.W = a.W; p.H = a.H;
-    p.gx = (a.W + R3DG_TILE - 1) / R3DG_TILE; p.gy = (a.H + R3DG_TILE - 1) / R3DG_TILE;
-    p.recf = gl.recf; p.ng = num_groups(a.S);
+    p.gx = b.gx; p.gy = b.gy;
+    p.recf = b.recf; p.ng = num_groups(a.S);
     p.means3D = a.means3D; p.shs = a.shs; p.colors_precomp = a.colors_precomp; p.features = a.features;
     p.opacities = a.opacities; p.scales = a.scales; p.rotations = a.rotations; p.cov3D_precomp = a.cov3D_precomp;
     p.viewmatrix = a.viewmatrix; p.projmatrix = a.projmatrix; p.campos = a.campos;
@@ -471,16 +470,15 @@ int launch_projection(const r3dg_raster_fwd_args& a, const GeomLayout& gl, cudaS
     p.focal_y = a.H / (2.0f * a.tan_fovy);            // rasterizer_impl.cu:232-233
     p.focal_x = a.W / (2.0f * a.tan_fovx);
     p.prefiltered = a.prefiltered;
-    p.rec = (float*)(geom + gl.rec); p.tiles_touched = (uint32_t*)(geom + gl.tiles_touched);
-    p.clamped = (uint8_t*)(geom + gl.clamped); p.radii = a.radii; p.out_weights = a.out_weights;
-    p.header = (GeomHeader*)(geom + gl.header);
-    const SortLayout sl(a.P);
-    p.sort_keys = (uint32_t*)(geom + gl.sort + sl.keys_a);
-    p.sort_vals = (uint32_t*)(geom + gl.sort + sl.vals_a);
-    p.rects = (uint2*)(geom + gl.rects); p.brects = (uint2*)(geom + gl.brects);
+    p.rec = b.rec; p.tiles_touched = b.tiles_touched;
+    p.clamped = b.clamped; p.radii = a.radii; p.out_weights = a.out_weights;
+    p.header = b.header;
+    p.sort_keys = (uint32_t*)(b.sort + b.sort_layout.keys_a);
+    p.sort_vals = (uint32_t*)(b.sort + b.sort_layout.vals_a);
+    p.rects = b.rects; p.brects = b.brects;
     // dynamic shared memory: the SH slab (transposed fallback layout is the larger one), reused for the record slab
     size_t sh_smem = a.shs ? (size_t)3 * a.M * (PROJ_THREADS + 1) * sizeof(float) : 0;
-    const size_t rec_smem = (size_t)PROJ_THREADS * gl.recf * sizeof(float);
+    const size_t rec_smem = (size_t)PROJ_THREADS * b.recf * sizeof(float);
     if (rec_smem > sh_smem) sh_smem = rec_smem;
     project_kernel<<<(a.P + PROJ_THREADS - 1) / PROJ_THREADS, PROJ_THREADS, sh_smem, stream>>>(p);
     R3DG_CUDA_TRY(cudaGetLastError());

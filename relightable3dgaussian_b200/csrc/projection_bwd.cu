@@ -400,24 +400,21 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     *reinterpret_cast<float4*>(p.dL_drotations + 4 * (size_t)idx) = make_float4(drot[0], drot[1], drot[2], drot[3]);
 }
 
-int launch_projection_backward(const r3dg_raster_bwd_args& a, const GeomLayout& gl, cudaStream_t stream) {
-    char* geom = (char*)a.geom;
+int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
     ProjBwdParams p;
-    p.P = a.P; p.S = a.S; p.D = a.D; p.M = a.M; p.W = a.W; p.H = a.H; p.recf = gl.recf;
+    p.P = a.P; p.S = a.S; p.D = a.D; p.M = a.M; p.W = a.W; p.H = a.H; p.recf = b.recf;
     p.means3D = a.means3D; p.shs = a.shs; p.colors_precomp = a.colors_precomp; p.scales = a.scales;
     p.rotations = a.rotations; p.cov3D_precomp = a.cov3D_precomp; p.viewmatrix = a.viewmatrix;
     p.projmatrix = a.projmatrix; p.campos = a.campos;
     p.scale_modifier = a.scale_modifier; p.tan_fovx = a.tan_fovx; p.tan_fovy = a.tan_fovy;
     p.h_y = a.H / (2.0f * a.tan_fovy); p.h_x = a.W / (2.0f * a.tan_fovx);
-    p.radii_rec = (const int*)(geom + gl.tiles_touched);   // tiles_touched > 0  <=>  radii > 0
-    p.rec = (const float*)(geom + gl.rec);
-    p.grad = (const float*)(geom + gl.grad);
-    p.clamped = (const uint8_t*)(geom + gl.clamped);
+    p.radii_rec = (const int*)b.tiles_touched;   // tiles_touched > 0  <=>  radii > 0
+    p.rec = b.rec; p.grad = b.grad; p.clamped = b.clamped;
     p.dL_dmeans2D = a.dL_dmeans2D; p.dL_dcolors = a.dL_dcolors; p.dL_dopacity = a.dL_dopacity;
     p.dL_dmeans3D = a.dL_dmeans3D; p.dL_dfeatures = a.dL_dfeatures; p.dL_dcov3D = a.dL_dcov3D;
     p.dL_dsh = a.dL_dsh; p.dL_dscales = a.dL_dscales; p.dL_drotations = a.dL_drotations;
     p.dL_dsh_factor = a.dL_dsh_factor;
-    p.det = det_acc(a.det_work, (size_t)a.P * gl.recf);
+    p.det = det_acc(a.det_work, (size_t)a.P * b.recf);
     const size_t sh_smem = a.shs ? (size_t)3 * a.M * SLAB_LD * sizeof(float) : 0;
     const int blocks = (a.P + PROJ_THREADS - 1) / PROJ_THREADS;
     if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);

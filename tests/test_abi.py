@@ -118,7 +118,40 @@ def test_symbols_match_prototypes():
             assert _param_ok(ctype, bound), f"{name} argument {k}: header {ctype}, bound as {_ctype_name(bound)}"
 
 
-def test_sizing_functions_monotone_and_aligned():
+# Shapes at the edges of the work-buffer layout: P = 0 (sized as one Gaussian), record widths of one to nine float4
+# groups, images of one pixel, one tile row and more than 256 tile columns, capacities around the 64-instance granule.
+SIZING_P, SIZING_S = (0, 1, 1000, 10**6), (0, 5, 16, 24, 33)
+SIZING_WH = ((1, 1), (37, 1), (800, 800), (1920, 1080), (4100, 16))
+SIZING_CAP = (0, 1, 63, 64, 10**6)
+
+
+def _sizing(lib):
+    return {"geom": [lib.r3dg_raster_geom_bytes(P, S) for P in SIZING_P for S in SIZING_S],
+            "img": [lib.r3dg_raster_img_bytes(W, H) for W, H in SIZING_WH],
+            "n_contrib": [lib.r3dg_raster_img_n_contrib_offset(W, H) for W, H in SIZING_WH],
+            "binning": [lib.r3dg_raster_binning_bytes(c) for c in SIZING_CAP],
+            "fwd_det": [lib.r3dg_raster_fwd_det_bytes(P) for P in SIZING_P],
+            "bwd_det": [lib.r3dg_raster_bwd_det_bytes(P, S) for P in SIZING_P for S in SIZING_S]}
+
+
+# The sizes callers allocate: any change here is a change of the work-buffer layout.
+SIZING = {"geom": [11264, 11264, 11264, 11264, 11264,
+                   11264, 11264, 11264, 11264, 11264,
+                   142848, 174592, 270848, 334848, 398848,
+                   134010112, 166010112, 262010112, 326010112, 390010112],
+          "img": [6144, 14336, 15461376, 50338816, 1589248],
+          "n_contrib": [256, 256, 2560000, 8294400, 262400],
+          "binning": [1152, 1152, 1152, 1152, 6000768],
+          "fwd_det": [256, 256, 8192, 8000000],
+          "bwd_det": [768, 768, 1024, 1280, 1536,
+                      768, 768, 1024, 1280, 1536,
+                      291072, 388096, 679168, 873216, 1067008,
+                      291000064, 388000000, 679000064, 873000192, 1067000064]}
+# The same with R3DG_BIN_MAX_CHUNKS=3: only the binning matrix in the img buffer shrinks.
+SIZING_IMG_3_CHUNKS = [2048, 2048, 5251328, 17013248, 539648]
+
+
+def test_sizing_functions_monotone_and_aligned(monkeypatch):
     lib = _lib.load()
     g1, g2 = lib.r3dg_raster_geom_bytes(1000, 5), lib.r3dg_raster_geom_bytes(2000, 5)
     assert 0 < g1 < g2 and g1 % 256 == 0
@@ -129,6 +162,12 @@ def test_sizing_functions_monotone_and_aligned():
     assert 0 < off < i1 and off % 256 == 0
     b1, b2 = lib.r3dg_raster_binning_bytes(10_000), lib.r3dg_raster_binning_bytes(20_000)
     assert 4 * 10_000 <= b1 < b2          # one u32 list entry per (tile, Gaussian) instance
+    assert _sizing(lib) == SIZING
+    monkeypatch.setenv("R3DG_BIN_MAX_CHUNKS", "3")
+    assert _sizing(lib) == dict(SIZING, img=SIZING_IMG_3_CHUNKS)
+
+
+FAKE = 0x10000      # never dereferenced: every call below is refused before anything is enqueued
 
 
 def test_bad_arguments_are_rejected_without_touching_the_gpu():
@@ -141,6 +180,34 @@ def test_bad_arguments_are_rejected_without_touching_the_gpu():
     b = _lib.RasterBwdArgs()
     b.P, b.W, b.H, b.S = 10, 16, 16, 25           # backward.cu:449 limit
     assert lib.r3dg_raster_backward(ctypes.byref(b), None) == -10002
+
+    # work buffers smaller than the sizing functions ask for; 1151 bytes of binning buffer hold no instance
+    P, S, W, H = 100, 5, 64, 48
+    short = (("geom_bytes", lib.r3dg_raster_geom_bytes(P, S) - 1), ("img_bytes", lib.r3dg_raster_img_bytes(W, H) - 1),
+             ("binning_bytes", 1151))
+    for call, cls in ((lib.r3dg_raster_forward, _lib.RasterFwdArgs), (lib.r3dg_raster_backward, _lib.RasterBwdArgs)):
+        for field, size in short:
+            a = cls()
+            a.P, a.S, a.W, a.H = P, S, W, H
+            if cls is _lib.RasterFwdArgs:
+                a.colors_precomp = a.cov3D_precomp = FAKE
+            a.geom, a.geom_bytes = FAKE, lib.r3dg_raster_geom_bytes(P, S)
+            a.img, a.img_bytes = FAKE, lib.r3dg_raster_img_bytes(W, H)
+            a.binning, a.binning_bytes = FAKE, lib.r3dg_raster_binning_bytes(10_000)
+            setattr(a, field, size)
+            assert call(ctypes.byref(a), None) == -10001, (call.__name__, field)
+    b = _lib.RasterBwdArgs()
+    b.P, b.S, b.W, b.H = 0, S, W, H               # no Gaussians: nothing to do, the buffers are not needed
+    assert lib.r3dg_raster_backward(ctypes.byref(b), None) == 0
+
+    def debug_copy(id_, max_bytes, binning_bytes):
+        return lib.r3dg_raster_debug_copy(id_, P, S, W, H, FAKE, FAKE, FAKE, binning_bytes, FAKE, max_bytes, None)
+    for id_, row_bytes in ((0, 4), (1, 3), (3, 8), (5, 16), (6, 12), (8, 4)):
+        assert debug_copy(id_, row_bytes * P - 1, lib.r3dg_raster_binning_bytes(10_000)) == -1, id_
+    for id_ in (-1, 2, 11, 21):
+        assert debug_copy(id_, 1 << 20, lib.r3dg_raster_binning_bytes(10_000)) == -1, id_
+    for id_ in (9, 10, 18, 19):                   # the binning lists need a binning buffer
+        assert debug_copy(id_, 1 << 20, 0) == -1, id_
 
 
 def test_tune_keys_and_error_codes():
