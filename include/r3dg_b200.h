@@ -40,6 +40,12 @@ size_t r3dg_raster_binning_bytes(long long capacity);
 /* Byte offset of the int32 n_contrib[H,W] plane inside the image buffer: the reference returns
  * n_contrib as a view of imgBuffer (rasterize_points.cu:136-139) and so does the host glue. */
 size_t r3dg_raster_img_n_contrib_offset(int W, int H);
+/* The same for a call that renders V views (the `V` field below); V = 1 gives the sizes above.  The deterministic
+ * workspaces of such a call are r3dg_raster_fwd_det_bytes(V * P) and r3dg_raster_bwd_det_bytes(V * P, S). */
+size_t r3dg_raster_views_geom_bytes(int P, int S, int V);
+size_t r3dg_raster_views_img_bytes(int W, int H, int V);
+size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V);
+#define R3DG_MAX_VIEWS 64
 
 typedef struct r3dg_raster_fwd_args {
     int P, S, D, M, W, H;          /* Gaussians, feature channels, SH degree, SH coeffs, image */
@@ -81,6 +87,16 @@ typedef struct r3dg_raster_fwd_args {
      * a host that waits on this event instead of the stream gets the count while the compositor is still running and
      * can already enqueue what follows the forward.  NULL: not used. */
     void* count_ready_event;
+    /* Several views of the same Gaussians in one call.  V = 0 or 1: the single view described above.  With
+     * 1 < V <= R3DG_MAX_VIEWS: background [V,3], viewmatrix [V,16], projmatrix [V,16] and campos [V,3] hold one row per
+     * view; view_cams is a HOST array [V][4] of {tan_fovx, tan_fovy, cx, cy} (the scalar fields are not used); every
+     * image output gains a leading V (out_color [V,3,H,W], ..., n_contrib [V,H,W]), out_weights and radii are [V,P];
+     * num_rendered_host receives V ints, the instance count of each view (their sum > capacity = overflow).
+     * features_per_view / colors_per_view: features is [V,P,S] / colors_precomp is [V,P,3] (0: shared [P,...]).
+     * Every view's images are those of a one-view call with its camera.  V * P must stay below 2^30. */
+    int V;
+    const float* view_cams;
+    int features_per_view, colors_per_view;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_raster_fwd_det_bytes(P) bytes, zeroed by the call.  0 = the default path (det_work unused). */
@@ -128,6 +144,14 @@ typedef struct r3dg_raster_bwd_args {
     void* geom;   size_t geom_bytes;
     void* img;    size_t img_bytes;
     void* binning; size_t binning_bytes;
+    /* Several views (see r3dg_raster_fwd_args; the same V, camera rows, view_cams and per-view flags as the forward).
+     * The cotangents are [V,...]; dL_dmeans2D is [V,P,3]; dL_dfeatures / dL_dcolors are [V,P,*] when the input was per
+     * view.  Every other gradient is the sum over the views, accumulated in fp32 in view order (g_0 + g_1 + ...).
+     * With `shs`, dL_dsh_factor [V,P,3] is required: each view writes its rank-1 factor there and dL_dsh is rebuilt
+     * from the factors (r3dg_sh_grad_from_factors, scale 1). */
+    int V;
+    const float* view_cams;
+    int features_per_view, colors_per_view;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_raster_bwd_det_bytes(P, S) bytes, zeroed by the call.  0 = the default path (det_work unused). */

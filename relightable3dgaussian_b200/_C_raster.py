@@ -311,3 +311,162 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
     if rc < 0:
         raise RuntimeError(f"debug_intermediate({name}) failed: {rc}")
     return out
+
+
+# ---- several views of the same Gaussians in one call (r3dg_raster_forward / _backward with V > 1) ----------------------
+_views_capacity = {}     # (device, P, W, H, V) -> binning capacity that held the last call of that shape
+
+
+def _view_cams(cams):
+    """Host table [V][4] {tan_fovx, tan_fovy, cx, cy} (kept alive by the caller until the call is enqueued)."""
+    flat = [float(x) for c in cams for x in c]
+    return (ctypes.c_float * len(flat))(*flat)
+
+
+def rasterize_views(background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+                    viewmatrix, projmatrix, cams, image_height, image_width, sh, degree, campos, prefiltered,
+                    computer_pseudo_normal, _min_capacity=None):
+    """V views of one set of Gaussians in one forward.  background [V,3], viewmatrix / projmatrix [V,4,4], campos [V,3],
+    cams: V tuples (tan_fovx, tan_fovy, cx, cy); features [P,S] or [V,P,S], colors [P,3] or [V,P,3] (or empty).
+    Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
+    out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
+    radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once."""
+    lib = _lib.load()
+    V = len(cams)
+    P = means3D.size(0)
+    S = features.size(-1)
+    H, W = int(image_height), int(image_width)
+    dev = means3D.device
+    features_pv = features.dim() == 3
+    colors_pv = colors is not None and colors.numel() != 0 and colors.dim() == 3
+    means3D = _prep(means3D, "means3D")
+    features = _prep(features, "features"); colors = _prep(colors, "colors")
+    opacity = _prep(opacity, "opacity"); scales = _prep(scales, "scales")
+    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
+    sh = _prep(sh, "sh"); background = _prep(background, "background")
+    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
+    campos = _prep(campos, "campos")
+    M = sh.size(1) if sh.numel() != 0 else 0
+
+    f32 = dict(dtype=torch.float32, device=dev)
+    out_color = torch.empty((V, 3, H, W), **f32)
+    out_opacity = torch.empty((V, 1, H, W), **f32)
+    out_depth = torch.empty((V, 1, H, W), **f32)
+    out_feature = torch.empty((V, S, H, W), **f32)
+    out_normal = torch.empty((V, 3, H, W), **f32)
+    out_surface_xyz = torch.empty((V, 3, H, W), **f32)
+    out_weights = torch.empty((V, P, 1), **f32)
+    radii = torch.empty((V, P), dtype=torch.int32, device=dev)
+    geomBuffer = torch.empty((lib.r3dg_raster_views_geom_bytes(P, S, V),), dtype=torch.uint8, device=dev)
+    imgBuffer = torch.empty((lib.r3dg_raster_views_img_bytes(W, H, V),), dtype=torch.uint8, device=dev)
+    key = (dev.index if dev.index is not None else torch.cuda.current_device(), P, W, H, V)
+    capacity = int(_min_capacity) if _min_capacity is not None else max(_views_capacity.get(key, 0), 4 * V * P + 4096)
+    table = _view_cams(cams)
+    a = _lib.RasterFwdArgs()
+    a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
+    a.V, a.view_cams = V, ctypes.cast(table, ctypes.c_void_p)
+    a.features_per_view, a.colors_per_view = int(features_pv), int(colors_pv)
+    a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
+    a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.opacities = _lib.ptr(opacity)
+    a.scales = _lib.ptr(scales); a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
+    a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
+    a.scale_modifier = float(scale_modifier); a.tan_fovx, a.tan_fovy, a.cx, a.cy = (float(x) for x in cams[0])
+    a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
+    a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
+    a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
+    a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
+    a.out_weights = _lib.ptr(out_weights); a.radii = _lib.ptr(radii); a.n_contrib = None
+    a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
+    a.img = imgBuffer.data_ptr(); a.img_bytes = imgBuffer.numel()
+    det_ws = _lib.det_workspace(a, lib.r3dg_raster_fwd_det_bytes(V * P), dev)
+    pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
+    a.num_rendered_host = pinned.data_ptr()
+    stream = torch.cuda.current_stream(dev)
+    while True:
+        binningBuffer = torch.empty((lib.r3dg_raster_binning_bytes(capacity),), dtype=torch.uint8, device=dev)
+        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        a.count_ready_event = ev.cuda_event
+        _lib.call("r3dg_raster_forward", dev, ctypes.byref(a), what="rasterize_views")
+        ev.synchronize()                  # the one read-back: the V counts, after the last view's binning offsets
+        rendered = [int(x) for x in pinned.tolist()]
+        if sum(rendered) <= capacity:
+            break
+        capacity = int(sum(rendered) * 1.25) + 4096   # speculation missed: rerun with room to spare
+    _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
+    off = lib.r3dg_raster_views_img_n_contrib_offset(W, H, V)
+    n_contrib = imgBuffer[off:off + 4 * V * H * W].view(torch.int32).view(V, H, W)
+    return (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
+            out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer)
+
+
+def rasterize_views_backward(background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
+                             viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
+                             dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
+                             backward_geometry):
+    """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
+    dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
+    input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
+    in view order; dL_dsh is rebuilt from the views' rank-1 factors."""
+    lib = _lib.load()
+    V = len(cams)
+    P = means3D.size(0)
+    S = features.size(-1)
+    H, W = dL_dout_color.size(2), dL_dout_color.size(3)
+    dev = means3D.device
+    features_pv = features.dim() == 3
+    colors_pv = colors is not None and colors.numel() != 0 and colors.dim() == 3
+    means3D = _prep(means3D, "means3D"); features = _prep(features, "features")
+    colors = _prep(colors, "colors"); scales = _prep(scales, "scales")
+    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
+    sh = _prep(sh, "sh"); background = _prep(background, "background")
+    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
+    campos = _prep(campos, "campos")
+    dL_dout_color = _prep(dL_dout_color, "dL_dout_color")
+    dL_dout_opacity = _prep(dL_dout_opacity, "dL_dout_opacity")
+    dL_dout_depth = _prep(dL_dout_depth, "dL_dout_depth")
+    dL_dout_feature = _prep(dL_dout_feature, "dL_dout_feature")
+    M = sh.size(1) if sh.numel() != 0 else 0
+
+    f32 = dict(dtype=torch.float32, device=dev)
+    dL_dmeans2D = torch.empty((V, P, 3), **f32)
+    dL_dmeans3D = torch.empty((P, 3), **f32)
+    dL_dfeatures = torch.empty((V, P, S) if features_pv else (P, S), **f32)
+    dL_dcolors = torch.empty((V, P, 3) if colors_pv else (P, 3), **f32)
+    dL_dopacity = torch.empty((P, 1), **f32)
+    dL_dcov3D = torch.empty((P, 6), **f32)
+    dL_dsh = torch.empty((P, M, 3), **f32)
+    sh_factor = torch.empty((V, P, 3), **f32) if M > 0 else None
+    dL_dscales = torch.empty((P, 3), **f32)
+    dL_drotations = torch.empty((P, 4), **f32)
+    if P != 0:
+        table = _view_cams(cams)
+        a = _lib.RasterBwdArgs()
+        a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
+        a.V, a.view_cams = V, ctypes.cast(table, ctypes.c_void_p)
+        a.features_per_view, a.colors_per_view = int(features_pv), int(colors_pv)
+        a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
+        a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.scales = _lib.ptr(scales)
+        a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
+        a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
+        a.scale_modifier = float(scale_modifier); a.tan_fovx, a.tan_fovy = float(cams[0][0]), float(cams[0][1])
+        a.backward_geometry = int(bool(backward_geometry)); a.debug = 0
+        a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
+        a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
+        a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
+        a.dL_dopacity = _lib.ptr(dL_dopacity); a.dL_dmeans3D = _lib.ptr(dL_dmeans3D)
+        a.dL_dfeatures = _lib.ptr(dL_dfeatures); a.dL_dcov3D = _lib.ptr(dL_dcov3D); a.dL_dsh = _lib.ptr(dL_dsh)
+        a.dL_dscales = _lib.ptr(dL_dscales); a.dL_drotations = _lib.ptr(dL_drotations)
+        a.dL_dsh_factor = _lib.ptr(sh_factor)
+        a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
+        a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
+        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
+        det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(V * P, S), dev)
+        _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_views_backward")
+    else:
+        for t in (dL_dmeans2D, dL_dmeans3D, dL_dfeatures, dL_dcolors, dL_dopacity, dL_dcov3D, dL_dsh, dL_dscales,
+                  dL_drotations):
+            t.zero_()
+    return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
+            dL_dscales, dL_drotations)

@@ -30,6 +30,7 @@ class RasterFwdArgs(ctypes.Structure):
                                  "n_contrib")] +
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
          ("binning", c_void_p), ("binning_bytes", c_size_t), ("num_rendered_host", c_void_p), ("count_ready_event", c_void_p),
+         ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
          ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -47,6 +48,7 @@ class RasterBwdArgs(ctypes.Structure):
                                  "dL_dscales", "dL_drotations", "dL_dsh_factor")] +
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
          ("binning", c_void_p), ("binning_bytes", c_size_t),
+         ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
          ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -100,6 +102,9 @@ SYMBOLS = [
     ("r3dg_raster_img_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_raster_binning_bytes", c_size_t, [c_ll]),
     ("r3dg_raster_img_n_contrib_offset", c_size_t, [c_int, c_int]),
+    ("r3dg_raster_views_geom_bytes", c_size_t, [c_int, c_int, c_int]),
+    ("r3dg_raster_views_img_bytes", c_size_t, [c_int, c_int, c_int]),
+    ("r3dg_raster_views_img_n_contrib_offset", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_raster_forward", c_int, [ctypes.POINTER(RasterFwdArgs), c_void_p]),
     ("r3dg_raster_backward", c_int, [ctypes.POINTER(RasterBwdArgs), c_void_p]),
     ("r3dg_sh_grad_from_factors", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p]),

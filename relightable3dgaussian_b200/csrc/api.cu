@@ -40,38 +40,44 @@ inline void prof_mark(bool fwd, int i, cudaStream_t s) {
 }
 
 // ---- the rasterizer's work buffers: regions in this order, each 256-byte aligned ---------------------------------
+// V views: V rows per Gaussian (row v * P + g), one header and one depth-sort region per view.  V = 1 is the one-view
+// layout.
 struct GeomLayout {
-    size_t header, rec, tiles_touched, rects, brects, clamped, scan_state, sort, grad, total;
+    size_t header, rec, tiles_touched, rects, brects, clamped, scan_state, sort, sort_stride, grad, total;
     int recf;
     SortLayout sl;
-    GeomLayout(int P, int S) : recf(rec_floats(S)), sl(P) {
+    GeomLayout(int P, int S, int V = 1) : recf(rec_floats(S)), sl(P) {
+        const size_t R = (size_t)V * P;
+        sort_stride = align_up(sl.total, 256);
         size_t off = 0;
-        header = off;        off = align_up(off + sizeof(GeomHeader), 256);
-        rec = off;           off = align_up(off + (size_t)P * recf * 4, 256);
-        tiles_touched = off; off = align_up(off + (size_t)P * 4, 256);
-        rects = off;         off = align_up(off + (size_t)P * 8, 256);         // packed tile rectangles
-        brects = off;        off = align_up(off + (size_t)P * 8, 256);         // packed block rectangles (block_rect())
-        clamped = off;       off = align_up(off + (size_t)P, 256);
+        header = off;        off = align_up(off + V * sizeof(GeomHeader), 256);
+        rec = off;           off = align_up(off + R * recf * 4, 256);
+        tiles_touched = off; off = align_up(off + R * 4, 256);
+        rects = off;         off = align_up(off + R * 8, 256);                 // packed tile rectangles
+        brects = off;        off = align_up(off + R * 8, 256);                 // packed block rectangles (block_rect())
+        clamped = off;       off = align_up(off + R, 256);
         scan_state = off;    off = align_up(off + ((size_t)P / R3DG_SCAN_ITEMS + 2) * 4, 256);
-        sort = off;          off = align_up(off + sl.total, 256);               // depth sort of the Gaussians
-        grad = off;          off = align_up(off + (size_t)P * recf * 4, 256);   // backward scratch
+        sort = off;          off = align_up(off + V * sort_stride, 256);        // depth sort of the Gaussians, per view
+        grad = off;          off = align_up(off + R * recf * 4, 256);           // backward scratch
         total = off;
     }
 };
 
+// V views: V images stacked as one tall tile grid (view v owns tile rows [v * gy, (v + 1) * gy)); the binning scratch
+// (slab sums, count matrix) is per view and reused by the views one after the other.
 struct ImgLayout {
     size_t final_T, n_contrib, ranges, tile_order, bwd_work, bwd_order, slab_sum, bin_matrix, total;
     int gx, gy, max_chunks;
-    ImgLayout(int W, int H) : gx((W + R3DG_TILE - 1) / R3DG_TILE), gy((H + R3DG_TILE - 1) / R3DG_TILE) {
-        const size_t HW = (size_t)W * H, T = (size_t)gx * gy;
+    ImgLayout(int W, int H, int V = 1) : gx((W + R3DG_TILE - 1) / R3DG_TILE), gy((H + R3DG_TILE - 1) / R3DG_TILE) {
+        const size_t HW = (size_t)W * H * V, T = (size_t)gx * gy, VT = T * V;
         max_chunks = bin_max_chunks(T);
         size_t off = 0;
         final_T = off;   off = align_up(off + HW * 4, 256);
         n_contrib = off; off = align_up(off + HW * 4, 256);
-        ranges = off;    off = align_up(off + T * 8, 256);
-        tile_order = off; off = align_up(off + T * 4, 256);      // tiles by descending list length
-        bwd_work = off;  off = align_up(off + 2 * T * 4, 256);    // per half-tile CTA: entries its busiest warp composited (forward)
-        bwd_order = off; off = align_up(off + 2 * T * 4, 256);    // half-tile CTAs by descending bwd_work (backward launch order)
+        ranges = off;    off = align_up(off + VT * 8, 256);
+        tile_order = off; off = align_up(off + VT * 4, 256);      // tiles by descending list length
+        bwd_work = off;  off = align_up(off + 2 * VT * 4, 256);   // per half-tile CTA: entries its busiest warp composited (forward)
+        bwd_order = off; off = align_up(off + 2 * VT * 4, 256);  // half-tile CTAs by descending bwd_work (backward launch order)
         slab_sum = off;  off = align_up(off + T * 4 * ((R3DG_BIN_MAX_CHUNKS + 511) / 512), 256);   // per 512-chunk slab
         bin_matrix = off; off = align_up(off + ((size_t)max_chunks + 1) * T * 4, 256);   // + the row of list ends
         total = off;
@@ -104,9 +110,9 @@ size_t bin_bytes_for_capacity(long long cap) { return (size_t)((cap + 63) / 64 *
 // when a buffer is smaller than its layout or the binning buffer holds no instance, and fills `b` either way
 // (r3dg_raster_debug_copy passes SIZE_MAX for the sizes it is not given, and needs the binning only for some ids).
 int raster_buffers(int P, int S, int W, int H, void* geom_, size_t geom_bytes, void* img_, size_t img_bytes,
-                   void* bin_, size_t bin_bytes, RasterBuffers& b) {
-    const GeomLayout gl(P < 1 ? 1 : P, S);
-    const ImgLayout il(W, H);
+                   void* bin_, size_t bin_bytes, RasterBuffers& b, int V = 1) {
+    const GeomLayout gl(P < 1 ? 1 : P, S, V);
+    const ImgLayout il(W, H, V);
     const BinLayout bl(bin_capacity_for_bytes(bin_bytes));
     char *geom = (char*)geom_, *img = (char*)img_, *bin = (char*)bin_;
     b.header = (GeomHeader*)(geom + gl.header);
@@ -125,9 +131,34 @@ int raster_buffers(int P, int S, int W, int H, void* geom_, size_t geom_bytes, v
     b.recf = gl.recf; b.gx = il.gx; b.gy = il.gy; b.tiles = il.gx * il.gy;
     b.chunk_len = bin_chunk_len(P, il.max_chunks);          // one read of R3DG_BIN_MAX_CHUNKS sizes M and the chunks
     b.chunks = (P + b.chunk_len - 1) / b.chunk_len;
+    b.V = V; b.P = P; b.sort_stride = gl.sort_stride; b.row_base = 0; b.prev_header = nullptr;
     return geom_bytes < gl.total || img_bytes < il.total || bl.capacity < 1 ? R3DG_ERR_BAD_ARG : 0;
 }
+
+// views of one call: 1 for V = 0 or 1, V when 1 < V <= R3DG_MAX_VIEWS with the per-view camera table, 0 (refused)
+// otherwise; V * P below 2^30 keeps every row id and per-view count inside 32 bits with room to spare
+int views_of(int V, const float* view_cams, int P) {
+    if (V <= 1) return V < 0 ? 0 : 1;
+    if (V > R3DG_MAX_VIEWS || !view_cams || (long long)V * P >= (1LL << 30)) return 0;
+    return V;
+}
 }  // namespace
+
+RasterBuffers r3dg::view_slice(const RasterBuffers& b, int v) {
+    RasterBuffers s = b;
+    const size_t r = (size_t)v * b.P;
+    s.header = b.header + v;
+    s.rec = b.rec + r * b.recf; s.grad = b.grad + r * b.recf;
+    s.tiles_touched = b.tiles_touched + r;
+    s.rects = b.rects + r; s.brects = b.brects + r;
+    s.clamped = b.clamped + r;
+    s.sort = b.sort + (size_t)v * b.sort_stride;
+    s.ranges = b.ranges + (size_t)v * b.tiles;
+    s.row_base = (uint32_t)r;
+    s.prev_header = v > 0 ? b.header + v - 1 : nullptr;
+    if (b.V > 1) s.tile_order = nullptr;            // built once over the whole tall grid (launch_tile_order)
+    return s;
+}
 
 extern "C" {
 
@@ -137,6 +168,9 @@ size_t r3dg_raster_geom_bytes(int P, int S) { return GeomLayout(P < 1 ? 1 : P, S
 size_t r3dg_raster_img_bytes(int W, int H) { return ImgLayout(W, H).total; }
 size_t r3dg_raster_binning_bytes(long long capacity) { return bin_bytes_for_capacity(capacity < 1 ? 1 : capacity); }
 size_t r3dg_raster_img_n_contrib_offset(int W, int H) { return ImgLayout(W, H).n_contrib; }
+size_t r3dg_raster_views_geom_bytes(int P, int S, int V) { return GeomLayout(P < 1 ? 1 : P, S, V < 1 ? 1 : V).total; }
+size_t r3dg_raster_views_img_bytes(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).total; }
+size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).n_contrib; }
 size_t r3dg_raster_fwd_det_bytes(int P) { return align_up((size_t)(P < 1 ? 1 : P) * 8, 256); }
 size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S)); }
 
@@ -159,19 +193,33 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     if (a->P > 0 && ((a->shs == nullptr) == (a->colors_precomp == nullptr))) return R3DG_ERR_BAD_ARG;
     if (a->P > 0 && (a->cov3D_precomp == nullptr) && (a->scales == nullptr || a->rotations == nullptr)) return R3DG_ERR_BAD_ARG;
     if (a->shs && a->M > 16) return R3DG_ERR_UNSUPPORTED;
+    const int V = views_of(a->V, a->view_cams, a->P);
+    if (V == 0) return R3DG_ERR_BAD_ARG;
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
-                            a->binning_bytes, b);
+                            a->binning_bytes, b, V);
     if (rc != 0) return rc;
-    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(a->P))) return R3DG_ERR_BAD_ARG;
-    R3DG_CUDA_TRY(cudaMemsetAsync(b.header, 0, sizeof(GeomHeader), stream));
+    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(V * a->P))) return R3DG_ERR_BAD_ARG;
+    if (V > 1 && (b.gx > 65535 || b.gy > 65535 || b.tiles > 65535)) return R3DG_ERR_UNSUPPORTED;   // the binning's limits, before any launch
+    R3DG_CUDA_TRY(cudaMemsetAsync(b.header, 0, V * sizeof(GeomHeader), stream));
     auto mark = [](int i, cudaStream_t s) { prof_mark(true, i, s); };
+    auto no_mark = [](int, cudaStream_t) {};
     prof_mark(true, 0, stream);
     if (a->P > 0) {
-        if ((rc = launch_projection(*a, b, stream)) != 0) return rc;
-        prof_mark(true, 1, stream);
-        if ((rc = launch_binning(a->P, b, num_sms(), stream, mark, a->num_rendered_host, a->count_ready_event)) != 0) return rc;
-        g_launches += 1 + (1 + R3DG_SORT_MAX_PASSES) + 4;   // project; histogram + radix passes; count, colsum + starts, apply, scatter
+        // V views: every view is projected, depth-sorted and binned on its own (the binning appends its lists behind the
+        // previous view's in the one binning buffer); the compositors then run once over the tall grid of all views.
+        // The stage marks of the front end are those of the last view: the earlier views' binning counts as projection.
+        for (int v = 0; v < V; ++v) {
+            const RasterBuffers s = view_slice(b, v);
+            const bool last = v == V - 1;
+            if ((rc = launch_projection(*a, s, v, stream)) != 0) return rc;
+            if (last) prof_mark(true, 1, stream);
+            if ((rc = launch_binning(a->P, s, num_sms(), stream, last ? (stage_mark_fn)mark : (stage_mark_fn)no_mark,
+                                     a->num_rendered_host ? a->num_rendered_host + v : nullptr,
+                                     last ? a->count_ready_event : nullptr)) != 0) return rc;
+        }
+        if (V > 1 && (rc = launch_tile_order(b, stream)) != 0) return rc;
+        g_launches += V * (1 + (1 + R3DG_SORT_MAX_PASSES) + 4) + (V > 1 ? 1 : 0);   // per view: project; histogram + radix passes; count, colsum + starts, apply, scatter; tile order
     } else {
         if ((rc = launch_empty_binning(b, stream)) != 0) return rc;
         for (int i = 1; i <= 4; ++i) prof_mark(true, i, stream);
@@ -180,10 +228,11 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     prof_mark(true, 5, stream);
     if ((rc = launch_composite_forward(*a, b, stream, mark)) != 0) return rc;
     prof_mark(true, 7, stream);
-    g_launches += 1 + (a->computer_pseudo_normal ? 1 : 0) + (a->deterministic && a->P > 0 ? 1 : 0);   // composite, normals, weights
+    g_launches += 1 + (a->computer_pseudo_normal ? V : 0) + (a->deterministic && a->P > 0 ? 1 : 0);   // composite, normals, weights
     if (g_prof.on) g_prof.fwd_calls++;
-    if (a->P == 0) {      // (P > 0: the count was written, and the event recorded, as soon as the binning offsets existed)
-        if (a->num_rendered_host) R3DG_CUDA_TRY(cudaMemcpyAsync(a->num_rendered_host, b.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    if (a->P == 0) {      // (P > 0: the counts were written, and the event recorded, as soon as the binning offsets existed)
+        for (int v = 0; v < V && a->num_rendered_host; ++v)
+            R3DG_CUDA_TRY(cudaMemcpyAsync(a->num_rendered_host + v, b.header + v, sizeof(int), cudaMemcpyDeviceToHost, stream));
         if (a->count_ready_event) R3DG_CUDA_TRY(cudaEventRecord((cudaEvent_t)a->count_ready_event, stream));
     }
     if (a->debug) {   // reference CHECK_CUDA semantics (auxiliary.h:166-173): sync and report
@@ -197,18 +246,28 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!a || a->P < 0 || a->W <= 0 || a->H <= 0 || a->S < 0) return R3DG_ERR_BAD_ARG;
     if (a->S > R3DG_MAX_S_BWD) return R3DG_ERR_UNSUPPORTED;
-    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(a->P, a->S))) return R3DG_ERR_BAD_ARG;
+    const int V = views_of(a->V, a->view_cams, a->P);
+    if (V == 0) return R3DG_ERR_BAD_ARG;
+    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S))) return R3DG_ERR_BAD_ARG;
+    if (V > 1 && a->P > 0 && a->shs && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     if (a->P == 0) return 0;
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
-                            a->binning_bytes, b);
+                            a->binning_bytes, b, V);
     if (rc != 0) return rc;
     prof_mark(false, 8, stream);
     if ((rc = launch_composite_backward(*a, b, stream)) != 0) return rc;
     prof_mark(false, 9, stream);
-    if ((rc = launch_projection_backward(*a, b, stream)) != 0) return rc;
+    // one projection backward per view, in view order: view 0 writes the summed gradients, every later view adds its
+    // own to them (a left fold in fp32), per-view outputs go to the view's rows
+    for (int v = 0; v < V; ++v)
+        if ((rc = launch_projection_backward(*a, view_slice(b, v), v, stream)) != 0) return rc;
+    if (V > 1 && a->shs) {          // dL_dsh from the views' rank-1 factors, views in order
+        if ((rc = r3dg_sh_grad_from_factors(a->P, a->D, a->M, V, a->means3D, a->campos, a->dL_dsh_factor, 1.0f, a->dL_dsh,
+                                            stream_)) != 0) return rc;
+    }
     prof_mark(false, 10, stream);
-    g_launches += 3;   // CTA order, composite, projection
+    g_launches += 2 + V;   // CTA order, composite, projection per view (the SH rebuild counts itself)
     if (g_prof.on) g_prof.bwd_calls++;
     if (a->debug) {
         cudaError_t e = cudaStreamSynchronize(stream);

@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
     const uint32_t* __restrict__ vals_a,
     const uint32_t* __restrict__ vals_b, const uint2* __restrict__ rects, const uint2* __restrict__ brects,
     const uint32_t* __restrict__ M, uint32_t* __restrict__ point_list, uint8_t* __restrict__ bmask,
-    uint8_t* __restrict__ cmask, long long capacity, int starts_in_smem) {
+    uint8_t* __restrict__ cmask, long long capacity, int starts_in_smem, uint32_t row_base) {
     extern __shared__ __align__(16) uint32_t bin_smem[];
     const size_t T4 = ((size_t)T + 3) & ~(size_t)3;
     uint32_t* a = bin_smem;                               // [T] counts -> exclusive offsets -> cursors
@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
             const long long pos = (long long)base + rank;
             if (pos < capacity) {
                 const uint32_t seq = e & 0xffffu;
-                point_list[pos] = s_id[seq];
+                point_list[pos] = row_base + s_id[seq];                 // the view's rows start at row_base
                 const uint32_t ty = tile_row(t, gx_inv);
                 bmask[pos] = (uint8_t)block_mask_of_rect(s_br[seq], 2u * ((uint32_t)t - ty * (uint32_t)gx), 4u * ty);
                 cmask[pos] = 0;
@@ -252,7 +252,7 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
                     const uint32_t rank = bp[sq >> 5] + (uint32_t)__popc(bm[sq >> 5] & ((1u << (sq & 31u)) - 1u));
                     const long long pos = (long long)base + rank;
                     if (pos < capacity) {
-                        point_list[pos] = s_id[sq];
+                        point_list[pos] = row_base + s_id[sq];
                         bmask[pos] = (uint8_t)block_mask_of_rect(s_br[sq], c0, r0);
                         cmask[pos] = 0;
                     }
@@ -279,13 +279,15 @@ __global__ void __launch_bounds__(BIN_SCATTER_THREADS) bin_scatter_kernel(
 #define BIN_SLAB (32 * BIN_G)
 
 __device__ __forceinline__ void bin_starts_cta(int T, int slabs, uint32_t* __restrict__ slab_sum, uint2* ranges,
-                                               GeomHeader* header, long long capacity, uint32_t* __restrict__ tile_order,
-                                               uint32_t* __restrict__ bwd_work, volatile int* count_host);
+                                               GeomHeader* header, const GeomHeader* prev, long long capacity,
+                                               uint32_t* __restrict__ tile_order, uint32_t* __restrict__ bwd_work,
+                                               volatile int* count_host);
 
 __global__ void __launch_bounds__(1024) bin_colsum_kernel(int T, int chunks, int slabs, const uint32_t* __restrict__ M,
                                                           uint32_t* __restrict__ slab_sum, uint2* ranges, GeomHeader* header,
-                                                          long long capacity, uint32_t* __restrict__ tile_order,
-                                                          uint32_t* __restrict__ bwd_work, volatile int* count_host) {
+                                                          const GeomHeader* prev, long long capacity,
+                                                          uint32_t* __restrict__ tile_order, uint32_t* __restrict__ bwd_work,
+                                                          volatile int* count_host) {
     __shared__ uint32_t s[32][33];
     __shared__ bool s_last;
     const int tx = threadIdx.x, gy = threadIdx.y;
@@ -311,7 +313,7 @@ __global__ void __launch_bounds__(1024) bin_colsum_kernel(int T, int chunks, int
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    bin_starts_cta(T, slabs, slab_sum, ranges, header, capacity, tile_order, bwd_work, count_host);
+    bin_starts_cta(T, slabs, slab_sum, ranges, header, prev, capacity, tile_order, bwd_work, count_host);
 }
 
 // Longest-processing-time-first order of the tiles for the compositors: the CTAs of the heavy
@@ -352,14 +354,18 @@ __device__ __forceinline__ void tile_order_cta(int T, const uint2* ranges, uint3
     }
 }
 
-// Empty tiles stay (0,0) like the reference's zero-initialised imgState.ranges.  With slabs == 0 (P == 0) every
+// Empty tiles stay (0,0) like the reference's zero-initialised imgState.ranges.  prev: the previous view's header when
+// several views share the binning buffer (this view's lists start where that view's end), else null.  tile_order null:
+// the tile order is built later over all views (launch_tile_order).  With slabs == 0 (P == 0) every
 // list is empty: ranges (0,0), R = 0, and the tile order of all-empty tiles.  count_host: the caller's page-locked
 // host word for R, written straight from here (no copy in the stream between here and the scatter), or null.
 // One CTA of 1024 threads (1-D or 32 x 32); slab_sum is read through L2 (other CTAs wrote it).
 __device__ __forceinline__ void bin_starts_cta(int T, int slabs, uint32_t* __restrict__ slab_sum, uint2* ranges,
-                                               GeomHeader* header, long long capacity, uint32_t* __restrict__ tile_order,
-                                               uint32_t* __restrict__ bwd_work, volatile int* count_host) {
+                                               GeomHeader* header, const GeomHeader* prev, long long capacity,
+                                               uint32_t* __restrict__ tile_order, uint32_t* __restrict__ bwd_work,
+                                               volatile int* count_host) {
     __shared__ uint32_t s_warp[32];
+    const uint32_t base = prev ? __ldcg(&prev->list_base) + __ldcg(&prev->num_rendered) : 0u;
     const int tid = threadIdx.x + blockDim.x * threadIdx.y, lane = tid & 31, warp = tid >> 5;
     const int per = (T + 1023) / 1024;
     const int t0 = min(T, tid * per), t1 = min(T, t0 + per);
@@ -379,11 +385,12 @@ __device__ __forceinline__ void bin_starts_cta(int T, int slabs, uint32_t* __res
         s_warp[lane] = wi - wv;
         if (lane == 31) {
             header->num_rendered = wi;
+            header->list_base = base;
             if (count_host) *count_host = (int)wi;        // fenced after the ranges, by this thread
         }
     }
     __syncthreads();
-    uint32_t run = s_warp[warp] + inc - sum;
+    uint32_t run = base + s_warp[warp] + inc - sum;
     for (int t = t0; t < t1; ++t) {
         uint32_t n = 0;
         for (int k = 0; k < slabs; ++k) { const uint32_t v = __ldcg(slab_sum + (size_t)k * T + t); slab_sum[(size_t)k * T + t] = run + n; n += v; }
@@ -395,13 +402,19 @@ __device__ __forceinline__ void bin_starts_cta(int T, int slabs, uint32_t* __res
     // R reaches the host before the kernel counts as complete (by now the store has mostly travelled)
     if (count_host && tid == 31) __threadfence_system();
     __syncthreads();                                      // every range written above is visible to the whole CTA
+    if (tile_order) tile_order_cta(T, ranges, tile_order, bwd_work);
+}
+
+// Several views: the tile order of the tall grid, over the ranges every view's bin_starts wrote.
+__global__ void __launch_bounds__(1024) tile_order_kernel(int T, const uint2* ranges, uint32_t* __restrict__ tile_order,
+                                                          uint32_t* __restrict__ bwd_work) {
     tile_order_cta(T, ranges, tile_order, bwd_work);
 }
 
 // P == 0: every list empty (ranges (0,0), R = 0) and the tile order of all-empty tiles, by the same routine.
 __global__ void __launch_bounds__(1024) bin_starts_kernel(int T, uint2* ranges, GeomHeader* header,
                                                           uint32_t* __restrict__ tile_order, uint32_t* __restrict__ bwd_work) {
-    bin_starts_cta(T, 0, nullptr, ranges, header, 0, tile_order, bwd_work, nullptr);
+    bin_starts_cta(T, 0, nullptr, ranges, header, nullptr, 0, tile_order, bwd_work, nullptr);
 }
 
 __global__ void __launch_bounds__(1024) bin_apply_kernel(int T, int chunks, uint32_t* __restrict__ M,
@@ -497,8 +510,8 @@ int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stre
         else
             cudaGetLastError();                           // clear the query's error state
     }
-    bin_colsum_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, slabs, M, b.slab_sum, b.ranges, b.header, b.capacity,
-                                                    b.tile_order, b.bwd_work, count_host);
+    bin_colsum_kernel<<<sgrid, sblock, 0, stream>>>(T, chunks, slabs, M, b.slab_sum, b.ranges, b.header, b.prev_header,
+                                                    b.capacity, b.tile_order, b.bwd_work, count_host);
     if (num_rendered_host && !count_host)
         R3DG_CUDA_TRY(cudaMemcpyAsync(num_rendered_host, b.header, sizeof(int), cudaMemcpyDeviceToHost, stream));
     if (count_ready_event) R3DG_CUDA_TRY(cudaEventRecord((cudaEvent_t)count_ready_event, stream));
@@ -506,13 +519,19 @@ int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stre
     mark(4, stream);
     bin_scatter_kernel<<<chunks, BIN_SCATTER_THREADS, smem_scatter, stream>>>(
         P, T, gx, (1ull << 32) / (unsigned long long)gx + 1ull, CH, cap, b.header, va, vb, b.rects, b.brects, M, b.point_list,
-        b.bmask, b.cmask, b.capacity, starts_in_smem);
+        b.bmask, b.cmask, b.capacity, starts_in_smem, b.row_base);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
 int launch_empty_binning(const RasterBuffers& b, cudaStream_t stream) {
-    bin_starts_kernel<<<1, 1024, 0, stream>>>(b.tiles, b.ranges, b.header, b.tile_order, b.bwd_work);
+    bin_starts_kernel<<<1, 1024, 0, stream>>>(b.V * b.tiles, b.ranges, b.header, b.tile_order, b.bwd_work);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int launch_tile_order(const RasterBuffers& b, cudaStream_t stream) {
+    tile_order_kernel<<<1, 1024, 0, stream>>>(b.V * b.tiles, b.ranges, b.tile_order, b.bwd_work);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

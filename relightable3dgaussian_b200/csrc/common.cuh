@@ -37,7 +37,8 @@ struct GeomHeader {               // first 256 bytes of the geometry buffer
     uint32_t depth_nor;           // OR of their complements: bit varies across keys iff set in both
     uint32_t sort_exec;           // number of radix passes actually executed (parity = result buffer)
     uint32_t bin_ticket;          // CTAs of bin_colsum done (the last one scans the tile totals)
-    uint32_t pad[50];
+    uint32_t list_base;           // first binning slot of this view's lists (several views share one binning buffer)
+    uint32_t pad[49];
 };
 static_assert(sizeof(GeomHeader) == 256, "header size");
 

@@ -29,7 +29,7 @@
 namespace r3dg {
 
 struct CompositeFwdParams {
-    int W, H, gx, S, recf;
+    int W, H, gx, gy, S, recf;   // gy: tile rows of one view; view v of a several-view call owns rows [v gy, (v+1) gy)
     const uint2* ranges;
     const uint32_t* point_list;  // per-tile depth-sorted Gaussian ids (binning.cu)
     const uint32_t* bmask32;     // per-instance block-touch masks (bin_scatter), viewed as words of 4 instances
@@ -72,7 +72,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
     constexpr int PARTS = 8 / NW;
     const int tile = (int)p.tile_order[blockIdx.x / PARTS];
     const int wb = (blockIdx.x % PARTS) * NW + warp;          // pixel block 0..7 inside the tile
-    const int tx = tile % p.gx, ty = tile / p.gx;
+    const int tx = tile % p.gx, tyv = tile / p.gx;
+    const int view = tyv / p.gy, ty = tyv - view * p.gy;          // the view's image and its view-local tile row
     const int bx0 = tx * R3DG_TILE + (wb & 1) * 8, by0 = ty * R3DG_TILE + (wb >> 1) * 4;
     const int px = bx0 + (lane & 7), py = by0 + (lane >> 3);
     const bool inside = px < p.W && py < p.H;
@@ -260,16 +261,16 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
     }
     if (lane == 0 && composited) atomicMax(&p.bwd_work[blockIdx.x % PARTS + PARTS * tile], composited);
     if (inside) {
-        const size_t HW = (size_t)p.H * p.W, pix = (size_t)p.W * py + px;
-        p.final_T[pix] = T;
-        p.n_contrib[pix] = (int)last_contributor;
+        const size_t HW = (size_t)p.H * p.W, pix = (size_t)p.W * py + px, vpix = (size_t)view * HW + pix;
+        p.final_T[vpix] = T;
+        p.n_contrib[vpix] = (int)last_contributor;
 #pragma unroll
-        for (int ch = 0; ch < 3; ++ch) p.out_color[ch * HW + pix] = fma_(p.bg[ch], T, C[ch]);
+        for (int ch = 0; ch < 3; ++ch) p.out_color[(size_t)(3 * view + ch) * HW + pix] = fma_(p.bg[3 * view + ch], T, C[ch]);
 #pragma unroll
         for (int ch = 3; ch < 4 * NG; ++ch)
-            if (ch - 3 < p.S) p.out_feature[(size_t)(ch - 3) * HW + pix] = C[ch];
-        p.out_depth[pix] = Dp;
-        p.out_opacity[pix] = Op;
+            if (ch - 3 < p.S) p.out_feature[((size_t)view * p.S + (ch - 3)) * HW + pix] = C[ch];
+        p.out_depth[vpix] = Dp;
+        p.out_opacity[vpix] = Op;
     }
 }
 
@@ -369,7 +370,8 @@ static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, cudaStream_t s
 int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream,
                              stage_mark_fn mark) {
     CompositeFwdParams p;
-    p.W = a.W; p.H = a.H; p.gx = b.gx; p.S = a.S; p.recf = b.recf;
+    const int V = b.V;
+    p.W = a.W; p.H = a.H; p.gx = b.gx; p.gy = b.gy; p.S = a.S; p.recf = b.recf;
     p.ranges = b.ranges;
     p.point_list = b.point_list;
     p.bmask32 = (const uint32_t*)b.bmask; p.cmask32 = (uint32_t*)b.cmask;
@@ -383,8 +385,9 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
     p.out_color = a.out_color; p.out_opacity = a.out_opacity; p.out_depth = a.out_depth;
     p.out_feature = a.out_feature; p.out_weights = a.out_weights;
     p.det_weights = a.deterministic ? (uint64_t*)a.det_work : nullptr;
-    if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, (size_t)a.P * 8, stream));
-    const int tiles = b.tiles;
+    const size_t rows = (size_t)V * a.P;
+    if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, rows * 8, stream));
+    const int tiles = V * b.tiles;                    // the tall grid of all views
     switch (num_groups(a.S)) {
         case 1: launch_fwd_ng<1>(p, tiles, stream); break;
         case 2: launch_fwd_ng<2>(p, tiles, stream); break;
@@ -397,20 +400,25 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
         case 9: launch_fwd_ng<9>(p, tiles, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;
     }
-    if (p.det_weights && a.P > 0) det_weights_kernel<<<(a.P + 255) / 256, 256, 0, stream>>>(a.P, p.det_weights, a.out_weights);
+    if (p.det_weights && a.P > 0) det_weights_kernel<<<(int)((rows + 255) / 256), 256, 0, stream>>>((int)rows, p.det_weights, a.out_weights);
     const size_t HW = (size_t)a.H * a.W;
     mark(6, stream);
     if (a.computer_pseudo_normal) {
-        const float focal_y = a.H / (2.0f * a.tan_fovy), focal_x = a.W / (2.0f * a.tan_fovx);
-        dim3 grid((a.W + 31) / 32, (a.H + 7) / 8);
-        surface_normal_kernel<<<grid, 256, 0, stream>>>(a.W, a.H, a.viewmatrix, focal_x, focal_y, a.cx, a.cy,
-                                                        a.out_opacity, a.out_depth, a.out_normal, a.out_surface_xyz);
+        for (int v = 0; v < V; ++v) {                 // each view with its own intrinsics
+            float tan_fovx = a.tan_fovx, tan_fovy = a.tan_fovy, cx = a.cx, cy = a.cy;
+            view_cam(V, a.view_cams, v, tan_fovx, tan_fovy, cx, cy);
+            const float focal_y = a.H / (2.0f * tan_fovy), focal_x = a.W / (2.0f * tan_fovx);
+            dim3 grid((a.W + 31) / 32, (a.H + 7) / 8);
+            surface_normal_kernel<<<grid, 256, 0, stream>>>(a.W, a.H, a.viewmatrix + 16 * v, focal_x, focal_y, cx, cy,
+                                                            a.out_opacity + v * HW, a.out_depth + v * HW,
+                                                            a.out_normal + 3 * v * HW, a.out_surface_xyz + 3 * v * HW);
+        }
     } else {
-        R3DG_CUDA_TRY(cudaMemsetAsync(a.out_normal, 0, 3 * HW * 4, stream));
-        R3DG_CUDA_TRY(cudaMemsetAsync(a.out_surface_xyz, 0, 3 * HW * 4, stream));
+        R3DG_CUDA_TRY(cudaMemsetAsync(a.out_normal, 0, 3 * V * HW * 4, stream));
+        R3DG_CUDA_TRY(cudaMemsetAsync(a.out_surface_xyz, 0, 3 * V * HW * 4, stream));
     }
     if (a.n_contrib)   // the reference returns n_contrib as a view of imgBuffer (rasterize_points.cu:136-139)
-        R3DG_CUDA_TRY(cudaMemcpyAsync(a.n_contrib, b.n_contrib, HW * 4, cudaMemcpyDeviceToDevice, stream));
+        R3DG_CUDA_TRY(cudaMemcpyAsync(a.n_contrib, b.n_contrib, V * HW * 4, cudaMemcpyDeviceToDevice, stream));
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

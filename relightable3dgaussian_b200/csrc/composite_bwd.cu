@@ -31,7 +31,7 @@ namespace r3dg {
 template <int NG> struct BwdIlp { static constexpr int v = NG <= 2 ? 2 : 1; };
 
 struct CompositeBwdParams {
-    int W, H, gx, S, recf, backward_geometry;
+    int W, H, gx, gy, S, recf, backward_geometry;   // gy: tile rows of one view (see CompositeFwdParams)
     const uint2* ranges;
     const uint32_t* point_list;  // per-tile depth-sorted Gaussian ids (binning.cu)
     const uint32_t* cmask32;     // per-instance contributor masks written by the forward compositor
@@ -161,22 +161,23 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     const int cta = (int)p.cta_order[blockIdx.x];
     const int tile = cta / PARTS;
     const int wb = (cta % PARTS) * NW + warp;
-    const int tx = tile % p.gx, ty = tile / p.gx;
+    const int tx = tile % p.gx, tyv = tile / p.gx;
+    const int view = tyv / p.gy, ty = tyv - view * p.gy;          // the view's image and its view-local tile row
     const int bx0 = tx * R3DG_TILE + (wb & 1) * 8, by0 = ty * R3DG_TILE + (wb >> 1) * 4;
     const int px = bx0 + (lane & 7), py = by0 + (lane >> 3);
     const bool inside = px < p.W && py < p.H;
     const float pxf = (float)px, pyf = (float)py;
     const uint2 range = p.ranges[tile];
     const uint32_t lo = range.x;
-    const size_t HW = (size_t)p.H * p.W, pix = (size_t)p.W * py + px;
+    const size_t HW = (size_t)p.H * p.W, pix = (size_t)p.W * py + px, vpix = (size_t)view * HW + pix;
     const float4* __restrict__ rec4 = reinterpret_cast<const float4*>(p.rec);
     const int rec4n = p.recf >> 2;
     const uint32_t* __restrict__ plist = p.point_list + lo;
     uint32_t* q = sQ[warp];
 
-    const float T_final = inside ? p.final_T[pix] : 0.0f;
+    const float T_final = inside ? p.final_T[vpix] : 0.0f;
     float T = T_final;
-    const int last_contributor = inside ? p.n_contrib[pix] : 0;
+    const int last_contributor = inside ? p.n_contrib[vpix] : 0;
     // nothing behind the warp's deepest last contributor matters to this warp
     int total = last_contributor;
 #pragma unroll
@@ -186,8 +187,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 
     auto load_dpix = [&](int c) -> float {                   // cotangent of channel c of {r,g,b,f0..} at this lane's pixel
         if (!inside) return 0.0f;
-        if (c < 3) return p.dL_dpix[c * HW + pix];
-        return c - 3 < p.S ? p.dL_dpix_f[(size_t)(c - 3) * HW + pix] : 0.0f;
+        if (c < 3) return p.dL_dpix[(size_t)(3 * view + c) * HW + pix];
+        return c - 3 < p.S ? p.dL_dpix_f[((size_t)view * p.S + (c - 3)) * HW + pix] : 0.0f;
     };
     float dpix[NC];
 #pragma unroll
@@ -219,9 +220,10 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     else if (C8 > 0 && (lane & 3) == 2) { my_sel = 2; my_off = 8 + B8 + (lane >> 2); }
     if (C4 > 0 && !C4_SECOND && (lane & 7) == (C16 > 0 ? 2 : 1)) { my_sel = 3; my_off = 8 + B4 + (lane >> 3); }
     if (my_sel > 0 && my_off - 8 >= 3 + p.S) my_sel = -1;    // zero padding channel
-    const float dpix_d = inside ? p.dL_dpix_d[pix] : 0.0f;
-    const float dpix_o = inside ? p.dL_dpix_o[pix] : 0.0f;
-    const float bg_dot = p.bg[0] * dpix[0] + p.bg[1] * dpix[1] + p.bg[2] * dpix[2];
+    const float dpix_d = inside ? p.dL_dpix_d[vpix] : 0.0f;
+    const float dpix_o = inside ? p.dL_dpix_o[vpix] : 0.0f;
+    const float* bg = p.bg + 3 * view;
+    const float bg_dot = bg[0] * dpix[0] + bg[1] * dpix[1] + bg[2] * dpix[2];
     const float ddelx_dx = 0.5f * p.W, ddely_dy = 0.5f * p.H;
     const bool geo = p.backward_geometry != 0;
     // The reference keeps, per channel, the colour accumulated BEHIND the current entry (accum_rec[ch], backward.cu:
@@ -431,7 +433,8 @@ static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, cudaStream_t s
 
 int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
     CompositeBwdParams p;
-    p.W = a.W; p.H = a.H; p.gx = b.gx; p.S = a.S; p.recf = b.recf;
+    const int V = b.V;
+    p.W = a.W; p.H = a.H; p.gx = b.gx; p.gy = b.gy; p.S = a.S; p.recf = b.recf;
     p.backward_geometry = a.backward_geometry;
     p.ranges = b.ranges;
     p.point_list = b.point_list; p.cmask32 = (const uint32_t*)b.cmask;
@@ -445,10 +448,10 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     p.grad = b.grad;
     p.n_contrib = b.n_contrib;
     const bool det = a.deterministic != 0;
-    p.det = det_acc(a.det_work, (size_t)a.P * b.recf);
+    p.det = det_acc(a.det_work, (size_t)V * a.P * b.recf);
     if (det) R3DG_CUDA_TRY(cudaMemsetAsync(a.det_work, 0, det_bytes(p.det.n), stream));
-    else R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)a.P * b.recf * 4, stream));
-    const int tiles = b.tiles;
+    else R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)V * a.P * b.recf * 4, stream));
+    const int tiles = V * b.tiles;                    // the tall grid of all views
     int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;
     switch (num_groups(a.S)) {

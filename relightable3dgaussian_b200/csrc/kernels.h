@@ -23,12 +23,33 @@ struct RasterBuffers {
     uint32_t* point_list;                                                          // binning: per instance
     uint8_t *bmask, *cmask;
     long long capacity;                                                            // instances the binning holds
-    int recf, gx, gy, tiles;
+    int recf, gx, gy, tiles;                                                       // tiles: of one view (gx * gy)
     int chunk_len, chunks;                                                         // binning: depth-sorted runs
+    // Several views (V > 1): per-Gaussian regions hold V * P rows (row v * P + g = Gaussian g seen from view v), the
+    // per-pixel planes and per-tile arrays hold V images stacked as one tall tile grid (view v owns tile rows
+    // [v * gy, (v + 1) * gy)), and every view has its own header and depth-sort region.  view_slice() narrows the
+    // buffers to one view for the per-view front end and the projection backward.
+    int V, P;
+    size_t sort_stride;                                                            // bytes between the views' sort regions
+    uint32_t row_base;                                                             // slice: first row of the view (v * P)
+    const GeomHeader* prev_header;                                                 // slice: the previous view's header or null
 };
 
+// api.cu: view v's slice: header, sort region, per-Gaussian rows and tile ranges of that view.  The binning lists stay
+// shared (the views' lists follow each other in one buffer) and the tall grid's tile order is built once for all views.
+RasterBuffers view_slice(const RasterBuffers& b, int v);
+
+// view v's {tan_fovx, tan_fovy, cx, cy}: a one-view call keeps its scalar fields (passed in), a V-view call reads row v
+// of its host table
+inline void view_cam(int V, const float* view_cams, int v, float& tan_fovx, float& tan_fovy, float& cx, float& cy) {
+    if (V <= 1) return;
+    const float* c = view_cams + 4 * v;
+    tan_fovx = c[0]; tan_fovy = c[1]; cx = c[2]; cy = c[3];
+}
+
 typedef void (*stage_mark_fn)(int, cudaStream_t);
-int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream);
+// projection.cu / projection_bwd.cu: view v of the call (its camera, per-view inputs and outputs), on view_slice(b, v)
+int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream);
 int launch_point_offsets(int P, const uint32_t* tiles_touched, uint32_t* out, uint32_t* state,
                          GeomHeader* ticket_header, cudaStream_t stream);
 int launch_cta_order(const uint32_t* work, uint32_t* order, int n, cudaStream_t stream);
@@ -42,12 +63,14 @@ int launch_sort(void* geom_header, char* buf, const SortLayout& sl, long long n,
 int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stream, stage_mark_fn mark,
                    int* num_rendered_host, void* count_ready_event);
 int launch_empty_binning(const RasterBuffers& b, cudaStream_t stream);
+// the compositors' tile order over all V * tiles tiles of the tall grid (and zeroed bwd_work), after every view's binning
+int launch_tile_order(const RasterBuffers& b, cudaStream_t stream);
 int launch_rebuild_keys(int T, const void* ranges, const uint32_t* point_list, const float* rec, int recf,
                         long long limit, uint64_t* keys, cudaStream_t stream);
 int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream,
                              stage_mark_fn mark);
 int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
-int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
+int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream);
 
 size_t bvh_build_tmp_bytes(int P);
 size_t bvh_packets_bytes(int P);

@@ -458,20 +458,25 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D,
 }
 
 // ---- host launchers -----------------------------------------------------------------------
-int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
+int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream) {
     ProjParams p;
+    float tan_fovx = a.tan_fovx, tan_fovy = a.tan_fovy, cx = a.cx, cy = a.cy;
+    view_cam(b.V, a.view_cams, v, tan_fovx, tan_fovy, cx, cy);
+    const size_t r = (size_t)v * a.P;                 // view v's rows of the per-view inputs and outputs
     p.P = a.P; p.S = a.S; p.D = a.D; p.M = a.M; p.W = a.W; p.H = a.H;
     p.gx = b.gx; p.gy = b.gy;
     p.recf = b.recf; p.ng = num_groups(a.S);
-    p.means3D = a.means3D; p.shs = a.shs; p.colors_precomp = a.colors_precomp; p.features = a.features;
-    p.opacities = a.opacities; p.scales = a.scales; p.rotations = a.rotations; p.cov3D_precomp = a.cov3D_precomp;
-    p.viewmatrix = a.viewmatrix; p.projmatrix = a.projmatrix; p.campos = a.campos;
-    p.scale_modifier = a.scale_modifier; p.tan_fovx = a.tan_fovx; p.tan_fovy = a.tan_fovy;
-    p.focal_y = a.H / (2.0f * a.tan_fovy);            // rasterizer_impl.cu:232-233
-    p.focal_x = a.W / (2.0f * a.tan_fovx);
+    p.means3D = a.means3D; p.shs = a.shs; p.opacities = a.opacities; p.scales = a.scales; p.rotations = a.rotations;
+    p.cov3D_precomp = a.cov3D_precomp;
+    p.colors_precomp = a.colors_precomp && a.colors_per_view ? a.colors_precomp + 3 * r : a.colors_precomp;
+    p.features = a.features && a.features_per_view ? a.features + (size_t)a.S * r : a.features;
+    p.viewmatrix = a.viewmatrix + 16 * v; p.projmatrix = a.projmatrix + 16 * v; p.campos = a.campos + 3 * v;
+    p.scale_modifier = a.scale_modifier; p.tan_fovx = tan_fovx; p.tan_fovy = tan_fovy;
+    p.focal_y = a.H / (2.0f * tan_fovy);              // rasterizer_impl.cu:232-233
+    p.focal_x = a.W / (2.0f * tan_fovx);
     p.prefiltered = a.prefiltered;
     p.rec = b.rec; p.tiles_touched = b.tiles_touched;
-    p.clamped = b.clamped; p.radii = a.radii; p.out_weights = a.out_weights;
+    p.clamped = b.clamped; p.radii = a.radii + r; p.out_weights = a.out_weights + r;
     p.header = b.header;
     p.sort_keys = (uint32_t*)(b.sort + b.sort_layout.keys_a);
     p.sort_vals = (uint32_t*)(b.sort + b.sort_layout.vals_a);

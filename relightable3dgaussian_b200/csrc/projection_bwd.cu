@@ -27,7 +27,15 @@ struct ProjBwdParams {
         *dL_dscales, *dL_drotations;
     float* dL_dsh_factor;       // [P,3] gated dL_dRGB (multi-GPU exchange, sh_exchange.cu); dL_dsh may then be NULL
     DetAcc det;                 // DET: the gradient rows as fixed-point accumulators (composite_bwd.cu), read instead of grad
+    size_t det_row0;            // DET: the view's first row in `det` (several views: v * P)
+    // several views, views after the first: add this view's gradient to what the earlier views wrote (fp32, view order)
+    // instead of writing it — acc for the gradients summed over the views, acc_colors / acc_features for dL_dcolors /
+    // dL_dfeatures when those inputs are shared (per-view inputs get per-view rows: no accumulation)
+    bool acc, acc_colors, acc_features;
 };
+
+// out = x, or out += x when `acc` (the left fold of several views' gradients)
+__device__ __forceinline__ void put(float* out, float x, bool acc) { *out = acc ? *out + x : x; }
 
 __device__ __forceinline__ void cov3d_plain(const float* s3, float mod, const float* q, float* c6,
                                             float R[3][3], float s[3]) {
@@ -87,7 +95,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     unsigned cl = 0;
     if (visible) {
         if constexpr (DET) {
-            const size_t r0 = (size_t)idx * p.recf;
+            const size_t r0 = (p.det_row0 + idx) * p.recf;
             gA = make_float4(det_load(p.det, r0), det_load(p.det, r0 + 1), det_load(p.det, r0 + 2), det_load(p.det, r0 + 3));
             gB = make_float4(det_load(p.det, r0 + 4), det_load(p.det, r0 + 5), det_load(p.det, r0 + 6), 0.0f);
             gC = make_float4(det_load(p.det, r0 + 8), det_load(p.det, r0 + 9), det_load(p.det, r0 + 10), 0.0f);
@@ -120,8 +128,8 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     if (p.S > 0 && in_range) {
         float* df = p.dL_dfeatures + (size_t)idx * p.S;
         for (int c = 0; c < p.S; ++c) {
-            if constexpr (DET) df[c] = visible ? det_load(p.det, (size_t)idx * p.recf + 11 + c) : 0.0f;
-            else df[c] = visible ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f;
+            if constexpr (DET) put(df + c, visible ? det_load(p.det, (p.det_row0 + idx) * p.recf + 11 + c) : 0.0f, p.acc_features);
+            else put(df + c, visible ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f, p.acc_features);
         }
     }
     if (visible) {
@@ -386,35 +394,54 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         p.dL_dmeans2D[3 * (size_t)idx + k] = dmean2[k];
-        p.dL_dcolors[3 * (size_t)idx + k] = dcol[k];
-        p.dL_dmeans3D[3 * (size_t)idx + k] = dmean3[k];
-        p.dL_dscales[3 * (size_t)idx + k] = dscale[k];
+        put(p.dL_dcolors + 3 * (size_t)idx + k, dcol[k], p.acc_colors);
+        put(p.dL_dmeans3D + 3 * (size_t)idx + k, dmean3[k], p.acc);
+        put(p.dL_dscales + 3 * (size_t)idx + k, dscale[k], p.acc);
     }
-    p.dL_dopacity[idx] = dop;
+    put(p.dL_dopacity + idx, dop, p.acc);
     if (p.dL_dsh_factor) {
 #pragma unroll
         for (int k = 0; k < 3; ++k) p.dL_dsh_factor[3 * (size_t)idx + k] = dfac[k];
     }
 #pragma unroll
-    for (int k = 0; k < 6; ++k) p.dL_dcov3D[6 * (size_t)idx + k] = dcov[k];
-    *reinterpret_cast<float4*>(p.dL_drotations + 4 * (size_t)idx) = make_float4(drot[0], drot[1], drot[2], drot[3]);
+    for (int k = 0; k < 6; ++k) put(p.dL_dcov3D + 6 * (size_t)idx + k, dcov[k], p.acc);
+    float4* drot4 = reinterpret_cast<float4*>(p.dL_drotations + 4 * (size_t)idx);
+    if (p.acc) {
+        const float4 o = *drot4;
+        *drot4 = make_float4(o.x + drot[0], o.y + drot[1], o.z + drot[2], o.w + drot[3]);
+    } else {
+        *drot4 = make_float4(drot[0], drot[1], drot[2], drot[3]);
+    }
 }
 
-int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
+int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream) {
     ProjBwdParams p;
+    float tan_fovx = a.tan_fovx, tan_fovy = a.tan_fovy, cx = 0.f, cy = 0.f;
+    view_cam(b.V, a.view_cams, v, tan_fovx, tan_fovy, cx, cy);
+    const size_t r = (size_t)v * a.P;                 // view v's rows of the per-view inputs and outputs
+    const bool later = v > 0;
     p.P = a.P; p.S = a.S; p.D = a.D; p.M = a.M; p.W = a.W; p.H = a.H; p.recf = b.recf;
-    p.means3D = a.means3D; p.shs = a.shs; p.colors_precomp = a.colors_precomp; p.scales = a.scales;
-    p.rotations = a.rotations; p.cov3D_precomp = a.cov3D_precomp; p.viewmatrix = a.viewmatrix;
-    p.projmatrix = a.projmatrix; p.campos = a.campos;
-    p.scale_modifier = a.scale_modifier; p.tan_fovx = a.tan_fovx; p.tan_fovy = a.tan_fovy;
-    p.h_y = a.H / (2.0f * a.tan_fovy); p.h_x = a.W / (2.0f * a.tan_fovx);
+    p.means3D = a.means3D; p.shs = a.shs; p.scales = a.scales;
+    p.colors_precomp = a.colors_precomp && a.colors_per_view ? a.colors_precomp + 3 * r : a.colors_precomp;
+    p.rotations = a.rotations; p.cov3D_precomp = a.cov3D_precomp; p.viewmatrix = a.viewmatrix + 16 * v;
+    p.projmatrix = a.projmatrix + 16 * v; p.campos = a.campos + 3 * v;
+    p.scale_modifier = a.scale_modifier; p.tan_fovx = tan_fovx; p.tan_fovy = tan_fovy;
+    p.h_y = a.H / (2.0f * tan_fovy); p.h_x = a.W / (2.0f * tan_fovx);
     p.radii_rec = (const int*)b.tiles_touched;   // tiles_touched > 0  <=>  radii > 0
     p.rec = b.rec; p.grad = b.grad; p.clamped = b.clamped;
-    p.dL_dmeans2D = a.dL_dmeans2D; p.dL_dcolors = a.dL_dcolors; p.dL_dopacity = a.dL_dopacity;
-    p.dL_dmeans3D = a.dL_dmeans3D; p.dL_dfeatures = a.dL_dfeatures; p.dL_dcov3D = a.dL_dcov3D;
-    p.dL_dsh = a.dL_dsh; p.dL_dscales = a.dL_dscales; p.dL_drotations = a.dL_drotations;
-    p.dL_dsh_factor = a.dL_dsh_factor;
-    p.det = det_acc(a.det_work, (size_t)a.P * b.recf);
+    p.dL_dmeans2D = a.dL_dmeans2D + 3 * r; p.dL_dopacity = a.dL_dopacity;
+    p.dL_dcolors = a.colors_per_view ? a.dL_dcolors + 3 * r : a.dL_dcolors;
+    p.dL_dfeatures = a.features_per_view ? a.dL_dfeatures + (size_t)a.S * r : a.dL_dfeatures;
+    p.dL_dmeans3D = a.dL_dmeans3D; p.dL_dcov3D = a.dL_dcov3D;
+    p.dL_dscales = a.dL_dscales; p.dL_drotations = a.dL_drotations;
+    // several views: each writes its rank-1 SH factor, dL_dsh is rebuilt from them afterwards (r3dg_raster_backward)
+    p.dL_dsh = b.V > 1 ? nullptr : a.dL_dsh;
+    p.dL_dsh_factor = a.dL_dsh_factor ? a.dL_dsh_factor + 3 * r : nullptr;
+    p.det = det_acc(a.det_work, (size_t)b.V * a.P * b.recf);
+    p.det_row0 = r;
+    p.acc = later;
+    p.acc_colors = later && !a.colors_per_view;
+    p.acc_features = later && !a.features_per_view;
     const size_t sh_smem = a.shs ? (size_t)3 * a.M * SLAB_LD * sizeof(float) : 0;
     const int blocks = (a.P + PROJ_THREADS - 1) / PROJ_THREADS;
     if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);

@@ -217,6 +217,111 @@ class GaussianRasterizer(nn.Module):
                                    scales, rotations, cov3D_precomp, self.raster_settings)
 
 
+_VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
+                 "computer_pseudo_normal")
+
+
+class _RasterizeViews(torch.autograd.Function):
+    """Autograd node of rasterize_views: V views of one set of Gaussians in one forward and one backward call."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                settings):
+        rs = settings[0]
+        bg = torch.stack([s.bg for s in settings])
+        viewmatrix = torch.stack([s.viewmatrix for s in settings])
+        projmatrix = torch.stack([s.projmatrix for s in settings])
+        campos = torch.stack([s.campos for s in settings])
+        cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
+        out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
+                                 cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
+                                 rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal)
+        (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz, weights,
+         radii, geomBuffer, binningBuffer, imgBuffer) = out
+        ctx.meta = (rs, cams)
+        ctx.set_materialize_grads(False)
+        ctx.out_shapes = (color.shape, opacity.shape, depth.shape, feature.shape)
+        ctx.save_for_backward(colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix,
+                              projmatrix, campos, geomBuffer, binningBuffer, imgBuffer)
+        return (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz, weights, radii)
+
+    @staticmethod
+    def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature, g_normal, g_surface_xyz,
+                 g_weights, g_radii):
+        rs, cams = ctx.meta
+        (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
+         geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors
+        zeros = lambda g, shape: g if g is not None else torch.zeros(shape, dtype=torch.float32, device=means3D.device)
+        g_color, g_opacity = zeros(g_color, ctx.out_shapes[0]), zeros(g_opacity, ctx.out_shapes[1])
+        g_depth, g_feature = zeros(g_depth, ctx.out_shapes[2]), zeros(g_feature, ctx.out_shapes[3])
+        grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
+                                            cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
+                                            g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
+                                            rs.backward_geometry)
+        (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
+         g_rotations) = grads
+        return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
+                g_rotations, g_cov3Ds, None)
+
+
+def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
+                    rotations=None, cov3D_precomp=None, features=None):
+    """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
+
+    `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
+    `prefiltered`, `backward_geometry` and `computer_pseudo_normal`; `bg`, the two matrices, `campos`, `tanfov*`, `cx`
+    and `cy` may differ.  `means2D` is [V,P,3] (its gradient holds each view's screen-space gradient, the input of
+    the per-view densification statistics).  `features` and `colors_precomp` are shared ([P,*]) or per view
+    ([V,P,*]); each gradient comes back in the shape of its input.  Every other gradient is the sum over the views.
+
+    Returns the ten outputs of `GaussianRasterizer.forward` with a leading V: `num_rendered` is a list of V ints,
+    the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
+    Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
+    `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
+    `MAX_VIEWS` views or V·P >= 2^30 rows."""
+    settings = list(settings)
+    V = len(settings)
+    if V < 1:
+        raise ValueError("rasterize_views needs at least one view")
+    if V > MAX_VIEWS:
+        raise ValueError(f"rasterize_views renders at most {MAX_VIEWS} views per call (got {V})")
+    for name in _VIEWS_SHARED:
+        vals = {getattr(s, name) for s in settings}
+        if len(vals) != 1:
+            raise ValueError(f"rasterize_views: the views disagree on {name} ({sorted(vals)}); it must be shared")
+    if any(s.debug for s in settings):
+        raise ValueError("rasterize_views does not support debug=True; render the views one by one to debug")
+    if _EXCHANGE is not None:
+        raise RuntimeError("rasterize_views cannot take part in an installed gradient exchange (set_grad_exchange); "
+                           "the multi-GPU path renders one view per rank")
+    if (shs is None) == (colors_precomp is None):
+        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+    have_sr = scales is not None or rotations is not None
+    if ((scales is None or rotations is None) and cov3D_precomp is None) or (have_sr and cov3D_precomp is not None):
+        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+    P = means3D.shape[0]
+    if V * P >= 1 << 30:
+        raise ValueError(f"rasterize_views: V*P = {V * P} rows exceed the limit of 2^30")
+    if tuple(means2D.shape) != (V, P, 3):
+        raise ValueError(f"rasterize_views: means2D must be [V,P,3] = {(V, P, 3)}, got {tuple(means2D.shape)}")
+    for name, t in (("features", features), ("colors_precomp", colors_precomp)):
+        if t is not None and t.dim() == 3 and t.shape[0] != V:
+            raise ValueError(f"rasterize_views: per-view {name} must have V = {V} rows, got {t.shape[0]}")
+    empty = torch.Tensor([])
+    shs = empty if shs is None else shs
+    colors_precomp = empty if colors_precomp is None else colors_precomp
+    scales = empty if scales is None else scales
+    rotations = empty if rotations is None else rotations
+    cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
+    if features is None:
+        features = torch.empty_like(means3D[..., :0])
+    return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
+                                 cov3D_precomp, tuple(settings))
+
+
+MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
+
+
 class _Unpremultiply(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feature, opacity, num_contrib):
