@@ -430,6 +430,15 @@ typedef struct r3dg_shade_args {
     float* dL_dviewdirs;               /* [P,3] */
     float* dL_dincidents;              /* [P,16,3] */
     float* dL_denv;                    /* [env_h,env_w,3] (zeroed, then accumulated) */
+    /* Several views of the same Gaussians and baked samples (V = 0 or 1: the one-view call above).
+     * 1 < V <= R3DG_MAX_VIEWS: viewdirs, pbr, diffuse_light, specular, the three means, dL_dpbr, dL_ddiffuse_light,
+     * dL_dspecular and dL_dviewdirs hold V blocks of the rows above ([V,P,3], mean_visibility [V,P]); dL_dbase_color,
+     * dL_droughness, dL_dincidents and dL_denv are the sums over the views.  The per-sample outputs must be NULL
+     * (R3DG_ERR_UNSUPPORTED).  The incident light is evaluated once per sample for all views; each view's forward
+     * outputs equal a one-view call's bit for bit.  V > R3DG_MAX_VIEWS: R3DG_ERR_BAD_ARG. */
+    int V;
+    int transform_per_view;            /* non-zero with V > 1: env_transform is [V,3,3]; forward only (the backward
+                                        * returns R3DG_ERR_UNSUPPORTED) */
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero (backward only) = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_shade_det_bytes(env_h, env_w) bytes, zeroed by the call.  0 = the default path (det_work unused). */

@@ -62,6 +62,7 @@ class ShadeArgs(ctypes.Structure):
                                  "incident_lights", "local_incident_lights", "global_incident_lights",
                                  "dL_dpbr", "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color",
                                  "dL_droughness", "dL_dviewdirs", "dL_dincidents", "dL_denv")] +
+        [("V", c_int), ("transform_per_view", c_int)] +
         [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 

@@ -19,6 +19,7 @@
 //    without atomics (see "environment-map gradient" below), summed and flushed once per CTA;
 //  * the backward recomputes the forward per sample instead of saving [P,N,*] activations.
 #include <cstring>
+#include <type_traits>
 #include "common.cuh"
 #include "detacc.cuh"
 #include "kernels.h"
@@ -87,19 +88,35 @@ struct GaussianOperands {
     float inc[48];
 };
 
+// the view-dependent operands of one Gaussian: V = normalize(viewdir) (|viewdir| in vnorm) and the normal flipped
+// towards the view, Ns = normalize(n) * sign(n . V)
+__device__ __forceinline__ void view_operands(const float* n, const float* viewdir, float* V, float& vnorm, float* Ns) {
+    const float v0 = viewdir[0], v1 = viewdir[1], v2 = viewdir[2];
+    vnorm = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);             // F.normalize eps
+    V[0] = v0 / vnorm; V[1] = v1 / vnorm; V[2] = v2 / vnorm;
+    const float nn = fmaxf(sqrtf(n[0] * n[0] + n[1] * n[1] + n[2] * n[2]), 1e-12f);
+    const float N0 = n[0] / nn, N1 = n[1] / nn, N2 = n[2] / nn;
+    const float nov = V[0] * N0 + V[1] * N1 + V[2] * N2;
+    const float sg = nov > 0.f ? 1.f : (nov < 0.f ? -1.f : 0.f);             // torch.sign
+    Ns[0] = N0 * sg; Ns[1] = N1 * sg; Ns[2] = N2 * sg;
+}
+
+// the view-independent operands: material, raw normal, alpha^2 and k of the roughness
+__device__ __forceinline__ void load_material(const ShadeArgs& a, int g, GaussianOperands& o) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { o.base[c] = a.base_color[3 * (size_t)g + c]; o.n[c] = a.normals[3 * (size_t)g + c]; }
+    o.rough = a.roughness[g];
+    const float al = o.rough * o.rough;
+    o.a2 = al * al;
+    o.k = (al + 2.0f * o.rough + 1.0f) / 8.0f;
+}
+
 template <bool INC_REGS>
 __device__ __forceinline__ void load_operands(const ShadeArgs& a, int g, GaussianOperands& o) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) { o.base[c] = a.base_color[3 * (size_t)g + c]; o.n[c] = a.normals[3 * (size_t)g + c]; }
     o.rough = a.roughness[g];
-    const float v0 = a.viewdirs[3 * (size_t)g], v1 = a.viewdirs[3 * (size_t)g + 1], v2 = a.viewdirs[3 * (size_t)g + 2];
-    o.vnorm = fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);           // F.normalize eps
-    o.V[0] = v0 / o.vnorm; o.V[1] = v1 / o.vnorm; o.V[2] = v2 / o.vnorm;
-    const float nn = fmaxf(sqrtf(o.n[0] * o.n[0] + o.n[1] * o.n[1] + o.n[2] * o.n[2]), 1e-12f);
-    const float N0 = o.n[0] / nn, N1 = o.n[1] / nn, N2 = o.n[2] / nn;
-    const float nov = o.V[0] * N0 + o.V[1] * N1 + o.V[2] * N2;
-    const float sg = nov > 0.f ? 1.f : (nov < 0.f ? -1.f : 0.f);             // torch.sign
-    o.Ns[0] = N0 * sg; o.Ns[1] = N1 * sg; o.Ns[2] = N2 * sg;
+    view_operands(o.n, a.viewdirs + 3 * (size_t)g, o.V, o.vnorm, o.Ns);
     const float al = o.rough * o.rough;
     o.a2 = al * al;
     o.k = (al + 2.0f * o.rough + 1.0f) / 8.0f;
@@ -145,19 +162,20 @@ struct SampleEval {       // forward quantities of one (Gaussian, direction) pai
     float H[3], hn, NoL, NoV, NoH, VoH, NoL_r, NoV_r, NoH_r, VoH_r, p2, frac0, nom0, nom1, nom2, nom_r, nom;
 };
 
-// FAST: one-MUFU reciprocals (the backward kernel); the forward keeps IEEE divisions
-template <bool SMEM_ENV, bool INC_SMEM, bool FAST = false>
-__device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOperands& o, const float* __restrict__ env,
-                                            const float* __restrict__ sinc, float dx, float dy, float dz, float vis, SampleEval& e) {
-    // ---- environment + local SH light --------------------------------------------------------
+// Each sample's evaluation comes in three parts, so that the view kernels can run the first two once for all views:
+// the environment light (depends on the env transform), the local SH light and n.w (depend on the Gaussian only),
+// and GGX_specular (depends on the view).
+// the global light env(T d) * vis and its texel taps; T: the [3,3] env transform or NULL
+template <bool SMEM_ENV>
+__device__ __forceinline__ void eval_env(const float* T, const float* __restrict__ env, int He, int We, float dx, float dy,
+                                         float dz, float vis, SampleEval& e) {
     float ex = dx, ey = dy, ez = dz;
-    if (a.transform) {                                     // dirs @ transform.T  (scene/envmap.py:39-42)
+    if (T) {                                               // dirs @ transform.T  (scene/envmap.py:39-42)
         // the sums start from +0 like a BLAS product: a row of -0 terms gives +0 (not -0), which decides the env
         // column at the seam (atan2(+0, x < 0) = +pi -> column 0, atan2(-0, x < 0) = -pi -> column We-1)
-        const float* T = a.transform;
         ex = 0.f + dx * T[0] + dy * T[1] + dz * T[2]; ey = 0.f + dx * T[3] + dy * T[4] + dz * T[5]; ez = 0.f + dx * T[6] + dy * T[7] + dz * T[8];
     }
-    e.taps = env_taps(ex, ey, ez, a.He, a.We);
+    e.taps = env_taps(ex, ey, ez, He, We);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         float s = 0.f;
@@ -165,6 +183,12 @@ __device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOp
         for (int t = 0; t < 4; ++t) if (e.taps.idx[t] >= 0) s += (SMEM_ENV ? env[e.taps.idx[t] + c] : __ldg(env + e.taps.idx[t] + c)) * e.taps.w[t];
         e.glob[c] = s * vis;
     }
+}
+
+// the local SH light (before its clamp) and n.w with the raw normal
+template <bool INC_SMEM>
+__device__ __forceinline__ void eval_local(const GaussianOperands& o, const float* __restrict__ sinc, float dx, float dy, float dz,
+                                           SampleEval& e) {
     sh_basis3(dx, dy, dz, e.w);
     if (INC_SMEM) {
         float acc[3] = {0.f, 0.f, 0.f};
@@ -187,19 +211,25 @@ __device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOp
         }
     }
     e.ndi = fmaxf(o.n[0] * dx + o.n[1] * dy + o.n[2] * dz, 0.f);
-    // ---- GGX_specular (neilf.py:374-406) ----------------------------------------------------------
+}
+
+// GGX_specular (neilf.py:374-406) for the view V with the flipped normal Ns (o: alpha^2 and k)
+// FAST: one-MUFU reciprocals (the backward kernels); the forward keeps IEEE divisions
+template <bool FAST>
+__device__ __forceinline__ void eval_ggx(const float* V, const float* Ns, const GaussianOperands& o, float dx, float dy, float dz,
+                                         SampleEval& e) {
     const float ln = fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-12f);
     float L0, L1, L2;
     if (FAST) { const float il = fast_rcp(ln); L0 = dx * il; L1 = dy * il; L2 = dz * il; }
     else { L0 = dx / ln; L1 = dy / ln; L2 = dz / ln; }
-    const float h0 = (L0 + o.V[0]) / 2.0f, h1 = (L1 + o.V[1]) / 2.0f, h2 = (L2 + o.V[2]) / 2.0f;
+    const float h0 = (L0 + V[0]) / 2.0f, h1 = (L1 + V[1]) / 2.0f, h2 = (L2 + V[2]) / 2.0f;
     e.hn = fmaxf(sqrtf(h0 * h0 + h1 * h1 + h2 * h2), 1e-12f);
     if (FAST) { const float ih = fast_rcp(e.hn); e.H[0] = h0 * ih; e.H[1] = h1 * ih; e.H[2] = h2 * ih; }
     else { e.H[0] = h0 / e.hn; e.H[1] = h1 / e.hn; e.H[2] = h2 / e.hn; }
-    e.NoL_r = o.Ns[0] * L0 + o.Ns[1] * L1 + o.Ns[2] * L2;
-    e.NoV_r = o.Ns[0] * o.V[0] + o.Ns[1] * o.V[1] + o.Ns[2] * o.V[2];
-    e.NoH_r = o.Ns[0] * e.H[0] + o.Ns[1] * e.H[1] + o.Ns[2] * e.H[2];
-    e.VoH_r = o.V[0] * e.H[0] + o.V[1] * e.H[1] + o.V[2] * e.H[2];
+    e.NoL_r = Ns[0] * L0 + Ns[1] * L1 + Ns[2] * L2;
+    e.NoV_r = Ns[0] * V[0] + Ns[1] * V[1] + Ns[2] * V[2];
+    e.NoH_r = Ns[0] * e.H[0] + Ns[1] * e.H[1] + Ns[2] * e.H[2];
+    e.VoH_r = V[0] * e.H[0] + V[1] * e.H[1] + V[2] * e.H[2];
     e.NoL = fminf(fmaxf(e.NoL_r, 1e-6f), 1.f); e.NoV = fminf(fmaxf(e.NoV_r, 1e-6f), 1.f);
     e.NoH = fminf(fmaxf(e.NoH_r, 1e-6f), 1.f); e.VoH = fminf(fmaxf(e.VoH_r, 1e-6f), 1.f);
     const float FMi = (-5.55473f * e.VoH - 6.98316f) * e.VoH;
@@ -211,6 +241,14 @@ __device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOp
     e.nom_r = 4.0f * PI_F * e.nom0 * e.nom0 * e.nom1 * e.nom2;
     e.nom = fminf(fmaxf(e.nom_r, 1e-6f), 4.0f * PI_F);
     e.fs = FAST ? e.frac0 * o.a2 * fast_rcp(e.nom) : e.frac0 * o.a2 / e.nom;
+}
+
+template <bool SMEM_ENV, bool INC_SMEM, bool FAST = false>
+__device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOperands& o, const float* __restrict__ env,
+                                            const float* __restrict__ sinc, float dx, float dy, float dz, float vis, SampleEval& e) {
+    eval_env<SMEM_ENV>(a.transform, env, a.He, a.We, dx, dy, dz, vis, e);
+    eval_local<INC_SMEM>(o, sinc, dx, dy, dz, e);
+    eval_ggx<FAST>(o.V, o.Ns, o, dx, dy, dz, e);
 }
 
 // ---- sub-warp groups ---------------------------------------------------------------------------
@@ -334,6 +372,150 @@ __device__ __forceinline__ void warp_private_add(float4* wg, volatile unsigned c
         }
         __syncwarp();
         if (!__any_sync(0xffffffffu, pending)) break;
+    }
+}
+
+// The env-gradient state of one backward CTA in its shared memory `s_mem`: the constructor stages the texture and
+// zeroes the accumulators of ENV_MODE, scatter() adds one sample's taps, flush() adds the CTA's total to dL/denv.
+// This, accumulate_dinc and ggx_backward serve the view kernels; shade_bwd_kernel keeps the same code inline, because
+// routing it through these helpers changes its machine code (equivalent predicates, other registers).
+template <int ENV_MODE>
+struct EnvGrad {
+    static constexpr bool SMEM_ENV = ENV_MODE != ENV_GLOBAL && ENV_MODE != ENV_DET_GLOBAL;
+    int nt, ne, nflag;
+    float *s_env, *s_genv;
+    float4 *wgrad_all, *wgrad;
+    volatile unsigned char* wtag;
+    uint64_t* s_dwords;
+    uint32_t* s_dflags;
+    const float* env;                                // the texture the samples read (shared or global memory)
+    float* genv;                                     // ENV_CAS / ENV_GLOBAL: where the taps are added
+
+    __device__ __forceinline__ EnvGrad(const ShadeArgs& a, float* s_mem, int warp) {
+        nt = a.He * a.We; ne = nt * 3;
+        // ENV_CAS: [env ne][grad ne]; ENV_TAG: [env ne (padded to 4)][per warp: float4 grad[nt]][per warp: tag[nt] padded to 16]
+        s_env = s_mem;
+        s_genv = s_mem + ne;
+        const int ne4 = (ne + 3) & ~3, ntp = (nt + 15) & ~15;
+        wgrad_all = reinterpret_cast<float4*>(s_mem + ne4);
+        wgrad = wgrad_all + (size_t)warp * nt;
+        wtag = reinterpret_cast<unsigned char*>(wgrad_all + (size_t)SHADE_WARPS * nt) + (size_t)warp * ntp;
+        // ENV_DET_SMEM: [env ne (padded to 2)][accumulator words 3 ne][flag words (ne + 15) / 16]
+        s_dwords = reinterpret_cast<uint64_t*>(s_mem + ((ne + 1) & ~1));
+        s_dflags = reinterpret_cast<uint32_t*>(s_dwords + 3 * (size_t)ne);
+        nflag = (ne + 15) >> 4;
+        if (SMEM_ENV) {
+            for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_env[i] = a.env[i];
+            if (ENV_MODE == ENV_CAS) for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_genv[i] = 0.f;
+            if (ENV_MODE == ENV_TAG) for (int i = threadIdx.x; i < SHADE_WARPS * nt; i += SHADE_THREADS) wgrad_all[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (ENV_MODE == ENV_DET_SMEM) {
+                for (int i = threadIdx.x; i < 3 * ne; i += SHADE_THREADS) s_dwords[i] = 0u;
+                for (int i = threadIdx.x; i < nflag; i += SHADE_THREADS) s_dflags[i] = 0u;
+            }
+            __syncthreads();
+        }
+        env = SMEM_ENV ? s_env : a.env;
+        genv = ENV_MODE == ENV_CAS ? s_genv : a.d_env;
+    }
+
+    // dG: the sample's light cotangent times its visibility (zero for an inactive lane); called by every lane of the warp
+    __device__ __forceinline__ void scatter(const ShadeArgs& a, const EnvTap& taps, const float* dG, int lane) {
+        if (ENV_MODE == ENV_TAG) {
+            const bool any = dG[0] != 0.f || dG[1] != 0.f || dG[2] != 0.f;
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const int texel = (any && taps.idx[t] >= 0) ? taps.idx[t] / 3 : -1;
+                warp_private_add(wgrad, wtag, texel, dG[0] * taps.w[t], dG[1] * taps.w[t], dG[2] * taps.w[t], lane);
+            }
+        } else if (ENV_MODE == ENV_DET_SMEM || ENV_MODE == ENV_DET_GLOBAL) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                if (dG[c] != 0.f) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t)
+                        if (taps.idx[t] >= 0) {
+                            if (ENV_MODE == ENV_DET_SMEM) det_add(s_dwords, s_dflags, ne, taps.idx[t] + c, dG[c] * taps.w[t], true);
+                            else det_add(a.det, taps.idx[t] + c, dG[c] * taps.w[t]);
+                        }
+                }
+        } else {
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                if (dG[c] != 0.f) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) if (taps.idx[t] >= 0) atomicAdd(genv + taps.idx[t] + c, dG[c] * taps.w[t]);
+                }
+        }
+    }
+
+    __device__ __forceinline__ void flush(const ShadeArgs& a) {
+        if (ENV_MODE == ENV_CAS) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) { const float v = s_genv[i]; if (v != 0.f) atomicAdd(a.d_env + i, v); }
+        }
+        if (ENV_MODE == ENV_TAG) {
+            __syncthreads();
+            for (int t = threadIdx.x; t < nt; t += SHADE_THREADS) {
+                float4 s = wgrad_all[t];
+#pragma unroll
+                for (int w = 1; w < SHADE_WARPS; ++w) { const float4 v = wgrad_all[(size_t)w * nt + t]; s.x += v.x; s.y += v.y; s.z += v.z; }
+                if (s.x != 0.f) atomicAdd(a.d_env + 3 * t, s.x);
+                if (s.y != 0.f) atomicAdd(a.d_env + 3 * t + 1, s.y);
+                if (s.z != 0.f) atomicAdd(a.d_env + 3 * t + 2, s.z);
+            }
+        }
+        if (ENV_MODE == ENV_DET_SMEM) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < 3 * ne; i += SHADE_THREADS) {
+                const uint64_t v = s_dwords[i];
+                if (v) det_red_u64(a.det.words + (size_t)(i / ne) * a.det.n + (i % ne), v);
+            }
+            for (int i = threadIdx.x; i < nflag; i += SHADE_THREADS) { const uint32_t f = s_dflags[i]; if (f) atomicOr(a.det.flags + i, f); }
+        }
+    }
+};
+
+// dinc[3k + c] += dLg[c] * w[k]: the lane's 48 accumulators as 12 float4 in shared memory (acc4: the lane's first slot
+// of [12][threads] 16-byte slots: conflict-free 128-bit accesses) — 12 LDS.128 + 48 FFMA + 12 STS.128 per sample
+__device__ __forceinline__ void accumulate_dinc(float4* acc4, const float* dLg, const float* w) {
+#pragma unroll
+    for (int q = 0; q < 12; ++q) {
+        float4 v = acc4[q * SHADE_THREADS];
+        v.x = fmaf(dLg[(4 * q) % 3], w[(4 * q) / 3], v.x);
+        v.y = fmaf(dLg[(4 * q + 1) % 3], w[(4 * q + 1) / 3], v.y);
+        v.z = fmaf(dLg[(4 * q + 2) % 3], w[(4 * q + 2) / 3], v.z);
+        v.w = fmaf(dLg[(4 * q + 3) % 3], w[(4 * q + 3) / 3], v.w);
+        acc4[q * SHADE_THREADS] = v;
+    }
+}
+
+// GGX_specular backward for the view V (flipped normal Ns) from dfs = dL/dfs: adds to drough and to dV = dL/dV
+__device__ __forceinline__ void ggx_backward(const float* V, const float* Ns, const GaussianOperands& o, const SampleEval& e,
+                                             float dfs, float& drough, float (&dV)[3]) {
+    const float inom = fast_rcp(e.nom);
+    const float dfrac = dfs * inom;
+    const float dnom = -dfs * (e.frac0 * o.a2) * inom * inom;
+    const float dnom_r = (e.nom_r >= 1e-6f && e.nom_r <= 4.0f * PI_F) ? dnom : 0.f;
+    const float dnom0 = dnom_r * 8.0f * PI_F * e.nom0 * e.nom1 * e.nom2;
+    const float dnom1 = dnom_r * 4.0f * PI_F * e.nom0 * e.nom0 * e.nom2;
+    const float dnom2 = dnom_r * 4.0f * PI_F * e.nom0 * e.nom0 * e.nom1;
+    const float dfrac0 = dfrac * o.a2;
+    const float da2 = dfrac * e.frac0 + dnom0 * e.NoH * e.NoH;
+    const float dk = dnom1 * (1.0f - e.NoV) + dnom2 * (1.0f - e.NoL);
+    const float r = o.rough;
+    drough += da2 * 4.0f * r * r * r + dk * (2.0f * r + 2.0f) / 8.0f;
+    const float dNoH = (e.NoH_r >= 1e-6f && e.NoH_r <= 1.f) ? dnom0 * 2.0f * e.NoH * (o.a2 - 1.0f) : 0.f;
+    const float dNoV = (e.NoV_r >= 1e-6f && e.NoV_r <= 1.f) ? dnom1 * (1.0f - o.k) : 0.f;
+    const float dVoH = (e.VoH_r >= 1e-6f && e.VoH_r <= 1.f)
+                           ? dfrac0 * (1.0f - 0.04f) * e.p2 * 0.693147180559945f * (2.0f * -5.55473f * e.VoH - 6.98316f) : 0.f;
+    float dH[3], hdot = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { dH[c] = dNoH * Ns[c] + dVoH * V[c]; hdot += e.H[c] * dH[c]; }
+    const float ihn = fast_rcp(e.hn);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float dHraw = (dH[c] - e.H[c] * hdot) * ihn;
+        dV[c] += dNoV * Ns[c] + dVoH * e.H[c] + 0.5f * dHraw;
     }
 }
 
@@ -560,6 +742,254 @@ __global__ void __launch_bounds__(256) det_env_kernel(const DetAcc acc, float* _
     if (i < acc.n) out[i] = det_load(acc, i);
 }
 
+// ---- several views per call ----------------------------------------------------------------------
+// V view directions of the same Gaussians and baked samples.  Per group and sample the view-independent part runs once
+// (baked loads, env taps and global light, SH basis and local light, n.w, and T = L area n.w); a loop over the views
+// of the launch then runs GGX_specular forward (and backward).  One configuration: the default one-view one (groups of
+// 8 lanes, incident SH coefficients staged in shared memory, the backward's 48 SH-gradient accumulators in shared
+// memory).  A launch takes at most SHADE_VIEW_CHUNK views; each group keeps the operands of those views in a slot of
+// shared memory, and each lane its per-view partial sums.  The forward runs each view's arithmetic in the one-view
+// kernel's order, so every view's outputs equal a one-view call's bit for bit.
+#define SHADE_VIEW_CHUNK 8
+#define VIEW_FWD_SLOT 8           // floats per view and group: V[3], Ns[3] (padded)
+#define VIEW_BWD_SLOT 16          // V[3], Ns[3], dL/dpbr, dL/dspecular, dL/ddiffuse_light (each [3], times 1/N), |viewdir|
+
+struct ViewChunk {
+    int v0, nv;                   // first view of the launch and its view count (<= SHADE_VIEW_CHUNK)
+    int per_view_transform;       // forward: the env transform holds one [3,3] per view
+    int accumulate;               // backward: add the leaf gradients to the earlier launches' (0: write them)
+};
+
+// per-lane partial sums of one view in the forward: pbr, specular, diffuse (+ mean lights, mean global with per-view transforms)
+__host__ __device__ inline int view_fwd_sums(bool per_view_means) { return per_view_means ? 15 : 9; }
+
+template <bool SMEM_ENV>
+__global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const ShadeArgs a, const ViewChunk vc) {
+    constexpr int G = 8, GPW = 32 / G;
+    constexpr int INC_FLOATS = SHADE_WARPS * GPW * SHADE_INC_STRIDE;
+    constexpr int SLOT_FLOATS = SHADE_WARPS * GPW * SHADE_VIEW_CHUNK * VIEW_FWD_SLOT;
+    extern __shared__ __align__(16) float s_vfwd[];   // [incident slots][view slots][per-lane sums K][view][threads][env]
+    const bool pvt = vc.per_view_transform != 0, means = a.mean_lights != nullptr;
+    const int K = view_fwd_sums(pvt && means);
+    float* s_acc = s_vfwd + INC_FLOATS + SLOT_FLOATS;
+    float* s_env = s_acc + K * SHADE_VIEW_CHUNK * SHADE_THREADS;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane & (G - 1), grp = lane / G;
+    float* sinc = s_vfwd + (warp * GPW + grp) * SHADE_INC_STRIDE;
+    float* slot = s_vfwd + INC_FLOATS + (warp * GPW + grp) * SHADE_VIEW_CHUNK * VIEW_FWD_SLOT;
+    if (SMEM_ENV) {
+        for (int i = threadIdx.x; i < a.He * a.We * 3; i += SHADE_THREADS) s_env[i] = a.env[i];
+        __syncthreads();
+    }
+    const float* env = SMEM_ENV ? s_env : a.env;
+    const float invN = 1.0f / (float)a.N;
+    const int units = (a.P + GPW - 1) / GPW;
+    for (int u = blockIdx.x * SHADE_WARPS + warp; u < units; u += gridDim.x * SHADE_WARPS) {
+        const int g_raw = u * GPW + grp;
+        const bool valid = g_raw < a.P;
+        const int g = valid ? g_raw : a.P - 1;
+        GaussianOperands o;
+        load_material(a, g, o);
+        stage_incidents<G>(a, g, sinc, sub);
+        if (sub < vc.nv) {
+            float* vs = slot + sub * VIEW_FWD_SLOT;
+            float vnorm;
+            view_operands(o.n, a.viewdirs + 3 * ((size_t)(vc.v0 + sub) * a.P + g), vs, vnorm, vs + 3);
+        }
+        for (int j = 0; j < K * vc.nv; ++j) s_acc[j * SHADE_THREADS + threadIdx.x] = 0.f;
+        __syncwarp();
+        float ml[3] = {0, 0, 0}, mloc[3] = {0, 0, 0}, mg[3] = {0, 0, 0}, mv = 0;
+        const size_t row = (size_t)g * a.N;
+        for (int i = sub; i < a.N; i += G) {
+            const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
+            const float vis = a.visibility[row + i], area = a.areas[row + i];
+            SampleEval e;
+            if (!pvt) eval_env<SMEM_ENV>(a.transform, env, a.He, a.We, dx, dy, dz, vis, e);
+            eval_local<true>(o, sinc, dx, dy, dz, e);
+            float loc[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                loc[c] = fmaxf(e.local_raw[c], 0.f);
+                mloc[c] += loc[c];
+                if (!pvt) { ml[c] += loc[c] + e.glob[c]; mg[c] += e.glob[c]; }
+            }
+            mv += vis;
+            for (int v = 0; v < vc.nv; ++v) {
+                const float* vs = slot + v * VIEW_FWD_SLOT;
+                if (pvt) eval_env<SMEM_ENV>(a.transform + 9 * (size_t)(vc.v0 + v), env, a.He, a.We, dx, dy, dz, vis, e);
+                eval_ggx<false>(vs, vs + 3, o, dx, dy, dz, e);
+                float* acc = s_acc + v * K * SHADE_THREADS + threadIdx.x;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {                 // the one-view kernel's expressions
+                    const float Lc = loc[c] + e.glob[c];
+                    const float T = Lc * area * e.ndi;
+                    const float fd = o.base[c] / PI_F;
+                    acc[c * SHADE_THREADS] += (fd + e.fs) * T; acc[(3 + c) * SHADE_THREADS] += e.fs * T; acc[(6 + c) * SHADE_THREADS] += T;
+                    if (K == 15) { acc[(9 + c) * SHADE_THREADS] += Lc; acc[(12 + c) * SHADE_THREADS] += e.glob[c]; }
+                }
+            }
+        }
+        __syncwarp();
+        if (means) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                mloc[c] = group_sum<G>(mloc[c]);
+                if (!pvt) { ml[c] = group_sum<G>(ml[c]); mg[c] = group_sum<G>(mg[c]); }
+            }
+            mv = group_sum<G>(mv);
+        }
+        for (int v = 0; v < vc.nv; ++v) {
+            const float* acc = s_acc + v * K * SHADE_THREADS + threadIdx.x;
+            float r[15];
+#pragma unroll
+            for (int j = 0; j < 15; ++j) if (j < K) r[j] = group_sum<G>(acc[j * SHADE_THREADS]);
+            if (sub == 0 && valid) {
+                const size_t vg = (size_t)(vc.v0 + v) * a.P + g;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    a.pbr[3 * vg + c] = r[c] * invN; a.specular[3 * vg + c] = r[3 + c] * invN; a.diffuse[3 * vg + c] = r[6 + c] * invN;
+                    if (means) {
+                        a.mean_lights[3 * vg + c] = (pvt ? r[9 + c] : ml[c]) * invN; a.mean_local[3 * vg + c] = mloc[c] * invN;
+                        a.mean_global[3 * vg + c] = (pvt ? r[12 + c] : mg[c]) * invN;
+                    }
+                }
+                if (means) a.mean_vis[vg] = mv * invN;
+            }
+        }
+    }
+}
+
+// Backward over the views of one launch, with the environment transform shared by all views.  Per sample the view
+// loop sums dT = sum_v dL/dT_v; the SH-gradient contraction and the env scatter then run once on that sum, and dL/dbase
+// uses the summed dL/dpbr.  dL/dviewdirs stays per view.  `accumulate` adds the leaf gradients to those of the earlier
+// launches, in launch order (a fixed fold, so the deterministic mode stays reproducible).
+template <int ENV_MODE>
+__global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_bwd_kernel(const ShadeArgs a, const ViewChunk vc) {
+    constexpr bool SMEM_ENV = EnvGrad<ENV_MODE>::SMEM_ENV;
+    constexpr int G = 8, GPW = 32 / G, RQ = 48 / G;
+    constexpr int INC_FLOATS = SHADE_WARPS * GPW * SHADE_INC_STRIDE;
+    constexpr int DINC_FLOATS = 48 * SHADE_THREADS;
+    constexpr int SLOT_FLOATS = SHADE_WARPS * GPW * SHADE_VIEW_CHUNK * VIEW_BWD_SLOT;
+    constexpr int DV_FLOATS = 3 * SHADE_VIEW_CHUNK * SHADE_THREADS;
+    // [incident slots][SH-gradient accumulators][view slots][per-lane dL/dV: 3][view][threads][env ...]
+    extern __shared__ __align__(16) float s_vbwd[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane & (G - 1), grp = lane / G;
+    float* sinc = s_vbwd + (warp * GPW + grp) * SHADE_INC_STRIDE;
+    float4* acc4 = reinterpret_cast<float4*>(s_vbwd + INC_FLOATS) + threadIdx.x;
+    float* slot = s_vbwd + INC_FLOATS + DINC_FLOATS + (warp * GPW + grp) * SHADE_VIEW_CHUNK * VIEW_BWD_SLOT;
+    float* s_dv = s_vbwd + INC_FLOATS + DINC_FLOATS + SLOT_FLOATS + threadIdx.x;
+    EnvGrad<ENV_MODE> eg(a, s_vbwd + INC_FLOATS + DINC_FLOATS + SLOT_FLOATS + DV_FLOATS, warp);
+    const float invN = 1.0f / (float)a.N;
+    const int units = (a.P + GPW - 1) / GPW;
+    for (int u = blockIdx.x * SHADE_WARPS + warp; u < units; u += gridDim.x * SHADE_WARPS) {
+        const int g_raw = u * GPW + grp;
+        const bool valid = g_raw < a.P;
+        const int g = valid ? g_raw : a.P - 1;
+        GaussianOperands o;
+        load_material(a, g, o);
+        stage_incidents<G>(a, g, sinc, sub);
+        if (sub < vc.nv) {
+            float* vs = slot + sub * VIEW_BWD_SLOT;
+            const size_t vg = (size_t)(vc.v0 + sub) * a.P + g;
+            view_operands(o.n, a.viewdirs + 3 * vg, vs, vs[15], vs + 3);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                vs[6 + c] = a.g_pbr[3 * vg + c] * invN;
+                vs[9 + c] = a.g_specular ? a.g_specular[3 * vg + c] * invN : 0.f;
+                vs[12 + c] = a.g_diffuse ? a.g_diffuse[3 * vg + c] * invN : 0.f;
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < 12; ++q) acc4[q * SHADE_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int j = 0; j < 3 * vc.nv; ++j) s_dv[j * SHADE_THREADS] = 0.f;
+        __syncwarp();
+        float gp_sum[3] = {0, 0, 0};
+        for (int v = 0; v < vc.nv; ++v)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) gp_sum[c] += slot[v * VIEW_BWD_SLOT + 6 + c];
+        float dbase[3] = {0, 0, 0}, drough = 0.f;
+        const size_t row = (size_t)g * a.N;
+        for (int i0 = 0; i0 < a.N; i0 += G) {          // warp-uniform trip count (collectives inside in ENV_TAG mode)
+            const bool act = valid && (i0 + sub) < a.N;
+            const int i = (i0 + sub) < a.N ? (i0 + sub) : a.N - 1;
+            const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
+            const float vis = a.visibility[row + i], area = a.areas[row + i];
+            SampleEval e;
+            eval_env<SMEM_ENV>(a.transform, eg.env, a.He, a.We, dx, dy, dz, vis, e);
+            eval_local<true>(o, sinc, dx, dy, dz, e);
+            float T[3], dT[3] = {0, 0, 0};
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                T[c] = (fmaxf(e.local_raw[c], 0.f) + e.glob[c]) * area * e.ndi;
+                if (act) dbase[c] += gp_sum[c] * T[c] * INV_PI_F;
+            }
+            if (act) {
+                for (int v = 0; v < vc.nv; ++v) {
+                    const float* vs = slot + v * VIEW_BWD_SLOT;
+                    eval_ggx<true>(vs, vs + 3, o, dx, dy, dz, e);
+                    float dfs = 0.f;
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        const float gp = vs[6 + c], gs = vs[9 + c];
+                        dT[c] += gp * (o.base[c] * INV_PI_F + e.fs) + gs * e.fs + vs[12 + c];
+                        dfs += (gp + gs) * T[c];
+                    }
+                    float dV[3] = {0, 0, 0};
+                    ggx_backward(vs, vs + 3, o, e, dfs, drough, dV);
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) s_dv[(3 * v + c) * SHADE_THREADS] += dV[c];
+                }
+            }
+            float dG[3], dLg[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float dL = dT[c] * area * e.ndi;
+                dLg[c] = (act && e.local_raw[c] >= 0.f) ? dL : 0.f;  // clamp_min(0) passes the gradient at equality
+                dG[c] = act ? dL * vis : 0.f;                        // -> env texels (grid_sample backward)
+            }
+            accumulate_dinc(acc4, dLg, e.w);
+            eg.scatter(a, e.taps, dG, lane);
+        }
+        __syncwarp();
+        // ---- group reduction and per-Gaussian outputs ---------------------------------------------
+#pragma unroll
+        for (int c = 0; c < 3; ++c) dbase[c] = group_sum<G>(dbase[c]);
+        drough = group_sum<G>(drough);
+        for (int v = 0; v < vc.nv; ++v) {
+            float dV[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) dV[c] = group_sum<G>(s_dv[(3 * v + c) * SHADE_THREADS]);
+            if (sub == 0 && valid) {
+                const float* vs = slot + v * VIEW_BWD_SLOT;
+                const float vd = vs[0] * dV[0] + vs[1] * dV[1] + vs[2] * dV[2];
+                float* dview = a.d_view + 3 * ((size_t)(vc.v0 + v) * a.P + g);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) dview[c] = (dV[c] - vs[c] * vd) / vs[15];      // through V = normalize(viewdirs)
+            }
+        }
+        float dinc[48];
+#pragma unroll
+        for (int q = 0; q < 12; ++q) { const float4 v = acc4[q * SHADE_THREADS]; dinc[4 * q] = v.x; dinc[4 * q + 1] = v.y; dinc[4 * q + 2] = v.z; dinc[4 * q + 3] = v.w; }
+        group_reduce_scatter<G, 48>(dinc, sub);        // lane `sub` now owns components [sub*RQ, sub*RQ + RQ)
+        if (valid) {
+            if (sub == 0) {
+#pragma unroll
+                for (int c = 0; c < 3; ++c) a.d_base[3 * (size_t)g + c] = vc.accumulate ? a.d_base[3 * (size_t)g + c] + dbase[c] : dbase[c];
+                a.d_rough[g] = vc.accumulate ? a.d_rough[g] + drough : drough;
+            }
+            float* dp = a.d_incidents + 48 * (size_t)g + sub * RQ;    // the group writes the 192 B row contiguously
+#pragma unroll
+            for (int q = 0; q < RQ; q += 2) {
+                float2 w = make_float2(dinc[q], dinc[q + 1]);
+                if (vc.accumulate) { const float2 p = *reinterpret_cast<const float2*>(dp + q); w.x = p.x + w.x; w.y = p.y + w.y; }
+                *reinterpret_cast<float2*>(dp + q) = w;
+            }
+        }
+    }
+    eg.flush(a);
+}
+
 // ---- launch ---------------------------------------------------------------------------------------
 // tuning knobs (A/B measurements and tests of the non-default paths), changed at run time through r3dg_tune
 // (include/r3dg_b200.h); each starts at its default
@@ -588,15 +1018,15 @@ int shade_tune(const char* key, int value, int* previous) {
     return R3DG_ERR_UNSUPPORTED;
 }
 
-template <typename K>
-static int shade_launch(K kernel, const ShadeArgs& a, int units, int num_sms, size_t smem, cudaStream_t stream) {
+template <typename K, typename... X>
+static int shade_launch(K kernel, const ShadeArgs& a, int units, int num_sms, size_t smem, cudaStream_t stream, const X&... extra) {
     if (smem > 48 * 1024) R3DG_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, SHADE_THREADS, smem) != cudaSuccess || per_sm <= 0) per_sm = 2;
     const int want = (units + SHADE_WARPS - 1) / SHADE_WARPS;
     const int cap = num_sms * per_sm;                 // persistent CTAs: one env staging / flush per resident CTA
     const int grid = want < cap ? (want > 0 ? want : 1) : cap;
-    kernel<<<grid, SHADE_THREADS, smem, stream>>>(a);
+    kernel<<<grid, SHADE_THREADS, smem, stream>>>(a, extra...);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }
@@ -639,7 +1069,13 @@ static int launch_bwd(const ShadeArgs& a, int num_sms, size_t env_smem, cudaStre
 // shared memory of ENV_DET_SMEM (env, accumulator words, flag words); larger textures use ENV_DET_GLOBAL
 static size_t det_smem_bytes(size_t ne) { return ((ne + 1) & ~(size_t)1) * sizeof(float) + 3 * ne * 8 + (ne + 15) / 16 * 4; }
 
-int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
+template <int M> using EnvMode = std::integral_constant<int, M>;
+
+// Clears dL/denv (or the deterministic accumulators), picks the env-gradient mode from the texture size, the deterministic
+// flag and the highest mode allowed (`cap`), and calls run(EnvMode<mode>, args, env shared-memory bytes) unless P = 0;
+// the deterministic mode then converts its accumulators into dL/denv.
+template <typename Run>
+static int shade_backward(ShadeArgs a, int cap, cudaStream_t stream, Run run) {
     const size_t nt = (size_t)a.He * a.We, env_bytes = nt * 3 * sizeof(float);
     if (a.det.words) {
         R3DG_CUDA_TRY(cudaMemsetAsync(a.det.words, 0, det_bytes(a.det.n), stream));
@@ -647,7 +1083,7 @@ int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
         if (a.P > 0) {
             const size_t smem = det_smem_bytes(a.det.n);
             a.env_in_smem = smem <= 64 * 1024;
-            rc = a.env_in_smem ? launch_bwd<ENV_DET_SMEM>(a, num_sms, smem, stream) : launch_bwd<ENV_DET_GLOBAL>(a, num_sms, 0, stream);
+            rc = a.env_in_smem ? run(EnvMode<ENV_DET_SMEM>(), a, smem) : run(EnvMode<ENV_DET_GLOBAL>(), a, 0);
         }
         if (rc) return rc;
         det_env_kernel<<<(unsigned)((a.det.n + 255) / 256), 256, 0, stream>>>(a.det, a.d_env);
@@ -659,11 +1095,55 @@ int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
     // shared-memory cost of the env-gradient modes (kept within the 48 KB that need no opt-in on their own)
     const size_t tag_bytes = ((nt * 3 + 3) & ~(size_t)3) * sizeof(float) + SHADE_WARPS * (nt * sizeof(float4) + ((nt + 15) & ~(size_t)15));
     const size_t cas_bytes = 2 * env_bytes;
-    const int cap = knob(1);
-    if (cap >= ENV_TAG && tag_bytes <= 48 * 1024) { a.env_in_smem = 1; return launch_bwd<ENV_TAG>(a, num_sms, tag_bytes, stream); }
-    if (cap >= ENV_CAS && cas_bytes <= 40 * 1024) { a.env_in_smem = 1; return launch_bwd<ENV_CAS>(a, num_sms, cas_bytes, stream); }
+    if (cap >= ENV_TAG && tag_bytes <= 48 * 1024) { a.env_in_smem = 1; return run(EnvMode<ENV_TAG>(), a, tag_bytes); }
+    if (cap >= ENV_CAS && cas_bytes <= 40 * 1024) { a.env_in_smem = 1; return run(EnvMode<ENV_CAS>(), a, cas_bytes); }
     a.env_in_smem = 0;
-    return launch_bwd<ENV_GLOBAL>(a, num_sms, 0, stream);
+    return run(EnvMode<ENV_GLOBAL>(), a, 0);
+}
+
+int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
+    return shade_backward(a, knob(1), stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
+        return launch_bwd<decltype(mode)::value>(x, num_sms, env_smem, stream);
+    });
+}
+
+// ---- several views: one launch per SHADE_VIEW_CHUNK views ------------------------------------------
+static size_t view_slot_bytes(int slot_floats) { return (size_t)SHADE_WARPS * 4 * SHADE_VIEW_CHUNK * slot_floats * sizeof(float); }
+
+int launch_shade_views_forward(ShadeArgs a, int V, int per_view_transform, int num_sms, cudaStream_t stream) {
+    if (a.P <= 0) return 0;
+    const size_t env_bytes = (size_t)a.He * a.We * 3 * sizeof(float);
+    const bool smem_env = env_bytes <= 40 * 1024;     // as the one-view forward
+    a.env_in_smem = smem_env;
+    const int K = view_fwd_sums(per_view_transform && a.mean_lights);
+    const size_t smem = inc_slot_bytes(8, 1) + view_slot_bytes(VIEW_FWD_SLOT) + (size_t)K * SHADE_VIEW_CHUNK * SHADE_THREADS * sizeof(float) +
+                        (smem_env ? env_bytes : 0);
+    const int units = (a.P + 3) / 4;
+    for (int v0 = 0; v0 < V; v0 += SHADE_VIEW_CHUNK) {
+        const ViewChunk vc{v0, V - v0 < SHADE_VIEW_CHUNK ? V - v0 : SHADE_VIEW_CHUNK, per_view_transform, 0};
+        const int rc = smem_env ? shade_launch(shade_views_fwd_kernel<true>, a, units, num_sms, smem, stream, vc)
+                                : shade_launch(shade_views_fwd_kernel<false>, a, units, num_sms, smem, stream, vc);
+        if (rc) return rc;
+    }
+    return 0;
+}
+
+// the env-gradient mode as the one-view backward picks it at its default highest mode (the view kernels have no knobs)
+int launch_shade_views_backward(ShadeArgs a, int V, int num_sms, cudaStream_t stream) {
+    return shade_backward(a, ENV_CAS, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
+        constexpr int M = decltype(mode)::value;
+        if constexpr (M == ENV_TAG) return (int)R3DG_ERR_UNSUPPORTED;     // above the cap: never selected
+        else {
+            const size_t smem = inc_slot_bytes(8, 2) + (size_t)48 * SHADE_THREADS * sizeof(float) + view_slot_bytes(VIEW_BWD_SLOT) +
+                                (size_t)3 * SHADE_VIEW_CHUNK * SHADE_THREADS * sizeof(float) + env_smem;
+            for (int v0 = 0; v0 < V; v0 += SHADE_VIEW_CHUNK) {
+                const ViewChunk vc{v0, V - v0 < SHADE_VIEW_CHUNK ? V - v0 : SHADE_VIEW_CHUNK, 0, v0 > 0};
+                const int rc = shade_launch(shade_views_bwd_kernel<M>, x, (x.P + 3) / 4, num_sms, smem, stream, vc);
+                if (rc) return rc;
+            }
+            return 0;
+        }
+    });
 }
 
 }  // namespace r3dg
@@ -674,6 +1154,7 @@ extern "C" {
 
 static int fill_args(const r3dg_shade_args* s, ShadeArgs& a) {
     if (!s || s->P < 0 || s->N <= 0 || s->env_h <= 0 || s->env_w <= 0) return R3DG_ERR_BAD_ARG;
+    if (s->V < 0 || s->V > R3DG_MAX_VIEWS) return R3DG_ERR_BAD_ARG;
     if (s->sh_coeffs != 16) return R3DG_ERR_UNSUPPORTED;          // incidents are degree-3 SH ([P,16,3]) in the reference
     a.P = s->P; a.N = s->N; a.He = s->env_h; a.We = s->env_w; a.env_in_smem = 0;
     a.base_color = s->base_color; a.roughness = s->roughness; a.normals = s->normals; a.viewdirs = s->viewdirs;
@@ -697,6 +1178,11 @@ int r3dg_render_equation_forward(const r3dg_shade_args* s, r3dg_stream_t stream)
     if (a.P > 0 && (!a.pbr || !a.diffuse || !a.specular)) return R3DG_ERR_BAD_ARG;
     if ((a.mean_lights != nullptr) != (a.mean_local != nullptr) || (a.mean_lights != nullptr) != (a.mean_global != nullptr)) return R3DG_ERR_BAD_ARG;
     if ((a.s_lights != nullptr) != (a.s_local != nullptr) || (a.s_lights != nullptr) != (a.s_global != nullptr)) return R3DG_ERR_BAD_ARG;
+    if (s->V > 1) {
+        if (a.s_lights) return R3DG_ERR_UNSUPPORTED;               // no per-sample [V,P,N,3] outputs
+        if (a.mean_lights && !a.mean_vis) return R3DG_ERR_BAD_ARG;
+        return launch_shade_views_forward(a, s->V, s->transform_per_view && a.transform, num_sms(), (cudaStream_t)stream);
+    }
     return launch_shade_forward(a, num_sms(), (cudaStream_t)stream);
 }
 
@@ -705,12 +1191,14 @@ int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream
     int rc = fill_args(s, a);
     if (rc) return rc;
     if (!a.g_pbr || !a.d_base || !a.d_rough || !a.d_view || !a.d_incidents || !a.d_env) return R3DG_ERR_BAD_ARG;
+    if (s->V > 1 && s->transform_per_view && a.transform) return R3DG_ERR_UNSUPPORTED;    // forward only
     if (s->deterministic) {
         const size_t n = (size_t)a.He * a.We * 3;
         if (!s->det_work || s->det_work_bytes < det_bytes(n)) return R3DG_ERR_BAD_ARG;
         a.det = det_acc(s->det_work, n);
     }
-    return launch_shade_backward(a, num_sms(), (cudaStream_t)stream);
+    return s->V > 1 ? launch_shade_views_backward(a, s->V, num_sms(), (cudaStream_t)stream)
+                    : launch_shade_backward(a, num_sms(), (cudaStream_t)stream);
 }
 
 size_t r3dg_shade_det_bytes(int env_h, int env_w) {

@@ -153,6 +153,92 @@ def rendering_equation(base_color, roughness, normals, viewdirs, incidents, dire
     return pbr, extra
 
 
+MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
+_MEANS = ("mean_incident_lights", "mean_local_incident_lights", "mean_global_incident_lights", "mean_incident_visibility")
+
+
+class _RenderEquationViews(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, base_color, roughness, viewdirs, incidents, env, normals, visibility, dirs, areas, transform, want_means):
+        V, P = viewdirs.shape[0], dirs.shape[0]
+        f = dict(dtype=torch.float32, device=dirs.device)
+        a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas), transform)
+        a.V, a.transform_per_view = V, int(tr is not None and tr.dim() == 3)
+        pbr, diffuse, specular = (torch.empty((V, P, 3), **f) for _ in range(3))
+        a.pbr, a.diffuse_light, a.specular = pbr.data_ptr(), diffuse.data_ptr(), specular.data_ptr()
+        means = []
+        if want_means:
+            means = [torch.empty((V, P, 3), **f) for _ in range(3)] + [torch.empty((V, P, 1), **f)]
+            a.mean_incident_lights, a.mean_local_lights, a.mean_global_lights, a.mean_visibility = [m.data_ptr() for m in means]
+        if P > 0:
+            _lib.call("r3dg_render_equation_forward", dirs.device, ctypes.byref(a), what="rendering_equation_views")
+        ctx.save_for_backward(*ts)
+        ctx.transform = tr
+        ctx.mark_non_differentiable(*means)
+        return (pbr, diffuse, specular) + tuple(means)
+
+    @staticmethod
+    def backward(ctx, g_pbr, g_diffuse, g_specular, *_):
+        a, ts, _ = _shade_args(ctx.saved_tensors, ctx.transform)
+        env, viewdirs, dirs = ts[5], ts[3], ts[7]
+        V, P = viewdirs.shape[0], dirs.shape[0]
+        a.V = V
+        dev = dirs.device
+        f = dict(dtype=torch.float32, device=dev)
+        d_base, d_view = torch.empty((P, 3), **f), torch.empty((V, P, 3), **f)
+        d_rough = torch.empty((P, 1), **f)
+        d_inc = torch.empty((P, 16, 3), **f)
+        d_env = torch.empty(env.shape, **f)
+        if P == 0:                      # nothing to shade: empty gradients (no device pointers to pass)
+            return d_base, d_rough, d_view, d_inc, d_env.zero_(), None, None, None, None, None, None
+        gz = torch.zeros((V, P, 3), **f)
+        g = [gz if t is None else _lib.f32(t) for t in (g_pbr, g_diffuse, g_specular)]
+        a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = [t.data_ptr() for t in g]
+        a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = d_base.data_ptr(), d_rough.data_ptr(), d_view.data_ptr()
+        a.dL_dincidents, a.dL_denv = d_inc.data_ptr(), d_env.data_ptr()
+        det_ws = _lib.det_workspace(a, _lib.load().r3dg_shade_det_bytes(env.shape[0], env.shape[1]), dev)
+        _lib.call("r3dg_render_equation_backward", dev, ctypes.byref(a), what="rendering_equation_views backward")
+        return d_base, d_rough, d_view, d_inc, d_env, None, None, None, None, None, None
+
+
+def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents, direct_light_env_light=None,
+                             visibility_precompute=None, incident_dirs_precompute=None, incident_areas_precompute=None,
+                             means=False):
+    """`rendering_equation` for V view directions of the same Gaussians in one call: viewdirs [V,P,3], every other input
+    as in `rendering_equation`.  The incident light of each sample is evaluated once for all views.
+
+    Returns (pbr [V,P,3], extra) with extra = {incident_dirs, incident_visibility (the baked tensors), diffuse_light
+    [V,P,3], specular [V,P,3]} and, with means=True, mean_incident_lights, mean_local_incident_lights,
+    mean_global_incident_lights [V,P,3] and mean_incident_visibility [V,P,1] (the `.mean(-2)` of the per-sample lights;
+    no gradient).  Each view's outputs equal a one-view call with that view's direction and transform bit for bit.
+
+    An EnvLight `transform` may be [3,3] or [V,3,3] (one per view, forward only).  Gradients: viewdirs per view;
+    base_color, roughness, incidents and the environment map summed over the views; none for normals and the baked
+    tensors.  Refused before anything is launched: V outside 1..MAX_VIEWS, viewdirs not [V,P,3], incidents not [P,16,3],
+    a [V',3,3] transform with V' != V, and per-view transforms when autograd would need a backward."""
+    dirs, areas, vis = incident_dirs_precompute, incident_areas_precompute, visibility_precompute
+    P = dirs.shape[0]
+    if viewdirs.dim() != 3 or viewdirs.shape[1:] != (P, 3):
+        raise ValueError(f"viewdirs must be [V,P,3] with P = {P} (got {tuple(viewdirs.shape)})")
+    V = viewdirs.shape[0]
+    if not 1 <= V <= MAX_VIEWS:
+        raise ValueError(f"rendering_equation_views shades 1 to {MAX_VIEWS} views per call (got {V})")
+    if incidents.shape[1:] != (16, 3):
+        raise RuntimeError("incidents must be degree-3 SH coefficients [P,16,3]")
+    env, transform = _env_texture(direct_light_env_light)
+    if transform is not None and transform.dim() == 3:
+        if transform.shape != (V, 3, 3):
+            raise ValueError(f"a per-view transform must be [V,3,3] with V = {V} (got {tuple(transform.shape)})")
+        if torch.is_grad_enabled() and any(t.requires_grad for t in (base_color, roughness, viewdirs, incidents, env)):
+            raise ValueError("per-view transforms are forward-only: call under torch.no_grad() or with detached inputs")
+    outs = _RenderEquationViews.apply(base_color, roughness, viewdirs, incidents, env, normals, vis, dirs, areas, transform,
+                                      bool(means))
+    pbr, diffuse, specular = outs[:3]
+    extra = {"incident_dirs": dirs, "incident_visibility": vis, "diffuse_light": diffuse, "specular": specular}
+    extra.update(zip(_MEANS, outs[3:]))
+    return pbr, extra
+
+
 def install(module=None):
     """Rebind `rendering_equation` inside the reference's gaussian_renderer.neilf (or `module`)."""
     if module is None:
