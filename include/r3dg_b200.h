@@ -152,6 +152,23 @@ typedef struct r3dg_raster_bwd_args {
     int V;
     const float* view_cams;
     int features_per_view, colors_per_view;
+    /* Camera gradients (optional; all three NULL = none, the default).  One row per view, never summed over views:
+     *   dL_dviewmatrix [V,16] and dL_dprojmatrix [V,16] in the element order of `viewmatrix` / `projmatrix`, i.e. the
+     *   memory of torch's world_view_transform / full_proj_transform: element 4j + k is matrix[j][k];
+     *   dL_dcampos [V,3].
+     * Entries the projection never reads (column 3 of viewmatrix, column 2 of projmatrix) are exactly 0, and so is the
+     * whole row of a view in which every Gaussian is culled, or of every view when P = 0.  The gradients are those of
+     * the projection's closed form: through t = [m,1] viewmatrix and T = W J into the 2D covariance and depth, through
+     * the homogeneous projection into the 2D mean (with the forward's + 1e-7), and through the SH view direction.  Each
+     * CTA of the projection backward sums its Gaussians' terms in a fixed order into cam_work, and one more launch adds
+     * those partial sums in CTA order: no float atomics, so equal gradient rows give equal bits (in deterministic mode
+     * the camera gradients are bitwise reproducible).
+     * cam_work: device workspace of at least r3dg_raster_cam_grad_bytes(P, V) bytes.  Only some of the three outputs,
+     * or too small a workspace, returns R3DG_ERR_BAD_ARG before anything is launched. */
+    float* dL_dviewmatrix;
+    float* dL_dprojmatrix;
+    float* dL_dcampos;
+    void* cam_work; size_t cam_work_bytes;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_raster_bwd_det_bytes(P, S) bytes, zeroed by the call.  0 = the default path (det_work unused). */
@@ -162,6 +179,9 @@ typedef struct r3dg_raster_bwd_args {
 /* Replaces CudaRasterizer::Rasterizer::backward (rasterizer.h:67-100, rasterizer_impl.cu:384-491)
  * == `_C.rasterize_gaussians_backward` (rasterize_points.cu:143-235). */
 int r3dg_raster_backward(const r3dg_raster_bwd_args* args, r3dg_stream_t stream);
+/* Workspace of the camera gradients of a V-view backward (r3dg_raster_bwd_args.cam_work); P = 0 and V < 1 are sized
+ * as 1.  r3dg_raster_cam_grad_bytes(P, 1) also covers the workspace of r3dg_pack_features_backward. */
+size_t r3dg_raster_cam_grad_bytes(int P, int V);
 
 /* Multi-GPU exchange step (SURVEY.md §8e; the reference is single-GPU).  For one view the SH
  * gradient is rank-1 per Gaussian: dL_dsh[g,k,:] = basis_k(normalize(mean_g - campos)) * f[g,:]
@@ -297,7 +317,11 @@ int r3dg_unpremultiply_backward(int S, long long HW, const float* feature, const
  * render.py:88-93): features[P,S] = cat([depths, depths^2, src_0, src_1, ...], -1) with
  * depths = (cat([means3D, 1]) @ viewmatrix)[:, 2] — means3D / viewmatrix NULL: no depth channels.  S must equal
  * (2 if depth) + sum(width).  Backward: writes every source's gradient slice contiguous (ptr NULL: skipped) and, when
- * dL_dmeans3D is given, the gradient through the two depth channels. */
+ * dL_dmeans3D is given, the gradient through the two depth channels.  dL_dviewmatrix [16] (optional, NULL = none):
+ * the gradient of the depth channels with respect to viewmatrix, sum_g (g_z + 2 z g_z2) [m_g,1] in elements 2, 6, 10,
+ * 14 (the column that gives the depth) and exactly 0 elsewhere; summed in a fixed order through `work` (at least
+ * r3dg_raster_cam_grad_bytes(P, 1) bytes) like the rasterizer's camera gradients.  dL_dviewmatrix without depth
+ * channels or with too small a workspace returns R3DG_ERR_BAD_ARG. */
 #define R3DG_PACK_MAX 16
 typedef struct r3dg_pack_src {
     const float* ptr;              /* [P,width] contiguous (backward: destination of the gradient slice) */
@@ -307,7 +331,8 @@ int r3dg_pack_features_forward(int P, int S, const float* means3D, const float* 
                                const r3dg_pack_src* srcs, float* out, r3dg_stream_t stream);
 int r3dg_pack_features_backward(int P, int S, const float* means3D, const float* viewmatrix,
                                 const float* dL_dout, int num, const r3dg_pack_src* dsts,
-                                float* dL_dmeans3D, r3dg_stream_t stream);
+                                float* dL_dmeans3D, float* dL_dviewmatrix, void* work, size_t work_bytes,
+                                r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Densification surgery (SURVEY.md §8(f)3): stable compaction of the rows of MANY per-Gaussian tensors

@@ -198,10 +198,12 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
                                  tan_fovy, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
-                                 imageBuffer, backward_geometry, debug, _out=None):
+                                 imageBuffer, backward_geometry, debug, _out=None, cam_grads=False):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
-     dL_dscales, dL_drotations)."""
+     dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
+    follow: dL_dviewmatrix [4,4], dL_dprojmatrix [4,4] and dL_dcampos [3], in the element order of `viewmatrix`,
+    `projmatrix` and `campos`."""
     lib = _lib.load()
     P = means3D.size(0)
     S = features.size(1)
@@ -248,6 +250,7 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
         dL_dsh = _alloc("sh", (P, M, 3))
     dL_dscales = _alloc("scales", (P, 3))
     dL_drotations = _alloc("rotations", (P, 4))
+    cam = _cam_outputs(1, dev) if cam_grads else ()
     if P != 0:
         a = _lib.RasterBwdArgs()
         a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
@@ -268,9 +271,29 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
         det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(P, S), dev)
+        cam_ws = _cam_args(a, cam, P, 1, dev)
         _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_gaussians_backward")
     return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
-            dL_dscales, dL_drotations)
+            dL_dscales, dL_drotations) + tuple(t[0] for t in cam)
+
+
+def _cam_outputs(V, device):
+    """The camera-gradient outputs of a V-view backward: viewmatrix [V,4,4], projmatrix [V,4,4], campos [V,3], zeroed
+    (a call with P = 0 writes nothing; otherwise the library overwrites every element)."""
+    return (torch.zeros((V, 4, 4), dtype=torch.float32, device=device),
+            torch.zeros((V, 4, 4), dtype=torch.float32, device=device),
+            torch.zeros((V, 3), dtype=torch.float32, device=device))
+
+
+def _cam_args(a, cam, P, V, device):
+    """Enters the camera-gradient outputs `cam` (or none) and their workspace into the backward arguments `a`; returns
+    the workspace, which the caller holds until the call is enqueued."""
+    if not cam:
+        return None
+    ws = _lib.scratch(_lib.load().r3dg_raster_cam_grad_bytes(P, V), device)
+    a.dL_dviewmatrix, a.dL_dprojmatrix, a.dL_dcampos = (t.data_ptr() for t in cam)
+    a.cam_work, a.cam_work_bytes = ws.data_ptr(), ws.numel()
+    return ws
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):
@@ -404,11 +427,12 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
 def rasterize_views_backward(background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
                              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
-                             backward_geometry):
+                             backward_geometry, cam_grads=False):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
-    in view order; dL_dsh is rebuilt from the views' rank-1 factors."""
+    in view order; dL_dsh is rebuilt from the views' rank-1 factors.  With `cam_grads=True` each view's camera
+    gradients follow, never summed: dL_dviewmatrix [V,4,4], dL_dprojmatrix [V,4,4], dL_dcampos [V,3]."""
     lib = _lib.load()
     V = len(cams)
     P = means3D.size(0)
@@ -440,6 +464,7 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     sh_factor = torch.empty((V, P, 3), **f32) if M > 0 else None
     dL_dscales = torch.empty((P, 3), **f32)
     dL_drotations = torch.empty((P, 4), **f32)
+    cam = _cam_outputs(V, dev) if cam_grads else ()
     if P != 0:
         table = _view_cams(cams)
         a = _lib.RasterBwdArgs()
@@ -463,10 +488,11 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
         det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(V * P, S), dev)
+        cam_ws = _cam_args(a, cam, P, V, dev)
         _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_views_backward")
     else:
         for t in (dL_dmeans2D, dL_dmeans3D, dL_dfeatures, dL_dcolors, dL_dopacity, dL_dcov3D, dL_dsh, dL_dscales,
                   dL_drotations):
             t.zero_()
     return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
-            dL_dscales, dL_drotations)
+            dL_dscales, dL_drotations) + cam

@@ -49,6 +49,8 @@ class RasterBwdArgs(ctypes.Structure):
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
          ("binning", c_void_p), ("binning_bytes", c_size_t),
          ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
+         ("dL_dviewmatrix", c_void_p), ("dL_dprojmatrix", c_void_p), ("dL_dcampos", c_void_p),
+         ("cam_work", c_void_p), ("cam_work_bytes", c_size_t),
          ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -108,6 +110,7 @@ SYMBOLS = [
     ("r3dg_raster_views_img_n_contrib_offset", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_raster_forward", c_int, [ctypes.POINTER(RasterFwdArgs), c_void_p]),
     ("r3dg_raster_backward", c_int, [ctypes.POINTER(RasterBwdArgs), c_void_p]),
+    ("r3dg_raster_cam_grad_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_sh_grad_from_factors", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p]),
     ("r3dg_exchange_p2p", c_int, [ctypes.POINTER(ExchangeArgs), c_void_p]),
     ("r3dg_mark_visible", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -126,7 +129,8 @@ SYMBOLS = [
     ("r3dg_render_equation_forward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),
     ("r3dg_render_equation_backward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),
     ("r3dg_pack_features_forward", c_int, [c_int, c_int, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p, c_void_p]),
-    ("r3dg_pack_features_backward", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p, c_void_p]),
+    ("r3dg_pack_features_backward", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p,
+                                            c_void_p, c_void_p, c_size_t, c_void_p]),
     ("r3dg_compact_tmp_bytes", c_size_t, [c_int]),
     ("r3dg_compact_scan", c_int, [c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     ("r3dg_compact_rows", c_int, [c_int, c_int, ctypes.POINTER(CompactTensor), c_void_p, c_void_p, c_void_p]),

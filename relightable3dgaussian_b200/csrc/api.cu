@@ -173,6 +173,9 @@ size_t r3dg_raster_views_img_bytes(int W, int H, int V) { return ImgLayout(W, H,
 size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).n_contrib; }
 size_t r3dg_raster_fwd_det_bytes(int P) { return align_up((size_t)(P < 1 ? 1 : P) * 8, 256); }
 size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S)); }
+size_t r3dg_raster_cam_grad_bytes(int P, int V) {
+    return align_up((size_t)(V < 1 ? 1 : V) * kCamGradFloats * cam_grad_blocks(P) * sizeof(float), 256);
+}
 
 int r3dg_det_sum_host(long long n, const float* terms, float* out) {
     if (n < 0 || (n > 0 && !terms) || !out) return R3DG_ERR_BAD_ARG;
@@ -250,7 +253,18 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (V == 0) return R3DG_ERR_BAD_ARG;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S))) return R3DG_ERR_BAD_ARG;
     if (V > 1 && a->P > 0 && a->shs && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
-    if (a->P == 0) return 0;
+    const int cam_outs = (a->dL_dviewmatrix != nullptr) + (a->dL_dprojmatrix != nullptr) + (a->dL_dcampos != nullptr);
+    if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;
+    const bool cam = cam_outs == 3;
+    if (cam && (!a->cam_work || a->cam_work_bytes < r3dg_raster_cam_grad_bytes(a->P, V))) return R3DG_ERR_BAD_ARG;
+    if (a->P == 0) {
+        if (cam) {
+            R3DG_CUDA_TRY(cudaMemsetAsync(a->dL_dviewmatrix, 0, (size_t)V * 16 * sizeof(float), stream));
+            R3DG_CUDA_TRY(cudaMemsetAsync(a->dL_dprojmatrix, 0, (size_t)V * 16 * sizeof(float), stream));
+            R3DG_CUDA_TRY(cudaMemsetAsync(a->dL_dcampos, 0, (size_t)V * 3 * sizeof(float), stream));
+        }
+        return 0;
+    }
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
                             a->binning_bytes, b, V);
@@ -266,8 +280,12 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
         if ((rc = r3dg_sh_grad_from_factors(a->P, a->D, a->M, V, a->means3D, a->campos, a->dL_dsh_factor, 1.0f, a->dL_dsh,
                                             stream_)) != 0) return rc;
     }
+    if (cam) {                      // every view's camera gradients from its CTAs' partial sums
+        const CamGradOut o = {{a->dL_dviewmatrix, a->dL_dprojmatrix, a->dL_dcampos}, {16, 16, 3}};
+        if ((rc = launch_cam_grad_sum((const float*)a->cam_work, cam_grad_blocks(a->P), V, o, stream)) != 0) return rc;
+    }
     prof_mark(false, 10, stream);
-    g_launches += 2 + V;   // CTA order, composite, projection per view (the SH rebuild counts itself)
+    g_launches += 2 + V + (cam ? 1 : 0);   // CTA order, composite, projection per view, camera sums (the SH rebuild counts itself)
     if (g_prof.on) g_prof.bwd_calls++;
     if (a->debug) {
         cudaError_t e = cudaStreamSynchronize(stream);
@@ -392,10 +410,12 @@ int r3dg_pack_features_forward(int P, int S, const float* means3D, const float* 
     return launch_pack_features_forward(P, S, means3D, viewmatrix, num, srcs, out, num_sms(), (cudaStream_t)stream);
 }
 int r3dg_pack_features_backward(int P, int S, const float* means3D, const float* viewmatrix, const float* dL_dout, int num,
-                                const r3dg_pack_src* dsts, float* dL_dmeans3D, r3dg_stream_t stream) {
+                                const r3dg_pack_src* dsts, float* dL_dmeans3D, float* dL_dviewmatrix, void* work,
+                                size_t work_bytes, r3dg_stream_t stream) {
     if (num > 0 && !dsts) return R3DG_ERR_BAD_ARG;
-    g_launches += P > 0 ? 1 : 0;
-    return launch_pack_features_backward(P, S, means3D, viewmatrix, dL_dout, num, dsts, dL_dmeans3D, num_sms(), (cudaStream_t)stream);
+    g_launches += P > 0 ? (dL_dviewmatrix ? 3 : 1) : 0;
+    return launch_pack_features_backward(P, S, means3D, viewmatrix, dL_dout, num, dsts, dL_dmeans3D, dL_dviewmatrix, work,
+                                         work_bytes, num_sms(), (cudaStream_t)stream);
 }
 
 size_t r3dg_compact_tmp_bytes(int P) { return compact_tmp_bytes(P < 0 ? 0 : P); }

@@ -128,6 +128,39 @@ __global__ void __launch_bounds__(256) pack_features_bwd_kernel(const PackTable 
     }
 }
 
+// dL/dviewmatrix of the depth channels, one partial sum per CTA of 256 Gaussians: column j of the stored matrix
+// (elements 4j + 2) gets sum_g (g_z + 2 z g_z2) [m_g,1]_j, every other element 0.  Fixed order: a butterfly per warp,
+// then the 8 warps in order.  work: [16][gridDim.x], one column per CTA.
+__global__ void __launch_bounds__(256) pack_view_grad_kernel(const PackTable t, const float* __restrict__ g,
+                                                             float* __restrict__ work) {
+    __shared__ float part[4][8];
+    const long long p = (long long)blockIdx.x * 256 + threadIdx.x;
+    float c[4] = {0.f, 0.f, 0.f, 0.f};
+    if (p < t.P) {
+        const float* m = t.means3D + 3 * p;
+        const float z = view_depth(t.view, m);
+        const float s = g[p * t.S] + 2.0f * z * g[p * t.S + 1];
+        c[0] = s * m[0]; c[1] = s * m[1]; c[2] = s * m[2]; c[3] = s;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c[j] += __shfl_xor_sync(0xffffffffu, c[j], o);
+        if ((threadIdx.x & 31) == 0) part[j][threadIdx.x >> 5] = c[j];
+    }
+    __syncthreads();
+    if (threadIdx.x < 16) {
+        const int k = threadIdx.x;
+        float s = 0.f;
+        if ((k & 3) == 2) {
+            s = part[k >> 2][0];
+#pragma unroll
+            for (int w = 1; w < 8; ++w) s += part[k >> 2][w];
+        }
+        work[(size_t)k * gridDim.x + blockIdx.x] = s;
+    }
+}
+
 static int make_table(PackTable& t, int P, int S, const float* means3D, const float* view, int num, const r3dg_pack_src* srcs,
                       bool need_ptr) {
     if (P < 0 || S <= 0 || num < 0 || num > R3DG_PACK_MAX) return R3DG_ERR_BAD_ARG;
@@ -151,12 +184,26 @@ int launch_pack_features_forward(int P, int S, const float* means3D, const float
 }
 
 int launch_pack_features_backward(int P, int S, const float* means3D, const float* view, const float* g, int num,
-                                  const r3dg_pack_src* dsts, float* d_means3D, int num_sms, cudaStream_t stream) {
+                                  const r3dg_pack_src* dsts, float* d_means3D, float* d_view, void* work, size_t work_bytes,
+                                  int num_sms, cudaStream_t stream) {
     PackTable t;
     const int rc = make_table(t, P, S, means3D, view, num, dsts, false);
-    if (rc != 0 || P == 0) return rc;
+    if (rc != 0) return rc;
+    const int nblk = (P + 255) / 256;
+    if (d_view && (t.depth == 0 || !work || work_bytes < r3dg_raster_cam_grad_bytes(P, 1))) return R3DG_ERR_BAD_ARG;
+    static_assert(16 * 2 <= kCamGradFloats, "the pack's [16][P / 256] partials fit in r3dg_raster_cam_grad_bytes(P, 1)");
+    if (P == 0) {
+        if (d_view) R3DG_CUDA_TRY(cudaMemsetAsync(d_view, 0, 16 * sizeof(float), stream));
+        return 0;
+    }
     pack_features_bwd_kernel<<<grid_for((long long)P * S, num_sms), 256, 0, stream>>>(t, g, d_means3D);
     R3DG_CUDA_TRY(cudaGetLastError());
+    if (d_view) {
+        pack_view_grad_kernel<<<nblk, 256, 0, stream>>>(t, g, (float*)work);
+        R3DG_CUDA_TRY(cudaGetLastError());
+        const CamGradOut o = {{d_view, nullptr, nullptr}, {16, 0, 0}};
+        return launch_cam_grad_sum((const float*)work, nblk, 1, o, stream);
+    }
     return 0;
 }
 

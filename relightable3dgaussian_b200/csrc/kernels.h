@@ -72,6 +72,19 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
 int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
 int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream);
 
+// Camera gradients: the terms of one view in the order viewmatrix [16], projmatrix [16], campos [3].  The projection
+// backward writes one partial sum of them per CTA of kCamGradThreads Gaussians; launch_cam_grad_sum adds the partials
+// in CTA order.
+constexpr int kCamGradFloats = 35;
+constexpr int kCamGradThreads = 128;
+inline int cam_grad_blocks(int P) { return ((P < 1 ? 1 : P) + kCamGradThreads - 1) / kCamGradThreads; }
+struct CamGradOut {
+    float* out[3];                 // column k of the partials goes to the segment it falls in, [V, n[s]] per segment
+    int n[3];
+};
+// projection_bwd.cu: out from the [V][sum n][nblk] partials in `work`, one fixed-order sum per (view, column)
+int launch_cam_grad_sum(const float* work, int nblk, int V, const CamGradOut& o, cudaStream_t stream);
+
 size_t bvh_build_tmp_bytes(int P);
 size_t bvh_packets_bytes(int P);
 int launch_bvh_leaf_aabbs(int P, const float* means3D, const float* scales, const float* rotations,
@@ -97,7 +110,8 @@ int launch_unpremultiply_backward(int S, long long HW, const float* feature, con
 int launch_pack_features_forward(int P, int S, const float* means3D, const float* view, int num, const r3dg_pack_src* srcs,
                                  float* out, int num_sms, cudaStream_t stream);
 int launch_pack_features_backward(int P, int S, const float* means3D, const float* view, const float* g, int num,
-                                  const r3dg_pack_src* dsts, float* d_means3D, int num_sms, cudaStream_t stream);
+                                  const r3dg_pack_src* dsts, float* d_means3D, float* d_view, void* work, size_t work_bytes,
+                                  int num_sms, cudaStream_t stream);
 
 int shade_tune(const char* key, int value, int* previous);
 int composite_tune(const char* key, int value, int* previous);

@@ -32,7 +32,10 @@ struct ProjBwdParams {
     // instead of writing it — acc for the gradients summed over the views, acc_colors / acc_features for dL_dcolors /
     // dL_dfeatures when those inputs are shared (per-view inputs get per-view rows: no accumulation)
     bool acc, acc_colors, acc_features;
+    // CAM: this view's [kCamGradFloats][gridDim.x] partial sums of the camera gradients (column-major: one column per CTA)
+    float* cam_work;
 };
+static_assert(kCamGradThreads == 128, "cam_grad_blocks() counts projection-backward CTAs");
 
 // out = x, or out += x when `acc` (the left fold of several views' gradients)
 __device__ __forceinline__ void put(float* out, float x, bool acc) { *out = acc ? *out + x : x; }
@@ -62,7 +65,9 @@ __device__ __forceinline__ void cov3d_plain(const float* s3, float mod, const fl
 #define PROJ_THREADS 128
 #define SLAB_LD (PROJ_THREADS + 1)
 // DET (deterministic mode): the packed gradient row is read from the fixed-point accumulators and converted on load.
-template <bool DET = false>
+// CAM (camera gradients): every thread also stages its Gaussian's 35 camera-gradient terms in a [35][SLAB_LD] slab
+// behind the SH slab, and the CTA writes their sums in a fixed order to its column of p.cam_work.
+template <bool DET = false, bool CAM = false>
 __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const ProjBwdParams p) {
     // SH rows (192 B at M=16) travel through shared memory: the CTA's [128][3M] slab of shs is ONE contiguous
     // 24 KB block, fetched by a single TMA-unit bulk copy (cp.async.bulk, mbarrier-signalled) into a row-major
@@ -86,6 +91,11 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     const int idx = in_range ? idx_raw : p.P - 1;      // clamp: out-of-range threads only help with the slab
     const int rowf = 3 * p.M, block_base = blockIdx.x * PROJ_THREADS;
     const int nvalid = min(PROJ_THREADS, p.P - block_base);
+    float* sG = sSH + (p.shs ? rowf * SLAB_LD : 0) + threadIdx.x;   // CAM: this thread's terms at sG[k * SLAB_LD]
+    if constexpr (CAM) {
+#pragma unroll
+        for (int k = 0; k < kCamGradFloats; ++k) sG[k * SLAB_LD] = 0.f;   // culled and out-of-range rows add nothing
+    }
     // the thread's own rows are requested before the cooperative slab load so that both are in flight
     // together (nothing can be hoisted across the barrier below by the compiler)
     const float4* g4 = reinterpret_cast<const float4*>(p.grad + (size_t)idx * p.recf);
@@ -220,6 +230,27 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
         dmean3[0] += (proj[0] * m_w - proj[3] * mul1) * dmean2[0] + (proj[1] * m_w - proj[3] * mul2) * dmean2[1];
         dmean3[1] += (proj[4] * m_w - proj[7] * mul1) * dmean2[0] + (proj[5] * m_w - proj[7] * mul2) * dmean2[1];
         dmean3[2] += (proj[8] * m_w - proj[11] * mul1) * dmean2[0] + (proj[9] * m_w - proj[11] * mul2) * dmean2[1];
+        if constexpr (CAM) {
+            // viewmatrix: t_k = sum_j [m,1]_j V[4j + k] (k < 3) gives dL/dt (x) [m,1]; the 3x3 block also enters
+            // T = W J directly (T0[r] = V[4r] J00 + V[4r + 2] J02, T1[r] = V[4r + 1] J11 + V[4r + 2] J12).  Column 3 is
+            // never read.
+            const float mt[4] = {mx, my, mz, 1.f};
+            const float dt[3] = {dL_dtx, dL_dty, gz};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                float d0 = dt[0] * mt[j], d1 = dt[1] * mt[j], d2 = dt[2] * mt[j];
+                if (j < 3) { d0 += dT0[j] * J00; d1 += dT1[j] * J11; d2 += dT0[j] * J02 + dT1[j] * J12; }
+                sG[(4 * j + 0) * SLAB_LD] = d0; sG[(4 * j + 1) * SLAB_LD] = d1; sG[(4 * j + 2) * SLAB_LD] = d2;
+            }
+            // projmatrix: ndc = (h_0, h_1) / (h_3 + 1e-7) with h_k = sum_j [m,1]_j P[4j + k]; column 2 is never read
+            const float dh0 = dmean2[0] * m_w, dh1 = dmean2[1] * m_w, dh3 = -(dmean2[0] * mul1 + dmean2[1] * mul2);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                sG[(16 + 4 * j + 0) * SLAB_LD] = dh0 * mt[j];
+                sG[(16 + 4 * j + 1) * SLAB_LD] = dh1 * mt[j];
+                sG[(16 + 4 * j + 3) * SLAB_LD] = dh3 * mt[j];
+            }
+        }
 
         // ---- cov3D -> scale / rotation (backward.cu:280-343) ----------------------------------
         if (have_sr) {
@@ -352,9 +383,18 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             // dnormvdv (auxiliary.h:105-116)
             const float sum2 = dox * dox + doy * doy + doz * doz;
             const float invsum32 = 1.0f / sqrtf(sum2 * sum2 * sum2);
-            dmean3[0] += ((+sum2 - dox * dox) * ddx - doy * dox * ddy - doz * dox * ddz) * invsum32;
-            dmean3[1] += (-dox * doy * ddx + (sum2 - doy * doy) * ddy - doz * doy * ddz) * invsum32;
-            dmean3[2] += (-dox * doz * ddx - doy * doz * ddy + (sum2 - doz * doz) * ddz) * invsum32;
+            const float ddir[3] = {(+sum2 - dox * dox) * ddx - doy * dox * ddy - doz * dox * ddz,
+                                   -dox * doy * ddx + (sum2 - doy * doy) * ddy - doz * doy * ddz,
+                                   -dox * doz * ddx - doy * doz * ddy + (sum2 - doz * doz) * ddz};
+            // explicit FMAs: the contraction of `dmean3 += ddir * invsum32` must not depend on whether the product
+            // has a second use (CAM), so that dL/dmeans3D is the same with and without camera gradients
+            dmean3[0] = __fmaf_rn(ddir[0], invsum32, dmean3[0]);
+            dmean3[1] = __fmaf_rn(ddir[1], invsum32, dmean3[1]);
+            dmean3[2] = __fmaf_rn(ddir[2], invsum32, dmean3[2]);
+            if constexpr (CAM) {            // campos: the view direction is mean - campos
+#pragma unroll
+                for (int k = 0; k < 3; ++k) sG[(32 + k) * SLAB_LD] = -(ddir[k] * invsum32);
+            }
         }
     } else if (p.shs && p.dL_dsh) {
         if (bulk) {
@@ -390,6 +430,20 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             }
         }
     }
+    if constexpr (CAM) {
+        // the CTA's sum of each term: warp w takes terms w, w + 4, ...; each lane adds rows lane, +32, +64, +96 in that
+        // order, then a butterfly over the lanes — a fixed order, so equal gradient rows give equal bits
+        __syncthreads();
+        const float* col = sSH + (p.shs ? rowf * SLAB_LD : 0);
+        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+        for (int k = warp; k < kCamGradFloats; k += PROJ_THREADS / 32) {
+            const float* r = col + k * SLAB_LD;
+            float s = ((r[lane] + r[lane + 32]) + r[lane + 64]) + r[lane + 96];
+#pragma unroll
+            for (int m = 16; m > 0; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
+            if (lane == 0) p.cam_work[(size_t)k * gridDim.x + blockIdx.x] = s;
+        }
+    }
     if (!in_range) return;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -412,6 +466,37 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     } else {
         *drot4 = make_float4(drot[0], drot[1], drot[2], drot[3]);
     }
+}
+
+// One CTA per (column k, view v): the sum of the column's nblk partials work[(v * width + k) * nblk + i] in a fixed
+// order (each thread adds i = t, t + 256, ... in turn, then a butterfly per warp, then the 8 warps in order), written
+// to the output segment column k falls in.
+__global__ void __launch_bounds__(256) cam_grad_sum_kernel(const float* __restrict__ work, int nblk, const CamGradOut o) {
+    __shared__ float part[8];
+    const int k = blockIdx.x, v = blockIdx.y, width = gridDim.x;
+    const float* col = work + ((size_t)v * width + k) * nblk;
+    float s = 0.f;
+    for (int i = threadIdx.x; i < nblk; i += 256) s += col[i];
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = part[0];
+#pragma unroll
+        for (int w = 1; w < 8; ++w) t += part[w];
+        const int k1 = o.n[0], k2 = o.n[0] + o.n[1];
+        if (k < k1) o.out[0][(size_t)v * o.n[0] + k] = t;
+        else if (k < k2) o.out[1][(size_t)v * o.n[1] + (k - k1)] = t;
+        else o.out[2][(size_t)v * o.n[2] + (k - k2)] = t;
+    }
+}
+
+int launch_cam_grad_sum(const float* work, int nblk, int V, const CamGradOut& o, cudaStream_t stream) {
+    const int width = o.n[0] + o.n[1] + o.n[2];
+    cam_grad_sum_kernel<<<dim3(width, V), 256, 0, stream>>>(work, nblk, o);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
 }
 
 int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream) {
@@ -444,7 +529,14 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     p.acc_features = later && !a.features_per_view;
     const size_t sh_smem = a.shs ? (size_t)3 * a.M * SLAB_LD * sizeof(float) : 0;
     const int blocks = (a.P + PROJ_THREADS - 1) / PROJ_THREADS;
-    if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    // camera gradients (r3dg_raster_backward checked that all three outputs and the workspace are given): view v's
+    // partials follow the earlier views' in the workspace
+    const bool cam = a.dL_dviewmatrix != nullptr;
+    p.cam_work = cam ? (float*)a.cam_work + (size_t)v * kCamGradFloats * blocks : nullptr;
+    const size_t cam_smem = sh_smem + (size_t)kCamGradFloats * SLAB_LD * sizeof(float);
+    if (cam && a.deterministic) projection_bwd_kernel<true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
+    else if (cam) projection_bwd_kernel<false, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
+    else if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
     else projection_bwd_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;

@@ -85,13 +85,14 @@ def _snapshot(args):
 
 
 class _RasterizeGaussians(torch.autograd.Function):
-    """Autograd node (reference :58-185).  Inputs/outputs and the set of differentiable inputs
-    are the reference's; cotangents of normal / surface_xyz / weights / n_contrib / radii are
-    ignored exactly as there (:123-124 vs :132-157)."""
+    """Autograd node (reference :58-185).  Inputs/outputs are the reference's; cotangents of normal / surface_xyz /
+    weights / n_contrib / radii are ignored exactly as there (:123-124 vs :132-157).  Unlike the reference, the
+    settings' `viewmatrix`, `projmatrix` and `campos` are inputs of the node as well (the same tensors, passed after
+    the settings): they get gradients when they require them, and the backward computes those only then."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings):
+                cov3Ds_precomp, raster_settings, viewmatrix, projmatrix, campos):
         rs = raster_settings
         args = (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations,
                 rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
@@ -144,10 +145,12 @@ class _RasterizeGaussians(torch.autograd.Function):
                                    "part in it (debug mode or no `shs` input): every rank must run the same collectives")
             ex = _EXCHANGE
         kw = {} if ex is None else {"_out": {"sh_factor": ex[0].factor}}
+        if any(ctx.needs_input_grad[10:13]):         # viewmatrix, projmatrix, campos
+            kw["cam_grads"] = True
         if rs.debug:
             saved = _snapshot(args)
             try:
-                grads = _C.rasterize_gaussians_backward(*args)
+                grads = _C.rasterize_gaussians_backward(*args, **kw)
             except Exception:
                 torch.save(saved, "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
@@ -171,9 +174,26 @@ class _RasterizeGaussians(torch.autograd.Function):
             g_sh_avg = exchange.rebuild_sh(means3D, campos_all, rs.sh_degree)
             grads = grads[:6] + (g_sh_avg,) + grads[7:]
         (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
-         g_rotations) = grads
+         g_rotations) = grads[:9]
         return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
-                g_rotations, g_cov3Ds, None)
+                g_rotations, g_cov3Ds, None) + _camera_grads(ctx, grads[9:], (rs.viewmatrix, rs.projmatrix, rs.campos))
+
+
+def _camera_grads(ctx, grads, inputs):
+    """The gradients of the node's last three inputs (viewmatrix, projmatrix, campos) in their shapes: None for those
+    that do not need one (and for all three when none was computed)."""
+    need = ctx.needs_input_grad[-3:]
+    if not grads:
+        return (None, None, None)
+    return tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads, inputs, need))
+
+
+def _refuse_camera_grad_with_exchange(*cameras):
+    """A gradient exchange renders one view per rank; camera gradients are not part of it."""
+    if _EXCHANGE is not None and torch.is_grad_enabled() and any(
+            isinstance(t, torch.Tensor) and t.requires_grad for t in cameras):
+        raise RuntimeError("camera gradients (a viewmatrix, projmatrix or campos that requires grad) cannot be combined "
+                           "with an installed gradient exchange (set_grad_exchange)")
 
 
 _CALL_GRAD_MODE = True      # grad mode of the caller (inside autograd.Function.forward it is always off)
@@ -182,9 +202,12 @@ _CALL_GRAD_MODE = True      # grad mode of the caller (inside autograd.Function.
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
                         rotations, cov3Ds_precomp, raster_settings):
     global _CALL_GRAD_MODE
+    rs = raster_settings
+    _refuse_camera_grad_with_exchange(rs.viewmatrix, rs.projmatrix, rs.campos)
     _CALL_GRAD_MODE = torch.is_grad_enabled()
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
-                                     scales, rotations, cov3Ds_precomp, raster_settings)
+                                     scales, rotations, cov3Ds_precomp, raster_settings, rs.viewmatrix,
+                                     rs.projmatrix, rs.campos)
 
 
 class GaussianRasterizer(nn.Module):
@@ -226,12 +249,9 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings):
+                settings, viewmatrix, projmatrix, campos):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
-        viewmatrix = torch.stack([s.viewmatrix for s in settings])
-        projmatrix = torch.stack([s.projmatrix for s in settings])
-        campos = torch.stack([s.campos for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
         out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
@@ -257,11 +277,11 @@ class _RasterizeViews(torch.autograd.Function):
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
                                             cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
                                             g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
-                                            rs.backward_geometry)
+                                            rs.backward_geometry, cam_grads=any(ctx.needs_input_grad[10:13]))
         (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
-         g_rotations) = grads
+         g_rotations) = grads[:9]
         return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
-                g_rotations, g_cov3Ds, None)
+                g_rotations, g_cov3Ds, None) + _camera_grads(ctx, grads[9:], (viewmatrix, projmatrix, campos))
 
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
@@ -315,8 +335,12 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
     if features is None:
         features = torch.empty_like(means3D[..., :0])
+    # stacked here, outside the node, so that autograd routes each view's camera gradients to that view's tensors
+    viewmatrix = torch.stack([s.viewmatrix for s in settings])
+    projmatrix = torch.stack([s.projmatrix for s in settings])
+    campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
-                                 cov3D_precomp, tuple(settings))
+                                 cov3D_precomp, tuple(settings), viewmatrix, projmatrix, campos)
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
@@ -372,26 +396,32 @@ class _PackFeatures(torch.autograd.Function):
         if P > 0:
             _lib.call("r3dg_pack_features_forward", dev, P, S, _lib.ptr(m), _lib.ptr(v), len(srcs), arr, out.data_ptr(),
                       what="pack_features")
-        ctx.meta = (P, S, [tuple(t.shape) for t in tensors], [t.shape[1] for t in srcs], depth)
+        ctx.meta = (P, S, [tuple(t.shape) for t in tensors], [t.shape[1] for t in srcs], depth,
+                    tuple(viewmatrix.shape) if depth else None)
         ctx.save_for_backward(*([m, v] if depth else []))
         return out
 
     @staticmethod
     def backward(ctx, g):
-        P, S, shapes, widths, depth = ctx.meta
+        P, S, shapes, widths, depth, v_shape = ctx.meta
         m, v = ctx.saved_tensors if depth else (None, None)
         dev = g.device
         g = _lib.f32(g)
         need = ctx.needs_input_grad
         outs = [torch.empty((P, w), dtype=torch.float32, device=dev) if need[2 + k] else None for k, w in enumerate(widths)]
         d_m = torch.empty((P, 3), dtype=torch.float32, device=dev) if depth and need[0] else None
+        # dL/dviewmatrix: zeros for P = 0 (no call), otherwise every element is written
+        d_v = torch.zeros((16,), dtype=torch.float32, device=dev) if depth and need[1] else None
+        ws = _lib.scratch(_lib.load().r3dg_raster_cam_grad_bytes(P, 1), dev) if d_v is not None else None
         arr = (_lib.PackSrc * max(len(widths), 1))()
         for k, w in enumerate(widths):
             arr[k].ptr, arr[k].width = (outs[k].data_ptr() if outs[k] is not None else None), w
         if P > 0:
             _lib.call("r3dg_pack_features_backward", dev, P, S, _lib.ptr(m), _lib.ptr(v), g.data_ptr(), len(widths), arr,
-                      _lib.ptr(d_m), what="pack_features backward")
-        return (d_m, None) + tuple(o.view(s) if o is not None else None for o, s in zip(outs, shapes))
+                      _lib.ptr(d_m), _lib.ptr(d_v), _lib.ptr(ws), ws.numel() if ws is not None else 0,
+                      what="pack_features backward")
+        return ((d_m, d_v.view(v_shape) if d_v is not None else None) +
+                tuple(o.view(s) if o is not None else None for o, s in zip(outs, shapes)))
 
 
 def pack_features(tensors, means3D=None, viewmatrix=None):
@@ -399,5 +429,6 @@ def pack_features(tensors, means3D=None, viewmatrix=None):
     the rasterizer (gaussian_renderer/neilf.py:110-126, render.py:88-93):
         depths = (cat([means3D, 1]) @ viewmatrix)[:, 2:3];  features = cat([depths, depths.square(), *tensors], -1)
     (without means3D / viewmatrix: a plain fused cat).  One pass forward, one backward that writes every source
-    gradient contiguous.  No gradient flows to `viewmatrix` (a camera constant in the reference)."""
+    gradient contiguous.  When `viewmatrix` requires grad it gets the gradient of the depth channels,
+    sum_g (g_z + 2 z g_z2) [m_g,1] in the column that gives the depth (zero elsewhere), summed in a fixed order."""
     return _PackFeatures.apply(means3D, viewmatrix, *tensors)
