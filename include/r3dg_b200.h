@@ -169,6 +169,29 @@ typedef struct r3dg_raster_bwd_args {
     float* dL_dprojmatrix;
     float* dL_dcampos;
     void* cam_work; size_t cam_work_bytes;
+    /* Gradients of the pseudo-normal and surface-xyz outputs (optional; both cotangents NULL = none, the default: the
+     * forward's out_normal / out_surface_xyz are then constants, as in the reference).
+     *   dL_dout_normal, dL_dout_surface_xyz: [V,3,H,W]; either may be NULL, which means zero.
+     *   fwd_opacity, fwd_depth: [V,1,H,W], the forward's out_opacity / out_depth (required with either cotangent).
+     *   cx, cy: the principal point of a call with V = 0 or 1, which must be set (a call with V > 1 reads each view's
+     *           from view_cams; there these fields are unused).
+     * One launch per view runs the adjoint of the forward's surface/normal pass: it adds the cotangents' pull-back to
+     * dL_dout_depth and dL_dout_opacity, writes the sums to surface_work, and the backward compositor runs unchanged on
+     * them.  With dL_dviewmatrix, the pseudo-normal's term sum_pixels g_normal_k N_i is added to element 4k + i after
+     * the projection's term, summed in a fixed order (one more launch).  No float atomics: bitwise reproducible.
+     * surface_work: device workspace of at least r3dg_raster_surface_grad_bytes(W, H, V) bytes, laid out as
+     *   [0]                                   float [2][V][H][W]: the combined depth cotangents of all views, then the
+     *                                         combined opacity cotangents (the planes the compositor consumed);
+     *   [align256(8 V H W)]                   float [V][9][blocks]: per-CTA partials of the camera term, blocks =
+     *                                         ceil(W / 32) ceil(H / 8).
+     * A cotangent without both forward images, or a missing or too small workspace, returns R3DG_ERR_BAD_ARG before
+     * anything is launched.  P = 0 launches nothing (every gradient is zero). */
+    const float* dL_dout_normal;
+    const float* dL_dout_surface_xyz;
+    const float* fwd_opacity;
+    const float* fwd_depth;
+    float cx, cy;
+    void* surface_work; size_t surface_work_bytes;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_raster_bwd_det_bytes(P, S) bytes, zeroed by the call.  0 = the default path (det_work unused). */
@@ -182,6 +205,9 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* args, r3dg_stream_t stream)
 /* Workspace of the camera gradients of a V-view backward (r3dg_raster_bwd_args.cam_work); P = 0 and V < 1 are sized
  * as 1.  r3dg_raster_cam_grad_bytes(P, 1) also covers the workspace of r3dg_pack_features_backward. */
 size_t r3dg_raster_cam_grad_bytes(int P, int V);
+/* Workspace of the pseudo-normal / surface-xyz gradients of a V-view backward (r3dg_raster_bwd_args.surface_work):
+ * align256(8 V W H) + align256(36 V ceil(W / 32) ceil(H / 8)) bytes; W, H and V below 1 are sized as 1. */
+size_t r3dg_raster_surface_grad_bytes(int W, int H, int V);
 
 /* Multi-GPU exchange step (SURVEY.md §8e; the reference is single-GPU).  For one view the SH
  * gradient is rank-1 per Gaussian: dL_dsh[g,k,:] = basis_k(normalize(mean_g - campos)) * f[g,:]

@@ -198,12 +198,16 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx,
                                  tan_fovy, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
-                                 imageBuffer, backward_geometry, debug, _out=None, cam_grads=False):
+                                 imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
+                                 surface_work=None):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
     follow: dL_dviewmatrix [4,4], dL_dprojmatrix [4,4] and dL_dcampos [3], in the element order of `viewmatrix`,
-    `projmatrix` and `campos`."""
+    `projmatrix` and `campos`.  `surface` (not part of the reference surface either) differentiates the pseudo-normal
+    and surface-xyz outputs: (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth, cx, cy) with the forward's
+    opacity and depth images; a cotangent may be None.  `surface_work` optionally supplies the workspace
+    (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards."""
     lib = _lib.load()
     P = means3D.size(0)
     S = features.size(1)
@@ -272,6 +276,8 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
         det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(P, S), dev)
         cam_ws = _cam_args(a, cam, P, 1, dev)
+        surface_ws = _surface_args(a, surface and surface[:4], W, H, 1, dev, surface_work,
+                                   principal=surface[4:6] if surface is not None and len(surface) == 6 else None)
         _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_gaussians_backward")
     return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
             dL_dscales, dL_drotations) + tuple(t[0] for t in cam)
@@ -294,6 +300,29 @@ def _cam_args(a, cam, P, V, device):
     a.dL_dviewmatrix, a.dL_dprojmatrix, a.dL_dcampos = (t.data_ptr() for t in cam)
     a.cam_work, a.cam_work_bytes = ws.data_ptr(), ws.numel()
     return ws
+
+
+def _surface_args(a, surface, W, H, V, device, work=None, principal=None):
+    """Enters the pseudo-normal / surface-xyz cotangents `surface` = (dL_dout_normal, dL_dout_surface_xyz, opacity,
+    depth) (or none) and their workspace into the backward arguments `a`; returns the cotangents and the workspace,
+    which the caller holds until the call is enqueued.  Both cotangents None: nothing is entered.  `principal` = (cx, cy)
+    is the principal point of a one-view call (V = 1), which the library reads from `a.cx, a.cy`, and is required
+    then: a V-view call (V > 1) reads every view's own from its camera table."""
+    if surface is None or (surface[0] is None and surface[1] is None):
+        return None
+    if V <= 1 and principal is None:
+        raise ValueError("the surface gradients of a one-view call need the forward's principal point (cx, cy)")
+    g_normal, g_xyz = (None if g is None else _prep(g, name) for g, name in
+                       ((surface[0], "dL_dout_normal"), (surface[1], "dL_dout_surface_xyz")))
+    opacity, depth = _prep(surface[2], "out_opacity"), _prep(surface[3], "out_depth")
+    if work is None:
+        work = _lib.scratch(_lib.load().r3dg_raster_surface_grad_bytes(W, H, V), device)
+    a.dL_dout_normal, a.dL_dout_surface_xyz = _lib.ptr(g_normal), _lib.ptr(g_xyz)
+    a.fwd_opacity, a.fwd_depth = _lib.ptr(opacity), _lib.ptr(depth)
+    if principal is not None:
+        a.cx, a.cy = float(principal[0]), float(principal[1])
+    a.surface_work, a.surface_work_bytes = work.data_ptr(), work.numel()
+    return g_normal, g_xyz, opacity, depth, work
 
 
 def mark_visible(means3D, viewmatrix, projmatrix):
@@ -427,12 +456,15 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
 def rasterize_views_backward(background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
                              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
-                             backward_geometry, cam_grads=False):
+                             backward_geometry, cam_grads=False, surface=None, surface_work=None):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
     in view order; dL_dsh is rebuilt from the views' rank-1 factors.  With `cam_grads=True` each view's camera
-    gradients follow, never summed: dL_dviewmatrix [V,4,4], dL_dprojmatrix [V,4,4], dL_dcampos [V,3]."""
+    gradients follow, never summed: dL_dviewmatrix [V,4,4], dL_dprojmatrix [V,4,4], dL_dcampos [V,3].  `surface` =
+    (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth), all [V,*,H,W] (a cotangent may be None), and
+    `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
+    one view, cams[0]'s, entered as the call's cx, cy)."""
     lib = _lib.load()
     V = len(cams)
     P = means3D.size(0)
@@ -489,6 +521,7 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
         det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(V * P, S), dev)
         cam_ws = _cam_args(a, cam, P, V, dev)
+        surface_ws = _surface_args(a, surface, W, H, V, dev, surface_work, principal=(cams[0][2], cams[0][3]))
         _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_views_backward")
     else:
         for t in (dL_dmeans2D, dL_dmeans3D, dL_dfeatures, dL_dcolors, dL_dopacity, dL_dcov3D, dL_dsh, dL_dscales,

@@ -51,6 +51,8 @@ class RasterBwdArgs(ctypes.Structure):
          ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
          ("dL_dviewmatrix", c_void_p), ("dL_dprojmatrix", c_void_p), ("dL_dcampos", c_void_p),
          ("cam_work", c_void_p), ("cam_work_bytes", c_size_t),
+         ("dL_dout_normal", c_void_p), ("dL_dout_surface_xyz", c_void_p), ("fwd_opacity", c_void_p), ("fwd_depth", c_void_p),
+         ("cx", c_float), ("cy", c_float), ("surface_work", c_void_p), ("surface_work_bytes", c_size_t),
          ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -111,6 +113,7 @@ SYMBOLS = [
     ("r3dg_raster_forward", c_int, [ctypes.POINTER(RasterFwdArgs), c_void_p]),
     ("r3dg_raster_backward", c_int, [ctypes.POINTER(RasterBwdArgs), c_void_p]),
     ("r3dg_raster_cam_grad_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_raster_surface_grad_bytes", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_sh_grad_from_factors", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p]),
     ("r3dg_exchange_p2p", c_int, [ctypes.POINTER(ExchangeArgs), c_void_p]),
     ("r3dg_mark_visible", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -176,6 +176,10 @@ size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1
 size_t r3dg_raster_cam_grad_bytes(int P, int V) {
     return align_up((size_t)(V < 1 ? 1 : V) * kCamGradFloats * cam_grad_blocks(P) * sizeof(float), 256);
 }
+size_t r3dg_raster_surface_grad_bytes(int W, int H, int V) {
+    const size_t v = V < 1 ? 1 : V, hw = (size_t)(W < 1 ? 1 : W) * (H < 1 ? 1 : H);
+    return align_up(2 * v * hw * sizeof(float), 256) + align_up(v * 9 * surface_grad_blocks(W, H) * sizeof(float), 256);
+}
 
 int r3dg_det_sum_host(long long n, const float* terms, float* out) {
     if (n < 0 || (n > 0 && !terms) || !out) return R3DG_ERR_BAD_ARG;
@@ -257,6 +261,9 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;
     const bool cam = cam_outs == 3;
     if (cam && (!a->cam_work || a->cam_work_bytes < r3dg_raster_cam_grad_bytes(a->P, V))) return R3DG_ERR_BAD_ARG;
+    const bool surface = a->dL_dout_normal || a->dL_dout_surface_xyz;
+    if (surface && (!a->fwd_opacity || !a->fwd_depth || !a->dL_dout_opacity || !a->dL_dout_depth || !a->surface_work ||
+                    a->surface_work_bytes < r3dg_raster_surface_grad_bytes(a->W, a->H, V))) return R3DG_ERR_BAD_ARG;
     if (a->P == 0) {
         if (cam) {
             R3DG_CUDA_TRY(cudaMemsetAsync(a->dL_dviewmatrix, 0, (size_t)V * 16 * sizeof(float), stream));
@@ -270,6 +277,22 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
                             a->binning_bytes, b, V);
     if (rc != 0) return rc;
     prof_mark(false, 8, stream);
+    // pseudo-normal / surface-xyz cotangents: their pull-back joins the depth and opacity cotangents, and the compositor
+    // runs on the sums (its stage of the profiler includes this pass)
+    r3dg_raster_bwd_args sa;
+    const bool surface_cam = surface && cam && a->dL_dout_normal;
+    const int surface_blocks = surface_grad_blocks(a->W, a->H);
+    float* surface_part = nullptr;
+    if (surface) {
+        float* planes = (float*)a->surface_work;
+        surface_part = surface_cam ? (float*)((char*)a->surface_work + align_up(2 * (size_t)V * a->W * a->H * sizeof(float), 256))
+                                   : nullptr;
+        if ((rc = launch_surface_backward(*a, V, planes, surface_part, stream)) != 0) return rc;
+        sa = *a;
+        sa.dL_dout_depth = planes;
+        sa.dL_dout_opacity = planes + (size_t)V * a->W * a->H;
+        a = &sa;
+    }
     if ((rc = launch_composite_backward(*a, b, stream)) != 0) return rc;
     prof_mark(false, 9, stream);
     // one projection backward per view, in view order: view 0 writes the summed gradients, every later view adds its
@@ -284,8 +307,12 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
         const CamGradOut o = {{a->dL_dviewmatrix, a->dL_dprojmatrix, a->dL_dcampos}, {16, 16, 3}};
         if ((rc = launch_cam_grad_sum((const float*)a->cam_work, cam_grad_blocks(a->P), V, o, stream)) != 0) return rc;
     }
+    if (surface_cam &&              // then the pseudo-normal's term of dL/dviewmatrix, added after the projection's
+        (rc = launch_surface_cam_sum(surface_part, surface_blocks, V, a->dL_dviewmatrix, stream)) != 0) return rc;
     prof_mark(false, 10, stream);
-    g_launches += 2 + V + (cam ? 1 : 0);   // CTA order, composite, projection per view, camera sums (the SH rebuild counts itself)
+    // CTA order, composite, projection per view, camera sums (the SH rebuild counts itself); surface pass per view and
+    // its camera sums
+    g_launches += 2 + V + (cam ? 1 : 0) + (surface ? V : 0) + (surface_cam ? 1 : 0);
     if (g_prof.on) g_prof.bwd_calls++;
     if (a->debug) {
         cudaError_t e = cudaStreamSynchronize(stream);

@@ -85,6 +85,13 @@ struct CamGradOut {
 // projection_bwd.cu: out from the [V][sum n][nblk] partials in `work`, one fixed-order sum per (view, column)
 int launch_cam_grad_sum(const float* work, int nblk, int V, const CamGradOut& o, cudaStream_t stream);
 
+// surface_bwd.cu: the adjoint of the pseudo-normal / surface-xyz pass, one launch per view.  planes: [2][V][H][W] (the
+// combined depth cotangents, then opacity); cam_part: [V][9][surface_grad_blocks(W, H)] or null (no camera term).
+int surface_grad_blocks(int W, int H);
+int launch_surface_backward(const r3dg_raster_bwd_args& a, int V, float* planes, float* cam_part, cudaStream_t stream);
+// dL_dviewmatrix[v][4k + i] += the sum of view v's partials of entry 3k + i in CTA order (one launch for all views)
+int launch_surface_cam_sum(const float* cam_part, int nblk, int V, float* dL_dviewmatrix, cudaStream_t stream);
+
 size_t bvh_build_tmp_bytes(int P);
 size_t bvh_packets_bytes(int P);
 int launch_bvh_leaf_aabbs(int P, const float* means3D, const float* scales, const float* rotations,

@@ -85,14 +85,15 @@ def _snapshot(args):
 
 
 class _RasterizeGaussians(torch.autograd.Function):
-    """Autograd node (reference :58-185).  Inputs/outputs are the reference's; cotangents of normal / surface_xyz /
-    weights / n_contrib / radii are ignored exactly as there (:123-124 vs :132-157).  Unlike the reference, the
-    settings' `viewmatrix`, `projmatrix` and `campos` are inputs of the node as well (the same tensors, passed after
-    the settings): they get gradients when they require them, and the backward computes those only then."""
+    """Autograd node (reference :58-185).  Inputs/outputs are the reference's; cotangents of weights / n_contrib /
+    radii are ignored exactly as there (:123-124 vs :132-157), and so are those of normal / surface_xyz unless
+    `surface_grads` is set.  Unlike the reference, the settings' `viewmatrix`, `projmatrix` and `campos` are inputs of
+    the node as well (the same tensors, passed after the settings): they get gradients when they require them, and the
+    backward computes those only then."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, viewmatrix, projmatrix, campos):
+                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos):
         rs = raster_settings
         args = (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations,
                 rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
@@ -117,8 +118,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         # cotangents are filled in below when a loss does not touch one of them
         ctx.set_materialize_grads(False)
         ctx.out_shapes = (color.shape, opacity.shape, depth.shape, feature.shape)
+        ctx.surface_grads = surface_grads
         ctx.save_for_backward(colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
-                              radii, sh, geomBuffer, binningBuffer, imgBuffer, opacities)
+                              radii, sh, geomBuffer, binningBuffer, imgBuffer, opacities,
+                              *((opacity, depth) if surface_grads else ()))
         return (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz,
                 weights, radii)
 
@@ -127,7 +130,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                  g_normal, g_surface_xyz, g_weights, g_radii):
         rs = ctx.raster_settings
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, radii, sh,
-         geomBuffer, binningBuffer, imgBuffer, opacities) = ctx.saved_tensors
+         geomBuffer, binningBuffer, imgBuffer, opacities) = ctx.saved_tensors[:12]
         zeros = lambda g, shape: g if g is not None else torch.zeros(shape, dtype=torch.float32, device=means3D.device)
         g_color, g_opacity = zeros(g_color, ctx.out_shapes[0]), zeros(g_opacity, ctx.out_shapes[1])
         g_depth, g_feature = zeros(g_depth, ctx.out_shapes[2]), zeros(g_feature, ctx.out_shapes[3])
@@ -145,8 +148,11 @@ class _RasterizeGaussians(torch.autograd.Function):
                                    "part in it (debug mode or no `shs` input): every rank must run the same collectives")
             ex = _EXCHANGE
         kw = {} if ex is None else {"_out": {"sh_factor": ex[0].factor}}
-        if any(ctx.needs_input_grad[10:13]):         # viewmatrix, projmatrix, campos
+        if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
             kw["cam_grads"] = True
+        surface = ctx.surface_grads and (g_normal is not None or g_surface_xyz is not None)
+        if surface:                                  # with the forward's opacity and depth images
+            kw["surface"] = (g_normal, g_surface_xyz) + tuple(ctx.saved_tensors[12:14]) + (rs.cx, rs.cy)
         if rs.debug:
             saved = _snapshot(args)
             try:
@@ -167,6 +173,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                                              rs.tanfovy, rs.cx, rs.cy, rs.image_height, rs.image_width, sh, rs.sh_degree,
                                              rs.campos, rs.prefiltered, rs.computer_pseudo_normal, False,
                                              _min_capacity=int(ctx.num_rendered) + 4096)
+                if surface:                     # the adjoint of the re-run's own surface pass
+                    kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
                 grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
         if ex is not None:                      # SH gradient: gather the views' factors, rebuild the mean locally
             exchange, campos_all = ex
@@ -176,7 +184,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
          g_rotations) = grads[:9]
         return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
-                g_rotations, g_cov3Ds, None) + _camera_grads(ctx, grads[9:], (rs.viewmatrix, rs.projmatrix, rs.campos))
+                g_rotations, g_cov3Ds, None, None) + _camera_grads(ctx, grads[9:], (rs.viewmatrix, rs.projmatrix, rs.campos))
 
 
 def _camera_grads(ctx, grads, inputs):
@@ -199,21 +207,35 @@ def _refuse_camera_grad_with_exchange(*cameras):
 _CALL_GRAD_MODE = True      # grad mode of the caller (inside autograd.Function.forward it is always off)
 
 
+def _refuse_surface_grads_without_normals(surface_grads, computer_pseudo_normal):
+    """Without the pseudo-normal pass both outputs are zeros: there is nothing to differentiate."""
+    if surface_grads and not computer_pseudo_normal:
+        raise ValueError("surface_grads=True needs computer_pseudo_normal=True: without it the normal and surface_xyz "
+                         "outputs are zeros and have no gradient")
+
+
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
-                        rotations, cov3Ds_precomp, raster_settings):
+                        rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False):
+    """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
+    cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
+    when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
+    ignored as in the reference."""
     global _CALL_GRAD_MODE
     rs = raster_settings
+    _refuse_surface_grads_without_normals(surface_grads, rs.computer_pseudo_normal)
     _refuse_camera_grad_with_exchange(rs.viewmatrix, rs.projmatrix, rs.campos)
     _CALL_GRAD_MODE = torch.is_grad_enabled()
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
-                                     scales, rotations, cov3Ds_precomp, raster_settings, rs.viewmatrix,
-                                     rs.projmatrix, rs.campos)
+                                     scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
+                                     rs.viewmatrix, rs.projmatrix, rs.campos)
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings):
+    def __init__(self, raster_settings, surface_grads=False):
+        """`surface_grads` (not part of the reference surface): see rasterize_gaussians."""
         super().__init__()
         self.raster_settings = raster_settings
+        self.surface_grads = surface_grads
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -237,7 +259,8 @@ class GaussianRasterizer(nn.Module):
         if features is None:
             features = torch.empty_like(means3D[..., :0])
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
-                                   scales, rotations, cov3D_precomp, self.raster_settings)
+                                   scales, rotations, cov3D_precomp, self.raster_settings,
+                                   surface_grads=self.surface_grads)
 
 
 _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
@@ -249,7 +272,7 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, viewmatrix, projmatrix, campos):
+                settings, surface_grads, viewmatrix, projmatrix, campos):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
@@ -261,8 +284,10 @@ class _RasterizeViews(torch.autograd.Function):
         ctx.meta = (rs, cams)
         ctx.set_materialize_grads(False)
         ctx.out_shapes = (color.shape, opacity.shape, depth.shape, feature.shape)
+        ctx.surface_grads = surface_grads
         ctx.save_for_backward(colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix,
-                              projmatrix, campos, geomBuffer, binningBuffer, imgBuffer)
+                              projmatrix, campos, geomBuffer, binningBuffer, imgBuffer,
+                              *((opacity, depth) if surface_grads else ()))
         return (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz, weights, radii)
 
     @staticmethod
@@ -270,22 +295,26 @@ class _RasterizeViews(torch.autograd.Function):
                  g_weights, g_radii):
         rs, cams = ctx.meta
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
-         geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors
+         geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors[:14]
         zeros = lambda g, shape: g if g is not None else torch.zeros(shape, dtype=torch.float32, device=means3D.device)
         g_color, g_opacity = zeros(g_color, ctx.out_shapes[0]), zeros(g_opacity, ctx.out_shapes[1])
         g_depth, g_feature = zeros(g_depth, ctx.out_shapes[2]), zeros(g_feature, ctx.out_shapes[3])
+        surface = None
+        if ctx.surface_grads and (g_normal is not None or g_surface_xyz is not None):
+            surface = (g_normal, g_surface_xyz) + tuple(ctx.saved_tensors[14:16])
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
                                             cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
                                             g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
-                                            rs.backward_geometry, cam_grads=any(ctx.needs_input_grad[10:13]))
+                                            rs.backward_geometry, cam_grads=any(ctx.needs_input_grad[11:14]),
+                                            surface=surface)
         (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
          g_rotations) = grads[:9]
         return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
-                g_rotations, g_cov3Ds, None) + _camera_grads(ctx, grads[9:], (viewmatrix, projmatrix, campos))
+                g_rotations, g_cov3Ds, None, None) + _camera_grads(ctx, grads[9:], (viewmatrix, projmatrix, campos))
 
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
-                    rotations=None, cov3D_precomp=None, features=None):
+                    rotations=None, cov3D_precomp=None, features=None, surface_grads=False):
     """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
 
     `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
@@ -298,7 +327,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
     Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
-    `MAX_VIEWS` views or V·P >= 2^30 rows."""
+    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads` is that of rasterize_gaussians, per view."""
     settings = list(settings)
     V = len(settings)
     if V < 1:
@@ -309,6 +338,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
         vals = {getattr(s, name) for s in settings}
         if len(vals) != 1:
             raise ValueError(f"rasterize_views: the views disagree on {name} ({sorted(vals)}); it must be shared")
+    _refuse_surface_grads_without_normals(surface_grads, settings[0].computer_pseudo_normal)
     if any(s.debug for s in settings):
         raise ValueError("rasterize_views does not support debug=True; render the views one by one to debug")
     if _EXCHANGE is not None:
@@ -340,7 +370,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     projmatrix = torch.stack([s.projmatrix for s in settings])
     campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
-                                 cov3D_precomp, tuple(settings), viewmatrix, projmatrix, campos)
+                                 cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos)
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
