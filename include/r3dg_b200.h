@@ -261,7 +261,8 @@ int r3dg_mark_visible(int P, const float* means3D, const float* viewmatrix,
  *      | 18 bmask u8[R]: per list entry, bit b = 8x4 pixel block b of the entry's tile (row b >> 1,
  *      column b & 1) meets the Gaussian's block rectangle | 19 cmask u8[R]: per list entry, bit b =
  *      block b composited the entry in the forward | 20 brects u32[2P]: per Gaussian the inclusive
- *      block rectangle {bx0 | bx1 << 16, by0 | by1 << 16} (empty when bx0 > bx1)
+ *      block rectangle {bx0 | bx1 << 16, by0 | by1 << 16} (empty when bx0 > bx1) | 22 composited
+ *      u8[P]: 1 when some pixel composited the Gaussian (the backward reads and zeroes its rows only)
  *      (9, 18, 19: the copy stops at max_bytes, pass R entries' worth)
  * Returns bytes written or a negative error. */
 long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom,

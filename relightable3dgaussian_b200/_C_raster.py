@@ -350,7 +350,8 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
             "final_T": (13, torch.float32, (H, W)), "n_contrib": (14, torch.int32, (H, W)),
             "ranges": (15, torch.int32, (T, 2)), "bwd_work": (16, torch.int32, (T, 2)),
             "bwd_order": (17, torch.int32, (2 * T,)), "bmask": (18, torch.uint8, (num_rendered,)),
-            "cmask": (19, torch.uint8, (num_rendered,)), "brects": (20, torch.int32, (P, 2))}[name]
+            "cmask": (19, torch.uint8, (num_rendered,)), "brects": (20, torch.int32, (P, 2)),
+            "composited": (22, torch.uint8, (P,))}[name]
     out = torch.empty(spec[2], dtype=spec[1], device=geomBuffer.device)
     if out.numel() == 0:
         return out

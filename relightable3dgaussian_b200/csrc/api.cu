@@ -310,9 +310,9 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (surface_cam &&              // then the pseudo-normal's term of dL/dviewmatrix, added after the projection's
         (rc = launch_surface_cam_sum(surface_part, surface_blocks, V, a->dL_dviewmatrix, stream)) != 0) return rc;
     prof_mark(false, 10, stream);
-    // CTA order, composite, projection per view, camera sums (the SH rebuild counts itself); surface pass per view and
-    // its camera sums
-    g_launches += 2 + V + (cam ? 1 : 0) + (surface ? V : 0) + (surface_cam ? 1 : 0);
+    // zeroing of the composited rows, CTA order, composite, projection per view, camera sums (the SH rebuild counts
+    // itself); surface pass per view and its camera sums
+    g_launches += 3 + V + (cam ? 1 : 0) + (surface ? V : 0) + (surface_cam ? 1 : 0);
     if (g_prof.on) g_prof.bwd_calls++;
     if (a->debug) {
         cudaError_t e = cudaStreamSynchronize(stream);
@@ -559,6 +559,10 @@ __global__ void unpack_clamped_kernel(int P, const uint8_t* __restrict__ cl, con
     const unsigned c = tiles[i] > 0 ? cl[i] : 0u;
     dst[3 * i] = c & 1u; dst[3 * i + 1] = (c >> 1) & 1u; dst[3 * i + 2] = (c >> 2) & 1u;
 }
+__global__ void unpack_composited_kernel(int P, const uint8_t* __restrict__ cl, uint8_t* __restrict__ dst) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < P) dst[i] = (cl[i] & kComposited) ? 1 : 0;
+}
 }  // namespace
 
 long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom_, const void* img_,
@@ -601,6 +605,7 @@ long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void*
         case 16: return copy(b.bwd_work, 8 * (size_t)b.tiles);
         case 17: return copy(b.bwd_order, 8 * (size_t)b.tiles);
         case 20: return copy(b.brects, 8 * (size_t)P);
+        case 22: if (max_bytes < P) return -1; if (P) unpack_composited_kernel<<<nb, 256, 0, stream>>>(P, b.clamped, (uint8_t*)dst); return P;
         case 9: case 10: case 18: case 19: {
             if (!binned) return -1;
             // caller limits the copy to R entries through max_bytes

@@ -147,14 +147,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
 
 // Asynchronous, coalesced copy of a CTA's [nvalid][rowf] float slab into the TRANSPOSED shared slab
 // s[k * ld + t] (element k of row t): every warp instruction moves 32 consecutive floats (128 B of
-// global memory) to 32 different banks.  nthreads = blockDim.x.
+// global memory) to 32 different banks.  nthreads = blockDim.x.  rows: null, or a bit mask of the rows to copy (bit
+// t & 31 of rows[t >> 5]); the other rows' slab entries are left as they are.
 __device__ __forceinline__ void load_rows_transposed_async(float* s, int ld, const float* __restrict__ src,
-                                                           int nvalid, int rowf, int nthreads) {
+                                                           int nvalid, int rowf, int nthreads,
+                                                           const uint32_t* rows = nullptr) {
     const int total = nvalid * rowf;
     const int dq = nthreads / rowf, dm = nthreads - dq * rowf;
     int t = (int)threadIdx.x / rowf, k = (int)threadIdx.x - t * rowf;
     for (int i = threadIdx.x; i < total; i += nthreads) {
-        cp_async4(s + k * ld + t, src + i);
+        if (!rows || ((rows[t >> 5] >> (t & 31)) & 1u)) cp_async4(s + k * ld + t, src + i);
         k += dm; t += dq;
         if (k >= rowf) { k -= rowf; ++t; }
     }

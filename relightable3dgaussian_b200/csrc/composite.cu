@@ -43,6 +43,7 @@ struct CompositeFwdParams {
     int* n_contrib;
     float *out_color, *out_opacity, *out_depth, *out_feature, *out_weights;
     uint64_t* det_weights;             // DET: [P] out_weights in exact 2^-24 units (zeroed), converted by det_weights_kernel
+    uint32_t* clamped32;               // the rows' clamped bytes as words: kComposited is set for every composited row
 };
 
 // NW = warps per CTA (4: two CTAs per tile).  Warps are autonomous: no
@@ -246,10 +247,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             if (__all_sync(0xffffffffu, done)) { all_done = true; break; }      // once per round: entries after the last
         }                                                                        // pixel finished change nothing (valid needs !done)
         if (last_j >= 0) last_contributor = q[(h0 + last_j) & (R3DG_QCAP - 1)] + 1u;     // 1-based position in the tile list
-        if constexpr (DET) {
-            if (my_wsum != 0) det_red_u64(p.det_weights + sId[warp][lane], (uint64_t)(uint32_t)my_wsum);   // my_wsum > 0
-        } else {
-            if (my_wsum != 0) atomicAdd(&p.out_weights[sId[warp][lane]], (float)my_wsum * (1.0f / 16777216.0f));
+        if (my_wsum != 0) {
+            const uint32_t id = sId[warp][lane];
+            if constexpr (DET) det_red_u64(p.det_weights + id, (uint64_t)(uint32_t)my_wsum);   // my_wsum > 0
+            else atomicAdd(&p.out_weights[id], (float)my_wsum * (1.0f / 16777216.0f));
+            // the row was composited: its gradient row is zeroed and read in the backward (no byte atomics: OR the word)
+            atomicOr(&p.clamped32[id >> 2], kComposited << (8 * (id & 3u)));
         }
         stage ^= 1;
         composited += (uint32_t)__popc(cw);
@@ -385,6 +388,7 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
     p.out_color = a.out_color; p.out_opacity = a.out_opacity; p.out_depth = a.out_depth;
     p.out_feature = a.out_feature; p.out_weights = a.out_weights;
     p.det_weights = a.deterministic ? (uint64_t*)a.det_work : nullptr;
+    p.clamped32 = (uint32_t*)b.clamped;               // 256-byte aligned, padded to whole words (api.cu GeomLayout)
     const size_t rows = (size_t)V * a.P;
     if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, rows * 8, stream));
     const int tiles = V * b.tiles;                    // the tall grid of all views

@@ -42,8 +42,8 @@ struct CompositeBwdParams {
     const float* final_T;
     const int* n_contrib;
     const float *dL_dpix, *dL_dpix_o, *dL_dpix_d, *dL_dpix_f;
-    float* grad;     // [P][recf], zero-initialised
-    DetAcc det;      // DET: the same rows as fixed-point accumulators (detacc.cuh), [P * recf], zero-initialised
+    float* grad;     // [P][recf], the composited rows zero-initialised (zero_composited_rows_kernel)
+    DetAcc det;      // DET: the same rows as fixed-point accumulators (detacc.cuh), [P * recf], as grad
 };
 
 // Sum v[i] over the 32 lanes for every i in [0,N) (N power of two, 4 <= N <= 32) with a
@@ -415,6 +415,29 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     }
 }
 
+// Zeroes the gradient rows the kernel above adds to: exactly the rows the forward pass composited (kComposited), since
+// it walks only their contributor bits.  Every other row is neither written nor read in the backward, so ~80 % of the
+// rows of a dense scene are never touched.  One thread per row.  DET: the row's accumulators in the three word planes
+// and its flag bits, which are recf / 4 whole bytes (2 bits per accumulator, recf a multiple of 4).
+template <bool DET>
+__global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, int recf, const uint8_t* __restrict__ clamped,
+                                                                   float* __restrict__ grad, const DetAcc det) {
+    const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= rows || !(clamped[r] & kComposited)) return;
+    if constexpr (DET) {
+#pragma unroll 1
+        for (int plane = 0; plane < 3; ++plane) {
+            uint4* w = reinterpret_cast<uint4*>(det.words + plane * det.n + r * recf);
+            for (int i = 0; i < recf / 2; ++i) w[i] = make_uint4(0u, 0u, 0u, 0u);
+        }
+        uint8_t* f = reinterpret_cast<uint8_t*>(det.flags) + r * (recf / 4);
+        for (int i = 0; i < recf / 4; ++i) f[i] = 0;
+    } else {
+        float4* g = reinterpret_cast<float4*>(grad + r * recf);
+        for (int i = 0; i < recf / 4; ++i) g[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+}
+
 // resident CTAs per SM the register allocation is pinned to, by channel groups NG (the occupancy sweep in DESIGN.md §4.2)
 template <int NG> struct BwdOcc { static constexpr int v = NG <= 3 ? 5 : (NG <= 5 ? 4 : 3); };
 int g_bwd_ctas = 0;             // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
@@ -448,9 +471,12 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     p.grad = b.grad;
     p.n_contrib = b.n_contrib;
     const bool det = a.deterministic != 0;
-    p.det = det_acc(a.det_work, (size_t)V * a.P * b.recf);
-    if (det) R3DG_CUDA_TRY(cudaMemsetAsync(a.det_work, 0, det_bytes(p.det.n), stream));
-    else R3DG_CUDA_TRY(cudaMemsetAsync(p.grad, 0, (size_t)V * a.P * b.recf * 4, stream));
+    const size_t rows = (size_t)V * a.P;
+    p.det = det_acc(a.det_work, rows * b.recf);
+    // zeroed here, in the backward, so that every backward over one forward (retain_graph) starts from zero
+    const int zblocks = (int)((rows + 255) / 256);
+    if (det) zero_composited_rows_kernel<true><<<zblocks, 256, 0, stream>>>(rows, b.recf, b.clamped, p.grad, p.det);
+    else zero_composited_rows_kernel<false><<<zblocks, 256, 0, stream>>>(rows, b.recf, b.clamped, p.grad, p.det);
     const int tiles = V * b.tiles;                    // the tall grid of all views
     int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;

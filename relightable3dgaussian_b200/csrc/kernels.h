@@ -13,7 +13,7 @@ struct RasterBuffers {
     float *rec, *grad;
     uint32_t* tiles_touched;
     uint2 *rects, *brects;
-    uint8_t* clamped;
+    uint8_t* clamped;                                                              // bits 0-2: SH colour clamped; kComposited
     char* sort;                                                                    // laid out by sort_layout
     SortLayout sort_layout{0};
     float* final_T;                                                                // img: per pixel and per tile
@@ -34,6 +34,11 @@ struct RasterBuffers {
     uint32_t row_base;                                                             // slice: first row of the view (v * P)
     const GeomHeader* prev_header;                                                 // slice: the previous view's header or null
 };
+
+// Bit 3 of a row's clamped byte: some pixel composited the row in the forward pass (its out_weights is > 0).  The
+// projection writes every row's byte with the bit clear, the forward compositor sets it.  Every other row's gradient is
+// exactly zero, so the backward neither zeroes nor reads it.
+constexpr unsigned kComposited = 8u;
 
 // api.cu: view v's slice: header, sort region, per-Gaussian rows and tile ranges of that view.  The binning lists stay
 // shared (the views' lists follow each other in one buffer) and the tall grid's tile order is built once for all views.

@@ -272,24 +272,17 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
         }
     }
     float rgb[3] = {0.f, 0.f, 0.f};
+    unsigned cl = 0;                                   // clamped channels; kComposited is set by the forward compositor
     if (p.colors_precomp == nullptr) {
         if (slab_loaded) {
             if (slab_bulk) {
                 mbar_wait(&sBar, 0);                       // all transaction bytes of the slab have landed
-                if (alive) {
-                    // row-major slab: this thread's row as 16-byte vectors (LDS.128: 4 consecutive rows span all banks)
-                    unsigned cl = 0;
-                    sh_to_rgb(p.D, px, py, pz, sCam, sSH + (size_t)threadIdx.x * rowf, 0, rgb, cl);
-                    p.clamped[idx] = (uint8_t)cl;
-                }
+                // row-major slab: this thread's row as 16-byte vectors (LDS.128: 4 consecutive rows span all banks)
+                if (alive) sh_to_rgb(p.D, px, py, pz, sCam, sSH + (size_t)threadIdx.x * rowf, 0, rgb, cl);
             } else {
                 cp_async_wait_all();
                 __syncthreads();
-                if (alive) {
-                    unsigned cl = 0;
-                    sh_to_rgb(p.D, px, py, pz, sCam, sSH + threadIdx.x, PROJ_THREADS + 1, rgb, cl);
-                    p.clamped[idx] = (uint8_t)cl;
-                }
+                if (alive) sh_to_rgb(p.D, px, py, pz, sCam, sSH + threadIdx.x, PROJ_THREADS + 1, rgb, cl);
             }
         }
     } else if (alive) {
@@ -332,8 +325,10 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
         }
         p.radii[idx] = my_radius;
         p.tiles_touched[idx] = (uint32_t)((y1 - y0) * (x1 - x0));
+        p.clamped[idx] = (uint8_t)cl;
     } else if (idx < p.P) {
         for (int g = 0; g < rec4n; ++g) srow[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+        p.clamped[idx] = 0;                            // culled: never composited
     }
     fence_proxy_async_smem();                          // this thread's shared-memory stores -> visible to the bulk-copy engine
     __syncthreads();

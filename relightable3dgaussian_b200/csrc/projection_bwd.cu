@@ -19,10 +19,9 @@ struct ProjBwdParams {
     const float *means3D, *shs, *colors_precomp, *scales, *rotations, *cov3D_precomp, *viewmatrix,
         *projmatrix, *campos;
     float scale_modifier, tan_fovx, tan_fovy, h_x, h_y;
-    const int* radii_rec;       // unused (radius is read from the record)
     const float* rec;
     const float* grad;
-    const uint8_t* clamped;
+    const uint8_t* clamped;     // bits 0-2: SH colour clamped, kComposited: the row is live (read and differentiated)
     float *dL_dmeans2D, *dL_dcolors, *dL_dopacity, *dL_dmeans3D, *dL_dfeatures, *dL_dcov3D, *dL_dsh,
         *dL_dscales, *dL_drotations;
     float* dL_dsh_factor;       // [P,3] gated dL_dRGB (multi-GPU exchange, sh_exchange.cu); dL_dsh may then be NULL
@@ -72,10 +71,16 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     // SH rows (192 B at M=16) travel through shared memory: the CTA's [128][3M] slab of shs is ONE contiguous
     // 24 KB block, fetched by a single TMA-unit bulk copy (cp.async.bulk, mbarrier-signalled) into a row-major
     // slab; every thread turns its row into dL/dsh in place (16-byte vector accesses) and ONE bulk store writes the
-    // slab back (zeros for culled rows).  Rows that are not 16-byte multiples (SH degree 0 / 2) or ragged / unaligned
-    // tails use the transposed slab s[k * SLAB_LD + t] with 4-byte LDGSTS copies and a coalesced write-back loop.
+    // slab back (zeros for rows that are not live).  Rows that are not 16-byte multiples (SH degree 0 / 2) or ragged /
+    // unaligned tails use the transposed slab s[k * SLAB_LD + t] with 4-byte LDGSTS copies and a coalesced write-back
+    // loop.
+    // Only LIVE rows — some pixel composited them in the forward pass (kComposited) — read anything: every other row's
+    // gradients are exactly zero, and it writes +0 to its outputs without reading its gradient row, parameters or SH.
+    // A CTA whose rows are all live fetches its SH slab with the one bulk copy; otherwise each live row is fetched on its
+    // own (one bulk copy per row, or the transposed LDGSTS loads of the live rows only).
     extern __shared__ __align__(16) float sSH[];
     __shared__ float sV[16], sPr[16], sCam[3];
+    __shared__ uint32_t sLive[PROJ_THREADS / 32];
     __shared__ __align__(8) uint64_t sBar;
     const int rowf_ = 3 * p.M, base_ = blockIdx.x * PROJ_THREADS;
     const unsigned slab_bytes = (unsigned)min(PROJ_THREADS, p.P - base_) * (unsigned)rowf_ * 4u;
@@ -85,25 +90,26 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     if (threadIdx.x == 0 && bulk) { mbar_init(&sBar, 1); fence_proxy_async_smem(); }
     if (threadIdx.x < 16) { sV[threadIdx.x] = p.viewmatrix[threadIdx.x]; sPr[threadIdx.x] = p.projmatrix[threadIdx.x]; }
     if (threadIdx.x < 3) sCam[threadIdx.x] = p.campos[threadIdx.x];
-    __syncthreads();
     const int idx_raw = blockIdx.x * blockDim.x + threadIdx.x;
     const bool in_range = idx_raw < p.P;
     const int idx = in_range ? idx_raw : p.P - 1;      // clamp: out-of-range threads only help with the slab
+    const unsigned cl = in_range ? p.clamped[idx] : 0u;
+    const bool live = (cl & kComposited) != 0;         // composited => visible
+    const uint32_t live_warp = __ballot_sync(0xffffffffu, live);
+    if ((threadIdx.x & 31) == 0) sLive[threadIdx.x >> 5] = live_warp;
+    const int nlive = __syncthreads_count(live);
     const int rowf = 3 * p.M, block_base = blockIdx.x * PROJ_THREADS;
     const int nvalid = min(PROJ_THREADS, p.P - block_base);
     float* sG = sSH + (p.shs ? rowf * SLAB_LD : 0) + threadIdx.x;   // CAM: this thread's terms at sG[k * SLAB_LD]
     if constexpr (CAM) {
 #pragma unroll
-        for (int k = 0; k < kCamGradFloats; ++k) sG[k * SLAB_LD] = 0.f;   // culled and out-of-range rows add nothing
+        for (int k = 0; k < kCamGradFloats; ++k) sG[k * SLAB_LD] = 0.f;   // rows that are not live add nothing
     }
-    // the thread's own rows are requested before the cooperative slab load so that both are in flight
-    // together (nothing can be hoisted across the barrier below by the compiler)
+    // the thread's own rows are requested before the cooperative slab load so that both are in flight together
     const float4* g4 = reinterpret_cast<const float4*>(p.grad + (size_t)idx * p.recf);
-    const bool visible = in_range && p.radii_rec[idx] > 0;
     float4 gA = make_float4(0, 0, 0, 0), gB = gA, gC = gA, q4 = gA;
     float m3[3] = {0, 0, 0}, s3[3] = {0, 0, 0};
-    unsigned cl = 0;
-    if (visible) {
+    if (live) {
         if constexpr (DET) {
             const size_t r0 = (p.det_row0 + idx) * p.recf;
             gA = make_float4(det_load(p.det, r0), det_load(p.det, r0 + 1), det_load(p.det, r0 + 2), det_load(p.det, r0 + 3));
@@ -117,32 +123,40 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             q4 = *reinterpret_cast<const float4*>(p.rotations + 4 * (size_t)idx);
             s3[0] = p.scales[3 * (size_t)idx]; s3[1] = p.scales[3 * (size_t)idx + 1]; s3[2] = p.scales[3 * (size_t)idx + 2];
         }
-        if (p.shs) cl = p.clamped[idx];
     }
-    if (p.shs) {     // asynchronous copy of the slab, overlapped with the covariance chain below
+    const bool fetch_sh = p.shs && nlive > 0;          // (CTA-uniform)
+    if (fetch_sh) {  // asynchronous copy of the live rows of the slab, overlapped with the covariance chain below
         if (bulk) {
-            if (threadIdx.x == 0) { mbar_arrive_expect_tx(&sBar, slab_bytes); bulk_copy_g2s(sSH, p.shs + (size_t)block_base * rowf, slab_bytes, &sBar); }
+            const unsigned row_bytes = (unsigned)rowf * 4u;
+            if (nlive == nvalid) {                     // every row: the one contiguous slab
+                if (threadIdx.x == 0) { mbar_arrive_expect_tx(&sBar, slab_bytes); bulk_copy_g2s(sSH, p.shs + (size_t)block_base * rowf, slab_bytes, &sBar); }
+            } else {
+                // one copy per live row into its slab row; a copy may land before thread 0 announces the bytes (the
+                // barrier's transaction count may go negative), the phase completes only after that single arrival
+                if (threadIdx.x == 0) mbar_arrive_expect_tx(&sBar, (unsigned)nlive * row_bytes);
+                if (live) bulk_copy_g2s(sSH + (size_t)threadIdx.x * rowf, p.shs + (size_t)idx * rowf, row_bytes, &sBar);
+            }
         } else {
-            load_rows_transposed_async(sSH, SLAB_LD, p.shs + (size_t)block_base * rowf, nvalid, rowf, PROJ_THREADS);
+            load_rows_transposed_async(sSH, SLAB_LD, p.shs + (size_t)block_base * rowf, nvalid, rowf, PROJ_THREADS,
+                                       nlive == nvalid ? nullptr : sLive);
             cp_async_commit();
         }
     }
     const float* V = sV;
     const float* proj = sPr;
-    // (visibility comes from tiles_touched: the record row of a culled Gaussian is never written)
 
     float dmean2[3] = {0, 0, 0}, dcol[3] = {0, 0, 0}, dop = 0, dmean3[3] = {0, 0, 0}, dfac[3] = {0, 0, 0};
     float dcov[6] = {0, 0, 0, 0, 0, 0}, dscale[3] = {0, 0, 0}, drot[4] = {0, 0, 0, 0};
 
-    // feature gradients: straight copy-out of the packed row
-    if (p.S > 0 && in_range) {
+    // feature gradients: straight copy-out of the packed row (a row that is not live adds nothing to earlier views')
+    if (p.S > 0 && in_range && (live || !p.acc_features)) {
         float* df = p.dL_dfeatures + (size_t)idx * p.S;
         for (int c = 0; c < p.S; ++c) {
-            if constexpr (DET) put(df + c, visible ? det_load(p.det, (p.det_row0 + idx) * p.recf + 11 + c) : 0.0f, p.acc_features);
-            else put(df + c, visible ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f, p.acc_features);
+            if constexpr (DET) put(df + c, live ? det_load(p.det, (p.det_row0 + idx) * p.recf + 11 + c) : 0.0f, p.acc_features);
+            else put(df + c, live ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f, p.acc_features);
         }
     }
-    if (visible) {
+    if (live) {
         dmean2[0] = gA.x; dmean2[1] = gA.y; dmean2[2] = gA.z; dop = gA.w;
         dcol[0] = gC.x; dcol[1] = gC.y; dcol[2] = gC.z;
         const float mx = m3[0], my = m3[1], mz = m3[2];
@@ -289,11 +303,11 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
         }
     }
     // the SH slab was requested asynchronously at the top; it is first needed here
-    if (p.shs) {
+    if (fetch_sh) {
         if (bulk) mbar_wait(&sBar, 0);
         else { cp_async_wait_all(); __syncthreads(); }
     }
-    if (visible) {
+    if (live) {
         // ---- SH backward (backward.cu:20-139) -------------------------------------------------
         if (p.shs) {
             const float dox = m3[0] - sCam[0], doy = m3[1] - sCam[1], doz = m3[2] - sCam[2];
@@ -446,17 +460,22 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     }
     if (!in_range) return;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        p.dL_dmeans2D[3 * (size_t)idx + k] = dmean2[k];
-        put(p.dL_dcolors + 3 * (size_t)idx + k, dcol[k], p.acc_colors);
-        put(p.dL_dmeans3D + 3 * (size_t)idx + k, dmean3[k], p.acc);
-        put(p.dL_dscales + 3 * (size_t)idx + k, dscale[k], p.acc);
-    }
-    put(p.dL_dopacity + idx, dop, p.acc);
+    for (int k = 0; k < 3; ++k) p.dL_dmeans2D[3 * (size_t)idx + k] = dmean2[k];
     if (p.dL_dsh_factor) {
 #pragma unroll
         for (int k = 0; k < 3; ++k) p.dL_dsh_factor[3 * (size_t)idx + k] = dfac[k];
     }
+    if (live || !p.acc_colors) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) put(p.dL_dcolors + 3 * (size_t)idx + k, dcol[k], p.acc_colors);
+    }
+    if (!live && p.acc) return;                     // later views: a row that is not live adds nothing
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        put(p.dL_dmeans3D + 3 * (size_t)idx + k, dmean3[k], p.acc);
+        put(p.dL_dscales + 3 * (size_t)idx + k, dscale[k], p.acc);
+    }
+    put(p.dL_dopacity + idx, dop, p.acc);
 #pragma unroll
     for (int k = 0; k < 6; ++k) put(p.dL_dcov3D + 6 * (size_t)idx + k, dcov[k], p.acc);
     float4* drot4 = reinterpret_cast<float4*>(p.dL_drotations + 4 * (size_t)idx);
@@ -512,7 +531,6 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     p.projmatrix = a.projmatrix + 16 * v; p.campos = a.campos + 3 * v;
     p.scale_modifier = a.scale_modifier; p.tan_fovx = tan_fovx; p.tan_fovy = tan_fovy;
     p.h_y = a.H / (2.0f * tan_fovy); p.h_x = a.W / (2.0f * tan_fovx);
-    p.radii_rec = (const int*)b.tiles_touched;   // tiles_touched > 0  <=>  radii > 0
     p.rec = b.rec; p.grad = b.grad; p.clamped = b.clamped;
     p.dL_dmeans2D = a.dL_dmeans2D + 3 * r; p.dL_dopacity = a.dL_dopacity;
     p.dL_dcolors = a.colors_per_view ? a.dL_dcolors + 3 * r : a.dL_dcolors;
