@@ -594,6 +594,12 @@ int r3dg_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, 
  * maximize — the only configuration the reference uses).  `tensors` is a HOST array; every
  * entry updates param / exp_avg / exp_avg_sq in place from grad.  `step` is the 1-based count of
  * this update for that tensor (torch increments state['step'] before using it).
+ *
+ * Selective step: with `row_mask` set, the tensor is n / row_elems rows of `row_elems` elements and
+ * only the rows whose mask byte is nonzero are updated, with the dense step's arithmetic; every
+ * other row keeps param / exp_avg / exp_avg_sq bit for bit and its gradient is not used.
+ * `row_mask` NULL (a zero-filled struct) is the dense step.  R3DG_ERR_BAD_ARG when a mask is given
+ * with row_elems < 1 or n not a multiple of row_elems; R3DG_ERR_UNSUPPORTED when row_elems > INT_MAX.
  * ------------------------------------------------------------------------------------------ */
 typedef struct r3dg_adam_tensor {
     float* param;              /* [n] */
@@ -603,6 +609,8 @@ typedef struct r3dg_adam_tensor {
     long long n;
     long long step;
     double lr, beta1, beta2, eps;
+    const unsigned char* row_mask;   /* [n / row_elems] device bytes, or NULL */
+    long long row_elems;
 } r3dg_adam_tensor;
 int r3dg_adam_step(int num_tensors, const r3dg_adam_tensor* tensors, r3dg_stream_t stream);
 

@@ -97,7 +97,8 @@ class DensifyThresholds(ctypes.Structure):
 class AdamTensor(ctypes.Structure):
     _fields_ = ([(n, c_void_p) for n in ("param", "grad", "exp_avg", "exp_avg_sq")] +
                 [("n", c_ll), ("step", c_ll)] +
-                [(n, ctypes.c_double) for n in ("lr", "beta1", "beta2", "eps")])
+                [(n, ctypes.c_double) for n in ("lr", "beta1", "beta2", "eps")] +
+                [("row_mask", c_void_p), ("row_elems", c_ll)])
 
 
 # every symbol include/r3dg_b200.h declares: (name, restype, argtypes)

@@ -35,15 +35,22 @@ class FusedAdam(torch.optim.Optimizer):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=0, amsgrad=False, maximize=False))
 
     @torch.no_grad()
-    def step(self, closure=None):
+    def step(self, closure=None, *, visibility=None):
+        """One Adam step over every parameter that has a gradient.
+
+        `visibility` (optional): a CUDA bool or uint8 tensor of P elements, shaped [P] or [P, 1], for a selective
+        step.  Parameters with P rows (`param.shape[0] == P`, the rule of `prune_optimizer`) update only the rows
+        whose byte is nonzero, with exactly the dense step's arithmetic; the other rows keep param, exp_avg and
+        exp_avg_sq bit for bit and their gradient is not read.  Other parameters take the dense step, and
+        `state["step"]` counts every step, so an all-ones mask is the dense step.  This is not Adam: a row left
+        out keeps its moments instead of decaying them and moving on them.  No host synchronisation."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        entries, keep = [], []
+        todo = []
         device = None
         for group in self.param_groups:
-            beta1, beta2 = group["betas"]
             for p in group["params"]:
                 if p.grad is None:
                     continue
@@ -54,32 +61,60 @@ class FusedAdam(torch.optim.Optimizer):
                 device = device or p.device
                 if p.device != device:
                     raise RuntimeError("FusedAdam: all parameters must live on one device")
-                st = self.state[p]
-                if len(st) == 0:
-                    st["step"] = torch.tensor(0.0, dtype=torch.float32)
-                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                step = st["step"]
-                if torch.is_tensor(step):
-                    step += 1
-                    t = int(step.item())
-                else:                                   # state dicts written by torch < 1.12 hold a Python int
-                    t = st["step"] = step + 1
-                g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
-                m, v = st["exp_avg"], st["exp_avg_sq"]
-                if not (m.is_contiguous() and v.is_contiguous()):
-                    m = st["exp_avg"] = m.contiguous()
-                    v = st["exp_avg_sq"] = v.contiguous()
-                keep.append(g)
-                e = _lib.AdamTensor()
-                e.param, e.grad, e.exp_avg, e.exp_avg_sq = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
-                e.n, e.step = p.numel(), t
-                e.lr, e.beta1, e.beta2, e.eps = float(group["lr"]), float(beta1), float(beta2), float(group["eps"])
-                entries.append(e)
+                todo.append((group, p))
+        mask = None if visibility is None else _row_mask(visibility, device, [p for _, p in todo])
+        entries, keep = [], [mask]
+        for group, p in todo:
+            beta1, beta2 = group["betas"]
+            st = self.state[p]
+            if len(st) == 0:
+                st["step"] = torch.tensor(0.0, dtype=torch.float32)
+                st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+            step = st["step"]
+            if torch.is_tensor(step):
+                step += 1
+                t = int(step.item())
+            else:                                   # state dicts written by torch < 1.12 hold a Python int
+                t = st["step"] = step + 1
+            g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
+            m, v = st["exp_avg"], st["exp_avg_sq"]
+            if not (m.is_contiguous() and v.is_contiguous()):
+                m = st["exp_avg"] = m.contiguous()
+                v = st["exp_avg_sq"] = v.contiguous()
+            keep.append(g)
+            e = _lib.AdamTensor()
+            e.param, e.grad, e.exp_avg, e.exp_avg_sq = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
+            e.n, e.step = p.numel(), t
+            e.lr, e.beta1, e.beta2, e.eps = float(group["lr"]), float(beta1), float(beta2), float(group["eps"])
+            if mask is not None and is_per_gaussian(p, mask.shape[0]) and mask.shape[0] > 0:
+                e.row_mask, e.row_elems = mask.data_ptr(), p.numel() // mask.shape[0]
+            entries.append(e)
         if entries:
             arr = (_lib.AdamTensor * len(entries))(*entries)
             _lib.call("r3dg_adam_step", device, len(entries), arr, what="FusedAdam.step")
         return loss
+
+
+def is_per_gaussian(p, P):
+    """A tensor holds one row per Gaussian of a model of P Gaussians when its first dimension is P."""
+    return p.dim() > 0 and p.shape[0] == P
+
+
+def _row_mask(visibility, device, params):
+    """`visibility` as a contiguous uint8 tensor [P] for FusedAdam.step, checked against the parameters that have a
+    gradient (none: the step is a no-op and any length is accepted)."""
+    if not torch.is_tensor(visibility) or visibility.dtype not in (torch.bool, torch.uint8):
+        raise ValueError("FusedAdam.step: visibility must be a bool or uint8 tensor")
+    if not visibility.is_cuda or (device is not None and visibility.device != device):
+        raise ValueError("FusedAdam.step: visibility must be on the parameters' CUDA device")
+    if not (visibility.dim() == 1 or (visibility.dim() == 2 and visibility.shape[1] == 1)):
+        raise ValueError(f"FusedAdam.step: visibility must be shaped [P] or [P, 1], got {tuple(visibility.shape)}")
+    P = visibility.shape[0]
+    if params and not any(is_per_gaussian(p, P) for p in params):
+        raise ValueError(f"FusedAdam.step: no parameter with a gradient has {P} rows to match visibility")
+    mask = visibility.reshape(P).contiguous()
+    return mask.view(torch.uint8) if mask.dtype == torch.bool else mask
 
 
 _torch_adam = None
@@ -157,7 +192,7 @@ def prune_optimizer(optimizer, keep, extra=()):
     per-Gaussian tensors, e.g. xyz_gradient_accum / denom / max_radii2D of prune_points :702-729) are compacted by ONE
     launch.  Returns ({group name: new nn.Parameter}, [compacted extras]); optimizer state is re-keyed like the reference."""
     P = keep.reshape(-1).shape[0]
-    groups = [g for g in optimizer.param_groups if len(g["params"]) == 1 and g["params"][0].dim() > 0 and g["params"][0].shape[0] == P]
+    groups = [g for g in optimizer.param_groups if len(g["params"]) == 1 and is_per_gaussian(g["params"][0], P)]
     work, slots = [], []
     for g in groups:
         p = g["params"][0]
