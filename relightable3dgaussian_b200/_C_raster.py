@@ -17,6 +17,9 @@ Differences that are not observable through the reference's Python wrapper
 Under torch.use_deterministic_algorithms(True), read at call time, both calls run the library's
 deterministic mode: out_weights and the nine gradients are then bitwise reproducible (the reference's
 float atomics make them run-to-run nondeterministic).  Its workspace comes from the torch allocator.
+
+One view and V views of the same Gaussians (rasterize_views / rasterize_views_backward) run through the same two
+host paths, _forward and _backward: the library treats a one-view call as V = 1.
 """
 import ctypes
 import warnings
@@ -89,6 +92,105 @@ def _prep(t, name):
     return t.contiguous()
 
 
+def _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means3D, features, colors, scales,
+                 rotations, cov3D_precomp, viewmatrix, projmatrix, sh, campos):
+    """Preps the inputs the forward and the backward share and enters them, with the sizes and the first view's
+    tan_fov*, into the argument struct `a` (RasterFwdArgs or RasterBwdArgs).  A one-view call (`views` False) leaves
+    V = 0; a V-view call enters its camera table, each row {tan_fovx, tan_fovy, cx, cy}, and whether features / colors
+    are per view ([V,P,*]).  Returns what the caller holds until the call is enqueued: the prepped inputs and the
+    table."""
+    features_pv = views and features.dim() == 3
+    colors_pv = views and colors is not None and colors.numel() != 0 and colors.dim() == 3
+    background = _prep(background, "background"); means3D = _prep(means3D, "means3D"); sh = _prep(sh, "sh")
+    colors = _prep(colors, "colors"); features = _prep(features, "features"); scales = _prep(scales, "scales")
+    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
+    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
+    campos = _prep(campos, "campos")
+    a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
+    a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.scales = _lib.ptr(scales)
+    a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
+    a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
+    a.P, a.S, a.D, a.W, a.H = means3D.size(0), features.size(-1), int(degree), W, H
+    a.M = sh.size(1) if sh.numel() != 0 else 0
+    a.scale_modifier, a.tan_fovx, a.tan_fovy = float(scale_modifier), float(cams[0][0]), float(cams[0][1])
+    keep = [background, means3D, sh, colors, features, scales, rotations, cov3D_precomp, viewmatrix, projmatrix, campos]
+    if views:
+        table = (ctypes.c_float * (4 * len(cams)))(*(float(x) for c in cams for x in c))   # [V][4]
+        keep.append(table)
+        a.V, a.view_cams = len(cams), ctypes.cast(table, ctypes.c_void_p)
+        a.features_per_view, a.colors_per_view = int(features_pv), int(colors_pv)
+    return keep
+
+
+def _forward(views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+             viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered, computer_pseudo_normal, debug,
+             capacity, pinned, defer):
+    """The forward of the len(cams) views `cams` = [(tan_fovx, tan_fovy, cx, cy), ...]: one view (`views` False,
+    outputs in the one-view shapes) or V views (outputs with a leading V).  Sizes the binning buffer for `capacity`
+    instances and re-runs with room to spare while the counts, read back into the pinned int32 `pinned` (one per
+    view), exceed it.  Returns the 12 outputs after num_rendered, the event recorded once the counts are copied, and the
+    counts as a list: None when `defer`, which returns after the first attempt without waiting."""
+    lib = _lib.load()
+    V, P, S = len(cams), means3D.size(0), features.size(-1)
+    dev = means3D.device
+    a = _lib.RasterFwdArgs()
+    keep = _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means3D, features, colors, scales,
+                        rotations, cov3D_precomp, viewmatrix, projmatrix, sh, campos)
+    opacity = _prep(opacity, "opacity")
+    a.opacities = _lib.ptr(opacity)
+    a.cx, a.cy = float(cams[0][2]), float(cams[0][3])
+    a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
+    a.debug = int(bool(debug))
+
+    lead = (V,) if views else ()
+    f32 = dict(dtype=torch.float32, device=dev)
+    out_color = torch.empty(lead + (3, H, W), **f32)
+    out_opacity = torch.empty(lead + (1, H, W), **f32)
+    out_depth = torch.empty(lead + (1, H, W), **f32)
+    out_feature = torch.empty(lead + (S, H, W), **f32)
+    out_normal = torch.empty(lead + (3, H, W), **f32)
+    out_surface_xyz = torch.empty(lead + (3, H, W), **f32)
+    out_weights = torch.empty(lead + (P, 1), **f32)
+    radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
+    geomBuffer = torch.empty((lib.r3dg_raster_views_geom_bytes(P, S, V),), dtype=torch.uint8, device=dev)
+    imgBuffer = torch.empty((lib.r3dg_raster_views_img_bytes(W, H, V),), dtype=torch.uint8, device=dev)
+    a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
+    a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
+    a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
+    a.out_weights = _lib.ptr(out_weights); a.radii = _lib.ptr(radii); a.n_contrib = None
+    a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
+    a.img = imgBuffer.data_ptr(); a.img_bytes = imgBuffer.numel()
+    det_ws = _lib.det_workspace(a, lib.r3dg_raster_fwd_det_bytes(V * P), dev)
+    a.num_rendered_host = pinned.data_ptr()
+    stream = torch.cuda.current_stream(dev)
+    while True:
+        # this module's torch.empty, not _lib.scratch: tests substitute it to hand the forward a reused binning buffer
+        binningBuffer = torch.empty((lib.r3dg_raster_binning_bytes(capacity),), dtype=torch.uint8, device=dev)
+        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
+        # recorded by the library right after the last view's count is copied, a quarter into the forward
+        ev = torch.cuda.Event()
+        ev.record(stream)                 # (creates the underlying cudaEvent_t; re-recorded inside the call)
+        a.count_ready_event = ev.cuda_event
+        _lib.call("r3dg_raster_forward", dev, ctypes.byref(a),
+                  what="rasterize_views" if views else "rasterize_gaussians")
+        if defer:                         # opt-in: let the host run ahead; the caller resolves the count later
+            counts = None
+            break
+        if debug:
+            stream.synchronize()
+        else:
+            ev.synchronize()              # the one read-back: the counts are part of the return tuple.  The host
+                                          # resumes while the compositor still runs and can enqueue the loss / backward
+        counts = pinned.tolist()
+        if sum(counts) <= capacity:
+            break
+        capacity = int(sum(counts) * 1.25) + 4096       # speculation missed: rerun with room to spare
+    off = lib.r3dg_raster_views_img_n_contrib_offset(W, H, V)
+    n_contrib = imgBuffer[off:off + 4 * V * H * W].view(torch.int32).view(lead + (H, W))   # view, like the reference
+    return (n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal, out_surface_xyz, out_weights, radii,
+            geomBuffer, binningBuffer, imgBuffer), ev, counts
+
+
 def rasterize_gaussians(background, means3D, features, colors, opacity, scales, rotations,
                         scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                         cx, cy, image_height, image_width, sh, degree, campos, prefiltered,
@@ -96,35 +198,11 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     """== RasterizeGaussiansCUDA (rasterize_points.cu:36-141).  Returns the 13-tuple
     (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
      out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer)."""
-    lib = _lib.load()
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")   # rasterize_points.cu:62-64
     P = means3D.size(0)
-    S = features.size(1)
     H, W = int(image_height), int(image_width)
-    dev = means3D.device
-    means3D = _prep(means3D, "means3D")
-    features = _prep(features, "features"); colors = _prep(colors, "colors")
-    opacity = _prep(opacity, "opacity"); scales = _prep(scales, "scales")
-    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
-    sh = _prep(sh, "sh"); background = _prep(background, "background")
-    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
-    campos = _prep(campos, "campos")
-    M = sh.size(1) if sh.numel() != 0 else 0
-
-    f32 = dict(dtype=torch.float32, device=dev)
-    out_color = torch.empty((3, H, W), **f32)
-    out_opacity = torch.empty((1, H, W), **f32)
-    out_depth = torch.empty((1, H, W), **f32)
-    out_feature = torch.empty((S, H, W), **f32)
-    out_normal = torch.empty((3, H, W), **f32)
-    out_surface_xyz = torch.empty((3, H, W), **f32)
-    out_weights = torch.empty((P, 1), **f32)
-    radii = torch.empty((P,), dtype=torch.int32, device=dev)
-    geomBuffer = torch.empty((lib.r3dg_raster_geom_bytes(P, S),), dtype=torch.uint8, device=dev)
-    imgBuffer = torch.empty((lib.r3dg_raster_img_bytes(W, H),), dtype=torch.uint8, device=dev)
-
-    st = _dev_state(dev)
+    st = _dev_state(means3D.device)
     shape = (P, W, H)
     if st["shape"] != shape:             # new model size / resolution (e.g. after densification): re-learn the counts
         st.update(shape=shape, seen=0, rmax=0, capacity=0)
@@ -142,56 +220,96 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
         capacity = max(int(st["rmax"] * _HEADROOM) + 4096, 4 * P + 4096)
     else:
         capacity = max(st["capacity"], 4 * P + 4096)
-    a = _lib.RasterFwdArgs()
-    a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
-    a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
-    a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.opacities = _lib.ptr(opacity)
-    a.scales = _lib.ptr(scales); a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
-    a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
-    a.scale_modifier = float(scale_modifier); a.tan_fovx = float(tan_fovx)
-    a.tan_fovy = float(tan_fovy); a.cx = float(cx); a.cy = float(cy)
-    a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
-    a.debug = int(bool(debug))
-    a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
-    a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
-    a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
-    a.out_weights = _lib.ptr(out_weights); a.radii = _lib.ptr(radii); a.n_contrib = None
-    a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
-    a.img = imgBuffer.data_ptr(); a.img_bytes = imgBuffer.numel()
-    det_ws = _lib.det_workspace(a, lib.r3dg_raster_fwd_det_bytes(P), dev)
     slot = st["next"]
     st["next"] = (slot + 1) % _SLOTS
     pinned = st["pinned"][slot:slot + 1]
-    a.num_rendered_host = pinned.data_ptr()
-    stream = torch.cuda.current_stream(dev)
-    while True:
-        # this module's torch.empty, not _lib.scratch: tests substitute it to hand the forward a reused binning buffer
-        binningBuffer = torch.empty((lib.r3dg_raster_binning_bytes(capacity),), dtype=torch.uint8, device=dev)
-        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-        # recorded by the library right after the count's D2H copy — a quarter into the forward, not at its end
-        ev = torch.cuda.Event()
-        ev.record(stream)                 # (creates the underlying cudaEvent_t; re-recorded inside the call)
-        a.count_ready_event = ev.cuda_event
-        _lib.call("r3dg_raster_forward", dev, ctypes.byref(a), what="rasterize_gaussians")
-        if _defer:                        # opt-in: let the host run ahead; the count is resolved later
-            rendered = DeferredCount(ev, pinned, capacity, st, P)
-            st["pending"] = rendered
-            break
-        if debug:
-            stream.synchronize()
-        else:
-            ev.synchronize()              # the one readback: num_rendered is part of the return tuple.  The host resumes
-                                          # while the compositor still runs and can enqueue the loss / backward behind it
-        rendered = int(pinned.item())
-        if rendered <= capacity:
-            break
-        capacity = int(rendered * 1.25) + 4096          # speculation missed: rerun with room to spare
-    if not _defer:
+    out, ev, counts = _forward(False, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
+                               cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy, cx, cy)], H, W, sh, degree,
+                               campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer)
+    if _defer:
+        rendered = DeferredCount(ev, pinned, capacity, st, P)
+        st["pending"] = rendered
+    else:
+        rendered = counts[0]
         _observe(st, rendered, P)
-    off = lib.r3dg_raster_img_n_contrib_offset(W, H)
-    n_contrib = imgBuffer[off:off + 4 * H * W].view(torch.int32).view(H, W)   # view, like the reference
-    return (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
-            out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer)
+    return (rendered,) + out
+
+
+def _backward(views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
+              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
+              campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
+              surface_work, principal):
+    """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
+    is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
+    one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
+    are those of rasterize_gaussians_backward (`surface` without the principal point)."""
+    lib = _lib.load()
+    V, P, S = len(cams), means3D.size(0), features.size(-1)
+    H, W = dL_dout_color.size(-2), dL_dout_color.size(-1)
+    dev = means3D.device
+    a = _lib.RasterBwdArgs()
+    keep = _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means3D, features, colors, scales,
+                        rotations, cov3D_precomp, viewmatrix, projmatrix, sh, campos)
+    M = a.M
+    dL_dout_color = _prep(dL_dout_color, "dL_dout_color")
+    dL_dout_opacity = _prep(dL_dout_opacity, "dL_dout_opacity")
+    dL_dout_depth = _prep(dL_dout_depth, "dL_dout_depth")
+    dL_dout_feature = _prep(dL_dout_feature, "dL_dout_feature")
+    f32 = dict(dtype=torch.float32, device=dev)
+
+    def _alloc(name, shape):
+        # `_out` (dist.GradBucket views) lets the multi-GPU path have the kernels write straight
+        # into the flat all-reduce buffer; every element is written, so empty() is enough.
+        if _out is not None and name in _out:
+            t = _out[name]
+            assert t.is_contiguous() and tuple(t.shape) == tuple(shape) and t.dtype == torch.float32
+            return t
+        return torch.empty(shape, **f32)
+
+    dL_dmeans3D = _alloc("means3D", (P, 3))
+    dL_dmeans2D = _alloc("means2D", ((V,) if views else ()) + (P, 3))
+    dL_dfeatures = _alloc("features", (V, P, S) if a.features_per_view else (P, S))
+    dL_dcolors = _alloc("colors", (V, P, 3) if a.colors_per_view else (P, 3))
+    dL_dopacity = _alloc("opacity", (P, 1))
+    dL_dcov3D = _alloc("cov3D", (P, 6))
+    # multi-GPU exchange (dist.FactoredGradExchange): `_out["sh_factor"]` [P,3] asks for the view's rank-1
+    # factor of dL_dsh INSTEAD of the dense tensor (returned empty), see r3dg_sh_grad_from_factors
+    sh_factor = _out.get("sh_factor") if _out is not None else None
+    if sh_factor is not None:
+        assert sh_factor.is_contiguous() and tuple(sh_factor.shape) == (P, 3) and sh_factor.dtype == torch.float32
+        if M == 0:
+            raise RuntimeError("the SH-gradient factor needs `sh` inputs (colors_precomp has no SH gradient)")
+        dL_dsh = _alloc("sh", (P, M, 3)) if "sh" in _out else torch.empty((0,), **f32)     # both on request (tests)
+    else:
+        dL_dsh = _alloc("sh", (P, M, 3))
+        if V > 1 and M > 0:               # the library rebuilds dL_dsh from the views' rank-1 factors
+            sh_factor = torch.empty((V, P, 3), **f32)
+    dL_dscales = _alloc("scales", (P, 3))
+    dL_drotations = _alloc("rotations", (P, 4))
+    # zeroed: a call with P = 0 writes nothing, otherwise the library overwrites every element
+    cam = tuple(torch.zeros(shape, **f32) for shape in ((V, 4, 4), (V, 4, 4), (V, 3))) if cam_grads else ()
+    if P != 0:
+        a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
+        a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
+        a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
+        a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
+        a.dL_dopacity = _lib.ptr(dL_dopacity); a.dL_dmeans3D = _lib.ptr(dL_dmeans3D)
+        a.dL_dfeatures = _lib.ptr(dL_dfeatures); a.dL_dcov3D = _lib.ptr(dL_dcov3D); a.dL_dsh = _lib.ptr(dL_dsh)
+        a.dL_dscales = _lib.ptr(dL_dscales); a.dL_drotations = _lib.ptr(dL_drotations)
+        a.dL_dsh_factor = _lib.ptr(sh_factor)
+        a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
+        a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
+        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
+        det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(V * P, S), dev)
+        if cam:
+            cam_ws = _lib.scratch(lib.r3dg_raster_cam_grad_bytes(P, V), dev)
+            a.dL_dviewmatrix, a.dL_dprojmatrix, a.dL_dcampos = (t.data_ptr() for t in cam)
+            a.cam_work, a.cam_work_bytes = cam_ws.data_ptr(), cam_ws.numel()
+        surface_ws = _surface_args(a, surface, W, H, V, dev, surface_work, principal=principal)
+        _lib.call("r3dg_raster_backward", dev, ctypes.byref(a),
+                  what="rasterize_views_backward" if views else "rasterize_gaussians_backward")
+    return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
+            dL_dscales, dL_drotations), cam
 
 
 def rasterize_gaussians_backward(background, means3D, features, radii, colors, scales, rotations,
@@ -208,98 +326,13 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     and surface-xyz outputs: (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth, cx, cy) with the forward's
     opacity and depth images; a cotangent may be None.  `surface_work` optionally supplies the workspace
     (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards."""
-    lib = _lib.load()
-    P = means3D.size(0)
-    S = features.size(1)
-    H, W = dL_dout_color.size(1), dL_dout_color.size(2)
-    dev = means3D.device
-    means3D = _prep(means3D, "means3D"); features = _prep(features, "features")
-    colors = _prep(colors, "colors"); scales = _prep(scales, "scales")
-    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
-    sh = _prep(sh, "sh"); background = _prep(background, "background")
-    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
-    campos = _prep(campos, "campos")
-    dL_dout_color = _prep(dL_dout_color, "dL_dout_color")
-    dL_dout_opacity = _prep(dL_dout_opacity, "dL_dout_opacity")
-    dL_dout_depth = _prep(dL_dout_depth, "dL_dout_depth")
-    dL_dout_feature = _prep(dL_dout_feature, "dL_dout_feature")
-    M = sh.size(1) if sh.numel() != 0 else 0
-
-    f32 = dict(dtype=torch.float32, device=dev)
-
-    def _alloc(name, shape):
-        # `_out` (dist.GradBucket views) lets the multi-GPU path have the kernels write straight
-        # into the flat all-reduce buffer; every element is written, so empty() is enough.
-        if _out is not None and name in _out:
-            t = _out[name]
-            assert t.is_contiguous() and tuple(t.shape) == tuple(shape) and t.dtype == torch.float32
-            return t
-        return torch.empty(shape, **f32)
-
-    dL_dmeans3D = _alloc("means3D", (P, 3))
-    dL_dmeans2D = _alloc("means2D", (P, 3))
-    dL_dfeatures = _alloc("features", (P, S))
-    dL_dcolors = _alloc("colors", (P, 3))
-    dL_dopacity = _alloc("opacity", (P, 1))
-    dL_dcov3D = _alloc("cov3D", (P, 6))
-    # multi-GPU exchange (dist.FactoredGradExchange): `_out["sh_factor"]` [P,3] asks for the view's rank-1
-    # factor of dL_dsh INSTEAD of the dense tensor (returned empty), see r3dg_sh_grad_from_factors
-    sh_factor = _out.get("sh_factor") if _out is not None else None
-    if sh_factor is not None:
-        assert sh_factor.is_contiguous() and tuple(sh_factor.shape) == (P, 3) and sh_factor.dtype == torch.float32
-        if M == 0:
-            raise RuntimeError("the SH-gradient factor needs `sh` inputs (colors_precomp has no SH gradient)")
-        dL_dsh = _alloc("sh", (P, M, 3)) if "sh" in _out else torch.empty((0,), **f32)     # both on request (tests)
-    else:
-        dL_dsh = _alloc("sh", (P, M, 3))
-    dL_dscales = _alloc("scales", (P, 3))
-    dL_drotations = _alloc("rotations", (P, 4))
-    cam = _cam_outputs(1, dev) if cam_grads else ()
-    if P != 0:
-        a = _lib.RasterBwdArgs()
-        a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
-        a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
-        a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.scales = _lib.ptr(scales)
-        a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
-        a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
-        a.scale_modifier = float(scale_modifier); a.tan_fovx = float(tan_fovx); a.tan_fovy = float(tan_fovy)
-        a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
-        a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
-        a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
-        a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
-        a.dL_dopacity = _lib.ptr(dL_dopacity); a.dL_dmeans3D = _lib.ptr(dL_dmeans3D)
-        a.dL_dfeatures = _lib.ptr(dL_dfeatures); a.dL_dcov3D = _lib.ptr(dL_dcov3D); a.dL_dsh = _lib.ptr(dL_dsh)
-        a.dL_dscales = _lib.ptr(dL_dscales); a.dL_drotations = _lib.ptr(dL_drotations)
-        a.dL_dsh_factor = _lib.ptr(sh_factor)
-        a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
-        a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
-        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-        det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(P, S), dev)
-        cam_ws = _cam_args(a, cam, P, 1, dev)
-        surface_ws = _surface_args(a, surface and surface[:4], W, H, 1, dev, surface_work,
-                                   principal=surface[4:6] if surface is not None and len(surface) == 6 else None)
-        _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_gaussians_backward")
-    return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
-            dL_dscales, dL_drotations) + tuple(t[0] for t in cam)
-
-
-def _cam_outputs(V, device):
-    """The camera-gradient outputs of a V-view backward: viewmatrix [V,4,4], projmatrix [V,4,4], campos [V,3], zeroed
-    (a call with P = 0 writes nothing; otherwise the library overwrites every element)."""
-    return (torch.zeros((V, 4, 4), dtype=torch.float32, device=device),
-            torch.zeros((V, 4, 4), dtype=torch.float32, device=device),
-            torch.zeros((V, 3), dtype=torch.float32, device=device))
-
-
-def _cam_args(a, cam, P, V, device):
-    """Enters the camera-gradient outputs `cam` (or none) and their workspace into the backward arguments `a`; returns
-    the workspace, which the caller holds until the call is enqueued."""
-    if not cam:
-        return None
-    ws = _lib.scratch(_lib.load().r3dg_raster_cam_grad_bytes(P, V), device)
-    a.dL_dviewmatrix, a.dL_dprojmatrix, a.dL_dcampos = (t.data_ptr() for t in cam)
-    a.cam_work, a.cam_work_bytes = ws.data_ptr(), ws.numel()
-    return ws
+    principal = surface[4:6] if surface is not None and len(surface) == 6 else None
+    grads, cam = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
+                           cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
+                           dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
+                           binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
+                           surface and surface[:4], surface_work, principal)
+    return grads + tuple(t[0] for t in cam)
 
 
 def _surface_args(a, surface, W, H, V, device, work=None, principal=None):
@@ -370,12 +403,6 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
 _views_capacity = {}     # (device, P, W, H, V) -> binning capacity that held the last call of that shape
 
 
-def _view_cams(cams):
-    """Host table [V][4] {tan_fovx, tan_fovy, cx, cy} (kept alive by the caller until the call is enqueued)."""
-    flat = [float(x) for c in cams for x in c]
-    return (ctypes.c_float * len(flat))(*flat)
-
-
 def rasterize_views(background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                     viewmatrix, projmatrix, cams, image_height, image_width, sh, degree, campos, prefiltered,
                     computer_pseudo_normal, _min_capacity=None):
@@ -384,74 +411,17 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
     Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
     out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
     radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once."""
-    lib = _lib.load()
-    V = len(cams)
-    P = means3D.size(0)
-    S = features.size(-1)
+    V, P = len(cams), means3D.size(0)
     H, W = int(image_height), int(image_width)
     dev = means3D.device
-    features_pv = features.dim() == 3
-    colors_pv = colors is not None and colors.numel() != 0 and colors.dim() == 3
-    means3D = _prep(means3D, "means3D")
-    features = _prep(features, "features"); colors = _prep(colors, "colors")
-    opacity = _prep(opacity, "opacity"); scales = _prep(scales, "scales")
-    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
-    sh = _prep(sh, "sh"); background = _prep(background, "background")
-    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
-    campos = _prep(campos, "campos")
-    M = sh.size(1) if sh.numel() != 0 else 0
-
-    f32 = dict(dtype=torch.float32, device=dev)
-    out_color = torch.empty((V, 3, H, W), **f32)
-    out_opacity = torch.empty((V, 1, H, W), **f32)
-    out_depth = torch.empty((V, 1, H, W), **f32)
-    out_feature = torch.empty((V, S, H, W), **f32)
-    out_normal = torch.empty((V, 3, H, W), **f32)
-    out_surface_xyz = torch.empty((V, 3, H, W), **f32)
-    out_weights = torch.empty((V, P, 1), **f32)
-    radii = torch.empty((V, P), dtype=torch.int32, device=dev)
-    geomBuffer = torch.empty((lib.r3dg_raster_views_geom_bytes(P, S, V),), dtype=torch.uint8, device=dev)
-    imgBuffer = torch.empty((lib.r3dg_raster_views_img_bytes(W, H, V),), dtype=torch.uint8, device=dev)
     key = (dev.index if dev.index is not None else torch.cuda.current_device(), P, W, H, V)
     capacity = int(_min_capacity) if _min_capacity is not None else max(_views_capacity.get(key, 0), 4 * V * P + 4096)
-    table = _view_cams(cams)
-    a = _lib.RasterFwdArgs()
-    a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
-    a.V, a.view_cams = V, ctypes.cast(table, ctypes.c_void_p)
-    a.features_per_view, a.colors_per_view = int(features_pv), int(colors_pv)
-    a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
-    a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.opacities = _lib.ptr(opacity)
-    a.scales = _lib.ptr(scales); a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
-    a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
-    a.scale_modifier = float(scale_modifier); a.tan_fovx, a.tan_fovy, a.cx, a.cy = (float(x) for x in cams[0])
-    a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
-    a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
-    a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
-    a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
-    a.out_weights = _lib.ptr(out_weights); a.radii = _lib.ptr(radii); a.n_contrib = None
-    a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
-    a.img = imgBuffer.data_ptr(); a.img_bytes = imgBuffer.numel()
-    det_ws = _lib.det_workspace(a, lib.r3dg_raster_fwd_det_bytes(V * P), dev)
     pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
-    a.num_rendered_host = pinned.data_ptr()
-    stream = torch.cuda.current_stream(dev)
-    while True:
-        binningBuffer = torch.empty((lib.r3dg_raster_binning_bytes(capacity),), dtype=torch.uint8, device=dev)
-        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-        ev = torch.cuda.Event()
-        ev.record(stream)
-        a.count_ready_event = ev.cuda_event
-        _lib.call("r3dg_raster_forward", dev, ctypes.byref(a), what="rasterize_views")
-        ev.synchronize()                  # the one read-back: the V counts, after the last view's binning offsets
-        rendered = [int(x) for x in pinned.tolist()]
-        if sum(rendered) <= capacity:
-            break
-        capacity = int(sum(rendered) * 1.25) + 4096   # speculation missed: rerun with room to spare
+    out, _, rendered = _forward(True, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
+                                cov3D_precomp, viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered,
+                                computer_pseudo_normal, False, capacity, pinned, False)
     _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
-    off = lib.r3dg_raster_views_img_n_contrib_offset(W, H, V)
-    n_contrib = imgBuffer[off:off + 4 * V * H * W].view(torch.int32).view(V, H, W)
-    return (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
-            out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer)
+    return (rendered,) + out
 
 
 def rasterize_views_backward(background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
@@ -466,67 +436,8 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth), all [V,*,H,W] (a cotangent may be None), and
     `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
     one view, cams[0]'s, entered as the call's cx, cy)."""
-    lib = _lib.load()
-    V = len(cams)
-    P = means3D.size(0)
-    S = features.size(-1)
-    H, W = dL_dout_color.size(2), dL_dout_color.size(3)
-    dev = means3D.device
-    features_pv = features.dim() == 3
-    colors_pv = colors is not None and colors.numel() != 0 and colors.dim() == 3
-    means3D = _prep(means3D, "means3D"); features = _prep(features, "features")
-    colors = _prep(colors, "colors"); scales = _prep(scales, "scales")
-    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
-    sh = _prep(sh, "sh"); background = _prep(background, "background")
-    viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
-    campos = _prep(campos, "campos")
-    dL_dout_color = _prep(dL_dout_color, "dL_dout_color")
-    dL_dout_opacity = _prep(dL_dout_opacity, "dL_dout_opacity")
-    dL_dout_depth = _prep(dL_dout_depth, "dL_dout_depth")
-    dL_dout_feature = _prep(dL_dout_feature, "dL_dout_feature")
-    M = sh.size(1) if sh.numel() != 0 else 0
-
-    f32 = dict(dtype=torch.float32, device=dev)
-    dL_dmeans2D = torch.empty((V, P, 3), **f32)
-    dL_dmeans3D = torch.empty((P, 3), **f32)
-    dL_dfeatures = torch.empty((V, P, S) if features_pv else (P, S), **f32)
-    dL_dcolors = torch.empty((V, P, 3) if colors_pv else (P, 3), **f32)
-    dL_dopacity = torch.empty((P, 1), **f32)
-    dL_dcov3D = torch.empty((P, 6), **f32)
-    dL_dsh = torch.empty((P, M, 3), **f32)
-    sh_factor = torch.empty((V, P, 3), **f32) if M > 0 else None
-    dL_dscales = torch.empty((P, 3), **f32)
-    dL_drotations = torch.empty((P, 4), **f32)
-    cam = _cam_outputs(V, dev) if cam_grads else ()
-    if P != 0:
-        table = _view_cams(cams)
-        a = _lib.RasterBwdArgs()
-        a.P, a.S, a.D, a.M, a.W, a.H = P, S, int(degree), M, W, H
-        a.V, a.view_cams = V, ctypes.cast(table, ctypes.c_void_p)
-        a.features_per_view, a.colors_per_view = int(features_pv), int(colors_pv)
-        a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)
-        a.colors_precomp = _lib.ptr(colors); a.features = _lib.ptr(features); a.scales = _lib.ptr(scales)
-        a.rotations = _lib.ptr(rotations); a.cov3D_precomp = _lib.ptr(cov3D_precomp)
-        a.viewmatrix = _lib.ptr(viewmatrix); a.projmatrix = _lib.ptr(projmatrix); a.campos = _lib.ptr(campos)
-        a.scale_modifier = float(scale_modifier); a.tan_fovx, a.tan_fovy = float(cams[0][0]), float(cams[0][1])
-        a.backward_geometry = int(bool(backward_geometry)); a.debug = 0
-        a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
-        a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
-        a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
-        a.dL_dopacity = _lib.ptr(dL_dopacity); a.dL_dmeans3D = _lib.ptr(dL_dmeans3D)
-        a.dL_dfeatures = _lib.ptr(dL_dfeatures); a.dL_dcov3D = _lib.ptr(dL_dcov3D); a.dL_dsh = _lib.ptr(dL_dsh)
-        a.dL_dscales = _lib.ptr(dL_dscales); a.dL_drotations = _lib.ptr(dL_drotations)
-        a.dL_dsh_factor = _lib.ptr(sh_factor)
-        a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
-        a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
-        a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-        det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(V * P, S), dev)
-        cam_ws = _cam_args(a, cam, P, V, dev)
-        surface_ws = _surface_args(a, surface, W, H, V, dev, surface_work, principal=(cams[0][2], cams[0][3]))
-        _lib.call("r3dg_raster_backward", dev, ctypes.byref(a), what="rasterize_views_backward")
-    else:
-        for t in (dL_dmeans2D, dL_dmeans3D, dL_dfeatures, dL_dcolors, dL_dopacity, dL_dcov3D, dL_dsh, dL_dscales,
-                  dL_drotations):
-            t.zero_()
-    return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
-            dL_dscales, dL_drotations) + cam
+    grads, cam = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
+                           cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
+                           dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
+                           backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4])
+    return grads + cam

@@ -80,8 +80,63 @@ def set_grad_exchange(exchange, campos_all=None):
     _EXCHANGE = None if exchange is None else (exchange, campos_all)
 
 
-def _snapshot(args):
-    return tuple(a.cpu().clone() if isinstance(a, torch.Tensor) else a for a in args)
+def _debug_call(debug, fn, args, dump, message, **kw):
+    """fn(*args, **kw).  In debug mode, as in the reference, a CPU snapshot of `args` taken before the call is saved to
+    `dump` if it raises."""
+    if not debug:
+        return fn(*args, **kw)
+    saved = tuple(a.cpu().clone() if isinstance(a, torch.Tensor) else a for a in args)
+    try:
+        return fn(*args, **kw)
+    except Exception:
+        torch.save(saved, dump)
+        print(message)
+        raise
+
+
+def _save_forward(ctx, out, surface_grads, *tensors):
+    """Keeps what the backward of a forward with outputs `out` needs: `tensors`, then with `surface_grads` the forward's
+    opacity and depth images (see _surface_cotangents), and the shapes of the four image outputs (_image_cotangents)."""
+    # cotangents of outputs the reference's backward ignores (num_contrib, normal, surface_xyz, weights, radii)
+    # stay None instead of being materialised as zero tensors (5 fill kernels per step); the four image
+    # cotangents are filled in by _image_cotangents when a loss does not touch one of them
+    ctx.set_materialize_grads(False)
+    ctx.out_shapes = tuple(t.shape for t in out[2:6])
+    ctx.surface_grads = surface_grads
+    ctx.save_for_backward(*tensors, *(out[3:5] if surface_grads else ()))
+
+
+def _image_cotangents(ctx, device, *grads):
+    """The cotangents of the color, opacity, depth and feature outputs, zeros for those the loss does not touch."""
+    return tuple(torch.zeros(shape, dtype=torch.float32, device=device) if g is None else g
+                 for g, shape in zip(grads, ctx.out_shapes))
+
+
+def _surface_cotangents(ctx, g_normal, g_surface_xyz):
+    """(dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth) when the node differentiates the pseudo-normal and
+    surface-xyz outputs and the loss touches one of them; None otherwise."""
+    if not ctx.surface_grads or (g_normal is None and g_surface_xyz is None):
+        return None
+    return (g_normal, g_surface_xyz) + tuple(ctx.saved_tensors[-2:])
+
+
+def _input_grads(ctx, grads, cameras):
+    """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
+    last three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
+    one, and for all three when none was computed."""
+    g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
+    cam = (None, None, None)
+    if grads[9:]:
+        cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[-3:]))
+    return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
+            None, None) + cam
+
+
+def _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
+    """The positional arguments of _C.rasterize_gaussians for the settings `rs`."""
+    return (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
+            rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.cx, rs.cy, rs.image_height, rs.image_width, sh,
+            rs.sh_degree, rs.campos, rs.prefiltered, rs.computer_pseudo_normal, rs.debug)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -95,35 +150,16 @@ class _RasterizeGaussians(torch.autograd.Function):
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos):
         rs = raster_settings
-        args = (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations,
-                rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
-                rs.tanfovy, rs.cx, rs.cy, rs.image_height, rs.image_width, sh, rs.sh_degree,
-                rs.campos, rs.prefiltered, rs.computer_pseudo_normal, rs.debug)
-        if rs.debug:
-            saved = _snapshot(args)
-            try:
-                out = _C.rasterize_gaussians(*args)
-            except Exception:
-                torch.save(saved, "snapshot_fw.dump")
-                print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
-                raise
-        else:
-            out = _C.rasterize_gaussians(*args, _defer=_DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad))
-        (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz, weights,
-         radii, geomBuffer, binningBuffer, imgBuffer) = out
+        out = _debug_call(rs.debug, _C.rasterize_gaussians,
+                          _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
+                                        cov3Ds_precomp),
+                          "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
+                          _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad))
         ctx.raster_settings = rs
-        ctx.num_rendered = num_rendered
-        # cotangents of outputs the reference's backward ignores (num_contrib, normal, surface_xyz, weights, radii)
-        # stay None instead of being materialised as zero tensors (5 fill kernels per step); the four image
-        # cotangents are filled in below when a loss does not touch one of them
-        ctx.set_materialize_grads(False)
-        ctx.out_shapes = (color.shape, opacity.shape, depth.shape, feature.shape)
-        ctx.surface_grads = surface_grads
-        ctx.save_for_backward(colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
-                              radii, sh, geomBuffer, binningBuffer, imgBuffer, opacities,
-                              *((opacity, depth) if surface_grads else ()))
-        return (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz,
-                weights, radii)
+        ctx.num_rendered = out[0]
+        _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
+                      out[9], sh, *out[10:13], opacities)
+        return out[:10]
 
     @staticmethod
     def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature,
@@ -131,16 +167,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         rs = ctx.raster_settings
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, radii, sh,
          geomBuffer, binningBuffer, imgBuffer, opacities) = ctx.saved_tensors[:12]
-        zeros = lambda g, shape: g if g is not None else torch.zeros(shape, dtype=torch.float32, device=means3D.device)
-        g_color, g_opacity = zeros(g_color, ctx.out_shapes[0]), zeros(g_opacity, ctx.out_shapes[1])
-        g_depth, g_feature = zeros(g_depth, ctx.out_shapes[2]), zeros(g_feature, ctx.out_shapes[3])
+        g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
+                                                                   g_feature)
 
         def bwd_args(geom, num_rendered, binning, img):
             return (rs.bg, means3D, features, radii, colors_precomp, scales, rotations,
                     rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
                     rs.tanfovy, g_color, g_opacity, g_depth, g_feature, sh, rs.sh_degree, rs.campos,
                     geom, num_rendered, binning, img, rs.backward_geometry, rs.debug)
-        args = bwd_args(geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer)
         ex = None
         if _EXCHANGE is not None:
             if rs.debug or sh.numel() == 0:
@@ -150,30 +184,21 @@ class _RasterizeGaussians(torch.autograd.Function):
         kw = {} if ex is None else {"_out": {"sh_factor": ex[0].factor}}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
             kw["cam_grads"] = True
-        surface = ctx.surface_grads and (g_normal is not None or g_surface_xyz is not None)
-        if surface:                                  # with the forward's opacity and depth images
-            kw["surface"] = (g_normal, g_surface_xyz) + tuple(ctx.saved_tensors[12:14]) + (rs.cx, rs.cy)
-        if rs.debug:
-            saved = _snapshot(args)
-            try:
-                grads = _C.rasterize_gaussians_backward(*args, **kw)
-            except Exception:
-                torch.save(saved, "snapshot_bw.dump")
-                print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
-                raise
-        else:
-            grads = _C.rasterize_gaussians_backward(*args, **kw)
+        surface = _surface_cotangents(ctx, g_normal, g_surface_xyz)
+        if surface is not None:
+            kw["surface"] = surface + (rs.cx, rs.cy)
+        grads = _debug_call(rs.debug, _C.rasterize_gaussians_backward,
+                            bwd_args(geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer), "snapshot_bw.dump",
+                            "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n", **kw)
         if isinstance(ctx.num_rendered, _C.DeferredCount):
             ctx.num_rendered.resolve()          # after the backward kernels are in flight
             if ctx.num_rendered.overflowed:     # rare: re-run the forward with the exact size, differentiate that
                 warnings.warn(f"deferred rasterization overflowed its binning buffer ({int(ctx.num_rendered)} instances); "
                               "forward re-run inside backward (cotangents come from the truncated first attempt)")
-                out = _C.rasterize_gaussians(rs.bg, means3D, features, colors_precomp, opacities, scales, rotations,
-                                             rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
-                                             rs.tanfovy, rs.cx, rs.cy, rs.image_height, rs.image_width, sh, rs.sh_degree,
-                                             rs.campos, rs.prefiltered, rs.computer_pseudo_normal, False,
+                out = _C.rasterize_gaussians(*_forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales,
+                                                            rotations, cov3Ds_precomp),
                                              _min_capacity=int(ctx.num_rendered) + 4096)
-                if surface:                     # the adjoint of the re-run's own surface pass
+                if surface is not None:         # the adjoint of the re-run's own surface pass
                     kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
                 grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
         if ex is not None:                      # SH gradient: gather the views' factors, rebuild the mean locally
@@ -181,19 +206,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             exchange.gather_factors()
             g_sh_avg = exchange.rebuild_sh(means3D, campos_all, rs.sh_degree)
             grads = grads[:6] + (g_sh_avg,) + grads[7:]
-        (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
-         g_rotations) = grads[:9]
-        return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
-                g_rotations, g_cov3Ds, None, None) + _camera_grads(ctx, grads[9:], (rs.viewmatrix, rs.projmatrix, rs.campos))
-
-
-def _camera_grads(ctx, grads, inputs):
-    """The gradients of the node's last three inputs (viewmatrix, projmatrix, campos) in their shapes: None for those
-    that do not need one (and for all three when none was computed)."""
-    need = ctx.needs_input_grad[-3:]
-    if not grads:
-        return (None, None, None)
-    return tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads, inputs, need))
+        return _input_grads(ctx, grads, (rs.viewmatrix, rs.projmatrix, rs.campos))
 
 
 def _refuse_camera_grad_with_exchange(*cameras):
@@ -212,6 +225,21 @@ def _refuse_surface_grads_without_normals(surface_grads, computer_pseudo_normal)
     if surface_grads and not computer_pseudo_normal:
         raise ValueError("surface_grads=True needs computer_pseudo_normal=True: without it the normal and surface_xyz "
                          "outputs are zeros and have no gradient")
+
+
+def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features):
+    """The reference's input checks (exactly one of SHs and precomputed colours, and one of a scale/rotation pair and
+    a precomputed covariance), then (features, shs, colors_precomp, scales, rotations, cov3D_precomp) with every absent
+    input empty and absent features [P,0]."""
+    if (shs is None) == (colors_precomp is None):
+        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+    have_sr = scales is not None or rotations is not None
+    if ((scales is None or rotations is None) and cov3D_precomp is None) or (have_sr and cov3D_precomp is not None):
+        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+    empty = torch.Tensor([])
+    if features is None:
+        features = torch.empty_like(means3D[..., :0])
+    return (features,) + tuple(empty if t is None else t for t in (shs, colors_precomp, scales, rotations, cov3D_precomp))
 
 
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
@@ -244,20 +272,8 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                 rotations=None, cov3D_precomp=None, features=None):
-        if (shs is None) == (colors_precomp is None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        have_sr = scales is not None or rotations is not None
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                (have_sr and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        empty = torch.Tensor([])
-        shs = empty if shs is None else shs
-        colors_precomp = empty if colors_precomp is None else colors_precomp
-        scales = empty if scales is None else scales
-        rotations = empty if rotations is None else rotations
-        cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
-        if features is None:
-            features = torch.empty_like(means3D[..., :0])
+        features, shs, colors_precomp, scales, rotations, cov3D_precomp = _inputs(
+            means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features)
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
                                    scales, rotations, cov3D_precomp, self.raster_settings,
                                    surface_grads=self.surface_grads)
@@ -279,16 +295,10 @@ class _RasterizeViews(torch.autograd.Function):
         out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
                                  rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal)
-        (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz, weights,
-         radii, geomBuffer, binningBuffer, imgBuffer) = out
         ctx.meta = (rs, cams)
-        ctx.set_materialize_grads(False)
-        ctx.out_shapes = (color.shape, opacity.shape, depth.shape, feature.shape)
-        ctx.surface_grads = surface_grads
-        ctx.save_for_backward(colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix,
-                              projmatrix, campos, geomBuffer, binningBuffer, imgBuffer,
-                              *((opacity, depth) if surface_grads else ()))
-        return (num_rendered, num_contrib, color, opacity, depth, feature, normal, surface_xyz, weights, radii)
+        _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
+                      bg, viewmatrix, projmatrix, campos, *out[10:13])
+        return out[:10]
 
     @staticmethod
     def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature, g_normal, g_surface_xyz,
@@ -296,21 +306,14 @@ class _RasterizeViews(torch.autograd.Function):
         rs, cams = ctx.meta
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
          geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors[:14]
-        zeros = lambda g, shape: g if g is not None else torch.zeros(shape, dtype=torch.float32, device=means3D.device)
-        g_color, g_opacity = zeros(g_color, ctx.out_shapes[0]), zeros(g_opacity, ctx.out_shapes[1])
-        g_depth, g_feature = zeros(g_depth, ctx.out_shapes[2]), zeros(g_feature, ctx.out_shapes[3])
-        surface = None
-        if ctx.surface_grads and (g_normal is not None or g_surface_xyz is not None):
-            surface = (g_normal, g_surface_xyz) + tuple(ctx.saved_tensors[14:16])
+        g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
+                                                                   g_feature)
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
                                             cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
                                             g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
                                             rs.backward_geometry, cam_grads=any(ctx.needs_input_grad[11:14]),
-                                            surface=surface)
-        (g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales,
-         g_rotations) = grads[:9]
-        return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales,
-                g_rotations, g_cov3Ds, None, None) + _camera_grads(ctx, grads[9:], (viewmatrix, projmatrix, campos))
+                                            surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
+        return _input_grads(ctx, grads, (viewmatrix, projmatrix, campos))
 
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
@@ -344,27 +347,16 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     if _EXCHANGE is not None:
         raise RuntimeError("rasterize_views cannot take part in an installed gradient exchange (set_grad_exchange); "
                            "the multi-GPU path renders one view per rank")
-    if (shs is None) == (colors_precomp is None):
-        raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-    have_sr = scales is not None or rotations is not None
-    if ((scales is None or rotations is None) and cov3D_precomp is None) or (have_sr and cov3D_precomp is not None):
-        raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
+    features, shs, colors_precomp, scales, rotations, cov3D_precomp = _inputs(
+        means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features)
     P = means3D.shape[0]
     if V * P >= 1 << 30:
         raise ValueError(f"rasterize_views: V*P = {V * P} rows exceed the limit of 2^30")
     if tuple(means2D.shape) != (V, P, 3):
         raise ValueError(f"rasterize_views: means2D must be [V,P,3] = {(V, P, 3)}, got {tuple(means2D.shape)}")
     for name, t in (("features", features), ("colors_precomp", colors_precomp)):
-        if t is not None and t.dim() == 3 and t.shape[0] != V:
+        if t.dim() == 3 and t.shape[0] != V:
             raise ValueError(f"rasterize_views: per-view {name} must have V = {V} rows, got {t.shape[0]}")
-    empty = torch.Tensor([])
-    shs = empty if shs is None else shs
-    colors_precomp = empty if colors_precomp is None else colors_precomp
-    scales = empty if scales is None else scales
-    rotations = empty if rotations is None else rotations
-    cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
-    if features is None:
-        features = torch.empty_like(means3D[..., :0])
     # stacked here, outside the node, so that autograd routes each view's camera gradients to that view's tensors
     viewmatrix = torch.stack([s.viewmatrix for s in settings])
     projmatrix = torch.stack([s.projmatrix for s in settings])

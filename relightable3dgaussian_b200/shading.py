@@ -40,49 +40,57 @@ def _args(P, N, He, We):
 
 def _shade_args(inputs, transform):
     """ShadeArgs for the nine inputs (base_color, roughness, normals, viewdirs, incidents, env, visibility,
-    incident_dirs, incident_areas) and the optional [3,3] env transform, all as contiguous float32.  Returns the
-    struct and the converted inputs and transform, which must outlive the launch."""
+    incident_dirs, incident_areas) and the optional env transform, all as contiguous float32.  viewdirs [P,3] is one
+    view; viewdirs [V,P,3] is V views, with a [3,3] transform or one [V,3,3] per view.  Returns the struct and the
+    converted inputs and transform, which must outlive the launch."""
     ts = [_lib.f32(t) for t in inputs]
     tr = None if transform is None else _lib.f32(transform)
-    env, dirs = ts[5], ts[7]
+    viewdirs, env, dirs = ts[3], ts[5], ts[7]
     a = _args(dirs.shape[0], dirs.shape[1], env.shape[0], env.shape[1])
     (a.base_color, a.roughness, a.normals, a.viewdirs, a.incidents, a.env, a.visibility, a.incident_dirs,
      a.incident_areas) = [t.data_ptr() for t in ts]
     a.env_transform = None if tr is None else tr.data_ptr()
+    if viewdirs.dim() == 3:
+        a.V, a.transform_per_view = viewdirs.shape[0], int(tr is not None and tr.dim() == 3)
     return a, ts, tr
 
 
 class _RenderEquation(torch.autograd.Function):
+    """The shading step of one view (viewdirs [P,3], outputs [P,*]) or of V views (viewdirs [V,P,3], outputs [V,P,*])."""
+
     @staticmethod
     def forward(ctx, base_color, roughness, viewdirs, incidents, env, normals, visibility, dirs, areas, transform, want_means):
         P = dirs.shape[0]
+        lead = tuple(viewdirs.shape[:-2])
         f = dict(dtype=torch.float32, device=dirs.device)
         a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas), transform)
-        pbr, diffuse, specular = (torch.empty((P, 3), **f) for _ in range(3))
+        pbr, diffuse, specular = (torch.empty(lead + (P, 3), **f) for _ in range(3))
         a.pbr, a.diffuse_light, a.specular = pbr.data_ptr(), diffuse.data_ptr(), specular.data_ptr()
-        means = None
+        means = []
         if want_means:
-            means = [torch.empty((P, 3), **f) for _ in range(3)] + [torch.empty((P, 1), **f)]
+            means = [torch.empty(lead + (P, 3), **f) for _ in range(3)] + [torch.empty(lead + (P, 1), **f)]
             a.mean_incident_lights, a.mean_local_lights, a.mean_global_lights, a.mean_visibility = [m.data_ptr() for m in means]
         if P > 0:
             _lib.call("r3dg_render_equation_forward", dirs.device, ctypes.byref(a), what="rendering_equation")
         ctx.save_for_backward(*ts)
         ctx.transform = tr
-        ctx.mark_non_differentiable(*(means or []))
-        return (pbr, diffuse, specular) + tuple(means or [])
+        ctx.mark_non_differentiable(*means)
+        return (pbr, diffuse, specular) + tuple(means)
 
     @staticmethod
     def backward(ctx, g_pbr, g_diffuse, g_specular, *_):
         a, ts, _ = _shade_args(ctx.saved_tensors, ctx.transform)
-        env, dirs = ts[5], ts[7]
+        env, viewdirs, dirs = ts[5], ts[3], ts[7]
         P = dirs.shape[0]
         dev = dirs.device
         f = dict(dtype=torch.float32, device=dev)
-        d_base, d_view = torch.empty((P, 3), **f), torch.empty((P, 3), **f)
+        d_base, d_view = torch.empty((P, 3), **f), torch.empty(viewdirs.shape, **f)
         d_rough = torch.empty((P, 1), **f)
         d_inc = torch.empty((P, 16, 3), **f)
         d_env = torch.empty(env.shape, **f)
-        gz = torch.zeros((P, 3), **f)
+        if P == 0:                      # nothing to shade: empty gradients (no device pointers to pass)
+            return d_base, d_rough, d_view, d_inc, d_env.zero_(), None, None, None, None, None, None
+        gz = torch.zeros(viewdirs.shape, **f)
         g = [gz if t is None else _lib.f32(t) for t in (g_pbr, g_diffuse, g_specular)]
         a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = [t.data_ptr() for t in g]
         a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = d_base.data_ptr(), d_rough.data_ptr(), d_view.data_ptr()
@@ -157,50 +165,6 @@ MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
 _MEANS = ("mean_incident_lights", "mean_local_incident_lights", "mean_global_incident_lights", "mean_incident_visibility")
 
 
-class _RenderEquationViews(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, base_color, roughness, viewdirs, incidents, env, normals, visibility, dirs, areas, transform, want_means):
-        V, P = viewdirs.shape[0], dirs.shape[0]
-        f = dict(dtype=torch.float32, device=dirs.device)
-        a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas), transform)
-        a.V, a.transform_per_view = V, int(tr is not None and tr.dim() == 3)
-        pbr, diffuse, specular = (torch.empty((V, P, 3), **f) for _ in range(3))
-        a.pbr, a.diffuse_light, a.specular = pbr.data_ptr(), diffuse.data_ptr(), specular.data_ptr()
-        means = []
-        if want_means:
-            means = [torch.empty((V, P, 3), **f) for _ in range(3)] + [torch.empty((V, P, 1), **f)]
-            a.mean_incident_lights, a.mean_local_lights, a.mean_global_lights, a.mean_visibility = [m.data_ptr() for m in means]
-        if P > 0:
-            _lib.call("r3dg_render_equation_forward", dirs.device, ctypes.byref(a), what="rendering_equation_views")
-        ctx.save_for_backward(*ts)
-        ctx.transform = tr
-        ctx.mark_non_differentiable(*means)
-        return (pbr, diffuse, specular) + tuple(means)
-
-    @staticmethod
-    def backward(ctx, g_pbr, g_diffuse, g_specular, *_):
-        a, ts, _ = _shade_args(ctx.saved_tensors, ctx.transform)
-        env, viewdirs, dirs = ts[5], ts[3], ts[7]
-        V, P = viewdirs.shape[0], dirs.shape[0]
-        a.V = V
-        dev = dirs.device
-        f = dict(dtype=torch.float32, device=dev)
-        d_base, d_view = torch.empty((P, 3), **f), torch.empty((V, P, 3), **f)
-        d_rough = torch.empty((P, 1), **f)
-        d_inc = torch.empty((P, 16, 3), **f)
-        d_env = torch.empty(env.shape, **f)
-        if P == 0:                      # nothing to shade: empty gradients (no device pointers to pass)
-            return d_base, d_rough, d_view, d_inc, d_env.zero_(), None, None, None, None, None, None
-        gz = torch.zeros((V, P, 3), **f)
-        g = [gz if t is None else _lib.f32(t) for t in (g_pbr, g_diffuse, g_specular)]
-        a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = [t.data_ptr() for t in g]
-        a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = d_base.data_ptr(), d_rough.data_ptr(), d_view.data_ptr()
-        a.dL_dincidents, a.dL_denv = d_inc.data_ptr(), d_env.data_ptr()
-        det_ws = _lib.det_workspace(a, _lib.load().r3dg_shade_det_bytes(env.shape[0], env.shape[1]), dev)
-        _lib.call("r3dg_render_equation_backward", dev, ctypes.byref(a), what="rendering_equation_views backward")
-        return d_base, d_rough, d_view, d_inc, d_env, None, None, None, None, None, None
-
-
 def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents, direct_light_env_light=None,
                              visibility_precompute=None, incident_dirs_precompute=None, incident_areas_precompute=None,
                              means=False):
@@ -231,8 +195,8 @@ def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents
             raise ValueError(f"a per-view transform must be [V,3,3] with V = {V} (got {tuple(transform.shape)})")
         if torch.is_grad_enabled() and any(t.requires_grad for t in (base_color, roughness, viewdirs, incidents, env)):
             raise ValueError("per-view transforms are forward-only: call under torch.no_grad() or with detached inputs")
-    outs = _RenderEquationViews.apply(base_color, roughness, viewdirs, incidents, env, normals, vis, dirs, areas, transform,
-                                      bool(means))
+    outs = _RenderEquation.apply(base_color, roughness, viewdirs, incidents, env, normals, vis, dirs, areas, transform,
+                                 bool(means))
     pbr, diffuse, specular = outs[:3]
     extra = {"incident_dirs": dirs, "incident_visibility": vis, "diffuse_light": diffuse, "specular": specular}
     extra.update(zip(_MEANS, outs[3:]))

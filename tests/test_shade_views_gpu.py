@@ -190,6 +190,15 @@ def test_empty_gaussian_set():
     (pbr.sum() + ex["diffuse_light"].sum()).backward()
     assert env_raw.grad is not None and not env_raw.grad.any()
     assert vd.grad.shape == (3, 0, 3) and bc.grad.shape == (0, 3)
+    # one view: the same node, forward and backward
+    vd1 = c["viewdirs_v"][0].clone().requires_grad_(True)
+    env_raw.grad = bc.grad = None
+    pbr, ex = rendering_equation(bc, c["roughness"], c["normals"], vd1, c["incidents"], SoftplusLight(env_raw),
+                                 c["visibility"], c["incident_dirs"], c["incident_areas"])
+    assert pbr.shape == (0, 3) and ex["specular"].shape == (0, 3) and ex["incident_lights"].shape == (0, 8, 3)
+    (pbr.sum() + ex["diffuse_light"].sum()).backward()
+    assert env_raw.grad is not None and not env_raw.grad.any()
+    assert vd1.grad.shape == (0, 3) and bc.grad.shape == (0, 3)
 
 
 # ---- 6. a V-view stage-2 step against V one-view steps --------------------------------------------------------------------

@@ -255,7 +255,8 @@ def test_views_planes_equal_one_view_calls(det):
 
 def test_one_view_rasterize_views_equals_gaussian_rasterizer(det_mode):
     """rasterize_views with a single setting runs the one-view library call: its surface adjoint must use that
-    setting's principal point (here off-centre) and give GaussianRasterizer's gradients."""
+    setting's principal point (here off-centre) and give GaussianRasterizer's gradients, bit for bit in the
+    deterministic mode (both make the same library call)."""
     P, W, H, S = 100_000, 240, 180, 5
     leaves = make_leaves(P, S)
     cam = synth.make_camera(1, W, H, center_shift=True)
@@ -275,6 +276,7 @@ def test_one_view_rasterize_views_equals_gaussian_rasterizer(det_mode):
         assert torch.isfinite(gs[k]).all(), k
         e = rel_l2(gs[k].cpu().numpy(), want[k].cpu().numpy())
         assert e <= 1e-6, (k, e)
+    assert [k for k in names if not bits_equal(gs[k], want[k])] == []
 
 
 # ---- 5. reproducibility and the deferred-count repair -------------------------------------------------------------
