@@ -140,6 +140,22 @@ typedef struct r3dg_raster_bwd_args {
     float* dL_dscales;             /* [P,3] */
     float* dL_drotations;          /* [P,4] */
     float* dL_dsh_factor;          /* [P,3] or NULL: the view's rank-1 factor of dL_dsh, see r3dg_sh_grad_from_factors */
+    /* APPEARANCE-ONLY MODE (for training with frozen geometry): every geometry output NULL — dL_dmeans2D,
+     * dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dscales, dL_drotations and the three camera gradients.  The backward
+     * then computes only the colour / feature / SH gradients: the compositor forms and reduces only the 3 + S colour
+     * and feature components of each entry (no dL/dalpha), and no covariance, mean or camera chain runs.
+     *   - Some of the six per-Gaussian geometry outputs NULL and others not, or a camera gradient with all six NULL,
+     *     returns R3DG_ERR_BAD_ARG before any launch.
+     *   - dL_dcolors, dL_dfeatures and dL_dsh may each be NULL (not computed); all three NULL returns
+     *     R3DG_ERR_BAD_ARG.  Every element of a requested output is written, rows no pixel composited as +0.  (P = 0
+     *     writes no per-Gaussian output and refuses none of these combinations.)
+     *   - The cotangents of opacity, depth, pseudo-normal and surface-xyz are ignored (they may be NULL): those outputs
+     *     depend only on the geometry and have no appearance gradient.
+     *   - One view and V views (per-view features / colors included) and the deterministic mode work as in the full
+     *     backward, with the same workspace; a requested gradient equals the full backward's (bitwise in deterministic
+     *     mode).  With `shs`, dL_dsh_factor, when given, receives each view's factor exactly as in the full backward;
+     *     V > 1 with dL_dsh requires it, as there.
+     * The per-view projection backward is replaced by one launch over all views. */
     /* work buffers written by the matching forward */
     void* geom;   size_t geom_bytes;
     void* img;    size_t img_bytes;

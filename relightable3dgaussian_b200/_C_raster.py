@@ -20,6 +20,10 @@ float atomics make them run-to-run nondeterministic).  Its workspace comes from 
 
 One view and V views of the same Gaussians (rasterize_views / rasterize_views_backward) run through the same two
 host paths, _forward and _backward: the library treats a one-view call as V = 1.
+
+`geometry=False` on the two backward functions (not part of the reference surface) runs the library's appearance-only
+backward: only the colour / feature / SH gradients, for training with frozen geometry.  The reference's
+rasterize_gaussians_backward, as the dropin calls it, always runs the full backward.
 """
 import ctypes
 import warnings
@@ -238,11 +242,16 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
 def _backward(views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
-              surface_work, principal):
+              surface_work, principal, geometry=True, appearance=(True, True, True)):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
     one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
-    are those of rasterize_gaussians_backward (`surface` without the principal point)."""
+    are those of rasterize_gaussians_backward (`surface` without the principal point).
+    `geometry=False`: the appearance-only backward.  Nothing is allocated for the six geometry gradients, which come
+    back None, and of dL_dfeatures, dL_dcolors, dL_dsh only those `appearance` = (features, colors, sh) asks for are
+    computed (the others are None too); the opacity, depth and surface cotangents are not read."""
+    if not geometry and (cam_grads or _out is not None):
+        raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     H, W = dL_dout_color.size(-2), dL_dout_color.size(-1)
@@ -266,29 +275,39 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
             return t
         return torch.empty(shape, **f32)
 
-    dL_dmeans3D = _alloc("means3D", (P, 3))
-    dL_dmeans2D = _alloc("means2D", ((V,) if views else ()) + (P, 3))
-    dL_dfeatures = _alloc("features", (V, P, S) if a.features_per_view else (P, S))
-    dL_dcolors = _alloc("colors", (V, P, 3) if a.colors_per_view else (P, 3))
-    dL_dopacity = _alloc("opacity", (P, 1))
-    dL_dcov3D = _alloc("cov3D", (P, 6))
-    # multi-GPU exchange (dist.FactoredGradExchange): `_out["sh_factor"]` [P,3] asks for the view's rank-1
-    # factor of dL_dsh INSTEAD of the dense tensor (returned empty), see r3dg_sh_grad_from_factors
-    sh_factor = _out.get("sh_factor") if _out is not None else None
-    if sh_factor is not None:
-        assert sh_factor.is_contiguous() and tuple(sh_factor.shape) == (P, 3) and sh_factor.dtype == torch.float32
-        if M == 0:
-            raise RuntimeError("the SH-gradient factor needs `sh` inputs (colors_precomp has no SH gradient)")
-        dL_dsh = _alloc("sh", (P, M, 3)) if "sh" in _out else torch.empty((0,), **f32)     # both on request (tests)
+    if not geometry:                      # appearance-only: the requested appearance gradients, nothing else
+        need_features, need_colors, need_sh = appearance
+        dL_dmeans3D = dL_dmeans2D = dL_dopacity = dL_dcov3D = dL_dscales = dL_drotations = None
+        dL_dfeatures = torch.empty((V, P, S) if a.features_per_view else (P, S), **f32) if need_features else None
+        dL_dcolors = (torch.empty((V, P, 3) if a.colors_per_view else (P, 3), **f32)
+                      if need_colors and a.colors_precomp else None)
+        dL_dsh = torch.empty((P, M, 3), **f32) if need_sh and M > 0 else None
+        sh_factor = torch.empty((V, P, 3), **f32) if dL_dsh is not None and V > 1 else None
     else:
-        dL_dsh = _alloc("sh", (P, M, 3))
-        if V > 1 and M > 0:               # the library rebuilds dL_dsh from the views' rank-1 factors
-            sh_factor = torch.empty((V, P, 3), **f32)
-    dL_dscales = _alloc("scales", (P, 3))
-    dL_drotations = _alloc("rotations", (P, 4))
+        dL_dmeans3D = _alloc("means3D", (P, 3))
+        dL_dmeans2D = _alloc("means2D", ((V,) if views else ()) + (P, 3))
+        dL_dfeatures = _alloc("features", (V, P, S) if a.features_per_view else (P, S))
+        dL_dcolors = _alloc("colors", (V, P, 3) if a.colors_per_view else (P, 3))
+        dL_dopacity = _alloc("opacity", (P, 1))
+        dL_dcov3D = _alloc("cov3D", (P, 6))
+        # multi-GPU exchange (dist.FactoredGradExchange): `_out["sh_factor"]` [P,3] asks for the view's rank-1
+        # factor of dL_dsh INSTEAD of the dense tensor (returned empty), see r3dg_sh_grad_from_factors
+        sh_factor = _out.get("sh_factor") if _out is not None else None
+        if sh_factor is not None:
+            assert sh_factor.is_contiguous() and tuple(sh_factor.shape) == (P, 3) and sh_factor.dtype == torch.float32
+            if M == 0:
+                raise RuntimeError("the SH-gradient factor needs `sh` inputs (colors_precomp has no SH gradient)")
+            dL_dsh = _alloc("sh", (P, M, 3)) if "sh" in _out else torch.empty((0,), **f32)     # both on request (tests)
+        else:
+            dL_dsh = _alloc("sh", (P, M, 3))
+            if V > 1 and M > 0:               # the library rebuilds dL_dsh from the views' rank-1 factors
+                sh_factor = torch.empty((V, P, 3), **f32)
+        dL_dscales = _alloc("scales", (P, 3))
+        dL_drotations = _alloc("rotations", (P, 4))
     # zeroed: a call with P = 0 writes nothing, otherwise the library overwrites every element
     cam = tuple(torch.zeros(shape, **f32) for shape in ((V, 4, 4), (V, 4, 4), (V, 3))) if cam_grads else ()
-    if P != 0:
+    # (appearance-only with nothing to compute: no call, e.g. S = 0 features the only input that needs a gradient)
+    if P != 0 and (geometry or any(_lib.ptr(t) for t in (dL_dfeatures, dL_dcolors, dL_dsh))):
         a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
         a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
         a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
@@ -305,7 +324,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
             cam_ws = _lib.scratch(lib.r3dg_raster_cam_grad_bytes(P, V), dev)
             a.dL_dviewmatrix, a.dL_dprojmatrix, a.dL_dcampos = (t.data_ptr() for t in cam)
             a.cam_work, a.cam_work_bytes = cam_ws.data_ptr(), cam_ws.numel()
-        surface_ws = _surface_args(a, surface, W, H, V, dev, surface_work, principal=principal)
+        surface_ws = _surface_args(a, surface if geometry else None, W, H, V, dev, surface_work, principal=principal)
         _lib.call("r3dg_raster_backward", dev, ctypes.byref(a),
                   what="rasterize_views_backward" if views else "rasterize_gaussians_backward")
     return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
@@ -317,7 +336,7 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  tan_fovy, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
                                  imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
-                                 surface_work=None):
+                                 surface_work=None, geometry=True, appearance=(True, True, True)):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
@@ -325,13 +344,16 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     `projmatrix` and `campos`.  `surface` (not part of the reference surface either) differentiates the pseudo-normal
     and surface-xyz outputs: (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth, cx, cy) with the forward's
     opacity and depth images; a cotangent may be None.  `surface_work` optionally supplies the workspace
-    (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards."""
+    (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards.
+    `geometry=False` (not part of the reference surface either) is the appearance-only backward of _backward: the
+    gradients of the geometry inputs, and of the appearance inputs `appearance` = (features, colors, sh) leaves out,
+    come back None."""
     principal = surface[4:6] if surface is not None and len(surface) == 6 else None
     grads, cam = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
                            dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
                            binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
-                           surface and surface[:4], surface_work, principal)
+                           surface and surface[:4], surface_work, principal, geometry, appearance)
     return grads + tuple(t[0] for t in cam)
 
 
@@ -427,7 +449,8 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
 def rasterize_views_backward(background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
                              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
-                             backward_geometry, cam_grads=False, surface=None, surface_work=None):
+                             backward_geometry, cam_grads=False, surface=None, surface_work=None, geometry=True,
+                             appearance=(True, True, True)):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
@@ -435,9 +458,11 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     gradients follow, never summed: dL_dviewmatrix [V,4,4], dL_dprojmatrix [V,4,4], dL_dcampos [V,3].  `surface` =
     (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth), all [V,*,H,W] (a cotangent may be None), and
     `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
-    one view, cams[0]'s, entered as the call's cx, cy)."""
+    one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
+    rasterize_gaussians_backward."""
     grads, cam = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                            dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
-                           backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4])
+                           backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
+                           appearance)
     return grads + cam

@@ -256,12 +256,20 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     const int V = views_of(a->V, a->view_cams, a->P);
     if (V == 0) return R3DG_ERR_BAD_ARG;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S))) return R3DG_ERR_BAD_ARG;
-    if (V > 1 && a->P > 0 && a->shs && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     const int cam_outs = (a->dL_dviewmatrix != nullptr) + (a->dL_dprojmatrix != nullptr) + (a->dL_dcampos != nullptr);
+    // appearance-only mode: every geometry output NULL (the six per-Gaussian ones and the camera gradients).  P = 0
+    // writes no per-Gaussian output, and is refused for none of them, as before this mode existed.
+    const int geo_outs = (a->dL_dmeans2D != nullptr) + (a->dL_dopacity != nullptr) + (a->dL_dmeans3D != nullptr) +
+                         (a->dL_dcov3D != nullptr) + (a->dL_dscales != nullptr) + (a->dL_drotations != nullptr);
+    const bool geometry = geo_outs == 6 || a->P == 0;
+    if (a->P > 0 && geo_outs != 0 && geo_outs != 6) return R3DG_ERR_BAD_ARG;
+    if (!geometry && (cam_outs != 0 || (!a->dL_dcolors && !a->dL_dfeatures && !a->dL_dsh))) return R3DG_ERR_BAD_ARG;
+    if (V > 1 && a->P > 0 && a->shs && (geometry || a->dL_dsh) && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;
     const bool cam = cam_outs == 3;
     if (cam && (!a->cam_work || a->cam_work_bytes < r3dg_raster_cam_grad_bytes(a->P, V))) return R3DG_ERR_BAD_ARG;
-    const bool surface = a->dL_dout_normal || a->dL_dout_surface_xyz;
+    // (appearance-only: the opacity, depth, pseudo-normal and surface-xyz cotangents have no appearance gradient)
+    const bool surface = geometry && (a->dL_dout_normal || a->dL_dout_surface_xyz);
     if (surface && (!a->fwd_opacity || !a->fwd_depth || !a->dL_dout_opacity || !a->dL_dout_depth || !a->surface_work ||
                     a->surface_work_bytes < r3dg_raster_surface_grad_bytes(a->W, a->H, V))) return R3DG_ERR_BAD_ARG;
     if (a->P == 0) {
@@ -293,13 +301,18 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
         sa.dL_dout_opacity = planes + (size_t)V * a->W * a->H;
         a = &sa;
     }
-    if ((rc = launch_composite_backward(*a, b, stream)) != 0) return rc;
+    if ((rc = launch_composite_backward(*a, b, geometry, stream)) != 0) return rc;
     prof_mark(false, 9, stream);
     // one projection backward per view, in view order: view 0 writes the summed gradients, every later view adds its
-    // own to them (a left fold in fp32), per-view outputs go to the view's rows
-    for (int v = 0; v < V; ++v)
-        if ((rc = launch_projection_backward(*a, view_slice(b, v), v, stream)) != 0) return rc;
-    if (V > 1 && a->shs) {          // dL_dsh from the views' rank-1 factors, views in order
+    // own to them (a left fold in fp32), per-view outputs go to the view's rows.  Appearance-only: one launch for all
+    // views writes the colour, feature and SH outputs the same way (the profiler counts it as the projection backward).
+    if (geometry) {
+        for (int v = 0; v < V; ++v)
+            if ((rc = launch_projection_backward(*a, view_slice(b, v), v, stream)) != 0) return rc;
+    } else if ((rc = launch_appearance_backward(*a, b, stream)) != 0) {
+        return rc;
+    }
+    if (V > 1 && a->shs && a->dL_dsh) {     // dL_dsh from the views' rank-1 factors, views in order
         if ((rc = r3dg_sh_grad_from_factors(a->P, a->D, a->M, V, a->means3D, a->campos, a->dL_dsh_factor, 1.0f, a->dL_dsh,
                                             stream_)) != 0) return rc;
     }
@@ -310,9 +323,9 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (surface_cam &&              // then the pseudo-normal's term of dL/dviewmatrix, added after the projection's
         (rc = launch_surface_cam_sum(surface_part, surface_blocks, V, a->dL_dviewmatrix, stream)) != 0) return rc;
     prof_mark(false, 10, stream);
-    // zeroing of the composited rows, CTA order, composite, projection per view, camera sums (the SH rebuild counts
-    // itself); surface pass per view and its camera sums
-    g_launches += 3 + V + (cam ? 1 : 0) + (surface ? V : 0) + (surface_cam ? 1 : 0);
+    // zeroing of the composited rows, CTA order, composite, projection per view (appearance-only: one launch), camera
+    // sums (the SH rebuild counts itself); surface pass per view and its camera sums
+    g_launches += 3 + (geometry ? V : 1) + (cam ? 1 : 0) + (surface ? V : 0) + (surface_cam ? 1 : 0);
     if (g_prof.on) g_prof.bwd_calls++;
     if (a->debug) {
         cudaError_t e = cudaStreamSynchronize(stream);

@@ -142,9 +142,14 @@ __device__ __forceinline__ void reduce_scatter_permuted_multi(float (&x)[U][W], 
 // block composited in the forward pass — no culling test, no record fetch and no exp() for anything else.
 // DET (deterministic mode): each finished row component is added through the order-independent fixed-point primitive
 // (detacc.cuh) into p.det instead of by a float atomic into p.grad.  Everything else is the same code.
-template <int NG, int NW, int MINB, bool DET = false>
+// GEOM = false (appearance-only backward, no geometry gradient requested): the same walk, CTA order and alpha / T
+// arithmetic, but only the NC colour and feature components are formed and reduced — no dL/dalpha, no A recurrence, no
+// geometry butterfly — into a narrower row of NC floats (channel c at slot c).  Every channel component goes through the
+// same butterfly as with GEOM, so each added value, and in DET mode each row total, is bitwise the full kernel's.
+template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const CompositeBwdParams p) {
     constexpr int NC = 4 * NG;              // padded channel count {r,g,b,f...}; gradient row = 8 geometry slots + NC
+    constexpr int GOFF = GEOM ? 8 : 0;      // slot of channel 0 in the gradient row (GEOM = false: no geometry slots)
     // the NC channel components are reduced in power-of-two chunks of 16 / 8 / 4 (select-free butterflies)
     constexpr int C16 = NC >= 16 ? 16 : 0, C8 = (NC - C16) >= 8 ? 8 : 0, C4 = NC - C16 - C8;
     constexpr int B8 = C16, B4 = C16 + C8;
@@ -212,18 +217,21 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     }
     // which finished component this lane adds to the Gaussian's gradient row: geometry slot lane >> 2 on lanes 0 mod 4,
     // the 16-chunk on odd lanes, the 8-chunk on lanes 2 mod 4, the 4-chunk on a free lane class (second instruction
-    // only when all three chunks exist, NG == 7)
-    constexpr bool C4_SECOND = C16 > 0 && C8 > 0 && C4 > 0;
+    // only when all three chunks exist, NG == 7, and the geometry slots take lanes 0 mod 4; without them the 4-chunk
+    // takes lanes 0 mod 8)
+    constexpr bool C4_SECOND = GEOM && C16 > 0 && C8 > 0 && C4 > 0;
+    constexpr int C4_CLASS = C16 > 0 ? (C8 > 0 ? 0 : 2) : 1;
     int my_sel = -1, my_off = 0;
-    if ((lane & 3) == 0) { if ((lane >> 2) != 7) { my_sel = 0; my_off = lane >> 2; } }
-    else if (C16 > 0 && (lane & 1)) { my_sel = 1; my_off = 8 + (lane >> 1); }
-    else if (C8 > 0 && (lane & 3) == 2) { my_sel = 2; my_off = 8 + B8 + (lane >> 2); }
-    if (C4 > 0 && !C4_SECOND && (lane & 7) == (C16 > 0 ? 2 : 1)) { my_sel = 3; my_off = 8 + B4 + (lane >> 3); }
-    if (my_sel > 0 && my_off - 8 >= 3 + p.S) my_sel = -1;    // zero padding channel
-    const float dpix_d = inside ? p.dL_dpix_d[vpix] : 0.0f;
-    const float dpix_o = inside ? p.dL_dpix_o[vpix] : 0.0f;
+    if ((lane & 3) == 0) { if (GEOM && (lane >> 2) != 7) { my_sel = 0; my_off = lane >> 2; } }
+    else if (C16 > 0 && (lane & 1)) { my_sel = 1; my_off = GOFF + (lane >> 1); }
+    else if (C8 > 0 && (lane & 3) == 2) { my_sel = 2; my_off = GOFF + B8 + (lane >> 2); }
+    if (C4 > 0 && !C4_SECOND && (lane & 7) == C4_CLASS) { my_sel = 3; my_off = GOFF + B4 + (lane >> 3); }
+    if (my_sel > 0 && my_off - GOFF >= 3 + p.S) my_sel = -1;    // zero padding channel
+    // GEOM = false: the opacity and depth cotangents have no appearance gradient and are not read
+    const float dpix_d = GEOM && inside ? p.dL_dpix_d[vpix] : 0.0f;
+    const float dpix_o = GEOM && inside ? p.dL_dpix_o[vpix] : 0.0f;
     const float* bg = p.bg + 3 * view;
-    const float bg_dot = bg[0] * dpix[0] + bg[1] * dpix[1] + bg[2] * dpix[2];
+    const float bg_dot = GEOM ? bg[0] * dpix[0] + bg[1] * dpix[1] + bg[2] * dpix[2] : 0.0f;
     const float ddelx_dx = 0.5f * p.W, ddely_dy = 0.5f * p.H;
     const bool geo = p.backward_geometry != 0;
     // The reference keeps, per channel, the colour accumulated BEHIND the current entry (accum_rec[ch], backward.cu:
@@ -279,7 +287,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     while (qcount > 0) {
         const int n = min(32, qcount);
         __syncwarp();
-        sId[warp][lane] = id_cur * (uint32_t)p.recf;                   // element offset of the Gaussian's gradient row
+        sId[warp][lane] = id_cur * (uint32_t)(GEOM ? p.recf : NC);     // element offset of the Gaussian's gradient row
         sK[warp][lane] = k_cur;                                        // 0-based list position == contributor index
 #pragma unroll
         for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = r[g];
@@ -321,14 +329,17 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                 // products below (0 * inf) would be NaN.  Composited entries have power <= 0, so G <= 1 is unchanged.
                 G[u] = valid[u] ? G[u] : 0.0f;
                 asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv[u]) : "f"(1.0f - alpha[u]));   // 1 - alpha in [0.01, 1]: one MUFU
-                float d = fmaf(b.z, dpix_d, dpix_o);                        // depth * dL_ddepth + 1 * dL_dopacity
+                float d = 0.0f;
+                if constexpr (GEOM) {
+                    d = fmaf(b.z, dpix_d, dpix_o);                          // depth * dL_ddepth + 1 * dL_dopacity
 #pragma unroll
-                for (int g = 0; g < NG; ++g) {
-                    const float4 c4 = sRec[warp][2 + g][ju[u]];
-                    d = fmaf(c4.x, dsel[4 * g + 0], d);
-                    d = fmaf(c4.y, dsel[4 * g + 1], d);
-                    d = fmaf(c4.z, dsel[4 * g + 2], d);
-                    d = fmaf(c4.w, dsel[4 * g + 3], d);
+                    for (int g = 0; g < NG; ++g) {
+                        const float4 c4 = sRec[warp][2 + g][ju[u]];
+                        d = fmaf(c4.x, dsel[4 * g + 0], d);
+                        d = fmaf(c4.y, dsel[4 * g + 1], d);
+                        d = fmaf(c4.z, dsel[4 * g + 2], d);
+                        d = fmaf(c4.w, dsel[4 * g + 3], d);
+                    }
                 }
                 D[u] = d;
             }
@@ -338,12 +349,20 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                 const float gate = valid[u] ? 1.0f : 0.0f;                  // the entry contribute zeros and keep their state
                 const float Tn = T * inv[u];                                // T before this entry (backward.cu:533)
                 dcc[u] = gate * alpha[u] * Tn;
-                dL_dalpha[u] = gate * fmaf(D[u] - A, Tn, -(T_final * inv[u]) * bg_dot);
-                if (valid[u]) { A = fmaf(alpha[u], D[u] - A, A); T = Tn; } // A <- alpha D + (1 - alpha) A
+                if constexpr (GEOM) {
+                    dL_dalpha[u] = gate * fmaf(D[u] - A, Tn, -(T_final * inv[u]) * bg_dot);
+                    if (valid[u]) { A = fmaf(alpha[u], D[u] - A, A); T = Tn; } // A <- alpha D + (1 - alpha) A
+                } else if (valid[u]) {
+                    T = Tn;
+                }
             }
             float v0[U][8], mine[U];
+            if constexpr (!GEOM) {
 #pragma unroll
-            for (int u = 0; u < U; ++u) {                                   // (3)
+                for (int u = 0; u < U; ++u) mine[u] = 0.0f;
+            }
+#pragma unroll
+            for (int u = 0; u < U && GEOM; ++u) {                           // (3)
                 const float4 a = sRec[warp][0][ju[u]];
                 const float4 b = sRec[warp][1][ju[u]];
                 const float dL_dG = b.y * dL_dalpha[u];
@@ -359,7 +378,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                 v0[u][6] = -0.5f * gdy * dy[u] * dL_dG;
                 v0[u][7] = 0.0f;
             }
-            reduce_scatter_multi<U, 8>(v0, lane, mine);                     // geometry slots: lanes 0 mod 4
+            if constexpr (GEOM) reduce_scatter_multi<U, 8>(v0, lane, mine); // geometry slots: lanes 0 mod 4
             if constexpr (C16 > 0) {
                 float x[U][16], t[U];
 #pragma unroll
@@ -448,13 +467,20 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
     g_bwd_ctas = value;
     return 0;
 }
-template <int NG, bool DET>
-static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
-    constexpr auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET>;
+template <int NG, bool DET, bool GEOM>
+static void launch_bwd_kernel(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
+    constexpr auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET, GEOM>;
     kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
+template <int NG>
+static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, bool det, bool geometry, cudaStream_t stream) {
+    if (geometry) det ? launch_bwd_kernel<NG, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true>(p, tiles, stream);
+    else det ? launch_bwd_kernel<NG, true, false>(p, tiles, stream) : launch_bwd_kernel<NG, false, false>(p, tiles, stream);
+}
 
-int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
+int composite_bwd_row_floats(int S, bool geometry) { return geometry ? rec_floats(S) : 4 * num_groups(S); }
+
+int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, bool geometry, cudaStream_t stream) {
     CompositeBwdParams p;
     const int V = b.V;
     p.W = a.W; p.H = a.H; p.gx = b.gx; p.gy = b.gy; p.S = a.S; p.recf = b.recf;
@@ -472,22 +498,23 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     p.n_contrib = b.n_contrib;
     const bool det = a.deterministic != 0;
     const size_t rows = (size_t)V * a.P;
-    p.det = det_acc(a.det_work, rows * b.recf);
+    const int gradf = composite_bwd_row_floats(a.S, geometry);     // the gradient row: b.recf, or NC without geometry
+    p.det = det_acc(a.det_work, rows * gradf);
     // zeroed here, in the backward, so that every backward over one forward (retain_graph) starts from zero
     const int zblocks = (int)((rows + 255) / 256);
-    if (det) zero_composited_rows_kernel<true><<<zblocks, 256, 0, stream>>>(rows, b.recf, b.clamped, p.grad, p.det);
-    else zero_composited_rows_kernel<false><<<zblocks, 256, 0, stream>>>(rows, b.recf, b.clamped, p.grad, p.det);
+    if (det) zero_composited_rows_kernel<true><<<zblocks, 256, 0, stream>>>(rows, gradf, b.clamped, p.grad, p.det);
+    else zero_composited_rows_kernel<false><<<zblocks, 256, 0, stream>>>(rows, gradf, b.clamped, p.grad, p.det);
     const int tiles = V * b.tiles;                    // the tall grid of all views
     int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;
     switch (num_groups(a.S)) {
-        case 1: det ? launch_bwd_ng<1, true>(p, tiles, stream) : launch_bwd_ng<1, false>(p, tiles, stream); break;
-        case 2: det ? launch_bwd_ng<2, true>(p, tiles, stream) : launch_bwd_ng<2, false>(p, tiles, stream); break;
-        case 3: det ? launch_bwd_ng<3, true>(p, tiles, stream) : launch_bwd_ng<3, false>(p, tiles, stream); break;
-        case 4: det ? launch_bwd_ng<4, true>(p, tiles, stream) : launch_bwd_ng<4, false>(p, tiles, stream); break;
-        case 5: det ? launch_bwd_ng<5, true>(p, tiles, stream) : launch_bwd_ng<5, false>(p, tiles, stream); break;
-        case 6: det ? launch_bwd_ng<6, true>(p, tiles, stream) : launch_bwd_ng<6, false>(p, tiles, stream); break;
-        case 7: det ? launch_bwd_ng<7, true>(p, tiles, stream) : launch_bwd_ng<7, false>(p, tiles, stream); break;
+        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, stream); break;
+        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, stream); break;
+        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, stream); break;
+        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, stream); break;
+        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, stream); break;
+        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, stream); break;
+        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;   // S > 24: reference backward limit (backward.cu:449)
     }
     R3DG_CUDA_TRY(cudaGetLastError());

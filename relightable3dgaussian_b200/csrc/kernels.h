@@ -74,8 +74,13 @@ int launch_rebuild_keys(int T, const void* ranges, const uint32_t* point_list, c
                         long long limit, uint64_t* keys, cudaStream_t stream);
 int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers& b, cudaStream_t stream,
                              stage_mark_fn mark);
-int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
+// geometry = false: the appearance-only backward (r3dg_raster_backward with every geometry output NULL).  The
+// compositor then leaves rows of composite_bwd_row_floats(S, false) = 4 * num_groups(S) channel gradients, and
+// launch_appearance_backward turns them into dL_dcolors / dL_dfeatures / dL_dsh (or the SH factors) for all views.
+int composite_bwd_row_floats(int S, bool geometry);
+int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, bool geometry, cudaStream_t stream);
 int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream);
+int launch_appearance_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
 
 // Camera gradients: the terms of one view in the order viewmatrix [16], projmatrix [16], campos [3].  The projection
 // backward writes one partial sum of them per CTA of kCamGradThreads Gaussians; launch_cam_grad_sum adds the partials

@@ -61,6 +61,62 @@ __device__ __forceinline__ void cov3d_plain(const float* s3, float mod, const fl
     c6[5] = M[2][0] * M[2][0] + M[2][1] * M[2][1] + M[2][2] * M[2][2];
 }
 
+// The SH basis (backward.cu:20-139) at the unit view direction (x, y, z) for degree D, and its derivatives; zero above
+// (D + 1)^2.  One definition for the projection backward and the appearance-only backward, so that both compute the
+// same dL/dsh bits.
+__device__ __forceinline__ void sh_basis(int D, float x, float y, float z, float (&w)[16], float (&wx)[16], float (&wy)[16],
+                                         float (&wz)[16]) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k) { w[k] = 0.f; wx[k] = 0.f; wy[k] = 0.f; wz[k] = 0.f; }
+    const float C1 = 0.4886025119029199f;
+    w[0] = 0.28209479177387814f;
+    if (D > 0) {
+        w[1] = -C1 * y; w[2] = C1 * z; w[3] = -C1 * x;
+        wy[1] = -C1; wz[2] = C1; wx[3] = -C1;
+        if (D > 1) {
+            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+            const float c20 = 1.0925484305920792f, c21 = -1.0925484305920792f, c22 = 0.31539156525252005f,
+                        c23 = -1.0925484305920792f, c24 = 0.5462742152960396f;
+            w[4] = c20 * xy; w[5] = c21 * yz; w[6] = c22 * (2.f * zz - xx - yy); w[7] = c23 * xz; w[8] = c24 * (xx - yy);
+            wx[4] = c20 * y;  wy[4] = c20 * x;
+            wy[5] = c21 * z;  wz[5] = c21 * y;
+            wx[6] = c22 * 2.f * -x; wy[6] = c22 * 2.f * -y; wz[6] = c22 * 2.f * 2.f * z;
+            wx[7] = c23 * z;  wz[7] = c23 * x;
+            wx[8] = c24 * 2.f * x; wy[8] = c24 * 2.f * -y;
+            if (D > 2) {
+                const float c30 = -0.5900435899266435f, c31 = 2.890611442640554f, c32 = -0.4570457994644658f,
+                            c33 = 0.3731763325901154f, c34 = -0.4570457994644658f, c35 = 1.445305721320277f,
+                            c36 = -0.5900435899266435f;
+                w[9] = c30 * y * (3.f * xx - yy); w[10] = c31 * xy * z; w[11] = c32 * y * (4.f * zz - xx - yy);
+                w[12] = c33 * z * (2.f * zz - 3.f * xx - 3.f * yy); w[13] = c34 * x * (4.f * zz - xx - yy);
+                w[14] = c35 * z * (xx - yy); w[15] = c36 * x * (xx - 3.f * yy);
+                wx[9] = c30 * 3.f * 2.f * xy;  wy[9] = c30 * 3.f * (xx - yy);
+                wx[10] = c31 * yz;             wy[10] = c31 * xz;            wz[10] = c31 * xy;
+                wx[11] = c32 * -2.f * xy;      wy[11] = c32 * (-3.f * yy + 4.f * zz - xx); wz[11] = c32 * 4.f * 2.f * yz;
+                wx[12] = c33 * -3.f * 2.f * xz; wy[12] = c33 * -3.f * 2.f * yz; wz[12] = c33 * 3.f * (2.f * zz - xx - yy);
+                wx[13] = c34 * (-3.f * xx + 4.f * zz - yy); wy[13] = c34 * -2.f * xy; wz[13] = c34 * 4.f * 2.f * xz;
+                wx[14] = c35 * 2.f * xz;       wy[14] = c35 * -2.f * yz;     wz[14] = c35 * (xx - yy);
+                wx[15] = c36 * 3.f * (xx - yy); wy[15] = c36 * -3.f * 2.f * xy;
+            }
+        }
+    }
+}
+
+// The view direction of a Gaussian (backward.cu:20-139): d = m - cam, its squares, |d|^2 and the unit vector (x, y, z).
+// |d|^2 is three rounded products and two rounded sums in this order — explicit, so that the compiler cannot contract
+// it differently in the projection backward (where the squares have other uses) and in the appearance-only backward:
+// both compute the same direction, and so the same dL/dsh bits.
+struct ViewDir { float dx, dy, dz, xx, yy, zz, sum2, x, y, z; };
+__device__ __forceinline__ ViewDir view_dir(const float* m, const float* cam) {
+    ViewDir d;
+    d.dx = m[0] - cam[0]; d.dy = m[1] - cam[1]; d.dz = m[2] - cam[2];
+    d.xx = __fmul_rn(d.dx, d.dx); d.yy = __fmul_rn(d.dy, d.dy); d.zz = __fmul_rn(d.dz, d.dz);
+    d.sum2 = __fadd_rn(__fadd_rn(d.xx, d.yy), d.zz);
+    const float len = sqrtf(d.sum2);
+    d.x = d.dx / len; d.y = d.dy / len; d.z = d.dz / len;
+    return d;
+}
+
 #define PROJ_THREADS 128
 #define SLAB_LD (PROJ_THREADS + 1)
 // DET (deterministic mode): the packed gradient row is read from the fixed-point accumulators and converted on load.
@@ -310,47 +366,13 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     if (live) {
         // ---- SH backward (backward.cu:20-139) -------------------------------------------------
         if (p.shs) {
-            const float dox = m3[0] - sCam[0], doy = m3[1] - sCam[1], doz = m3[2] - sCam[2];
-            const float len = sqrtf(dox * dox + doy * doy + doz * doz);
-            const float x = dox / len, y = doy / len, z = doz / len;
+            const ViewDir vd = view_dir(m3, sCam);
+            const float dox = vd.dx, doy = vd.dy, doz = vd.dz, x = vd.x, y = vd.y, z = vd.z;
             float* slab = sSH + threadIdx.x;                 // element (k, c) at slab[(3k + c) * SLAB_LD]
             const float dRGB[3] = {(cl & 1u) ? 0.f : dcol[0], (cl & 2u) ? 0.f : dcol[1], (cl & 4u) ? 0.f : dcol[2]};
             dfac[0] = dRGB[0]; dfac[1] = dRGB[1]; dfac[2] = dRGB[2];
             float w[16], wx[16], wy[16], wz[16];   // basis and its derivatives w.r.t. x,y,z
-#pragma unroll
-            for (int k = 0; k < 16; ++k) { w[k] = 0.f; wx[k] = 0.f; wy[k] = 0.f; wz[k] = 0.f; }
-            const float C1 = 0.4886025119029199f;
-            w[0] = 0.28209479177387814f;
-            if (p.D > 0) {
-                w[1] = -C1 * y; w[2] = C1 * z; w[3] = -C1 * x;
-                wy[1] = -C1; wz[2] = C1; wx[3] = -C1;
-                if (p.D > 1) {
-                    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                    const float c20 = 1.0925484305920792f, c21 = -1.0925484305920792f, c22 = 0.31539156525252005f,
-                                c23 = -1.0925484305920792f, c24 = 0.5462742152960396f;
-                    w[4] = c20 * xy; w[5] = c21 * yz; w[6] = c22 * (2.f * zz - xx - yy); w[7] = c23 * xz; w[8] = c24 * (xx - yy);
-                    wx[4] = c20 * y;  wy[4] = c20 * x;
-                    wy[5] = c21 * z;  wz[5] = c21 * y;
-                    wx[6] = c22 * 2.f * -x; wy[6] = c22 * 2.f * -y; wz[6] = c22 * 2.f * 2.f * z;
-                    wx[7] = c23 * z;  wz[7] = c23 * x;
-                    wx[8] = c24 * 2.f * x; wy[8] = c24 * 2.f * -y;
-                    if (p.D > 2) {
-                        const float c30 = -0.5900435899266435f, c31 = 2.890611442640554f, c32 = -0.4570457994644658f,
-                                    c33 = 0.3731763325901154f, c34 = -0.4570457994644658f, c35 = 1.445305721320277f,
-                                    c36 = -0.5900435899266435f;
-                        w[9] = c30 * y * (3.f * xx - yy); w[10] = c31 * xy * z; w[11] = c32 * y * (4.f * zz - xx - yy);
-                        w[12] = c33 * z * (2.f * zz - 3.f * xx - 3.f * yy); w[13] = c34 * x * (4.f * zz - xx - yy);
-                        w[14] = c35 * z * (xx - yy); w[15] = c36 * x * (xx - 3.f * yy);
-                        wx[9] = c30 * 3.f * 2.f * xy;  wy[9] = c30 * 3.f * (xx - yy);
-                        wx[10] = c31 * yz;             wy[10] = c31 * xz;            wz[10] = c31 * xy;
-                        wx[11] = c32 * -2.f * xy;      wy[11] = c32 * (-3.f * yy + 4.f * zz - xx); wz[11] = c32 * 4.f * 2.f * yz;
-                        wx[12] = c33 * -3.f * 2.f * xz; wy[12] = c33 * -3.f * 2.f * yz; wz[12] = c33 * 3.f * (2.f * zz - xx - yy);
-                        wx[13] = c34 * (-3.f * xx + 4.f * zz - yy); wy[13] = c34 * -2.f * xy; wz[13] = c34 * 4.f * 2.f * xz;
-                        wx[14] = c35 * 2.f * xz;       wy[14] = c35 * -2.f * yz;     wz[14] = c35 * (xx - yy);
-                        wx[15] = c36 * 3.f * (xx - yy); wy[15] = c36 * -3.f * 2.f * xy;
-                    }
-                }
-            }
+            sh_basis(p.D, x, y, z, w, wx, wy, wz);
             const int ncoef = (p.D + 1) * (p.D + 1);
             float ddx = 0.f, ddy = 0.f, ddz = 0.f;
             if (bulk) {
@@ -395,11 +417,11 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             }
             }
             // dnormvdv (auxiliary.h:105-116)
-            const float sum2 = dox * dox + doy * doy + doz * doz;
+            const float sum2 = vd.sum2;
             const float invsum32 = 1.0f / sqrtf(sum2 * sum2 * sum2);
-            const float ddir[3] = {(+sum2 - dox * dox) * ddx - doy * dox * ddy - doz * dox * ddz,
-                                   -dox * doy * ddx + (sum2 - doy * doy) * ddy - doz * doy * ddz,
-                                   -dox * doz * ddx - doy * doz * ddy + (sum2 - doz * doz) * ddz};
+            const float ddir[3] = {(+sum2 - vd.xx) * ddx - doy * dox * ddy - doz * dox * ddz,
+                                   -dox * doy * ddx + (sum2 - vd.yy) * ddy - doz * doy * ddz,
+                                   -dox * doz * ddx - doy * doz * ddy + (sum2 - vd.zz) * ddz};
             // explicit FMAs: the contraction of `dmean3 += ddir * invsum32` must not depend on whether the product
             // has a second use (CAM), so that dL/dmeans3D is the same with and without camera gradients
             dmean3[0] = __fmaf_rn(ddir[0], invsum32, dmean3[0]);
@@ -556,6 +578,137 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     else if (cam) projection_bwd_kernel<false, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
     else if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
     else projection_bwd_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// ---- appearance-only backward (r3dg_raster_backward with every geometry output NULL) ---------------------------------
+// The compositor (composite_bwd_kernel<GEOM = false>) left one row of nc = 4 * num_groups(S) channel gradients
+// {r, g, b, f0, ...} per view and Gaussian.  One thread per Gaussian walks the views in order and writes what
+// projection_bwd_kernel writes for the same outputs, with the same arithmetic: per-view rows, or the fp32 left fold over
+// the views of shared inputs (a row that is not live adds nothing to the earlier views'); with `shs`, the colour
+// gradient gated by the clamp flags becomes the SH factor, or (one view) the dense dL/dsh from the same basis.  Only
+// live rows read anything: their packed row, their clamp flags, their mean and the view's campos.
+struct AppBwdParams {
+    int P, S, D, M, V, nc;
+    const float *means3D, *campos;
+    const uint8_t* clamped;     // [V][P]: bits 0-2 SH colour clamped, kComposited
+    const float* grad;          // [V * P][nc]
+    DetAcc det;                 // DET: the same rows as fixed-point accumulators, read instead of grad
+    float *dL_dcolors, *dL_dfeatures, *dL_dsh, *dL_dsh_factor;   // each may be NULL (not requested)
+    bool sh, colors_per_view, features_per_view;
+};
+
+// The feature rows of the CTA's Gaussians are one contiguous range per view: the CTA writes it element by element
+// (coalesced), the rest is one thread per Gaussian.
+template <bool DET>
+__global__ void __launch_bounds__(128) appearance_bwd_kernel(const AppBwdParams p) {
+    auto load = [&](size_t row, int c) -> float {
+        if constexpr (DET) return det_load(p.det, row * p.nc + c);
+        else return p.grad[row * p.nc + c];
+    };
+    const int g0 = blockIdx.x * blockDim.x;
+    if (p.dL_dfeatures && p.S > 0) {
+        const int n = min((int)blockDim.x, p.P - g0) * p.S;
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+            const int gi = g0 + i / p.S, c = i - (i / p.S) * p.S;
+            for (int v = 0; v < p.V; ++v) {
+                const size_t r = (size_t)v * p.P + gi;
+                const bool live = (p.clamped[r] & kComposited) != 0, acc = v > 0 && !p.features_per_view;
+                if (live || !acc) put(p.dL_dfeatures + (p.features_per_view ? r : (size_t)gi) * p.S + c,
+                                      live ? load(r, 3 + c) : 0.0f, acc);
+            }
+        }
+    }
+    // the colour rows are read only for dL_dcolors, the SH factors or the dense dL/dsh (not in the stage-2 case, where
+    // only dL_dfeatures is requested)
+    if (!p.dL_dcolors && !(p.sh && (p.dL_dsh_factor || p.dL_dsh))) return;          // (grid-uniform)
+    // one view's dense dL/dsh: each thread fills its row of the CTA's slab s[k * SLAB_LD + t] (conflict-free), and the
+    // CTA writes the slab's contiguous range of dL_dsh with coalesced stores, as projection_bwd_kernel's write-back
+    extern __shared__ float sOut[];
+    const int g = g0 + threadIdx.x, rowf = 3 * p.M;
+    float m3[3] = {0.f, 0.f, 0.f};
+    bool have_m3 = false;
+    for (int v = 0; g < p.P && v < p.V; ++v) {
+        const size_t r = (size_t)v * p.P + g;
+        const unsigned cl = p.clamped[r];
+        const bool live = (cl & kComposited) != 0;
+        float dcol[3] = {0.f, 0.f, 0.f};
+        if (live) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) dcol[k] = load(r, k);
+        }
+        if (p.dL_dcolors) {
+            const bool acc = v > 0 && !p.colors_per_view;
+            if (live || !acc) {
+                float* dc = p.dL_dcolors + 3 * (p.colors_per_view ? r : (size_t)g);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) put(dc + k, dcol[k], acc);
+            }
+        }
+        if (!p.sh) continue;
+        const float dRGB[3] = {(cl & 1u) ? 0.f : dcol[0], (cl & 2u) ? 0.f : dcol[1], (cl & 4u) ? 0.f : dcol[2]};
+        if (p.dL_dsh_factor) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) p.dL_dsh_factor[3 * r + k] = live ? dRGB[k] : 0.f;
+        }
+        if (!p.dL_dsh) continue;                       // (one view only: several views rebuild it from the factors)
+        float w[16], wx[16], wy[16], wz[16];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) w[k] = 0.f;
+        if (live) {
+            if (!have_m3) {
+                m3[0] = p.means3D[3 * (size_t)g]; m3[1] = p.means3D[3 * (size_t)g + 1]; m3[2] = p.means3D[3 * (size_t)g + 2];
+                have_m3 = true;
+            }
+            const ViewDir vd = view_dir(m3, p.campos + 3 * v);
+            sh_basis(p.D, vd.x, vd.y, vd.z, w, wx, wy, wz);
+        }
+        const int ncoef = (p.D + 1) * (p.D + 1);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            if (k < p.M) {
+                const bool act = live && k < ncoef;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) sOut[(3 * k + c) * SLAB_LD + threadIdx.x] = act ? w[k] * dRGB[c] : 0.f;
+            }
+        }
+    }
+    if (!p.dL_dsh || !p.sh) return;                     // (grid-uniform)
+    __syncthreads();
+    const int total = min((int)blockDim.x, p.P - g0) * rowf;
+    float* dst = p.dL_dsh + (size_t)g0 * rowf;
+    if ((rowf & 3) == 0 && (reinterpret_cast<uintptr_t>(p.dL_dsh) & 15) == 0) {
+        float4* dst4 = reinterpret_cast<float4*>(dst);
+        for (int i4 = threadIdx.x; i4 < total / 4; i4 += blockDim.x) {
+            const int i = 4 * i4, t = i / rowf, k = i - t * rowf;
+            dst4[i4] = make_float4(sOut[(k + 0) * SLAB_LD + t], sOut[(k + 1) * SLAB_LD + t], sOut[(k + 2) * SLAB_LD + t],
+                                   sOut[(k + 3) * SLAB_LD + t]);
+        }
+    } else {
+        for (int i = threadIdx.x; i < total; i += blockDim.x) {
+            const int t = i / rowf, k = i - t * rowf;
+            dst[i] = sOut[k * SLAB_LD + t];
+        }
+    }
+}
+
+int launch_appearance_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream) {
+    AppBwdParams p;
+    p.P = a.P; p.S = a.S; p.D = a.D; p.M = a.M; p.V = b.V; p.nc = composite_bwd_row_floats(a.S, false);
+    p.means3D = a.means3D; p.campos = a.campos;
+    p.clamped = b.clamped; p.grad = b.grad;
+    p.det = det_acc(a.det_work, (size_t)b.V * a.P * p.nc);
+    p.dL_dcolors = a.dL_dcolors; p.dL_dfeatures = a.dL_dfeatures;
+    p.dL_dsh = b.V > 1 ? nullptr : a.dL_dsh;       // several views: from the factors afterwards (r3dg_raster_backward)
+    p.dL_dsh_factor = a.dL_dsh_factor;
+    p.sh = a.shs != nullptr;
+    p.colors_per_view = a.colors_per_view != 0; p.features_per_view = a.features_per_view != 0;
+    static_assert(PROJ_THREADS == 128, "the dL/dsh slab holds one CTA of 128 rows");
+    const int blocks = (a.P + 127) / 128;
+    const size_t smem = p.sh && p.dL_dsh ? (size_t)3 * a.M * SLAB_LD * sizeof(float) : 0;
+    if (a.deterministic) appearance_bwd_kernel<true><<<blocks, 128, smem, stream>>>(p);
+    else appearance_bwd_kernel<false><<<blocks, 128, smem, stream>>>(p);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

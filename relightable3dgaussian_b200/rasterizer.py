@@ -75,7 +75,9 @@ def set_grad_exchange(exchange, campos_all=None):
     skipping the SH leaves.  `campos_all` [world,3] holds the camera centres of the views the ranks
     render this step, in rank order (call again per step).  All ranks must take the same path:
     a backward that cannot use an installed exchange (debug mode, no `shs`) raises instead of silently
-    skipping its collectives.  `set_grad_exchange(None)` turns it off."""
+    skipping its collectives.  While an exchange is installed the backward is always the full one, even when no
+    geometry input requires grad (the appearance-only backward is not part of the exchange).
+    `set_grad_exchange(None)` turns it off."""
     global _EXCHANGE
     _EXCHANGE = None if exchange is None else (exchange, campos_all)
 
@@ -132,6 +134,21 @@ def _input_grads(ctx, grads, cameras):
             None, None) + cam
 
 
+# the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
+# scales, rotations, cov3Ds_precomp, viewmatrix, projmatrix, campos (features, sh and colors_precomp are appearance)
+_GEOMETRY_INPUTS = (0, 1, 5, 6, 7, 8, 11, 12, 13)
+
+
+def _backward_mode(ctx):
+    """Keyword arguments of the node's library backward: none (the full backward) when a geometry input needs a
+    gradient or a gradient exchange is installed (set_grad_exchange), otherwise the appearance-only backward for the
+    appearance inputs that need one.  Frozen geometry (means2D included) thus pays only for the gradients it uses."""
+    need = ctx.needs_input_grad
+    if _EXCHANGE is not None or any(need[i] for i in _GEOMETRY_INPUTS):
+        return {}
+    return {"geometry": False, "appearance": (need[2], need[4], need[3])}
+
+
 def _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
     """The positional arguments of _C.rasterize_gaussians for the settings `rs`."""
     return (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
@@ -181,10 +198,13 @@ class _RasterizeGaussians(torch.autograd.Function):
                 raise RuntimeError("a gradient exchange is installed (set_grad_exchange) but this backward cannot take "
                                    "part in it (debug mode or no `shs` input): every rank must run the same collectives")
             ex = _EXCHANGE
-        kw = {} if ex is None else {"_out": {"sh_factor": ex[0].factor}}
+        kw = _backward_mode(ctx)
+        if ex is not None:
+            kw["_out"] = {"sh_factor": ex[0].factor}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
             kw["cam_grads"] = True
-        surface = _surface_cotangents(ctx, g_normal, g_surface_xyz)
+        # (appearance-only: the surface outputs depend only on the geometry, their cotangents have nothing to reach)
+        surface = _surface_cotangents(ctx, g_normal, g_surface_xyz) if kw.get("geometry", True) else None
         if surface is not None:
             kw["surface"] = surface + (rs.cx, rs.cy)
         grads = _debug_call(rs.debug, _C.rasterize_gaussians_backward,
@@ -247,7 +267,12 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
     cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
     when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
-    ignored as in the reference."""
+    ignored as in the reference.
+
+    When no geometry input (means3D, means2D, opacities, scales, rotations, cov3Ds_precomp and the settings' viewmatrix,
+    projmatrix, campos) requires grad, the backward computes only the gradients of features, sh and colors_precomp
+    that are needed (frozen-geometry training; not part of the reference surface, which always runs the full
+    backward).  The cotangents of opacity, depth, normal and surface_xyz then reach nothing and are not read."""
     global _CALL_GRAD_MODE
     rs = raster_settings
     _refuse_surface_grads_without_normals(surface_grads, rs.computer_pseudo_normal)
@@ -308,11 +333,13 @@ class _RasterizeViews(torch.autograd.Function):
          geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors[:14]
         g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
                                                                    g_feature)
+        kw = _backward_mode(ctx)
+        if kw.get("geometry", True):
+            kw.update(cam_grads=any(ctx.needs_input_grad[11:14]), surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
                                             cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
                                             g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
-                                            rs.backward_geometry, cam_grads=any(ctx.needs_input_grad[11:14]),
-                                            surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
+                                            rs.backward_geometry, **kw)
         return _input_grads(ctx, grads, (viewmatrix, projmatrix, campos))
 
 
