@@ -113,13 +113,8 @@ __device__ __forceinline__ void load_material(const ShadeArgs& a, int g, Gaussia
 
 template <bool INC_REGS>
 __device__ __forceinline__ void load_operands(const ShadeArgs& a, int g, GaussianOperands& o) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) { o.base[c] = a.base_color[3 * (size_t)g + c]; o.n[c] = a.normals[3 * (size_t)g + c]; }
-    o.rough = a.roughness[g];
+    load_material(a, g, o);
     view_operands(o.n, a.viewdirs + 3 * (size_t)g, o.V, o.vnorm, o.Ns);
-    const float al = o.rough * o.rough;
-    o.a2 = al * al;
-    o.k = (al + 2.0f * o.rough + 1.0f) / 8.0f;
     if (INC_REGS) {
         const float4* ip = reinterpret_cast<const float4*>(a.incidents + 48 * (size_t)g);
 #pragma unroll
@@ -377,8 +372,6 @@ __device__ __forceinline__ void warp_private_add(float4* wg, volatile unsigned c
 
 // The env-gradient state of one backward CTA in its shared memory `s_mem`: the constructor stages the texture and
 // zeroes the accumulators of ENV_MODE, scatter() adds one sample's taps, flush() adds the CTA's total to dL/denv.
-// This, accumulate_dinc and ggx_backward serve the view kernels; shade_bwd_kernel keeps the same code inline, because
-// routing it through these helpers changes its machine code (equivalent predicates, other registers).
 template <int ENV_MODE>
 struct EnvGrad {
     static constexpr bool SMEM_ENV = ENV_MODE != ENV_GLOBAL && ENV_MODE != ENV_DET_GLOBAL;
@@ -391,16 +384,25 @@ struct EnvGrad {
     const float* env;                                // the texture the samples read (shared or global memory)
     float* genv;                                     // ENV_CAS / ENV_GLOBAL: where the taps are added
 
+    // bytes of `s_mem` the constructor lays out for an He x We texture (0 for the global-memory modes):
+    // ENV_CAS: [env ne][grad ne]; ENV_TAG: [env ne (padded to 4)][per warp: float4 grad[nt]][per warp: tag[nt] padded to 16];
+    // ENV_DET_SMEM: [env ne (padded to 2)][accumulator words 3 ne][flag words (ne + 15) / 16]
+    static __host__ __device__ size_t smem_bytes(int He, int We) {
+        const size_t nt = (size_t)He * We, ne = nt * 3;
+        if (ENV_MODE == ENV_CAS) return 2 * ne * sizeof(float);
+        if (ENV_MODE == ENV_TAG) return ((ne + 3) & ~(size_t)3) * sizeof(float) + SHADE_WARPS * (nt * sizeof(float4) + ((nt + 15) & ~(size_t)15));
+        if (ENV_MODE == ENV_DET_SMEM) return ((ne + 1) & ~(size_t)1) * sizeof(float) + 3 * ne * sizeof(uint64_t) + (ne + 15) / 16 * sizeof(uint32_t);
+        return 0;
+    }
+
     __device__ __forceinline__ EnvGrad(const ShadeArgs& a, float* s_mem, int warp) {
         nt = a.He * a.We; ne = nt * 3;
-        // ENV_CAS: [env ne][grad ne]; ENV_TAG: [env ne (padded to 4)][per warp: float4 grad[nt]][per warp: tag[nt] padded to 16]
         s_env = s_mem;
         s_genv = s_mem + ne;
         const int ne4 = (ne + 3) & ~3, ntp = (nt + 15) & ~15;
         wgrad_all = reinterpret_cast<float4*>(s_mem + ne4);
         wgrad = wgrad_all + (size_t)warp * nt;
         wtag = reinterpret_cast<unsigned char*>(wgrad_all + (size_t)SHADE_WARPS * nt) + (size_t)warp * ntp;
-        // ENV_DET_SMEM: [env ne (padded to 2)][accumulator words 3 ne][flag words (ne + 15) / 16]
         s_dwords = reinterpret_cast<uint64_t*>(s_mem + ((ne + 1) & ~1));
         s_dflags = reinterpret_cast<uint32_t*>(s_dwords + 3 * (size_t)ne);
         nflag = (ne + 15) >> 4;
@@ -525,40 +527,18 @@ __device__ __forceinline__ void ggx_backward(const float* V, const float* Ns, co
 template <int ENV_MODE, int G, int VAR>
 __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (ENV_MODE <= 1 ? 5 : 3)) shade_bwd_kernel(const ShadeArgs a) {
     extern __shared__ __align__(16) float s_bwd[];    // [incident slots (VAR >= 1)][gradient accumulators (VAR 2)][env ...]
-    constexpr bool SMEM_ENV = ENV_MODE != ENV_GLOBAL && ENV_MODE != ENV_DET_GLOBAL;
+    constexpr bool SMEM_ENV = EnvGrad<ENV_MODE>::SMEM_ENV;
     constexpr int GPW = 32 / G;
     constexpr int INC_FLOATS = VAR >= 1 ? SHADE_WARPS * GPW * SHADE_INC_STRIDE : 0;
     constexpr int DINC_FLOATS = VAR == 2 ? 48 * SHADE_THREADS : 0;
     float* s_mem = s_bwd + INC_FLOATS + DINC_FLOATS;
     float* sinc = s_bwd + ((threadIdx.x >> 5) * GPW + (threadIdx.x & 31) / G) * SHADE_INC_STRIDE;
+    float4* acc4 = reinterpret_cast<float4*>(s_bwd + INC_FLOATS) + threadIdx.x;    // VAR 2
     constexpr int VP = (48 + G - 1) / G * G;         // SH-gradient row padded to a multiple of G
     constexpr int RQ = VP / G;                       // finished components per lane
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane & (G - 1), grp = lane / G;
-    const int nt = a.He * a.We, ne = nt * 3;
-    // ENV_CAS: [env ne][grad ne]; ENV_TAG: [env ne (padded to 4)][per warp: float4 grad[nt]][per warp: tag[nt] padded to 16]
-    float* s_env = s_mem;
-    float* s_genv = s_mem + ne;
-    const int ne4 = (ne + 3) & ~3, ntp = (nt + 15) & ~15;
-    float4* wgrad_all = reinterpret_cast<float4*>(s_mem + ne4);
-    float4* wgrad = wgrad_all + (size_t)warp * nt;
-    volatile unsigned char* wtag = reinterpret_cast<unsigned char*>(wgrad_all + (size_t)SHADE_WARPS * nt) + (size_t)warp * ntp;
-    // ENV_DET_SMEM: [env ne (padded to 2)][accumulator words 3 ne][flag words (ne + 15) / 16]
-    uint64_t* s_dwords = reinterpret_cast<uint64_t*>(s_mem + ((ne + 1) & ~1));
-    uint32_t* s_dflags = reinterpret_cast<uint32_t*>(s_dwords + 3 * (size_t)ne);
-    const int nflag = (ne + 15) >> 4;
-    if (SMEM_ENV) {
-        for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_env[i] = a.env[i];
-        if (ENV_MODE == ENV_CAS) for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_genv[i] = 0.f;
-        if (ENV_MODE == ENV_TAG) for (int i = threadIdx.x; i < SHADE_WARPS * nt; i += SHADE_THREADS) wgrad_all[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (ENV_MODE == ENV_DET_SMEM) {
-            for (int i = threadIdx.x; i < 3 * ne; i += SHADE_THREADS) s_dwords[i] = 0u;
-            for (int i = threadIdx.x; i < nflag; i += SHADE_THREADS) s_dflags[i] = 0u;
-        }
-        __syncthreads();
-    }
-    const float* env = SMEM_ENV ? s_env : a.env;
-    float* genv = ENV_MODE == ENV_CAS ? s_genv : a.d_env;
+    EnvGrad<ENV_MODE> eg(a, s_mem, warp);
     const float invN = 1.0f / (float)a.N;
     const int units = (a.P + GPW - 1) / GPW;
     for (int u = blockIdx.x * SHADE_WARPS + warp; u < units; u += gridDim.x * SHADE_WARPS) {
@@ -580,7 +560,6 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
 #pragma unroll
         for (int q = 0; q < VP; ++q) dinc[q] = 0.f;
         if (VAR == 2) {
-            float4* acc4 = reinterpret_cast<float4*>(s_bwd + INC_FLOATS) + threadIdx.x;
 #pragma unroll
             for (int q = 0; q < 12; ++q) acc4[q * SHADE_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
@@ -591,7 +570,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
             const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
             const float vis = a.visibility[row + i], area = a.areas[row + i];
             SampleEval e;
-            eval_sample<SMEM_ENV, (VAR >= 1), true>(a, o, env, sinc, dx, dy, dz, vis, e);
+            eval_sample<SMEM_ENV, (VAR >= 1), true>(a, o, eg.env, sinc, dx, dy, dz, vis, e);
             float dfs = 0.f;
             float dG[3], dLg[3];
 #pragma unroll
@@ -609,74 +588,9 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
                 }
                 dG[c] = act ? dL * vis : 0.f;                        // -> env texels (grid_sample backward)
             }
-            if (VAR == 2) {
-                // dinc[3k + c] += dL[c] * w[k]: the lane's 48 accumulators as 12 float4 in shared memory ([12][threads]
-                // 16-byte slots: conflict-free 128-bit accesses) — 12 LDS.128 + 48 FFMA + 12 STS.128 per sample
-                float4* acc4 = reinterpret_cast<float4*>(s_bwd + INC_FLOATS) + threadIdx.x;
-#pragma unroll
-                for (int q = 0; q < 12; ++q) {
-                    float4 v = acc4[q * SHADE_THREADS];
-                    v.x = fmaf(dLg[(4 * q) % 3], e.w[(4 * q) / 3], v.x);
-                    v.y = fmaf(dLg[(4 * q + 1) % 3], e.w[(4 * q + 1) / 3], v.y);
-                    v.z = fmaf(dLg[(4 * q + 2) % 3], e.w[(4 * q + 2) / 3], v.z);
-                    v.w = fmaf(dLg[(4 * q + 3) % 3], e.w[(4 * q + 3) / 3], v.w);
-                    acc4[q * SHADE_THREADS] = v;
-                }
-            }
-            if (ENV_MODE == ENV_TAG) {
-                const bool any = dG[0] != 0.f || dG[1] != 0.f || dG[2] != 0.f;
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                    const int texel = (any && e.taps.idx[t] >= 0) ? e.taps.idx[t] / 3 : -1;
-                    warp_private_add(wgrad, wtag, texel, dG[0] * e.taps.w[t], dG[1] * e.taps.w[t], dG[2] * e.taps.w[t], lane);
-                }
-            } else if (ENV_MODE == ENV_DET_SMEM || ENV_MODE == ENV_DET_GLOBAL) {
-#pragma unroll
-                for (int c = 0; c < 3; ++c)
-                    if (dG[c] != 0.f) {
-#pragma unroll
-                        for (int t = 0; t < 4; ++t)
-                            if (e.taps.idx[t] >= 0) {
-                                if (ENV_MODE == ENV_DET_SMEM) det_add(s_dwords, s_dflags, ne, e.taps.idx[t] + c, dG[c] * e.taps.w[t], true);
-                                else det_add(a.det, e.taps.idx[t] + c, dG[c] * e.taps.w[t]);
-                            }
-                    }
-            } else {
-#pragma unroll
-                for (int c = 0; c < 3; ++c)
-                    if (dG[c] != 0.f) {
-#pragma unroll
-                        for (int t = 0; t < 4; ++t) if (e.taps.idx[t] >= 0) atomicAdd(genv + e.taps.idx[t] + c, dG[c] * e.taps.w[t]);
-                    }
-            }
-            if (act) {
-                // ---- GGX backward --------------------------------------------------------------
-                const float inom = fast_rcp(e.nom);
-                const float dfrac = dfs * inom;
-                const float dnom = -dfs * (e.frac0 * o.a2) * inom * inom;
-                const float dnom_r = (e.nom_r >= 1e-6f && e.nom_r <= 4.0f * PI_F) ? dnom : 0.f;
-                const float dnom0 = dnom_r * 8.0f * PI_F * e.nom0 * e.nom1 * e.nom2;
-                const float dnom1 = dnom_r * 4.0f * PI_F * e.nom0 * e.nom0 * e.nom2;
-                const float dnom2 = dnom_r * 4.0f * PI_F * e.nom0 * e.nom0 * e.nom1;
-                const float dfrac0 = dfrac * o.a2;
-                const float da2 = dfrac * e.frac0 + dnom0 * e.NoH * e.NoH;
-                const float dk = dnom1 * (1.0f - e.NoV) + dnom2 * (1.0f - e.NoL);
-                const float r = o.rough;
-                drough += da2 * 4.0f * r * r * r + dk * (2.0f * r + 2.0f) / 8.0f;
-                const float dNoH = (e.NoH_r >= 1e-6f && e.NoH_r <= 1.f) ? dnom0 * 2.0f * e.NoH * (o.a2 - 1.0f) : 0.f;
-                const float dNoV = (e.NoV_r >= 1e-6f && e.NoV_r <= 1.f) ? dnom1 * (1.0f - o.k) : 0.f;
-                const float dVoH = (e.VoH_r >= 1e-6f && e.VoH_r <= 1.f)
-                                       ? dfrac0 * (1.0f - 0.04f) * e.p2 * 0.693147180559945f * (2.0f * -5.55473f * e.VoH - 6.98316f) : 0.f;
-                float dH[3], hdot = 0.f;
-#pragma unroll
-                for (int c = 0; c < 3; ++c) { dH[c] = dNoH * o.Ns[c] + dVoH * o.V[c]; hdot += e.H[c] * dH[c]; }
-                const float ihn = fast_rcp(e.hn);
-#pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    const float dHraw = (dH[c] - e.H[c] * hdot) * ihn;
-                    dV[c] += dNoV * o.Ns[c] + dVoH * e.H[c] + 0.5f * dHraw;
-                }
-            }
+            if (VAR == 2) accumulate_dinc(acc4, dLg, e.w);
+            eg.scatter(a, e.taps, dG, lane);
+            if (act) ggx_backward(o.V, o.Ns, o, e, dfs, drough, dV);
         }
         __syncwarp();
         // ---- group reduction and per-Gaussian outputs ---------------------------------------------
@@ -684,7 +598,6 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
         for (int c = 0; c < 3; ++c) { dbase[c] = group_sum<G>(dbase[c]); dV[c] = group_sum<G>(dV[c]); }
         drough = group_sum<G>(drough);
         if (VAR == 2) {
-            const float4* acc4 = reinterpret_cast<const float4*>(s_bwd + INC_FLOATS) + threadIdx.x;
 #pragma unroll
             for (int q = 0; q < 12; ++q) { const float4 v = acc4[q * SHADE_THREADS]; dinc[4 * q] = v.x; dinc[4 * q + 1] = v.y; dinc[4 * q + 2] = v.z; dinc[4 * q + 3] = v.w; }
         }
@@ -711,29 +624,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
             }
         }
     }
-    if (ENV_MODE == ENV_CAS) {
-        __syncthreads();
-        for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) { const float v = s_genv[i]; if (v != 0.f) atomicAdd(a.d_env + i, v); }
-    }
-    if (ENV_MODE == ENV_TAG) {
-        __syncthreads();
-        for (int t = threadIdx.x; t < nt; t += SHADE_THREADS) {
-            float4 s = wgrad_all[t];
-#pragma unroll
-            for (int w = 1; w < SHADE_WARPS; ++w) { const float4 v = wgrad_all[(size_t)w * nt + t]; s.x += v.x; s.y += v.y; s.z += v.z; }
-            if (s.x != 0.f) atomicAdd(a.d_env + 3 * t, s.x);
-            if (s.y != 0.f) atomicAdd(a.d_env + 3 * t + 1, s.y);
-            if (s.z != 0.f) atomicAdd(a.d_env + 3 * t + 2, s.z);
-        }
-    }
-    if (ENV_MODE == ENV_DET_SMEM) {
-        __syncthreads();
-        for (int i = threadIdx.x; i < 3 * ne; i += SHADE_THREADS) {
-            const uint64_t v = s_dwords[i];
-            if (v) det_red_u64(a.det.words + (size_t)(i / ne) * a.det.n + (i % ne), v);
-        }
-        for (int i = threadIdx.x; i < nflag; i += SHADE_THREADS) { const uint32_t f = s_dflags[i]; if (f) atomicOr(a.det.flags + i, f); }
-    }
+    eg.flush(a);
 }
 
 // deterministic mode: dL/denv from its accumulators, every element written
@@ -1066,9 +957,6 @@ static int launch_bwd(const ShadeArgs& a, int num_sms, size_t env_smem, cudaStre
     return shade_launch(shade_bwd_kernel<MODE, 32, 0>, a, units, num_sms, smem, stream);
 }
 
-// shared memory of ENV_DET_SMEM (env, accumulator words, flag words); larger textures use ENV_DET_GLOBAL
-static size_t det_smem_bytes(size_t ne) { return ((ne + 1) & ~(size_t)1) * sizeof(float) + 3 * ne * 8 + (ne + 15) / 16 * 4; }
-
 template <int M> using EnvMode = std::integral_constant<int, M>;
 
 // Clears dL/denv (or the deterministic accumulators), picks the env-gradient mode from the texture size, the deterministic
@@ -1076,12 +964,11 @@ template <int M> using EnvMode = std::integral_constant<int, M>;
 // the deterministic mode then converts its accumulators into dL/denv.
 template <typename Run>
 static int shade_backward(ShadeArgs a, int cap, cudaStream_t stream, Run run) {
-    const size_t nt = (size_t)a.He * a.We, env_bytes = nt * 3 * sizeof(float);
     if (a.det.words) {
         R3DG_CUDA_TRY(cudaMemsetAsync(a.det.words, 0, det_bytes(a.det.n), stream));
         int rc = 0;
         if (a.P > 0) {
-            const size_t smem = det_smem_bytes(a.det.n);
+            const size_t smem = EnvGrad<ENV_DET_SMEM>::smem_bytes(a.He, a.We);     // larger textures use ENV_DET_GLOBAL
             a.env_in_smem = smem <= 64 * 1024;
             rc = a.env_in_smem ? run(EnvMode<ENV_DET_SMEM>(), a, smem) : run(EnvMode<ENV_DET_GLOBAL>(), a, 0);
         }
@@ -1090,11 +977,10 @@ static int shade_backward(ShadeArgs a, int cap, cudaStream_t stream, Run run) {
         R3DG_CUDA_TRY(cudaGetLastError());
         return 0;
     }
-    R3DG_CUDA_TRY(cudaMemsetAsync(a.d_env, 0, env_bytes, stream));
+    R3DG_CUDA_TRY(cudaMemsetAsync(a.d_env, 0, (size_t)a.He * a.We * 3 * sizeof(float), stream));
     if (a.P <= 0) return 0;
     // shared-memory cost of the env-gradient modes (kept within the 48 KB that need no opt-in on their own)
-    const size_t tag_bytes = ((nt * 3 + 3) & ~(size_t)3) * sizeof(float) + SHADE_WARPS * (nt * sizeof(float4) + ((nt + 15) & ~(size_t)15));
-    const size_t cas_bytes = 2 * env_bytes;
+    const size_t tag_bytes = EnvGrad<ENV_TAG>::smem_bytes(a.He, a.We), cas_bytes = EnvGrad<ENV_CAS>::smem_bytes(a.He, a.We);
     if (cap >= ENV_TAG && tag_bytes <= 48 * 1024) { a.env_in_smem = 1; return run(EnvMode<ENV_TAG>(), a, tag_bytes); }
     if (cap >= ENV_CAS && cas_bytes <= 40 * 1024) { a.env_in_smem = 1; return run(EnvMode<ENV_CAS>(), a, cas_bytes); }
     a.env_in_smem = 0;
