@@ -97,6 +97,13 @@ typedef struct r3dg_raster_fwd_args {
     int V;
     const float* view_cams;
     int features_per_view, colors_per_view;
+    /* Antialiased mode (the opacity-compensated screen-space filter of upstream 3DGS and gsplat).  Non-zero: with
+     * a0, b, c0 the 2D covariance before the fixed 0.3 px^2 dilation and a1 = a0 + 0.3, c1 = c0 + 0.3, every Gaussian's
+     * opacity is multiplied by rho = sqrt(max(r, 2.5e-5)), r = (a0 c0 - b^2) / (a1 c1 - b^2) (r = 0 when a0 c0 - b^2
+     * <= 0), so that the dilated Gaussian keeps the integrated weight of the undilated one.  The compensated opacity
+     * replaces the opacity in the record every compositor reads (and so in out_weights and the block pre-filter);
+     * the conic, radius, tile rectangle, depth key and colours are those of 0.  0 = the default path. */
+    int antialiasing;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_raster_fwd_det_bytes(P) bytes, zeroed by the call.  0 = the default path (det_work unused). */
@@ -208,6 +215,11 @@ typedef struct r3dg_raster_bwd_args {
     const float* fwd_depth;
     float cx, cy;
     void* surface_work; size_t surface_work_bytes;
+    /* Antialiased mode: must equal the matching forward's (zero or non-zero), like scale_modifier and the matrices;
+     * the backward reads the compensated opacity from the forward's record and differentiates rho too.  dL_dopacity is
+     * then rho times the gradient of the compensated opacity, and rho's dependence on the 2D covariance reaches
+     * dL_dcov3D, dL_dscales, dL_drotations, dL_dmeans3D and dL_dviewmatrix.  The appearance-only mode ignores it. */
+    int antialiasing;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_raster_bwd_det_bytes(P, S) bytes, zeroed by the call.  0 = the default path (det_work unused). */

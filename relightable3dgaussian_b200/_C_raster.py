@@ -128,12 +128,13 @@ def _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means
 
 def _forward(views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
              viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered, computer_pseudo_normal, debug,
-             capacity, pinned, defer):
+             capacity, pinned, defer, antialiasing=False):
     """The forward of the len(cams) views `cams` = [(tan_fovx, tan_fovy, cx, cy), ...]: one view (`views` False,
     outputs in the one-view shapes) or V views (outputs with a leading V).  Sizes the binning buffer for `capacity`
     instances and re-runs with room to spare while the counts, read back into the pinned int32 `pinned` (one per
     view), exceed it.  Returns the 12 outputs after num_rendered, the event recorded once the counts are copied, and the
-    counts as a list: None when `defer`, which returns after the first attempt without waiting."""
+    counts as a list: None when `defer`, which returns after the first attempt without waiting.  `antialiasing`: the
+    library's antialiased mode (see rasterize_gaussians)."""
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     dev = means3D.device
@@ -144,7 +145,7 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     a.opacities = _lib.ptr(opacity)
     a.cx, a.cy = float(cams[0][2]), float(cams[0][3])
     a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
-    a.debug = int(bool(debug))
+    a.debug = int(bool(debug)); a.antialiasing = int(bool(antialiasing))
 
     lead = (V,) if views else ()
     f32 = dict(dtype=torch.float32, device=dev)
@@ -198,10 +199,13 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
 def rasterize_gaussians(background, means3D, features, colors, opacity, scales, rotations,
                         scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                         cx, cy, image_height, image_width, sh, degree, campos, prefiltered,
-                        computer_pseudo_normal, debug, _defer=False, _min_capacity=None):
+                        computer_pseudo_normal, debug, _defer=False, _min_capacity=None, *, antialiasing=False):
     """== RasterizeGaussiansCUDA (rasterize_points.cu:36-141).  Returns the 13-tuple
     (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
-     out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer)."""
+     out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer).
+    `antialiasing=True` (not part of the reference surface) multiplies each Gaussian's opacity by
+    rho = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)), the opacity compensation of the fixed 0.3 px^2
+    dilation; the backward must then be called with the same flag."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")   # rasterize_points.cu:62-64
     P = means3D.size(0)
@@ -229,7 +233,8 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     pinned = st["pinned"][slot:slot + 1]
     out, ev, counts = _forward(False, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy, cx, cy)], H, W, sh, degree,
-                               campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer)
+                               campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer,
+                               antialiasing)
     if _defer:
         rendered = DeferredCount(ev, pinned, capacity, st, P)
         st["pending"] = rendered
@@ -242,14 +247,15 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
 def _backward(views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
-              surface_work, principal, geometry=True, appearance=(True, True, True)):
+              surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
     one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
     are those of rasterize_gaussians_backward (`surface` without the principal point).
     `geometry=False`: the appearance-only backward.  Nothing is allocated for the six geometry gradients, which come
     back None, and of dL_dfeatures, dL_dcolors, dL_dsh only those `appearance` = (features, colors, sh) asks for are
-    computed (the others are None too); the opacity, depth and surface cotangents are not read."""
+    computed (the others are None too); the opacity, depth and surface cotangents are not read.  `antialiasing` must
+    be the forward's."""
     if not geometry and (cam_grads or _out is not None):
         raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
@@ -309,6 +315,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     # (appearance-only with nothing to compute: no call, e.g. S = 0 features the only input that needs a gradient)
     if P != 0 and (geometry or any(_lib.ptr(t) for t in (dL_dfeatures, dL_dcolors, dL_dsh))):
         a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
+        a.antialiasing = int(bool(antialiasing))
         a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
         a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
         a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
@@ -336,7 +343,7 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  tan_fovy, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
                                  imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
-                                 surface_work=None, geometry=True, appearance=(True, True, True)):
+                                 surface_work=None, geometry=True, appearance=(True, True, True), *, antialiasing=False):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
@@ -347,13 +354,13 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards.
     `geometry=False` (not part of the reference surface either) is the appearance-only backward of _backward: the
     gradients of the geometry inputs, and of the appearance inputs `appearance` = (features, colors, sh) leaves out,
-    come back None."""
+    come back None.  `antialiasing` (not part of the reference surface) must be the forward's: rasterize_gaussians."""
     principal = surface[4:6] if surface is not None and len(surface) == 6 else None
     grads, cam = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
                            dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
                            binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
-                           surface and surface[:4], surface_work, principal, geometry, appearance)
+                           surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing)
     return grads + tuple(t[0] for t in cam)
 
 
@@ -427,12 +434,13 @@ _views_capacity = {}     # (device, P, W, H, V) -> binning capacity that held th
 
 def rasterize_views(background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                     viewmatrix, projmatrix, cams, image_height, image_width, sh, degree, campos, prefiltered,
-                    computer_pseudo_normal, _min_capacity=None):
+                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False):
     """V views of one set of Gaussians in one forward.  background [V,3], viewmatrix / projmatrix [V,4,4], campos [V,3],
     cams: V tuples (tan_fovx, tan_fovy, cx, cy); features [P,S] or [V,P,S], colors [P,3] or [V,P,3] (or empty).
     Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
     out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
-    radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once."""
+    radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once.
+    `antialiasing` applies to every view (see rasterize_gaussians)."""
     V, P = len(cams), means3D.size(0)
     H, W = int(image_height), int(image_width)
     dev = means3D.device
@@ -441,7 +449,7 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
     pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
     out, _, rendered = _forward(True, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                 cov3D_precomp, viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered,
-                                computer_pseudo_normal, False, capacity, pinned, False)
+                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing)
     _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
     return (rendered,) + out
 
@@ -450,7 +458,7 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
                              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                              backward_geometry, cam_grads=False, surface=None, surface_work=None, geometry=True,
-                             appearance=(True, True, True)):
+                             appearance=(True, True, True), *, antialiasing=False):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
@@ -459,10 +467,10 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth), all [V,*,H,W] (a cotangent may be None), and
     `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
     one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
-    rasterize_gaussians_backward."""
+    rasterize_gaussians_backward, and `antialiasing` must be the forward's."""
     grads, cam = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                            dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                            backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
-                           appearance)
+                           appearance, antialiasing)
     return grads + cam

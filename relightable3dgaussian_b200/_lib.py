@@ -31,7 +31,7 @@ class RasterFwdArgs(ctypes.Structure):
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
          ("binning", c_void_p), ("binning_bytes", c_size_t), ("num_rendered_host", c_void_p), ("count_ready_event", c_void_p),
          ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
-         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+         ("antialiasing", c_int), ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class RasterBwdArgs(ctypes.Structure):
@@ -53,7 +53,7 @@ class RasterBwdArgs(ctypes.Structure):
          ("cam_work", c_void_p), ("cam_work_bytes", c_size_t),
          ("dL_dout_normal", c_void_p), ("dL_dout_surface_xyz", c_void_p), ("fwd_opacity", c_void_p), ("fwd_depth", c_void_p),
          ("cx", c_float), ("cy", c_float), ("surface_work", c_void_p), ("surface_work_bytes", c_size_t),
-         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+         ("antialiasing", c_int), ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class ShadeArgs(ctypes.Structure):

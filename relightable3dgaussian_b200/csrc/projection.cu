@@ -133,7 +133,7 @@ struct ProjParams {
     const float *means3D, *shs, *colors_precomp, *features, *opacities, *scales, *rotations,
         *cov3D_precomp, *viewmatrix, *projmatrix, *campos;
     float scale_modifier, tan_fovx, tan_fovy, focal_x, focal_y;
-    int prefiltered;
+    int prefiltered, antialiasing;
     float* rec;
     uint32_t* tiles_touched;
     uint8_t* clamped;
@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
             }
         }
     }
-    float pix_x = 0.f, pix_y = 0.f, con_a = 0.f, con_b = 0.f, con_c = 0.f;
+    float pix_x = 0.f, pix_y = 0.f, con_a = 0.f, con_b = 0.f, con_c = 0.f, aa_rho = 1.f;
     int my_radius = 0, x0 = 0, y0 = 0, x1 = 0, y1 = 0;
     if (alive) {
         const float hx = xform_row_(sPr, 0, px, py, pz);
@@ -252,13 +252,19 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
         const float b0 = dot3_(T1[0], c6[0], T1[1], c6[1], T1[2], c6[2]);
         const float b1 = dot3_(T1[0], c6[1], T1[1], c6[3], T1[2], c6[4]);
         const float b2 = dot3_(T1[0], c6[2], T1[1], c6[4], T1[2], c6[5]);
-        const float cov_a = add_(dot3_(T0[0], a0, T0[1], a1, T0[2], a2), 0.3f);
-        const float cov_c = add_(dot3_(T1[0], b0, T1[1], b1, T1[2], b2), 0.3f);
+        const float cov_a0 = dot3_(T0[0], a0, T0[1], a1, T0[2], a2);
+        const float cov_c0 = dot3_(T1[0], b0, T1[1], b1, T1[2], b2);
+        const float cov_a = add_(cov_a0, 0.3f);
+        const float cov_c = add_(cov_c0, 0.3f);
         const float cov_b = dot3_(T0[0], b0, T0[1], b1, T0[2], b2);
         const float det = fma_(cov_a, cov_c, -mul_(cov_b, cov_b));
         if (det == 0.0f) {
             alive = false;
         } else {
+            if (p.antialiasing) {                      // (uniform) rho = sqrt(max(det0 / det, 2.5e-5)), r = 0 for det0 <= 0
+                const float det0 = fma_(cov_a0, cov_c0, -mul_(cov_b, cov_b));
+                aa_rho = sqrt_(fmaxf(det0 > 0.0f ? div_(det0, det) : 0.0f, 2.5e-5f));
+            }
             const float det_inv = rcp_(det);
             con_a = mul_(cov_c, det_inv); con_b = mul_(cov_b, -det_inv); con_c = mul_(cov_a, det_inv);
             const float mid = mul_(add_(cov_a, cov_c), 0.5f);
@@ -308,7 +314,8 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
     float4* srow = reinterpret_cast<float4*>(sSH) + (size_t)threadIdx.x * rec4n;
     __syncthreads();                                   // every thread is done with the SH slab
     if (alive) {
-        const float op = p.opacities[idx];
+        // antialiased mode: the compensated opacity o * rho is the opacity of everything downstream
+        const float op = p.antialiasing ? mul_(p.opacities[idx], aa_rho) : p.opacities[idx];
         p.brects[idx] = block_rect(pix_x, pix_y, con_a, con_b, con_c, op);
         srow[0] = make_float4(pix_x, pix_y, con_a, con_b);
         srow[1] = make_float4(con_c, op, tz, __int_as_float(my_radius));
@@ -469,7 +476,7 @@ int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, int
     p.scale_modifier = a.scale_modifier; p.tan_fovx = tan_fovx; p.tan_fovy = tan_fovy;
     p.focal_y = a.H / (2.0f * tan_fovy);              // rasterizer_impl.cu:232-233
     p.focal_x = a.W / (2.0f * tan_fovx);
-    p.prefiltered = a.prefiltered;
+    p.prefiltered = a.prefiltered; p.antialiasing = a.antialiasing;
     p.rec = b.rec; p.tiles_touched = b.tiles_touched;
     p.clamped = b.clamped; p.radii = a.radii + r; p.out_weights = a.out_weights + r;
     p.header = b.header;

@@ -19,6 +19,7 @@ struct ProjBwdParams {
     const float *means3D, *shs, *colors_precomp, *scales, *rotations, *cov3D_precomp, *viewmatrix,
         *projmatrix, *campos;
     float scale_modifier, tan_fovx, tan_fovy, h_x, h_y;
+    bool antialiasing;          // the record's opacity slot holds o rho (projection.cu): differentiate rho too
     const float* rec;
     const float* grad;
     const uint8_t* clamped;     // bits 0-2: SH colour clamped, kComposited: the row is live (read and differentiated)
@@ -164,8 +165,9 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     // the thread's own rows are requested before the cooperative slab load so that both are in flight together
     const float4* g4 = reinterpret_cast<const float4*>(p.grad + (size_t)idx * p.recf);
     float4 gA = make_float4(0, 0, 0, 0), gB = gA, gC = gA, q4 = gA;
-    float m3[3] = {0, 0, 0}, s3[3] = {0, 0, 0};
+    float m3[3] = {0, 0, 0}, s3[3] = {0, 0, 0}, aa_op = 0.f;
     if (live) {
+        if (p.antialiasing) aa_op = p.rec[(size_t)idx * p.recf + 5];   // the forward's compensated opacity o rho
         if constexpr (DET) {
             const size_t r0 = (p.det_row0 + idx) * p.recf;
             gA = make_float4(det_load(p.det, r0), det_load(p.det, r0 + 1), det_load(p.det, r0 + 2), det_load(p.det, r0 + 3));
@@ -254,16 +256,31 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             VT0[r] = Vrk[r][0] * T0[0] + Vrk[r][1] * T0[1] + Vrk[r][2] * T0[2];
             VT1[r] = Vrk[r][0] * T1[0] + Vrk[r][1] * T1[1] + Vrk[r][2] * T1[2];
         }
-        const float a = (T0[0] * VT0[0] + T0[1] * VT0[1] + T0[2] * VT0[2]) + 0.3f;
+        const float a0 = T0[0] * VT0[0] + T0[1] * VT0[1] + T0[2] * VT0[2];
+        const float c0 = T1[0] * VT1[0] + T1[1] * VT1[1] + T1[2] * VT1[2];
+        const float a = a0 + 0.3f;
         const float b = T1[0] * VT0[0] + T1[1] * VT0[1] + T1[2] * VT0[2];
-        const float c = (T1[0] * VT1[0] + T1[1] * VT1[1] + T1[2] * VT1[2]) + 0.3f;
+        const float c = c0 + 0.3f;
         const float denom = a * c - b * b;
+        // antialiased mode: r = det0 / det1 (0 for det0 <= 0) of the forward's rho = sqrt(max(r, 2.5e-5)); the record
+        // holds o rho and dop = dL/d(o rho)
+        float aa_r = 0.f;
+        if (p.antialiasing) {
+            const float det0 = a0 * c0 - b * b;
+            aa_r = det0 > 0.f ? det0 / denom : 0.f;
+        }
         float dL_da = 0, dL_db = 0, dL_dc = 0;
         const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
         if (denom2inv != 0) {
             dL_da = denom2inv * (-c * c * dcx + 2 * b * c * dcy + (denom - a * c) * dcz);
             dL_dc = denom2inv * (-a * a * dcz + 2 * a * b * dcy + (denom - a * c) * dcx);
             dL_db = denom2inv * 2 * (b * c * dcx - (denom + 2 * b * b) * dcy + a * b * dcz);
+            if (p.antialiasing && aa_r > 2.5e-5f) {     // (uniform) rho's path: dL/dr = dL/d(o rho) (o rho) / (2 r)
+                const float inv1 = 1.0f / denom, gr = dop * aa_op / (2.0f * aa_r) * (inv1 * inv1);
+                dL_da = __fadd_rn(dL_da, gr * (0.3f * (c0 * c + b * b)));
+                dL_dc = __fadd_rn(dL_dc, gr * (0.3f * (a0 * a + b * b)));
+                dL_db = __fadd_rn(dL_db, gr * (-2.0f * b * (0.3f * (a0 + c0) + 0.09f)));
+            }
             dcov[0] = (T0[0] * T0[0] * dL_da + T0[0] * T1[0] * dL_db + T1[0] * T1[0] * dL_dc);
             dcov[3] = (T0[1] * T0[1] * dL_da + T0[1] * T1[1] * dL_db + T1[1] * T1[1] * dL_dc);
             dcov[5] = (T0[2] * T0[2] * dL_da + T0[2] * T1[2] * dL_db + T1[2] * T1[2] * dL_dc);
@@ -271,6 +288,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             dcov[2] = 2 * T0[0] * T0[2] * dL_da + (T0[0] * T1[2] + T0[2] * T1[0]) * dL_db + 2 * T1[0] * T1[2] * dL_dc;
             dcov[4] = 2 * T0[2] * T0[1] * dL_da + (T0[1] * T1[2] + T0[2] * T1[1]) * dL_db + 2 * T1[1] * T1[2] * dL_dc;
         }
+        if (p.antialiasing) dop = __fmul_rn(dop, sqrtf(fmaxf(aa_r, 2.5e-5f)));   // dL/do = rho dL/d(o rho)
         float dT0[3], dT1[3];
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
@@ -553,6 +571,7 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     p.projmatrix = a.projmatrix + 16 * v; p.campos = a.campos + 3 * v;
     p.scale_modifier = a.scale_modifier; p.tan_fovx = tan_fovx; p.tan_fovy = tan_fovy;
     p.h_y = a.H / (2.0f * tan_fovy); p.h_x = a.W / (2.0f * tan_fovx);
+    p.antialiasing = a.antialiasing != 0;
     p.rec = b.rec; p.grad = b.grad; p.clamped = b.clamped;
     p.dL_dmeans2D = a.dL_dmeans2D + 3 * r; p.dL_dopacity = a.dL_dopacity;
     p.dL_dcolors = a.colors_per_view ? a.dL_dcolors + 3 * r : a.dL_dcolors;

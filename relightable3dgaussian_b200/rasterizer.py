@@ -84,10 +84,10 @@ def set_grad_exchange(exchange, campos_all=None):
 
 def _debug_call(debug, fn, args, dump, message, **kw):
     """fn(*args, **kw).  In debug mode, as in the reference, a CPU snapshot of `args` taken before the call is saved to
-    `dump` if it raises."""
+    `dump` if it raises, followed by the keyword arguments `kw` (e.g. `antialiasing`) as one dict."""
     if not debug:
         return fn(*args, **kw)
-    saved = tuple(a.cpu().clone() if isinstance(a, torch.Tensor) else a for a in args)
+    saved = tuple(a.cpu().clone() if isinstance(a, torch.Tensor) else a for a in args) + (dict(kw),)
     try:
         return fn(*args, **kw)
     except Exception:
@@ -124,14 +124,14 @@ def _surface_cotangents(ctx, g_normal, g_surface_xyz):
 
 def _input_grads(ctx, grads, cameras):
     """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
-    last three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
-    one, and for all three when none was computed."""
+    three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
+    one, and for all three when none was computed.  The last input, the antialiasing flag, gets None."""
     g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
     cam = (None, None, None)
     if grads[9:]:
-        cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[-3:]))
+        cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[11:14]))
     return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
-            None, None) + cam
+            None, None) + cam + (None,)
 
 
 # the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
@@ -147,6 +147,12 @@ def _backward_mode(ctx):
     if _EXCHANGE is not None or any(need[i] for i in _GEOMETRY_INPUTS):
         return {}
     return {"geometry": False, "appearance": (need[2], need[4], need[3])}
+
+
+def _aa_kw(antialiasing):
+    """The keyword that turns on the library's antialiased mode, only when it is on: an off call is the call without
+    the mode."""
+    return {"antialiasing": True} if antialiasing else {}
 
 
 def _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
@@ -165,14 +171,16 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos):
+                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing):
         rs = raster_settings
         out = _debug_call(rs.debug, _C.rasterize_gaussians,
                           _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
                                         cov3Ds_precomp),
                           "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
-                          _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad))
+                          _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad),
+                          **_aa_kw(antialiasing))
         ctx.raster_settings = rs
+        ctx.antialiasing = antialiasing
         ctx.num_rendered = out[0]
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
                       out[9], sh, *out[10:13], opacities)
@@ -199,6 +207,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                                    "part in it (debug mode or no `shs` input): every rank must run the same collectives")
             ex = _EXCHANGE
         kw = _backward_mode(ctx)
+        kw.update(_aa_kw(ctx.antialiasing))
         if ex is not None:
             kw["_out"] = {"sh_factor": ex[0].factor}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
@@ -217,7 +226,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                               "forward re-run inside backward (cotangents come from the truncated first attempt)")
                 out = _C.rasterize_gaussians(*_forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales,
                                                             rotations, cov3Ds_precomp),
-                                             _min_capacity=int(ctx.num_rendered) + 4096)
+                                             _min_capacity=int(ctx.num_rendered) + 4096, **_aa_kw(ctx.antialiasing))
                 if surface is not None:         # the adjoint of the re-run's own surface pass
                     kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
                 grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
@@ -263,7 +272,7 @@ def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, feat
 
 
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
-                        rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False):
+                        rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False, antialiasing=False):
     """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
     cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
     when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
@@ -272,7 +281,14 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     When no geometry input (means3D, means2D, opacities, scales, rotations, cov3Ds_precomp and the settings' viewmatrix,
     projmatrix, campos) requires grad, the backward computes only the gradients of features, sh and colors_precomp
     that are needed (frozen-geometry training; not part of the reference surface, which always runs the full
-    backward).  The cotangents of opacity, depth, normal and surface_xyz then reach nothing and are not read."""
+    backward).  The cotangents of opacity, depth, normal and surface_xyz then reach nothing and are not read.
+
+    With `antialiasing=True` (not part of the reference surface) each Gaussian's opacity is multiplied by
+    rho = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)) before compositing, so that the fixed 0.3 px^2 screen-space
+    dilation keeps the Gaussian's integrated weight instead of spreading a sub-pixel Gaussian over a pixel at full
+    opacity: a model trained with it renders consistently at other resolutions and distances.  The gradients include
+    rho's dependence on the 2D covariance and so reach means3D, scales, rotations, cov3Ds_precomp and the view matrix.
+    Radii, tile lists and colours are those of the default mode; the images, weights and counts differ."""
     global _CALL_GRAD_MODE
     rs = raster_settings
     _refuse_surface_grads_without_normals(surface_grads, rs.computer_pseudo_normal)
@@ -280,15 +296,16 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     _CALL_GRAD_MODE = torch.is_grad_enabled()
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
                                      scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
-                                     rs.viewmatrix, rs.projmatrix, rs.campos)
+                                     rs.viewmatrix, rs.projmatrix, rs.campos, bool(antialiasing))
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, surface_grads=False):
-        """`surface_grads` (not part of the reference surface): see rasterize_gaussians."""
+    def __init__(self, raster_settings, surface_grads=False, antialiasing=False):
+        """`surface_grads` and `antialiasing` (not part of the reference surface): see rasterize_gaussians."""
         super().__init__()
         self.raster_settings = raster_settings
         self.surface_grads = surface_grads
+        self.antialiasing = antialiasing
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -301,7 +318,7 @@ class GaussianRasterizer(nn.Module):
             means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features)
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
                                    scales, rotations, cov3D_precomp, self.raster_settings,
-                                   surface_grads=self.surface_grads)
+                                   surface_grads=self.surface_grads, antialiasing=self.antialiasing)
 
 
 _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
@@ -313,14 +330,14 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, surface_grads, viewmatrix, projmatrix, campos):
+                settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
         out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
-                                 rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal)
-        ctx.meta = (rs, cams)
+                                 rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing))
+        ctx.meta = (rs, cams, antialiasing)
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
                       bg, viewmatrix, projmatrix, campos, *out[10:13])
         return out[:10]
@@ -328,7 +345,7 @@ class _RasterizeViews(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature, g_normal, g_surface_xyz,
                  g_weights, g_radii):
-        rs, cams = ctx.meta
+        rs, cams, antialiasing = ctx.meta
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
          geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors[:14]
         g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
@@ -339,12 +356,12 @@ class _RasterizeViews(torch.autograd.Function):
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
                                             cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
                                             g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
-                                            rs.backward_geometry, **kw)
+                                            rs.backward_geometry, **_aa_kw(antialiasing), **kw)
         return _input_grads(ctx, grads, (viewmatrix, projmatrix, campos))
 
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
-                    rotations=None, cov3D_precomp=None, features=None, surface_grads=False):
+                    rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False):
     """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
 
     `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
@@ -357,7 +374,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
     Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
-    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads` is that of rasterize_gaussians, per view."""
+    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads` and `antialiasing` are those of rasterize_gaussians and
+    apply to every view."""
     settings = list(settings)
     V = len(settings)
     if V < 1:
@@ -389,7 +407,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     projmatrix = torch.stack([s.projmatrix for s in settings])
     campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
-                                 cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos)
+                                 cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos,
+                                 bool(antialiasing))
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
