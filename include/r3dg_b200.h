@@ -536,22 +536,32 @@ int r3dg_render_equation_backward(const r3dg_shade_args* args, r3dg_stream_t str
  * per-Gaussian gradient rows of the backward (hence all nine rasterizer gradients) and dL_denv of the
  * shading backward.  Results are then bitwise reproducible for the same inputs on the same device,
  * whatever the scheduling (r3dg_tune knobs included).  Everything else these calls compute is already
- * order-independent and unchanged.  Each term is rounded to a multiple of 2^-48 (|term| < 2^47;
- * larger finite terms saturate to +-Inf, NaN / +-Inf propagate as in IEEE addition); each total is
- * rounded to fp32 once.  out_weights is exact (integer units of 2^-24 per pixel).
+ * order-independent and unchanged.  The fixed point is anchored to each call's cotangent scale: a
+ * device reduction (no host sync) takes the largest |cotangent| m that a class of sums is linear in,
+ * e = floor(log2 m) (0 for zero, NaN or Inf; |e| <= 100), and each term is rounded to a multiple of
+ * 2^(e-48) (|term| < 2^(e+47); larger finite terms saturate to +-Inf, NaN / +-Inf propagate as in IEEE
+ * addition); each total is rounded to fp32 once.  The classes: per view, the colour and feature slots
+ * of the rasterizer's gradient rows (colour and feature cotangents) and their geometry slots (every
+ * cotangent plane the compositor reads); per shading call, dL_denv (dL_dpbr, dL_ddiffuse_light,
+ * dL_dspecular).  So the results are bitwise equivariant under power-of-two scaling of the cotangents,
+ * and their resolution is relative to that scale, as fine at a training loss's ~2^-21 per-pixel
+ * cotangents as at unit ones.  out_weights is exact (integer units of 2^-24 per pixel).
  * The workspace is the caller's, separate from `geom` (default memory use is unchanged); missing or
  * too small a workspace returns R3DG_ERR_BAD_ARG before anything is launched.
  *   r3dg_raster_fwd_det_bytes : 8 B per Gaussian;
  *   r3dg_raster_bwd_det_bytes : ~24 B per gradient-row float (8 + 4 ceil((3 + S) / 4) floats per
- *                               Gaussian): 384 MB at P = 1M, S = 5;
- *   r3dg_shade_det_bytes      : ~24 B per env-texel channel.
- * r3dg_det_sum_host: the accumulation primitive's host build (tests): *out = the sum of the n
- * host floats `terms` as the deterministic mode computes it.
+ *                               Gaussian): 384 MB at P = 1M, S = 5 (the per-view scale words use
+ *                               the float gradient scratch of `geom`, unused in this mode);
+ *   r3dg_shade_det_bytes      : ~24 B per env-texel channel + 256 B.
+ * r3dg_det_sum_scaled_host: the accumulation primitive's host build (tests): *out = the sum of the n
+ * host floats `terms` as the deterministic mode computes it for a class whose largest |cotangent| is
+ * |anchor|.  r3dg_det_sum_host: the same with anchor 0 (e = 0).
  * ------------------------------------------------------------------------------------------ */
 size_t r3dg_raster_fwd_det_bytes(int P);
 size_t r3dg_raster_bwd_det_bytes(int P, int S);
 size_t r3dg_shade_det_bytes(int env_h, int env_w);
 int r3dg_det_sum_host(long long n, const float* terms, float* out);
+int r3dg_det_sum_scaled_host(long long n, const float* terms, float anchor, float* out);
 
 /* Replaces `simple_knn._C.distCUDA2` (submodules/simple-knn/spatial.cu:15-26, simple_knn.cu:185-221):
  * mean_dist2[i] = mean of the 3 smallest squared distances from point i to the other points.

@@ -149,6 +149,7 @@ SYMBOLS = [
     ("r3dg_raster_bwd_det_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_shade_det_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_det_sum_host", c_int, [c_ll, c_void_p, c_void_p]),
+    ("r3dg_det_sum_scaled_host", c_int, [c_ll, c_void_p, c_float, c_void_p]),
     ("r3dg_knn_tmp_bytes", c_size_t, [c_int]),
     ("r3dg_knn_dist2", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("r3dg_ssim_tmp_bytes", c_size_t, [c_int, c_int, c_int, c_int]),

@@ -181,17 +181,19 @@ size_t r3dg_raster_surface_grad_bytes(int W, int H, int V) {
     return align_up(2 * v * hw * sizeof(float), 256) + align_up(v * 9 * surface_grad_blocks(W, H) * sizeof(float), 256);
 }
 
-int r3dg_det_sum_host(long long n, const float* terms, float* out) {
+int r3dg_det_sum_scaled_host(long long n, const float* terms, float anchor, float* out) {
     if (n < 0 || (n > 0 && !terms) || !out) return R3DG_ERR_BAD_ARG;
+    const int e = det_scale_exp(det_f32_bits(anchor) & 0x7fffffffu);
     uint64_t lo = 0, mid = 0, hi = 0;
     uint32_t flag = 0;
     for (long long i = 0; i < n; ++i) {
-        const DetTerm t = det_term(terms[i]);
+        const DetTerm t = det_term(terms[i], e);
         lo += t.lo; mid += t.mid; hi += t.hi; flag |= t.flag;
     }
-    *out = det_value(lo, mid, hi, flag);
+    *out = det_value(lo, mid, hi, flag, e);
     return 0;
 }
+int r3dg_det_sum_host(long long n, const float* terms, float* out) { return r3dg_det_sum_scaled_host(n, terms, 0.0f, out); }
 
 int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -323,7 +325,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (surface_cam &&              // then the pseudo-normal's term of dL/dviewmatrix, added after the projection's
         (rc = launch_surface_cam_sum(surface_part, surface_blocks, V, a->dL_dviewmatrix, stream)) != 0) return rc;
     prof_mark(false, 10, stream);
-    // zeroing of the composited rows, CTA order, composite, projection per view (appearance-only: one launch), camera
+    // zeroing of the composited rows (deterministic mode: and the cotangent scale), CTA order, composite, projection per view (appearance-only: one launch), camera
     // sums (the SH rebuild counts itself); surface pass per view and its camera sums
     g_launches += 3 + (geometry ? V : 1) + (cam ? 1 : 0) + (surface ? V : 0) + (surface_cam ? 1 : 0);
     if (g_prof.on) g_prof.bwd_calls++;

@@ -19,6 +19,7 @@
 //    float[24] arrays in local memory and 36 KB of shared memory per CTA;
 //  * gradients differ from the reference only by fp32 summation order (the reference's own
 //    atomics make it run-to-run nondeterministic), tolerance 1e-3 relative.
+#include <algorithm>
 #include <cstring>
 #include "common.cuh"
 #include "detacc.cuh"
@@ -44,6 +45,7 @@ struct CompositeBwdParams {
     const float *dL_dpix, *dL_dpix_o, *dL_dpix_d, *dL_dpix_f;
     float* grad;     // [P][recf], the composited rows zero-initialised (zero_composited_rows_kernel)
     DetAcc det;      // DET: the same rows as fixed-point accumulators (detacc.cuh), [P * recf], as grad
+    const uint32_t* det_scale;   // DET: per view, the scale words of its colour / feature and geometry slots (det_scale_reduce)
 };
 
 // Sum v[i] over the 32 lanes for every i in [0,N) (N power of two, 4 <= N <= 32) with a
@@ -141,7 +143,8 @@ __device__ __forceinline__ void reduce_scatter_permuted_multi(float (&x)[U][W], 
 // circular queue (warp scan) and processes batches of 32 of them: every staged entry is one that some pixel of the
 // block composited in the forward pass — no culling test, no record fetch and no exp() for anything else.
 // DET (deterministic mode): each finished row component is added through the order-independent fixed-point primitive
-// (detacc.cuh) into p.det instead of by a float atomic into p.grad.  Everything else is the same code.
+// (detacc.cuh) into p.det instead of by a float atomic into p.grad, scaled by its view's exponent of the colour /
+// feature slots or of the geometry slots (det_scale_reduce).  Everything else is the same code.
 // GEOM = false (appearance-only backward, no geometry gradient requested): the same walk, CTA order and alpha / T
 // arithmetic, but only the NC colour and feature components are formed and reduced — no dL/dalpha, no A recurrence, no
 // geometry butterfly — into a narrower row of NC floats (channel c at slot c).  Every channel component goes through the
@@ -234,6 +237,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     const float bg_dot = GEOM ? bg[0] * dpix[0] + bg[1] * dpix[1] + bg[2] * dpix[2] : 0.0f;
     const float ddelx_dx = 0.5f * p.W, ddely_dy = 0.5f * p.H;
     const bool geo = p.backward_geometry != 0;
+    int e_app = 0, e_geo = 0;
+    if constexpr (DET) { e_app = det_scale_exp(p.det_scale[2 * view]); e_geo = det_scale_exp(p.det_scale[2 * view + 1]); }
     // The reference keeps, per channel, the colour accumulated BEHIND the current entry (accum_rec[ch], backward.cu:
     // 541-566) only to form  dL_dalpha = sum_ch (c_ch - accum_rec[ch]) * dL_dpix[ch].  With D = sum_ch c_ch * dL_dpix[ch]
     // (the entry's own channels, depth and opacity terms included) the same quantity is  D - A  where the ONE scalar
@@ -418,9 +423,9 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                     if constexpr (DET) {
                         const size_t row = sId[warp][ju[u]];
                         if constexpr (C4_SECOND) {
-                            if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) det_add(p.det, row + 8 + B4 + (lane >> 3), t4[u]);
+                            if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) det_add(p.det, row + 8 + B4 + (lane >> 3), t4[u], e_app);
                         }
-                        if (my_sel >= 0) det_add(p.det, row + my_off, mine[u]);
+                        if (my_sel >= 0) det_add(p.det, row + my_off, mine[u], my_sel == 0 ? e_geo : e_app);
                     } else {
                         float* grow = p.grad + sId[warp][ju[u]];
                         if constexpr (C4_SECOND) {
@@ -434,14 +439,55 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     }
 }
 
+// DET: the largest |cotangent| of each of the V views as float bits, combined by atomicMax (exact, order-independent)
+// into the zeroed scale words: scale[2 v] over the colour and feature planes, the cotangents of the colour / feature
+// slots (dcc * dL_dpix); scale[2 v + 1] over those and the opacity and depth planes (the surface pull-back already
+// added), every plane the geometry slots are linear in.  GEOM = false reads only the former.  The compositor and the
+// kernels that read its rows take the class exponents from these words (det_scale_exp): a V-view call scales each
+// view as its one-view call does.  Every thread of the first `nblocks` blocks calls it (256 threads each): one
+// atomicMax per block and word.
+__device__ void det_scale_reduce(const CompositeBwdParams& p, int V, bool geometry, int nblocks, uint32_t* __restrict__ scale) {
+    __shared__ uint32_t s_max[2][8];
+    const size_t HW = (size_t)p.H * p.W, n_app = (size_t)(3 + p.S) * HW, n = n_app + (geometry ? 2 * HW : 0);
+    const size_t stride = (size_t)nblocks * blockDim.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int v = 0; v < V; ++v) {
+        const float* col = p.dL_dpix + (size_t)v * 3 * HW;
+        const float* feat = p.dL_dpix_f + (size_t)v * p.S * HW;
+        uint32_t m_app = 0u, m_geo = 0u;
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+            if (i < 3 * HW) m_app = max(m_app, det_abs_bits(col[i]));
+            else if (i < n_app) m_app = max(m_app, det_abs_bits(feat[i - 3 * HW]));
+            else if (i < n_app + HW) m_geo = max(m_geo, det_abs_bits(p.dL_dpix_o[(size_t)v * HW + (i - n_app)]));
+            else m_geo = max(m_geo, det_abs_bits(p.dL_dpix_d[(size_t)v * HW + (i - n_app - HW)]));
+        }
+        m_geo = max(m_app, m_geo);
+        m_app = __reduce_max_sync(0xffffffffu, m_app);
+        m_geo = __reduce_max_sync(0xffffffffu, m_geo);
+        if (lane == 0) { s_max[0][warp] = m_app; s_max[1][warp] = m_geo; }
+        __syncthreads();
+        if (warp == 0) {
+            const uint32_t a = lane < 8 ? s_max[0][lane] : 0u, g = lane < 8 ? s_max[1][lane] : 0u;
+            det_max_bits(scale + 2 * v, a);
+            det_max_bits(scale + 2 * v + 1, g);
+        }
+        __syncthreads();
+    }
+}
+
 // Zeroes the gradient rows the kernel above adds to: exactly the rows the forward pass composited (kComposited), since
 // it walks only their contributor bits.  Every other row is neither written nor read in the backward, so ~80 % of the
 // rows of a dense scene are never touched.  One thread per row.  DET: the row's accumulators in the three word planes
-// and its flag bits, which are recf / 4 whole bytes (2 bits per accumulator, recf a multiple of 4).
+// and its flag bits, which are recf / 4 whole bytes (2 bits per accumulator, recf a multiple of 4); and, before that,
+// the views' cotangent scale (det_scale_reduce) into the scale words the caller zeroed.
 template <bool DET>
 __global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, int recf, const uint8_t* __restrict__ clamped,
-                                                                   float* __restrict__ grad, const DetAcc det) {
+                                                                   float* __restrict__ grad, const DetAcc det,
+                                                                   const CompositeBwdParams p, int V, bool geometry, int nred) {
     const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr (DET) {
+        if ((int)blockIdx.x < nred) det_scale_reduce(p, V, geometry, nred, const_cast<uint32_t*>(p.det_scale));   // (block-uniform)
+    }
     if (r >= rows || !(clamped[r] & kComposited)) return;
     if constexpr (DET) {
 #pragma unroll 1
@@ -455,6 +501,10 @@ __global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, 
         float4* g = reinterpret_cast<float4*>(grad + r * recf);
         for (int i = 0; i < recf / 4; ++i) g[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
+}
+
+uint32_t* raster_det_scale(const RasterBuffers& b) {
+    return reinterpret_cast<uint32_t*>(b.grad - (size_t)b.row_base * b.recf);     // the whole call's grad region
 }
 
 // resident CTAs per SM the register allocation is pinned to, by channel groups NG (the occupancy sweep in DESIGN.md §4.2)
@@ -500,10 +550,16 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     const size_t rows = (size_t)V * a.P;
     const int gradf = composite_bwd_row_floats(a.S, geometry);     // the gradient row: b.recf, or NC without geometry
     p.det = det_acc(a.det_work, rows * gradf);
+    p.det_scale = det ? raster_det_scale(b) : nullptr;
     // zeroed here, in the backward, so that every backward over one forward (retain_graph) starts from zero
     const int zblocks = (int)((rows + 255) / 256);
-    if (det) zero_composited_rows_kernel<true><<<zblocks, 256, 0, stream>>>(rows, gradf, b.clamped, p.grad, p.det);
-    else zero_composited_rows_kernel<false><<<zblocks, 256, 0, stream>>>(rows, gradf, b.clamped, p.grad, p.det);
+    if (det) {
+        R3DG_CUDA_TRY(cudaMemsetAsync(const_cast<uint32_t*>(p.det_scale), 0, 2 * (size_t)V * sizeof(uint32_t), stream));
+        const int nred = std::min(zblocks, 4 * num_sms());          // the blocks that also reduce the cotangent scale
+        zero_composited_rows_kernel<true><<<zblocks, 256, 0, stream>>>(rows, gradf, b.clamped, p.grad, p.det, p, V, geometry, nred);
+    } else {
+        zero_composited_rows_kernel<false><<<zblocks, 256, 0, stream>>>(rows, gradf, b.clamped, p.grad, p.det, p, V, geometry, 0);
+    }
     const int tiles = V * b.tiles;                    // the tall grid of all views
     int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;

@@ -79,6 +79,11 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
 // launch_appearance_backward turns them into dL_dcolors / dL_dfeatures / dL_dsh (or the SH factors) for all views.
 int composite_bwd_row_floats(int S, bool geometry);
 int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, bool geometry, cudaStream_t stream);
+// deterministic mode: the 2 V scale words of the compositor's rows (per view: colour / feature slots, geometry slots).
+// They sit at the start of the float gradient rows' scratch region of `geom` (the call's, also for a view slice `b`),
+// which the deterministic backward otherwise neither writes nor reads: its rows live in the det workspace.  That
+// region holds V * P * recf >= 8 V floats.
+uint32_t* raster_det_scale(const RasterBuffers& b);
 int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream);
 int launch_appearance_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
 

@@ -28,6 +28,7 @@ struct ProjBwdParams {
     float* dL_dsh_factor;       // [P,3] gated dL_dRGB (multi-GPU exchange, sh_exchange.cu); dL_dsh may then be NULL
     DetAcc det;                 // DET: the gradient rows as fixed-point accumulators (composite_bwd.cu), read instead of grad
     size_t det_row0;            // DET: the view's first row in `det` (several views: v * P)
+    const uint32_t* det_scale;  // DET: the view's scale words of the colour / feature and geometry slots (composite_bwd.cu)
     // several views, views after the first: add this view's gradient to what the earlier views wrote (fp32, view order)
     // instead of writing it — acc for the gradients summed over the views, acc_colors / acc_features for dL_dcolors /
     // dL_dfeatures when those inputs are shared (per-view inputs get per-view rows: no accumulation)
@@ -170,9 +171,10 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
         if (p.antialiasing) aa_op = p.rec[(size_t)idx * p.recf + 5];   // the forward's compensated opacity o rho
         if constexpr (DET) {
             const size_t r0 = (p.det_row0 + idx) * p.recf;
-            gA = make_float4(det_load(p.det, r0), det_load(p.det, r0 + 1), det_load(p.det, r0 + 2), det_load(p.det, r0 + 3));
-            gB = make_float4(det_load(p.det, r0 + 4), det_load(p.det, r0 + 5), det_load(p.det, r0 + 6), 0.0f);
-            gC = make_float4(det_load(p.det, r0 + 8), det_load(p.det, r0 + 9), det_load(p.det, r0 + 10), 0.0f);
+            const int eg = det_scale_exp(p.det_scale[1]), ea = det_scale_exp(p.det_scale[0]);
+            gA = make_float4(det_load(p.det, r0, eg), det_load(p.det, r0 + 1, eg), det_load(p.det, r0 + 2, eg), det_load(p.det, r0 + 3, eg));
+            gB = make_float4(det_load(p.det, r0 + 4, eg), det_load(p.det, r0 + 5, eg), det_load(p.det, r0 + 6, eg), 0.0f);
+            gC = make_float4(det_load(p.det, r0 + 8, ea), det_load(p.det, r0 + 9, ea), det_load(p.det, r0 + 10, ea), 0.0f);
         } else {
             gA = g4[0]; gB = g4[1]; gC = g4[2];
         }
@@ -210,7 +212,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     if (p.S > 0 && in_range && (live || !p.acc_features)) {
         float* df = p.dL_dfeatures + (size_t)idx * p.S;
         for (int c = 0; c < p.S; ++c) {
-            if constexpr (DET) put(df + c, live ? det_load(p.det, (p.det_row0 + idx) * p.recf + 11 + c) : 0.0f, p.acc_features);
+            if constexpr (DET) put(df + c, live ? det_load(p.det, (p.det_row0 + idx) * p.recf + 11 + c, det_scale_exp(p.det_scale[0])) : 0.0f, p.acc_features);
             else put(df + c, live ? p.grad[(size_t)idx * p.recf + 11 + c] : 0.0f, p.acc_features);
         }
     }
@@ -583,6 +585,7 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     p.dL_dsh_factor = a.dL_dsh_factor ? a.dL_dsh_factor + 3 * r : nullptr;
     p.det = det_acc(a.det_work, (size_t)b.V * a.P * b.recf);
     p.det_row0 = r;
+    p.det_scale = a.deterministic ? raster_det_scale(b) + 2 * v : nullptr;
     p.acc = later;
     p.acc_colors = later && !a.colors_per_view;
     p.acc_features = later && !a.features_per_view;
@@ -614,6 +617,7 @@ struct AppBwdParams {
     const uint8_t* clamped;     // [V][P]: bits 0-2 SH colour clamped, kComposited
     const float* grad;          // [V * P][nc]
     DetAcc det;                 // DET: the same rows as fixed-point accumulators, read instead of grad
+    const uint32_t* det_scale;  // DET: per view, the scale word of the rows (composite_bwd.cu; [2 v], colour / feature)
     float *dL_dcolors, *dL_dfeatures, *dL_dsh, *dL_dsh_factor;   // each may be NULL (not requested)
     bool sh, colors_per_view, features_per_view;
 };
@@ -623,7 +627,7 @@ struct AppBwdParams {
 template <bool DET>
 __global__ void __launch_bounds__(128) appearance_bwd_kernel(const AppBwdParams p) {
     auto load = [&](size_t row, int c) -> float {
-        if constexpr (DET) return det_load(p.det, row * p.nc + c);
+        if constexpr (DET) return det_load(p.det, row * p.nc + c, det_scale_exp(p.det_scale[2 * (row / p.P)]));
         else return p.grad[row * p.nc + c];
     };
     const int g0 = blockIdx.x * blockDim.x;
@@ -718,6 +722,7 @@ int launch_appearance_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     p.means3D = a.means3D; p.campos = a.campos;
     p.clamped = b.clamped; p.grad = b.grad;
     p.det = det_acc(a.det_work, (size_t)b.V * a.P * p.nc);
+    p.det_scale = a.deterministic ? raster_det_scale(b) : nullptr;
     p.dL_dcolors = a.dL_dcolors; p.dL_dfeatures = a.dL_dfeatures;
     p.dL_dsh = b.V > 1 ? nullptr : a.dL_dsh;       // several views: from the factors afterwards (r3dg_raster_backward)
     p.dL_dsh_factor = a.dL_dsh_factor;

@@ -18,6 +18,7 @@
 //    grid_sample's scatter-add of P*N*4 taps — is accumulated in warp-private shared-memory copies
 //    without atomics (see "environment-map gradient" below), summed and flushed once per CTA;
 //  * the backward recomputes the forward per sample instead of saving [P,N,*] activations.
+#include <algorithm>
 #include <cstring>
 #include <type_traits>
 #include "common.cuh"
@@ -41,6 +42,7 @@ struct ShadeArgs {
     const float *g_pbr, *g_diffuse, *g_specular;
     float *d_base, *d_rough, *d_view, *d_incidents, *d_env;
     DetAcc det;                                  // deterministic mode: dL/denv accumulators [He * We * 3] (detacc.cuh)
+    uint32_t* det_scale;                         // deterministic mode: the call's scale word, behind the accumulators
 };
 
 __device__ __forceinline__ void sh_basis3(float x, float y, float z, float* w) {
@@ -352,6 +354,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? 6 : 1) shade_fwd_ker
 // The deterministic mode accumulates every tap through the fixed-point primitive (detacc.cuh): ENV_DET_SMEM into
 // per-CTA integer accumulators in shared memory whose words are added to the global ones once per CTA (integer sums,
 // so the flush order does not matter either), ENV_DET_GLOBAL straight into the global accumulators (larger textures).
+// Every tap is linear in the call's cotangents dL_dpbr, dL_ddiffuse_light and dL_dspecular; its fixed point is scaled
+// by the exponent of their largest magnitude (det_scale_kernel), one exponent per call.
 enum { ENV_GLOBAL = 0, ENV_CAS = 1, ENV_TAG = 2, ENV_DET_SMEM = 3, ENV_DET_GLOBAL = 4 };
 
 __device__ __forceinline__ void warp_private_add(float4* wg, volatile unsigned char* tag, int texel, float x, float y, float z, int lane) {
@@ -375,7 +379,7 @@ __device__ __forceinline__ void warp_private_add(float4* wg, volatile unsigned c
 template <int ENV_MODE>
 struct EnvGrad {
     static constexpr bool SMEM_ENV = ENV_MODE != ENV_GLOBAL && ENV_MODE != ENV_DET_GLOBAL;
-    int nt, ne, nflag;
+    int nt, ne, nflag, det_e;
     float *s_env, *s_genv;
     float4 *wgrad_all, *wgrad;
     volatile unsigned char* wtag;
@@ -406,6 +410,7 @@ struct EnvGrad {
         s_dwords = reinterpret_cast<uint64_t*>(s_mem + ((ne + 1) & ~1));
         s_dflags = reinterpret_cast<uint32_t*>(s_dwords + 3 * (size_t)ne);
         nflag = (ne + 15) >> 4;
+        det_e = ENV_MODE == ENV_DET_SMEM || ENV_MODE == ENV_DET_GLOBAL ? det_scale_exp(*a.det_scale) : 0;
         if (SMEM_ENV) {
             for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_env[i] = a.env[i];
             if (ENV_MODE == ENV_CAS) for (int i = threadIdx.x; i < ne; i += SHADE_THREADS) s_genv[i] = 0.f;
@@ -436,8 +441,8 @@ struct EnvGrad {
 #pragma unroll
                     for (int t = 0; t < 4; ++t)
                         if (taps.idx[t] >= 0) {
-                            if (ENV_MODE == ENV_DET_SMEM) det_add(s_dwords, s_dflags, ne, taps.idx[t] + c, dG[c] * taps.w[t], true);
-                            else det_add(a.det, taps.idx[t] + c, dG[c] * taps.w[t]);
+                            if (ENV_MODE == ENV_DET_SMEM) det_add(s_dwords, s_dflags, ne, taps.idx[t] + c, dG[c] * taps.w[t], det_e, true);
+                            else det_add(a.det, taps.idx[t] + c, dG[c] * taps.w[t], det_e);
                         }
                 }
         } else {
@@ -627,10 +632,23 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
     eg.flush(a);
 }
 
+// deterministic mode: the largest |cotangent| of the call over dL_dpbr, dL_ddiffuse_light and dL_dspecular (n floats
+// each, NULL skipped) as float bits into *scale (zeroed), by atomicMax: exact and order-independent
+__global__ void __launch_bounds__(256) det_scale_kernel(size_t n, const float* __restrict__ g0, const float* __restrict__ g1,
+                                                        const float* __restrict__ g2, uint32_t* __restrict__ scale) {
+    uint32_t m = 0u;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        m = max(m, det_abs_bits(g0[i]));
+        if (g1) m = max(m, det_abs_bits(g1[i]));
+        if (g2) m = max(m, det_abs_bits(g2[i]));
+    }
+    det_max_bits(scale, m);
+}
+
 // deterministic mode: dL/denv from its accumulators, every element written
-__global__ void __launch_bounds__(256) det_env_kernel(const DetAcc acc, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) det_env_kernel(const DetAcc acc, const uint32_t* __restrict__ scale, float* __restrict__ out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < acc.n) out[i] = det_load(acc, i);
+    if (i < acc.n) out[i] = det_load(acc, i, det_scale_exp(*scale));
 }
 
 // ---- several views per call ----------------------------------------------------------------------
@@ -961,19 +979,23 @@ template <int M> using EnvMode = std::integral_constant<int, M>;
 
 // Clears dL/denv (or the deterministic accumulators), picks the env-gradient mode from the texture size, the deterministic
 // flag and the highest mode allowed (`cap`), and calls run(EnvMode<mode>, args, env shared-memory bytes) unless P = 0;
-// the deterministic mode then converts its accumulators into dL/denv.
+// the deterministic mode first reduces the scale of the V views' cotangents and then converts its accumulators into
+// dL/denv.
 template <typename Run>
-static int shade_backward(ShadeArgs a, int cap, cudaStream_t stream, Run run) {
+static int shade_backward(ShadeArgs a, int V, int cap, int num_sms, cudaStream_t stream, Run run) {
     if (a.det.words) {
-        R3DG_CUDA_TRY(cudaMemsetAsync(a.det.words, 0, det_bytes(a.det.n), stream));
+        R3DG_CUDA_TRY(cudaMemsetAsync(a.det.words, 0, det_bytes(a.det.n) + sizeof(uint32_t), stream));   // + the scale word
         int rc = 0;
         if (a.P > 0) {
+            const size_t n = (size_t)(V < 1 ? 1 : V) * a.P * 3;
+            const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)4 * num_sms);
+            det_scale_kernel<<<blocks, 256, 0, stream>>>(n, a.g_pbr, a.g_diffuse, a.g_specular, a.det_scale);
             const size_t smem = EnvGrad<ENV_DET_SMEM>::smem_bytes(a.He, a.We);     // larger textures use ENV_DET_GLOBAL
             a.env_in_smem = smem <= 64 * 1024;
             rc = a.env_in_smem ? run(EnvMode<ENV_DET_SMEM>(), a, smem) : run(EnvMode<ENV_DET_GLOBAL>(), a, 0);
         }
         if (rc) return rc;
-        det_env_kernel<<<(unsigned)((a.det.n + 255) / 256), 256, 0, stream>>>(a.det, a.d_env);
+        det_env_kernel<<<(unsigned)((a.det.n + 255) / 256), 256, 0, stream>>>(a.det, a.det_scale, a.d_env);
         R3DG_CUDA_TRY(cudaGetLastError());
         return 0;
     }
@@ -988,7 +1010,7 @@ static int shade_backward(ShadeArgs a, int cap, cudaStream_t stream, Run run) {
 }
 
 int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
-    return shade_backward(a, knob(1), stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
+    return shade_backward(a, 1, knob(1), num_sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
         return launch_bwd<decltype(mode)::value>(x, num_sms, env_smem, stream);
     });
 }
@@ -1016,7 +1038,7 @@ int launch_shade_views_forward(ShadeArgs a, int V, int per_view_transform, int n
 
 // the env-gradient mode as the one-view backward picks it at its default highest mode (the view kernels have no knobs)
 int launch_shade_views_backward(ShadeArgs a, int V, int num_sms, cudaStream_t stream) {
-    return shade_backward(a, ENV_CAS, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
+    return shade_backward(a, V, ENV_CAS, num_sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
         constexpr int M = decltype(mode)::value;
         if constexpr (M == ENV_TAG) return (int)R3DG_ERR_UNSUPPORTED;     // above the cap: never selected
         else {
@@ -1054,6 +1076,7 @@ static int fill_args(const r3dg_shade_args* s, ShadeArgs& a) {
     a.d_base = s->dL_dbase_color; a.d_rough = s->dL_droughness; a.d_view = s->dL_dviewdirs; a.d_incidents = s->dL_dincidents;
     a.d_env = s->dL_denv;
     a.det = DetAcc{nullptr, nullptr, 0};
+    a.det_scale = nullptr;
     return 0;
 }
 
@@ -1080,15 +1103,17 @@ int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream
     if (s->V > 1 && s->transform_per_view && a.transform) return R3DG_ERR_UNSUPPORTED;    // forward only
     if (s->deterministic) {
         const size_t n = (size_t)a.He * a.We * 3;
-        if (!s->det_work || s->det_work_bytes < det_bytes(n)) return R3DG_ERR_BAD_ARG;
+        if (!s->det_work || s->det_work_bytes < r3dg_shade_det_bytes(a.He, a.We)) return R3DG_ERR_BAD_ARG;
         a.det = det_acc(s->det_work, n);
+        a.det_scale = (uint32_t*)((char*)s->det_work + det_bytes(n));
     }
     return s->V > 1 ? launch_shade_views_backward(a, s->V, num_sms(), (cudaStream_t)stream)
                     : launch_shade_backward(a, num_sms(), (cudaStream_t)stream);
 }
 
+// the accumulators and the call's scale word
 size_t r3dg_shade_det_bytes(int env_h, int env_w) {
-    return env_h > 0 && env_w > 0 ? det_bytes((size_t)env_h * env_w * 3) : 0;
+    return env_h > 0 && env_w > 0 ? det_bytes((size_t)env_h * env_w * 3) + 256 : 0;
 }
 
 }  // extern "C"

@@ -126,6 +126,55 @@ def test_non_finite_and_out_of_range_terms(terms, want):
     assert (np.isnan(det_sum(pad)) and np.isnan(want)) or det_sum(pad) == want
 
 
+def det_sum_scaled(terms, anchor):
+    a = np.ascontiguousarray(np.asarray(terms, dtype=np.float32))
+    out = ctypes.c_float(0.0)
+    assert _lib.load().r3dg_det_sum_scaled_host(a.size, a.ctypes.data if a.size else None, float(anchor),
+                                                ctypes.byref(out)) == 0
+    return np.float32(out.value)
+
+
+def test_scaled_sum_is_the_unit_sum_scaled_by_the_anchor_exponent():
+    """Anchored at |anchor| in [2^e, 2^(e+1)), a sum is the unit-anchored sum of the terms times 2^-e, times 2^e, bit for
+    bit: resolution and range follow the anchor's scale.  So scaling terms and anchor by 2^-k scales the result by 2^-k
+    exactly, at the training-loss scales (k = 21, 30) where a fixed 2^-48 unit rounds faint terms away."""
+    rng = np.random.default_rng(4)
+    for seed in range(4):
+        r = np.random.default_rng(seed)
+        cot = np.float32(r.uniform(1.0, 2.0))                        # the class's largest |cotangent|, in [1, 2)
+        terms = (r.choice([-1.0, 1.0], 400) * 10.0 ** r.uniform(-18, 1, 400)).astype(np.float32)
+        unit = det_sum_scaled(terms, cot)
+        assert unit.view(np.uint32) == det_sum(terms).view(np.uint32)          # e = 0: the unit-scale primitive
+        for k in (1, 8, 21, 30, 60, -20):
+            s = np.float32(2.0 ** -k)
+            got = det_sum_scaled(terms * s, cot * s)
+            assert got.view(np.uint32) == (unit * s).view(np.uint32), (seed, k)
+            check_permutations(list(terms * s), rng, 20)
+    # a term 2^-30 below the anchor keeps its 18 bits above the unit at any scale; a fixed 2^-48 unit would round
+    # 2^-30 * 2^-21 (a training-scale term) to zero
+    t = np.float32(1.0 + 2.0 ** -10) * np.float32(2.0 ** -51)
+    assert det_sum([t]) == 0.0
+    assert det_sum_scaled([t], 2.0 ** -21) == t                    # exact: 11 significant bits of the 18 kept
+
+
+@pytest.mark.parametrize("anchor", [0.0, -0.0, np.inf, -np.inf, np.nan, 1e-45, 1.5])
+def test_zero_subnormal_or_non_finite_anchor_means_unit_scale(anchor):
+    terms = np.array([0.5, -2.0 ** -40, 3.0, 2.0 ** -49 * 3], np.float32)
+    assert det_sum_scaled(terms, anchor).view(np.uint32) == det_sum(terms).view(np.uint32)
+
+
+def test_scaled_range_and_non_finite_terms():
+    """Range |term| < 2^(e+47): beyond it a finite term saturates to +-Inf; NaN and Inf terms propagate as unscaled."""
+    assert det_sum_scaled([2.0 ** 56, 1.0], 2.0 ** 10) == np.float32(2.0 ** 56 + 1.0)
+    assert det_sum_scaled([2.0 ** 57], 2.0 ** 9) == np.inf
+    assert det_sum_scaled([-2.0 ** 37], 2.0 ** -10) == -np.inf
+    assert np.isnan(det_sum_scaled([np.inf, -np.inf], 2.0 ** -20))
+    assert det_sum_scaled([np.inf, 1.0], 2.0 ** 20) == np.inf
+    # the exponent is clamped to |e| <= 100: far below, the unit is 2^-148, resolution still relative to 2^-100
+    tiny = np.float32(2.0 ** -120)
+    assert det_sum_scaled([tiny, tiny], 2.0 ** -125) == np.float32(2.0 ** -119)
+
+
 def test_bad_arguments():
     lib = _lib.load()
     out = ctypes.c_float(0)
@@ -133,6 +182,8 @@ def test_bad_arguments():
     assert lib.r3dg_det_sum_host(3, None, ctypes.byref(out)) == -10001
     assert lib.r3dg_det_sum_host(0, None, None) == -10001
     assert lib.r3dg_det_sum_host(0, None, ctypes.byref(out)) == 0 and out.value == 0.0
+    assert lib.r3dg_det_sum_scaled_host(-1, None, 1.0, ctypes.byref(out)) == -10001
+    assert lib.r3dg_det_sum_scaled_host(0, None, 1.0, None) == -10001
 
 
 def test_workspace_sizes():
@@ -143,7 +194,7 @@ def test_workspace_sizes():
         n = lib.r3dg_raster_bwd_det_bytes(P, S)
         assert 24 * P * rec(S) <= n <= 24 * P * rec(S) + P * rec(S) // 4 + 1024 and n % 256 == 0
     assert 350e6 < lib.r3dg_raster_bwd_det_bytes(1_000_000, 5) < 420e6          # "a few hundred MB" at the headline
-    assert lib.r3dg_shade_det_bytes(16, 32) >= 24 * 16 * 32 * 3
+    assert 24 * 16 * 32 * 3 < lib.r3dg_shade_det_bytes(16, 32) <= 24 * 16 * 32 * 3 + 1024
     assert lib.r3dg_shade_det_bytes(0, 32) == 0
 
 
