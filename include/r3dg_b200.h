@@ -215,6 +215,15 @@ typedef struct r3dg_raster_bwd_args {
     const float* fwd_depth;
     float cx, cy;
     void* surface_work; size_t surface_work_bytes;
+    /* Absolute screen-space gradients (absgrad, AbsGS / gsplat's absgrad=True; optional, NULL = none, the default):
+     * [P,2] ([V,P,2] for V views), next to dL_dmeans2D and in its units (0.5 W and 0.5 H per pixel): per Gaussian and
+     * view, sum over pixels of |dL/dmean2D.x| and of |dL/dmean2D.y|, each pixel's term taken before the pixel sum, so
+     * that pixels pulling a Gaussian in opposite directions do not cancel.  +0 for rows no pixel composited; every
+     * element is written.  It includes the pseudo-normal / surface-xyz pull-back and the antialiased mode's
+     * compensated opacity as dL_dmeans2D does.  The appearance-only mode ignores it.  In deterministic mode det_work
+     * must then hold r3dg_raster_bwd_det_bytes(V * P, S) + r3dg_raster_bwd_det_absgrad_bytes(V * P) bytes (too small
+     * returns R3DG_ERR_BAD_ARG before any launch); the sums are fixed-point sums of the geometry class. */
+    float* dL_dmeans2D_abs;
     /* Antialiased mode: must equal the matching forward's (zero or non-zero), like scale_modifier and the matrices;
      * the backward reads the compensated opacity from the forward's record and differentiates rho too.  dL_dopacity is
      * then rho times the gradient of the compensated opacity, and rho's dependence on the 2D covariance reaches
@@ -559,6 +568,9 @@ int r3dg_render_equation_backward(const r3dg_shade_args* args, r3dg_stream_t str
  * ------------------------------------------------------------------------------------------ */
 size_t r3dg_raster_fwd_det_bytes(int P);
 size_t r3dg_raster_bwd_det_bytes(int P, int S);
+/* The deterministic workspace a backward with dL_dmeans2D_abs needs on top of r3dg_raster_bwd_det_bytes: ~48 B per
+ * row (two accumulators), 48 MB at P = 1M. */
+size_t r3dg_raster_bwd_det_absgrad_bytes(int P);
 size_t r3dg_shade_det_bytes(int env_h, int env_w);
 int r3dg_det_sum_host(long long n, const float* terms, float* out);
 int r3dg_det_sum_scaled_host(long long n, const float* terms, float anchor, float* out);

@@ -24,6 +24,10 @@ host paths, _forward and _backward: the library treats a one-view call as V = 1.
 `geometry=False` on the two backward functions (not part of the reference surface) runs the library's appearance-only
 backward: only the colour / feature / SH gradients, for training with frozen geometry.  The reference's
 rasterize_gaussians_backward, as the dropin calls it, always runs the full backward.
+
+`absgrad=True` on the two backward functions (not part of the reference surface either) also computes the absolute
+screen-space gradients dL_dmeans2D_abs (AbsGS, gsplat's absgrad): per Gaussian and view, the sum over pixels of
+|dL/dmean2D.x| and |dL/dmean2D.y|, returned as one more element after all others.
 """
 import ctypes
 import warnings
@@ -247,7 +251,7 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
 def _backward(views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
-              surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False):
+              surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False, absgrad=False):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
     one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
@@ -255,7 +259,8 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     `geometry=False`: the appearance-only backward.  Nothing is allocated for the six geometry gradients, which come
     back None, and of dL_dfeatures, dL_dcolors, dL_dsh only those `appearance` = (features, colors, sh) asks for are
     computed (the others are None too); the opacity, depth and surface cotangents are not read.  `antialiasing` must
-    be the forward's."""
+    be the forward's.  `absgrad`: the third element returned is (dL_dmeans2D_abs,) ([P,2], or [V,P,2] for V views;
+    None without the geometry half, geometry=False, which never computes it); () without absgrad."""
     if not geometry and (cam_grads or _out is not None):
         raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
@@ -310,6 +315,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
                 sh_factor = torch.empty((V, P, 3), **f32)
         dL_dscales = _alloc("scales", (P, 3))
         dL_drotations = _alloc("rotations", (P, 4))
+    dL_dmeans2D_abs = torch.empty(((V,) if views else ()) + (P, 2), **f32) if absgrad and geometry else None
     # zeroed: a call with P = 0 writes nothing, otherwise the library overwrites every element
     cam = tuple(torch.zeros(shape, **f32) for shape in ((V, 4, 4), (V, 4, 4), (V, 3))) if cam_grads else ()
     # (appearance-only with nothing to compute: no call, e.g. S = 0 features the only input that needs a gradient)
@@ -326,7 +332,11 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
         a.geom = geomBuffer.data_ptr(); a.geom_bytes = geomBuffer.numel()
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
-        det_ws = _lib.det_workspace(a, lib.r3dg_raster_bwd_det_bytes(V * P, S), dev)
+        a.dL_dmeans2D_abs = _lib.ptr(dL_dmeans2D_abs)
+        det_bytes = lib.r3dg_raster_bwd_det_bytes(V * P, S)
+        if dL_dmeans2D_abs is not None:                 # absgrad's fixed-point sums follow the gradient rows'
+            det_bytes += lib.r3dg_raster_bwd_det_absgrad_bytes(V * P)
+        det_ws = _lib.det_workspace(a, det_bytes, dev)
         if cam:
             cam_ws = _lib.scratch(lib.r3dg_raster_cam_grad_bytes(P, V), dev)
             a.dL_dviewmatrix, a.dL_dprojmatrix, a.dL_dcampos = (t.data_ptr() for t in cam)
@@ -334,8 +344,10 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
         surface_ws = _surface_args(a, surface if geometry else None, W, H, V, dev, surface_work, principal=principal)
         _lib.call("r3dg_raster_backward", dev, ctypes.byref(a),
                   what="rasterize_views_backward" if views else "rasterize_gaussians_backward")
+    elif dL_dmeans2D_abs is not None:                   # P = 0: nothing to write
+        dL_dmeans2D_abs.zero_()
     return (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
-            dL_dscales, dL_drotations), cam
+            dL_dscales, dL_drotations), cam, ((dL_dmeans2D_abs,) if absgrad else ())
 
 
 def rasterize_gaussians_backward(background, means3D, features, radii, colors, scales, rotations,
@@ -343,7 +355,8 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  tan_fovy, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
                                  imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
-                                 surface_work=None, geometry=True, appearance=(True, True, True), *, antialiasing=False):
+                                 surface_work=None, geometry=True, appearance=(True, True, True), *, antialiasing=False,
+                                 absgrad=False):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
@@ -354,14 +367,17 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards.
     `geometry=False` (not part of the reference surface either) is the appearance-only backward of _backward: the
     gradients of the geometry inputs, and of the appearance inputs `appearance` = (features, colors, sh) leaves out,
-    come back None.  `antialiasing` (not part of the reference surface) must be the forward's: rasterize_gaussians."""
+    come back None.  `antialiasing` (not part of the reference surface) must be the forward's: rasterize_gaussians.
+    `absgrad=True` (not part of the reference surface): dL_dmeans2D_abs [P,2] is the last element (None when
+    geometry=False)."""
     principal = surface[4:6] if surface is not None and len(surface) == 6 else None
-    grads, cam = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
+    grads, cam, extra = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
                            dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
                            binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
-                           surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing)
-    return grads + tuple(t[0] for t in cam)
+                           surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing,
+                           absgrad)
+    return grads + tuple(t[0] for t in cam) + extra
 
 
 def _surface_args(a, surface, W, H, V, device, work=None, principal=None):
@@ -458,7 +474,7 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
                              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                              backward_geometry, cam_grads=False, surface=None, surface_work=None, geometry=True,
-                             appearance=(True, True, True), *, antialiasing=False):
+                             appearance=(True, True, True), *, antialiasing=False, absgrad=False):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
@@ -467,10 +483,11 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth), all [V,*,H,W] (a cotangent may be None), and
     `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
     one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
-    rasterize_gaussians_backward, and `antialiasing` must be the forward's."""
-    grads, cam = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
+    rasterize_gaussians_backward, and `antialiasing` must be the forward's.  `absgrad=True`: dL_dmeans2D_abs [V,P,2]
+    is the last element, as in rasterize_gaussians_backward."""
+    grads, cam, extra = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                            dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                            backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
-                           appearance, antialiasing)
-    return grads + cam
+                           appearance, antialiasing, absgrad)
+    return grads + cam + extra

@@ -53,6 +53,7 @@ class RasterBwdArgs(ctypes.Structure):
          ("cam_work", c_void_p), ("cam_work_bytes", c_size_t),
          ("dL_dout_normal", c_void_p), ("dL_dout_surface_xyz", c_void_p), ("fwd_opacity", c_void_p), ("fwd_depth", c_void_p),
          ("cx", c_float), ("cy", c_float), ("surface_work", c_void_p), ("surface_work_bytes", c_size_t),
+         ("dL_dmeans2D_abs", c_void_p),
          ("antialiasing", c_int), ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -147,6 +148,7 @@ SYMBOLS = [
                                    c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
     ("r3dg_raster_fwd_det_bytes", c_size_t, [c_int]),
     ("r3dg_raster_bwd_det_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_raster_bwd_det_absgrad_bytes", c_size_t, [c_int]),
     ("r3dg_shade_det_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_det_sum_host", c_int, [c_ll, c_void_p, c_void_p]),
     ("r3dg_det_sum_scaled_host", c_int, [c_ll, c_void_p, c_float, c_void_p]),

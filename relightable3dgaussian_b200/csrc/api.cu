@@ -173,6 +173,7 @@ size_t r3dg_raster_views_img_bytes(int W, int H, int V) { return ImgLayout(W, H,
 size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).n_contrib; }
 size_t r3dg_raster_fwd_det_bytes(int P) { return align_up((size_t)(P < 1 ? 1 : P) * 8, 256); }
 size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S)); }
+size_t r3dg_raster_bwd_det_absgrad_bytes(int P) { return det_bytes(2 * (size_t)(P < 1 ? 1 : P)); }
 size_t r3dg_raster_cam_grad_bytes(int P, int V) {
     return align_up((size_t)(V < 1 ? 1 : V) * kCamGradFloats * cam_grad_blocks(P) * sizeof(float), 256);
 }
@@ -265,6 +266,9 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
                          (a->dL_dcov3D != nullptr) + (a->dL_dscales != nullptr) + (a->dL_drotations != nullptr);
     const bool geometry = geo_outs == 6 || a->P == 0;
     if (a->P > 0 && geo_outs != 0 && geo_outs != 6) return R3DG_ERR_BAD_ARG;
+    // absgrad: the deterministic workspace grows only when it is requested (the appearance-only mode ignores it)
+    if (a->deterministic && geometry && a->dL_dmeans2D_abs &&
+        a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S) + r3dg_raster_bwd_det_absgrad_bytes(V * a->P)) return R3DG_ERR_BAD_ARG;
     if (!geometry && (cam_outs != 0 || (!a->dL_dcolors && !a->dL_dfeatures && !a->dL_dsh))) return R3DG_ERR_BAD_ARG;
     if (V > 1 && a->P > 0 && a->shs && (geometry || a->dL_dsh) && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;

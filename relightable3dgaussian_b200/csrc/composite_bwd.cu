@@ -46,6 +46,11 @@ struct CompositeBwdParams {
     float* grad;     // [P][recf], the composited rows zero-initialised (zero_composited_rows_kernel)
     DetAcc det;      // DET: the same rows as fixed-point accumulators (detacc.cuh), [P * recf], as grad
     const uint32_t* det_scale;   // DET: per view, the scale words of its colour / feature and geometry slots (det_scale_reduce)
+    // ABS (absgrad): per row, sum_pixels |dL/dmean2D.x| and |dL/dmean2D.y|, [rows][2]: in the default mode the caller's
+    // dL_dmeans2D_abs itself (its composited rows zeroed by zero_composited_rows_kernel), in DET mode fixed-point
+    // accumulators of the geometry class behind the gradient rows' (det_abs)
+    float* abs_grad;
+    DetAcc det_abs;
 };
 
 // Sum v[i] over the 32 lanes for every i in [0,N) (N power of two, 4 <= N <= 32) with a
@@ -149,8 +154,13 @@ __device__ __forceinline__ void reduce_scatter_permuted_multi(float (&x)[U][W], 
 // arithmetic, but only the NC colour and feature components are formed and reduced — no dL/dalpha, no A recurrence, no
 // geometry butterfly — into a narrower row of NC floats (channel c at slot c).  Every channel component goes through the
 // same butterfly as with GEOM, so each added value, and in DET mode each row total, is bitwise the full kernel's.
-template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true>
+// ABS (absgrad, GEOM only): each lane also takes the magnitudes |v0[0]|, |v0[1]| of its pixel's two dL/dmean2D terms
+// (0 on gated lanes) before the geometry butterfly sums the signed terms away; one more 2-wide butterfly reduces them
+// over the warp's 32 pixels, and lanes 0 and 16 add the two totals to p.abs_grad (DET: p.det_abs, class exponent
+// e_geo) once per entry.  Everything else, the gradient row included, is the same code.
+template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true, bool ABS = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const CompositeBwdParams p) {
+    static_assert(GEOM || !ABS, "absgrad needs the geometry half of the backward");
     constexpr int NC = 4 * NG;              // padded channel count {r,g,b,f...}; gradient row = 8 geometry slots + NC
     constexpr int GOFF = GEOM ? 8 : 0;      // slot of channel 0 in the gradient row (GEOM = false: no geometry slots)
     // the NC channel components are reduced in power-of-two chunks of 16 / 8 / 4 (select-free butterflies)
@@ -292,7 +302,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     while (qcount > 0) {
         const int n = min(32, qcount);
         __syncwarp();
-        sId[warp][lane] = id_cur * (uint32_t)(GEOM ? p.recf : NC);     // element offset of the Gaussian's gradient row
+        // element offset of the Gaussian's gradient row (ABS: the row index itself, also that of its absgrad pair)
+        sId[warp][lane] = ABS ? id_cur : id_cur * (uint32_t)(GEOM ? p.recf : NC);
         sK[warp][lane] = k_cur;                                        // 0-based list position == contributor index
 #pragma unroll
         for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = r[g];
@@ -383,6 +394,15 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                 v0[u][6] = -0.5f * gdy * dy[u] * dL_dG;
                 v0[u][7] = 0.0f;
             }
+            float av[U][2], asum[U];
+            if constexpr (ABS) {                                            // before the butterfly below overwrites v0
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    av[u][0] = valid[u] ? fabsf(v0[u][0]) : 0.0f;
+                    av[u][1] = valid[u] ? fabsf(v0[u][1]) : 0.0f;
+                }
+                reduce_scatter_multi<U, 2>(av, lane, asum);                 // |x| total on lanes 0-15, |y| on 16-31
+            }
             if constexpr (GEOM) reduce_scatter_multi<U, 8>(v0, lane, mine); // geometry slots: lanes 0 mod 4
             if constexpr (C16 > 0) {
                 float x[U][16], t[U];
@@ -420,14 +440,25 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll
             for (int u = 0; u < U; ++u) {
                 if (j0 + u < n) {                                           // (warp-uniform)
+                    if constexpr (ABS) {
+                        const size_t a = 2 * (size_t)sId[warp][ju[u]] + (lane >> 4);
+                        if ((lane & 15) == 0) {
+                            if constexpr (DET) det_add(p.det_abs, a, asum[u], e_geo);
+                            else atomicAdd(p.abs_grad + a, asum[u]);
+                        }
+                    }
                     if constexpr (DET) {
-                        const size_t row = sId[warp][ju[u]];
+                        size_t row;
+                        if constexpr (ABS) row = (size_t)sId[warp][ju[u]] * p.recf;
+                        else row = sId[warp][ju[u]];
                         if constexpr (C4_SECOND) {
                             if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) det_add(p.det, row + 8 + B4 + (lane >> 3), t4[u], e_app);
                         }
                         if (my_sel >= 0) det_add(p.det, row + my_off, mine[u], my_sel == 0 ? e_geo : e_app);
                     } else {
-                        float* grow = p.grad + sId[warp][ju[u]];
+                        float* grow;
+                        if constexpr (ABS) grow = p.grad + (size_t)sId[warp][ju[u]] * p.recf;
+                        else grow = p.grad + sId[warp][ju[u]];
                         if constexpr (C4_SECOND) {
                             if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) atomicAdd(grow + 8 + B4 + (lane >> 3), t4[u]);
                         }
@@ -479,7 +510,9 @@ __device__ void det_scale_reduce(const CompositeBwdParams& p, int V, bool geomet
 // it walks only their contributor bits.  Every other row is neither written nor read in the backward, so ~80 % of the
 // rows of a dense scene are never touched.  One thread per row.  DET: the row's accumulators in the three word planes
 // and its flag bits, which are recf / 4 whole bytes (2 bits per accumulator, recf a multiple of 4); and, before that,
-// the views' cotangent scale (det_scale_reduce) into the scale words the caller zeroed.
+// the views' cotangent scale (det_scale_reduce) into the scale words the caller zeroed.  Absgrad (p.abs_grad or
+// p.det_abs set): also the row's pair of absgrad sums; in DET mode their flag bits, 8 rows to a word, are zeroed whole
+// by the first thread of each 8 rows (the flags of rows that are not composited are never read).
 template <bool DET>
 __global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, int recf, const uint8_t* __restrict__ clamped,
                                                                    float* __restrict__ grad, const DetAcc det,
@@ -488,8 +521,16 @@ __global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, 
     if constexpr (DET) {
         if ((int)blockIdx.x < nred) det_scale_reduce(p, V, geometry, nred, const_cast<uint32_t*>(p.det_scale));   // (block-uniform)
     }
+    if constexpr (DET) {
+        if (p.det_abs.words && (r & 7) == 0 && r < rows) p.det_abs.flags[r >> 3] = 0u;
+    }
     if (r >= rows || !(clamped[r] & kComposited)) return;
     if constexpr (DET) {
+        if (p.det_abs.words) {
+#pragma unroll 1
+            for (int plane = 0; plane < 3; ++plane)
+                *reinterpret_cast<uint4*>(p.det_abs.words + plane * p.det_abs.n + 2 * r) = make_uint4(0u, 0u, 0u, 0u);
+        }
 #pragma unroll 1
         for (int plane = 0; plane < 3; ++plane) {
             uint4* w = reinterpret_cast<uint4*>(det.words + plane * det.n + r * recf);
@@ -498,9 +539,14 @@ __global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, 
         uint8_t* f = reinterpret_cast<uint8_t*>(det.flags) + r * (recf / 4);
         for (int i = 0; i < recf / 4; ++i) f[i] = 0;
     } else {
+        if (p.abs_grad) { p.abs_grad[2 * r] = 0.0f; p.abs_grad[2 * r + 1] = 0.0f; }
         float4* g = reinterpret_cast<float4*>(grad + r * recf);
         for (int i = 0; i < recf / 4; ++i) g[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
+}
+
+DetAcc raster_det_abs(const r3dg_raster_bwd_args& a, size_t rows) {
+    return det_acc((char*)a.det_work + det_bytes(rows * rec_floats(a.S)), 2 * rows);   // behind r3dg_raster_bwd_det_bytes
 }
 
 uint32_t* raster_det_scale(const RasterBuffers& b) {
@@ -509,6 +555,9 @@ uint32_t* raster_det_scale(const RasterBuffers& b) {
 
 // resident CTAs per SM the register allocation is pinned to, by channel groups NG (the occupancy sweep in DESIGN.md §4.2)
 template <int NG> struct BwdOcc { static constexpr int v = NG <= 3 ? 5 : (NG <= 5 ? 4 : 3); };
+// the pin of an absgrad instantiation: BwdOcc's, except in deterministic mode at NG = 5, where the absgrad sums' fixed-
+// point adds do not fit the 128 registers of 4 CTAs per SM (ptxas spills) and 3 CTAs are resident instead
+template <int NG, bool DET> struct BwdOccAbs { static constexpr int v = DET && NG == 5 ? 3 : BwdOcc<NG>::v; };
 int g_bwd_ctas = 0;             // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
 int composite_bwd_tune(const char* key, int value, int* previous) {
     if (strcmp(key, "composite_bwd_ctas") != 0) return R3DG_ERR_UNSUPPORTED;
@@ -517,14 +566,15 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
     g_bwd_ctas = value;
     return 0;
 }
-template <int NG, bool DET, bool GEOM>
+template <int NG, bool DET, bool GEOM, bool ABS = false>
 static void launch_bwd_kernel(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
-    constexpr auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET, GEOM>;
+    constexpr auto kernel = composite_bwd_kernel<NG, 4, ABS ? BwdOccAbs<NG, DET>::v : BwdOcc<NG>::v, DET, GEOM, ABS>;
     kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
-static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, bool det, bool geometry, cudaStream_t stream) {
-    if (geometry) det ? launch_bwd_kernel<NG, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true>(p, tiles, stream);
+static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, bool det, bool geometry, bool absgrad, cudaStream_t stream) {
+    if (absgrad) det ? launch_bwd_kernel<NG, true, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, true>(p, tiles, stream);
+    else if (geometry) det ? launch_bwd_kernel<NG, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true>(p, tiles, stream);
     else det ? launch_bwd_kernel<NG, true, false>(p, tiles, stream) : launch_bwd_kernel<NG, false, false>(p, tiles, stream);
 }
 
@@ -551,6 +601,11 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     const int gradf = composite_bwd_row_floats(a.S, geometry);     // the gradient row: b.recf, or NC without geometry
     p.det = det_acc(a.det_work, rows * gradf);
     p.det_scale = det ? raster_det_scale(b) : nullptr;
+    // absgrad (geometry only; the appearance-only backward ignores dL_dmeans2D_abs): the default mode adds into the
+    // output itself, DET mode into its own accumulators behind the gradient rows' in det_work
+    const bool absgrad = geometry && a.dL_dmeans2D_abs != nullptr;
+    p.abs_grad = absgrad && !det ? a.dL_dmeans2D_abs : nullptr;
+    p.det_abs = absgrad && det ? raster_det_abs(a, rows) : det_acc(nullptr, 0);
     // zeroed here, in the backward, so that every backward over one forward (retain_graph) starts from zero
     const int zblocks = (int)((rows + 255) / 256);
     if (det) {
@@ -564,13 +619,13 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;
     switch (num_groups(a.S)) {
-        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, stream); break;
-        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, stream); break;
-        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, stream); break;
-        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, stream); break;
-        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, stream); break;
-        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, stream); break;
-        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, stream); break;
+        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, absgrad, stream); break;
+        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, absgrad, stream); break;
+        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, absgrad, stream); break;
+        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, absgrad, stream); break;
+        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, absgrad, stream); break;
+        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, absgrad, stream); break;
+        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, absgrad, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;   // S > 24: reference backward limit (backward.cu:449)
     }
     R3DG_CUDA_TRY(cudaGetLastError());

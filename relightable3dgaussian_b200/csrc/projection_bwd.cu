@@ -35,6 +35,9 @@ struct ProjBwdParams {
     bool acc, acc_colors, acc_features;
     // CAM: this view's [kCamGradFloats][gridDim.x] partial sums of the camera gradients (column-major: one column per CTA)
     float* cam_work;
+    // ABS: this view's dL_dmeans2D_abs [P,2] (composite_bwd.cu); DET: read from det_abs (rows det_row0 + idx)
+    float* dL_dmeans2D_abs;
+    DetAcc det_abs;
 };
 static_assert(kCamGradThreads == 128, "cam_grad_blocks() counts projection-backward CTAs");
 
@@ -124,7 +127,9 @@ __device__ __forceinline__ ViewDir view_dir(const float* m, const float* cam) {
 // DET (deterministic mode): the packed gradient row is read from the fixed-point accumulators and converted on load.
 // CAM (camera gradients): every thread also stages its Gaussian's 35 camera-gradient terms in a [35][SLAB_LD] slab
 // behind the SH slab, and the CTA writes their sums in a fixed order to its column of p.cam_work.
-template <bool DET = false, bool CAM = false>
+// ABS (absgrad): dL_dmeans2D_abs next to dL_dmeans2D — +0 for rows that are not live; a live row's sums the compositor
+// added in place (default mode, nothing to write) or into fixed-point accumulators (DET: read and written here).
+template <bool DET = false, bool CAM = false, bool ABS = false>
 __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const ProjBwdParams p) {
     // SH rows (192 B at M=16) travel through shared memory: the CTA's [128][3M] slab of shs is ONE contiguous
     // 24 KB block, fetched by a single TMA-unit bulk copy (cp.async.bulk, mbarrier-signalled) into a row-major
@@ -503,6 +508,17 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     if (!in_range) return;
 #pragma unroll
     for (int k = 0; k < 3; ++k) p.dL_dmeans2D[3 * (size_t)idx + k] = dmean2[k];
+    if constexpr (ABS) {
+        float* ab = p.dL_dmeans2D_abs + 2 * (size_t)idx;
+        if constexpr (DET) {
+            const size_t i = 2 * (p.det_row0 + idx);
+            const int eg = det_scale_exp(p.det_scale[1]);
+            ab[0] = live ? det_load(p.det_abs, i, eg) : 0.0f;
+            ab[1] = live ? det_load(p.det_abs, i + 1, eg) : 0.0f;
+        } else if (!live) {
+            ab[0] = 0.0f; ab[1] = 0.0f;
+        }
+    }
     if (p.dL_dsh_factor) {
 #pragma unroll
         for (int k = 0; k < 3; ++k) p.dL_dsh_factor[3 * (size_t)idx + k] = dfac[k];
@@ -596,7 +612,15 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     const bool cam = a.dL_dviewmatrix != nullptr;
     p.cam_work = cam ? (float*)a.cam_work + (size_t)v * kCamGradFloats * blocks : nullptr;
     const size_t cam_smem = sh_smem + (size_t)kCamGradFloats * SLAB_LD * sizeof(float);
-    if (cam && a.deterministic) projection_bwd_kernel<true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
+    const bool abs = a.dL_dmeans2D_abs != nullptr;
+    p.dL_dmeans2D_abs = abs ? a.dL_dmeans2D_abs + 2 * r : nullptr;
+    p.det_abs = abs && a.deterministic ? raster_det_abs(a, (size_t)b.V * a.P) : det_acc(nullptr, 0);
+    if (abs) {
+        if (cam && a.deterministic) projection_bwd_kernel<true, true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
+        else if (cam) projection_bwd_kernel<false, true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
+        else if (a.deterministic) projection_bwd_kernel<true, false, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+        else projection_bwd_kernel<false, false, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    } else if (cam && a.deterministic) projection_bwd_kernel<true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
     else if (cam) projection_bwd_kernel<false, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
     else if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
     else projection_bwd_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);

@@ -67,12 +67,29 @@ def _check(t, what, rows=None, cols=None):
     return t
 
 
-def add_densification_stats(model, viewspace_point_tensor, update_filter, weights, radii=None):
+def add_densification_stats(model, viewspace_point_tensor, update_filter, weights, radii=None, absgrad=False):
     """`GaussianModel.add_densification_stats` (gaussian_model.py:931-937): weights_accum += weights and, for the rows
     in `update_filter`, xyz_gradient_accum += |grad[:, :2]|, normal_gradient_accum += |_normal.grad|, denom += 1.
-    With `radii` it also folds in train.py:164-165's max_radii2D update over the same rows.  One launch, no sync."""
+    With `radii` it also folds in train.py:164-165's max_radii2D update over the same rows.  One launch, no sync.
+
+    `absgrad=True` (AbsGS; not part of the reference surface): xyz_gradient_accum accumulates |absgrad| instead, the
+    norm of `viewspace_point_tensor.absgrad` [P,2] that the rasterizer's backward sets in its absgrad mode
+    (rasterizer.set_absgrad), the per-pixel magnitudes summed before cancelling.  That statistic is larger than
+    |grad[:, :2]|, so it wants a larger densify_grad_threshold: gsplat defaults to grow_grad2d = 0.0008 with absgrad
+    and 0.0002 without (gsplat's defaults, not a value tuned for this project).  A missing or mis-shaped `.absgrad` is
+    refused before anything is launched."""
     P = model._xyz.shape[0]
-    grad = viewspace_point_tensor.grad
+    if absgrad:
+        grad = getattr(viewspace_point_tensor, "absgrad", None)
+        if grad is None:
+            raise RuntimeError("add_densification_stats(absgrad=True): viewspace_point_tensor has no .absgrad (the "
+                               "rasterizer sets it in its absgrad mode: rasterizer.set_absgrad(True) or absgrad=True)")
+        if not torch.is_tensor(grad) or tuple(grad.shape) != (P, 2):
+            raise ValueError(f"viewspace_point_tensor.absgrad: expected a [P, 2] = {(P, 2)} tensor, got "
+                             f"{tuple(grad.shape) if torch.is_tensor(grad) else type(grad).__name__}")
+        _check(grad, "viewspace_point_tensor.absgrad", P)
+    else:
+        grad = viewspace_point_tensor.grad
     if grad is None:
         raise RuntimeError("add_densification_stats: viewspace_point_tensor has no .grad")
     ngrad = model._normal.grad
@@ -215,9 +232,11 @@ def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, max
 _saved = None
 
 
-def install(cls=None):
+def install(cls=None, absgrad=False):
     """Rebind `cls.add_densification_stats` and `cls.densify_and_prune` (default: the reference's
-    scene.gaussian_model.GaussianModel) to the fused versions.  Raises if already installed."""
+    scene.gaussian_model.GaussianModel) to the fused versions.  Raises if already installed.  `absgrad=True`: the
+    installed add_densification_stats accumulates the absgrad statistic (add_densification_stats(absgrad=True)); with
+    rasterizer.set_absgrad(True) these are the two lines that give the reference's training loop AbsGS densification."""
     global _saved
     if _saved is not None:
         raise RuntimeError("densify.install(): already installed; call uninstall() first")
@@ -226,7 +245,7 @@ def install(cls=None):
     _saved = (cls, cls.__dict__.get("add_densification_stats"), cls.__dict__.get("densify_and_prune"))
 
     def _stats(self, viewspace_point_tensor, update_filter, weights):
-        return add_densification_stats(self, viewspace_point_tensor, update_filter, weights)
+        return add_densification_stats(self, viewspace_point_tensor, update_filter, weights, absgrad=absgrad)
 
     def _dp(self, max_grad, min_opacity, extent, max_screen_size, max_grad_normal, weights_threshold=1e-4):
         return densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size, max_grad_normal, weights_threshold)

@@ -56,6 +56,30 @@ def set_deferred_count(enabled: bool):
     _DEFER_COUNT = bool(enabled)
 
 
+_ABSGRAD = False
+
+
+def set_absgrad(enabled: bool):
+    """Process default of the absolute screen-space gradients (not part of the reference surface): with it on, every
+    `GaussianRasterizer`, `rasterize_gaussians` and `rasterize_views` call runs as with `absgrad=True`.  Together with
+    `densify.install(absgrad=True)` this gives the reference's unmodified training loop the AbsGS densification
+    statistic.  `set_absgrad(False)` restores the default (off)."""
+    global _ABSGRAD
+    _ABSGRAD = bool(enabled)
+
+
+def _absgrad_on(absgrad):
+    """The call's absgrad mode: its keyword, or the process default (set_absgrad)."""
+    return bool(absgrad) or _ABSGRAD
+
+
+def _set_absgrad(means2D, g_abs):
+    """Adds g_abs to `means2D.absgrad` on the caller's tensor object, as autograd accumulates `.grad`: set on the first
+    backward, summed with what is there on later ones (retain_graph, or a tensor used in several graphs)."""
+    prev = getattr(means2D, "absgrad", None)
+    means2D.absgrad = g_abs if prev is None else prev + g_abs
+
+
 _EXCHANGE = None
 
 
@@ -125,13 +149,13 @@ def _surface_cotangents(ctx, g_normal, g_surface_xyz):
 def _input_grads(ctx, grads, cameras):
     """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
     three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
-    one, and for all three when none was computed.  The last input, the antialiasing flag, gets None."""
+    one, and for all three when none was computed.  The last two inputs, the antialiasing and absgrad flags, get None."""
     g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
     cam = (None, None, None)
     if grads[9:]:
         cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[11:14]))
     return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
-            None, None) + cam + (None,)
+            None, None) + cam + (None, None)
 
 
 # the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
@@ -155,6 +179,12 @@ def _aa_kw(antialiasing):
     return {"antialiasing": True} if antialiasing else {}
 
 
+def _absgrad_kw(ctx, kw):
+    """The keyword that asks the library backward for dL_dmeans2D_abs: only when the node's absgrad mode is on, means2D
+    needs a gradient and the backward runs its geometry half (`kw` from _backward_mode)."""
+    return {"absgrad": True} if ctx.absgrad and ctx.needs_input_grad[1] and kw.get("geometry", True) else {}
+
+
 def _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
     """The positional arguments of _C.rasterize_gaussians for the settings `rs`."""
     return (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
@@ -171,7 +201,7 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing):
+                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing, absgrad):
         rs = raster_settings
         out = _debug_call(rs.debug, _C.rasterize_gaussians,
                           _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
@@ -181,6 +211,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                           **_aa_kw(antialiasing))
         ctx.raster_settings = rs
         ctx.antialiasing = antialiasing
+        ctx.absgrad = absgrad
+        ctx.means2D = means2D if absgrad else None      # the caller's tensor object: the backward sets .absgrad on it
         ctx.num_rendered = out[0]
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
                       out[9], sh, *out[10:13], opacities)
@@ -208,6 +240,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             ex = _EXCHANGE
         kw = _backward_mode(ctx)
         kw.update(_aa_kw(ctx.antialiasing))
+        kw.update(_absgrad_kw(ctx, kw))
         if ex is not None:
             kw["_out"] = {"sh_factor": ex[0].factor}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
@@ -235,6 +268,9 @@ class _RasterizeGaussians(torch.autograd.Function):
             exchange.gather_factors()
             g_sh_avg = exchange.rebuild_sh(means3D, campos_all, rs.sh_degree)
             grads = grads[:6] + (g_sh_avg,) + grads[7:]
+        if kw.get("absgrad"):
+            _set_absgrad(ctx.means2D, grads[-1])
+            grads = grads[:-1]
         return _input_grads(ctx, grads, (rs.viewmatrix, rs.projmatrix, rs.campos))
 
 
@@ -272,7 +308,8 @@ def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, feat
 
 
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
-                        rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False, antialiasing=False):
+                        rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False, antialiasing=False,
+                        absgrad=False):
     """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
     cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
     when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
@@ -288,7 +325,14 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     dilation keeps the Gaussian's integrated weight instead of spreading a sub-pixel Gaussian over a pixel at full
     opacity: a model trained with it renders consistently at other resolutions and distances.  The gradients include
     rho's dependence on the 2D covariance and so reach means3D, scales, rotations, cov3Ds_precomp and the view matrix.
-    Radii, tile lists and colours are those of the default mode; the images, weights and counts differ."""
+    Radii, tile lists and colours are those of the default mode; the images, weights and counts differ.
+
+    With `absgrad=True`, or after `set_absgrad(True)` (not part of the reference surface), the backward also sets
+    `means2D.absgrad` [P,2] on the caller's `means2D` tensor when means2D needs a gradient: per Gaussian, the sum over
+    pixels of |dL/dmean2D.x| and |dL/dmean2D.y|, each pixel's term taken before the sum, in the units of
+    `means2D.grad` (AbsGS; gsplat's absgrad).  Opposite pulls then no longer cancel, so the statistic of
+    densify.add_densification_stats(absgrad=True) sees Gaussians that cover high-frequency detail.  Like `.grad` it
+    accumulates over backward calls; the caller resets it (`means2D.absgrad = None`).  Everything else is unchanged."""
     global _CALL_GRAD_MODE
     rs = raster_settings
     _refuse_surface_grads_without_normals(surface_grads, rs.computer_pseudo_normal)
@@ -296,16 +340,17 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     _CALL_GRAD_MODE = torch.is_grad_enabled()
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
                                      scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
-                                     rs.viewmatrix, rs.projmatrix, rs.campos, bool(antialiasing))
+                                     rs.viewmatrix, rs.projmatrix, rs.campos, bool(antialiasing), _absgrad_on(absgrad))
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, surface_grads=False, antialiasing=False):
-        """`surface_grads` and `antialiasing` (not part of the reference surface): see rasterize_gaussians."""
+    def __init__(self, raster_settings, surface_grads=False, antialiasing=False, absgrad=False):
+        """`surface_grads`, `antialiasing` and `absgrad` (not part of the reference surface): see rasterize_gaussians."""
         super().__init__()
         self.raster_settings = raster_settings
         self.surface_grads = surface_grads
         self.antialiasing = antialiasing
+        self.absgrad = absgrad
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -318,7 +363,8 @@ class GaussianRasterizer(nn.Module):
             means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features)
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
                                    scales, rotations, cov3D_precomp, self.raster_settings,
-                                   surface_grads=self.surface_grads, antialiasing=self.antialiasing)
+                                   surface_grads=self.surface_grads, antialiasing=self.antialiasing,
+                                   absgrad=self.absgrad)
 
 
 _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
@@ -330,7 +376,7 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing):
+                settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing, absgrad):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
@@ -338,6 +384,8 @@ class _RasterizeViews(torch.autograd.Function):
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
                                  rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing))
         ctx.meta = (rs, cams, antialiasing)
+        ctx.absgrad = absgrad
+        ctx.means2D = means2D if absgrad else None
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
                       bg, viewmatrix, projmatrix, campos, *out[10:13])
         return out[:10]
@@ -351,17 +399,22 @@ class _RasterizeViews(torch.autograd.Function):
         g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
                                                                    g_feature)
         kw = _backward_mode(ctx)
+        kw.update(_absgrad_kw(ctx, kw))
         if kw.get("geometry", True):
             kw.update(cam_grads=any(ctx.needs_input_grad[11:14]), surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
                                             cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
                                             g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
                                             rs.backward_geometry, **_aa_kw(antialiasing), **kw)
+        if kw.get("absgrad"):
+            _set_absgrad(ctx.means2D, grads[-1])
+            grads = grads[:-1]
         return _input_grads(ctx, grads, (viewmatrix, projmatrix, campos))
 
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
-                    rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False):
+                    rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False,
+                    absgrad=False):
     """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
 
     `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
@@ -374,8 +427,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
     Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
-    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads` and `antialiasing` are those of rasterize_gaussians and
-    apply to every view."""
+    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing` and `absgrad` are those of
+    rasterize_gaussians and apply to every view; `means2D.absgrad` is then [V,P,2], each view's own."""
     settings = list(settings)
     V = len(settings)
     if V < 1:
@@ -408,7 +461,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
                                  cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos,
-                                 bool(antialiasing))
+                                 bool(antialiasing), _absgrad_on(absgrad))
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
