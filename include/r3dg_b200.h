@@ -478,6 +478,55 @@ int r3dg_densify_apply(int P, const int* totals, int num_tensors, const r3dg_den
                        const void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * MCMC densification (3DGS-MCMC, Kheradmand et al. 2024; gsplat's MCMCStrategy): relocation of
+ * dead Gaussians onto live ones and growth under a budget, and the per-step position noise.  The
+ * host side is relightable3dgaussian_b200/mcmc.py.  sigma32(l) = 1 / (1 + expf(-l)) with IEEE
+ * division (torch's CUDA fp32 sigmoid).  Nothing here synchronises with the host.
+ *
+ * r3dg_mcmc_noise: in place, xyz += scale * sigma(-k (sigma32(l) - t)) * Sigma z per row, with
+ *   Sigma = R diag(exp(s))^2 R^T, R the rotation matrix of the normalised quaternion `rotation`
+ *   [P,4], s = `scaling` [P,3] (log scales), l = `opacity` [P] (logits), z [P,3] standard normals.
+ *   Evaluated in fp64 from the fp32 inputs, rounded once to fp32.  1 launch (0 for P = 0).
+ *
+ * r3dg_mcmc_classify: row i is alive when sigma32(l_i) > min_opacity and weighs w_i = sigma32(l_i)
+ *   if alive, else 0.  Writes into `tmp` the alive flags, zeroed per-row draw counts and the
+ *   inclusive fp64 CDF of w, summed in a fixed order (bitwise reproducible).  3 launches.
+ *
+ * r3dg_mcmc_apply: draws, per-source counts, the source update and the row writes, from the
+ *   classify results in `tmp`.  Draw d with uniform u_d picks the smallest i with cdf[i] >
+ *   u_d * total (total = cdf[P-1]); when no row is alive every row weighs 1 (i = floor(u_d P)).
+ *     n_new == 0, relocation, in place (every dst == src): uniforms [P], one per row; each dead row
+ *       draws when some row is alive, and is rewritten as a copy of its source;
+ *     n_new  > 0, growth (dst != src, dst holding P + n_new rows): uniforms [n_new]; output rows
+ *       0..P-1 are the input rows, then one copy of the source per draw, in draw order.
+ *   A source drawn c >= 1 times is corrected with N = min(c + 1, n_max) (so every copy of a source
+ *   drawn more than n_max - 1 times gets the N = n_max values), o = sigma32(l) in fp64:
+ *     x = 1 - (1 - o)^(1/N), coef = o / sum_{j=1..N} (-1)^(j-1) C(N,j) x^j / sqrt(j)  (fp64;
+ *     coef = 1 when x = 0), l' = fp32(logit(clamp(x, min_opacity, 1 - 2^-23))),
+ *     s'_k = fp32(s_k + log coef).
+ *   Rewritten rows (drawn sources and their copies) take the source's row with these kinds:
+ *     COPY     the source's values;      MOMENT   zero (Adam moments and the statistics);
+ *     R3DG_MCMC_OPACITY (row_bytes 4)  l';  R3DG_MCMC_SCALING (row_bytes 12)  s'.
+ *   Every other row keeps its values.  `opacity` / `scaling` are the same tensors the OPACITY /
+ *   SCALING descriptors read.  At most R3DG_DENSIFY_MAX tensors; 2 <= n_max <= R3DG_MCMC_MAX_N;
+ *   r3dg_mcmc_tmp_bytes(P, n_new) bytes of tmp (16-byte aligned) serve both phases.  3 launches.
+ *   A draw never picks a dead row: where the CDF's partial sums meet it can step by one ulp, and a
+ *   target inside such a step that lands on a dead row moves on to the next live row.
+ * P <= 0 and every other bad argument return R3DG_ERR_BAD_ARG before anything is launched (except
+ * r3dg_mcmc_noise, for which P = 0 is a no-op).
+ * ------------------------------------------------------------------------------------------ */
+#define R3DG_MCMC_MAX_N 64
+enum { R3DG_MCMC_OPACITY = 5, R3DG_MCMC_SCALING = 6 };
+size_t r3dg_mcmc_tmp_bytes(int P, int n_new);
+int r3dg_mcmc_noise(int P, float* xyz, const float* rotation, const float* scaling, const float* opacity,
+                    const float* z, double scale, double k, double t, r3dg_stream_t stream);
+int r3dg_mcmc_classify(int P, const float* opacity, float min_opacity, void* tmp, size_t tmp_bytes,
+                       r3dg_stream_t stream);
+int r3dg_mcmc_apply(int P, int n_new, const float* uniforms, const float* opacity, const float* scaling,
+                    double min_opacity, int n_max, int num_tensors, const r3dg_densify_tensor* tensors,
+                    void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * BRDF shading: fused `rendering_equation` (gaussian_renderer/neilf.py:339-371) + `GGX_specular`
  * (:374-406) + lat-long environment lookup (scene/direct_light_map.py:70-83) + SH incident light.
  * The reference has no extension boundary here (pure PyTorch; its render_equation.cu is dead,

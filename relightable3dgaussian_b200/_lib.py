@@ -146,6 +146,12 @@ SYMBOLS = [
                                       ctypes.POINTER(DensifyThresholds), c_void_p, c_size_t, c_void_p, c_void_p]),
     ("r3dg_densify_apply", c_int, [c_int, ctypes.POINTER(c_int), c_int, ctypes.POINTER(DensifyTensor), c_void_p, c_void_p,
                                    c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_mcmc_tmp_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_mcmc_noise", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_double, ctypes.c_double,
+                                ctypes.c_double, c_void_p]),
+    ("r3dg_mcmc_classify", c_int, [c_int, c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_mcmc_apply", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_double, c_int, c_int,
+                                ctypes.POINTER(DensifyTensor), c_void_p, c_size_t, c_void_p]),
     ("r3dg_raster_fwd_det_bytes", c_size_t, [c_int]),
     ("r3dg_raster_bwd_det_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_raster_bwd_det_absgrad_bytes", c_size_t, [c_int]),

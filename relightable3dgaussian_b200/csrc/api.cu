@@ -507,6 +507,28 @@ int r3dg_densify_apply(int P, const int* totals, int num_tensors, const r3dg_den
     return rc;
 }
 
+// ---- MCMC densification (mcmc.py) ----------------------------------------------------------------
+size_t r3dg_mcmc_tmp_bytes(int P, int n_new) { return mcmc_tmp_bytes(P < 0 ? 0 : P, n_new < 0 ? 0 : n_new); }
+int r3dg_mcmc_noise(int P, float* xyz, const float* rotation, const float* scaling, const float* opacity, const float* z,
+                    double scale, double k, double t, r3dg_stream_t stream) {
+    const int rc = launch_mcmc_noise(P, xyz, rotation, scaling, opacity, z, scale, k, t, (cudaStream_t)stream);
+    if (rc == 0 && P > 0) g_launches += 1;
+    return rc;
+}
+int r3dg_mcmc_classify(int P, const float* opacity, float min_opacity, void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_mcmc_classify(P, opacity, min_opacity, tmp, tmp_bytes, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 3;        // classify, block-sum scan, cdf
+    return rc;
+}
+int r3dg_mcmc_apply(int P, int n_new, const float* uniforms, const float* opacity, const float* scaling, double min_opacity,
+                    int n_max, int num_tensors, const r3dg_densify_tensor* tensors, void* tmp, size_t tmp_bytes,
+                    r3dg_stream_t stream) {
+    const int rc = launch_mcmc_apply(P, n_new, uniforms, opacity, scaling, min_opacity, n_max, num_tensors, tensors, tmp,
+                                     tmp_bytes, num_sms(), (cudaStream_t)stream);
+    if (rc == 0) g_launches += 3;        // draw, source update, apply
+    return rc;
+}
+
 // ---- simple_knn._C.distCUDA2 ----------------------------------------------------------------
 size_t r3dg_knn_tmp_bytes(int P) { return knn_tmp_bytes(P); }
 int r3dg_knn_dist2(int P, const float* points, float* mean_dist2, void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {

@@ -205,6 +205,15 @@ int launch_densify_apply(int P, const int* totals, int num, const r3dg_densify_t
                          const float* scaling, const float* samples, float split_recip, const void* tmp, size_t tmp_bytes,
                          int num_sms, cudaStream_t stream);
 
+// mcmc.cu: MCMC densification (relocation, growth) and position noise; launchers validate before launching
+size_t mcmc_tmp_bytes(int P, int n_new);
+int launch_mcmc_noise(int P, float* xyz, const float* rotation, const float* scaling, const float* opacity, const float* z,
+                      double scale, double k, double t, cudaStream_t stream);
+int launch_mcmc_classify(int P, const float* opacity, float min_opacity, void* tmp, size_t tmp_bytes, cudaStream_t stream);
+int launch_mcmc_apply(int P, int n_new, const float* u, const float* opacity, const float* scaling, double min_opacity, int n_max,
+                      int num, const r3dg_densify_tensor* tensors, void* tmp, size_t tmp_bytes, int num_sms,
+                      cudaStream_t stream);
+
 size_t knn_tmp_bytes(int P);
 int launch_knn(int P, const float* points, float* out, void* tmp, size_t tmp_bytes, int num_sms, cudaStream_t stream);
 

@@ -120,30 +120,30 @@ def add_densification_stats(model, viewspace_point_tensor, update_filter, weight
               model.denom.data_ptr(), mr.data_ptr() if mr is not None else None, what="densify_stats")
 
 
-def _groups(model, P):
-    """[(group, name, param, state or None)] in param_groups order, validated."""
+def _groups(model, P, what="densify_and_prune"):
+    """[(group, name, param, state or None)] in param_groups order, validated; errors name the caller `what`."""
     opt = model.optimizer
     out = []
     for g in opt.param_groups:
         name = g.get("name")
         if len(g["params"]) != 1:
-            raise ValueError(f"densify_and_prune: group {name!r} must hold exactly one parameter")
+            raise ValueError(f"{what}: group {name!r} must hold exactly one parameter")
         if name not in ATTRS:
-            raise KeyError(f"densify_and_prune: unknown parameter group {name!r}")
+            raise KeyError(f"{what}: unknown parameter group {name!r}")
         p = _check(g["params"][0], f"parameter {name!r}", P)
         st = opt.state.get(p, None)
         if st is not None:
             if "exp_avg" not in st or "exp_avg_sq" not in st:
-                raise ValueError(f"densify_and_prune: optimizer state of {name!r} has no Adam moments")
+                raise ValueError(f"{what}: optimizer state of {name!r} has no Adam moments")
             for k in ("exp_avg", "exp_avg_sq"):
                 _check(st[k], f"{k} of {name!r}", P)
                 if st[k].shape != p.shape:
-                    raise ValueError(f"densify_and_prune: {k} of {name!r} has shape {tuple(st[k].shape)}, parameter {tuple(p.shape)}")
+                    raise ValueError(f"{what}: {k} of {name!r} has shape {tuple(st[k].shape)}, parameter {tuple(p.shape)}")
         out.append((g, name, p, st))
     names = [n for _, n, _, _ in out]
     want = STAGE1_GROUPS + (PBR_GROUPS if getattr(model, "use_pbr", False) else ())
     if sorted(names) != sorted(want):
-        raise ValueError(f"densify_and_prune: parameter groups {names} do not match the model's {list(want)}")
+        raise ValueError(f"{what}: parameter groups {names} do not match the model's {list(want)}")
     return out
 
 
@@ -242,6 +242,9 @@ def install(cls=None, absgrad=False):
         raise RuntimeError("densify.install(): already installed; call uninstall() first")
     if cls is None:
         from scene.gaussian_model import GaussianModel as cls
+    from . import mcmc
+    if mcmc.installed_on() is cls:
+        raise RuntimeError(f"densify.install(): mcmc.install() holds {cls.__name__}; call mcmc.uninstall() first")
     _saved = (cls, cls.__dict__.get("add_densification_stats"), cls.__dict__.get("densify_and_prune"))
 
     def _stats(self, viewspace_point_tensor, update_filter, weights):
