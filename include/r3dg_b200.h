@@ -97,6 +97,16 @@ typedef struct r3dg_raster_fwd_args {
     int V;
     const float* view_cams;
     int features_per_view, colors_per_view;
+    /* 3D smoothing filter (Mip-Splatting's 3D filter; optional, NULL = off, the default): [P] filter sizes f >= 0, one
+     * per Gaussian and shared by every view of the call (r3dg_filter3d_compute).  Each Gaussian is drawn with scales
+     * s'_k = sqrt(s_k^2 + f^2) and opacity o' = o * coef, coef = sqrt((r_0 r_1) r_2), r_k = s_k^2 / s'_k^2 (1 when
+     * s'_k = 0): the covariance dilated by f^2 I keeps the Gaussian's integrated weight.  Every operation is a
+     * correctly rounded fp32 operation in that order (q_k = s_k s_k, g = f f, e_k = q_k + g, s'_k = sqrt(e_k),
+     * r_k = q_k / e_k), so a call with the filter equals, bit for bit, a call without it on (s', o') computed the same
+     * way.  scale_modifier multiplies s'.  With `antialiasing`, the record holds o' rho.  f = 0 gives s' = |s| and
+     * coef = 1 (for s = 0 and every s whose square is a normal float).  With cov3D_precomp: R3DG_ERR_BAD_ARG before
+     * any launch. */
+    const float* filter_3d;
     /* Antialiased mode (the opacity-compensated screen-space filter of upstream 3DGS and gsplat).  Non-zero: with
      * a0, b, c0 the 2D covariance before the fixed 0.3 px^2 dilation and a1 = a0 + 0.3, c1 = c0 + 0.3, every Gaussian's
      * opacity is multiplied by rho = sqrt(max(r, 2.5e-5)), r = (a0 c0 - b^2) / (a1 c1 - b^2) (r = 0 when a0 c0 - b^2
@@ -215,6 +225,14 @@ typedef struct r3dg_raster_bwd_args {
     const float* fwd_depth;
     float cx, cy;
     void* surface_work; size_t surface_work_bytes;
+    /* 3D smoothing filter (see r3dg_raster_fwd_args): NULL, or [P] holding the matching forward's values, like
+     * scale_modifier.  `opacities` [P] is the forward's opacity o, required with filter_3d (the record holds o coef,
+     * and coef may be 0 or subnormal, so o is not recovered from it).  Live rows then get dL_dopacity = coef dL/do' and
+     * dL_dscales_k = dL/ds'_k s_k / s'_k + o dL/do' dcoef/ds_k (s_k / s'_k = 1 where s'_k = 0); there is no gradient
+     * with respect to f.  filter_3d with cov3D_precomp, or without opacities, returns R3DG_ERR_BAD_ARG before any
+     * launch.  The appearance-only mode ignores both fields. */
+    const float* filter_3d;
+    const float* opacities;
     /* Absolute screen-space gradients (absgrad, AbsGS / gsplat's absgrad=True; optional, NULL = none, the default):
      * [P,2] ([V,P,2] for V views), next to dL_dmeans2D and in its units (0.5 W and 0.5 H per pixel): per Gaussian and
      * view, sum over pixels of |dL/dmean2D.x| and of |dL/dmean2D.y|, each pixel's term taken before the pixel sum, so
@@ -525,6 +543,27 @@ int r3dg_mcmc_classify(int P, const float* opacity, float min_opacity, void* tmp
 int r3dg_mcmc_apply(int P, int n_new, const float* uniforms, const float* opacity, const float* scaling,
                     double min_opacity, int n_max, int num_tensors, const r3dg_densify_tensor* tensors,
                     void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * 3D smoothing filter (Mip-Splatting's compute_3D_filter, Yu et al. 2024): the per-Gaussian
+ * filter size f [P] that r3dg_raster_fwd_args.filter_3d takes, from the V training cameras.
+ *   means3D [P,3]; viewmatrices [V,16] in the rasterizer's `viewmatrix` layout; intrinsics [V,6]
+ *   {fx, fy, cx, cy, W, H} (device); focal_max = F, the largest fx of the V cameras (host).
+ * For Gaussian i and camera c: t = [m_i, 1] V_c with z = t.z associated exactly as the
+ * rasterizer's near-cull depth, u = (t.x / z) fx + cx, v = (t.y / z) fy + cy (each operation
+ * rounded on its own, in that order).  The pair is valid when z > 0.2, -0.15 W <= u <= 1.15 W and
+ * -0.15 H <= v <= 1.15 H, each bound the fp32 rounding of the double product.  d_i = the least z
+ * of the valid pairs; a Gaussian no camera sees takes the largest d of the seen ones.  Then
+ * f_i = (d_i / F) * sqrt(0.2) (fp32, in that order); f = 0 everywhere when no Gaussian is seen.
+ * Differences from Mip-Splatting: each camera's own principal point (cx, cy) instead of (W/2, H/2),
+ * and no 1e5 cap on d.  min and max are order-free, so the result is bitwise reproducible; nothing
+ * synchronises with the host.  2 launches (0 for P = 0); tmp: r3dg_filter3d_tmp_bytes(P) bytes.
+ * P < 0, V < 1 with P > 0, F not finite and positive, or a missing pointer return
+ * R3DG_ERR_BAD_ARG before anything is launched.
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_filter3d_tmp_bytes(int P);
+int r3dg_filter3d_compute(int P, int V, const float* means3D, const float* viewmatrices, const float* intrinsics,
+                          float focal_max, float* filter_3d, void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * BRDF shading: fused `rendering_equation` (gaussian_renderer/neilf.py:339-371) + `GGX_specular`

@@ -28,6 +28,11 @@ rasterize_gaussians_backward, as the dropin calls it, always runs the full backw
 `absgrad=True` on the two backward functions (not part of the reference surface either) also computes the absolute
 screen-space gradients dL_dmeans2D_abs (AbsGS, gsplat's absgrad): per Gaussian and view, the sum over pixels of
 |dL/dmean2D.x| and |dL/dmean2D.y|, returned as one more element after all others.
+
+`filter_3d=` on all four functions (not part of the reference surface) runs the library's 3D smoothing filter
+(Mip-Splatting): a [P] or [P,1] fp32 CUDA tensor of per-Gaussian filter sizes f, shared by every view (filter3d.py).
+Each Gaussian is drawn with scales sqrt(s^2 + f^2) and its opacity times sqrt(prod_k s_k^2 / (s_k^2 + f^2)).  The
+backward takes the forward's tensor again and, with it, the forward's `opacities`; f gets no gradient.
 """
 import ctypes
 import warnings
@@ -90,6 +95,28 @@ class DeferredCount:
         return f"DeferredCount({self._value if self._value is not None else 'pending'})"
 
 
+def _check_filter_3d(filter_3d, P, cov3D_precomp):
+    """`filter_3d` as the library takes it ([P] fp32, contiguous, on the GPU), or None when absent.  Raises ValueError,
+    before anything is enqueued, for a wrong length (e.g. a filter computed before densification changed P), a CPU,
+    non-fp32 or non-contiguous tensor, one that requires grad (no gradient flows to it), or together with
+    cov3D_precomp (the filter is defined on scales)."""
+    if filter_3d is None:
+        return None
+    if not isinstance(filter_3d, torch.Tensor):
+        raise ValueError("filter_3d must be a tensor or None")
+    if cov3D_precomp is not None and cov3D_precomp.numel() != 0:
+        raise ValueError("filter_3d is defined on scales and cannot be combined with cov3D_precomp")
+    if tuple(filter_3d.shape) not in ((P,), (P, 1)):
+        raise ValueError(f"filter_3d must have shape [{P}] or [{P},1] (one value per Gaussian), got "
+                         f"{list(filter_3d.shape)}: recompute it after the number of Gaussians changed")
+    if not filter_3d.is_cuda or filter_3d.dtype != torch.float32 or not filter_3d.is_contiguous():
+        raise ValueError(f"filter_3d must be a contiguous float32 CUDA tensor, got {filter_3d.dtype} on "
+                         f"{filter_3d.device}{'' if filter_3d.is_contiguous() else ' (not contiguous)'}")
+    if filter_3d.requires_grad:
+        raise ValueError("filter_3d must not require grad: the rasterizer computes no gradient for it (detach it)")
+    return filter_3d
+
+
 def _prep(t, name):
     if t is None or t.numel() == 0:
         return t
@@ -132,15 +159,16 @@ def _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means
 
 def _forward(views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
              viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered, computer_pseudo_normal, debug,
-             capacity, pinned, defer, antialiasing=False):
+             capacity, pinned, defer, antialiasing=False, filter_3d=None):
     """The forward of the len(cams) views `cams` = [(tan_fovx, tan_fovy, cx, cy), ...]: one view (`views` False,
     outputs in the one-view shapes) or V views (outputs with a leading V).  Sizes the binning buffer for `capacity`
     instances and re-runs with room to spare while the counts, read back into the pinned int32 `pinned` (one per
     view), exceed it.  Returns the 12 outputs after num_rendered, the event recorded once the counts are copied, and the
     counts as a list: None when `defer`, which returns after the first attempt without waiting.  `antialiasing`: the
-    library's antialiased mode (see rasterize_gaussians)."""
+    library's antialiased mode (see rasterize_gaussians); `filter_3d`: the 3D filter (see the module notes)."""
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
+    filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
     dev = means3D.device
     a = _lib.RasterFwdArgs()
     keep = _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means3D, features, colors, scales,
@@ -150,6 +178,7 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     a.cx, a.cy = float(cams[0][2]), float(cams[0][3])
     a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
     a.debug = int(bool(debug)); a.antialiasing = int(bool(antialiasing))
+    a.filter_3d = _lib.ptr(filter_3d)
 
     lead = (V,) if views else ()
     f32 = dict(dtype=torch.float32, device=dev)
@@ -203,13 +232,15 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
 def rasterize_gaussians(background, means3D, features, colors, opacity, scales, rotations,
                         scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                         cx, cy, image_height, image_width, sh, degree, campos, prefiltered,
-                        computer_pseudo_normal, debug, _defer=False, _min_capacity=None, *, antialiasing=False):
+                        computer_pseudo_normal, debug, _defer=False, _min_capacity=None, *, antialiasing=False,
+                        filter_3d=None):
     """== RasterizeGaussiansCUDA (rasterize_points.cu:36-141).  Returns the 13-tuple
     (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
      out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer).
     `antialiasing=True` (not part of the reference surface) multiplies each Gaussian's opacity by
     rho = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)), the opacity compensation of the fixed 0.3 px^2
-    dilation; the backward must then be called with the same flag."""
+    dilation; the backward must then be called with the same flag.  `filter_3d` (not part of the reference surface):
+    Mip-Splatting's 3D filter, see the module notes; the backward must be given the same tensor."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")   # rasterize_points.cu:62-64
     P = means3D.size(0)
@@ -238,7 +269,7 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     out, ev, counts = _forward(False, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy, cx, cy)], H, W, sh, degree,
                                campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer,
-                               antialiasing)
+                               antialiasing, filter_3d)
     if _defer:
         rendered = DeferredCount(ev, pinned, capacity, st, P)
         st["pending"] = rendered
@@ -251,7 +282,8 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
 def _backward(views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
-              surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False, absgrad=False):
+              surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False, absgrad=False,
+              filter_3d=None, opacities=None):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
     one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
@@ -260,11 +292,15 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     back None, and of dL_dfeatures, dL_dcolors, dL_dsh only those `appearance` = (features, colors, sh) asks for are
     computed (the others are None too); the opacity, depth and surface cotangents are not read.  `antialiasing` must
     be the forward's.  `absgrad`: the third element returned is (dL_dmeans2D_abs,) ([P,2], or [V,P,2] for V views;
-    None without the geometry half, geometry=False, which never computes it); () without absgrad."""
+    None without the geometry half, geometry=False, which never computes it); () without absgrad.  `filter_3d` must be
+    the forward's, and `opacities` the forward's opacities (required with it)."""
     if not geometry and (cam_grads or _out is not None):
         raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
+    filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
+    if filter_3d is not None and (opacities is None or opacities.numel() != P):
+        raise ValueError("the backward with filter_3d needs the forward's opacities ([P] or [P,1])")
     H, W = dL_dout_color.size(-2), dL_dout_color.size(-1)
     dev = means3D.device
     a = _lib.RasterBwdArgs()
@@ -322,6 +358,9 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     if P != 0 and (geometry or any(_lib.ptr(t) for t in (dL_dfeatures, dL_dcolors, dL_dsh))):
         a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
         a.antialiasing = int(bool(antialiasing))
+        if filter_3d is not None:
+            opacities = _prep(opacities, "opacities")
+            a.filter_3d, a.opacities = _lib.ptr(filter_3d), _lib.ptr(opacities)
         a.dL_dout_color = _lib.ptr(dL_dout_color); a.dL_dout_opacity = _lib.ptr(dL_dout_opacity)
         a.dL_dout_depth = _lib.ptr(dL_dout_depth); a.dL_dout_feature = _lib.ptr(dL_dout_feature)
         a.dL_dmeans2D = _lib.ptr(dL_dmeans2D); a.dL_dcolors = _lib.ptr(dL_dcolors)
@@ -356,7 +395,7 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
                                  imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
                                  surface_work=None, geometry=True, appearance=(True, True, True), *, antialiasing=False,
-                                 absgrad=False):
+                                 absgrad=False, filter_3d=None, opacities=None):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
@@ -369,14 +408,15 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     gradients of the geometry inputs, and of the appearance inputs `appearance` = (features, colors, sh) leaves out,
     come back None.  `antialiasing` (not part of the reference surface) must be the forward's: rasterize_gaussians.
     `absgrad=True` (not part of the reference surface): dL_dmeans2D_abs [P,2] is the last element (None when
-    geometry=False)."""
+    geometry=False).  `filter_3d` (not part of the reference surface) must be the forward's, and then `opacities` the
+    forward's opacities: rasterize_gaussians."""
     principal = surface[4:6] if surface is not None and len(surface) == 6 else None
     grads, cam, extra = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
                            dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
                            binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
                            surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing,
-                           absgrad)
+                           absgrad, filter_3d, opacities)
     return grads + tuple(t[0] for t in cam) + extra
 
 
@@ -450,13 +490,13 @@ _views_capacity = {}     # (device, P, W, H, V) -> binning capacity that held th
 
 def rasterize_views(background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                     viewmatrix, projmatrix, cams, image_height, image_width, sh, degree, campos, prefiltered,
-                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False):
+                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False, filter_3d=None):
     """V views of one set of Gaussians in one forward.  background [V,3], viewmatrix / projmatrix [V,4,4], campos [V,3],
     cams: V tuples (tan_fovx, tan_fovy, cx, cy); features [P,S] or [V,P,S], colors [P,3] or [V,P,3] (or empty).
     Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
     out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
     radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once.
-    `antialiasing` applies to every view (see rasterize_gaussians)."""
+    `antialiasing` and `filter_3d` apply to every view (see rasterize_gaussians)."""
     V, P = len(cams), means3D.size(0)
     H, W = int(image_height), int(image_width)
     dev = means3D.device
@@ -465,7 +505,7 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
     pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
     out, _, rendered = _forward(True, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                 cov3D_precomp, viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered,
-                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing)
+                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing, filter_3d)
     _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
     return (rendered,) + out
 
@@ -474,7 +514,8 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
                              viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                              backward_geometry, cam_grads=False, surface=None, surface_work=None, geometry=True,
-                             appearance=(True, True, True), *, antialiasing=False, absgrad=False):
+                             appearance=(True, True, True), *, antialiasing=False, absgrad=False, filter_3d=None,
+                             opacities=None):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
@@ -484,10 +525,11 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
     one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
     rasterize_gaussians_backward, and `antialiasing` must be the forward's.  `absgrad=True`: dL_dmeans2D_abs [V,P,2]
-    is the last element, as in rasterize_gaussians_backward."""
+    is the last element, as in rasterize_gaussians_backward.  `filter_3d` and `opacities` are those of
+    rasterize_gaussians_backward."""
     grads, cam, extra = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                            dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                            backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
-                           appearance, antialiasing, absgrad)
+                           appearance, antialiasing, absgrad, filter_3d, opacities)
     return grads + cam + extra

@@ -31,7 +31,8 @@ class RasterFwdArgs(ctypes.Structure):
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
          ("binning", c_void_p), ("binning_bytes", c_size_t), ("num_rendered_host", c_void_p), ("count_ready_event", c_void_p),
          ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
-         ("antialiasing", c_int), ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+         ("filter_3d", c_void_p), ("antialiasing", c_int),
+         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class RasterBwdArgs(ctypes.Structure):
@@ -53,8 +54,8 @@ class RasterBwdArgs(ctypes.Structure):
          ("cam_work", c_void_p), ("cam_work_bytes", c_size_t),
          ("dL_dout_normal", c_void_p), ("dL_dout_surface_xyz", c_void_p), ("fwd_opacity", c_void_p), ("fwd_depth", c_void_p),
          ("cx", c_float), ("cy", c_float), ("surface_work", c_void_p), ("surface_work_bytes", c_size_t),
-         ("dL_dmeans2D_abs", c_void_p),
-         ("antialiasing", c_int), ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+         ("filter_3d", c_void_p), ("opacities", c_void_p), ("dL_dmeans2D_abs", c_void_p), ("antialiasing", c_int),
+         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class ShadeArgs(ctypes.Structure):
@@ -152,6 +153,9 @@ SYMBOLS = [
     ("r3dg_mcmc_classify", c_int, [c_int, c_void_p, c_float, c_void_p, c_size_t, c_void_p]),
     ("r3dg_mcmc_apply", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_double, c_int, c_int,
                                 ctypes.POINTER(DensifyTensor), c_void_p, c_size_t, c_void_p]),
+    ("r3dg_filter3d_tmp_bytes", c_size_t, [c_int]),
+    ("r3dg_filter3d_compute", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_size_t,
+                                      c_void_p]),
     ("r3dg_raster_fwd_det_bytes", c_size_t, [c_int]),
     ("r3dg_raster_bwd_det_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_raster_bwd_det_absgrad_bytes", c_size_t, [c_int]),

@@ -203,6 +203,7 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     if (a->P > 0 && ((a->shs == nullptr) == (a->colors_precomp == nullptr))) return R3DG_ERR_BAD_ARG;
     if (a->P > 0 && (a->cov3D_precomp == nullptr) && (a->scales == nullptr || a->rotations == nullptr)) return R3DG_ERR_BAD_ARG;
     if (a->shs && a->M > 16) return R3DG_ERR_UNSUPPORTED;
+    if (a->filter_3d && a->cov3D_precomp) return R3DG_ERR_BAD_ARG;       // the 3D filter is defined on scales
     const int V = views_of(a->V, a->view_cams, a->P);
     if (V == 0) return R3DG_ERR_BAD_ARG;
     RasterBuffers b;
@@ -272,6 +273,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (!geometry && (cam_outs != 0 || (!a->dL_dcolors && !a->dL_dfeatures && !a->dL_dsh))) return R3DG_ERR_BAD_ARG;
     if (V > 1 && a->P > 0 && a->shs && (geometry || a->dL_dsh) && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;
+    if (geometry && a->filter_3d && (a->cov3D_precomp || !a->opacities)) return R3DG_ERR_BAD_ARG;
     const bool cam = cam_outs == 3;
     if (cam && (!a->cam_work || a->cam_work_bytes < r3dg_raster_cam_grad_bytes(a->P, V))) return R3DG_ERR_BAD_ARG;
     // (appearance-only: the opacity, depth, pseudo-normal and surface-xyz cotangents have no appearance gradient)
@@ -526,6 +528,16 @@ int r3dg_mcmc_apply(int P, int n_new, const float* uniforms, const float* opacit
     const int rc = launch_mcmc_apply(P, n_new, uniforms, opacity, scaling, min_opacity, n_max, num_tensors, tensors, tmp,
                                      tmp_bytes, num_sms(), (cudaStream_t)stream);
     if (rc == 0) g_launches += 3;        // draw, source update, apply
+    return rc;
+}
+
+// ---- Mip-Splatting's 3D filter (filter3d.py) -------------------------------------------------------
+size_t r3dg_filter3d_tmp_bytes(int P) { return filter3d_tmp_bytes(P < 0 ? 0 : P); }
+int r3dg_filter3d_compute(int P, int V, const float* means3D, const float* viewmatrices, const float* intrinsics,
+                          float focal_max, float* filter_3d, void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_filter3d(P, V, means3D, viewmatrices, intrinsics, focal_max, filter_3d, tmp, tmp_bytes, num_sms(),
+                                   (cudaStream_t)stream);
+    if (rc == 0 && P > 0) g_launches += 2;        // least valid depth, finish
     return rc;
 }
 

@@ -200,6 +200,22 @@ __device__ __forceinline__ float xform_row_(const float* __restrict__ m, int r, 
     return add_(dot3_(x, m[r], y, m[4 + r], z, m[8 + r]), m[12 + r]);
 }
 
+// Mip-Splatting's 3D filter of size f on scales s (filter3d.py fold, in the same op order): s'_k = sqrt(s_k^2 + f^2)
+// replaces s in place, and the opacity factor coef = sqrt((r_0 r_1) r_2), r_k = s_k^2 / s'_k^2 (1 when s'_k = 0), is
+// returned.  The per-axis ratios do not underflow where det(Sigma) would (s ~ 1e-7).  f = 0: s' = |s|, coef = 1 (for
+// s = 0 and every s whose square is a normal float).
+__device__ __forceinline__ float filter3d_fold(float (&s)[3], float f) {
+    const float g = mul_(f, f);
+    float r[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float q = mul_(s[k], s[k]), e = add_(q, g);
+        s[k] = sqrt_(e);
+        r[k] = e == 0.0f ? 1.0f : div_(q, e);
+    }
+    return sqrt_(mul_(mul_(r[0], r[1]), r[2]));
+}
+
 // getRect (reference auxiliary.h:46-56), /16 compiled to an exact *0.0625f
 __device__ __forceinline__ void get_rect(float px, float py, int radius, int gx, int gy, int& x0,
                                          int& y0, int& x1, int& y1) {

@@ -205,6 +205,10 @@ int launch_densify_apply(int P, const int* totals, int num, const r3dg_densify_t
                          const float* scaling, const float* samples, float split_recip, const void* tmp, size_t tmp_bytes,
                          int num_sms, cudaStream_t stream);
 
+// filter3d.cu: Mip-Splatting's 3D filter sizes from the training cameras; the launcher validates before launching
+size_t filter3d_tmp_bytes(int P);
+int launch_filter3d(int P, int V, const float* means3D, const float* viewmatrices, const float* intrinsics, float F,
+                    float* out, void* tmp, size_t tmp_bytes, int sms, cudaStream_t stream);
 // mcmc.cu: MCMC densification (relocation, growth) and position noise; launchers validate before launching
 size_t mcmc_tmp_bytes(int P, int n_new);
 int launch_mcmc_noise(int P, float* xyz, const float* rotation, const float* scaling, const float* opacity, const float* z,

@@ -143,6 +143,7 @@ struct ProjParams {
     uint32_t *sort_keys, *sort_vals;      // depth-sort input (radix_sort.cu)
     uint2* rects;                         // packed tile rectangles (binning.cu)
     uint2* brects;                        // packed block rectangles (compositor pre-filter, common.cuh block_rect)
+    const float* filter_3d;               // F3D: [P] Mip-Splatting 3D filter sizes (last: the other fields keep their offsets)
 };
 
 #define PROJ_THREADS 128
@@ -166,6 +167,9 @@ __device__ __forceinline__ void load_rows_transposed(float* s, const float* __re
     }
 }
 
+// F3D: Mip-Splatting's 3D filter (common.cuh filter3d_fold) — the Gaussian is projected with the dilated scales s' and
+// its opacity is o coef; cov3D_precomp is refused by the caller.
+template <bool F3D = false>
 __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams p) {
     extern __shared__ __align__(16) float sSH[];   // SH slab ([3M][PROJ_THREADS + 1] transposed, or row-major), later the record slab
     __shared__ float sV[16], sPr[16], sCam[3];
@@ -213,7 +217,7 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
             }
         }
     }
-    float pix_x = 0.f, pix_y = 0.f, con_a = 0.f, con_b = 0.f, con_c = 0.f, aa_rho = 1.f;
+    float pix_x = 0.f, pix_y = 0.f, con_a = 0.f, con_b = 0.f, con_c = 0.f, aa_rho = 1.f, f3d_coef = 1.f;
     int my_radius = 0, x0 = 0, y0 = 0, x1 = 0, y1 = 0;
     if (alive) {
         const float hx = xform_row_(sPr, 0, px, py, pz);
@@ -227,8 +231,14 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
             for (int i = 0; i < 6; ++i) c6[i] = p.cov3D_precomp[6 * (size_t)idx + i];
         } else {
             const float4 q = *reinterpret_cast<const float4*>(p.rotations + 4 * (size_t)idx);
-            const float s3[3] = {p.scales[3 * (size_t)idx], p.scales[3 * (size_t)idx + 1], p.scales[3 * (size_t)idx + 2]};
-            cov3d_from_scale_rot(s3, p.scale_modifier, q, c6);
+            if constexpr (F3D) {
+                float s3[3] = {p.scales[3 * (size_t)idx], p.scales[3 * (size_t)idx + 1], p.scales[3 * (size_t)idx + 2]};
+                f3d_coef = filter3d_fold(s3, p.filter_3d[idx]);
+                cov3d_from_scale_rot(s3, p.scale_modifier, q, c6);
+            } else {
+                const float s3[3] = {p.scales[3 * (size_t)idx], p.scales[3 * (size_t)idx + 1], p.scales[3 * (size_t)idx + 2]};
+                cov3d_from_scale_rot(s3, p.scale_modifier, q, c6);
+            }
         }
         // computeCov2D (forward.cu:74-113), association as compiled
         const float tx = xform_row_(sV, 0, px, py, pz), ty = xform_row_(sV, 1, px, py, pz);
@@ -314,8 +324,9 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
     float4* srow = reinterpret_cast<float4*>(sSH) + (size_t)threadIdx.x * rec4n;
     __syncthreads();                                   // every thread is done with the SH slab
     if (alive) {
-        // antialiased mode: the compensated opacity o * rho is the opacity of everything downstream
-        const float op = p.antialiasing ? mul_(p.opacities[idx], aa_rho) : p.opacities[idx];
+        // antialiased mode: the compensated opacity o * rho is the opacity of everything downstream (3D filter: o coef rho)
+        const float o = F3D ? mul_(p.opacities[idx], f3d_coef) : p.opacities[idx];
+        const float op = p.antialiasing ? mul_(o, aa_rho) : o;
         p.brects[idx] = block_rect(pix_x, pix_y, con_a, con_b, con_c, op);
         srow[0] = make_float4(pix_x, pix_y, con_a, con_b);
         srow[1] = make_float4(con_c, op, tz, __int_as_float(my_radius));
@@ -483,11 +494,14 @@ int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, int
     p.sort_keys = (uint32_t*)(b.sort + b.sort_layout.keys_a);
     p.sort_vals = (uint32_t*)(b.sort + b.sort_layout.vals_a);
     p.rects = b.rects; p.brects = b.brects;
+    p.filter_3d = a.filter_3d;
     // dynamic shared memory: the SH slab (transposed fallback layout is the larger one), reused for the record slab
     size_t sh_smem = a.shs ? (size_t)3 * a.M * (PROJ_THREADS + 1) * sizeof(float) : 0;
     const size_t rec_smem = (size_t)PROJ_THREADS * b.recf * sizeof(float);
     if (rec_smem > sh_smem) sh_smem = rec_smem;
-    project_kernel<<<(a.P + PROJ_THREADS - 1) / PROJ_THREADS, PROJ_THREADS, sh_smem, stream>>>(p);
+    const int blocks = (a.P + PROJ_THREADS - 1) / PROJ_THREADS;
+    if (a.filter_3d) project_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    else project_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

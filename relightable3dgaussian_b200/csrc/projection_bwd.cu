@@ -38,6 +38,9 @@ struct ProjBwdParams {
     // ABS: this view's dL_dmeans2D_abs [P,2] (composite_bwd.cu); DET: read from det_abs (rows det_row0 + idx)
     float* dL_dmeans2D_abs;
     DetAcc det_abs;
+    // F3D: Mip-Splatting's 3D filter sizes [P] and the forward's opacities o [P] (last: the other fields keep their
+    // offsets)
+    const float *filter_3d, *opacities;
 };
 static_assert(kCamGradThreads == 128, "cam_grad_blocks() counts projection-backward CTAs");
 
@@ -129,7 +132,9 @@ __device__ __forceinline__ ViewDir view_dir(const float* m, const float* cam) {
 // behind the SH slab, and the CTA writes their sums in a fixed order to its column of p.cam_work.
 // ABS (absgrad): dL_dmeans2D_abs next to dL_dmeans2D — +0 for rows that are not live; a live row's sums the compositor
 // added in place (default mode, nothing to write) or into fixed-point accumulators (DET: read and written here).
-template <bool DET = false, bool CAM = false, bool ABS = false>
+// F3D (3D filter): the covariance chain runs on the forward's dilated scales s' (common.cuh filter3d_fold) and gives
+// dL/ds' and dL/do'; the end of the scale chain turns them into dL/ds and dL/do.
+template <bool DET = false, bool CAM = false, bool ABS = false, bool F3D = false>
 __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const ProjBwdParams p) {
     // SH rows (192 B at M=16) travel through shared memory: the CTA's [128][3M] slab of shs is ONE contiguous
     // 24 KB block, fetched by a single TMA-unit bulk copy (cp.async.bulk, mbarrier-signalled) into a row-major
@@ -187,6 +192,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
         if (!p.cov3D_precomp) {
             q4 = *reinterpret_cast<const float4*>(p.rotations + 4 * (size_t)idx);
             s3[0] = p.scales[3 * (size_t)idx]; s3[1] = p.scales[3 * (size_t)idx + 1]; s3[2] = p.scales[3 * (size_t)idx + 2];
+            if constexpr (F3D) filter3d_fold(s3, p.filter_3d[idx]);   // s' (the coefficient is formed again below)
         }
     }
     const bool fetch_sh = p.shs && nlive > 0;          // (CTA-uniform)
@@ -373,6 +379,34 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
                     dMt[rr][cc] = 2.0f * (Mm[0][rr] * dSig[cc][0] + Mm[1][rr] * dSig[cc][1] + Mm[2][rr] * dSig[cc][2]);
 #pragma unroll
             for (int k = 0; k < 3; ++k) dscale[k] = R[0][k] * dMt[k][0] + R[1][k] * dMt[k][1] + R[2][k] * dMt[k][2];
+            if constexpr (F3D) {
+                // dscale = dL/ds', dop = dL/do'.  s'_k = sqrt(s_k^2 + g) and coef = prod_j |s_j| / s'_j, so
+                //   dL/ds_k = dL/ds'_k s_k / s'_k + o dL/do' dcoef/ds_k,
+                //   dcoef/ds_k = sign(s_k) (prod_{j != k} |s_j| / s'_j) (g / e_k) / s'_k,
+                // finite for every e_k > 0 (s'_k >= sqrt(2^-149)), s_k = 0 included; s_k / s'_k = 1 and dcoef/ds_k = 0
+                // where s'_k = 0.  The scales, f and o are read again rather than kept live across the chain.
+                float sk[3], sp[3], a[3], h[3];
+                const float f = p.filter_3d[idx], g = __fmul_rn(f, f);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    sk[k] = p.scales[3 * (size_t)idx + k]; sp[k] = sk[k];
+                }
+                const float coef = filter3d_fold(sp, f);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    const float e = __fadd_rn(__fmul_rn(sk[k], sk[k]), g);     // the forward's e_k = s'_k^2 before the sqrt
+                    a[k] = sp[k] > 0.0f ? __fdiv_rn(fabsf(sk[k]), sp[k]) : 1.0f;
+                    h[k] = sp[k] > 0.0f ? copysignf(__fdiv_rn(__fdiv_rn(g, e), sp[k]), sk[k]) : 0.0f;
+                }
+                const float od = __fmul_rn(p.opacities[idx], dop);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    const float other = __fmul_rn(a[(k + 1) % 3], a[(k + 2) % 3]);
+                    const float ratio = sp[k] > 0.0f ? __fdiv_rn(sk[k], sp[k]) : 1.0f;
+                    dscale[k] = __fadd_rn(__fmul_rn(dscale[k], ratio), __fmul_rn(od, __fmul_rn(other, h[k])));
+                }
+                dop = __fmul_rn(coef, dop);
+            }
 #pragma unroll
             for (int k = 0; k < 3; ++k)
 #pragma unroll
@@ -615,7 +649,19 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     const bool abs = a.dL_dmeans2D_abs != nullptr;
     p.dL_dmeans2D_abs = abs ? a.dL_dmeans2D_abs + 2 * r : nullptr;
     p.det_abs = abs && a.deterministic ? raster_det_abs(a, (size_t)b.V * a.P) : det_acc(nullptr, 0);
-    if (abs) {
+    p.filter_3d = a.filter_3d; p.opacities = a.opacities;
+    if (a.filter_3d) {               // (r3dg_raster_backward refused it with cov3D_precomp or without opacities)
+        auto launch = [&](auto kernel, size_t smem) { kernel<<<blocks, PROJ_THREADS, smem, stream>>>(p); };
+        if (abs) {
+            if (cam && a.deterministic) launch(projection_bwd_kernel<true, true, true, true>, cam_smem);
+            else if (cam) launch(projection_bwd_kernel<false, true, true, true>, cam_smem);
+            else if (a.deterministic) launch(projection_bwd_kernel<true, false, true, true>, sh_smem);
+            else launch(projection_bwd_kernel<false, false, true, true>, sh_smem);
+        } else if (cam && a.deterministic) launch(projection_bwd_kernel<true, true, false, true>, cam_smem);
+        else if (cam) launch(projection_bwd_kernel<false, true, false, true>, cam_smem);
+        else if (a.deterministic) launch(projection_bwd_kernel<true, false, false, true>, sh_smem);
+        else launch(projection_bwd_kernel<false, false, false, true>, sh_smem);
+    } else if (abs) {
         if (cam && a.deterministic) projection_bwd_kernel<true, true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
         else if (cam) projection_bwd_kernel<false, true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
         else if (a.deterministic) projection_bwd_kernel<true, false, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);

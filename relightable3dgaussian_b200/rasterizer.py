@@ -149,13 +149,14 @@ def _surface_cotangents(ctx, g_normal, g_surface_xyz):
 def _input_grads(ctx, grads, cameras):
     """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
     three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
-    one, and for all three when none was computed.  The last two inputs, the antialiasing and absgrad flags, get None."""
+    one, and for all three when none was computed.  The last three inputs, the 3D filter (a buffer, as in
+    Mip-Splatting) and the antialiasing and absgrad flags, get None."""
     g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
     cam = (None, None, None)
     if grads[9:]:
         cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[11:14]))
     return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
-            None, None) + cam + (None, None)
+            None, None) + cam + (None, None, None)
 
 
 # the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
@@ -177,6 +178,14 @@ def _aa_kw(antialiasing):
     """The keyword that turns on the library's antialiased mode, only when it is on: an off call is the call without
     the mode."""
     return {"antialiasing": True} if antialiasing else {}
+
+
+def _f3d_kw(filter_3d, opacities=None):
+    """The keywords that turn on the library's 3D filter, only when a filter is given; the backward also takes the
+    forward's opacities."""
+    if filter_3d is None:
+        return {}
+    return {"filter_3d": filter_3d} if opacities is None else {"filter_3d": filter_3d, "opacities": opacities}
 
 
 def _absgrad_kw(ctx, kw):
@@ -201,21 +210,22 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing, absgrad):
+                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing,
+                absgrad):
         rs = raster_settings
         out = _debug_call(rs.debug, _C.rasterize_gaussians,
                           _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
                                         cov3Ds_precomp),
                           "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
                           _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad),
-                          **_aa_kw(antialiasing))
+                          **_aa_kw(antialiasing), **_f3d_kw(filter_3d))
         ctx.raster_settings = rs
         ctx.antialiasing = antialiasing
         ctx.absgrad = absgrad
         ctx.means2D = means2D if absgrad else None      # the caller's tensor object: the backward sets .absgrad on it
         ctx.num_rendered = out[0]
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
-                      out[9], sh, *out[10:13], opacities)
+                      out[9], sh, *out[10:13], opacities, filter_3d)
         return out[:10]
 
     @staticmethod
@@ -223,7 +233,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                  g_normal, g_surface_xyz, g_weights, g_radii):
         rs = ctx.raster_settings
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, radii, sh,
-         geomBuffer, binningBuffer, imgBuffer, opacities) = ctx.saved_tensors[:12]
+         geomBuffer, binningBuffer, imgBuffer, opacities, filter_3d) = ctx.saved_tensors[:13]
         g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
                                                                    g_feature)
 
@@ -241,6 +251,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         kw = _backward_mode(ctx)
         kw.update(_aa_kw(ctx.antialiasing))
         kw.update(_absgrad_kw(ctx, kw))
+        kw.update(_f3d_kw(filter_3d, opacities))
         if ex is not None:
             kw["_out"] = {"sh_factor": ex[0].factor}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
@@ -259,7 +270,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                               "forward re-run inside backward (cotangents come from the truncated first attempt)")
                 out = _C.rasterize_gaussians(*_forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales,
                                                             rotations, cov3Ds_precomp),
-                                             _min_capacity=int(ctx.num_rendered) + 4096, **_aa_kw(ctx.antialiasing))
+                                             _min_capacity=int(ctx.num_rendered) + 4096, **_aa_kw(ctx.antialiasing),
+                                             **_f3d_kw(filter_3d))
                 if surface is not None:         # the adjoint of the re-run's own surface pass
                     kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
                 grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
@@ -309,7 +321,7 @@ def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, feat
 
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
                         rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False, antialiasing=False,
-                        absgrad=False):
+                        absgrad=False, filter_3d=None):
     """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
     cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
     when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
@@ -332,15 +344,26 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     pixels of |dL/dmean2D.x| and |dL/dmean2D.y|, each pixel's term taken before the sum, in the units of
     `means2D.grad` (AbsGS; gsplat's absgrad).  Opposite pulls then no longer cancel, so the statistic of
     densify.add_densification_stats(absgrad=True) sees Gaussians that cover high-frequency detail.  Like `.grad` it
-    accumulates over backward calls; the caller resets it (`means2D.absgrad = None`).  Everything else is unchanged."""
+    accumulates over backward calls; the caller resets it (`means2D.absgrad = None`).  Everything else is unchanged.
+
+    `filter_3d` (not part of the reference surface) is Mip-Splatting's 3D smoothing filter: a [P] or [P,1] fp32 CUDA
+    tensor of per-Gaussian filter sizes f, from filter3d.compute_3d_filter over the training cameras.  Each Gaussian is
+    drawn with scales sqrt(s^2 + f^2) and opacity o * sqrt(prod_k s_k^2 / (s_k^2 + f^2)), so that no Gaussian gets
+    finer than the finest sampling any training camera gave it; zoomed-in or higher-resolution renders then show no
+    erosion or speckle.  The filter is a buffer: it gets no gradient and must not require one.  A filter of the wrong
+    length (stale after densification), on the CPU, not fp32 or not contiguous, and the combination with
+    cov3Ds_precomp, raise ValueError before anything runs.  filter3d.fold(scales, opacities, filter_3d) gives the
+    filtered Gaussians for consumers that take no filter; they render the same images."""
     global _CALL_GRAD_MODE
     rs = raster_settings
+    _C._check_filter_3d(filter_3d, means3D.shape[0], cov3Ds_precomp)
     _refuse_surface_grads_without_normals(surface_grads, rs.computer_pseudo_normal)
     _refuse_camera_grad_with_exchange(rs.viewmatrix, rs.projmatrix, rs.campos)
     _CALL_GRAD_MODE = torch.is_grad_enabled()
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
                                      scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
-                                     rs.viewmatrix, rs.projmatrix, rs.campos, bool(antialiasing), _absgrad_on(absgrad))
+                                     rs.viewmatrix, rs.projmatrix, rs.campos, filter_3d, bool(antialiasing),
+                                     _absgrad_on(absgrad))
 
 
 class GaussianRasterizer(nn.Module):
@@ -358,13 +381,14 @@ class GaussianRasterizer(nn.Module):
             return _C.mark_visible(positions, rs.viewmatrix, rs.projmatrix)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
-                rotations=None, cov3D_precomp=None, features=None):
+                rotations=None, cov3D_precomp=None, features=None, filter_3d=None):
+        """`filter_3d` (not part of the reference surface): the model's 3D filter, see rasterize_gaussians."""
         features, shs, colors_precomp, scales, rotations, cov3D_precomp = _inputs(
             means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features)
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
                                    scales, rotations, cov3D_precomp, self.raster_settings,
                                    surface_grads=self.surface_grads, antialiasing=self.antialiasing,
-                                   absgrad=self.absgrad)
+                                   absgrad=self.absgrad, filter_3d=filter_3d)
 
 
 _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
@@ -376,18 +400,20 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, surface_grads, viewmatrix, projmatrix, campos, antialiasing, absgrad):
+                settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing, absgrad):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
         out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
-                                 rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing))
+                                 rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing),
+                                 **_f3d_kw(filter_3d))
         ctx.meta = (rs, cams, antialiasing)
         ctx.absgrad = absgrad
         ctx.means2D = means2D if absgrad else None
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
-                      bg, viewmatrix, projmatrix, campos, *out[10:13])
+                      bg, viewmatrix, projmatrix, campos, *out[10:13], filter_3d,
+                      opacities if filter_3d is not None else None)
         return out[:10]
 
     @staticmethod
@@ -395,11 +421,12 @@ class _RasterizeViews(torch.autograd.Function):
                  g_weights, g_radii):
         rs, cams, antialiasing = ctx.meta
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
-         geomBuffer, binningBuffer, imgBuffer) = ctx.saved_tensors[:14]
+         geomBuffer, binningBuffer, imgBuffer, filter_3d, opacities) = ctx.saved_tensors[:16]
         g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
                                                                    g_feature)
         kw = _backward_mode(ctx)
         kw.update(_absgrad_kw(ctx, kw))
+        kw.update(_f3d_kw(filter_3d, opacities))
         if kw.get("geometry", True):
             kw.update(cam_grads=any(ctx.needs_input_grad[11:14]), surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
@@ -414,7 +441,7 @@ class _RasterizeViews(torch.autograd.Function):
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False,
-                    absgrad=False):
+                    absgrad=False, filter_3d=None):
     """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
 
     `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
@@ -427,7 +454,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
     Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
-    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing` and `absgrad` are those of
+    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing`, `absgrad` and `filter_3d` are those of
     rasterize_gaussians and apply to every view; `means2D.absgrad` is then [V,P,2], each view's own."""
     settings = list(settings)
     V = len(settings)
@@ -450,6 +477,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     P = means3D.shape[0]
     if V * P >= 1 << 30:
         raise ValueError(f"rasterize_views: V*P = {V * P} rows exceed the limit of 2^30")
+    _C._check_filter_3d(filter_3d, P, cov3D_precomp)
     if tuple(means2D.shape) != (V, P, 3):
         raise ValueError(f"rasterize_views: means2D must be [V,P,3] = {(V, P, 3)}, got {tuple(means2D.shape)}")
     for name, t in (("features", features), ("colors_precomp", colors_precomp)):
@@ -461,7 +489,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
                                  cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos,
-                                 bool(antialiasing), _absgrad_on(absgrad))
+                                 filter_3d, bool(antialiasing), _absgrad_on(absgrad))
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
