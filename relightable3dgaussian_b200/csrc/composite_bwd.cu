@@ -1,20 +1,18 @@
 // Stage 2 backward: per-tile back-to-front re-traversal (reference K10, backward.cu:401-614).
 //
 // Design notes
-//  * the reference issues 10+S global atomicAdds per contributing (pixel, Gaussian) pair.  Here a
-//    warp (8x4 pixels) first reduces its 32 per-pixel gradient rows with transposed butterflies
-//    ("reduce-scatter": ~V shuffles for V values instead of 5V), after which every lane holds one
-//    finished component and the warp adds the whole per-Gaussian gradient row with ONE reduction
-//    instruction into a packed [P][RECF] row (2-4 sectors).  The colour / feature components are
-//    all  (alpha T) * dL_dpix[c] : each lane keeps its dL_dpix in a lane-specific PERMUTED order,
-//    so that what a lane sends and what it keeps at every butterfly level sit in fixed registers —
-//    no select instructions (reduce_scatter_permuted); only the 7 geometry components pay them;
+//  * the reference issues 10+S global atomicAdds per contributing (pixel, Gaussian) pair.  Here a warp (8x4 pixels)
+//    works in two phases per sub-batch of E staged entries.  Pixel phase (lane = pixel): alpha, the tests and the T / A
+//    recurrences, and the two per-(entry, pixel) scalars every gradient component is linear in,  w = G dL_dalpha  and
+//    dcc = alpha T,  written to shared planes.  Entry phase (lane = entry): each lane sums its entry's row over the
+//    block's pixels with plain FMAs — the 6 centred moments of w (geometry), the cotangent dots of dcc (depth, colour,
+//    features) — one shuffle per accumulator joins the pixel parts, and the finished rows are added from shared memory
+//    by vector reductions that cover whole row segments (DESIGN.md §4.2);
 //  * warps are autonomous (no CTA barrier; see composite.cu): each walks ONLY the entries whose
 //    contributor bit the forward pass set for its pixel block, back to front from the block's
 //    deepest last contributor — no culling test, no record fetch, no exp() for anything else;
-//  * CTAs are launched in the order of the work the forward pass measured (cta_order_kernel), and
-//    the walk is laid out in rounds of U entries for instruction-level parallelism: the kernel is
-//    bound by per-warp latency and its heaviest warps (DESIGN.md §4.2);
+//  * CTAs are launched in the order of the work the forward pass measured (cta_order_kernel): the kernel is bound by
+//    per-warp latency and its heaviest warps (DESIGN.md §4.2);
 //  * per-pixel state is register resident (template on channel groups); the reference keeps three
 //    float[24] arrays in local memory and 36 KB of shared memory per CTA;
 //  * gradients differ from the reference only by fp32 summation order (the reference's own
@@ -26,10 +24,6 @@
 #include "kernels.h"
 
 namespace r3dg {
-
-// entries per round of the backward walk (composite_bwd_kernel): 2 for S <= 5, 1 for S > 5 (twice the accumulators:
-// registers)
-template <int NG> struct BwdIlp { static constexpr int v = NG <= 2 ? 2 : 1; };
 
 struct CompositeBwdParams {
     int W, H, gx, gy, S, recf, backward_geometry;   // gy: tile rows of one view (see CompositeFwdParams)
@@ -53,126 +47,53 @@ struct CompositeBwdParams {
     DetAcc det_abs;
 };
 
-// Sum v[i] over the 32 lanes for every i in [0,N) (N power of two, 4 <= N <= 32) with a
-// transposed butterfly; on return lane l holds the total of component (l >> (5 - log2 N)).
-template <int N>
-__device__ __forceinline__ float reduce_scatter(float (&v)[N], int lane) {
-    int m = 16;
-#pragma unroll
-    for (int n = N; n > 1; n >>= 1) {
-        const bool upper = (lane & m) != 0;
-#pragma unroll
-        for (int i = 0; i < n / 2; ++i) {
-            const float send = upper ? v[i] : v[i + n / 2];
-            const float keep = upper ? v[i + n / 2] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, m);
-        }
-        m >>= 1;
-    }
-    float r = v[0];
-#pragma unroll
-    for (int mm = 16 / N; mm > 0; mm >>= 1) r += __shfl_xor_sync(0xffffffffu, r, mm);
-    return r;
-}
-
-// U independent reduce-scatters advanced level by level together: U shuffle chains in flight instead of one (the last
-// levels of a single butterfly are one dependent SHFL -> FADD after the other).
-template <int U, int N>
-__device__ __forceinline__ void reduce_scatter_multi(float (&v)[U][N], int lane, float (&r)[U]) {
-    int m = 16;
-#pragma unroll
-    for (int n = N; n > 1; n >>= 1) {
-        const bool upper = (lane & m) != 0;
-#pragma unroll
-        for (int i = 0; i < n / 2; ++i) {
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const float send = upper ? v[u][i] : v[u][i + n / 2];
-                const float keep = upper ? v[u][i + n / 2] : v[u][i];
-                v[u][i] = keep + __shfl_xor_sync(0xffffffffu, send, m);
-            }
-        }
-        m >>= 1;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) r[u] = v[u][0];
-#pragma unroll
-    for (int mm = 16 / N; mm > 0; mm >>= 1) {
-#pragma unroll
-        for (int u = 0; u < U; ++u) r[u] += __shfl_xor_sync(0xffffffffu, r[u], mm);
-    }
-}
-
-// The same reduce-scatter without selects, for W values whose slot order the caller chose per lane: slot p of lane l
-// must hold component  p ^ (~(l >> (5 - log2 W)) & (W - 1)).  At level n every lane sends slots [0, n/2) and keeps
-// [n/2, n): with that order the kept slot i + n/2 and the partner's sent slot i are the same component.  On return
-// lane l holds the total of component  l >> (5 - log2 W)  (as reduce_scatter).
-template <int W>
-__device__ __forceinline__ float reduce_scatter_permuted(float (&x)[W]) {
-    int m = 16;
-#pragma unroll
-    for (int n = W; n > 1; n >>= 1) {
-#pragma unroll
-        for (int i = 0; i < n / 2; ++i) x[i] = x[i + n / 2] + __shfl_xor_sync(0xffffffffu, x[i], m);
-        m >>= 1;
-    }
-    float r = x[0];
-#pragma unroll
-    for (int mm = 16 / W; mm > 0; mm >>= 1) r += __shfl_xor_sync(0xffffffffu, r, mm);
-    return r;
-}
-
-template <int U, int W>
-__device__ __forceinline__ void reduce_scatter_permuted_multi(float (&x)[U][W], float (&r)[U]) {
-    int m = 16;
-#pragma unroll
-    for (int n = W; n > 1; n >>= 1) {
-#pragma unroll
-        for (int i = 0; i < n / 2; ++i) {
-#pragma unroll
-            for (int u = 0; u < U; ++u) x[u][i] = x[u][i + n / 2] + __shfl_xor_sync(0xffffffffu, x[u][i], m);
-        }
-        m >>= 1;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) r[u] = x[u][0];
-#pragma unroll
-    for (int mm = 16 / W; mm > 0; mm >>= 1) {
-#pragma unroll
-        for (int u = 0; u < U; ++u) r[u] += __shfl_xor_sync(0xffffffffu, r[u], mm);
-    }
-}
-
 // Per warp (one 8x4 pixel block): the forward pass left one contributor bit per (instance, block).  The warp streams
 // its tile's contributor bytes BACK TO FRONT, 128 instances per step, compacts the positions whose bit is set into a
 // circular queue (warp scan) and processes batches of 32 of them: every staged entry is one that some pixel of the
 // block composited in the forward pass — no culling test, no record fetch and no exp() for anything else.
-// DET (deterministic mode): each finished row component is added through the order-independent fixed-point primitive
+// A batch is processed in sub-batches of E entries, each in two phases:
+//  * pixel phase (lane = pixel): per entry G, alpha, the forward pass's tests, T and A in list order, then
+//    w = G dL_dalpha  and  dcc = gate alpha T  into the planes sW / sC [entry][pixel] (row stride 33: conflict-free);
+//  * entry phase (lane = entry): lane l sums entry l % E over pixel part l / E (E pixels, whole pixel rows) in a fixed
+//    order.  Every row component is such a sum times per-entry factors:  the two dL/dmean2D slots from the per-pixel
+//    terms  w (a dx + b dy)  and  w (c dy + b dx)  (a, b, c the conic), the conic slots from the centred moments
+//    sum w dx^2, w dx dy, w dy^2,  the opacity slot from  sum w  (dx, dy the entry's mean minus the pixel centre,
+//    exactly the pixel phase's: centred per pixel, so far-away Gaussians do not cancel), depth and channel slots from
+//    sum dcc dL_dpix.
+//    The parts are joined by shuffles, the rows are staged in shared memory (over the planes) and added by lanes that
+//    cover contiguous float4 segments of them (red.global.add.v4.f32).  Geometry slot 7 and the padding channels
+//    (>= 3 + S) are zero; a segment of padding channels only is not added.
+// DET (deterministic mode): each real row component is added through the order-independent fixed-point primitive
 // (detacc.cuh) into p.det instead of by a float atomic into p.grad, scaled by its view's exponent of the colour /
 // feature slots or of the geometry slots (det_scale_reduce).  Everything else is the same code.
 // GEOM = false (appearance-only backward, no geometry gradient requested): the same walk, CTA order and alpha / T
-// arithmetic, but only the NC colour and feature components are formed and reduced — no dL/dalpha, no A recurrence, no
-// geometry butterfly — into a narrower row of NC floats (channel c at slot c).  Every channel component goes through the
-// same butterfly as with GEOM, so each added value, and in DET mode each row total, is bitwise the full kernel's.
-// ABS (absgrad, GEOM only): each lane also takes the magnitudes |v0[0]|, |v0[1]| of its pixel's two dL/dmean2D terms
-// (0 on gated lanes) before the geometry butterfly sums the signed terms away; one more 2-wide butterfly reduces them
-// over the warp's 32 pixels, and lanes 0 and 16 add the two totals to p.abs_grad (DET: p.det_abs, class exponent
-// e_geo) once per entry.  Everything else, the gradient row included, is the same code.
+// arithmetic, but only the NC colour and feature components are formed — no dL/dalpha, no A recurrence, no geometry
+// moments — into a narrower row of NC floats (channel c at slot c).  The channel sums run the same loop as with GEOM,
+// so each added value, and in DET mode each row total, is bitwise the full kernel's.
+// ABS (absgrad, GEOM only): the entry phase also sums the magnitudes of the pixels' two dL/dmean2D terms in the order
+// of the signed sums, times |o| W/2 and |o| H/2, and adds the two totals to p.abs_grad (DET:
+// p.det_abs, class exponent e_geo) once per entry.  Everything else, the gradient row included, is the same code.
 template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true, bool ABS = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const CompositeBwdParams p) {
     static_assert(GEOM || !ABS, "absgrad needs the geometry half of the backward");
     constexpr int NC = 4 * NG;              // padded channel count {r,g,b,f...}; gradient row = 8 geometry slots + NC
     constexpr int GOFF = GEOM ? 8 : 0;      // slot of channel 0 in the gradient row (GEOM = false: no geometry slots)
-    // the NC channel components are reduced in power-of-two chunks of 16 / 8 / 4 (select-free butterflies)
-    constexpr int C16 = NC >= 16 ? 16 : 0, C8 = (NC - C16) >= 8 ? 8 : 0, C4 = NC - C16 - C8;
-    constexpr int B8 = C16, B4 = C16 + C8;
-    static_assert(C4 == 0 || C4 == 4, "channel groups come in fours");
+    constexpr int ROWF = GOFF + NC;         // floats per gradient row (p.recf with GEOM)
     constexpr int RG = 2 + NG;
-    constexpr int U = BwdIlp<NG>::v;                 // entries per round of the walk below
+    // entries per sub-batch: 16, or 8 from NG = 6 on (static shared memory stays under 48 KB); lane l of the entry
+    // phase sums entry l % E over the E pixels of part l / E
+    constexpr int E = NG <= 5 ? 16 : 8;
+    constexpr int PS = 33;                  // plane row stride
+    constexpr int SROW = 4 * ((ROWF / 4) | 1);   // staged row stride: an odd number of float4, conflict-free stores
+    static_assert(E * SROW <= 2 * E * PS, "the staged rows overlay the planes");
+    constexpr int UP = 2;                   // entries per step of the pixel phase (divides E)
     __shared__ float4 sRec[NW][RG][32];
     __shared__ uint32_t sId[NW][32];
     __shared__ uint32_t sK[NW][32];
     __shared__ uint32_t sQ[NW][R3DG_QCAP];
+    __shared__ __align__(16) float sPl[NW][2 * E * PS];   // sW = [0, E PS), sC = [E PS, 2 E PS); then the staged rows
+    __shared__ float4 sCot[NW][NG][32];                   // per pixel of the block its NC channel cotangents
+    __shared__ float sCotD[NW][32];                       // and its depth cotangent
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     constexpr int PARTS = 8 / NW;
     static_assert(PARTS == 2, "bwd_work / cta_order are per half tile");
@@ -203,46 +124,19 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     total = min(total, (int)(range.y - range.x));
     if (total == 0) return;
 
-    auto load_dpix = [&](int c) -> float {                   // cotangent of channel c of {r,g,b,f0..} at this lane's pixel
-        if (!inside) return 0.0f;
-        if (c < 3) return p.dL_dpix[(size_t)(3 * view + c) * HW + pix];
-        return c - 3 < p.S ? p.dL_dpix_f[((size_t)view * p.S + (c - 3)) * HW + pix] : 0.0f;
-    };
-    float dpix[NC];
+    float dpix[NC];                                          // cotangents of channels {r,g,b,f0..} at this lane's pixel
 #pragma unroll
-    for (int c = 0; c < NC; ++c) dpix[c] = load_dpix(c);
-    // the same cotangents in this lane's butterfly slot order (reduce_scatter_permuted), one array per chunk
-    float cst16[C16 ? C16 : 1], cst8[C8 ? C8 : 1], cst4[C4 ? C4 : 1];
-    if constexpr (C16 > 0) {
-        const int K = ~(lane >> 1) & 15;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) cst16[i] = load_dpix(i ^ K);
+    for (int c = 0; c < NC; ++c) {
+        if (!inside) dpix[c] = 0.0f;
+        else if (c < 3) dpix[c] = p.dL_dpix[(size_t)(3 * view + c) * HW + pix];
+        else dpix[c] = c - 3 < p.S ? p.dL_dpix_f[((size_t)view * p.S + (c - 3)) * HW + pix] : 0.0f;
     }
-    if constexpr (C8 > 0) {
-        const int K = ~(lane >> 2) & 7;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) cst8[i] = load_dpix(B8 + (i ^ K));
-    }
-    if constexpr (C4 > 0) {
-        const int K = ~(lane >> 3) & 3;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) cst4[i] = load_dpix(B4 + (i ^ K));
-    }
-    // which finished component this lane adds to the Gaussian's gradient row: geometry slot lane >> 2 on lanes 0 mod 4,
-    // the 16-chunk on odd lanes, the 8-chunk on lanes 2 mod 4, the 4-chunk on a free lane class (second instruction
-    // only when all three chunks exist, NG == 7, and the geometry slots take lanes 0 mod 4; without them the 4-chunk
-    // takes lanes 0 mod 8)
-    constexpr bool C4_SECOND = GEOM && C16 > 0 && C8 > 0 && C4 > 0;
-    constexpr int C4_CLASS = C16 > 0 ? (C8 > 0 ? 0 : 2) : 1;
-    int my_sel = -1, my_off = 0;
-    if ((lane & 3) == 0) { if (GEOM && (lane >> 2) != 7) { my_sel = 0; my_off = lane >> 2; } }
-    else if (C16 > 0 && (lane & 1)) { my_sel = 1; my_off = GOFF + (lane >> 1); }
-    else if (C8 > 0 && (lane & 3) == 2) { my_sel = 2; my_off = GOFF + B8 + (lane >> 2); }
-    if (C4 > 0 && !C4_SECOND && (lane & 7) == C4_CLASS) { my_sel = 3; my_off = GOFF + B4 + (lane >> 3); }
-    if (my_sel > 0 && my_off - GOFF >= 3 + p.S) my_sel = -1;    // zero padding channel
     // GEOM = false: the opacity and depth cotangents have no appearance gradient and are not read
     const float dpix_d = GEOM && inside ? p.dL_dpix_d[vpix] : 0.0f;
     const float dpix_o = GEOM && inside ? p.dL_dpix_o[vpix] : 0.0f;
+#pragma unroll
+    for (int g = 0; g < NG; ++g) sCot[warp][g][lane] = make_float4(dpix[4 * g], dpix[4 * g + 1], dpix[4 * g + 2], dpix[4 * g + 3]);
+    sCotD[warp][lane] = dpix_d;                              // (read by the entry phase after the first __syncwarp)
     const float* bg = p.bg + 3 * view;
     const float bg_dot = GEOM ? bg[0] * dpix[0] + bg[1] * dpix[1] + bg[2] * dpix[2] : 0.0f;
     const float ddelx_dx = 0.5f * p.W, ddely_dy = 0.5f * p.H;
@@ -255,10 +149,6 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     // A = sum_ch accum_rec[ch] * dL_dpix[ch] obeys the same recurrence  A <- alpha * D + (1 - alpha) * A : one FMA per
     // channel instead of four, and no per-channel state (20 registers at S = 16).  Gradients are compared at 1e-3.
     float A = 0.0f;
-    // feature channels enter dL_dalpha only when backward_geometry is set (backward.cu:563-566)
-    float dsel[NC];
-#pragma unroll
-    for (int c = 0; c < NC; ++c) dsel[c] = (c < 3 || geo) ? dpix[c] : 0.0f;
 
     // ---- contributor-mask stream, descending: word w holds instances [4w, 4w+4); lane takes word w_next - lane -------
     const uint32_t hi = lo + (uint32_t)total;                 // instances [lo, hi) matter
@@ -299,6 +189,9 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
         for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
     }
 
+    float* const sW = sPl[warp];
+    float* const sC = sPl[warp] + E * PS;
+    const int le = lane % E, part = lane / E;               // entry phase: entry and pixel part of this lane
     while (qcount > 0) {
         const int n = min(32, qcount);
         __syncwarp();
@@ -317,153 +210,170 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll
             for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
-        // Rounds of U entries.  The kernel is latency-bound, not issue-bound (fewer resident CTAs make it slower), and the
-        // heaviest pixel blocks walk hundreds of contributors one after the other,
-        // so the round is laid out for instruction-level parallelism inside the warp: (1) everything that depends only on
-        // the entry — record fetch, exp(), alpha, 1/(1-alpha), the entry's own cotangent dot D — for all U entries; (2) the
-        // two short recurrences T and A in list order; (3) gradient rows and butterflies of the U entries, advanced level
-        // by level together.  A round with fewer than U entries left re-evaluates the last one with its gate closed.
 #pragma unroll 1
-        for (int j0 = 0; j0 < n; j0 += U) {
-            int ju[U];
-            bool valid[U];
-            float dx[U], dy[U], G[U], alpha[U], inv[U], D[U];
+        for (int j0 = 0; j0 < n; j0 += E) {
+            const int ne = min(E, n - j0);
+            __syncwarp();                                   // the previous sub-batch's staged rows are added
+            // ---- pixel phase, steps of UP entries for instruction-level parallelism: (1) everything that depends only
+            // on the entry — exp(), alpha, 1/(1-alpha), the entry's own cotangent dot D — for all UP entries; (2) the two
+            // short recurrences T and A in list order; (3) the plane stores.  Entries past the sub-batch are evaluated
+            // with their gate closed.
+#pragma unroll 1
+            for (int u0 = 0; u0 < ne; u0 += UP) {
+                bool valid[UP];
+                float G[UP], alpha[UP], inv[UP], D[UP];
 #pragma unroll
-            for (int u = 0; u < U; ++u) {                                   // (1)
-                ju[u] = min(j0 + u, n - 1);
-                const int k = (int)sK[warp][ju[u]];
-                const float4 a = sRec[warp][0][ju[u]];
-                const float4 b = sRec[warp][1][ju[u]];
-                dx[u] = sub_(a.x, pxf); dy[u] = sub_(a.y, pyf);
-                const float qd = fma_(dx[u], mul_(dx[u], a.z), mul_(dy[u], mul_(dy[u], b.x)));
-                const float power = fma_(qd, -0.5f, -mul_(dy[u], mul_(dx[u], a.w)));
-                G[u] = expf(power);
-                alpha[u] = fminf(0.99f, mul_(b.y, G[u]));
-                // the same three tests as the forward pass (identical arithmetic) + "not behind this pixel's last contributor"
-                valid[u] = j0 + u < n && k < last_contributor && !(power > 0.0f) && !(alpha[u] < 1.0f / 255.0f);
-                // a skipped entry of a non-positive-definite conic can have power > 88: expf = inf, and the gated
-                // products below (0 * inf) would be NaN.  Composited entries have power <= 0, so G <= 1 is unchanged.
-                G[u] = valid[u] ? G[u] : 0.0f;
-                asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv[u]) : "f"(1.0f - alpha[u]));   // 1 - alpha in [0.01, 1]: one MUFU
-                float d = 0.0f;
+                for (int u = 0; u < UP; ++u) {                              // (1)
+                    const int j = min(j0 + u0 + u, n - 1);
+                    const int k = (int)sK[warp][j];
+                    const float4 a = sRec[warp][0][j];
+                    const float4 b = sRec[warp][1][j];
+                    const float dx = sub_(a.x, pxf), dy = sub_(a.y, pyf);
+                    const float qd = fma_(dx, mul_(dx, a.z), mul_(dy, mul_(dy, b.x)));
+                    const float power = fma_(qd, -0.5f, -mul_(dy, mul_(dx, a.w)));
+                    G[u] = expf(power);
+                    alpha[u] = fminf(0.99f, mul_(b.y, G[u]));
+                    // the same three tests as the forward pass (identical arithmetic) + "not behind this pixel's last
+                    // contributor"
+                    valid[u] = u0 + u < ne && k < last_contributor && !(power > 0.0f) && !(alpha[u] < 1.0f / 255.0f);
+                    // a skipped entry of a non-positive-definite conic can have power > 88: expf = inf, and the gated
+                    // product w (0 * inf) would be NaN.  Composited entries have power <= 0, so G <= 1 is unchanged.
+                    G[u] = valid[u] ? G[u] : 0.0f;
+                    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv[u]) : "f"(1.0f - alpha[u]));   // 1 - alpha in [0.01, 1]: one MUFU
+                    float d = 0.0f;
+                    if constexpr (GEOM) {
+                        d = fmaf(b.z, dpix_d, dpix_o);                      // depth * dL_ddepth + 1 * dL_dopacity
+                        const float4 c0 = sRec[warp][2][j], t0 = sCot[warp][0][lane];
+                        d = fmaf(c0.z, t0.z, fmaf(c0.y, t0.y, fmaf(c0.x, t0.x, d)));
+                        // feature channels enter dL_dalpha only when backward_geometry is set (backward.cu:563-566)
+                        if (geo) {
+                            d = fmaf(c0.w, t0.w, d);
+#pragma unroll
+                            for (int g = 1; g < NG; ++g) {
+                                const float4 c4 = sRec[warp][2 + g][j], t = sCot[warp][g][lane];
+                                d = fmaf(c4.w, t.w, fmaf(c4.z, t.z, fmaf(c4.y, t.y, fmaf(c4.x, t.x, d))));
+                            }
+                        }
+                    }
+                    D[u] = d;
+                }
+#pragma unroll
+                for (int u = 0; u < UP; ++u) {                              // (2) branch-free: lanes that did not composite
+                    const float gate = valid[u] ? 1.0f : 0.0f;              // the entry contribute zeros and keep their state
+                    const float Tn = T * inv[u];                            // T before this entry (backward.cu:533)
+                    sC[(u0 + u) * PS + lane] = gate * alpha[u] * Tn;        // (3)
+                    if constexpr (GEOM) {
+                        const float dL_dalpha = gate * fmaf(D[u] - A, Tn, -(T_final * inv[u]) * bg_dot);
+                        sW[(u0 + u) * PS + lane] = G[u] * dL_dalpha;
+                        if (valid[u]) { A = fmaf(alpha[u], D[u] - A, A); T = Tn; } // A <- alpha D + (1 - alpha) A
+                    } else if (valid[u]) {
+                        T = Tn;
+                    }
+                }
+            }
+            __syncwarp();
+            // ---- entry phase: lane sums entry le over pixels [part E, part E + E) (pixel rows of 8)
+            const int je = min(j0 + le, n - 1);
+            const float4 a = sRec[warp][0][je];
+            const float4 b = sRec[warp][1][je];
+            constexpr int ROWS = E / 8;
+            float sw = 0.f, s0 = 0.f, s1 = 0.f, sxx = 0.f, sxy = 0.f, syy = 0.f, sd = 0.f, ax = 0.f, ay = 0.f;
+            float sc[NC];
+#pragma unroll
+            for (int c = 0; c < NC; ++c) sc[c] = 0.0f;
+#pragma unroll 1
+            for (int rr = part * ROWS; rr < (part + 1) * ROWS; ++rr) {      // pixel rows of this lane's part
+              const float dy = sub_(a.y, (float)(by0 + rr));
+              const float* pw = sW + le * PS + 8 * rr;
+              const float* pc = sC + le * PS + 8 * rr;
+#pragma unroll 2                                                    // (more unrolling spills at 5 CTAs per SM)
+              for (int i = 0; i < 8; ++i) {
+                const int pb = 8 * rr + i;                                  // pixel of the block
+                const float c = pc[i];
                 if constexpr (GEOM) {
-                    d = fmaf(b.z, dpix_d, dpix_o);                          // depth * dL_ddepth + 1 * dL_dopacity
-#pragma unroll
-                    for (int g = 0; g < NG; ++g) {
-                        const float4 c4 = sRec[warp][2 + g][ju[u]];
-                        d = fmaf(c4.x, dsel[4 * g + 0], d);
-                        d = fmaf(c4.y, dsel[4 * g + 1], d);
-                        d = fmaf(c4.z, dsel[4 * g + 2], d);
-                        d = fmaf(c4.w, dsel[4 * g + 3], d);
-                    }
+                    const float w = pw[i], dx = sub_(a.x, (float)(bx0 + i));   // the pixel phase's dx, dy
+                    // the two dL/dmean2D terms per pixel (unfused: ABS sums their magnitudes in the same order, so that
+                    // |signed sum| <= sum of magnitudes holds bit for bit); the conic terms from centred moments
+                    const float t0 = mul_(w, fmaf(a.z, dx, mul_(a.w, dy))), t1 = mul_(w, fmaf(b.x, dy, mul_(a.w, dx)));
+                    s0 = add_(s0, t0); s1 = add_(s1, t1);
+                    const float wdx = w * dx, wdy = w * dy;
+                    sw += w;
+                    sxx = fmaf(wdx, dx, sxx); sxy = fmaf(wdx, dy, sxy); syy = fmaf(wdy, dy, syy);
+                    sd = fmaf(c, sCotD[warp][pb], sd);
+                    if constexpr (ABS) { ax = add_(ax, fabsf(t0)); ay = add_(ay, fabsf(t1)); }
                 }
-                D[u] = d;
-            }
-            float dcc[U], dL_dalpha[U];
 #pragma unroll
-            for (int u = 0; u < U; ++u) {                                   // (2) branch-free: lanes that did not composite
-                const float gate = valid[u] ? 1.0f : 0.0f;                  // the entry contribute zeros and keep their state
-                const float Tn = T * inv[u];                                // T before this entry (backward.cu:533)
-                dcc[u] = gate * alpha[u] * Tn;
+                for (int g = 0; g < NG; ++g) {
+                    const float4 t = sCot[warp][g][pb];
+                    sc[4 * g + 0] = fmaf(c, t.x, sc[4 * g + 0]);
+                    sc[4 * g + 1] = fmaf(c, t.y, sc[4 * g + 1]);
+                    sc[4 * g + 2] = fmaf(c, t.z, sc[4 * g + 2]);
+                    sc[4 * g + 3] = fmaf(c, t.w, sc[4 * g + 3]);
+                }
+              }
+            }
+#pragma unroll
+            for (int m = E; m < 32; m <<= 1) {                              // join the pixel parts
+#pragma unroll
+                for (int c = 0; c < NC; ++c) sc[c] += __shfl_xor_sync(0xffffffffu, sc[c], m);
                 if constexpr (GEOM) {
-                    dL_dalpha[u] = gate * fmaf(D[u] - A, Tn, -(T_final * inv[u]) * bg_dot);
-                    if (valid[u]) { A = fmaf(alpha[u], D[u] - A, A); T = Tn; } // A <- alpha D + (1 - alpha) A
-                } else if (valid[u]) {
-                    T = Tn;
+                    sw += __shfl_xor_sync(0xffffffffu, sw, m);
+                    s0 += __shfl_xor_sync(0xffffffffu, s0, m);
+                    s1 += __shfl_xor_sync(0xffffffffu, s1, m);
+                    sxx += __shfl_xor_sync(0xffffffffu, sxx, m);
+                    sxy += __shfl_xor_sync(0xffffffffu, sxy, m);
+                    syy += __shfl_xor_sync(0xffffffffu, syy, m);
+                    sd += __shfl_xor_sync(0xffffffffu, sd, m);
+                }
+                if constexpr (ABS) {
+                    ax += __shfl_xor_sync(0xffffffffu, ax, m);
+                    ay += __shfl_xor_sync(0xffffffffu, ay, m);
                 }
             }
-            float v0[U][8], mine[U];
-            if constexpr (!GEOM) {
-#pragma unroll
-                for (int u = 0; u < U; ++u) mine[u] = 0.0f;
+            float row[ROWF];
+            if constexpr (GEOM) {
+                const float o = b.y, ho = -0.5f * o;                        // dL_dG = o dL_dalpha
+                row[0] = mul_(-(o * ddelx_dx), s0);                         // sum dL_dG dG_ddelx W/2
+                row[1] = mul_(-(o * ddely_dy), s1);
+                row[2] = sd;
+                row[3] = sw;
+                row[4] = ho * sxx; row[5] = ho * sxy; row[6] = ho * syy;
+                row[7] = 0.0f;
             }
 #pragma unroll
-            for (int u = 0; u < U && GEOM; ++u) {                           // (3)
-                const float4 a = sRec[warp][0][ju[u]];
-                const float4 b = sRec[warp][1][ju[u]];
-                const float dL_dG = b.y * dL_dalpha[u];
-                const float gdx = G[u] * dx[u], gdy = G[u] * dy[u];
-                const float dG_ddelx = -gdx * a.z - gdy * a.w;
-                const float dG_ddely = -gdy * b.x - gdx * a.w;
-                v0[u][0] = dL_dG * dG_ddelx * ddelx_dx;
-                v0[u][1] = dL_dG * dG_ddely * ddely_dy;
-                v0[u][2] = dpix_d * dcc[u];
-                v0[u][3] = G[u] * dL_dalpha[u];
-                v0[u][4] = -0.5f * gdx * dx[u] * dL_dG;
-                v0[u][5] = -0.5f * gdx * dy[u] * dL_dG;
-                v0[u][6] = -0.5f * gdy * dy[u] * dL_dG;
-                v0[u][7] = 0.0f;
-            }
-            float av[U][2], asum[U];
-            if constexpr (ABS) {                                            // before the butterfly below overwrites v0
-#pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    av[u][0] = valid[u] ? fabsf(v0[u][0]) : 0.0f;
-                    av[u][1] = valid[u] ? fabsf(v0[u][1]) : 0.0f;
-                }
-                reduce_scatter_multi<U, 2>(av, lane, asum);                 // |x| total on lanes 0-15, |y| on 16-31
-            }
-            if constexpr (GEOM) reduce_scatter_multi<U, 8>(v0, lane, mine); // geometry slots: lanes 0 mod 4
-            if constexpr (C16 > 0) {
-                float x[U][16], t[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) x[u][i] = dcc[u] * cst16[i];
-                reduce_scatter_permuted_multi<U, 16>(x, t);
-#pragma unroll
-                for (int u = 0; u < U; ++u) if (my_sel == 1) mine[u] = t[u];
-            }
-            if constexpr (C8 > 0) {
-                float x[U][8], t[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) x[u][i] = dcc[u] * cst8[i];
-                reduce_scatter_permuted_multi<U, 8>(x, t);
-#pragma unroll
-                for (int u = 0; u < U; ++u) if (my_sel == 2) mine[u] = t[u];
-            }
-            float t4[U];
-            if constexpr (C4 > 0) {
-                float x[U][4];
-#pragma unroll
-                for (int u = 0; u < U; ++u)
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) x[u][i] = dcc[u] * cst4[i];
-                reduce_scatter_permuted_multi<U, 4>(x, t4);
-                if constexpr (!C4_SECOND) {
-#pragma unroll
-                    for (int u = 0; u < U; ++u) if (my_sel == 3) mine[u] = t4[u];
+            for (int c = 0; c < NC; ++c) row[GOFF + c] = sc[c];
+            if constexpr (ABS) {                                            // lane: pair component part & 1 of entry le
+                if (part < 2 && le < ne) {
+                    const float v = part ? mul_(fabsf(b.y) * ddely_dy, ay) : mul_(fabsf(b.y) * ddelx_dx, ax);
+                    const size_t ai = 2 * (size_t)sId[warp][j0 + le] + part;
+                    if constexpr (DET) det_add(p.det_abs, ai, v, e_geo);
+                    else atomicAdd(p.abs_grad + ai, v);
                 }
             }
+            __syncwarp();                                                   // every lane has read the planes
+            constexpr int CH = ROWF / 4, NPART = 32 / E;
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
-                if (j0 + u < n) {                                           // (warp-uniform)
-                    if constexpr (ABS) {
-                        const size_t a = 2 * (size_t)sId[warp][ju[u]] + (lane >> 4);
-                        if ((lane & 15) == 0) {
-                            if constexpr (DET) det_add(p.det_abs, a, asum[u], e_geo);
-                            else atomicAdd(p.abs_grad + a, asum[u]);
-                        }
-                    }
-                    if constexpr (DET) {
-                        size_t row;
-                        if constexpr (ABS) row = (size_t)sId[warp][ju[u]] * p.recf;
-                        else row = sId[warp][ju[u]];
-                        if constexpr (C4_SECOND) {
-                            if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) det_add(p.det, row + 8 + B4 + (lane >> 3), t4[u], e_app);
-                        }
-                        if (my_sel >= 0) det_add(p.det, row + my_off, mine[u], my_sel == 0 ? e_geo : e_app);
-                    } else {
-                        float* grow;
-                        if constexpr (ABS) grow = p.grad + (size_t)sId[warp][ju[u]] * p.recf;
-                        else grow = p.grad + sId[warp][ju[u]];
-                        if constexpr (C4_SECOND) {
-                            if ((lane & 7) == 0 && B4 + (lane >> 3) < 3 + p.S) atomicAdd(grow + 8 + B4 + (lane >> 3), t4[u]);
-                        }
-                        if (my_sel >= 0) atomicAdd(grow + my_off, mine[u]);
-                    }
+            for (int c4 = 0; c4 < CH; ++c4)
+                if (c4 % NPART == part)
+                    *reinterpret_cast<float4*>(sPl[warp] + le * SROW + 4 * c4) =
+                        make_float4(row[4 * c4], row[4 * c4 + 1], row[4 * c4 + 2], row[4 * c4 + 3]);
+            __syncwarp();
+            if constexpr (DET) {                                            // one fixed-point add per real component
+#pragma unroll 1
+                for (int i = lane; i < ne * ROWF; i += 32) {
+                    const int e = i / ROWF, s = i - e * ROWF;
+                    if ((GEOM && s == 7) || (s >= GOFF && s - GOFF >= 3 + p.S)) continue;
+                    const size_t row0 = ABS ? (size_t)sId[warp][j0 + e] * p.recf : (size_t)sId[warp][j0 + e];
+                    det_add(p.det, row0 + s, sPl[warp][e * SROW + s], s < GOFF ? e_geo : e_app);
+                }
+            } else {                                                        // 32 float4 segments per instruction
+#pragma unroll 1
+                for (int i = lane; i < ne * CH; i += 32) {
+                    const int e = i / CH, c4 = i - e * CH;
+                    if (4 * c4 >= GOFF && 4 * c4 - GOFF >= 3 + p.S) continue;   // padding channels only
+                    const size_t row0 = ABS ? (size_t)sId[warp][j0 + e] * p.recf : (size_t)sId[warp][j0 + e];
+                    atomicAdd(reinterpret_cast<float4*>(p.grad + row0) + c4,
+                              *reinterpret_cast<const float4*>(sPl[warp] + e * SROW + 4 * c4));
                 }
             }
         }
@@ -553,11 +463,9 @@ uint32_t* raster_det_scale(const RasterBuffers& b) {
     return reinterpret_cast<uint32_t*>(b.grad - (size_t)b.row_base * b.recf);     // the whole call's grad region
 }
 
-// resident CTAs per SM the register allocation is pinned to, by channel groups NG (the occupancy sweep in DESIGN.md §4.2)
-template <int NG> struct BwdOcc { static constexpr int v = NG <= 3 ? 5 : (NG <= 5 ? 4 : 3); };
-// the pin of an absgrad instantiation: BwdOcc's, except in deterministic mode at NG = 5, where the absgrad sums' fixed-
-// point adds do not fit the 128 registers of 4 CTAs per SM (ptxas spills) and 3 CTAs are resident instead
-template <int NG, bool DET> struct BwdOccAbs { static constexpr int v = DET && NG == 5 ? 3 : BwdOcc<NG>::v; };
+// resident CTAs per SM the register allocation is pinned to, by channel groups NG: the most at which no instantiation
+// (DET x GEOM x ABS) spills (DESIGN.md §4.2)
+template <int NG> struct BwdOcc { static constexpr int v = NG <= 2 ? 5 : (NG <= 4 ? 4 : 3); };
 int g_bwd_ctas = 0;             // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
 int composite_bwd_tune(const char* key, int value, int* previous) {
     if (strcmp(key, "composite_bwd_ctas") != 0) return R3DG_ERR_UNSUPPORTED;
@@ -568,7 +476,7 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
 }
 template <int NG, bool DET, bool GEOM, bool ABS = false>
 static void launch_bwd_kernel(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
-    constexpr auto kernel = composite_bwd_kernel<NG, 4, ABS ? BwdOccAbs<NG, DET>::v : BwdOcc<NG>::v, DET, GEOM, ABS>;
+    constexpr auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET, GEOM, ABS>;
     kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
