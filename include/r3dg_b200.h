@@ -56,7 +56,7 @@ typedef struct r3dg_raster_fwd_args {
     const float* features;         /* [P,S]  or NULL when S == 0 */
     const float* opacities;        /* [P] */
     const float* scales;           /* [P,3]  or NULL */
-    const float* rotations;        /* [P,4]  or NULL */
+    const float* rotations;        /* [P,4]  or NULL; 16-byte aligned (read as float4), else R3DG_ERR_BAD_ARG */
     const float* cov3D_precomp;    /* [P,6]  or NULL (exactly one of scales+rotations / cov3D) */
     const float* viewmatrix;       /* [16] world->view, stored transposed (scene/cameras.py:62) */
     const float* projmatrix;       /* [16] full projection, stored transposed */
@@ -134,7 +134,7 @@ typedef struct r3dg_raster_bwd_args {
     const float* colors_precomp;
     const float* features;
     const float* scales;
-    const float* rotations;
+    const float* rotations;        /* 16-byte aligned, as in the forward */
     const float* cov3D_precomp;
     const float* viewmatrix;
     const float* projmatrix;
@@ -155,7 +155,7 @@ typedef struct r3dg_raster_bwd_args {
     float* dL_dcov3D;              /* [P,6] */
     float* dL_dsh;                 /* [P,M,3]; may be NULL when dL_dsh_factor is given */
     float* dL_dscales;             /* [P,3] */
-    float* dL_drotations;          /* [P,4] */
+    float* dL_drotations;          /* [P,4]; 16-byte aligned (written as float4), else R3DG_ERR_BAD_ARG */
     float* dL_dsh_factor;          /* [P,3] or NULL: the view's rank-1 factor of dL_dsh, see r3dg_sh_grad_from_factors */
     /* APPEARANCE-ONLY MODE (for training with frozen geometry): every geometry output NULL — dL_dmeans2D,
      * dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dscales, dL_drotations and the three camera gradients.  The backward
@@ -334,7 +334,8 @@ size_t r3dg_bvh_trace_tmp_bytes(int P);
 /* Fused replacement of the PyTorch prologue of RayTracer.__init__ (bvh/__init__.py:29-57):
  * fills nodes i32[2P-1,5] (all -1, count column 0 for internal / 1 for leaf nodes) and aabbs
  * f32[2P-1,6] (internal: +1e5/-1e5, leaf i at row P-1+i: box of the 8 corners mu +- 3 s_a a +- ...),
- * with the same op-by-op fp32 rounding as the PyTorch expression. */
+ * with the same op-by-op fp32 rounding as the PyTorch expression.  rotations [P,4] must be 16-byte
+ * aligned (read as float4): otherwise R3DG_ERR_BAD_ARG before any launch. */
 int r3dg_bvh_leaf_aabbs(int P, const float* means3D, const float* scales, const float* rotations,
                         int32_t* nodes, float* aabbs, r3dg_stream_t stream);
 
@@ -462,7 +463,8 @@ int r3dg_compact_rows(int P, int num_tensors, const r3dg_compact_tensor* tensors
  *   samples[c |S| + k] ([2|S|,3] standard normals).  Kinds: COPY (every new row a copy), MOMENT (new
  *   rows zero), XYZ (split copies: R(q) (z * exp(s)) + x, from `rotation` [P,4] and `scaling` [P,3]),
  *   SCALING (split copies: log(exp(s) * split_recip)), ZERO (dst only: all final rows zero).
- *   At most R3DG_DENSIFY_MAX tensors; row_bytes a multiple of 4 (12 for XYZ / SCALING).
+ *   At most R3DG_DENSIFY_MAX tensors; row_bytes a multiple of 4 (12 for XYZ / SCALING).  `rotation`
+ *   is read as float4 and must be 16-byte aligned.
  * Bad arguments return R3DG_ERR_BAD_ARG before anything is launched.
  * ------------------------------------------------------------------------------------------ */
 #define R3DG_DENSIFY_MAX 48

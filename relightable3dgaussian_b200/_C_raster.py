@@ -138,7 +138,7 @@ def _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means
     colors_pv = views and colors is not None and colors.numel() != 0 and colors.dim() == 3
     background = _prep(background, "background"); means3D = _prep(means3D, "means3D"); sh = _prep(sh, "sh")
     colors = _prep(colors, "colors"); features = _prep(features, "features"); scales = _prep(scales, "scales")
-    rotations = _prep(rotations, "rotations"); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
+    rotations = _lib.aligned16(_prep(rotations, "rotations")); cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp")
     viewmatrix = _prep(viewmatrix, "viewmatrix"); projmatrix = _prep(projmatrix, "projmatrix")
     campos = _prep(campos, "campos")
     a.background = _lib.ptr(background); a.means3D = _lib.ptr(means3D); a.shs = _lib.ptr(sh)

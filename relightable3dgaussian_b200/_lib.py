@@ -242,6 +242,15 @@ def f32(t):
     return t.detach().float().contiguous()
 
 
+def aligned16(t):
+    """`t` itself when its data is 16-byte aligned (or it is absent / empty), else an aligned contiguous copy.  The
+    library reads quaternions as float4 and refuses a misaligned `rotations`, such as a contiguous view at a storage
+    offset that is not a multiple of 4 floats."""
+    if t is None or t.numel() == 0 or t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.contiguous_format)
+
+
 def det_workspace(args, nbytes, device):
     """Under torch.are_deterministic_algorithms_enabled(), read at call time: a workspace of `nbytes` for the
     library's deterministic mode, entered into the argument struct `args` (deterministic, det_work, det_work_bytes).

@@ -38,6 +38,9 @@ inline void prof_mark(bool fwd, int i, cudaStream_t s) {
     if (call >= g_prof.max_calls) return;
     cudaEventRecord(g_prof.at(call, i), s);
 }
+// The kernels read each quaternion (rotations) and write each dL_drotations row as one float4: a [P,4] array whose
+// base is not 16-byte aligned (a contiguous view at an odd storage offset) is refused before anything is launched.
+inline bool misaligned16(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 15u) != 0; }
 
 // ---- the rasterizer's work buffers: regions in this order, each 256-byte aligned ---------------------------------
 // V views: V rows per Gaussian (row v * P + g), one header and one depth-sort region per view.  V = 1 is the one-view
@@ -202,6 +205,7 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     if (a->S > R3DG_MAX_S_FWD) return R3DG_ERR_UNSUPPORTED;
     if (a->P > 0 && ((a->shs == nullptr) == (a->colors_precomp == nullptr))) return R3DG_ERR_BAD_ARG;
     if (a->P > 0 && (a->cov3D_precomp == nullptr) && (a->scales == nullptr || a->rotations == nullptr)) return R3DG_ERR_BAD_ARG;
+    if (misaligned16(a->rotations)) return R3DG_ERR_BAD_ARG;
     if (a->shs && a->M > 16) return R3DG_ERR_UNSUPPORTED;
     if (a->filter_3d && a->cov3D_precomp) return R3DG_ERR_BAD_ARG;       // the 3D filter is defined on scales
     const int V = views_of(a->V, a->view_cams, a->P);
@@ -259,6 +263,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (a->S > R3DG_MAX_S_BWD) return R3DG_ERR_UNSUPPORTED;
     const int V = views_of(a->V, a->view_cams, a->P);
     if (V == 0) return R3DG_ERR_BAD_ARG;
+    if (misaligned16(a->rotations) || misaligned16(a->dL_drotations)) return R3DG_ERR_BAD_ARG;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S))) return R3DG_ERR_BAD_ARG;
     const int cam_outs = (a->dL_dviewmatrix != nullptr) + (a->dL_dprojmatrix != nullptr) + (a->dL_dcampos != nullptr);
     // appearance-only mode: every geometry output NULL (the six per-Gaussian ones and the camera gradients).  P = 0
@@ -399,6 +404,7 @@ size_t r3dg_bvh_trace_tmp_bytes(int P) { return bvh_packets_bytes(P); }
 
 int r3dg_bvh_leaf_aabbs(int P, const float* means3D, const float* scales, const float* rotations,
                         int32_t* nodes, float* aabbs, r3dg_stream_t stream) {
+    if (misaligned16(rotations)) return R3DG_ERR_BAD_ARG;
     g_launches += P > 0 ? 1 : 0;
     return launch_bvh_leaf_aabbs(P, means3D, scales, rotations, nodes, aabbs, (cudaStream_t)stream);
 }
@@ -503,6 +509,7 @@ int r3dg_densify_classify(int P, const float* xyz_gradient_accum, const float* n
 int r3dg_densify_apply(int P, const int* totals, int num_tensors, const r3dg_densify_tensor* tensors, const float* rotation,
                        const float* scaling, const float* samples, float split_recip, const void* tmp, size_t tmp_bytes,
                        r3dg_stream_t stream) {
+    if (misaligned16(rotation)) return R3DG_ERR_BAD_ARG;
     const int rc = launch_densify_apply(P, totals, num_tensors, tensors, rotation, scaling, samples, split_recip, tmp, tmp_bytes,
                                         num_sms(), (cudaStream_t)stream);
     if (rc == 0 && P > 0 && num_tensors > 0) g_launches += 1;

@@ -214,7 +214,8 @@ def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, max
         descs.append(d)
     arr = (_lib.DensifyTensor * len(descs))(*descs)
     tot_c = (ctypes.c_int * 7)(*tot[:7])
-    _lib.call("r3dg_densify_apply", dev, P, tot_c, len(descs), arr, byname["rotation"].data_ptr(), byname["scaling"].data_ptr(),
+    rot = _lib.aligned16(byname["rotation"].detach())
+    _lib.call("r3dg_densify_apply", dev, P, tot_c, len(descs), arr, rot.data_ptr(), byname["scaling"].data_ptr(),
               z.data_ptr(), split_recip, tmp.data_ptr(), tmp.numel(), what="densify_apply")
     opt = model.optimizer
     for g, name, p, st, np_, moms in new:

@@ -63,7 +63,7 @@ class RayTracer:
         dev = means3D.device
         nodes = torch.empty((2 * P - 1, 5), dtype=torch.int32, device=dev)
         aabbs = torch.empty((2 * P - 1, 6), dtype=torch.float32, device=dev)
-        m, s, r = _lib.f32(means3D), _lib.f32(scales), _lib.f32(rotations)
+        m, s, r = _lib.f32(means3D), _lib.f32(scales), _lib.aligned16(_lib.f32(rotations))
         _lib.call("r3dg_bvh_leaf_aabbs", dev, P, m.data_ptr(), s.data_ptr(), r.data_ptr(), nodes.data_ptr(), aabbs.data_ptr(),
                   what="RayTracer leaf boxes")
         self.tree, self.aabb, self.morton = _C.create_bvh(m, s, r, nodes, aabbs)

@@ -14,9 +14,11 @@ cotangents, in the kernel's call and here alike, so that they add nothing to any
 
 Outputs (those of a colors_precomp + cov3D_precomp call): dL_dcolors, dL_dfeatures and dL_dopacity as the row holds
 them; dL_dmeans2D in the units the kernel writes (0.5 W, 0.5 H per pixel); dL_dcov3D through the fp64 projection of
-cov3D to the conic (aa_oracle.cov2d and the 0.3 px^2 dilation).  dL/dalpha of a pair comes from autograd of the fp64
-composite with alpha as a leaf; dalpha / d(mean2D, conic, opacity) is the closed form the reference differentiates
-(alpha = opacity G, G = exp(power): the 0.99 clamp is not differentiated)."""
+cov3D to the conic (aa_oracle.cov2d and the 0.3 px^2 dilation).  For the projection's truth (proj64.py) also the rest
+of the record's gradient: dL_ddepth, and dL_dconic (a, b, c; b the true derivative of the symmetric off-diagonal).
+dL/dalpha of a pair comes from autograd of the fp64 composite with alpha as a leaf; dalpha / d(mean2D, conic, opacity)
+is the closed form the reference differentiates (alpha = opacity G, G = exp(power): the 0.99 clamp is not
+differentiated)."""
 import torch
 
 import aa_oracle
@@ -112,7 +114,8 @@ def row_truth(st, walks, cots, bg, W, H, S, jac=None):
     P = st["means2D"].shape[0]
     dev = st["means2D"].device
     planes = torch.cat([c.reshape(c.shape[0], -1) for c in cots if c.numel()], 0).double()    # [3 + 2 + S, HW]
-    width = {"dL_dcolors": 3, "dL_dfeatures": S, "dL_dopacity": 1, "dL_dmeans2D": 2, "dL_dcov3D": 6}
+    width = {"dL_dcolors": 3, "dL_dfeatures": S, "dL_dopacity": 1, "dL_dmeans2D": 2, "dL_dcov3D": 6, "dL_dconic": 3,
+             "dL_ddepth": 1}
     out = {k: (torch.zeros(P, n, dtype=torch.float64, device=dev), torch.zeros(P, n, dtype=torch.float64, device=dev))
            for k, n in width.items() if n}
     for wk in walks:
@@ -127,6 +130,7 @@ def row_truth(st, walks, cots, bg, W, H, S, jac=None):
         terms = {"dL_dcolors": ccol, "dL_dopacity": (dA * wk.G)[v][:, None]}
         if S:
             terms["dL_dfeatures"] = w[:, None] * cot[:, 5:][:, None, :].expand(-1, v.shape[1], -1)[v]
+        terms["dL_ddepth"] = w[:, None] * cot[:, 4:5][:, None, :].expand(-1, v.shape[1], -1)[v]
         dpow = (dA * wk.op * wk.G)[v]
         dx, dy = wk.dx[v], wk.dy[v]
         ca, cb, cc = wk.ca[v], wk.cb[v], wk.cc[v]
@@ -135,8 +139,9 @@ def row_truth(st, walks, cots, bg, W, H, S, jac=None):
         # a term that is itself a sum of products counts the magnitudes of its products
         mags = {"dL_dmeans2D": dpow.abs()[:, None] * torch.stack([((ca * dx).abs() + (cb * dy).abs()) * (0.5 * W),
                                                                    ((cc * dy).abs() + (cb * dx).abs()) * (0.5 * H)], 1)}
+        dconic = torch.stack([-0.5 * dx * dx, -dx * dy, -0.5 * dy * dy], 1) * dpow[:, None]
+        terms["dL_dconic"] = dconic
         if jac is not None:
-            dconic = torch.stack([-0.5 * dx * dx, -dx * dy, -0.5 * dy * dy], 1) * dpow[:, None]
             J = jac[ids]
             terms["dL_dcov3D"] = torch.einsum("nk,nks->ns", dconic, J)
             mags["dL_dcov3D"] = torch.einsum("nk,nks->ns", dconic.abs(), J.abs())

@@ -210,6 +210,28 @@ def test_bad_arguments_are_rejected_without_touching_the_gpu():
         assert debug_copy(id_, 1 << 20, 0) == -1, id_
 
 
+def test_misaligned_rotations_are_refused_before_any_launch():
+    """rotations is read, and dL_drotations written, as float4: a base that is not 16-byte aligned is refused.  The
+    aligned twin of each refused call is one that returns 0 without launching anything (P = 0)."""
+    lib = _lib.load()
+    odd = FAKE + 4
+    a = _lib.RasterFwdArgs()
+    a.P, a.S, a.W, a.H = 100, 0, 64, 48
+    a.shs, a.scales, a.rotations = FAKE, FAKE, odd
+    assert lib.r3dg_raster_forward(ctypes.byref(a), None) == -10001
+    for field in ("rotations", "dL_drotations"):
+        for ptr, want in ((odd, -10001), (FAKE + 8, -10001), (FAKE, 0)):
+            b = _lib.RasterBwdArgs()
+            b.P, b.S, b.W, b.H = 0, 5, 64, 48
+            setattr(b, field, ptr)
+            assert lib.r3dg_raster_backward(ctypes.byref(b), None) == want, (field, hex(ptr))
+    for ptr, want in ((odd, -10001), (FAKE, 0)):
+        assert lib.r3dg_bvh_leaf_aabbs(0, None, None, ptr, None, None, None) == want
+        totals = (ctypes.c_int * 7)()
+        assert lib.r3dg_densify_apply(0, totals, 0, None, ptr, None, None, 0.625, FAKE, lib.r3dg_densify_tmp_bytes(0),
+                                      None) == want
+
+
 def test_tune_keys_and_error_codes():
     """r3dg_tune: every documented key round-trips, unknown keys / out-of-range values are refused (host state only)."""
     lib = _lib.load()
