@@ -728,6 +728,40 @@ int r3dg_tv_forward(int B, int H, int W, const float* x, float* out, void* tmp, 
 int r3dg_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, float* dL_dx, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Bilateral-grid colour correction (Wang et al., SIGGRAPH 2024; gsplat's BilateralGrid / slice), a
+ * per-image learnable, locally affine colour transform used during training only.
+ * grids [G,12,L,GY,GX] (gsplat's layout), rgb / out / dL_dout / dL_drgb [N,3,H,W], all contiguous;
+ * image_ids a DEVICE int32[N], each in [0, G) (not checked on the device: the caller validates them).
+ * For pixel (px, py) of image n with colour (r, g, b):
+ *   ix = (px + 0.5) (GX-1) / W, iy = (py + 0.5) (GY-1) / H, iz = (0.299 r + 0.587 g + 0.114 b) (L-1),
+ *   each clamped to [0, size-1] (F.grid_sample, align_corners=True, padding_mode="border");
+ *   A[12] = trilinear interpolation of grids[image_ids[n]] at (ix, iy, iz), as nested lerps
+ *           v0 + t (v1 - v0), x then y then z (a constant grid gives its value exactly; the identity
+ *           grid [1,0,0,0, 0,1,0,0, 0,0,1,0] returns rgb bit for bit);
+ *   out_c = A[4c] r + A[4c+1] g + A[4c+2] b + A[4c+3].
+ *   r3dg_bilagrid_backward: dL_drgb = A^T dL_dout + (dL/diz) (L-1) (0.299, 0.587, 0.114), the luma
+ *     term 0 where the unclamped iz <= 0 or >= L-1 (torch's border rule); dL_dgrids = the sum over
+ *     every pixel of every image with that id of the trilinear weight times dL/dout_c (r, g, b, 1)_j,
+ *     written in full (0 for ids no image uses).  Either output may be NULL, not both; dL_dgrids
+ *     needs `tmp` of r3dg_bilagrid_tmp_bytes (0 for an invalid shape): per 32x32-pixel tile one
+ *     partial sub-grid.
+ * Bitwise reproducible run to run, with no float atomics and no host synchronisation (so also
+ * under torch.use_deterministic_algorithms).  1 launch forward; 1 backward, 2 with dL_dgrids.
+ * R3DG_ERR_BAD_ARG for G, N, H or W <= 0, GX, GY or L < 2, a NULL pointer the call needs or too
+ * small a tmp; R3DG_ERR_UNSUPPORTED for N > 65535, H*W >= 2^31, H or W > 2^20, GX or GY > 1024,
+ * L > 16, G*12*L*GY*GX >= 2^31, or when the sub-grid one 32x32 tile touches, staged in shared
+ * memory, may exceed 1024 nodes: (min(GX, floor(31 (GX-1) / W) + 3)) (min(GY, floor(31 (GY-1) / H)
+ * + 3)) L > 1024.  gsplat's 16x16x8 grid fits at W, H >= 52 (5 x 5 x 8 = 200 nodes from 156 px up).
+ * Nothing is launched on an error.
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_bilagrid_tmp_bytes(int G, int N, int H, int W, int GX, int GY, int L);
+int r3dg_bilagrid_forward(int G, int N, int H, int W, int GX, int GY, int L, const float* grids, const int* image_ids,
+                          const float* rgb, float* out, r3dg_stream_t stream);
+int r3dg_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, const float* grids, const int* image_ids,
+                           const float* rgb, const float* dL_dout, float* dL_drgb, float* dL_dgrids, void* tmp,
+                           size_t tmp_bytes, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optimiser step (SURVEY.md §8f next #3).  Replaces, for all parameter groups at once, the
  * per-group `torch.optim.Adam(l, lr=0.0, eps=1e-15).step()` of scene/gaussian_model.py:489,495-497
  * (torch 1.12.1 torch/optim/adam.py:_single_tensor_adam: no weight decay, no amsgrad, no

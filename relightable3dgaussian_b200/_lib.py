@@ -173,6 +173,9 @@ SYMBOLS = [
     ("r3dg_tv_tmp_bytes", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_tv_forward", c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("r3dg_tv_backward", c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    ("r3dg_bilagrid_tmp_bytes", c_size_t, [c_int] * 7),
+    ("r3dg_bilagrid_forward", c_int, [c_int] * 7 + [c_void_p] * 5),
+    ("r3dg_bilagrid_backward", c_int, [c_int] * 7 + [c_void_p] * 7 + [c_size_t, c_void_p]),
     ("r3dg_adam_step", c_int, [c_int, ctypes.POINTER(AdamTensor), c_void_p]),
     ("r3dg_launch_count", ctypes.c_ulonglong, []),
     ("r3dg_tune", c_int, [ctypes.c_char_p, c_int, ctypes.POINTER(c_int)]),

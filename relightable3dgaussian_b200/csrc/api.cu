@@ -597,6 +597,25 @@ int r3dg_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, 
     return rc;
 }
 
+// ---- bilateral-grid colour correction (bilagrid.py) ------------------------------------------------
+size_t r3dg_bilagrid_tmp_bytes(int G, int N, int H, int W, int GX, int GY, int L) {
+    return bilagrid_tmp_bytes(G, N, H, W, GX, GY, L);
+}
+int r3dg_bilagrid_forward(int G, int N, int H, int W, int GX, int GY, int L, const float* grids, const int* image_ids,
+                          const float* rgb, float* out, r3dg_stream_t stream) {
+    const int rc = launch_bilagrid_forward(G, N, H, W, GX, GY, L, grids, image_ids, rgb, out, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 1;
+    return rc;
+}
+int r3dg_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, const float* grids, const int* image_ids,
+                           const float* rgb, const float* dL_dout, float* dL_drgb, float* dL_dgrids, void* tmp,
+                           size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_bilagrid_backward(G, N, H, W, GX, GY, L, grids, image_ids, rgb, dL_dout, dL_drgb, dL_dgrids, tmp,
+                                            tmp_bytes, (cudaStream_t)stream);
+    if (rc == 0) g_launches += dL_dgrids ? 2 : 1;        // tiles (+ partial reduction)
+    return rc;
+}
+
 namespace {
 __global__ void unpack_rec_kernel(int P, int recf, int what, const float* __restrict__ rec,
                                   const uint32_t* __restrict__ tiles, float* __restrict__ dst) {

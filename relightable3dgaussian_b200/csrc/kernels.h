@@ -238,4 +238,12 @@ size_t tv_tmp_bytes(int B, int H, int W);
 int launch_tv_forward(int B, int H, int W, const float* x, float* out, void* tmp, size_t tmp_bytes, cudaStream_t stream);
 int launch_tv_backward(int B, int H, int W, const float* x, const float* dL_dout, float* dL_dx, cudaStream_t stream);
 
+// bilagrid.cu: bilateral-grid slice and its gradients; both launchers validate every argument before launching anything
+size_t bilagrid_tmp_bytes(int G, int N, int H, int W, int GX, int GY, int L);
+int launch_bilagrid_forward(int G, int N, int H, int W, int GX, int GY, int L, const float* grids, const int* ids,
+                            const float* rgb, float* out, cudaStream_t stream);
+int launch_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, const float* grids, const int* ids,
+                             const float* rgb, const float* dL_dout, float* dL_drgb, float* dL_dgrids, void* tmp,
+                             size_t tmp_bytes, cudaStream_t stream);
+
 }  // namespace r3dg
