@@ -8,8 +8,9 @@
 //  * stream compaction instead of per-warp culling: the binning scatter leaves one pre-filter byte
 //    per (tile, Gaussian) instance; a warp streams the bytes 128 instances per step, compacts the
 //    positions whose bit for ITS block is set into a circular queue and composites batches of 32
-//    queued entries (id -> packed record prefetched one batch ahead, staged in a warp-private
-//    shared-memory slab, exact ellipse / block test once per entry by the lane that staged it);
+//    queued entries (id -> packed record prefetched one batch ahead, exact ellipse / block test once
+//    per entry by the lane that holds it, the accepted entries compacted in list order into a
+//    warp-private shared-memory slab);
 //  * the kernel is bound by per-warp latency and by its heaviest warps, not by issue slots
 //    (DESIGN.md §4.2): entries are composited in rounds of U whose alpha evaluations
 //    are in flight together, the sequential part is branch-free (predicated FMAs);
@@ -67,7 +68,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
     __shared__ __align__(16) float4 sRec[BULK ? 1 : NW][BULK ? 1 : RG][BULK ? 1 : 32];   // this warp's current 32-entry batch, SoA
     __shared__ __align__(16) float4 sRecB[BULK ? NW : 1][BULK ? 2 : 1][BULK ? 32 : 1][BULK ? RG : 1];   // BULK: [stage][entry][group]
     __shared__ __align__(8) uint64_t sBar[NW][2];
-    __shared__ uint32_t sId[NW][32];
+    __shared__ uint32_t sId[NW][32];                 // slab slot -> Gaussian id
+    __shared__ uint32_t sPos[NW][32];                // slab slot -> list position (relative to the tile's range)
     __shared__ uint32_t sQ[NW][R3DG_QCAP];           // queued list positions (relative to the tile's range)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     constexpr int PARTS = 8 / NW;
@@ -151,22 +153,35 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
 
     uint32_t composited = 0u;                                           // entries this warp composited = its backward twin's iterations
     bool all_done = __all_sync(0xffffffffu, done);
+    constexpr int U = NG <= 2 ? 4 : 2;                                  // entries per round of the loop below
     while (qcount > 0 && !all_done) {
         const int n = min(32, qcount);
         const uint32_t mypos = q[(qhead + lane) & (R3DG_QCAP - 1)];     // valid for lane < n
-        __syncwarp();
-        sId[warp][lane] = id_cur;
-        if (!BULK) {
-#pragma unroll
-            for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = r[g];
-        }
         // second, exact filter — each lane applies round 1's exact-conservative ellipse / rectangle test to ITS OWN staged
         // entry (one evaluation per entry): the block rectangle is conservative, the exact test drops the (warp, entry)
         // pairs whose ellipse misses the block, and every pair dropped here saves the alpha evaluation of the loop below
         uint32_t word;
         if (BULK) word = n == 32 ? 0xffffffffu : ((1u << n) - 1u);       // (records are not in registers in this variant)
         else word = __ballot_sync(0xffffffffu, lane < n && touch_block(r[0], r[1], (float)bx0, (float)by0));
-        const int h0 = qhead;
+        // the accepted entries are compacted in list order: entry k of the loop below is slab slot k (BULK: every entry
+        // is accepted and its bulk copy already sits at slot k = lane).  sId / sPos map a slot back to its Gaussian and
+        // its list position.  Slots [n_acc, n_acc + U) get a zero record: opacity 0 gives alpha 0 < 1/255, so a round
+        // running past n_acc fails the per-pixel test with finite values and no extra predicate.
+        const int n_acc = __popc(word);
+        const int k = __popc(word & ((1u << lane) - 1u));
+        __syncwarp();
+        if ((word >> lane) & 1u) {
+            sId[warp][k] = id_cur;
+            sPos[warp][k] = mypos;
+            if (!BULK) {
+#pragma unroll
+                for (int g = 0; g < RG; ++g) sRec[warp][g][k] = r[g];
+            }
+        }
+        if (!BULK && lane >= n_acc && lane < n_acc + U) {
+#pragma unroll
+            for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
         qhead = (qhead + n) & (R3DG_QCAP - 1);
         qcount -= n;
         while (qcount < 64 && w_next < w_end) scan_step();
@@ -181,29 +196,22 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
 #pragma unroll
             for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
-        uint32_t cw = 0u;                                               // bit j: entry j was composited by some pixel
-        int last_j = -1;                                                // this pixel's last accepted entry of the batch
-        int my_wsum = 0;                                                // lane j keeps the warp's weight sum of entry j
+        int last_k = -1;                                                // this pixel's last accepted entry of the batch
+        int my_wsum = 0;                                                // lane k keeps the warp's weight sum of entry k
         // U staged entries per round.  The alpha evaluations (record fetch, quadratic form, exp — two thirds of the
         // work) depend neither on one another nor on the pixel's state, so all U are issued back to back: U dependency
         // chains in flight per warp instead of one.  Only the short transmittance recurrence that follows is sequential,
         // in list order, with exactly the reference's arithmetic.  This is what bounds the kernel: the heaviest pixel
         // blocks composite many entries one after the other, and while the light tiles drain the machine those few
-        // warps decide the makespan (DESIGN.md §4.2).  A round with fewer than U
-        // entries left re-evaluates the last one, masked out.  U = 4 for S <= 5, 2 for S > 5 (more accumulators per
-        // pixel: registers).
-        constexpr int U = NG <= 2 ? 4 : 2;
-        while (word) {
-            int jj[U];
+        // warps decide the makespan (DESIGN.md §4.2).  U = 4 for S <= 5, 2 for S > 5 (more accumulators per pixel:
+        // registers).
+        for (int k0 = 0; k0 < n_acc; k0 += U) {
             bool pv[U];
             float al[U], om[U], dep[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) {                                // (1) independent: alpha of U entries
-                const bool have = word != 0u;
-                jj[u] = have ? __ffs(word) - 1 : jj[u ? u - 1 : 0];
-                word &= word - 1u;
-                const float4 a = BULK ? sRecB[warp][stage][jj[u]][0] : sRec[warp][0][jj[u]];
-                const float4 b = BULK ? sRecB[warp][stage][jj[u]][1] : sRec[warp][1][jj[u]];
+                const float4 a = BULK ? sRecB[warp][stage][k0 + u][0] : sRec[warp][0][k0 + u];
+                const float4 b = BULK ? sRecB[warp][stage][k0 + u][1] : sRec[warp][1][k0 + u];
                 const float dx = sub_(a.x, pxf), dy = sub_(a.y, pyf);
                 // power = -0.5f*(ca*dx*dx + cc*dy*dy) - cb*dx*dy  (forward.cu:344) as compiled
                 const float qd = fma_(dx, mul_(dx, a.z), mul_(dy, mul_(dy, b.x)));
@@ -211,7 +219,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
                 al[u] = fminf(0.99f, mul_(b.y, expf(power)));
                 om[u] = sub_(1.0f, al[u]);
                 dep[u] = b.z;
-                pv[u] = have && !(power > 0.0f) && !(al[u] < 1.0f / 255.0f);
+                // BULK has no zero-record padding: its slots past n_acc hold whatever the last copy left there
+                pv[u] = (!BULK || k0 + u < n_acc) && !(power > 0.0f) && !(al[u] < 1.0f / 255.0f);
             }
             int wq[U];
 #pragma unroll
@@ -224,12 +233,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
                 const float w = mul_(T, al[u]);
 #pragma unroll
                 for (int g = 0; g < NG; ++g) {
-                    const float4 c = BULK ? sRecB[warp][stage][jj[u]][2 + g] : sRec[warp][2 + g][jj[u]];
+                    const float4 c = BULK ? sRecB[warp][stage][k0 + u][2 + g] : sRec[warp][2 + g][k0 + u];
                     fma4_if(valid, w, c, C[4 * g + 0], C[4 * g + 1], C[4 * g + 2], C[4 * g + 3]);
                 }
                 fma_add_if(valid, w, dep[u], Dp, Op);
                 T = valid ? test_T : T;
-                last_j = valid ? jj[u] : last_j;
+                last_k = valid ? k0 + u : last_k;
                 // w in [0,1) in 2^-24 fixed point for the out_weights statistic (below); >= 6 whenever the entry was accepted
                 wq[u] = valid ? __float2int_rn(w * 16777216.0f) : 0;
             }
@@ -237,30 +246,26 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             for (int u = 0; u < U; ++u) {                                // (3) independent again: per-entry warp sums
                 // sum over the warp's pixels of w for out_weights: one integer REDUX instead of a 5-step float shuffle tree
                 // (error <= 1e-6 per warp, far below the reference's own atomic-order noise on this statistic); non-zero
-                // exactly when some pixel accepted the entry.  Lane j keeps entry j's sum: ONE atomic instruction per batch.
+                // exactly when some pixel accepted the entry.  Lane k keeps entry k's sum: ONE atomic instruction per batch.
                 const int wsum = __reduce_add_sync(0xffffffffu, wq[u]);
-                if (wsum != 0) {
-                    cw |= 1u << jj[u];
-                    if (lane == jj[u]) my_wsum = wsum;
-                }
+                if (lane == k0 + u) my_wsum = wsum;
             }
             if (__all_sync(0xffffffffu, done)) { all_done = true; break; }      // once per round: entries after the last
         }                                                                        // pixel finished change nothing (valid needs !done)
-        if (last_j >= 0) last_contributor = q[(h0 + last_j) & (R3DG_QCAP - 1)] + 1u;     // 1-based position in the tile list
+        if (last_k >= 0) last_contributor = sPos[warp][last_k] + 1u;    // 1-based position in the tile list
+        const uint32_t cw = __ballot_sync(0xffffffffu, my_wsum != 0);   // bit k: entry k was composited by some pixel
         if (my_wsum != 0) {
             const uint32_t id = sId[warp][lane];
             if constexpr (DET) det_red_u64(p.det_weights + id, (uint64_t)(uint32_t)my_wsum);   // my_wsum > 0
             else atomicAdd(&p.out_weights[id], (float)my_wsum * (1.0f / 16777216.0f));
             // the row was composited: its gradient row is zeroed and read in the backward (no byte atomics: OR the word)
             atomicOr(&p.clamped32[id >> 2], kComposited << (8 * (id & 3u)));
+            // contributor bit for the backward pass: one fire-and-forget atomic per composited entry
+            const uint32_t e = lo + sPos[warp][lane];
+            atomicOr(&p.cmask32[e >> 2], 1u << (8 * (e & 3u) + wb));
         }
         stage ^= 1;
         composited += (uint32_t)__popc(cw);
-        // contributor bits for the backward pass: one fire-and-forget atomic per composited entry
-        if ((cw >> lane) & 1u) {
-            const uint32_t e = lo + mypos;
-            atomicOr(&p.cmask32[e >> 2], 1u << (8 * (e & 3u) + wb));
-        }
     }
     if (lane == 0 && composited) atomicMax(&p.bwd_work[blockIdx.x % PARTS + PARTS * tile], composited);
     if (inside) {
