@@ -45,6 +45,9 @@ size_t r3dg_raster_img_n_contrib_offset(int W, int H);
 size_t r3dg_raster_views_geom_bytes(int P, int S, int V);
 size_t r3dg_raster_views_img_bytes(int W, int H, int V);
 size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V);
+/* The geometry buffer of a ray-depth call (r3dg_raster_fwd_args.ray_depth) of V views: its records and gradient rows
+ * hold 4 more floats per Gaussian and view.  V below 1 is sized as 1. */
+size_t r3dg_raster_ray_depth_geom_bytes(int P, int S, int V);
 #define R3DG_MAX_VIEWS 64
 
 typedef struct r3dg_raster_fwd_args {
@@ -107,6 +110,16 @@ typedef struct r3dg_raster_fwd_args {
      * coef = 1 (for s = 0 and every s whose square is a normal float).  With cov3D_precomp: R3DG_ERR_BAD_ARG before
      * any launch. */
     const float* filter_3d;
+    /* Ray-depth mode (the per-pixel Gaussian depth of RaDe-GS and PGSR).  Non-zero: each Gaussian contributes to
+     * out_depth, at pixel (x, y), the camera z at which it peaks along that pixel's ray under the projection's local
+     * affine approximation, d = tz + p.x (x - mean2D.x) + p.y (y - mean2D.y), instead of its centre's tz.  The depth
+     * plane p = conic (T0 Sigma w_z, T1 Sigma w_z) uses the record's (dilated) conic, the rows T0, T1 of T = J W, the
+     * 3D covariance Sigma (after scale_modifier and the 3D filter) and w_z = (V[2], V[6], V[10]), the view matrix's
+     * camera-z column.  out_depth, out_surface_xyz and out_normal change; every other output, the tile lists and
+     * radii are those of 0.  The geometry buffer must then hold r3dg_raster_ray_depth_geom_bytes(P, S, V) bytes
+     * (too small returns R3DG_ERR_BAD_ARG before any launch), which is always more than
+     * r3dg_raster_views_geom_bytes(P, S, V): a host can tell a buffer's mode from its size.  0 = the default path. */
+    int ray_depth;
     /* Antialiased mode (the opacity-compensated screen-space filter of upstream 3DGS and gsplat).  Non-zero: with
      * a0, b, c0 the 2D covariance before the fixed 0.3 px^2 dilation and a1 = a0 + 0.3, c1 = c0 + 0.3, every Gaussian's
      * opacity is multiplied by rho = sqrt(max(r, 2.5e-5)), r = (a0 c0 - b^2) / (a1 c1 - b^2) (r = 0 when a0 c0 - b^2
@@ -233,6 +246,12 @@ typedef struct r3dg_raster_bwd_args {
      * launch.  The appearance-only mode ignores both fields. */
     const float* filter_3d;
     const float* opacities;
+    /* Ray-depth mode: must equal the matching forward's (zero or non-zero).  The depth cotangent then also reaches the
+     * depth plane: dL_dmeans2D gains -p dL/dtz per pixel (dL_dmeans2D_abs includes it), and dL/dp reaches the conic and,
+     * through T, Sigma and w_z, dL_dmeans3D, dL_dcov3D, dL_dscales, dL_drotations and dL_dviewmatrix.  det_work must
+     * hold r3dg_raster_ray_depth_bwd_det_bytes(V * P, S) bytes (plus r3dg_raster_bwd_det_absgrad_bytes(V * P) with
+     * dL_dmeans2D_abs) in deterministic mode.  The appearance-only mode ignores it. */
+    int ray_depth;
     /* Absolute screen-space gradients (absgrad, AbsGS / gsplat's absgrad=True; optional, NULL = none, the default):
      * [P,2] ([V,P,2] for V views), next to dL_dmeans2D and in its units (0.5 W and 0.5 H per pixel): per Gaussian and
      * view, sum over pixels of |dL/dmean2D.x| and of |dL/dmean2D.y|, each pixel's term taken before the pixel sum, so
@@ -323,6 +342,11 @@ int r3dg_mark_visible(int P, const float* means3D, const float* viewmatrix,
 long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom,
                                  const void* img, const void* binning, size_t binning_bytes,
                                  void* dst, long long max_bytes, r3dg_stream_t stream);
+/* The same for the buffers of a ray-depth call (r3dg_raster_fwd_args.ray_depth): the geometry buffer's regions lie at
+ * the mode's offsets.  r3dg_raster_debug_copy reads buffers of the default mode only. */
+long long r3dg_raster_ray_depth_debug_copy(int id, int P, int S, int W, int H, const void* geom,
+                                           const void* img, const void* binning, size_t binning_bytes,
+                                           void* dst, long long max_bytes, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * BVH visibility: LBVH over the Gaussians' 3-sigma boxes + opacity ray trace.
@@ -658,6 +682,9 @@ int r3dg_render_equation_backward(const r3dg_shade_args* args, r3dg_stream_t str
  * ------------------------------------------------------------------------------------------ */
 size_t r3dg_raster_fwd_det_bytes(int P);
 size_t r3dg_raster_bwd_det_bytes(int P, int S);
+/* The deterministic backward workspace of a ray-depth call: its gradient rows hold 4 more floats (~96 B per row more
+ * than r3dg_raster_bwd_det_bytes). */
+size_t r3dg_raster_ray_depth_bwd_det_bytes(int P, int S);
 /* The deterministic workspace a backward with dL_dmeans2D_abs needs on top of r3dg_raster_bwd_det_bytes: ~48 B per
  * row (two accumulators), 48 MB at P = 1M. */
 size_t r3dg_raster_bwd_det_absgrad_bytes(int P);

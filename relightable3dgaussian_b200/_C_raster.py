@@ -157,18 +157,48 @@ def _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means
     return keep
 
 
+_RAY_DEPTH = False      # process default of the ray-depth mode (set_ray_depth)
+
+
+def set_ray_depth(enabled):
+    """Process default of the ray-depth mode for every forward that does not pass `ray_depth` (rasterizer.set_ray_depth
+    sets it).  It reaches every caller of this module, the reference's own wrapper over dropin/r3dg_rasterization
+    included; each backward takes the mode of its forward from the geometry buffer."""
+    global _RAY_DEPTH
+    _RAY_DEPTH = bool(enabled)
+
+
+def ray_depth_default():
+    return _RAY_DEPTH
+
+
+def _fwd_ray_depth(ray_depth):
+    """A forward's mode: its keyword, or the process default when it passes none (None)."""
+    return _RAY_DEPTH if ray_depth is None else bool(ray_depth)
+
+
+def _geom_ray_depth(ray_depth, geomBuffer, P, S, V):
+    """A backward's mode: its keyword, or (None) that of the forward that made `geomBuffer`: a ray-depth geometry buffer
+    is always larger than a default one of the same shape (r3dg_raster_ray_depth_geom_bytes)."""
+    if ray_depth is not None:
+        return bool(ray_depth)
+    return geomBuffer.numel() >= _lib.load().r3dg_raster_ray_depth_geom_bytes(P, S, V)
+
+
 def _forward(views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
              viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered, computer_pseudo_normal, debug,
-             capacity, pinned, defer, antialiasing=False, filter_3d=None):
+             capacity, pinned, defer, antialiasing=False, filter_3d=None, ray_depth=None):
     """The forward of the len(cams) views `cams` = [(tan_fovx, tan_fovy, cx, cy), ...]: one view (`views` False,
     outputs in the one-view shapes) or V views (outputs with a leading V).  Sizes the binning buffer for `capacity`
     instances and re-runs with room to spare while the counts, read back into the pinned int32 `pinned` (one per
     view), exceed it.  Returns the 12 outputs after num_rendered, the event recorded once the counts are copied, and the
     counts as a list: None when `defer`, which returns after the first attempt without waiting.  `antialiasing`: the
-    library's antialiased mode (see rasterize_gaussians); `filter_3d`: the 3D filter (see the module notes)."""
+    library's antialiased mode (see rasterize_gaussians); `filter_3d`: the 3D filter (see the module notes); `ray_depth`:
+    the ray-depth mode (see rasterize_gaussians)."""
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
+    ray_depth = _fwd_ray_depth(ray_depth)
     dev = means3D.device
     a = _lib.RasterFwdArgs()
     keep = _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means3D, features, colors, scales,
@@ -177,7 +207,7 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     a.opacities = _lib.ptr(opacity)
     a.cx, a.cy = float(cams[0][2]), float(cams[0][3])
     a.prefiltered = int(bool(prefiltered)); a.computer_pseudo_normal = int(bool(computer_pseudo_normal))
-    a.debug = int(bool(debug)); a.antialiasing = int(bool(antialiasing))
+    a.debug = int(bool(debug)); a.antialiasing = int(bool(antialiasing)); a.ray_depth = int(bool(ray_depth))
     a.filter_3d = _lib.ptr(filter_3d)
 
     lead = (V,) if views else ()
@@ -190,7 +220,8 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     out_surface_xyz = torch.empty(lead + (3, H, W), **f32)
     out_weights = torch.empty(lead + (P, 1), **f32)
     radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
-    geomBuffer = torch.empty((lib.r3dg_raster_views_geom_bytes(P, S, V),), dtype=torch.uint8, device=dev)
+    geom_bytes = lib.r3dg_raster_ray_depth_geom_bytes(P, S, V) if ray_depth else lib.r3dg_raster_views_geom_bytes(P, S, V)
+    geomBuffer = torch.empty((geom_bytes,), dtype=torch.uint8, device=dev)
     imgBuffer = torch.empty((lib.r3dg_raster_views_img_bytes(W, H, V),), dtype=torch.uint8, device=dev)
     a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
     a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
@@ -233,14 +264,19 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
                         scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                         cx, cy, image_height, image_width, sh, degree, campos, prefiltered,
                         computer_pseudo_normal, debug, _defer=False, _min_capacity=None, *, antialiasing=False,
-                        filter_3d=None):
+                        filter_3d=None, ray_depth=None):
     """== RasterizeGaussiansCUDA (rasterize_points.cu:36-141).  Returns the 13-tuple
     (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
      out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer).
     `antialiasing=True` (not part of the reference surface) multiplies each Gaussian's opacity by
     rho = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)), the opacity compensation of the fixed 0.3 px^2
     dilation; the backward must then be called with the same flag.  `filter_3d` (not part of the reference surface):
-    Mip-Splatting's 3D filter, see the module notes; the backward must be given the same tensor."""
+    Mip-Splatting's 3D filter, see the module notes; the backward must be given the same tensor.  `ray_depth=True`
+    (not part of the reference surface): each Gaussian adds, at each pixel, the camera z where it peaks along the
+    pixel's ray, tz + p . (pixel - mean2D) with the per-Gaussian depth plane p = conic (T0 Sigma w_z, T1 Sigma w_z),
+    instead of its centre's tz; out_depth, out_surface_xyz and out_normal change.  None (the default) takes the process
+    default (set_ray_depth, off unless set), so the reference's wrapper, which passes no such keyword, follows it.  The
+    backward takes the mode from the geometry buffer unless given."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")   # rasterize_points.cu:62-64
     P = means3D.size(0)
@@ -269,7 +305,7 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     out, ev, counts = _forward(False, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy, cx, cy)], H, W, sh, degree,
                                campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer,
-                               antialiasing, filter_3d)
+                               antialiasing, filter_3d, ray_depth)
     if _defer:
         rendered = DeferredCount(ev, pinned, capacity, st, P)
         st["pending"] = rendered
@@ -283,7 +319,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
               surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False, absgrad=False,
-              filter_3d=None, opacities=None):
+              filter_3d=None, opacities=None, ray_depth=None):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
     one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
@@ -293,12 +329,14 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     computed (the others are None too); the opacity, depth and surface cotangents are not read.  `antialiasing` must
     be the forward's.  `absgrad`: the third element returned is (dL_dmeans2D_abs,) ([P,2], or [V,P,2] for V views;
     None without the geometry half, geometry=False, which never computes it); () without absgrad.  `filter_3d` must be
-    the forward's, and `opacities` the forward's opacities (required with it)."""
+    the forward's, and `opacities` the forward's opacities (required with it).  `ray_depth`: the forward's, or None for
+    the mode of the forward that made `geomBuffer`."""
     if not geometry and (cam_grads or _out is not None):
         raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
+    ray_depth = _geom_ray_depth(ray_depth, geomBuffer, P, S, V)
     if filter_3d is not None and (opacities is None or opacities.numel() != P):
         raise ValueError("the backward with filter_3d needs the forward's opacities ([P] or [P,1])")
     H, W = dL_dout_color.size(-2), dL_dout_color.size(-1)
@@ -357,7 +395,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     # (appearance-only with nothing to compute: no call, e.g. S = 0 features the only input that needs a gradient)
     if P != 0 and (geometry or any(_lib.ptr(t) for t in (dL_dfeatures, dL_dcolors, dL_dsh))):
         a.backward_geometry = int(bool(backward_geometry)); a.debug = int(bool(debug))
-        a.antialiasing = int(bool(antialiasing))
+        a.antialiasing = int(bool(antialiasing)); a.ray_depth = int(bool(ray_depth))
         if filter_3d is not None:
             opacities = _prep(opacities, "opacities")
             a.filter_3d, a.opacities = _lib.ptr(filter_3d), _lib.ptr(opacities)
@@ -372,7 +410,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
         a.dL_dmeans2D_abs = _lib.ptr(dL_dmeans2D_abs)
-        det_bytes = lib.r3dg_raster_bwd_det_bytes(V * P, S)
+        det_bytes = lib.r3dg_raster_ray_depth_bwd_det_bytes(V * P, S) if ray_depth else lib.r3dg_raster_bwd_det_bytes(V * P, S)
         if dL_dmeans2D_abs is not None:                 # absgrad's fixed-point sums follow the gradient rows'
             det_bytes += lib.r3dg_raster_bwd_det_absgrad_bytes(V * P)
         det_ws = _lib.det_workspace(a, det_bytes, dev)
@@ -395,7 +433,7 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
                                  imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
                                  surface_work=None, geometry=True, appearance=(True, True, True), *, antialiasing=False,
-                                 absgrad=False, filter_3d=None, opacities=None):
+                                 absgrad=False, filter_3d=None, opacities=None, ray_depth=None):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
@@ -409,14 +447,15 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     come back None.  `antialiasing` (not part of the reference surface) must be the forward's: rasterize_gaussians.
     `absgrad=True` (not part of the reference surface): dL_dmeans2D_abs [P,2] is the last element (None when
     geometry=False).  `filter_3d` (not part of the reference surface) must be the forward's, and then `opacities` the
-    forward's opacities: rasterize_gaussians."""
+    forward's opacities: rasterize_gaussians.  `ray_depth` (not part of the reference surface): None (the default) takes the
+    forward's mode from `geomBuffer`, True / False must be the forward's."""
     principal = surface[4:6] if surface is not None and len(surface) == 6 else None
     grads, cam, extra = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
                            dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
                            binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
                            surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing,
-                           absgrad, filter_3d, opacities)
+                           absgrad, filter_3d, opacities, ray_depth)
     return grads + tuple(t[0] for t in cam) + extra
 
 
@@ -475,8 +514,10 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
         return out
     nbytes = out.numel() * out.element_size()
     stream = torch.cuda.current_stream(geomBuffer.device)
+    # a ray-depth geometry buffer has the mode's layout (records and gradient rows one float4 wider)
+    copy = lib.r3dg_raster_ray_depth_debug_copy if _geom_ray_depth(None, geomBuffer, P, S, 1) else lib.r3dg_raster_debug_copy
     with torch.cuda.device(geomBuffer.device):
-        rc = lib.r3dg_raster_debug_copy(spec[0], P, S, W, H, geomBuffer.data_ptr(), imgBuffer.data_ptr(),
+        rc = copy(spec[0], P, S, W, H, geomBuffer.data_ptr(), imgBuffer.data_ptr(),
                                         binningBuffer.data_ptr(), binningBuffer.numel(), out.data_ptr(),
                                         nbytes, stream.cuda_stream)
     if rc < 0:
@@ -490,13 +531,13 @@ _views_capacity = {}     # (device, P, W, H, V) -> binning capacity that held th
 
 def rasterize_views(background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                     viewmatrix, projmatrix, cams, image_height, image_width, sh, degree, campos, prefiltered,
-                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False, filter_3d=None):
+                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False, filter_3d=None, ray_depth=None):
     """V views of one set of Gaussians in one forward.  background [V,3], viewmatrix / projmatrix [V,4,4], campos [V,3],
     cams: V tuples (tan_fovx, tan_fovy, cx, cy); features [P,S] or [V,P,S], colors [P,3] or [V,P,3] (or empty).
     Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
     out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
     radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once.
-    `antialiasing` and `filter_3d` apply to every view (see rasterize_gaussians)."""
+    `antialiasing`, `filter_3d` and `ray_depth` apply to every view (see rasterize_gaussians)."""
     V, P = len(cams), means3D.size(0)
     H, W = int(image_height), int(image_width)
     dev = means3D.device
@@ -505,7 +546,7 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
     pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
     out, _, rendered = _forward(True, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                 cov3D_precomp, viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered,
-                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing, filter_3d)
+                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing, filter_3d, ray_depth)
     _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
     return (rendered,) + out
 
@@ -515,7 +556,7 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                              backward_geometry, cam_grads=False, surface=None, surface_work=None, geometry=True,
                              appearance=(True, True, True), *, antialiasing=False, absgrad=False, filter_3d=None,
-                             opacities=None):
+                             opacities=None, ray_depth=None):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
@@ -526,10 +567,10 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
     rasterize_gaussians_backward, and `antialiasing` must be the forward's.  `absgrad=True`: dL_dmeans2D_abs [V,P,2]
     is the last element, as in rasterize_gaussians_backward.  `filter_3d` and `opacities` are those of
-    rasterize_gaussians_backward."""
+    rasterize_gaussians_backward, and `ray_depth` is that of rasterize_gaussians_backward."""
     grads, cam, extra = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                            dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                            backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
-                           appearance, antialiasing, absgrad, filter_3d, opacities)
+                           appearance, antialiasing, absgrad, filter_3d, opacities, ray_depth)
     return grads + cam + extra

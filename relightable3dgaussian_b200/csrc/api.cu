@@ -44,12 +44,12 @@ inline bool misaligned16(const void* p) { return p && (reinterpret_cast<uintptr_
 
 // ---- the rasterizer's work buffers: regions in this order, each 256-byte aligned ---------------------------------
 // V views: V rows per Gaussian (row v * P + g), one header and one depth-sort region per view.  V = 1 is the one-view
-// layout.
+// layout.  Ray-depth mode: records and gradient rows one float4 wider (common.cuh rec_floats).
 struct GeomLayout {
     size_t header, rec, tiles_touched, rects, brects, clamped, scan_state, sort, sort_stride, grad, total;
     int recf;
     SortLayout sl;
-    GeomLayout(int P, int S, int V = 1) : recf(rec_floats(S)), sl(P) {
+    GeomLayout(int P, int S, int V = 1, bool ray_depth = false) : recf(rec_floats(S, ray_depth)), sl(P) {
         const size_t R = (size_t)V * P;
         sort_stride = align_up(sl.total, 256);
         size_t off = 0;
@@ -62,6 +62,9 @@ struct GeomLayout {
         scan_state = off;    off = align_up(off + ((size_t)P / R3DG_SCAN_ITEMS + 2) * 4, 256);
         sort = off;          off = align_up(off + V * sort_stride, 256);        // depth sort of the Gaussians, per view
         grad = off;          off = align_up(off + R * recf * 4, 256);           // backward scratch
+        // ray-depth mode: one more 256-byte block, so that a ray-depth buffer is always larger than a default one of
+        // the same shape and a host layer can tell the mode of a geometry buffer from its size (_C_raster.py)
+        if (ray_depth) off += 256;
         total = off;
     }
 };
@@ -113,8 +116,8 @@ size_t bin_bytes_for_capacity(long long cap) { return (size_t)((cap + 63) / 64 *
 // when a buffer is smaller than its layout or the binning buffer holds no instance, and fills `b` either way
 // (r3dg_raster_debug_copy passes SIZE_MAX for the sizes it is not given, and needs the binning only for some ids).
 int raster_buffers(int P, int S, int W, int H, void* geom_, size_t geom_bytes, void* img_, size_t img_bytes,
-                   void* bin_, size_t bin_bytes, RasterBuffers& b, int V = 1) {
-    const GeomLayout gl(P < 1 ? 1 : P, S, V);
+                   void* bin_, size_t bin_bytes, RasterBuffers& b, int V = 1, bool ray_depth = false) {
+    const GeomLayout gl(P < 1 ? 1 : P, S, V, ray_depth);
     const ImgLayout il(W, H, V);
     const BinLayout bl(bin_capacity_for_bytes(bin_bytes));
     char *geom = (char*)geom_, *img = (char*)img_, *bin = (char*)bin_;
@@ -174,8 +177,12 @@ size_t r3dg_raster_img_n_contrib_offset(int W, int H) { return ImgLayout(W, H).n
 size_t r3dg_raster_views_geom_bytes(int P, int S, int V) { return GeomLayout(P < 1 ? 1 : P, S, V < 1 ? 1 : V).total; }
 size_t r3dg_raster_views_img_bytes(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).total; }
 size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).n_contrib; }
+size_t r3dg_raster_ray_depth_geom_bytes(int P, int S, int V) { return GeomLayout(P < 1 ? 1 : P, S, V < 1 ? 1 : V, true).total; }
 size_t r3dg_raster_fwd_det_bytes(int P) { return align_up((size_t)(P < 1 ? 1 : P) * 8, 256); }
 size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S)); }
+size_t r3dg_raster_ray_depth_bwd_det_bytes(int P, int S) {
+    return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S, true));
+}
 size_t r3dg_raster_bwd_det_absgrad_bytes(int P) { return det_bytes(2 * (size_t)(P < 1 ? 1 : P)); }
 size_t r3dg_raster_cam_grad_bytes(int P, int V) {
     return align_up((size_t)(V < 1 ? 1 : V) * kCamGradFloats * cam_grad_blocks(P) * sizeof(float), 256);
@@ -212,7 +219,7 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     if (V == 0) return R3DG_ERR_BAD_ARG;
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
-                            a->binning_bytes, b, V);
+                            a->binning_bytes, b, V, a->ray_depth != 0);
     if (rc != 0) return rc;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(V * a->P))) return R3DG_ERR_BAD_ARG;
     if (V > 1 && (b.gx > 65535 || b.gy > 65535 || b.tiles > 65535)) return R3DG_ERR_UNSUPPORTED;   // the binning's limits, before any launch
@@ -264,7 +271,9 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     const int V = views_of(a->V, a->view_cams, a->P);
     if (V == 0) return R3DG_ERR_BAD_ARG;
     if (misaligned16(a->rotations) || misaligned16(a->dL_drotations)) return R3DG_ERR_BAD_ARG;
-    if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S))) return R3DG_ERR_BAD_ARG;
+    // ray-depth mode: the gradient rows are one float4 wider
+    const size_t det_rows_bytes = a->ray_depth ? r3dg_raster_ray_depth_bwd_det_bytes(V * a->P, a->S) : r3dg_raster_bwd_det_bytes(V * a->P, a->S);
+    if (a->deterministic && (!a->det_work || a->det_work_bytes < det_rows_bytes)) return R3DG_ERR_BAD_ARG;
     const int cam_outs = (a->dL_dviewmatrix != nullptr) + (a->dL_dprojmatrix != nullptr) + (a->dL_dcampos != nullptr);
     // appearance-only mode: every geometry output NULL (the six per-Gaussian ones and the camera gradients).  P = 0
     // writes no per-Gaussian output, and is refused for none of them, as before this mode existed.
@@ -274,7 +283,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (a->P > 0 && geo_outs != 0 && geo_outs != 6) return R3DG_ERR_BAD_ARG;
     // absgrad: the deterministic workspace grows only when it is requested (the appearance-only mode ignores it)
     if (a->deterministic && geometry && a->dL_dmeans2D_abs &&
-        a->det_work_bytes < r3dg_raster_bwd_det_bytes(V * a->P, a->S) + r3dg_raster_bwd_det_absgrad_bytes(V * a->P)) return R3DG_ERR_BAD_ARG;
+        a->det_work_bytes < det_rows_bytes + r3dg_raster_bwd_det_absgrad_bytes(V * a->P)) return R3DG_ERR_BAD_ARG;
     if (!geometry && (cam_outs != 0 || (!a->dL_dcolors && !a->dL_dfeatures && !a->dL_dsh))) return R3DG_ERR_BAD_ARG;
     if (V > 1 && a->P > 0 && a->shs && (geometry || a->dL_dsh) && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;
@@ -295,7 +304,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     }
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
-                            a->binning_bytes, b, V);
+                            a->binning_bytes, b, V, a->ray_depth != 0);
     if (rc != 0) return rc;
     prof_mark(false, 8, stream);
     // pseudo-normal / surface-xyz cotangents: their pull-back joins the depth and opacity cotangents, and the compositor
@@ -644,13 +653,13 @@ __global__ void unpack_composited_kernel(int P, const uint8_t* __restrict__ cl, 
 }
 }  // namespace
 
-long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom_, const void* img_,
-                                 const void* bin_, size_t binning_bytes, void* dst, long long max_bytes,
-                                 r3dg_stream_t stream_) {
+static long long debug_copy(bool ray_depth, int id, int P, int S, int W, int H, const void* geom_, const void* img_,
+                            const void* bin_, size_t binning_bytes, void* dst, long long max_bytes,
+                            r3dg_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     RasterBuffers b;       // the geom and img sizes are not given: only the binning buffer's is checked
     const bool binned = raster_buffers(P, S, W, H, const_cast<void*>(geom_), SIZE_MAX, const_cast<void*>(img_), SIZE_MAX,
-                                       const_cast<void*>(bin_), binning_bytes, b) == 0;
+                                       const_cast<void*>(bin_), binning_bytes, b, 1, ray_depth) == 0;
     const size_t HW = (size_t)W * H;
     const float* rec = b.rec;
     const uint32_t* tt = b.tiles_touched;
@@ -698,6 +707,17 @@ long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void*
         }
     }
     return -1;
+}
+
+long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom, const void* img,
+                                 const void* binning, size_t binning_bytes, void* dst, long long max_bytes,
+                                 r3dg_stream_t stream) {
+    return debug_copy(false, id, P, S, W, H, geom, img, binning, binning_bytes, dst, max_bytes, stream);
+}
+long long r3dg_raster_ray_depth_debug_copy(int id, int P, int S, int W, int H, const void* geom, const void* img,
+                                           const void* binning, size_t binning_bytes, void* dst, long long max_bytes,
+                                           r3dg_stream_t stream) {
+    return debug_copy(true, id, P, S, W, H, geom, img, binning, binning_bytes, dst, max_bytes, stream);
 }
 
 }  // extern "C"

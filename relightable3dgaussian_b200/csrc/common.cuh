@@ -20,13 +20,15 @@ namespace r3dg {
 //   [7] radius (int bits) | [8..] channels = {r,g,b,f0..f(S-1)} zero-padded to 4*NG
 // A compositor instance touches exactly this one row (2 sectors for S=5), instead of the
 // reference's 5 separate arrays (means2D, conic_opacity, depths, colors, features).
+// Ray-depth mode (r3dg_raster_fwd_args.ray_depth) appends one group: [8 + 4*NG] depth plane p.x [+1] p.y [+2, +3] 0.
 // ---------------------------------------------------------------------------------------------
 __host__ __device__ inline int num_groups(int S) { return (3 + S + 3) / 4; }
 __host__ __device__ inline int rec_floats(int S) { return 8 + 4 * num_groups(S); }
+__host__ __device__ inline int rec_floats(int S, bool ray_depth) { return rec_floats(S) + (ray_depth ? 4 : 0); }
 
 // Per-Gaussian gradient row accumulated by the backward compositor, same width as the record:
 //   [0] dmean2D.x [1] dmean2D.y [2] dmean2D.z(depth) [3] dopacity | [4] dconic.a [5] dconic.b
-//   [6] dconic.c  [7] unused | [8..] d channels
+//   [6] dconic.c  [7] unused | [8..] d channels (ray-depth mode: then dL/dp.x, dL/dp.y, 0, 0)
 // A warp reduces the row across its 32 pixels and adds it with one vector of atomics.
 
 struct GeomHeader {               // first 256 bytes of the geometry buffer

@@ -62,10 +62,14 @@ struct CompositeFwdParams {
 //   stores.  Selected with r3dg_tune("composite_bulk", 1); the register prefetch is the default.
 // DET (deterministic mode): the per-warp integer weight sums go to a u64 per Gaussian instead of a float atomic, so
 //   out_weights does not depend on the order in which warps finish.  Everything else is the same code.
-template <int NG, int NW, int MINB, bool BULK, bool DET = false>
+// RD (ray-depth mode, register prefetch only): the record's appended group, the depth plane p, is staged with the
+//   others, and an entry adds  tz - p.x dx - p.y dy  (dx, dy its mean minus the pixel) to the depth instead of tz.
+template <int NG, int NW, int MINB, bool BULK, bool DET = false, bool RD = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const CompositeFwdParams p) {
+    static_assert(!(BULK && RD), "the bulk-copy slab holds records without the depth plane");
     constexpr int RG = 2 + NG;                       // float4 groups per record
-    __shared__ __align__(16) float4 sRec[BULK ? 1 : NW][BULK ? 1 : RG][BULK ? 1 : 32];   // this warp's current 32-entry batch, SoA
+    constexpr int RGX = RG + (RD ? 1 : 0);           // staged groups: RD adds the depth plane (group RG)
+    __shared__ __align__(16) float4 sRec[BULK ? 1 : NW][BULK ? 1 : RGX][BULK ? 1 : 32];   // this warp's current 32-entry batch, SoA
     __shared__ __align__(16) float4 sRecB[BULK ? NW : 1][BULK ? 2 : 1][BULK ? 32 : 1][BULK ? RG : 1];   // BULK: [stage][entry][group]
     __shared__ __align__(8) uint64_t sBar[NW][2];
     __shared__ uint32_t sId[NW][32];                 // slab slot -> Gaussian id
@@ -125,7 +129,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
     // software pipeline: records of the next batch are in flight (registers, or bulk copies into the other slab stage)
     // while the current one is composited
     uint32_t id_cur = 0u;
-    float4 r[BULK ? 1 : RG];
+    float4 r[BULK ? 1 : RGX];
     int stage = 0;
     unsigned phase0 = 0u, phase1 = 0u;
     const unsigned rec_bytes = (unsigned)p.recf * 4u;
@@ -143,11 +147,11 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
         if (qcount > 0) issue_bulk(0, min(32, qcount), id_cur);
     } else {
 #pragma unroll
-        for (int g = 0; g < RG; ++g) r[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int g = 0; g < RGX; ++g) r[g] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (lane < qcount) {
             id_cur = plist[q[(qhead + lane) & (R3DG_QCAP - 1)]];
 #pragma unroll
-            for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
+            for (int g = 0; g < RGX; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
     }
 
@@ -175,12 +179,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             sPos[warp][k] = mypos;
             if (!BULK) {
 #pragma unroll
-                for (int g = 0; g < RG; ++g) sRec[warp][g][k] = r[g];
+                for (int g = 0; g < RGX; ++g) sRec[warp][g][k] = r[g];
             }
         }
         if (!BULK && lane >= n_acc && lane < n_acc + U) {
 #pragma unroll
-            for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int g = 0; g < RGX; ++g) sRec[warp][g][lane] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
         qhead = (qhead + n) & (R3DG_QCAP - 1);
         qcount -= n;
@@ -194,7 +198,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             if (stage) phase1 ^= 1u; else phase0 ^= 1u;
         } else if (lane < qcount) {
 #pragma unroll
-            for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
+            for (int g = 0; g < RGX; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
         int last_k = -1;                                                // this pixel's last accepted entry of the batch
         int my_wsum = 0;                                                // lane k keeps the warp's weight sum of entry k
@@ -218,7 +222,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
                 const float power = fma_(qd, -0.5f, -mul_(dy, mul_(dx, a.w)));
                 al[u] = fminf(0.99f, mul_(b.y, expf(power)));
                 om[u] = sub_(1.0f, al[u]);
-                dep[u] = b.z;
+                if constexpr (RD) {
+                    const float4 pl = sRec[warp][RG][k0 + u];
+                    dep[u] = fmaf(-pl.y, dy, fmaf(-pl.x, dx, b.z));     // tz + p . (pixel - mean)
+                } else {
+                    dep[u] = b.z;
+                }
                 // BULK has no zero-record padding: its slots past n_acc hold whatever the last copy left there
                 pv[u] = (!BULK || k0 + u < n_acc) && !(power > 0.0f) && !(al[u] < 1.0f / 255.0f);
             }
@@ -342,6 +351,8 @@ __global__ void __launch_bounds__(256) surface_normal_kernel(int W, int H, const
 // count that fits one more CTA): by channel groups NG, for the 4-warp CTA (the 8-warp variant is left to ptxas).
 // The values are those of the occupancy sweep in DESIGN.md §4.2.
 template <int NG> struct FwdOcc { static constexpr int v = NG <= 2 ? 7 : (NG <= 3 ? 6 : (NG <= 5 ? 5 : (NG <= 6 ? 4 : 3))); };
+// ray-depth mode (the depth plane's 4 more prefetch registers): fewer CTAs where the count above spills (-Xptxas -v)
+template <int NG> struct FwdOccRD { static constexpr int v = FwdOcc<NG>::v - (NG == 2 ? 2 : (NG == 5 ? 1 : 0)); };
 
 int g_composite_bulk = 0;       // r3dg_tune("composite_bulk"): 1 = TMA bulk-copy record staging in the forward compositor
 int g_fwd_ctas = 0;             // r3dg_tune("composite_fwd_ctas"): resident CTAs per SM (0 = whatever fits)
@@ -365,7 +376,12 @@ static void launch_fwd_kernel(const CompositeFwdParams& p, int tiles, cudaStream
     K<<<tiles * 2, 128, residency_pad<K>(g_fwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
-static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, cudaStream_t stream) {
+static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, bool ray_depth, cudaStream_t stream) {
+    if (ray_depth) {                                  // (register prefetch: r3dg_tune("composite_bulk") does not apply)
+        if (p.det_weights) launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccRD<NG>::v, false, true, true>>(p, tiles, stream);
+        else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccRD<NG>::v, false, false, true>>(p, tiles, stream);
+        return;
+    }
     if (p.det_weights) {
         if (g_composite_bulk == 1 && NG <= 6) launch_fwd_kernel<composite_fwd_kernel<NG <= 6 ? NG : 1, 4, FwdOcc<NG>::v, true, true>>(p, tiles, stream);
         else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOcc<NG>::v, false, true>>(p, tiles, stream);
@@ -397,16 +413,17 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
     const size_t rows = (size_t)V * a.P;
     if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, rows * 8, stream));
     const int tiles = V * b.tiles;                    // the tall grid of all views
+    const bool rd = a.ray_depth != 0;
     switch (num_groups(a.S)) {
-        case 1: launch_fwd_ng<1>(p, tiles, stream); break;
-        case 2: launch_fwd_ng<2>(p, tiles, stream); break;
-        case 3: launch_fwd_ng<3>(p, tiles, stream); break;
-        case 4: launch_fwd_ng<4>(p, tiles, stream); break;
-        case 5: launch_fwd_ng<5>(p, tiles, stream); break;
-        case 6: launch_fwd_ng<6>(p, tiles, stream); break;
-        case 7: launch_fwd_ng<7>(p, tiles, stream); break;
-        case 8: launch_fwd_ng<8>(p, tiles, stream); break;
-        case 9: launch_fwd_ng<9>(p, tiles, stream); break;
+        case 1: launch_fwd_ng<1>(p, tiles, rd, stream); break;
+        case 2: launch_fwd_ng<2>(p, tiles, rd, stream); break;
+        case 3: launch_fwd_ng<3>(p, tiles, rd, stream); break;
+        case 4: launch_fwd_ng<4>(p, tiles, rd, stream); break;
+        case 5: launch_fwd_ng<5>(p, tiles, rd, stream); break;
+        case 6: launch_fwd_ng<6>(p, tiles, rd, stream); break;
+        case 7: launch_fwd_ng<7>(p, tiles, rd, stream); break;
+        case 8: launch_fwd_ng<8>(p, tiles, rd, stream); break;
+        case 9: launch_fwd_ng<9>(p, tiles, rd, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;
     }
     if (p.det_weights && a.P > 0) det_weights_kernel<<<(int)((rows + 255) / 256), 256, 0, stream>>>((int)rows, p.det_weights, a.out_weights);

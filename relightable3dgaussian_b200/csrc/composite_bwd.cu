@@ -73,13 +73,20 @@ struct CompositeBwdParams {
 // ABS (absgrad, GEOM only): the entry phase also sums the magnitudes of the pixels' two dL/dmean2D terms in the order
 // of the signed sums, times |o| W/2 and |o| H/2, and adds the two totals to p.abs_grad (DET:
 // p.det_abs, class exponent e_geo) once per entry.  Everything else, the gradient row included, is the same code.
-template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true, bool ABS = false>
+// RD (ray-depth mode, GEOM only): an entry's depth at a pixel is d = tz - p.x dx - p.y dy (the record's appended depth
+// plane p), in dL/dalpha too.  The entry phase also sums  dcc dL_dD dx  and  dcc dL_dD dy : the row's appended group
+// gets dL/dp = -(those sums), and the dL/dmean2D slots get d's own term  -p dL/dtz  (times W/2, H/2), added after the
+// alpha term, so that a zero depth cotangent leaves them as they are.  With ABS, the per-pixel magnitudes are those of
+// the two terms together.
+template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true, bool ABS = false, bool RD = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const CompositeBwdParams p) {
     static_assert(GEOM || !ABS, "absgrad needs the geometry half of the backward");
+    static_assert(GEOM || !RD, "the depth plane's gradient needs the geometry half of the backward");
     constexpr int NC = 4 * NG;              // padded channel count {r,g,b,f...}; gradient row = 8 geometry slots + NC
     constexpr int GOFF = GEOM ? 8 : 0;      // slot of channel 0 in the gradient row (GEOM = false: no geometry slots)
-    constexpr int ROWF = GOFF + NC;         // floats per gradient row (p.recf with GEOM)
+    constexpr int ROWF = GOFF + NC + (RD ? 4 : 0);   // floats per gradient row (p.recf with GEOM); RD: + dL/dp group
     constexpr int RG = 2 + NG;
+    constexpr int RGX = RG + (RD ? 1 : 0);  // staged record groups: RD adds the depth plane (group RG)
     // entries per sub-batch: 16, or 8 from NG = 6 on (static shared memory stays under 48 KB); lane l of the entry
     // phase sums entry l % E over the E pixels of part l / E
     constexpr int E = NG <= 5 ? 16 : 8;
@@ -87,7 +94,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     constexpr int SROW = 4 * ((ROWF / 4) | 1);   // staged row stride: an odd number of float4, conflict-free stores
     static_assert(E * SROW <= 2 * E * PS, "the staged rows overlay the planes");
     constexpr int UP = 2;                   // entries per step of the pixel phase (divides E)
-    __shared__ float4 sRec[NW][RG][32];
+    __shared__ float4 sRec[NW][RGX][32];
     __shared__ uint32_t sId[NW][32];
     __shared__ uint32_t sK[NW][32];
     __shared__ uint32_t sQ[NW][R3DG_QCAP];
@@ -179,14 +186,14 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
     __syncwarp();
 
     uint32_t id_cur = 0u, k_cur = 0u;
-    float4 r[RG];
+    float4 r[RGX];
 #pragma unroll
-    for (int g = 0; g < RG; ++g) r[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int g = 0; g < RGX; ++g) r[g] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (lane < qcount) {
         k_cur = q[(qhead + lane) & (R3DG_QCAP - 1)];
         id_cur = plist[k_cur];
 #pragma unroll
-        for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
+        for (int g = 0; g < RGX; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
     }
 
     float* const sW = sPl[warp];
@@ -199,7 +206,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
         sId[warp][lane] = ABS ? id_cur : id_cur * (uint32_t)(GEOM ? p.recf : NC);
         sK[warp][lane] = k_cur;                                        // 0-based list position == contributor index
 #pragma unroll
-        for (int g = 0; g < RG; ++g) sRec[warp][g][lane] = r[g];
+        for (int g = 0; g < RGX; ++g) sRec[warp][g][lane] = r[g];
         qhead = (qhead + n) & (R3DG_QCAP - 1);
         qcount -= n;
         while (qcount < 64 && w_next >= w_low) scan_step();
@@ -208,7 +215,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
             k_cur = q[(qhead + lane) & (R3DG_QCAP - 1)];
             id_cur = plist[k_cur];
 #pragma unroll
-            for (int g = 0; g < RG; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
+            for (int g = 0; g < RGX; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
 #pragma unroll 1
         for (int j0 = 0; j0 < n; j0 += E) {
@@ -242,7 +249,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv[u]) : "f"(1.0f - alpha[u]));   // 1 - alpha in [0.01, 1]: one MUFU
                     float d = 0.0f;
                     if constexpr (GEOM) {
-                        d = fmaf(b.z, dpix_d, dpix_o);                      // depth * dL_ddepth + 1 * dL_dopacity
+                        float dep = b.z;
+                        if constexpr (RD) {                                 // the forward's plane depth
+                            const float4 pl = sRec[warp][RG][j];
+                            dep = fmaf(-pl.y, dy, fmaf(-pl.x, dx, b.z));
+                        }
+                        d = fmaf(dep, dpix_d, dpix_o);                      // depth * dL_ddepth + 1 * dL_dopacity
                         const float4 c0 = sRec[warp][2][j], t0 = sCot[warp][0][lane];
                         d = fmaf(c0.z, t0.z, fmaf(c0.y, t0.y, fmaf(c0.x, t0.x, d)));
                         // feature channels enter dL_dalpha only when backward_geometry is set (backward.cu:563-566)
@@ -278,6 +290,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
             const float4 b = sRec[warp][1][je];
             constexpr int ROWS = E / 8;
             float sw = 0.f, s0 = 0.f, s1 = 0.f, sxx = 0.f, sxy = 0.f, syy = 0.f, sd = 0.f, ax = 0.f, ay = 0.f;
+            float sdx = 0.f, sdy = 0.f;                                     // RD: sums of dcc dL_dD dx, dcc dL_dD dy
+            const float4 pl = RD ? sRec[warp][RGX - 1][je] : make_float4(0.f, 0.f, 0.f, 0.f);
             float sc[NC];
 #pragma unroll
             for (int c = 0; c < NC; ++c) sc[c] = 0.0f;
@@ -300,7 +314,15 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                     sw += w;
                     sxx = fmaf(wdx, dx, sxx); sxy = fmaf(wdx, dy, sxy); syy = fmaf(wdy, dy, syy);
                     sd = fmaf(c, sCotD[warp][pb], sd);
-                    if constexpr (ABS) { ax = add_(ax, fabsf(t0)); ay = add_(ay, fabsf(t1)); }
+                    if constexpr (RD) {
+                        const float cd = c * sCotD[warp][pb];
+                        sdx = fmaf(cd, dx, sdx); sdy = fmaf(cd, dy, sdy);
+                        if constexpr (ABS) {                                // the pixel's whole dL/dmean2D term / (W/2)
+                            ax = add_(ax, fabsf(fmaf(b.y, t0, pl.x * cd))); ay = add_(ay, fabsf(fmaf(b.y, t1, pl.y * cd)));
+                        }
+                    } else if constexpr (ABS) {
+                        ax = add_(ax, fabsf(t0)); ay = add_(ay, fabsf(t1));
+                    }
                 }
 #pragma unroll
                 for (int g = 0; g < NG; ++g) {
@@ -325,6 +347,10 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                     syy += __shfl_xor_sync(0xffffffffu, syy, m);
                     sd += __shfl_xor_sync(0xffffffffu, sd, m);
                 }
+                if constexpr (RD) {
+                    sdx += __shfl_xor_sync(0xffffffffu, sdx, m);
+                    sdy += __shfl_xor_sync(0xffffffffu, sdy, m);
+                }
                 if constexpr (ABS) {
                     ax += __shfl_xor_sync(0xffffffffu, ax, m);
                     ay += __shfl_xor_sync(0xffffffffu, ay, m);
@@ -339,12 +365,19 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                 row[3] = sw;
                 row[4] = ho * sxx; row[5] = ho * sxy; row[6] = ho * syy;
                 row[7] = 0.0f;
+                if constexpr (RD) {                                         // d's own dependence on the mean: -p dL/dtz
+                    row[0] = fmaf(-(ddelx_dx * pl.x), sd, row[0]);
+                    row[1] = fmaf(-(ddely_dy * pl.y), sd, row[1]);
+                    row[GOFF + NC] = -sdx; row[GOFF + NC + 1] = -sdy;       // dL/dp = sum dcc dL_dD (pixel - mean)
+                    row[GOFF + NC + 2] = 0.0f; row[GOFF + NC + 3] = 0.0f;
+                }
             }
 #pragma unroll
             for (int c = 0; c < NC; ++c) row[GOFF + c] = sc[c];
             if constexpr (ABS) {                                            // lane: pair component part & 1 of entry le
                 if (part < 2 && le < ne) {
-                    const float v = part ? mul_(fabsf(b.y) * ddely_dy, ay) : mul_(fabsf(b.y) * ddelx_dx, ax);
+                    const float v = RD ? (part ? mul_(ddely_dy, ay) : mul_(ddelx_dx, ax))
+                                       : (part ? mul_(fabsf(b.y) * ddely_dy, ay) : mul_(fabsf(b.y) * ddelx_dx, ax));
                     const size_t ai = 2 * (size_t)sId[warp][j0 + le] + part;
                     if constexpr (DET) det_add(p.det_abs, ai, v, e_geo);
                     else atomicAdd(p.abs_grad + ai, v);
@@ -362,15 +395,16 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll 1
                 for (int i = lane; i < ne * ROWF; i += 32) {
                     const int e = i / ROWF, s = i - e * ROWF;
-                    if ((GEOM && s == 7) || (s >= GOFF && s - GOFF >= 3 + p.S)) continue;
+                    const bool plane = RD && s >= GOFF + NC;                // RD: the dL/dp group, geometry class
+                    if ((GEOM && s == 7) || (!plane && s >= GOFF && s - GOFF >= 3 + p.S) || (plane && s >= GOFF + NC + 2)) continue;
                     const size_t row0 = ABS ? (size_t)sId[warp][j0 + e] * p.recf : (size_t)sId[warp][j0 + e];
-                    det_add(p.det, row0 + s, sPl[warp][e * SROW + s], s < GOFF ? e_geo : e_app);
+                    det_add(p.det, row0 + s, sPl[warp][e * SROW + s], s < GOFF || plane ? e_geo : e_app);
                 }
             } else {                                                        // 32 float4 segments per instruction
 #pragma unroll 1
                 for (int i = lane; i < ne * CH; i += 32) {
                     const int e = i / CH, c4 = i - e * CH;
-                    if (4 * c4 >= GOFF && 4 * c4 - GOFF >= 3 + p.S) continue;   // padding channels only
+                    if (4 * c4 >= GOFF && 4 * c4 - GOFF >= 3 + p.S && !(RD && 4 * c4 >= GOFF + NC)) continue;   // padding channels only
                     const size_t row0 = ABS ? (size_t)sId[warp][j0 + e] * p.recf : (size_t)sId[warp][j0 + e];
                     atomicAdd(reinterpret_cast<float4*>(p.grad + row0) + c4,
                               *reinterpret_cast<const float4*>(sPl[warp] + e * SROW + 4 * c4));
@@ -455,8 +489,8 @@ __global__ void __launch_bounds__(256) zero_composited_rows_kernel(size_t rows, 
     }
 }
 
-DetAcc raster_det_abs(const r3dg_raster_bwd_args& a, size_t rows) {
-    return det_acc((char*)a.det_work + det_bytes(rows * rec_floats(a.S)), 2 * rows);   // behind r3dg_raster_bwd_det_bytes
+DetAcc raster_det_abs(const r3dg_raster_bwd_args& a, size_t rows, int recf) {
+    return det_acc((char*)a.det_work + det_bytes(rows * recf), 2 * rows);   // behind r3dg_raster_(ray_depth_)bwd_det_bytes
 }
 
 uint32_t* raster_det_scale(const RasterBuffers& b) {
@@ -466,6 +500,8 @@ uint32_t* raster_det_scale(const RasterBuffers& b) {
 // resident CTAs per SM the register allocation is pinned to, by channel groups NG: the most at which no instantiation
 // (DET x GEOM x ABS) spills (DESIGN.md §4.2)
 template <int NG> struct BwdOcc { static constexpr int v = NG <= 2 ? 5 : (NG <= 4 ? 4 : 3); };
+// ray-depth mode (two more entry-phase sums and the depth plane): one CTA fewer where the count above spills
+template <int NG> struct BwdOccRD { static constexpr int v = BwdOcc<NG>::v - (NG == 1 || NG == 2 || NG == 4 ? 1 : 0); };
 int g_bwd_ctas = 0;             // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
 int composite_bwd_tune(const char* key, int value, int* previous) {
     if (strcmp(key, "composite_bwd_ctas") != 0) return R3DG_ERR_UNSUPPORTED;
@@ -474,13 +510,19 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
     g_bwd_ctas = value;
     return 0;
 }
-template <int NG, bool DET, bool GEOM, bool ABS = false>
+template <int NG, bool DET, bool GEOM, bool ABS = false, bool RD = false>
 static void launch_bwd_kernel(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
-    constexpr auto kernel = composite_bwd_kernel<NG, 4, BwdOcc<NG>::v, DET, GEOM, ABS>;
+    constexpr auto kernel = composite_bwd_kernel<NG, 4, RD ? BwdOccRD<NG>::v : BwdOcc<NG>::v, DET, GEOM, ABS, RD>;
     kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
-static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, bool det, bool geometry, bool absgrad, cudaStream_t stream) {
+static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, bool det, bool geometry, bool absgrad, bool rd,
+                          cudaStream_t stream) {
+    if (geometry && rd) {                             // (absgrad implies geometry)
+        if (absgrad) det ? launch_bwd_kernel<NG, true, true, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, true, true>(p, tiles, stream);
+        else det ? launch_bwd_kernel<NG, true, true, false, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, false, true>(p, tiles, stream);
+        return;
+    }
     if (absgrad) det ? launch_bwd_kernel<NG, true, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, true>(p, tiles, stream);
     else if (geometry) det ? launch_bwd_kernel<NG, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true>(p, tiles, stream);
     else det ? launch_bwd_kernel<NG, true, false>(p, tiles, stream) : launch_bwd_kernel<NG, false, false>(p, tiles, stream);
@@ -506,14 +548,14 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     p.n_contrib = b.n_contrib;
     const bool det = a.deterministic != 0;
     const size_t rows = (size_t)V * a.P;
-    const int gradf = composite_bwd_row_floats(a.S, geometry);     // the gradient row: b.recf, or NC without geometry
+    const int gradf = geometry ? b.recf : composite_bwd_row_floats(a.S, false);   // the gradient row: b.recf, or NC without geometry
     p.det = det_acc(a.det_work, rows * gradf);
     p.det_scale = det ? raster_det_scale(b) : nullptr;
     // absgrad (geometry only; the appearance-only backward ignores dL_dmeans2D_abs): the default mode adds into the
     // output itself, DET mode into its own accumulators behind the gradient rows' in det_work
     const bool absgrad = geometry && a.dL_dmeans2D_abs != nullptr;
     p.abs_grad = absgrad && !det ? a.dL_dmeans2D_abs : nullptr;
-    p.det_abs = absgrad && det ? raster_det_abs(a, rows) : det_acc(nullptr, 0);
+    p.det_abs = absgrad && det ? raster_det_abs(a, rows, b.recf) : det_acc(nullptr, 0);
     // zeroed here, in the backward, so that every backward over one forward (retain_graph) starts from zero
     const int zblocks = (int)((rows + 255) / 256);
     if (det) {
@@ -526,14 +568,15 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     const int tiles = V * b.tiles;                    // the tall grid of all views
     int rc = launch_cta_order(b.bwd_work, b.bwd_order, 2 * tiles, stream);
     if (rc != 0) return rc;
+    const bool rd = a.ray_depth != 0;
     switch (num_groups(a.S)) {
-        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, absgrad, stream); break;
-        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, absgrad, stream); break;
-        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, absgrad, stream); break;
-        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, absgrad, stream); break;
-        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, absgrad, stream); break;
-        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, absgrad, stream); break;
-        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, absgrad, stream); break;
+        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, absgrad, rd, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;   // S > 24: reference backward limit (backward.cu:449)
     }
     R3DG_CUDA_TRY(cudaGetLastError());

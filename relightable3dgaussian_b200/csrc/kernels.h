@@ -86,8 +86,9 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
 // region holds V * P * recf >= 8 V floats.
 uint32_t* raster_det_scale(const RasterBuffers& b);
 // deterministic mode with absgrad (dL_dmeans2D_abs given): the 2 accumulators per row of the `rows` = V * P rows'
-// absgrad sums, in det_work right behind the gradient rows' r3dg_raster_bwd_det_bytes(V * P, S)
-DetAcc raster_det_abs(const r3dg_raster_bwd_args& a, size_t rows);
+// absgrad sums, in det_work right behind the gradient rows of recf floats (r3dg_raster_bwd_det_bytes(V * P, S), or
+// r3dg_raster_ray_depth_bwd_det_bytes in ray-depth mode)
+DetAcc raster_det_abs(const r3dg_raster_bwd_args& a, size_t rows, int recf);
 int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, int v, cudaStream_t stream);
 int launch_appearance_backward(const r3dg_raster_bwd_args& a, const RasterBuffers& b, cudaStream_t stream);
 

@@ -169,7 +169,9 @@ __device__ __forceinline__ void load_rows_transposed(float* s, const float* __re
 
 // F3D: Mip-Splatting's 3D filter (common.cuh filter3d_fold) — the Gaussian is projected with the dilated scales s' and
 // its opacity is o coef; cov3D_precomp is refused by the caller.
-template <bool F3D = false>
+// RD (ray-depth mode): the record's appended group holds the depth plane p = conic (T0 Sigma w_z, T1 Sigma w_z), the
+// gradient of camera z's conditional mean given the screen position (w_z: the view matrix's camera-z column).
+template <bool F3D = false, bool RD = false>
 __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams p) {
     extern __shared__ __align__(16) float sSH[];   // SH slab ([3M][PROJ_THREADS + 1] transposed, or row-major), later the record slab
     __shared__ float sV[16], sPr[16], sCam[3];
@@ -218,6 +220,7 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
         }
     }
     float pix_x = 0.f, pix_y = 0.f, con_a = 0.f, con_b = 0.f, con_c = 0.f, aa_rho = 1.f, f3d_coef = 1.f;
+    float pl_x = 0.f, pl_y = 0.f;                      // RD: the depth plane
     int my_radius = 0, x0 = 0, y0 = 0, x1 = 0, y1 = 0;
     if (alive) {
         const float hx = xform_row_(sPr, 0, px, py, pz);
@@ -277,6 +280,12 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
             }
             const float det_inv = rcp_(det);
             con_a = mul_(cov_c, det_inv); con_b = mul_(cov_b, -det_inv); con_c = mul_(cov_a, det_inv);
+            if constexpr (RD) {                        // c = (T0 Sigma w_z, T1 Sigma w_z) from the a, b products, p = conic c
+                const float cu = fmaf(a2, sV[10], fmaf(a1, sV[6], a0 * sV[2]));
+                const float cv = fmaf(b2, sV[10], fmaf(b1, sV[6], b0 * sV[2]));
+                pl_x = fmaf(con_b, cv, con_a * cu);
+                pl_y = fmaf(con_c, cv, con_b * cu);
+            }
             const float mid = mul_(add_(cov_a, cov_c), 0.5f);
             const float disc = sqrt_(fmaxf(fma_(mid, mid, -det), 0.1f));
             const float lam = fmaxf(add_(mid, disc), sub_(mid, disc));
@@ -341,6 +350,7 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_kernel(const ProjParams 
             }
             srow[2 + g] = make_float4(v[0], v[1], v[2], v[3]);
         }
+        if constexpr (RD) srow[2 + p.ng] = make_float4(pl_x, pl_y, 0.f, 0.f);
         p.radii[idx] = my_radius;
         p.tiles_touched[idx] = (uint32_t)((y1 - y0) * (x1 - x0));
         p.clamped[idx] = (uint8_t)cl;
@@ -500,8 +510,14 @@ int launch_projection(const r3dg_raster_fwd_args& a, const RasterBuffers& b, int
     const size_t rec_smem = (size_t)PROJ_THREADS * b.recf * sizeof(float);
     if (rec_smem > sh_smem) sh_smem = rec_smem;
     const int blocks = (a.P + PROJ_THREADS - 1) / PROJ_THREADS;
-    if (a.filter_3d) project_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
-    else project_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    if (a.ray_depth) {
+        if (a.filter_3d) project_kernel<true, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+        else project_kernel<false, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    } else if (a.filter_3d) {
+        project_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    } else {
+        project_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    }
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

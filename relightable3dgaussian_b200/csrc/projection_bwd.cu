@@ -8,6 +8,7 @@
 //    in uninitialised memory (the reference zero-fills 320 MB at P=1M, rasterize_points.cu:183-192);
 //  * the input gradient is one packed [RECF] row per Gaussian produced by the compositor;
 //  * cov3D is recomputed from scale/rotation instead of being stored and re-read.
+#include <type_traits>
 #include "common.cuh"
 #include "detacc.cuh"
 #include "kernels.h"
@@ -134,7 +135,10 @@ __device__ __forceinline__ ViewDir view_dir(const float* m, const float* cam) {
 // added in place (default mode, nothing to write) or into fixed-point accumulators (DET: read and written here).
 // F3D (3D filter): the covariance chain runs on the forward's dilated scales s' (common.cuh filter3d_fold) and gives
 // dL/ds' and dL/do'; the end of the scale chain turns them into dL/ds and dL/do.
-template <bool DET = false, bool CAM = false, bool ABS = false, bool F3D = false>
+// RD (ray-depth mode): the row's appended group holds dL/dp of the depth plane p = conic c, c = (T0 Sigma w_z,
+// T1 Sigma w_z) (projection.cu).  It joins dL/dconic (slot 5 as half of dL/db, the row's convention) before the
+// covariance chain, and dL/dc reaches dL/dT0, dL/dT1 (so J, t and the means), dL/dSigma and, with CAM, dL/dw_z.
+template <bool DET = false, bool CAM = false, bool ABS = false, bool F3D = false, bool RD = false>
 __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const ProjBwdParams p) {
     // SH rows (192 B at M=16) travel through shared memory: the CTA's [128][3M] slab of shs is ONE contiguous
     // 24 KB block, fetched by a single TMA-unit bulk copy (cp.async.bulk, mbarrier-signalled) into a row-major
@@ -176,6 +180,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
     // the thread's own rows are requested before the cooperative slab load so that both are in flight together
     const float4* g4 = reinterpret_cast<const float4*>(p.grad + (size_t)idx * p.recf);
     float4 gA = make_float4(0, 0, 0, 0), gB = gA, gC = gA, q4 = gA;
+    float2 gP = make_float2(0.f, 0.f);                 // RD: dL/dp
     float m3[3] = {0, 0, 0}, s3[3] = {0, 0, 0}, aa_op = 0.f;
     if (live) {
         if (p.antialiasing) aa_op = p.rec[(size_t)idx * p.recf + 5];   // the forward's compensated opacity o rho
@@ -185,8 +190,10 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             gA = make_float4(det_load(p.det, r0, eg), det_load(p.det, r0 + 1, eg), det_load(p.det, r0 + 2, eg), det_load(p.det, r0 + 3, eg));
             gB = make_float4(det_load(p.det, r0 + 4, eg), det_load(p.det, r0 + 5, eg), det_load(p.det, r0 + 6, eg), 0.0f);
             gC = make_float4(det_load(p.det, r0 + 8, ea), det_load(p.det, r0 + 9, ea), det_load(p.det, r0 + 10, ea), 0.0f);
+            if constexpr (RD) gP = make_float2(det_load(p.det, r0 + p.recf - 4, eg), det_load(p.det, r0 + p.recf - 3, eg));
         } else {
             gA = g4[0]; gB = g4[1]; gC = g4[2];
+            if constexpr (RD) { const float4 t4 = g4[(p.recf >> 2) - 1]; gP = make_float2(t4.x, t4.y); }
         }
         m3[0] = p.means3D[3 * (size_t)idx]; m3[1] = p.means3D[3 * (size_t)idx + 1]; m3[2] = p.means3D[3 * (size_t)idx + 2];
         if (!p.cov3D_precomp) {
@@ -231,7 +238,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
         dmean2[0] = gA.x; dmean2[1] = gA.y; dmean2[2] = gA.z; dop = gA.w;
         dcol[0] = gC.x; dcol[1] = gC.y; dcol[2] = gC.z;
         const float mx = m3[0], my = m3[1], mz = m3[2];
-        const float dcx = gB.x, dcy = gB.y, dcz = gB.z;      // dL/d conic a,b,c
+        float dcx = gB.x, dcy = gB.y, dcz = gB.z;            // dL/d conic a,b,c
         float c6[6], R[3][3], s[3];
         const bool have_sr = p.scales != nullptr;
         if (p.cov3D_precomp) {
@@ -275,6 +282,23 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
         const float b = T1[0] * VT0[0] + T1[1] * VT0[1] + T1[2] * VT0[2];
         const float c = c0 + 0.3f;
         const float denom = a * c - b * b;
+        // RD: c = (T0 Sigma w_z, T1 Sigma w_z), p = conic c with conic = [[c, -b], [-b, a]] / denom
+        float wz[3] = {0.f, 0.f, 0.f}, gcu = 0.f, gcv = 0.f;
+        if constexpr (RD) {
+            wz[0] = V[2]; wz[1] = V[6]; wz[2] = V[10];
+            const float cu = VT0[0] * wz[0] + VT0[1] * wz[1] + VT0[2] * wz[2];
+            const float cv = VT1[0] * wz[0] + VT1[1] * wz[1] + VT1[2] * wz[2];
+            const float dinv = 1.0f / denom, ca = c * dinv, cb = -b * dinv, cc = a * dinv;
+            // dL/dp joins dL/dconic: p.x = ca cu + cb cv, p.y = cb cu + cc cv.  Explicit roundings here and below keep
+            // these terms out of the contraction of the neighbouring expressions.  A zero dL/dp still does not give the
+            // mode-off leaf gradients bit for bit: ptxas contracts parts of the shared chain differently in this
+            // instantiation (about 1e-6 of a leaf's largest element; tests/test_ray_depth_gpu.py)
+            dcx = __fadd_rn(dcx, __fmul_rn(gP.x, cu));
+            dcy = __fadd_rn(dcy, __fmul_rn(0.5f, __fadd_rn(__fmul_rn(gP.x, cv), __fmul_rn(gP.y, cu))));
+            dcz = __fadd_rn(dcz, __fmul_rn(gP.y, cv));
+            gcu = gP.x * ca + gP.y * cb;               // dL/dc
+            gcv = gP.x * cb + gP.y * cc;
+        }
         // antialiased mode: r = det0 / det1 (0 for det0 <= 0) of the forward's rho = sqrt(max(r, 2.5e-5)); the record
         // holds o rho and dop = dL/d(o rho)
         float aa_r = 0.f;
@@ -310,6 +334,22 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             dT0[k] = 2 * t0v * dL_da + t1v * dL_db;
             dT1[k] = 2 * t1v * dL_dc + t0v * dL_db;
         }
+        if constexpr (RD) {                            // c's own terms: dc/dT = Sigma w_z, dc/dSigma = sym(T w_z^T)
+            float u[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const float sw = Vrk[k][0] * wz[0] + Vrk[k][1] * wz[1] + Vrk[k][2] * wz[2];
+                dT0[k] = __fadd_rn(dT0[k], __fmul_rn(gcu, sw));
+                dT1[k] = __fadd_rn(dT1[k], __fmul_rn(gcv, sw));
+                u[k] = gcu * T0[k] + gcv * T1[k];
+            }
+            dcov[0] = __fadd_rn(dcov[0], __fmul_rn(u[0], wz[0]));
+            dcov[3] = __fadd_rn(dcov[3], __fmul_rn(u[1], wz[1]));
+            dcov[5] = __fadd_rn(dcov[5], __fmul_rn(u[2], wz[2]));
+            dcov[1] = __fadd_rn(dcov[1], __fadd_rn(__fmul_rn(u[0], wz[1]), __fmul_rn(u[1], wz[0])));
+            dcov[2] = __fadd_rn(dcov[2], __fadd_rn(__fmul_rn(u[0], wz[2]), __fmul_rn(u[2], wz[0])));
+            dcov[4] = __fadd_rn(dcov[4], __fadd_rn(__fmul_rn(u[1], wz[2]), __fmul_rn(u[2], wz[1])));
+        }
         // W[c][r] = V[4r + c]
         const float dL_dJ00 = V[0] * dT0[0] + V[4] * dT0[1] + V[8] * dT0[2];
         const float dL_dJ02 = V[2] * dT0[0] + V[6] * dT0[1] + V[10] * dT0[2];
@@ -341,6 +381,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 5) projection_bwd_kernel(const P
             for (int j = 0; j < 4; ++j) {
                 float d0 = dt[0] * mt[j], d1 = dt[1] * mt[j], d2 = dt[2] * mt[j];
                 if (j < 3) { d0 += dT0[j] * J00; d1 += dT1[j] * J11; d2 += dT0[j] * J02 + dT1[j] * J12; }
+                if (RD && j < 3) d2 = __fadd_rn(d2, __fadd_rn(__fmul_rn(gcu, VT0[j]), __fmul_rn(gcv, VT1[j])));   // c's own w_z term
                 sG[(4 * j + 0) * SLAB_LD] = d0; sG[(4 * j + 1) * SLAB_LD] = d1; sG[(4 * j + 2) * SLAB_LD] = d2;
             }
             // projmatrix: ndc = (h_0, h_1) / (h_3 + 1e-7) with h_k = sum_j [m,1]_j P[4j + k]; column 2 is never read
@@ -648,28 +689,16 @@ int launch_projection_backward(const r3dg_raster_bwd_args& a, const RasterBuffer
     const size_t cam_smem = sh_smem + (size_t)kCamGradFloats * SLAB_LD * sizeof(float);
     const bool abs = a.dL_dmeans2D_abs != nullptr;
     p.dL_dmeans2D_abs = abs ? a.dL_dmeans2D_abs + 2 * r : nullptr;
-    p.det_abs = abs && a.deterministic ? raster_det_abs(a, (size_t)b.V * a.P) : det_acc(nullptr, 0);
+    p.det_abs = abs && a.deterministic ? raster_det_abs(a, (size_t)b.V * a.P, b.recf) : det_acc(nullptr, 0);
     p.filter_3d = a.filter_3d; p.opacities = a.opacities;
-    if (a.filter_3d) {               // (r3dg_raster_backward refused it with cov3D_precomp or without opacities)
-        auto launch = [&](auto kernel, size_t smem) { kernel<<<blocks, PROJ_THREADS, smem, stream>>>(p); };
-        if (abs) {
-            if (cam && a.deterministic) launch(projection_bwd_kernel<true, true, true, true>, cam_smem);
-            else if (cam) launch(projection_bwd_kernel<false, true, true, true>, cam_smem);
-            else if (a.deterministic) launch(projection_bwd_kernel<true, false, true, true>, sh_smem);
-            else launch(projection_bwd_kernel<false, false, true, true>, sh_smem);
-        } else if (cam && a.deterministic) launch(projection_bwd_kernel<true, true, false, true>, cam_smem);
-        else if (cam) launch(projection_bwd_kernel<false, true, false, true>, cam_smem);
-        else if (a.deterministic) launch(projection_bwd_kernel<true, false, false, true>, sh_smem);
-        else launch(projection_bwd_kernel<false, false, false, true>, sh_smem);
-    } else if (abs) {
-        if (cam && a.deterministic) projection_bwd_kernel<true, true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
-        else if (cam) projection_bwd_kernel<false, true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
-        else if (a.deterministic) projection_bwd_kernel<true, false, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
-        else projection_bwd_kernel<false, false, true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
-    } else if (cam && a.deterministic) projection_bwd_kernel<true, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
-    else if (cam) projection_bwd_kernel<false, true><<<blocks, PROJ_THREADS, cam_smem, stream>>>(p);
-    else if (a.deterministic) projection_bwd_kernel<true><<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
-    else projection_bwd_kernel<<<blocks, PROJ_THREADS, sh_smem, stream>>>(p);
+    // (r3dg_raster_backward refused filter_3d with cov3D_precomp or without opacities)
+    auto pick = [](bool on, auto k) { if (on) k(std::true_type{}); else k(std::false_type{}); };
+    pick(a.deterministic != 0, [&](auto det) { pick(cam, [&](auto cm) { pick(abs, [&](auto ab) {
+    pick(a.filter_3d != nullptr, [&](auto f3) { pick(a.ray_depth != 0, [&](auto rd) {
+        constexpr bool C = decltype(cm)::value;
+        projection_bwd_kernel<decltype(det)::value, C, decltype(ab)::value, decltype(f3)::value, decltype(rd)::value>
+            <<<blocks, PROJ_THREADS, C ? cam_smem : sh_smem, stream>>>(p);
+    }); }); }); }); });
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -73,6 +73,34 @@ def _absgrad_on(absgrad):
     return bool(absgrad) or _ABSGRAD
 
 
+def set_ray_depth(enabled: bool):
+    """Process default of the ray-depth mode (not part of the reference surface).  After `set_ray_depth(True)` every
+    forward that does not ask otherwise runs as with `ray_depth=True`: `GaussianRasterizer`, `rasterize_gaussians` and
+    `rasterize_views` here, and `_C_raster.rasterize_gaussians` / `rasterize_views`, which the reference's own wrapper
+    (gaussian_renderer/r3dg_rasterization.py over dropin/r3dg_rasterization) calls.  The depth output, and so
+    surface_xyz and the pseudo-normal, then come from per-pixel depth planes instead of the Gaussians' centre depths,
+    and the reference's unmodified stage-1 loop trains its normals on the better pseudo-normal.  Each backward takes
+    its forward's mode from the geometry buffer.  `set_ray_depth(False)` restores the default (off)."""
+    _C.set_ray_depth(enabled)
+
+
+def _ray_depth_on(ray_depth):
+    """The call's ray-depth mode: its keyword, or the process default (set_ray_depth)."""
+    return bool(ray_depth) or _C.ray_depth_default()
+
+
+def _rd_kw(ray_depth):
+    """The keyword that turns on the library's ray-depth mode, only when it is on: an off call is the call without
+    the mode.  (A library backward without it takes the forward's mode from the geometry buffer.)"""
+    return {"ray_depth": True} if ray_depth else {}
+
+
+def _rerun_rd_kw(ray_depth):
+    """The deferred-count re-run's keyword: the node's mode, explicit whenever the process default could differ from
+    it (the default may have changed since the forward), and no keyword when the mode is not in use at all."""
+    return {"ray_depth": bool(ray_depth)} if ray_depth or _C.ray_depth_default() else {}
+
+
 def _set_absgrad(means2D, g_abs):
     """Adds g_abs to `means2D.absgrad` on the caller's tensor object, as autograd accumulates `.grad`: set on the first
     backward, summed with what is there on later ones (retain_graph, or a tensor used in several graphs)."""
@@ -150,13 +178,13 @@ def _input_grads(ctx, grads, cameras):
     """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
     three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
     one, and for all three when none was computed.  The last three inputs, the 3D filter (a buffer, as in
-    Mip-Splatting) and the antialiasing and absgrad flags, get None."""
+    Mip-Splatting) and the antialiasing, ray-depth and absgrad flags, get None."""
     g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
     cam = (None, None, None)
     if grads[9:]:
         cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[11:14]))
     return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
-            None, None) + cam + (None, None, None)
+            None, None) + cam + (None, None, None, None)
 
 
 # the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
@@ -211,16 +239,17 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing,
-                absgrad):
+                ray_depth, absgrad):
         rs = raster_settings
         out = _debug_call(rs.debug, _C.rasterize_gaussians,
                           _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
                                         cov3Ds_precomp),
                           "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
                           _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad),
-                          **_aa_kw(antialiasing), **_f3d_kw(filter_3d))
+                          **_aa_kw(antialiasing), **_f3d_kw(filter_3d), **_rd_kw(ray_depth))
         ctx.raster_settings = rs
         ctx.antialiasing = antialiasing
+        ctx.ray_depth = ray_depth
         ctx.absgrad = absgrad
         ctx.means2D = means2D if absgrad else None      # the caller's tensor object: the backward sets .absgrad on it
         ctx.num_rendered = out[0]
@@ -252,6 +281,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         kw.update(_aa_kw(ctx.antialiasing))
         kw.update(_absgrad_kw(ctx, kw))
         kw.update(_f3d_kw(filter_3d, opacities))
+        kw.update(_rd_kw(ctx.ray_depth))
         if ex is not None:
             kw["_out"] = {"sh_factor": ex[0].factor}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
@@ -271,7 +301,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                 out = _C.rasterize_gaussians(*_forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales,
                                                             rotations, cov3Ds_precomp),
                                              _min_capacity=int(ctx.num_rendered) + 4096, **_aa_kw(ctx.antialiasing),
-                                             **_f3d_kw(filter_3d))
+                                             **_f3d_kw(filter_3d), **_rerun_rd_kw(ctx.ray_depth))
                 if surface is not None:         # the adjoint of the re-run's own surface pass
                     kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
                 grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
@@ -321,7 +351,7 @@ def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, feat
 
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
                         rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False, antialiasing=False,
-                        absgrad=False, filter_3d=None):
+                        absgrad=False, filter_3d=None, ray_depth=False):
     """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
     cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
     when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
@@ -353,7 +383,15 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     erosion or speckle.  The filter is a buffer: it gets no gradient and must not require one.  A filter of the wrong
     length (stale after densification), on the CPU, not fp32 or not contiguous, and the combination with
     cov3Ds_precomp, raise ValueError before anything runs.  filter3d.fold(scales, opacities, filter_3d) gives the
-    filtered Gaussians for consumers that take no filter; they render the same images."""
+    filtered Gaussians for consumers that take no filter; they render the same images.
+
+    With `ray_depth=True`, or after `set_ray_depth(True)` (not part of the reference surface), each Gaussian adds to the
+    depth output, at each pixel, the camera z at which it peaks along that pixel's ray (RaDe-GS, PGSR) instead of its
+    centre's: tz + p . (pixel - mean2D), with the per-Gaussian depth plane p = conic (T0 Sigma w_z, T1 Sigma w_z) of the
+    projection's local affine approximation.  A flat Gaussian on a tilted surface then renders as a tilted plane, not a
+    fronto-parallel step, so surface_xyz and the pseudo-normal (outputs 6 and 7, derived from the depth) are smooth
+    inside each footprint.  The depth cotangent reaches the plane: the means, scales, rotations, cov3Ds_precomp and the
+    view matrix get its gradient, and means2D.grad includes -p dL/dtz.  Every other output is unchanged."""
     global _CALL_GRAD_MODE
     rs = raster_settings
     _C._check_filter_3d(filter_3d, means3D.shape[0], cov3Ds_precomp)
@@ -363,17 +401,19 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
                                      scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
                                      rs.viewmatrix, rs.projmatrix, rs.campos, filter_3d, bool(antialiasing),
-                                     _absgrad_on(absgrad))
+                                     _ray_depth_on(ray_depth), _absgrad_on(absgrad))
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, surface_grads=False, antialiasing=False, absgrad=False):
-        """`surface_grads`, `antialiasing` and `absgrad` (not part of the reference surface): see rasterize_gaussians."""
+    def __init__(self, raster_settings, surface_grads=False, antialiasing=False, absgrad=False, ray_depth=False):
+        """`surface_grads`, `antialiasing`, `absgrad` and `ray_depth` (not part of the reference surface): see
+        rasterize_gaussians."""
         super().__init__()
         self.raster_settings = raster_settings
         self.surface_grads = surface_grads
         self.antialiasing = antialiasing
         self.absgrad = absgrad
+        self.ray_depth = ray_depth
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -388,7 +428,7 @@ class GaussianRasterizer(nn.Module):
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
                                    scales, rotations, cov3D_precomp, self.raster_settings,
                                    surface_grads=self.surface_grads, antialiasing=self.antialiasing,
-                                   absgrad=self.absgrad, filter_3d=filter_3d)
+                                   absgrad=self.absgrad, filter_3d=filter_3d, ray_depth=self.ray_depth)
 
 
 _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
@@ -400,15 +440,16 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing, absgrad):
+                settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing, ray_depth, absgrad):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
         out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
                                  rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing),
-                                 **_f3d_kw(filter_3d))
+                                 **_f3d_kw(filter_3d), **_rd_kw(ray_depth))
         ctx.meta = (rs, cams, antialiasing)
+        ctx.ray_depth = ray_depth
         ctx.absgrad = absgrad
         ctx.means2D = means2D if absgrad else None
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
@@ -427,6 +468,7 @@ class _RasterizeViews(torch.autograd.Function):
         kw = _backward_mode(ctx)
         kw.update(_absgrad_kw(ctx, kw))
         kw.update(_f3d_kw(filter_3d, opacities))
+        kw.update(_rd_kw(ctx.ray_depth))
         if kw.get("geometry", True):
             kw.update(cam_grads=any(ctx.needs_input_grad[11:14]), surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
@@ -441,7 +483,7 @@ class _RasterizeViews(torch.autograd.Function):
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False,
-                    absgrad=False, filter_3d=None):
+                    absgrad=False, filter_3d=None, ray_depth=False):
     """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
 
     `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
@@ -454,8 +496,9 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
     Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
-    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing`, `absgrad` and `filter_3d` are those of
-    rasterize_gaussians and apply to every view; `means2D.absgrad` is then [V,P,2], each view's own."""
+    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing`, `absgrad`, `filter_3d` and `ray_depth` are
+    those of rasterize_gaussians and apply to every view (each view with its own depth planes); `means2D.absgrad` is
+    then [V,P,2], each view's own."""
     settings = list(settings)
     V = len(settings)
     if V < 1:
@@ -489,7 +532,7 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
                                  cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos,
-                                 filter_3d, bool(antialiasing), _absgrad_on(absgrad))
+                                 filter_3d, bool(antialiasing), _ray_depth_on(ray_depth), _absgrad_on(absgrad))
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)

@@ -1,0 +1,77 @@
+"""Cost of the ray-depth rasterizer mode (ray_depth=True) against the default mode.
+
+Rasterizer forward + backward at the headline configuration (1M Gaussians, 800x800, S=5) and at the stage-2 shape
+(1.5M, 1600x1200, S=16), the mode off and on over the same inputs.  Each timing is CUDA events around `iters` fwd+bwd
+pairs; the two arms alternate round by round in one process and the median over `rounds` is reported, with the
+project, composite and project_bwd stage times of the library's stage profiler in a separate run.  The mode adds one
+16-byte record group per composited entry in each compositor, a few FMAs per (pixel, entry) and two more moments in
+the backward's entry phase, and the plane's few FLOPs per Gaussian in the projection and its backward.
+
+Prints one JSON line that starts with the device name and power limit read in the same run.
+
+    python tools/bench_ray_depth.py [--rounds 5] [--iters 10]
+"""
+import argparse
+import json
+import os
+import statistics
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from bench_views import device_info, stage_times, timed  # noqa: E402
+from relightable3dgaussian_b200 import _C_raster, synth  # noqa: E402
+
+
+def raster_step(P, W, H, S, ray_depth):
+    sc = synth.make_scene(P, "shell-v1", 0, S)
+    cam = synth.make_camera(1, W, H)
+    d = lambda t: t.cuda().contiguous()
+    means, feats, opac, scales, rots, shs = (d(t) for t in (sc.means3D, sc.features, sc.opacities, sc.scales,
+                                                            sc.rotations, sc.shs))
+    bg, view, proj, campos = d(torch.tensor([0.0, 0.5, 1.0])), d(cam.viewmatrix), d(cam.projmatrix), d(cam.campos)
+    gen = torch.Generator(device="cuda").manual_seed(1)
+    cots = [torch.randn(c, H, W, device="cuda", generator=gen) for c in (3, 1, 1, S)]
+    empty = torch.empty(0, device="cuda")
+    kw = {"ray_depth": True} if ray_depth else {}
+
+    def run():
+        o = _C_raster.rasterize_gaussians(bg, means, feats, empty, opac, scales, rots, 1.0, empty, view, proj,
+                                          cam.tanfovx, cam.tanfovy, cam.cx, cam.cy, H, W, shs, 3, campos, False, True,
+                                          False, **kw)
+        _C_raster.rasterize_gaussians_backward(bg, means, feats, o[9], empty, scales, rots, 1.0, empty, view, proj,
+                                               cam.tanfovx, cam.tanfovy, *cots, shs, 3, campos, o[10], o[0], o[11],
+                                               o[12], True, False, **kw)
+    return run
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--iters", type=int, default=10)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_ray_depth.py needs a CUDA GPU")
+    res = device_info()
+    configs = {"1M_800x800_S5": (1_000_000, 800, 800, 5), "1.5M_1600x1200_S16": (1_500_000, 1600, 1200, 16)}
+    for name, (P, W, H, S) in configs.items():
+        arms = {"off": raster_step(P, W, H, S, False), "on": raster_step(P, W, H, S, True)}
+        ms = {k: [] for k in arms}
+        for _ in range(args.rounds):
+            for k, run in arms.items():
+                ms[k].append(timed(run, args.iters))
+        st = {k: stage_times(run, args.iters, 1) for k, run in arms.items()}
+        a, b = statistics.median(ms["off"]), statistics.median(ms["on"])
+        res[name] = {"fwd_bwd_off_ms": round(a, 3), "fwd_bwd_on_ms": round(b, 3), "ratio_on_off": round(b / a, 4),
+                     "spread_ms": {k: round(max(v) - min(v), 3) for k, v in ms.items()},
+                     **{f"{s}_ms": {k: t[s] for k, t in st.items()} for s in ("project", "composite", "project_bwd")}}
+        del arms
+        torch.cuda.empty_cache()
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
