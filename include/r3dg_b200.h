@@ -48,6 +48,10 @@ size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V);
 /* The geometry buffer of a ray-depth call (r3dg_raster_fwd_args.ray_depth) of V views: its records and gradient rows
  * hold 4 more floats per Gaussian and view.  V below 1 is sized as 1. */
 size_t r3dg_raster_ray_depth_geom_bytes(int P, int S, int V);
+/* The image buffer of a call with depth statistics (r3dg_raster_fwd_args.depth_stats) of V views: the default layout
+ * followed by the per-pixel median positions and one word per view.  Always larger than
+ * r3dg_raster_views_img_bytes(W, H, V); V below 1 is sized as 1. */
+size_t r3dg_raster_depth_stats_img_bytes(int W, int H, int V);
 #define R3DG_MAX_VIEWS 64
 
 typedef struct r3dg_raster_fwd_args {
@@ -110,6 +114,19 @@ typedef struct r3dg_raster_fwd_args {
      * coef = 1 (for s = 0 and every s whose square is a normal float).  With cov3D_precomp: R3DG_ERR_BAD_ARG before
      * any launch. */
     const float* filter_3d;
+    /* Depth statistics (optional; 0 = off, the default).  Non-zero: with d the depth each accepted entry adds to
+     * out_depth (tz, or the plane depth in ray-depth mode) and w = alpha T its weight,
+     *   out_depth2 [1,H,W] ([V,1,H,W]) = sum w (d d) over the accepted entries in list order, like out_depth not
+     *                                    normalised and without a background term;
+     *   out_median_depth [1,H,W]        = d of the last accepted entry whose transmittance before it is > 0.5 (the
+     *                                    entry that takes T through 0.5, or the last accepted one if T never gets
+     *                                    there), 0 where no entry is accepted.
+     * The image buffer must hold r3dg_raster_depth_stats_img_bytes(W, H, V) bytes (it also keeps each pixel's median
+     * entry for the backward); a smaller one, or a missing output, returns R3DG_ERR_BAD_ARG before any launch.  Every
+     * other output is that of 0, bit for bit. */
+    int depth_stats;
+    float* out_depth2;
+    float* out_median_depth;
     /* Ray-depth mode (the per-pixel Gaussian depth of RaDe-GS and PGSR).  Non-zero: each Gaussian contributes to
      * out_depth, at pixel (x, y), the camera z at which it peaks along that pixel's ray under the projection's local
      * affine approximation, d = tz + p.x (x - mean2D.x) + p.y (y - mean2D.y), instead of its centre's tz.  The depth
@@ -246,6 +263,15 @@ typedef struct r3dg_raster_bwd_args {
      * launch.  The appearance-only mode ignores both fields. */
     const float* filter_3d;
     const float* opacities;
+    /* Depth statistics: non-zero when the matching forward had them on, with the cotangents of its out_depth2 and
+     * out_median_depth ([V,1,H,W], both required; zeros for an output the loss does not use).  Per pixel and entry the
+     * depth cotangent w dL_ddepth becomes w (dL_ddepth + 2 d dL_ddepth2) + [the entry is the pixel's median]
+     * dL_dmedian, and dL/dalpha gains d^2 dL_ddepth2.  Non-zero with an image buffer smaller than
+     * r3dg_raster_depth_stats_img_bytes(W, H, V) or a missing cotangent, or a cotangent given with 0, returns
+     * R3DG_ERR_BAD_ARG before any launch.  The appearance-only mode ignores all three fields. */
+    int depth_stats;
+    const float* dL_dout_depth2;
+    const float* dL_dout_median_depth;
     /* Ray-depth mode: must equal the matching forward's (zero or non-zero).  The depth cotangent then also reaches the
      * depth plane: dL_dmeans2D gains -p dL/dtz per pixel (dL_dmeans2D_abs includes it), and dL/dp reaches the conic and,
      * through T, Sigma and w_z, dL_dmeans3D, dL_dcov3D, dL_dscales, dL_drotations and dL_dviewmatrix.  det_work must
@@ -337,6 +363,8 @@ int r3dg_mark_visible(int P, const float* means3D, const float* viewmatrix,
  *      block b composited the entry in the forward | 20 brects u32[2P]: per Gaussian the inclusive
  *      block rectangle {bx0 | bx1 << 16, by0 | by1 << 16} (empty when bx0 > bx1) | 22 composited
  *      u8[P]: 1 when some pixel composited the Gaussian (the backward reads and zeroes its rows only)
+ *      | 23 median_pos i32[HW]: per pixel the 1-based list position of its median entry, 0 for none (the image
+ *      buffer of a call with depth statistics only, r3dg_raster_depth_stats_img_bytes)
  *      (9, 18, 19: the copy stops at max_bytes, pass R entries' worth)
  * Returns bytes written or a negative error. */
 long long r3dg_raster_debug_copy(int id, int P, int S, int W, int H, const void* geom,

@@ -33,6 +33,13 @@ screen-space gradients dL_dmeans2D_abs (AbsGS, gsplat's absgrad): per Gaussian a
 (Mip-Splatting): a [P] or [P,1] fp32 CUDA tensor of per-Gaussian filter sizes f, shared by every view (filter3d.py).
 Each Gaussian is drawn with scales sqrt(s^2 + f^2) and its opacity times sqrt(prod_k s_k^2 / (s_k^2 + f^2)).  The
 backward takes the forward's tensor again and, with it, the forward's `opacities`; f gets no gradient.
+
+`depth_stats=True` on the two forward functions (not part of the reference surface) also renders, per pixel, depth2 =
+sum w d^2 over the composited entries (d: the depth the call composites, tz or the ray-depth plane) and the median
+depth (d of the entry at which the transmittance falls through 0.5); the two images follow every other element of the
+returned tuple.  None and False are off, and there is no process default: the reference's wrapper, which unpacks a
+fixed tuple, never sees them.  The backward functions take their cotangents as `dL_dout_depth2` and
+`dL_dout_median_depth` (None: zeros) and `depth_stats=None` for the forward's setting, read from the image buffer's size.
 """
 import ctypes
 import warnings
@@ -185,16 +192,25 @@ def _geom_ray_depth(ray_depth, geomBuffer, P, S, V):
     return geomBuffer.numel() >= _lib.load().r3dg_raster_ray_depth_geom_bytes(P, S, V)
 
 
+def _img_depth_stats(depth_stats, imageBuffer, W, H, V):
+    """A backward's depth-statistics setting: its keyword, or (None) that of the forward that made `imageBuffer`: such a
+    buffer is always larger than a default one of the same shape (r3dg_raster_depth_stats_img_bytes)."""
+    if depth_stats is not None:
+        return bool(depth_stats)
+    return imageBuffer.numel() >= _lib.load().r3dg_raster_depth_stats_img_bytes(W, H, V)
+
+
 def _forward(views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
              viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered, computer_pseudo_normal, debug,
-             capacity, pinned, defer, antialiasing=False, filter_3d=None, ray_depth=None):
+             capacity, pinned, defer, antialiasing=False, filter_3d=None, ray_depth=None, depth_stats=None):
     """The forward of the len(cams) views `cams` = [(tan_fovx, tan_fovy, cx, cy), ...]: one view (`views` False,
     outputs in the one-view shapes) or V views (outputs with a leading V).  Sizes the binning buffer for `capacity`
     instances and re-runs with room to spare while the counts, read back into the pinned int32 `pinned` (one per
     view), exceed it.  Returns the 12 outputs after num_rendered, the event recorded once the counts are copied, and the
     counts as a list: None when `defer`, which returns after the first attempt without waiting.  `antialiasing`: the
     library's antialiased mode (see rasterize_gaussians); `filter_3d`: the 3D filter (see the module notes); `ray_depth`:
-    the ray-depth mode (see rasterize_gaussians)."""
+    the ray-depth mode (see rasterize_gaussians); `depth_stats`: the depth statistics, whose two images then follow the 12
+    outputs."""
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
@@ -222,7 +238,12 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
     geom_bytes = lib.r3dg_raster_ray_depth_geom_bytes(P, S, V) if ray_depth else lib.r3dg_raster_views_geom_bytes(P, S, V)
     geomBuffer = torch.empty((geom_bytes,), dtype=torch.uint8, device=dev)
-    imgBuffer = torch.empty((lib.r3dg_raster_views_img_bytes(W, H, V),), dtype=torch.uint8, device=dev)
+    img_bytes = lib.r3dg_raster_depth_stats_img_bytes(W, H, V) if depth_stats else lib.r3dg_raster_views_img_bytes(W, H, V)
+    imgBuffer = torch.empty((img_bytes,), dtype=torch.uint8, device=dev)
+    stats = ()
+    if depth_stats:
+        stats = (torch.empty(lead + (1, H, W), **f32), torch.empty(lead + (1, H, W), **f32))    # depth2, median depth
+        a.depth_stats, a.out_depth2, a.out_median_depth = 1, stats[0].data_ptr(), stats[1].data_ptr()
     a.out_color = out_color.data_ptr(); a.out_opacity = out_opacity.data_ptr()
     a.out_depth = out_depth.data_ptr(); a.out_feature = _lib.ptr(out_feature)
     a.out_normal = out_normal.data_ptr(); a.out_surface_xyz = out_surface_xyz.data_ptr()
@@ -257,14 +278,14 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     off = lib.r3dg_raster_views_img_n_contrib_offset(W, H, V)
     n_contrib = imgBuffer[off:off + 4 * V * H * W].view(torch.int32).view(lead + (H, W))   # view, like the reference
     return (n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal, out_surface_xyz, out_weights, radii,
-            geomBuffer, binningBuffer, imgBuffer), ev, counts
+            geomBuffer, binningBuffer, imgBuffer) + stats, ev, counts
 
 
 def rasterize_gaussians(background, means3D, features, colors, opacity, scales, rotations,
                         scale_modifier, cov3D_precomp, viewmatrix, projmatrix, tan_fovx, tan_fovy,
                         cx, cy, image_height, image_width, sh, degree, campos, prefiltered,
                         computer_pseudo_normal, debug, _defer=False, _min_capacity=None, *, antialiasing=False,
-                        filter_3d=None, ray_depth=None):
+                        filter_3d=None, ray_depth=None, depth_stats=None):
     """== RasterizeGaussiansCUDA (rasterize_points.cu:36-141).  Returns the 13-tuple
     (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
      out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer).
@@ -276,7 +297,8 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     pixel's ray, tz + p . (pixel - mean2D) with the per-Gaussian depth plane p = conic (T0 Sigma w_z, T1 Sigma w_z),
     instead of its centre's tz; out_depth, out_surface_xyz and out_normal change.  None (the default) takes the process
     default (set_ray_depth, off unless set), so the reference's wrapper, which passes no such keyword, follows it.  The
-    backward takes the mode from the geometry buffer unless given."""
+    backward takes the mode from the geometry buffer unless given.  `depth_stats=True` (not part of the reference
+    surface): depth2 [1,H,W] and median_depth [1,H,W] follow imgBuffer (see the module notes)."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")   # rasterize_points.cu:62-64
     P = means3D.size(0)
@@ -305,7 +327,7 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     out, ev, counts = _forward(False, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy, cx, cy)], H, W, sh, degree,
                                campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer,
-                               antialiasing, filter_3d, ray_depth)
+                               antialiasing, filter_3d, ray_depth, depth_stats)
     if _defer:
         rendered = DeferredCount(ev, pinned, capacity, st, P)
         st["pending"] = rendered
@@ -319,7 +341,8 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
               surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False, absgrad=False,
-              filter_3d=None, opacities=None, ray_depth=None):
+              filter_3d=None, opacities=None, ray_depth=None, depth_stats=None, dL_dout_depth2=None,
+              dL_dout_median_depth=None):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
     one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
@@ -330,7 +353,9 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     be the forward's.  `absgrad`: the third element returned is (dL_dmeans2D_abs,) ([P,2], or [V,P,2] for V views;
     None without the geometry half, geometry=False, which never computes it); () without absgrad.  `filter_3d` must be
     the forward's, and `opacities` the forward's opacities (required with it).  `ray_depth`: the forward's, or None for
-    the mode of the forward that made `geomBuffer`."""
+    the mode of the forward that made `geomBuffer`.  `depth_stats`: the forward's, or None for that of the forward that
+    made `imageBuffer`; with it, `dL_dout_depth2` and `dL_dout_median_depth` are the cotangents of its two images (None:
+    zeros), which only the geometry half reads."""
     if not geometry and (cam_grads or _out is not None):
         raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
@@ -340,6 +365,9 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
     if filter_3d is not None and (opacities is None or opacities.numel() != P):
         raise ValueError("the backward with filter_3d needs the forward's opacities ([P] or [P,1])")
     H, W = dL_dout_color.size(-2), dL_dout_color.size(-1)
+    depth_stats = _img_depth_stats(depth_stats, imageBuffer, W, H, V)
+    if not depth_stats and (dL_dout_depth2 is not None or dL_dout_median_depth is not None):
+        raise ValueError("cotangents of depth2 / median_depth need a forward with depth_stats=True")
     dev = means3D.device
     a = _lib.RasterBwdArgs()
     keep = _shared_args(a, views, cams, W, H, degree, scale_modifier, background, means3D, features, colors, scales,
@@ -410,6 +438,13 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
         a.img = imageBuffer.data_ptr(); a.img_bytes = imageBuffer.numel()
         a.binning = binningBuffer.data_ptr(); a.binning_bytes = binningBuffer.numel()
         a.dL_dmeans2D_abs = _lib.ptr(dL_dmeans2D_abs)
+        if depth_stats and geometry:                    # (the appearance-only backward reads neither cotangent)
+            like = dL_dout_depth
+            dL_dout_depth2, dL_dout_median_depth = (torch.zeros_like(like) if g is None else _prep(g, name) for g, name in
+                                                    ((dL_dout_depth2, "dL_dout_depth2"),
+                                                     (dL_dout_median_depth, "dL_dout_median_depth")))
+            a.depth_stats = 1
+            a.dL_dout_depth2, a.dL_dout_median_depth = dL_dout_depth2.data_ptr(), dL_dout_median_depth.data_ptr()
         det_bytes = lib.r3dg_raster_ray_depth_bwd_det_bytes(V * P, S) if ray_depth else lib.r3dg_raster_bwd_det_bytes(V * P, S)
         if dL_dmeans2D_abs is not None:                 # absgrad's fixed-point sums follow the gradient rows'
             det_bytes += lib.r3dg_raster_bwd_det_absgrad_bytes(V * P)
@@ -433,7 +468,8 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
                                  dL_dout_feature, sh, degree, campos, geomBuffer, R, binningBuffer,
                                  imageBuffer, backward_geometry, debug, _out=None, cam_grads=False, surface=None,
                                  surface_work=None, geometry=True, appearance=(True, True, True), *, antialiasing=False,
-                                 absgrad=False, filter_3d=None, opacities=None, ray_depth=None):
+                                 absgrad=False, filter_3d=None, opacities=None, ray_depth=None, depth_stats=None,
+                                 dL_dout_depth2=None, dL_dout_median_depth=None):
     """== RasterizeGaussiansBackwardCUDA (rasterize_points.cu:143-235).  Returns the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dfeatures, dL_dcov3D, dL_dsh,
      dL_dscales, dL_drotations).  With `cam_grads=True` (not part of the reference surface) three camera gradients
@@ -448,14 +484,16 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     `absgrad=True` (not part of the reference surface): dL_dmeans2D_abs [P,2] is the last element (None when
     geometry=False).  `filter_3d` (not part of the reference surface) must be the forward's, and then `opacities` the
     forward's opacities: rasterize_gaussians.  `ray_depth` (not part of the reference surface): None (the default) takes the
-    forward's mode from `geomBuffer`, True / False must be the forward's."""
+    forward's mode from `geomBuffer`, True / False must be the forward's.  `depth_stats` (not part of the reference
+    surface): None takes the forward's setting from `imageBuffer`; `dL_dout_depth2` / `dL_dout_median_depth` [1,H,W] are
+    the cotangents of its two images (None: zeros)."""
     principal = surface[4:6] if surface is not None and len(surface) == 6 else None
     grads, cam, extra = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
                            dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
                            binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
                            surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing,
-                           absgrad, filter_3d, opacities, ray_depth)
+                           absgrad, filter_3d, opacities, ray_depth, depth_stats, dL_dout_depth2, dL_dout_median_depth)
     return grads + tuple(t[0] for t in cam) + extra
 
 
@@ -508,7 +546,9 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
             "ranges": (15, torch.int32, (T, 2)), "bwd_work": (16, torch.int32, (T, 2)),
             "bwd_order": (17, torch.int32, (2 * T,)), "bmask": (18, torch.uint8, (num_rendered,)),
             "cmask": (19, torch.uint8, (num_rendered,)), "brects": (20, torch.int32, (P, 2)),
-            "composited": (22, torch.uint8, (P,))}[name]
+            "composited": (22, torch.uint8, (P,)), "median_pos": (23, torch.int32, (H, W))}[name]
+    if name == "median_pos" and imgBuffer.numel() < lib.r3dg_raster_depth_stats_img_bytes(W, H, 1):
+        raise RuntimeError("debug_intermediate(median_pos) needs the image buffer of a forward with depth_stats=True")
     out = torch.empty(spec[2], dtype=spec[1], device=geomBuffer.device)
     if out.numel() == 0:
         return out
@@ -531,13 +571,15 @@ _views_capacity = {}     # (device, P, W, H, V) -> binning capacity that held th
 
 def rasterize_views(background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                     viewmatrix, projmatrix, cams, image_height, image_width, sh, degree, campos, prefiltered,
-                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False, filter_3d=None, ray_depth=None):
+                    computer_pseudo_normal, _min_capacity=None, *, antialiasing=False, filter_3d=None, ray_depth=None,
+                    depth_stats=None):
     """V views of one set of Gaussians in one forward.  background [V,3], viewmatrix / projmatrix [V,4,4], campos [V,3],
     cams: V tuples (tan_fovx, tan_fovy, cx, cy); features [P,S] or [V,P,S], colors [P,3] or [V,P,3] (or empty).
     Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
     out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
     radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once.
-    `antialiasing`, `filter_3d` and `ray_depth` apply to every view (see rasterize_gaussians)."""
+    `antialiasing`, `filter_3d` and `ray_depth` apply to every view (see rasterize_gaussians).  `depth_stats=True`:
+    depth2 [V,1,H,W] and median_depth [V,1,H,W] follow imgBuffer."""
     V, P = len(cams), means3D.size(0)
     H, W = int(image_height), int(image_width)
     dev = means3D.device
@@ -546,7 +588,8 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
     pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
     out, _, rendered = _forward(True, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
                                 cov3D_precomp, viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered,
-                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing, filter_3d, ray_depth)
+                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing, filter_3d, ray_depth,
+                                depth_stats)
     _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
     return (rendered,) + out
 
@@ -556,7 +599,8 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
                              dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                              backward_geometry, cam_grads=False, surface=None, surface_work=None, geometry=True,
                              appearance=(True, True, True), *, antialiasing=False, absgrad=False, filter_3d=None,
-                             opacities=None, ray_depth=None):
+                             opacities=None, ray_depth=None, depth_stats=None, dL_dout_depth2=None,
+                             dL_dout_median_depth=None):
     """Backward of rasterize_views.  Returns (dL_dmeans2D [V,P,3], dL_dcolors, dL_dopacity [P,1], dL_dmeans3D,
     dL_dfeatures, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations): dL_dfeatures / dL_dcolors have the shape of their
     input ([P,*] summed over the views, or [V,P,*] per view); every other leaf gradient is the fp32 sum over the views
@@ -567,10 +611,12 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
     rasterize_gaussians_backward, and `antialiasing` must be the forward's.  `absgrad=True`: dL_dmeans2D_abs [V,P,2]
     is the last element, as in rasterize_gaussians_backward.  `filter_3d` and `opacities` are those of
-    rasterize_gaussians_backward, and `ray_depth` is that of rasterize_gaussians_backward."""
+    rasterize_gaussians_backward, and `ray_depth` is that of rasterize_gaussians_backward.  `depth_stats`,
+    `dL_dout_depth2` and `dL_dout_median_depth` ([V,1,H,W]) are those of rasterize_gaussians_backward."""
     grads, cam, extra = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
                            cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
                            dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
                            backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
-                           appearance, antialiasing, absgrad, filter_3d, opacities, ray_depth)
+                           appearance, antialiasing, absgrad, filter_3d, opacities, ray_depth, depth_stats, dL_dout_depth2,
+                           dL_dout_median_depth)
     return grads + cam + extra

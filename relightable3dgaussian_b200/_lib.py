@@ -31,7 +31,8 @@ class RasterFwdArgs(ctypes.Structure):
         [("geom", c_void_p), ("geom_bytes", c_size_t), ("img", c_void_p), ("img_bytes", c_size_t),
          ("binning", c_void_p), ("binning_bytes", c_size_t), ("num_rendered_host", c_void_p), ("count_ready_event", c_void_p),
          ("V", c_int), ("view_cams", c_void_p), ("features_per_view", c_int), ("colors_per_view", c_int),
-         ("filter_3d", c_void_p), ("ray_depth", c_int), ("antialiasing", c_int),
+         ("filter_3d", c_void_p), ("depth_stats", c_int), ("out_depth2", c_void_p), ("out_median_depth", c_void_p),
+         ("ray_depth", c_int), ("antialiasing", c_int),
          ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -54,8 +55,10 @@ class RasterBwdArgs(ctypes.Structure):
          ("cam_work", c_void_p), ("cam_work_bytes", c_size_t),
          ("dL_dout_normal", c_void_p), ("dL_dout_surface_xyz", c_void_p), ("fwd_opacity", c_void_p), ("fwd_depth", c_void_p),
          ("cx", c_float), ("cy", c_float), ("surface_work", c_void_p), ("surface_work_bytes", c_size_t),
-         ("filter_3d", c_void_p), ("opacities", c_void_p), ("ray_depth", c_int), ("dL_dmeans2D_abs", c_void_p),
-         ("antialiasing", c_int), ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+         ("filter_3d", c_void_p), ("opacities", c_void_p),
+         ("depth_stats", c_int), ("dL_dout_depth2", c_void_p), ("dL_dout_median_depth", c_void_p),
+         ("ray_depth", c_int), ("dL_dmeans2D_abs", c_void_p), ("antialiasing", c_int),
+         ("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
 class ShadeArgs(ctypes.Structure):
@@ -114,6 +117,7 @@ SYMBOLS = [
     ("r3dg_raster_views_img_bytes", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_raster_views_img_n_contrib_offset", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_raster_ray_depth_geom_bytes", c_size_t, [c_int, c_int, c_int]),
+    ("r3dg_raster_depth_stats_img_bytes", c_size_t, [c_int, c_int, c_int]),
     ("r3dg_raster_forward", c_int, [ctypes.POINTER(RasterFwdArgs), c_void_p]),
     ("r3dg_raster_backward", c_int, [ctypes.POINTER(RasterBwdArgs), c_void_p]),
     ("r3dg_raster_cam_grad_bytes", c_size_t, [c_int, c_int]),

@@ -71,10 +71,14 @@ struct GeomLayout {
 
 // V views: V images stacked as one tall tile grid (view v owns tile rows [v * gy, (v + 1) * gy)); the binning scratch
 // (slab sums, count matrix) is per view and reused by the views one after the other.
+// Depth statistics: two more regions behind the default layout (whose offsets they leave as they are), so that such a
+// buffer is always larger than a default one of the same shape: the median entry's list position per pixel, and per
+// view the largest |d| of an accepted entry (the deterministic backward's scale).
 struct ImgLayout {
-    size_t final_T, n_contrib, ranges, tile_order, bwd_work, bwd_order, slab_sum, bin_matrix, total;
+    size_t final_T, n_contrib, ranges, tile_order, bwd_work, bwd_order, slab_sum, bin_matrix, median_pos, depth_bound, total;
     int gx, gy, max_chunks;
-    ImgLayout(int W, int H, int V = 1) : gx((W + R3DG_TILE - 1) / R3DG_TILE), gy((H + R3DG_TILE - 1) / R3DG_TILE) {
+    ImgLayout(int W, int H, int V = 1, bool depth_stats = false)
+        : gx((W + R3DG_TILE - 1) / R3DG_TILE), gy((H + R3DG_TILE - 1) / R3DG_TILE) {
         const size_t HW = (size_t)W * H * V, T = (size_t)gx * gy, VT = T * V;
         max_chunks = bin_max_chunks(T);
         size_t off = 0;
@@ -86,6 +90,8 @@ struct ImgLayout {
         bwd_order = off; off = align_up(off + 2 * VT * 4, 256);  // half-tile CTAs by descending bwd_work (backward launch order)
         slab_sum = off;  off = align_up(off + T * 4 * ((R3DG_BIN_MAX_CHUNKS + 511) / 512), 256);   // per 512-chunk slab
         bin_matrix = off; off = align_up(off + ((size_t)max_chunks + 1) * T * 4, 256);   // + the row of list ends
+        median_pos = off; depth_bound = align_up(off + HW * 4, 256);
+        if (depth_stats) off = align_up(depth_bound + (size_t)V * 4, 256);
         total = off;
     }
 };
@@ -116,9 +122,10 @@ size_t bin_bytes_for_capacity(long long cap) { return (size_t)((cap + 63) / 64 *
 // when a buffer is smaller than its layout or the binning buffer holds no instance, and fills `b` either way
 // (r3dg_raster_debug_copy passes SIZE_MAX for the sizes it is not given, and needs the binning only for some ids).
 int raster_buffers(int P, int S, int W, int H, void* geom_, size_t geom_bytes, void* img_, size_t img_bytes,
-                   void* bin_, size_t bin_bytes, RasterBuffers& b, int V = 1, bool ray_depth = false) {
+                   void* bin_, size_t bin_bytes, RasterBuffers& b, int V = 1, bool ray_depth = false,
+                   bool depth_stats = false) {
     const GeomLayout gl(P < 1 ? 1 : P, S, V, ray_depth);
-    const ImgLayout il(W, H, V);
+    const ImgLayout il(W, H, V, depth_stats);
     const BinLayout bl(bin_capacity_for_bytes(bin_bytes));
     char *geom = (char*)geom_, *img = (char*)img_, *bin = (char*)bin_;
     b.header = (GeomHeader*)(geom + gl.header);
@@ -128,6 +135,7 @@ int raster_buffers(int P, int S, int W, int H, void* geom_, size_t geom_bytes, v
     b.clamped = (uint8_t*)(geom + gl.clamped);
     b.sort = geom + gl.sort; b.sort_layout = gl.sl;
     b.final_T = (float*)(img + il.final_T); b.n_contrib = (int*)(img + il.n_contrib);
+    b.median_pos = (int*)(img + il.median_pos); b.depth_bound = (uint32_t*)(img + il.depth_bound);   // (depth statistics)
     b.ranges = (uint2*)(img + il.ranges); b.tile_order = (uint32_t*)(img + il.tile_order);
     b.bwd_work = (uint32_t*)(img + il.bwd_work); b.bwd_order = (uint32_t*)(img + il.bwd_order);
     b.slab_sum = (uint32_t*)(img + il.slab_sum); b.bin_matrix = (uint32_t*)(img + il.bin_matrix);
@@ -178,6 +186,7 @@ size_t r3dg_raster_views_geom_bytes(int P, int S, int V) { return GeomLayout(P <
 size_t r3dg_raster_views_img_bytes(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).total; }
 size_t r3dg_raster_views_img_n_contrib_offset(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V).n_contrib; }
 size_t r3dg_raster_ray_depth_geom_bytes(int P, int S, int V) { return GeomLayout(P < 1 ? 1 : P, S, V < 1 ? 1 : V, true).total; }
+size_t r3dg_raster_depth_stats_img_bytes(int W, int H, int V) { return ImgLayout(W, H, V < 1 ? 1 : V, true).total; }
 size_t r3dg_raster_fwd_det_bytes(int P) { return align_up((size_t)(P < 1 ? 1 : P) * 8, 256); }
 size_t r3dg_raster_bwd_det_bytes(int P, int S) { return det_bytes((size_t)(P < 1 ? 1 : P) * rec_floats(S < 0 ? 0 : S)); }
 size_t r3dg_raster_ray_depth_bwd_det_bytes(int P, int S) {
@@ -215,11 +224,12 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
     if (misaligned16(a->rotations)) return R3DG_ERR_BAD_ARG;
     if (a->shs && a->M > 16) return R3DG_ERR_UNSUPPORTED;
     if (a->filter_3d && a->cov3D_precomp) return R3DG_ERR_BAD_ARG;       // the 3D filter is defined on scales
+    if (a->depth_stats && (!a->out_depth2 || !a->out_median_depth)) return R3DG_ERR_BAD_ARG;
     const int V = views_of(a->V, a->view_cams, a->P);
     if (V == 0) return R3DG_ERR_BAD_ARG;
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
-                            a->binning_bytes, b, V, a->ray_depth != 0);
+                            a->binning_bytes, b, V, a->ray_depth != 0, a->depth_stats != 0);
     if (rc != 0) return rc;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(V * a->P))) return R3DG_ERR_BAD_ARG;
     if (V > 1 && (b.gx > 65535 || b.gy > 65535 || b.tiles > 65535)) return R3DG_ERR_UNSUPPORTED;   // the binning's limits, before any launch
@@ -288,6 +298,11 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     if (V > 1 && a->P > 0 && a->shs && (geometry || a->dL_dsh) && (!a->dL_dsh_factor || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     if (cam_outs != 0 && cam_outs != 3) return R3DG_ERR_BAD_ARG;
     if (geometry && a->filter_3d && (a->cov3D_precomp || !a->opacities)) return R3DG_ERR_BAD_ARG;
+    // depth statistics: the flag with both cotangents and the forward's larger image buffer, or neither cotangent
+    const bool ds = geometry && a->depth_stats != 0;
+    if (ds && (!a->dL_dout_depth2 || !a->dL_dout_median_depth ||
+               a->img_bytes < r3dg_raster_depth_stats_img_bytes(a->W, a->H, V))) return R3DG_ERR_BAD_ARG;
+    if (geometry && !ds && (a->dL_dout_depth2 || a->dL_dout_median_depth)) return R3DG_ERR_BAD_ARG;
     const bool cam = cam_outs == 3;
     if (cam && (!a->cam_work || a->cam_work_bytes < r3dg_raster_cam_grad_bytes(a->P, V))) return R3DG_ERR_BAD_ARG;
     // (appearance-only: the opacity, depth, pseudo-normal and surface-xyz cotangents have no appearance gradient)
@@ -304,7 +319,7 @@ int r3dg_raster_backward(const r3dg_raster_bwd_args* a, r3dg_stream_t stream_) {
     }
     RasterBuffers b;
     int rc = raster_buffers(a->P, a->S, a->W, a->H, a->geom, a->geom_bytes, a->img, a->img_bytes, a->binning,
-                            a->binning_bytes, b, V, a->ray_depth != 0);
+                            a->binning_bytes, b, V, a->ray_depth != 0, ds);
     if (rc != 0) return rc;
     prof_mark(false, 8, stream);
     // pseudo-normal / surface-xyz cotangents: their pull-back joins the depth and opacity cotangents, and the compositor
@@ -689,6 +704,7 @@ static long long debug_copy(bool ray_depth, int id, int P, int S, int W, int H, 
         }
         case 13: return copy(b.final_T, 4 * HW);
         case 14: return copy(b.n_contrib, 4 * HW);
+        case 23: return copy(b.median_pos, 4 * HW);    // (the caller checks that the buffer has the region)
         case 15: return copy(b.ranges, 8 * (size_t)b.tiles);
         case 16: return copy(b.bwd_work, 8 * (size_t)b.tiles);
         case 17: return copy(b.bwd_order, 8 * (size_t)b.tiles);

@@ -45,6 +45,9 @@ struct CompositeFwdParams {
     float *out_color, *out_opacity, *out_depth, *out_feature, *out_weights;
     uint64_t* det_weights;             // DET: [P] out_weights in exact 2^-24 units (zeroed), converted by det_weights_kernel
     uint32_t* clamped32;               // the rows' clamped bytes as words: kComposited is set for every composited row
+    float *out_depth2, *out_median;    // DS: sum w d^2 and the median depth per pixel
+    int* median_pos;                   // DS: the median entry's 1-based position in the tile list (0: none)
+    uint32_t* depth_bound;             // DS: per view, the largest |d| of an accepted entry as float bits (zeroed)
 };
 
 // NW = warps per CTA (4: two CTAs per tile).  Warps are autonomous: no
@@ -64,9 +67,14 @@ struct CompositeFwdParams {
 //   out_weights does not depend on the order in which warps finish.  Everything else is the same code.
 // RD (ray-depth mode, register prefetch only): the record's appended group, the depth plane p, is staged with the
 //   others, and an entry adds  tz - p.x dx - p.y dy  (dx, dy its mean minus the pixel) to the depth instead of tz.
-template <int NG, int NW, int MINB, bool BULK, bool DET = false, bool RD = false>
+// DS (depth statistics, register prefetch only): the entry's depth d (the one added to the depth) also goes into
+//   sum w d^2 (as w * (d * d), the rounding of a d^2 feature channel), and the running median: while T before an
+//   accepted entry is > 0.5 the entry's d and 1-based list position replace the previous ones (2DGS's rule).  The
+//   warp's largest |d| of an accepted entry goes to its view's bound word (the deterministic backward's scale).
+template <int NG, int NW, int MINB, bool BULK, bool DET = false, bool RD = false, bool DS = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const CompositeFwdParams p) {
     static_assert(!(BULK && RD), "the bulk-copy slab holds records without the depth plane");
+    static_assert(!(BULK && DS), "the depth statistics are instantiated with the register prefetch only");
     constexpr int RG = 2 + NG;                       // float4 groups per record
     constexpr int RGX = RG + (RD ? 1 : 0);           // staged groups: RD adds the depth plane (group RG)
     __shared__ __align__(16) float4 sRec[BULK ? 1 : NW][BULK ? 1 : RGX][BULK ? 1 : 32];   // this warp's current 32-entry batch, SoA
@@ -97,6 +105,8 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
 #pragma unroll
     for (int i = 0; i < 4 * NG; ++i) C[i] = 0.0f;
     uint32_t last_contributor = 0;
+    float D2 = 0.0f, med = 0.0f, dmax = 0.0f;                           // DS only
+    uint32_t med_pos = 0u;
     bool done = !inside;
 
     // ---- mask stream: word w holds instances [4w, 4w+4); lane takes word w_next + lane --------------------
@@ -201,6 +211,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             for (int g = 0; g < RGX; ++g) r[g] = rec4[(size_t)id_cur * rec4n + g];
         }
         int last_k = -1;                                                // this pixel's last accepted entry of the batch
+        int med_k = -1;                                                 // DS: its median entry of the batch, if any
         int my_wsum = 0;                                                // lane k keeps the warp's weight sum of entry k
         // U staged entries per round.  The alpha evaluations (record fetch, quadratic form, exp — two thirds of the
         // work) depend neither on one another nor on the pixel's state, so all U are issued back to back: U dependency
@@ -246,6 +257,14 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
                     fma4_if(valid, w, c, C[4 * g + 0], C[4 * g + 1], C[4 * g + 2], C[4 * g + 3]);
                 }
                 fma_add_if(valid, w, dep[u], Dp, Op);
+                if constexpr (DS) {
+                    const float d2 = mul_(dep[u], dep[u]);
+                    D2 = valid ? fma_(w, d2, D2) : D2;
+                    const bool m = valid && T > 0.5f;                    // T before the entry (2DGS's median rule)
+                    med = m ? dep[u] : med;
+                    med_k = m ? k0 + u : med_k;
+                    dmax = valid ? fmaxf(dmax, fabsf(dep[u])) : dmax;
+                }
                 T = valid ? test_T : T;
                 last_k = valid ? k0 + u : last_k;
                 // w in [0,1) in 2^-24 fixed point for the out_weights statistic (below); >= 6 whenever the entry was accepted
@@ -262,6 +281,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             if (__all_sync(0xffffffffu, done)) { all_done = true; break; }      // once per round: entries after the last
         }                                                                        // pixel finished change nothing (valid needs !done)
         if (last_k >= 0) last_contributor = sPos[warp][last_k] + 1u;    // 1-based position in the tile list
+        if (DS && med_k >= 0) med_pos = sPos[warp][med_k] + 1u;
         const uint32_t cw = __ballot_sync(0xffffffffu, my_wsum != 0);   // bit k: entry k was composited by some pixel
         if (my_wsum != 0) {
             const uint32_t id = sId[warp][lane];
@@ -277,6 +297,10 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
         composited += (uint32_t)__popc(cw);
     }
     if (lane == 0 && composited) atomicMax(&p.bwd_work[blockIdx.x % PARTS + PARTS * tile], composited);
+    if constexpr (DS) {                                 // |d| as float bits: integer order is float order
+        const uint32_t b = __reduce_max_sync(0xffffffffu, __float_as_uint(dmax));
+        if (lane == 0 && b) atomicMax(p.depth_bound + view, b);
+    }
     if (inside) {
         const size_t HW = (size_t)p.H * p.W, pix = (size_t)p.W * py + px, vpix = (size_t)view * HW + pix;
         p.final_T[vpix] = T;
@@ -288,6 +312,11 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_fwd_kernel(const Comp
             if (ch - 3 < p.S) p.out_feature[((size_t)view * p.S + (ch - 3)) * HW + pix] = C[ch];
         p.out_depth[vpix] = Dp;
         p.out_opacity[vpix] = Op;
+        if constexpr (DS) {
+            p.out_depth2[vpix] = D2;
+            p.out_median[vpix] = med;
+            p.median_pos[vpix] = (int)med_pos;
+        }
     }
 }
 
@@ -353,6 +382,11 @@ __global__ void __launch_bounds__(256) surface_normal_kernel(int W, int H, const
 template <int NG> struct FwdOcc { static constexpr int v = NG <= 2 ? 7 : (NG <= 3 ? 6 : (NG <= 5 ? 5 : (NG <= 6 ? 4 : 3))); };
 // ray-depth mode (the depth plane's 4 more prefetch registers): fewer CTAs where the count above spills (-Xptxas -v)
 template <int NG> struct FwdOccRD { static constexpr int v = FwdOcc<NG>::v - (NG == 2 ? 2 : (NG == 5 ? 1 : 0)); };
+// depth statistics (five more per-pixel registers), without and with the ray-depth mode: fewer CTAs where the counts
+// above spill (-Xptxas -v)
+template <int NG, bool RD> struct FwdOccDS {
+    static constexpr int v = RD ? FwdOccRD<NG>::v - (NG <= 3 ? 1 : 0) : FwdOcc<NG>::v - (NG == 2 ? 2 : (NG == 3 || NG == 5 ? 1 : 0));
+};
 
 int g_composite_bulk = 0;       // r3dg_tune("composite_bulk"): 1 = TMA bulk-copy record staging in the forward compositor
 int g_fwd_ctas = 0;             // r3dg_tune("composite_fwd_ctas"): resident CTAs per SM (0 = whatever fits)
@@ -376,7 +410,17 @@ static void launch_fwd_kernel(const CompositeFwdParams& p, int tiles, cudaStream
     K<<<tiles * 2, 128, residency_pad<K>(g_fwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
-static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, bool ray_depth, cudaStream_t stream) {
+static void launch_fwd_ng(const CompositeFwdParams& p, int tiles, bool ray_depth, bool ds, cudaStream_t stream) {
+    if (ds) {                                         // (register prefetch, as the ray-depth mode)
+        if (ray_depth) {
+            if (p.det_weights) launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccDS<NG, true>::v, false, true, true, true>>(p, tiles, stream);
+            else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccDS<NG, true>::v, false, false, true, true>>(p, tiles, stream);
+        } else {
+            if (p.det_weights) launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccDS<NG, false>::v, false, true, false, true>>(p, tiles, stream);
+            else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccDS<NG, false>::v, false, false, false, true>>(p, tiles, stream);
+        }
+        return;
+    }
     if (ray_depth) {                                  // (register prefetch: r3dg_tune("composite_bulk") does not apply)
         if (p.det_weights) launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccRD<NG>::v, false, true, true>>(p, tiles, stream);
         else launch_fwd_kernel<composite_fwd_kernel<NG, 4, FwdOccRD<NG>::v, false, false, true>>(p, tiles, stream);
@@ -410,20 +454,24 @@ int launch_composite_forward(const r3dg_raster_fwd_args& a, const RasterBuffers&
     p.out_feature = a.out_feature; p.out_weights = a.out_weights;
     p.det_weights = a.deterministic ? (uint64_t*)a.det_work : nullptr;
     p.clamped32 = (uint32_t*)b.clamped;               // 256-byte aligned, padded to whole words (api.cu GeomLayout)
+    const bool ds = a.depth_stats != 0;
+    p.out_depth2 = a.out_depth2; p.out_median = a.out_median_depth;
+    p.median_pos = b.median_pos; p.depth_bound = b.depth_bound;
+    if (ds) R3DG_CUDA_TRY(cudaMemsetAsync(b.depth_bound, 0, V * sizeof(uint32_t), stream));
     const size_t rows = (size_t)V * a.P;
     if (p.det_weights) R3DG_CUDA_TRY(cudaMemsetAsync(p.det_weights, 0, rows * 8, stream));
     const int tiles = V * b.tiles;                    // the tall grid of all views
     const bool rd = a.ray_depth != 0;
     switch (num_groups(a.S)) {
-        case 1: launch_fwd_ng<1>(p, tiles, rd, stream); break;
-        case 2: launch_fwd_ng<2>(p, tiles, rd, stream); break;
-        case 3: launch_fwd_ng<3>(p, tiles, rd, stream); break;
-        case 4: launch_fwd_ng<4>(p, tiles, rd, stream); break;
-        case 5: launch_fwd_ng<5>(p, tiles, rd, stream); break;
-        case 6: launch_fwd_ng<6>(p, tiles, rd, stream); break;
-        case 7: launch_fwd_ng<7>(p, tiles, rd, stream); break;
-        case 8: launch_fwd_ng<8>(p, tiles, rd, stream); break;
-        case 9: launch_fwd_ng<9>(p, tiles, rd, stream); break;
+        case 1: launch_fwd_ng<1>(p, tiles, rd, ds, stream); break;
+        case 2: launch_fwd_ng<2>(p, tiles, rd, ds, stream); break;
+        case 3: launch_fwd_ng<3>(p, tiles, rd, ds, stream); break;
+        case 4: launch_fwd_ng<4>(p, tiles, rd, ds, stream); break;
+        case 5: launch_fwd_ng<5>(p, tiles, rd, ds, stream); break;
+        case 6: launch_fwd_ng<6>(p, tiles, rd, ds, stream); break;
+        case 7: launch_fwd_ng<7>(p, tiles, rd, ds, stream); break;
+        case 8: launch_fwd_ng<8>(p, tiles, rd, ds, stream); break;
+        case 9: launch_fwd_ng<9>(p, tiles, rd, ds, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;
     }
     if (p.det_weights && a.P > 0) det_weights_kernel<<<(int)((rows + 255) / 256), 256, 0, stream>>>((int)rows, p.det_weights, a.out_weights);

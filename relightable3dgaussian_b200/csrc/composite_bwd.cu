@@ -45,6 +45,9 @@ struct CompositeBwdParams {
     // accumulators of the geometry class behind the gradient rows' (det_abs)
     float* abs_grad;
     DetAcc det_abs;
+    const float *dL_dpix_d2, *dL_dpix_m;   // DS: the cotangents of depth2 and of the median depth
+    const int* median_pos;                 // DS: the forward's median entry per pixel (1-based list position, 0: none)
+    const uint32_t* depth_bound;           // DS: per view, the forward's largest |d| of an accepted entry (float bits)
 };
 
 // Per warp (one 8x4 pixel block): the forward pass left one contributor bit per (instance, block).  The warp streams
@@ -78,10 +81,15 @@ struct CompositeBwdParams {
 // gets dL/dp = -(those sums), and the dL/dmean2D slots get d's own term  -p dL/dtz  (times W/2, H/2), added after the
 // alpha term, so that a zero depth cotangent leaves them as they are.  With ABS, the per-pixel magnitudes are those of
 // the two terms together.
-template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true, bool ABS = false, bool RD = false>
+// DS (depth statistics, GEOM only): with g2, gm the pixel's cotangents of depth2 and of the median depth, dL/dalpha's
+// per-pixel scalar gains  d^2 g2  and the entry's depth cotangent  dcc dL_dD  becomes  dcc (dL_dD + 2 d g2) + [the
+// entry is the pixel's median] gm  wherever it enters: the dL/dtz slot and, with RD, the dL/dp sums and  -p dL/dtz.
+// The median entry is the forward's (its stored list position), never re-derived from the recomputed T.
+template <int NG, int NW, int MINB, bool DET = false, bool GEOM = true, bool ABS = false, bool RD = false, bool DS = false>
 __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const CompositeBwdParams p) {
     static_assert(GEOM || !ABS, "absgrad needs the geometry half of the backward");
     static_assert(GEOM || !RD, "the depth plane's gradient needs the geometry half of the backward");
+    static_assert(GEOM || !DS, "the depth statistics' gradients need the geometry half of the backward");
     constexpr int NC = 4 * NG;              // padded channel count {r,g,b,f...}; gradient row = 8 geometry slots + NC
     constexpr int GOFF = GEOM ? 8 : 0;      // slot of channel 0 in the gradient row (GEOM = false: no geometry slots)
     constexpr int ROWF = GOFF + NC + (RD ? 4 : 0);   // floats per gradient row (p.recf with GEOM); RD: + dL/dp group
@@ -144,6 +152,12 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 #pragma unroll
     for (int g = 0; g < NG; ++g) sCot[warp][g][lane] = make_float4(dpix[4 * g], dpix[4 * g + 1], dpix[4 * g + 2], dpix[4 * g + 3]);
     sCotD[warp][lane] = dpix_d;                              // (read by the entry phase after the first __syncwarp)
+    // DS: this lane's pixel's depth2 and median cotangents and its median entry's 0-based list position (-1: none).
+    // The entry phase reads them by shuffles from the pixel's lane (the static shared memory is at its 48 KB limit).
+    const float dpix_d2 = DS && inside ? p.dL_dpix_d2[vpix] : 0.0f;
+    const float dpix_d2x2 = 2.0f * dpix_d2;
+    const float dpix_m = DS && inside ? p.dL_dpix_m[vpix] : 0.0f;
+    const int pix_med = DS && inside ? p.median_pos[vpix] - 1 : -1;
     const float* bg = p.bg + 3 * view;
     const float bg_dot = GEOM ? bg[0] * dpix[0] + bg[1] * dpix[1] + bg[2] * dpix[2] : 0.0f;
     const float ddelx_dx = 0.5f * p.W, ddely_dy = 0.5f * p.H;
@@ -255,6 +269,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                             dep = fmaf(-pl.y, dy, fmaf(-pl.x, dx, b.z));
                         }
                         d = fmaf(dep, dpix_d, dpix_o);                      // depth * dL_ddepth + 1 * dL_dopacity
+                        if constexpr (DS) d = fmaf(dep * dep, dpix_d2, d);  // + depth^2 * dL_ddepth2
                         const float4 c0 = sRec[warp][2][j], t0 = sCot[warp][0][lane];
                         d = fmaf(c0.z, t0.z, fmaf(c0.y, t0.y, fmaf(c0.x, t0.x, d)));
                         // feature channels enter dL_dalpha only when backward_geometry is set (backward.cu:563-566)
@@ -292,6 +307,7 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
             float sw = 0.f, s0 = 0.f, s1 = 0.f, sxx = 0.f, sxy = 0.f, syy = 0.f, sd = 0.f, ax = 0.f, ay = 0.f;
             float sdx = 0.f, sdy = 0.f;                                     // RD: sums of dcc dL_dD dx, dcc dL_dD dy
             const float4 pl = RD ? sRec[warp][RGX - 1][je] : make_float4(0.f, 0.f, 0.f, 0.f);
+            const int ke = DS ? (int)sK[warp][je] : 0;                     // DS: the entry's list position
             float sc[NC];
 #pragma unroll
             for (int c = 0; c < NC; ++c) sc[c] = 0.0f;
@@ -313,9 +329,20 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
                     const float wdx = w * dx, wdy = w * dy;
                     sw += w;
                     sxx = fmaf(wdx, dx, sxx); sxy = fmaf(wdx, dy, sxy); syy = fmaf(wdy, dy, syy);
-                    sd = fmaf(c, sCotD[warp][pb], sd);
+                    // the entry's depth cotangent at the pixel: dcc dL_dD (DS: dcc (dL_dD + 2 d g2) + [median] gm)
+                    float cot = sCotD[warp][pb], gm = 0.0f;
+                    bool is_med = false;
+                    if constexpr (DS) {
+                        const float dd = RD ? fmaf(-pl.y, dy, fmaf(-pl.x, dx, b.z)) : b.z;   // the forward's d
+                        cot = fmaf(dd, __shfl_sync(0xffffffffu, dpix_d2x2, pb), cot);
+                        is_med = __shfl_sync(0xffffffffu, pix_med, pb) == ke;
+                        gm = __shfl_sync(0xffffffffu, dpix_m, pb);
+                    }
+                    sd = fmaf(c, cot, sd);
+                    if (DS && is_med) sd = add_(sd, gm);
                     if constexpr (RD) {
-                        const float cd = c * sCotD[warp][pb];
+                        float cd = c * cot;
+                        if (DS && is_med) cd = add_(cd, gm);
                         sdx = fmaf(cd, dx, sdx); sdy = fmaf(cd, dy, sdy);
                         if constexpr (ABS) {                                // the pixel's whole dL/dmean2D term / (W/2)
                             ax = add_(ax, fabsf(fmaf(b.y, t0, pl.x * cd))); ay = add_(ay, fabsf(fmaf(b.y, t1, pl.y * cd)));
@@ -421,20 +448,36 @@ __global__ void __launch_bounds__(32 * NW, MINB) composite_bwd_kernel(const Comp
 // kernels that read its rows take the class exponents from these words (det_scale_exp): a V-view call scales each
 // view as its one-view call does.  Every thread of the first `nblocks` blocks calls it (256 threads each): one
 // atomicMax per block and word.
+// Depth statistics (p.depth_bound set): the cotangents of depth2 and of the median depth join the geometry class.  A
+// depth2 term carries d^2 g2 (in dL/dalpha) or 2 d g2 (in the depth cotangent), so its plane enters as
+// |g2| max(Z^2, 2 Z) with Z the view's largest |d| of an accepted entry (from the forward): scaled by the class
+// exponent, every new term is then bounded as the flag-off ones are (DESIGN.md §4.21).  A product beyond fp32 enters
+// as FLT_MAX (the exponent clamps at R3DG_DET_SCALE_MAX); a zero cotangent enters as 0, so that zero cotangents leave
+// the exponent, and every bit of the result, as without the statistics.
 __device__ void det_scale_reduce(const CompositeBwdParams& p, int V, bool geometry, int nblocks, uint32_t* __restrict__ scale) {
     __shared__ uint32_t s_max[2][8];
-    const size_t HW = (size_t)p.H * p.W, n_app = (size_t)(3 + p.S) * HW, n = n_app + (geometry ? 2 * HW : 0);
+    const bool ds = geometry && p.depth_bound != nullptr;
+    const size_t HW = (size_t)p.H * p.W, n_app = (size_t)(3 + p.S) * HW, n = n_app + (geometry ? (ds ? 4 : 2) * HW : 0);
     const size_t stride = (size_t)nblocks * blockDim.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int v = 0; v < V; ++v) {
         const float* col = p.dL_dpix + (size_t)v * 3 * HW;
         const float* feat = p.dL_dpix_f + (size_t)v * p.S * HW;
         uint32_t m_app = 0u, m_geo = 0u;
+        float zf = 0.0f;                                         // DS: max(Z^2, 2 Z)
+        if (ds) { const float z = __uint_as_float(p.depth_bound[v]); zf = fmaxf(z * z, 2.0f * z); }
         for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
             if (i < 3 * HW) m_app = max(m_app, det_abs_bits(col[i]));
             else if (i < n_app) m_app = max(m_app, det_abs_bits(feat[i - 3 * HW]));
             else if (i < n_app + HW) m_geo = max(m_geo, det_abs_bits(p.dL_dpix_o[(size_t)v * HW + (i - n_app)]));
-            else m_geo = max(m_geo, det_abs_bits(p.dL_dpix_d[(size_t)v * HW + (i - n_app - HW)]));
+            else if (i < n_app + 2 * HW) m_geo = max(m_geo, det_abs_bits(p.dL_dpix_d[(size_t)v * HW + (i - n_app - HW)]));
+            else if (i < n_app + 3 * HW) {
+                const float g = p.dL_dpix_d2[(size_t)v * HW + (i - n_app - 2 * HW)];
+                const uint32_t b = g == 0.0f ? 0u : (g != g ? det_abs_bits(g) : det_abs_bits(fminf(fabsf(g) * zf, 3.40282347e38f)));
+                m_geo = max(m_geo, b);
+            } else {
+                m_geo = max(m_geo, det_abs_bits(p.dL_dpix_m[(size_t)v * HW + (i - n_app - 3 * HW)]));
+            }
         }
         m_geo = max(m_app, m_geo);
         m_app = __reduce_max_sync(0xffffffffu, m_app);
@@ -502,6 +545,11 @@ uint32_t* raster_det_scale(const RasterBuffers& b) {
 template <int NG> struct BwdOcc { static constexpr int v = NG <= 2 ? 5 : (NG <= 4 ? 4 : 3); };
 // ray-depth mode (two more entry-phase sums and the depth plane): one CTA fewer where the count above spills
 template <int NG> struct BwdOccRD { static constexpr int v = BwdOcc<NG>::v - (NG == 1 || NG == 2 || NG == 4 ? 1 : 0); };
+// depth statistics (three more per-pixel planes read by the entry phase), without and with the ray-depth mode: fewer
+// CTAs where the counts above spill
+template <int NG, bool RD> struct BwdOccDS {
+    static constexpr int v = RD ? BwdOccRD<NG>::v - (NG == 3 || NG == 7 ? 1 : 0) : BwdOcc<NG>::v - (NG == 2 || NG == 4 ? 1 : 0);
+};
 int g_bwd_ctas = 0;             // r3dg_tune("composite_bwd_ctas"): resident CTAs per SM (0 = whatever fits)
 int composite_bwd_tune(const char* key, int value, int* previous) {
     if (strcmp(key, "composite_bwd_ctas") != 0) return R3DG_ERR_UNSUPPORTED;
@@ -510,14 +558,25 @@ int composite_bwd_tune(const char* key, int value, int* previous) {
     g_bwd_ctas = value;
     return 0;
 }
-template <int NG, bool DET, bool GEOM, bool ABS = false, bool RD = false>
+template <int NG, bool DET, bool GEOM, bool ABS = false, bool RD = false, bool DS = false>
 static void launch_bwd_kernel(const CompositeBwdParams& p, int tiles, cudaStream_t stream) {
-    constexpr auto kernel = composite_bwd_kernel<NG, 4, RD ? BwdOccRD<NG>::v : BwdOcc<NG>::v, DET, GEOM, ABS, RD>;
+    constexpr int minb = DS ? BwdOccDS<NG, RD>::v : (RD ? BwdOccRD<NG>::v : BwdOcc<NG>::v);
+    constexpr auto kernel = composite_bwd_kernel<NG, 4, minb, DET, GEOM, ABS, RD, DS>;
     kernel<<<tiles * 2, 128, residency_pad<kernel>(g_bwd_ctas), stream>>>(p);    // two 4-warp CTAs per tile
 }
 template <int NG>
 static void launch_bwd_ng(const CompositeBwdParams& p, int tiles, bool det, bool geometry, bool absgrad, bool rd,
-                          cudaStream_t stream) {
+                          bool ds, cudaStream_t stream) {
+    if (geometry && ds) {                             // (absgrad implies geometry)
+        if (rd) {
+            if (absgrad) det ? launch_bwd_kernel<NG, true, true, true, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, true, true, true>(p, tiles, stream);
+            else det ? launch_bwd_kernel<NG, true, true, false, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, false, true, true>(p, tiles, stream);
+        } else {
+            if (absgrad) det ? launch_bwd_kernel<NG, true, true, true, false, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, true, false, true>(p, tiles, stream);
+            else det ? launch_bwd_kernel<NG, true, true, false, false, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, false, false, true>(p, tiles, stream);
+        }
+        return;
+    }
     if (geometry && rd) {                             // (absgrad implies geometry)
         if (absgrad) det ? launch_bwd_kernel<NG, true, true, true, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, true, true>(p, tiles, stream);
         else det ? launch_bwd_kernel<NG, true, true, false, true>(p, tiles, stream) : launch_bwd_kernel<NG, false, true, false, true>(p, tiles, stream);
@@ -544,6 +603,10 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     p.final_T = b.final_T;
     p.dL_dpix = a.dL_dout_color; p.dL_dpix_o = a.dL_dout_opacity; p.dL_dpix_d = a.dL_dout_depth;
     p.dL_dpix_f = a.dL_dout_feature;
+    // depth statistics (geometry only: the appearance-only backward reads neither cotangent)
+    const bool ds = geometry && a.depth_stats != 0;
+    p.dL_dpix_d2 = ds ? a.dL_dout_depth2 : nullptr; p.dL_dpix_m = ds ? a.dL_dout_median_depth : nullptr;
+    p.median_pos = b.median_pos; p.depth_bound = ds ? b.depth_bound : nullptr;
     p.grad = b.grad;
     p.n_contrib = b.n_contrib;
     const bool det = a.deterministic != 0;
@@ -570,13 +633,13 @@ int launch_composite_backward(const r3dg_raster_bwd_args& a, const RasterBuffers
     if (rc != 0) return rc;
     const bool rd = a.ray_depth != 0;
     switch (num_groups(a.S)) {
-        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, absgrad, rd, stream); break;
-        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, absgrad, rd, stream); break;
-        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, absgrad, rd, stream); break;
-        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, absgrad, rd, stream); break;
-        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, absgrad, rd, stream); break;
-        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, absgrad, rd, stream); break;
-        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, absgrad, rd, stream); break;
+        case 1: launch_bwd_ng<1>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
+        case 2: launch_bwd_ng<2>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
+        case 3: launch_bwd_ng<3>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
+        case 4: launch_bwd_ng<4>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
+        case 5: launch_bwd_ng<5>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
+        case 6: launch_bwd_ng<6>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
+        case 7: launch_bwd_ng<7>(p, tiles, det, geometry, absgrad, rd, ds, stream); break;
         default: return R3DG_ERR_UNSUPPORTED;   // S > 24: reference backward limit (backward.cu:449)
     }
     R3DG_CUDA_TRY(cudaGetLastError());

@@ -19,6 +19,8 @@ struct RasterBuffers {
     SortLayout sort_layout{0};
     float* final_T;                                                                // img: per pixel and per tile
     int* n_contrib;
+    int* median_pos;                                                               // img, depth statistics only: per pixel
+    uint32_t* depth_bound;                                                         //   and per view (api.cu ImgLayout)
     uint2* ranges;
     uint32_t *tile_order, *bwd_work, *bwd_order, *slab_sum, *bin_matrix;
     uint32_t* point_list;                                                          // binning: per instance

@@ -101,6 +101,26 @@ def _rerun_rd_kw(ray_depth):
     return {"ray_depth": bool(ray_depth)} if ray_depth or _C.ray_depth_default() else {}
 
 
+def _ds_kw(depth_stats):
+    """The keyword that turns on the library's depth statistics, only when they are on: an off call is the call without
+    them."""
+    return {"depth_stats": True} if depth_stats else {}
+
+
+def _ds_bwd_kw(ctx, g_stats):
+    """The backward's depth-statistics keywords: the flag and the cotangents of depth2 and median_depth (None: zeros),
+    only when the node's forward had them on."""
+    if not getattr(ctx, "depth_stats", False):
+        return {}
+    g2, gm = (tuple(g_stats) + (None, None))[:2]
+    return {"depth_stats": True, "dL_dout_depth2": g2, "dL_dout_median_depth": gm}
+
+
+def _stats_outputs(ctx, out):
+    """The node's outputs: the reference's ten, then depth2 and median_depth when the depth statistics are on."""
+    return out[:10] + (tuple(out[13:15]) if ctx.depth_stats else ())
+
+
 def _set_absgrad(means2D, g_abs):
     """Adds g_abs to `means2D.absgrad` on the caller's tensor object, as autograd accumulates `.grad`: set on the first
     backward, summed with what is there on later ones (retain_graph, or a tensor used in several graphs)."""
@@ -177,14 +197,14 @@ def _surface_cotangents(ctx, g_normal, g_surface_xyz):
 def _input_grads(ctx, grads, cameras):
     """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
     three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
-    one, and for all three when none was computed.  The last three inputs, the 3D filter (a buffer, as in
-    Mip-Splatting) and the antialiasing, ray-depth and absgrad flags, get None."""
+    one, and for all three when none was computed.  The last five inputs, the 3D filter (a buffer, as in
+    Mip-Splatting) and the antialiasing, ray-depth, depth-statistics and absgrad flags, get None."""
     g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
     cam = (None, None, None)
     if grads[9:]:
         cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[11:14]))
     return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
-            None, None) + cam + (None, None, None, None)
+            None, None) + cam + (None, None, None, None, None)
 
 
 # the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
@@ -239,15 +259,16 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing,
-                ray_depth, absgrad):
+                ray_depth, depth_stats, absgrad):
         rs = raster_settings
         out = _debug_call(rs.debug, _C.rasterize_gaussians,
                           _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
                                         cov3Ds_precomp),
                           "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
                           _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad),
-                          **_aa_kw(antialiasing), **_f3d_kw(filter_3d), **_rd_kw(ray_depth))
+                          **_aa_kw(antialiasing), **_f3d_kw(filter_3d), **_rd_kw(ray_depth), **_ds_kw(depth_stats))
         ctx.raster_settings = rs
+        ctx.depth_stats = depth_stats
         ctx.antialiasing = antialiasing
         ctx.ray_depth = ray_depth
         ctx.absgrad = absgrad
@@ -255,11 +276,11 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.num_rendered = out[0]
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
                       out[9], sh, *out[10:13], opacities, filter_3d)
-        return out[:10]
+        return _stats_outputs(ctx, out)
 
     @staticmethod
     def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature,
-                 g_normal, g_surface_xyz, g_weights, g_radii):
+                 g_normal, g_surface_xyz, g_weights, g_radii, *g_stats):
         rs = ctx.raster_settings
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, radii, sh,
          geomBuffer, binningBuffer, imgBuffer, opacities, filter_3d) = ctx.saved_tensors[:13]
@@ -282,6 +303,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         kw.update(_absgrad_kw(ctx, kw))
         kw.update(_f3d_kw(filter_3d, opacities))
         kw.update(_rd_kw(ctx.ray_depth))
+        kw.update(_ds_bwd_kw(ctx, g_stats))
         if ex is not None:
             kw["_out"] = {"sh_factor": ex[0].factor}
         if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
@@ -301,7 +323,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 out = _C.rasterize_gaussians(*_forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales,
                                                             rotations, cov3Ds_precomp),
                                              _min_capacity=int(ctx.num_rendered) + 4096, **_aa_kw(ctx.antialiasing),
-                                             **_f3d_kw(filter_3d), **_rerun_rd_kw(ctx.ray_depth))
+                                             **_f3d_kw(filter_3d), **_rerun_rd_kw(ctx.ray_depth),
+                                             **_ds_kw(ctx.depth_stats))
                 if surface is not None:         # the adjoint of the re-run's own surface pass
                     kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
                 grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
@@ -351,7 +374,7 @@ def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, feat
 
 def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacities, scales,
                         rotations, cov3Ds_precomp, raster_settings, *, surface_grads=False, antialiasing=False,
-                        absgrad=False, filter_3d=None, ray_depth=False):
+                        absgrad=False, filter_3d=None, ray_depth=False, depth_stats=False):
     """The reference's rasterize_gaussians.  With `surface_grads=True` (not part of the reference surface) the
     cotangents of the pseudo-normal (output 6) and surface_xyz (output 7) flow into the gradients of the Gaussians and,
     when `viewmatrix` requires grad, of the camera; it needs `computer_pseudo_normal`.  Off (the default), they are
@@ -391,7 +414,15 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     projection's local affine approximation.  A flat Gaussian on a tilted surface then renders as a tilted plane, not a
     fronto-parallel step, so surface_xyz and the pseudo-normal (outputs 6 and 7, derived from the depth) are smooth
     inside each footprint.  The depth cotangent reaches the plane: the means, scales, rotations, cov3Ds_precomp and the
-    view matrix get its gradient, and means2D.grad includes -p dL/dtz.  Every other output is unchanged."""
+    view matrix get its gradient, and means2D.grad includes -p dL/dtz.  Every other output is unchanged.
+
+    With `depth_stats=True` (not part of the reference surface) two more outputs follow the ten: depth2 [1,H,W], the
+    sum over the composited entries of w d^2 (d the depth the call composites: the centre's tz, or the ray-depth plane),
+    and median_depth [1,H,W], d of the last composited entry whose transmittance before it is > 0.5 (0 where nothing
+    is composited).  With op = opacity.clamp_min(1e-5), depth2 / op - (depth / op)^2 is the per-pixel depth variance of
+    the reference's `lambda_depth_var`, and opacity depth2 - depth^2 the L2 depth distortion of 2DGS and Mip-NeRF 360.
+    Both have gradients (the median's through the selected entry's depth only).  Every other output is unchanged, bit
+    for bit.  There is no process default."""
     global _CALL_GRAD_MODE
     rs = raster_settings
     _C._check_filter_3d(filter_3d, means3D.shape[0], cov3Ds_precomp)
@@ -401,19 +432,21 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
                                      scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
                                      rs.viewmatrix, rs.projmatrix, rs.campos, filter_3d, bool(antialiasing),
-                                     _ray_depth_on(ray_depth), _absgrad_on(absgrad))
+                                     _ray_depth_on(ray_depth), bool(depth_stats), _absgrad_on(absgrad))
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, surface_grads=False, antialiasing=False, absgrad=False, ray_depth=False):
-        """`surface_grads`, `antialiasing`, `absgrad` and `ray_depth` (not part of the reference surface): see
-        rasterize_gaussians."""
+    def __init__(self, raster_settings, surface_grads=False, antialiasing=False, absgrad=False, ray_depth=False,
+                 depth_stats=False):
+        """`surface_grads`, `antialiasing`, `absgrad`, `ray_depth` and `depth_stats` (not part of the reference
+        surface): see rasterize_gaussians."""
         super().__init__()
         self.raster_settings = raster_settings
         self.surface_grads = surface_grads
         self.antialiasing = antialiasing
         self.absgrad = absgrad
         self.ray_depth = ray_depth
+        self.depth_stats = depth_stats
 
     def markVisible(self, positions):
         with torch.no_grad():
@@ -428,7 +461,8 @@ class GaussianRasterizer(nn.Module):
         return rasterize_gaussians(means3D, means2D, features, shs, colors_precomp, opacities,
                                    scales, rotations, cov3D_precomp, self.raster_settings,
                                    surface_grads=self.surface_grads, antialiasing=self.antialiasing,
-                                   absgrad=self.absgrad, filter_3d=filter_3d, ray_depth=self.ray_depth)
+                                   absgrad=self.absgrad, filter_3d=filter_3d, ray_depth=self.ray_depth,
+                                   depth_stats=self.depth_stats)
 
 
 _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "prefiltered", "backward_geometry",
@@ -440,26 +474,28 @@ class _RasterizeViews(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing, ray_depth, absgrad):
+                settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing, ray_depth, depth_stats,
+                absgrad):
         rs = settings[0]
         bg = torch.stack([s.bg for s in settings])
         cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
         out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
                                  cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
                                  rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing),
-                                 **_f3d_kw(filter_3d), **_rd_kw(ray_depth))
+                                 **_f3d_kw(filter_3d), **_rd_kw(ray_depth), **_ds_kw(depth_stats))
         ctx.meta = (rs, cams, antialiasing)
+        ctx.depth_stats = depth_stats
         ctx.ray_depth = ray_depth
         ctx.absgrad = absgrad
         ctx.means2D = means2D if absgrad else None
         _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
                       bg, viewmatrix, projmatrix, campos, *out[10:13], filter_3d,
                       opacities if filter_3d is not None else None)
-        return out[:10]
+        return _stats_outputs(ctx, out)
 
     @staticmethod
     def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature, g_normal, g_surface_xyz,
-                 g_weights, g_radii):
+                 g_weights, g_radii, *g_stats):
         rs, cams, antialiasing = ctx.meta
         (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
          geomBuffer, binningBuffer, imgBuffer, filter_3d, opacities) = ctx.saved_tensors[:16]
@@ -469,6 +505,7 @@ class _RasterizeViews(torch.autograd.Function):
         kw.update(_absgrad_kw(ctx, kw))
         kw.update(_f3d_kw(filter_3d, opacities))
         kw.update(_rd_kw(ctx.ray_depth))
+        kw.update(_ds_bwd_kw(ctx, g_stats))
         if kw.get("geometry", True):
             kw.update(cam_grads=any(ctx.needs_input_grad[11:14]), surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
         grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
@@ -483,7 +520,7 @@ class _RasterizeViews(torch.autograd.Function):
 
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False,
-                    absgrad=False, filter_3d=None, ray_depth=False):
+                    absgrad=False, filter_3d=None, ray_depth=False, depth_stats=False):
     """Render V views of the same Gaussians in one forward and one backward call (not part of the reference surface).
 
     `settings` holds V `GaussianRasterizationSettings`.  They must agree on image size, `sh_degree`, `scale_modifier`,
@@ -498,7 +535,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
     `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing`, `absgrad`, `filter_3d` and `ray_depth` are
     those of rasterize_gaussians and apply to every view (each view with its own depth planes); `means2D.absgrad` is
-    then [V,P,2], each view's own."""
+    then [V,P,2], each view's own.  With `depth_stats=True`, depth2 and median_depth [V,1,H,W] follow the ten outputs,
+    as in rasterize_gaussians."""
     settings = list(settings)
     V = len(settings)
     if V < 1:
@@ -532,7 +570,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     campos = torch.stack([s.campos for s in settings])
     return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
                                  cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos,
-                                 filter_3d, bool(antialiasing), _ray_depth_on(ray_depth), _absgrad_on(absgrad))
+                                 filter_3d, bool(antialiasing), _ray_depth_on(ray_depth), bool(depth_stats),
+                                 _absgrad_on(absgrad))
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)
