@@ -817,6 +817,68 @@ int r3dg_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, co
                            size_t tmp_bytes, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Multi-view consistency losses (PGSR, Chen et al. 2024).  Not part of the reference surface.
+ * For B pairs (r, n) of V rendered views of size H x W (r = n allowed; a view may be in several pairs):
+ *   depth [V,H,W] (camera z), normal [V,3,H,W] (world frame, normalised here: n_c = normalize(R_r n) with
+ *   F.normalize's eps 1e-12), gray [V,H,W] (ground truth, no gradient), all contiguous fp32 on the device;
+ *   viewmatrix [V,16] on the device (row-vector world -> camera, as the rasterizer's), R_r its rotation;
+ *   pair_cams a HOST [B][8] of {tan_fovx, tan_fovy, cx, cy} of the reference view, then of the neighbour;
+ *   fx = W / (2 tan_fovx), fy = H / (2 tan_fovy); pixel (x, y) has the ray ((x - cx)/fx, (y - cy)/fy, 1).
+ *   pairs a HOST int [B][2] of (r, n).
+ * Per pixel p of view r, with (R, t) the ref -> neighbour camera transform and K_r, K_n the intrinsics:
+ *   geometric: X = D K_r^-1 p~ (D = depth[r](p) > 0), Y = R X + t (Y.z > 1e-6), q = pi(K_n Y) inside
+ *     [0, W-1] x [0, H-1], D' = bilinear(depth[n], q) (align corners, zero padding) > 0,
+ *     X' = R^T (D' K_n^-1 q~ - t) (X'.z > 1e-6), p' = pi(K_r X'), phi = |p' - p|; geo-valid if all hold and
+ *     phi < pixel_noise_threshold; w = exp(-phi) (no gradient);
+ *     geo[b] = sum w phi over geo-valid pixels / max(count, 1);
+ *   photometric (geo-valid pixels): d = n_c . X (|d| > 1e-6), H = K_n (R + t n_c^T / d) K_r^-1; for the 49
+ *     offsets k in {-3..3}^2: a_k = gray[r](p + k) (0 outside), h_k = H (p + k, 1) (h_k.z > 1e-6),
+ *     b_k = bilinear(gray[n], pi(h_k)); ncc = cov(a, b) / sqrt(var(a) var(b) + 1e-8) (population moments,
+ *     cov = mean(ab) - mean(a) mean(b)); c = clamp(1 - ncc, 0, 2); photo-valid if all hold and c < 0.9;
+ *     photo[b] = sum w c over photo-valid pixels / max(count, 1).
+ * r3dg_multiview_forward writes geo [B], photo [B] and counts int [B][2] (geo-valid, photo-valid pixels), needs
+ *   `work` of r3dg_multiview_work_bytes(B, H, W) (fp64 per-CTA partials) and reduces them in a fixed order on the
+ *   device: deterministic, no host synchronisation.  2 launches.
+ * r3dg_multiview_backward reads dL_dgeo [B], dL_dphoto [B] and the forward's counts and writes every element of
+ *   dL_ddepth [V,H,W] and dL_dnormal [V,3,H,W]: the gradients along every path of the definition (through q, the
+ *   sampling location of D', D', p', n_c, d and H), the geometric term scattered into depth[n] at the four
+ *   bilinear taps of q; masks, w, counts and the clamp's flat region carry none.  It recomputes the forward per
+ *   pixel.  Default: float atomics into zeroed outputs (2 memsets + 1 launch).  deterministic != 0: fixed-point
+ *   accumulators (detacc.cuh) in det_work of r3dg_multiview_det_bytes(V, H, W) (96 B per view pixel), bitwise
+ *   reproducible (memset + 2 launches); a term beyond 2^47 times the largest |dL_dgeo[b]| / max(count, 1) or
+ *   |dL_dphoto[b]| / max(count, 1) saturates to +-Inf.
+ * R3DG_ERR_BAD_ARG for V, H or W <= 0, B outside 1..R3DG_MAX_VIEWS, a pair index outside [0, V), a
+ * non-finite camera row or tan_fov <= 0, a negative or NaN threshold, a NULL pointer the call needs, or too small
+ * a workspace; R3DG_ERR_UNSUPPORTED for H*W >= 2^31 or H > 1048560.  Nothing is launched on an error.
+ * ------------------------------------------------------------------------------------------ */
+struct r3dg_multiview_args {
+    int V, H, W, B;
+    const float* depth;            /* [V,H,W] */
+    const float* normal;           /* [V,3,H,W] */
+    const float* gray;             /* [V,H,W] */
+    const float* viewmatrix;       /* [V,16], device */
+    const float* pair_cams;        /* HOST [B][8] */
+    const int* pairs;              /* HOST [B][2] */
+    float pixel_noise_threshold;
+    float* geo;                    /* forward: [B] */
+    float* photo;                  /* forward: [B] */
+    int* counts;                   /* forward: written [B][2]; backward: read */
+    void* work;                    /* forward */
+    size_t work_bytes;
+    const float* dL_dgeo;          /* backward: [B] */
+    const float* dL_dphoto;        /* backward: [B] */
+    float* dL_ddepth;              /* backward: [V,H,W] */
+    float* dL_dnormal;             /* backward: [V,3,H,W] */
+    int deterministic;
+    void* det_work;
+    size_t det_work_bytes;
+};
+size_t r3dg_multiview_work_bytes(int B, int H, int W);
+size_t r3dg_multiview_det_bytes(int V, int H, int W);
+int r3dg_multiview_forward(const struct r3dg_multiview_args* args, r3dg_stream_t stream);
+int r3dg_multiview_backward(const struct r3dg_multiview_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optimiser step (SURVEY.md §8f next #3).  Replaces, for all parameter groups at once, the
  * per-group `torch.optim.Adam(l, lr=0.0, eps=1e-15).step()` of scene/gaussian_model.py:489,495-497
  * (torch 1.12.1 torch/optim/adam.py:_single_tensor_adam: no weight decay, no amsgrad, no

@@ -75,6 +75,15 @@ class ShadeArgs(ctypes.Structure):
         [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
+class MultiviewArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("V", "H", "W", "B")] +
+                [(n, c_void_p) for n in ("depth", "normal", "gray", "viewmatrix", "pair_cams", "pairs")] +
+                [("pixel_noise_threshold", c_float)] +
+                [(n, c_void_p) for n in ("geo", "photo", "counts", "work")] + [("work_bytes", c_size_t)] +
+                [(n, c_void_p) for n in ("dL_dgeo", "dL_dphoto", "dL_ddepth", "dL_dnormal")] +
+                [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+
+
 class ExchangeArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("P", "D", "M", "world", "rank")] +
                 [("means3D", c_void_p), ("campos", c_void_p), ("factors", c_void_p * 64), ("dL_dsh", c_void_p),
@@ -182,6 +191,11 @@ SYMBOLS = [
     ("r3dg_bilagrid_tmp_bytes", c_size_t, [c_int] * 7),
     ("r3dg_bilagrid_forward", c_int, [c_int] * 7 + [c_void_p] * 5),
     ("r3dg_bilagrid_backward", c_int, [c_int] * 7 + [c_void_p] * 7 + [c_size_t, c_void_p]),
+    ("r3dg_multiview_work_bytes", c_size_t, [c_int] * 3),
+    ("r3dg_multiview_det_bytes", c_size_t, [c_int] * 3),
+    # `const struct r3dg_multiview_args*`: pass ctypes.byref(MultiviewArgs(...))
+    ("r3dg_multiview_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_multiview_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_adam_step", c_int, [c_int, ctypes.POINTER(AdamTensor), c_void_p]),
     ("r3dg_launch_count", ctypes.c_ulonglong, []),
     ("r3dg_tune", c_int, [ctypes.c_char_p, c_int, ctypes.POINTER(c_int)]),

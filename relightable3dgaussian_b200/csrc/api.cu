@@ -640,6 +640,20 @@ int r3dg_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, co
     return rc;
 }
 
+// ---- multi-view consistency losses (multiview.py) -------------------------------------------------
+size_t r3dg_multiview_work_bytes(int B, int H, int W) { return multiview_work_bytes(B, H, W); }
+size_t r3dg_multiview_det_bytes(int V, int H, int W) { return multiview_det_bytes(V, H, W); }
+int r3dg_multiview_forward(const r3dg_multiview_args* args, r3dg_stream_t stream) {
+    const int rc = launch_multiview_forward(args, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 2;                         // pixels, fixed-order reduction
+    return rc;
+}
+int r3dg_multiview_backward(const r3dg_multiview_args* args, r3dg_stream_t stream) {
+    const int rc = launch_multiview_backward(args, (cudaStream_t)stream);
+    if (rc == 0) g_launches += args->deterministic ? 2 : 1;   // pixels (+ fixed-point read-back)
+    return rc;
+}
+
 namespace {
 __global__ void unpack_rec_kernel(int P, int recf, int what, const float* __restrict__ rec,
                                   const uint32_t* __restrict__ tiles, float* __restrict__ dst) {

@@ -249,4 +249,10 @@ int launch_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, 
                              const float* rgb, const float* dL_dout, float* dL_drgb, float* dL_dgrids, void* tmp,
                              size_t tmp_bytes, cudaStream_t stream);
 
+// multiview.cu: PGSR's multi-view consistency losses; both launchers validate every argument before launching anything
+size_t multiview_work_bytes(int B, int H, int W);
+size_t multiview_det_bytes(int V, int H, int W);
+int launch_multiview_forward(const r3dg_multiview_args* a, cudaStream_t stream);
+int launch_multiview_backward(const r3dg_multiview_args* a, cudaStream_t stream);
+
 }  // namespace r3dg

@@ -26,6 +26,25 @@ __device__ __forceinline__ void cta_partial(double acc, double* dst) {
     }
 }
 
+// dst[0..K) = the CTA's sums of acc[0..K), in cta_partial's order.  Every thread of the CTA must call it.
+template <int NT, int K>
+__device__ __forceinline__ void cta_partials(const double (&acc)[K], double* dst) {
+    __shared__ double warp_sum[K][NT / 32];
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double a = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if ((threadIdx.x & 31) == 0) warp_sum[k][threadIdx.x >> 5] = a;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = 0.0;
+        for (int w = 0; w < NT / 32; ++w) s += warp_sum[threadIdx.x][w];
+        dst[threadIdx.x] = s;
+    }
+}
+
 // out[b] = sum(partial[b * per .. (b+1) * per)) / count, one CTA per output, fixed summation order
 __global__ void __launch_bounds__(kReduceNT) reduce_partials_kernel(const double* __restrict__ partial, long long per,
                                                                    double count, float* __restrict__ out) {
