@@ -879,6 +879,73 @@ int r3dg_multiview_forward(const struct r3dg_multiview_args* args, r3dg_stream_t
 int r3dg_multiview_backward(const struct r3dg_multiview_args* args, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * TSDF fusion and marching-cubes mesh extraction (the 2DGS / PGSR / RaDe-GS mesh recipe).  Not part of the reference
+ * surface.
+ * Grid: NX, NY, NZ >= 2 points, point (i, j, k) at origin + voxel_size * (i, j, k); arrays [NX,NY,NZ] with k fastest:
+ *   tsdf (fp32, initialised to 1), weight (fp32, initialised to 0) and optionally color [NX,NY,NZ,3] (fp32,
+ *   initialised to 0), all contiguous on the device.
+ * Cameras as in the multiview block: p_cam = [x, 1] @ viewmatrix (row-vector world -> camera), fx = W / (2 tan_fovx),
+ *   fy = H / (2 tan_fovy), u = fx X/Z + cx, v = fy Y/Z + cy; the pixel is the nearest one, (floor(u + 0.5),
+ *   floor(v + 0.5)).
+ * Integration of V views, 1 <= V <= R3DG_MAX_VIEWS, depth [V,H,W] (camera z) and optional rgb [V,3,H,W], visited in
+ *   order: view v updates grid point g only if Z > 0, the pixel lies in [0, W) x [0, H), D = depth[v](pixel) is
+ *   finite with 0 < D <= depth_trunc, and sdf = D - Z >= -sdf_trunc.  Then, with obs = min(1, sdf / sdf_trunc):
+ *   tsdf = (tsdf w + obs) / (w + 1), color = (color w + rgb[v](pixel)) / (w + 1), w = w + 1 (Open3D's projective
+ *   TSDF with unit weights).  No gradients.  One launch, one thread per grid point: each reads its tsdf / weight /
+ *   color once, walks the V views in registers and stores only if a view updated it.  IEEE fp32, no atomics: the
+ *   result is bitwise reproducible, and V views in one call give the bits of V one-view calls in the same order.
+ *   A non-finite viewmatrix entry (read on the device) makes the comparisons fail: the view updates nothing.
+ * Extraction: a cell is valid when all 8 corners have weight > 0; a corner is inside when tsdf < 0.  A grid edge gets
+ *   one vertex when its end points differ in inside-ness and one of the (up to 4) cells sharing it is valid, at
+ *   p0 + t (p1 - p0), t = v0 / (v0 - v1), p0 the lower-index end; its colour is the same lerp of the corner colours.
+ *   Each valid cell emits the triangles of its cube index from csrc/mc_table.cuh (every ambiguous face separates its
+ *   inside corners, so the mesh is crack-free; normals point from inside to outside).  Vertices are in grid-point
+ *   order, then x, y, z edge order; faces in cell order, then table order: the mesh is a function of the volume.
+ *   r3dg_tsdf_extract_count classifies every grid point into `work` (r3dg_tsdf_extract_work_bytes) and scans the
+ *   per-block counts (2 launches), then copies the two totals to totals_host [2] (vertices, faces) and synchronises
+ *   the stream: R3DG_ERR_UNSUPPORTED when either is >= 2^31.  r3dg_tsdf_extract_emit (2 launches) then writes
+ *   verts [n_verts,3], vert_colors [n_verts,3] (when color is given) and faces int [n_faces,3] from that `work`; the
+ *   volume must be unchanged since the count and n_verts / n_faces must be its totals.
+ * R3DG_ERR_BAD_ARG for a dimension < 2 (H, W < 1), a non-finite origin, voxel_size or sdf_trunc <= 0 or non-finite,
+ * depth_trunc <= 0 or NaN (+Inf is allowed), V outside 1..R3DG_MAX_VIEWS, a camera row with tan_fov <= 0 or a
+ * non-finite value, rgb given without color or color without rgb, a NULL pointer the call needs, or too small a
+ * workspace; R3DG_ERR_UNSUPPORTED for NX*NY*NZ >= 2^31 or H*W >= 2^31.  Nothing is launched on an error, except
+ * that the count's R3DG_ERR_UNSUPPORTED for too many vertices or faces follows its own launches.
+ * ------------------------------------------------------------------------------------------ */
+struct r3dg_tsdf_integrate_args {
+    int NX, NY, NZ;
+    float origin[3];
+    float voxel_size, sdf_trunc, depth_trunc;
+    float* tsdf;                   /* [NX,NY,NZ] */
+    float* weight;                 /* [NX,NY,NZ] */
+    float* color;                  /* [NX,NY,NZ,3] or NULL */
+    int V, H, W;
+    const float* depth;            /* [V,H,W] */
+    const float* rgb;              /* [V,3,H,W]; iff color */
+    const float* viewmatrix;       /* [V,16], device */
+    const float* cams;             /* HOST [V][4]: tan_fovx, tan_fovy, cx, cy */
+};
+struct r3dg_tsdf_extract_args {
+    int NX, NY, NZ;
+    float origin[3];
+    float voxel_size;
+    const float* tsdf;             /* [NX,NY,NZ] */
+    const float* weight;           /* [NX,NY,NZ] */
+    const float* color;            /* [NX,NY,NZ,3] or NULL */
+    void* work;
+    size_t work_bytes;
+    long long* totals_host;        /* count: HOST [2], written */
+    long long n_verts, n_faces;    /* emit: the totals of the count */
+    float* verts;                  /* emit: [n_verts,3] */
+    float* vert_colors;            /* emit: [n_verts,3]; iff color */
+    int* faces;                    /* emit: [n_faces,3] */
+};
+size_t r3dg_tsdf_extract_work_bytes(int NX, int NY, int NZ);
+int r3dg_tsdf_integrate(const struct r3dg_tsdf_integrate_args* args, r3dg_stream_t stream);
+int r3dg_tsdf_extract_count(const struct r3dg_tsdf_extract_args* args, r3dg_stream_t stream);
+int r3dg_tsdf_extract_emit(const struct r3dg_tsdf_extract_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optimiser step (SURVEY.md §8f next #3).  Replaces, for all parameter groups at once, the
  * per-group `torch.optim.Adam(l, lr=0.0, eps=1e-15).step()` of scene/gaussian_model.py:489,495-497
  * (torch 1.12.1 torch/optim/adam.py:_single_tensor_adam: no weight decay, no amsgrad, no

@@ -84,6 +84,20 @@ class MultiviewArgs(ctypes.Structure):
                 [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
+class TsdfIntegrateArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("NX", "NY", "NZ")] + [("origin", c_float * 3)] +
+                [(n, c_float) for n in ("voxel_size", "sdf_trunc", "depth_trunc")] +
+                [(n, c_void_p) for n in ("tsdf", "weight", "color")] + [(n, c_int) for n in ("V", "H", "W")] +
+                [(n, c_void_p) for n in ("depth", "rgb", "viewmatrix", "cams")])
+
+
+class TsdfExtractArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("NX", "NY", "NZ")] + [("origin", c_float * 3), ("voxel_size", c_float)] +
+                [(n, c_void_p) for n in ("tsdf", "weight", "color", "work")] + [("work_bytes", c_size_t)] +
+                [("totals_host", c_void_p), ("n_verts", c_ll), ("n_faces", c_ll)] +
+                [(n, c_void_p) for n in ("verts", "vert_colors", "faces")])
+
+
 class ExchangeArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("P", "D", "M", "world", "rank")] +
                 [("means3D", c_void_p), ("campos", c_void_p), ("factors", c_void_p * 64), ("dL_dsh", c_void_p),
@@ -196,6 +210,11 @@ SYMBOLS = [
     # `const struct r3dg_multiview_args*`: pass ctypes.byref(MultiviewArgs(...))
     ("r3dg_multiview_forward", c_int, [c_void_p, c_void_p]),
     ("r3dg_multiview_backward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_tsdf_extract_work_bytes", c_size_t, [c_int] * 3),
+    # `const struct r3dg_tsdf_*_args*`: pass ctypes.byref(TsdfIntegrateArgs(...)) / ctypes.byref(TsdfExtractArgs(...))
+    ("r3dg_tsdf_integrate", c_int, [c_void_p, c_void_p]),
+    ("r3dg_tsdf_extract_count", c_int, [c_void_p, c_void_p]),
+    ("r3dg_tsdf_extract_emit", c_int, [c_void_p, c_void_p]),
     ("r3dg_adam_step", c_int, [c_int, ctypes.POINTER(AdamTensor), c_void_p]),
     ("r3dg_launch_count", ctypes.c_ulonglong, []),
     ("r3dg_tune", c_int, [ctypes.c_char_p, c_int, ctypes.POINTER(c_int)]),

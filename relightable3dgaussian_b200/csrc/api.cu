@@ -654,6 +654,25 @@ int r3dg_multiview_backward(const r3dg_multiview_args* args, r3dg_stream_t strea
     return rc;
 }
 
+// ---- TSDF fusion and marching cubes (tsdf.py) -----------------------------------------------------
+size_t r3dg_tsdf_extract_work_bytes(int NX, int NY, int NZ) { return tsdf_extract_work_bytes(NX, NY, NZ); }
+int r3dg_tsdf_integrate(const r3dg_tsdf_integrate_args* args, r3dg_stream_t stream) {
+    const int rc = launch_tsdf_integrate(args, (cudaStream_t)stream);
+    if (rc == 0) g_launches += 1;
+    return rc;
+}
+int r3dg_tsdf_extract_count(const r3dg_tsdf_extract_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_tsdf_extract_count(args, (cudaStream_t)stream, &launched);
+    if (launched) g_launches += 2;                        // classify, scan
+    return rc;
+}
+int r3dg_tsdf_extract_emit(const r3dg_tsdf_extract_args* args, r3dg_stream_t stream) {
+    const int rc = launch_tsdf_extract_emit(args, (cudaStream_t)stream);
+    if (rc == 0 && (args->n_verts > 0 || args->n_faces > 0)) g_launches += 2;   // vertices, faces
+    return rc;
+}
+
 namespace {
 __global__ void unpack_rec_kernel(int P, int recf, int what, const float* __restrict__ rec,
                                   const uint32_t* __restrict__ tiles, float* __restrict__ dst) {

@@ -255,4 +255,11 @@ size_t multiview_det_bytes(int V, int H, int W);
 int launch_multiview_forward(const r3dg_multiview_args* a, cudaStream_t stream);
 int launch_multiview_backward(const r3dg_multiview_args* a, cudaStream_t stream);
 
+// tsdf.cu: TSDF fusion and marching cubes; every launcher validates its arguments before launching anything
+size_t tsdf_extract_work_bytes(int NX, int NY, int NZ);
+int launch_tsdf_integrate(const r3dg_tsdf_integrate_args* a, cudaStream_t stream);
+// count: *launched tells whether its kernels ran (also when the totals then return R3DG_ERR_UNSUPPORTED)
+int launch_tsdf_extract_count(const r3dg_tsdf_extract_args* a, cudaStream_t stream, bool* launched);
+int launch_tsdf_extract_emit(const r3dg_tsdf_extract_args* a, cudaStream_t stream);
+
 }  // namespace r3dg

@@ -193,3 +193,43 @@ def load_bake(path, normals=None, device="cpu"):
         dirs = dirs.to(device)
         areas = areas.to(device) if areas is not None else torch.full_like(vis, 2 * np.pi)
     return vis, dirs, areas
+
+
+def save_mesh_ply(path, verts, faces, colors=None):
+    """A triangle mesh (e.g. tsdf.TSDFVolume.extract) as a binary little-endian PLY that mesh tools read: a `vertex`
+    element of float x, y, z (and uchar red, green, blue when `colors` [N,3] in [0, 1] is given, rounded and clamped)
+    and a `face` element of `list uchar int vertex_indices`.  verts [N,3], faces [F,3] with indices in [0, N)."""
+    v = verts.detach().cpu().numpy() if isinstance(verts, torch.Tensor) else np.asarray(verts)
+    fc = faces.detach().cpu().numpy() if isinstance(faces, torch.Tensor) else np.asarray(faces)
+    if v.ndim != 2 or v.shape[1] != 3:
+        raise ValueError(f"save_mesh_ply: verts must be [N,3] (got {v.shape})")
+    if fc.ndim != 2 or fc.shape[1] != 3 or not (fc.size == 0 or np.issubdtype(fc.dtype, np.integer)):
+        raise ValueError(f"save_mesh_ply: faces must be integer [F,3] (got {fc.shape}, {fc.dtype})")
+    if fc.size and (fc.min() < 0 or fc.max() >= v.shape[0]):
+        raise ValueError(f"save_mesh_ply: face indices outside [0, {v.shape[0]})")
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    if colors is not None:
+        c = colors.detach().cpu().numpy() if isinstance(colors, torch.Tensor) else np.asarray(colors)
+        if c.shape != v.shape:
+            raise ValueError(f"save_mesh_ply: colors must be [N,3] like verts (got {c.shape})")
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    vrec = np.empty(v.shape[0], dtype=fields)
+    for i, n in enumerate("xyz"):
+        vrec[n] = v[:, i]
+    if colors is not None:
+        c8 = np.clip(np.rint(np.nan_to_num(c.astype(np.float64)) * 255.0), 0, 255).astype(np.uint8)
+        for i, n in enumerate(("red", "green", "blue")):
+            vrec[n] = c8[:, i]
+    frec = np.empty(fc.shape[0], dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    frec["n"] = 3
+    frec["i"] = fc
+    header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % v.shape[0]
+    header += "".join(f"property {'float' if t == '<f4' else 'uchar'} {n}\n" for n, t in fields)
+    header += "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % fc.shape[0]
+    d = os.path.dirname(path)
+    if d:
+        os.makedirs(d, exist_ok=True)
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(vrec.tobytes())
+        f.write(frec.tobytes())

@@ -49,6 +49,28 @@ def _host_pairs(pairs, V):
     return out
 
 
+def check_settings(fn, settings, V, H, W):
+    """The V GaussianRasterizationSettings of V rendered H x W maps as a list, checked on the host (also used by
+    tsdf.py)."""
+    settings = list(settings)
+    if len(settings) != V:
+        raise ValueError(f"{fn}: {len(settings)} settings for {V} views")
+    for v, s in enumerate(settings):
+        if (s.image_height, s.image_width) != (H, W):
+            raise ValueError(f"{fn}: settings[{v}] is {s.image_height}x{s.image_width}, the maps are {H}x{W}")
+        if tuple(s.viewmatrix.shape) != (4, 4):
+            raise ValueError(f"{fn}: settings[{v}].viewmatrix must be [4,4]")
+        if not (s.tanfovx > 0 and s.tanfovy > 0):
+            raise ValueError(f"{fn}: settings[{v}] has tanfovx / tanfovy <= 0")
+    return settings
+
+
+def view_matrices(settings, device):
+    """The settings' row-vector view matrices as one float32 [V,16] tensor on `device`."""
+    view = torch.stack([s.viewmatrix.detach().to(device=device, dtype=torch.float32) for s in settings])
+    return view.reshape(len(settings), 16)
+
+
 def _args(depth, normal, gray, view, cams, pairs, tau):
     V, _, H, W = depth.shape
     a = _lib.MultiviewArgs()
@@ -121,16 +143,7 @@ def _prepare(depth, normal, gray, settings, pairs, pixel_noise_threshold):
             raise ValueError(f"{fn}: {name} {tuple(t.shape)} disagrees with depth {tuple(depth.shape)}")
     if V == 0 or H == 0 or W == 0:
         raise ValueError(f"{fn}: empty maps {tuple(depth.shape)}")
-    settings = list(settings)
-    if len(settings) != V:
-        raise ValueError(f"{fn}: {len(settings)} settings for {V} views")
-    for v, s in enumerate(settings):
-        if (s.image_height, s.image_width) != (H, W):
-            raise ValueError(f"{fn}: settings[{v}] is {s.image_height}x{s.image_width}, the maps are {H}x{W}")
-        if tuple(s.viewmatrix.shape) != (4, 4):
-            raise ValueError(f"{fn}: settings[{v}].viewmatrix must be [4,4]")
-        if not (s.tanfovx > 0 and s.tanfovy > 0):
-            raise ValueError(f"{fn}: settings[{v}] has tanfovx / tanfovy <= 0")
+    settings = check_settings(fn, settings, V, H, W)
     tau = float(pixel_noise_threshold)
     if not tau >= 0.0:
         raise ValueError(f"{fn}: pixel_noise_threshold must be >= 0 (got {pixel_noise_threshold})")
@@ -146,8 +159,7 @@ def _prepare(depth, normal, gray, settings, pairs, pixel_noise_threshold):
         sr, sn = settings[r], settings[n]
         cams[8 * b: 8 * b + 8] = [sr.tanfovx, sr.tanfovy, sr.cx, sr.cy, sn.tanfovx, sn.tanfovy, sn.cx, sn.cy]
         idx[2 * b], idx[2 * b + 1] = r, n
-    view = torch.stack([s.viewmatrix.detach().to(device=depth.device, dtype=torch.float32) for s in settings])
-    return view.reshape(V, 16), cams, idx, tau
+    return view_matrices(settings, depth.device), cams, idx, tau
 
 
 def consistency_loss(depth, normal, gray, settings, pairs, pixel_noise_threshold=1.0):
