@@ -21,25 +21,40 @@ float atomics make them run-to-run nondeterministic).  Its workspace comes from 
 One view and V views of the same Gaussians (rasterize_views / rasterize_views_backward) run through the same two
 host paths, _forward and _backward: the library treats a one-view call as V = 1.
 
-`geometry=False` on the two backward functions (not part of the reference surface) runs the library's appearance-only
-backward: only the colour / feature / SH gradients, for training with frozen geometry.  The reference's
-rasterize_gaussians_backward, as the dropin calls it, always runs the full backward.
+The modes below are not part of the reference surface.  Each is off by default, so the reference's wrapper, which
+passes none of them, gets the reference's calls (ray_depth: unless its process default is set).
 
-`absgrad=True` on the two backward functions (not part of the reference surface either) also computes the absolute
-screen-space gradients dL_dmeans2D_abs (AbsGS, gsplat's absgrad): per Gaussian and view, the sum over pixels of
-|dL/dmean2D.x| and |dL/dmean2D.y|, returned as one more element after all others.
+`geometry=False` on the two backward functions runs the library's appearance-only backward: only the colour / feature /
+SH gradients, for training with frozen geometry.  Nothing is allocated for the six geometry gradients, which come back
+None, and of dL_dfeatures, dL_dcolors, dL_dsh only those `appearance` = (features, colors, sh) asks for are computed (the
+others are None too); the opacity, depth and surface cotangents are not read.
 
-`filter_3d=` on all four functions (not part of the reference surface) runs the library's 3D smoothing filter
+`antialiasing=True` on all four functions multiplies each Gaussian's opacity by
+rho = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)), the opacity compensation of the fixed 0.3 px^2 dilation; the
+backward must be called with the forward's flag.
+
+`absgrad=True` on the two backward functions also computes the absolute screen-space gradients dL_dmeans2D_abs (AbsGS,
+gsplat's absgrad): per Gaussian and view, the sum over pixels of |dL/dmean2D.x| and |dL/dmean2D.y|, [P,2] or [V,P,2],
+returned as one more element after all others (None with geometry=False, which never computes it).
+
+`filter_3d=` on all four functions runs the library's 3D smoothing filter
 (Mip-Splatting): a [P] or [P,1] fp32 CUDA tensor of per-Gaussian filter sizes f, shared by every view (filter3d.py).
 Each Gaussian is drawn with scales sqrt(s^2 + f^2) and its opacity times sqrt(prod_k s_k^2 / (s_k^2 + f^2)).  The
 backward takes the forward's tensor again and, with it, the forward's `opacities`; f gets no gradient.
 
-`depth_stats=True` on the two forward functions (not part of the reference surface) also renders, per pixel, depth2 =
-sum w d^2 over the composited entries (d: the depth the call composites, tz or the ray-depth plane) and the median
-depth (d of the entry at which the transmittance falls through 0.5); the two images follow every other element of the
-returned tuple.  None and False are off, and there is no process default: the reference's wrapper, which unpacks a
-fixed tuple, never sees them.  The backward functions take their cotangents as `dL_dout_depth2` and
-`dL_dout_median_depth` (None: zeros) and `depth_stats=None` for the forward's setting, read from the image buffer's size.
+`ray_depth=True` on all four functions: each Gaussian adds, at each pixel, the camera z where it peaks along the pixel's
+ray, tz + p . (pixel - mean2D) with the per-Gaussian depth plane p = conic (T0 Sigma w_z, T1 Sigma w_z), instead of its
+centre's tz; out_depth, out_surface_xyz and out_normal change.  A forward's None (the default) takes the process default
+(set_ray_depth, off unless set), so the reference's wrapper follows it; a backward's None takes the forward's mode from
+the geometry buffer's size.
+
+`depth_stats=True` on the two forward functions also renders, per pixel, depth2 = sum w d^2 over the composited entries
+(d: the depth the call composites, tz or the ray-depth plane) and the median depth (d of the entry at which the
+transmittance falls through 0.5), [1,H,W] or [V,1,H,W]; the two images follow every other element of the returned
+tuple.  None and False are off, and there is no process default: the reference's wrapper, which unpacks a fixed tuple,
+never sees them.  The backward functions take their cotangents as `dL_dout_depth2` and `dL_dout_median_depth` (None:
+zeros; only the geometry half reads them) and `depth_stats=None` for the forward's setting, read from the image
+buffer's size.
 """
 import ctypes
 import warnings
@@ -77,7 +92,7 @@ class DeferredCount:
     buffer of a deferred forward is sized _HEADROOM x the largest count any view of this shape has
     produced (HBM is plentiful on an 80 GB H100: 6 B per instance); should a view still overflow it, nothing
     out of bounds was written, `overflowed` is set and the autograd backward re-runs the forward
-    with the exact size before differentiating (rasterizer._RasterizeGaussians.backward)."""
+    with the exact size before differentiating (rasterizer._Rasterize.backward)."""
 
     def __init__(self, event, slot_view, capacity, state, P):
         self._event, self._slot, self._capacity, self._state, self._P = event, slot_view, capacity, state, P
@@ -184,33 +199,42 @@ def _fwd_ray_depth(ray_depth):
     return _RAY_DEPTH if ray_depth is None else bool(ray_depth)
 
 
-def _geom_ray_depth(ray_depth, geomBuffer, P, S, V):
-    """A backward's mode: its keyword, or (None) that of the forward that made `geomBuffer`: a ray-depth geometry buffer
-    is always larger than a default one of the same shape (r3dg_raster_ray_depth_geom_bytes)."""
+def _buffer_bytes(P, S, W, H, V, ray_depth=False, depth_stats=False, absgrad=False):
+    """(geometry buffer, image buffer, backward deterministic workspace) bytes of a call over V views of P Gaussians
+    with S feature channels at W x H, in these modes.  A mode's buffer is always larger than the default one of the same
+    shape, which is how the two functions below tell a buffer's mode from its size."""
+    lib = _lib.load()
+    geom = (lib.r3dg_raster_ray_depth_geom_bytes if ray_depth else lib.r3dg_raster_views_geom_bytes)(P, S, V)
+    img = (lib.r3dg_raster_depth_stats_img_bytes if depth_stats else lib.r3dg_raster_views_img_bytes)(W, H, V)
+    det = (lib.r3dg_raster_ray_depth_bwd_det_bytes if ray_depth else lib.r3dg_raster_bwd_det_bytes)(V * P, S)
+    if absgrad:                 # absgrad's fixed-point sums follow the gradient rows'
+        det += lib.r3dg_raster_bwd_det_absgrad_bytes(V * P)
+    return geom, img, det
+
+
+def _geom_ray_depth(ray_depth, geomBuffer, P, S, W, H, V):
+    """A backward's ray-depth mode: its keyword, or (None) that of the forward that made `geomBuffer`."""
     if ray_depth is not None:
         return bool(ray_depth)
-    return geomBuffer.numel() >= _lib.load().r3dg_raster_ray_depth_geom_bytes(P, S, V)
+    return geomBuffer.numel() >= _buffer_bytes(P, S, W, H, V, ray_depth=True)[0]
 
 
-def _img_depth_stats(depth_stats, imageBuffer, W, H, V):
-    """A backward's depth-statistics setting: its keyword, or (None) that of the forward that made `imageBuffer`: such a
-    buffer is always larger than a default one of the same shape (r3dg_raster_depth_stats_img_bytes)."""
+def _img_depth_stats(depth_stats, imageBuffer, P, S, W, H, V):
+    """A backward's depth-statistics setting: its keyword, or (None) that of the forward that made `imageBuffer`."""
     if depth_stats is not None:
         return bool(depth_stats)
-    return imageBuffer.numel() >= _lib.load().r3dg_raster_depth_stats_img_bytes(W, H, V)
+    return imageBuffer.numel() >= _buffer_bytes(P, S, W, H, V, depth_stats=True)[1]
 
 
-def _forward(views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
+def _forward(*, views, background, means3D, features, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
              viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered, computer_pseudo_normal, debug,
-             capacity, pinned, defer, antialiasing=False, filter_3d=None, ray_depth=None, depth_stats=None):
+             capacity, pinned, defer, antialiasing, filter_3d, ray_depth, depth_stats):
     """The forward of the len(cams) views `cams` = [(tan_fovx, tan_fovy, cx, cy), ...]: one view (`views` False,
     outputs in the one-view shapes) or V views (outputs with a leading V).  Sizes the binning buffer for `capacity`
     instances and re-runs with room to spare while the counts, read back into the pinned int32 `pinned` (one per
-    view), exceed it.  Returns the 12 outputs after num_rendered, the event recorded once the counts are copied, and the
-    counts as a list: None when `defer`, which returns after the first attempt without waiting.  `antialiasing`: the
-    library's antialiased mode (see rasterize_gaussians); `filter_3d`: the 3D filter (see the module notes); `ray_depth`:
-    the ray-depth mode (see rasterize_gaussians); `depth_stats`: the depth statistics, whose two images then follow the 12
-    outputs."""
+    view), exceed it.  Returns the 12 outputs after num_rendered (then the two depth-statistics images), the event
+    recorded once the counts are copied, and the counts as a list: None when `defer`, which returns after the first
+    attempt without waiting."""
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
@@ -236,9 +260,8 @@ def _forward(views, background, means3D, features, colors, opacity, scales, rota
     out_surface_xyz = torch.empty(lead + (3, H, W), **f32)
     out_weights = torch.empty(lead + (P, 1), **f32)
     radii = torch.empty(lead + (P,), dtype=torch.int32, device=dev)
-    geom_bytes = lib.r3dg_raster_ray_depth_geom_bytes(P, S, V) if ray_depth else lib.r3dg_raster_views_geom_bytes(P, S, V)
+    geom_bytes, img_bytes, _ = _buffer_bytes(P, S, W, H, V, ray_depth, depth_stats)
     geomBuffer = torch.empty((geom_bytes,), dtype=torch.uint8, device=dev)
-    img_bytes = lib.r3dg_raster_depth_stats_img_bytes(W, H, V) if depth_stats else lib.r3dg_raster_views_img_bytes(W, H, V)
     imgBuffer = torch.empty((img_bytes,), dtype=torch.uint8, device=dev)
     stats = ()
     if depth_stats:
@@ -288,17 +311,8 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
                         filter_3d=None, ray_depth=None, depth_stats=None):
     """== RasterizeGaussiansCUDA (rasterize_points.cu:36-141).  Returns the 13-tuple
     (rendered, n_contrib, out_color, out_opacity, out_depth, out_feature, out_normal,
-     out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer).
-    `antialiasing=True` (not part of the reference surface) multiplies each Gaussian's opacity by
-    rho = sqrt(max(det(cov2D) / det(cov2D + 0.3 I), 2.5e-5)), the opacity compensation of the fixed 0.3 px^2
-    dilation; the backward must then be called with the same flag.  `filter_3d` (not part of the reference surface):
-    Mip-Splatting's 3D filter, see the module notes; the backward must be given the same tensor.  `ray_depth=True`
-    (not part of the reference surface): each Gaussian adds, at each pixel, the camera z where it peaks along the
-    pixel's ray, tz + p . (pixel - mean2D) with the per-Gaussian depth plane p = conic (T0 Sigma w_z, T1 Sigma w_z),
-    instead of its centre's tz; out_depth, out_surface_xyz and out_normal change.  None (the default) takes the process
-    default (set_ray_depth, off unless set), so the reference's wrapper, which passes no such keyword, follows it.  The
-    backward takes the mode from the geometry buffer unless given.  `depth_stats=True` (not part of the reference
-    surface): depth2 [1,H,W] and median_depth [1,H,W] follow imgBuffer (see the module notes)."""
+     out_surface_xyz, out_weights, radii, geomBuffer, binningBuffer, imgBuffer), with depth_stats then depth2 [1,H,W]
+    and median_depth [1,H,W].  The modes: see the module notes."""
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")   # rasterize_points.cu:62-64
     P = means3D.size(0)
@@ -324,10 +338,13 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     slot = st["next"]
     st["next"] = (slot + 1) % _SLOTS
     pinned = st["pinned"][slot:slot + 1]
-    out, ev, counts = _forward(False, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
-                               cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy, cx, cy)], H, W, sh, degree,
-                               campos, prefiltered, computer_pseudo_normal, debug, capacity, pinned, _defer,
-                               antialiasing, filter_3d, ray_depth, depth_stats)
+    out, ev, counts = _forward(
+        views=False, background=background, means3D=means3D, features=features, colors=colors, opacity=opacity,
+        scales=scales, rotations=rotations, scale_modifier=scale_modifier, cov3D_precomp=cov3D_precomp,
+        viewmatrix=viewmatrix, projmatrix=projmatrix, cams=[(tan_fovx, tan_fovy, cx, cy)], H=H, W=W, sh=sh,
+        degree=degree, campos=campos, prefiltered=prefiltered, computer_pseudo_normal=computer_pseudo_normal,
+        debug=debug, capacity=capacity, pinned=pinned, defer=_defer, antialiasing=antialiasing, filter_3d=filter_3d,
+        ray_depth=ray_depth, depth_stats=depth_stats)
     if _defer:
         rendered = DeferredCount(ev, pinned, capacity, st, P)
         st["pending"] = rendered
@@ -337,35 +354,26 @@ def rasterize_gaussians(background, means3D, features, colors, opacity, scales, 
     return (rendered,) + out
 
 
-def _backward(views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
+def _backward(*, views, background, means3D, features, colors, scales, rotations, scale_modifier, cov3D_precomp,
               viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree,
               campos, geomBuffer, binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads, surface,
-              surface_work, principal, geometry=True, appearance=(True, True, True), antialiasing=False, absgrad=False,
-              filter_3d=None, opacities=None, ray_depth=None, depth_stats=None, dL_dout_depth2=None,
-              dL_dout_median_depth=None):
+              surface_work, principal, geometry, appearance, antialiasing, absgrad, filter_3d, opacities, ray_depth,
+              depth_stats, dL_dout_depth2, dL_dout_median_depth):
     """The backward of a _forward over the len(cams) views `cams` (only each view's tan_fov* is read here; `principal`
     is the first view's (cx, cy), or None).  Returns the nine gradients of rasterize_views_backward (one view: in the
-    one-view shapes) and the V-view camera gradients (empty unless `cam_grads`).  `_out`, `surface` and `surface_work`
-    are those of rasterize_gaussians_backward (`surface` without the principal point).
-    `geometry=False`: the appearance-only backward.  Nothing is allocated for the six geometry gradients, which come
-    back None, and of dL_dfeatures, dL_dcolors, dL_dsh only those `appearance` = (features, colors, sh) asks for are
-    computed (the others are None too); the opacity, depth and surface cotangents are not read.  `antialiasing` must
-    be the forward's.  `absgrad`: the third element returned is (dL_dmeans2D_abs,) ([P,2], or [V,P,2] for V views;
-    None without the geometry half, geometry=False, which never computes it); () without absgrad.  `filter_3d` must be
-    the forward's, and `opacities` the forward's opacities (required with it).  `ray_depth`: the forward's, or None for
-    the mode of the forward that made `geomBuffer`.  `depth_stats`: the forward's, or None for that of the forward that
-    made `imageBuffer`; with it, `dL_dout_depth2` and `dL_dout_median_depth` are the cotangents of its two images (None:
-    zeros), which only the geometry half reads."""
+    one-view shapes), the V-view camera gradients (empty unless `cam_grads`) and (dL_dmeans2D_abs,) with absgrad, ()
+    without.  `_out`, `surface` and `surface_work` are those of rasterize_gaussians_backward (`surface` without the
+    principal point)."""
     if not geometry and (cam_grads or _out is not None):
         raise ValueError("the appearance-only backward (geometry=False) computes no camera gradient and takes no `_out`")
     lib = _lib.load()
     V, P, S = len(cams), means3D.size(0), features.size(-1)
     filter_3d = _check_filter_3d(filter_3d, P, cov3D_precomp)
-    ray_depth = _geom_ray_depth(ray_depth, geomBuffer, P, S, V)
     if filter_3d is not None and (opacities is None or opacities.numel() != P):
         raise ValueError("the backward with filter_3d needs the forward's opacities ([P] or [P,1])")
     H, W = dL_dout_color.size(-2), dL_dout_color.size(-1)
-    depth_stats = _img_depth_stats(depth_stats, imageBuffer, W, H, V)
+    ray_depth = _geom_ray_depth(ray_depth, geomBuffer, P, S, W, H, V)
+    depth_stats = _img_depth_stats(depth_stats, imageBuffer, P, S, W, H, V)
     if not depth_stats and (dL_dout_depth2 is not None or dL_dout_median_depth is not None):
         raise ValueError("cotangents of depth2 / median_depth need a forward with depth_stats=True")
     dev = means3D.device
@@ -445,9 +453,7 @@ def _backward(views, background, means3D, features, colors, scales, rotations, s
                                                      (dL_dout_median_depth, "dL_dout_median_depth")))
             a.depth_stats = 1
             a.dL_dout_depth2, a.dL_dout_median_depth = dL_dout_depth2.data_ptr(), dL_dout_median_depth.data_ptr()
-        det_bytes = lib.r3dg_raster_ray_depth_bwd_det_bytes(V * P, S) if ray_depth else lib.r3dg_raster_bwd_det_bytes(V * P, S)
-        if dL_dmeans2D_abs is not None:                 # absgrad's fixed-point sums follow the gradient rows'
-            det_bytes += lib.r3dg_raster_bwd_det_absgrad_bytes(V * P)
+        det_bytes = _buffer_bytes(P, S, W, H, V, ray_depth, depth_stats, dL_dmeans2D_abs is not None)[2]
         det_ws = _lib.det_workspace(a, det_bytes, dev)
         if cam:
             cam_ws = _lib.scratch(lib.r3dg_raster_cam_grad_bytes(P, V), dev)
@@ -477,23 +483,21 @@ def rasterize_gaussians_backward(background, means3D, features, radii, colors, s
     `projmatrix` and `campos`.  `surface` (not part of the reference surface either) differentiates the pseudo-normal
     and surface-xyz outputs: (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth, cx, cy) with the forward's
     opacity and depth images; a cotangent may be None.  `surface_work` optionally supplies the workspace
-    (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards.
-    `geometry=False` (not part of the reference surface either) is the appearance-only backward of _backward: the
-    gradients of the geometry inputs, and of the appearance inputs `appearance` = (features, colors, sh) leaves out,
-    come back None.  `antialiasing` (not part of the reference surface) must be the forward's: rasterize_gaussians.
-    `absgrad=True` (not part of the reference surface): dL_dmeans2D_abs [P,2] is the last element (None when
-    geometry=False).  `filter_3d` (not part of the reference surface) must be the forward's, and then `opacities` the
-    forward's opacities: rasterize_gaussians.  `ray_depth` (not part of the reference surface): None (the default) takes the
-    forward's mode from `geomBuffer`, True / False must be the forward's.  `depth_stats` (not part of the reference
-    surface): None takes the forward's setting from `imageBuffer`; `dL_dout_depth2` / `dL_dout_median_depth` [1,H,W] are
-    the cotangents of its two images (None: zeros)."""
-    principal = surface[4:6] if surface is not None and len(surface) == 6 else None
-    grads, cam, extra = _backward(False, background, means3D, features, colors, scales, rotations, scale_modifier,
-                           cov3D_precomp, viewmatrix, projmatrix, [(tan_fovx, tan_fovy)], dL_dout_color,
-                           dL_dout_opacity, dL_dout_depth, dL_dout_feature, sh, degree, campos, geomBuffer,
-                           binningBuffer, imageBuffer, backward_geometry, debug, _out, cam_grads,
-                           surface and surface[:4], surface_work, principal, geometry, appearance, antialiasing,
-                           absgrad, filter_3d, opacities, ray_depth, depth_stats, dL_dout_depth2, dL_dout_median_depth)
+    (r3dg_raster_surface_grad_bytes), e.g. to read the combined depth and opacity cotangents afterwards.  With absgrad,
+    dL_dmeans2D_abs [P,2] is the last element.  The modes, and the forward's `opacities` the filter needs: see the
+    module notes."""
+    grads, cam, extra = _backward(
+        views=False, background=background, means3D=means3D, features=features, colors=colors, scales=scales,
+        rotations=rotations, scale_modifier=scale_modifier, cov3D_precomp=cov3D_precomp, viewmatrix=viewmatrix,
+        projmatrix=projmatrix, cams=[(tan_fovx, tan_fovy)], dL_dout_color=dL_dout_color,
+        dL_dout_opacity=dL_dout_opacity, dL_dout_depth=dL_dout_depth, dL_dout_feature=dL_dout_feature, sh=sh,
+        degree=degree, campos=campos, geomBuffer=geomBuffer, binningBuffer=binningBuffer, imageBuffer=imageBuffer,
+        backward_geometry=backward_geometry, debug=debug, _out=_out, cam_grads=cam_grads,
+        surface=surface and surface[:4], surface_work=surface_work,
+        principal=surface[4:6] if surface is not None and len(surface) == 6 else None, geometry=geometry,
+        appearance=appearance, antialiasing=antialiasing, absgrad=absgrad, filter_3d=filter_3d, opacities=opacities,
+        ray_depth=ray_depth, depth_stats=depth_stats, dL_dout_depth2=dL_dout_depth2,
+        dL_dout_median_depth=dL_dout_median_depth)
     return grads + tuple(t[0] for t in cam) + extra
 
 
@@ -547,7 +551,7 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
             "bwd_order": (17, torch.int32, (2 * T,)), "bmask": (18, torch.uint8, (num_rendered,)),
             "cmask": (19, torch.uint8, (num_rendered,)), "brects": (20, torch.int32, (P, 2)),
             "composited": (22, torch.uint8, (P,)), "median_pos": (23, torch.int32, (H, W))}[name]
-    if name == "median_pos" and imgBuffer.numel() < lib.r3dg_raster_depth_stats_img_bytes(W, H, 1):
+    if name == "median_pos" and not _img_depth_stats(None, imgBuffer, P, S, W, H, 1):
         raise RuntimeError("debug_intermediate(median_pos) needs the image buffer of a forward with depth_stats=True")
     out = torch.empty(spec[2], dtype=spec[1], device=geomBuffer.device)
     if out.numel() == 0:
@@ -555,7 +559,7 @@ def debug_intermediate(name, P, S, W, H, geomBuffer, imgBuffer, binningBuffer, n
     nbytes = out.numel() * out.element_size()
     stream = torch.cuda.current_stream(geomBuffer.device)
     # a ray-depth geometry buffer has the mode's layout (records and gradient rows one float4 wider)
-    copy = lib.r3dg_raster_ray_depth_debug_copy if _geom_ray_depth(None, geomBuffer, P, S, 1) else lib.r3dg_raster_debug_copy
+    copy = lib.r3dg_raster_ray_depth_debug_copy if _geom_ray_depth(None, geomBuffer, P, S, W, H, 1) else lib.r3dg_raster_debug_copy
     with torch.cuda.device(geomBuffer.device):
         rc = copy(spec[0], P, S, W, H, geomBuffer.data_ptr(), imgBuffer.data_ptr(),
                                         binningBuffer.data_ptr(), binningBuffer.numel(), out.data_ptr(),
@@ -577,19 +581,21 @@ def rasterize_views(background, means3D, features, colors, opacity, scales, rota
     cams: V tuples (tan_fovx, tan_fovy, cx, cy); features [P,S] or [V,P,S], colors [P,3] or [V,P,3] (or empty).
     Returns (num_rendered: list of V ints, n_contrib [V,H,W], out_color [V,3,H,W], out_opacity [V,1,H,W],
     out_depth [V,1,H,W], out_feature [V,S,H,W], out_normal [V,3,H,W], out_surface_xyz [V,3,H,W], out_weights [V,P,1],
-    radii [V,P], geomBuffer, binningBuffer, imgBuffer).  Always synchronous: the V counts are read back once.
-    `antialiasing`, `filter_3d` and `ray_depth` apply to every view (see rasterize_gaussians).  `depth_stats=True`:
-    depth2 [V,1,H,W] and median_depth [V,1,H,W] follow imgBuffer."""
+    radii [V,P], geomBuffer, binningBuffer, imgBuffer), with depth_stats then depth2 [V,1,H,W] and median_depth
+    [V,1,H,W].  Always synchronous: the V counts are read back once.  The modes apply to every view."""
     V, P = len(cams), means3D.size(0)
     H, W = int(image_height), int(image_width)
     dev = means3D.device
     key = (dev.index if dev.index is not None else torch.cuda.current_device(), P, W, H, V)
     capacity = int(_min_capacity) if _min_capacity is not None else max(_views_capacity.get(key, 0), 4 * V * P + 4096)
     pinned = torch.zeros((V,), dtype=torch.int32).pin_memory()
-    out, _, rendered = _forward(True, background, means3D, features, colors, opacity, scales, rotations, scale_modifier,
-                                cov3D_precomp, viewmatrix, projmatrix, cams, H, W, sh, degree, campos, prefiltered,
-                                computer_pseudo_normal, False, capacity, pinned, False, antialiasing, filter_3d, ray_depth,
-                                depth_stats)
+    out, _, rendered = _forward(
+        views=True, background=background, means3D=means3D, features=features, colors=colors, opacity=opacity,
+        scales=scales, rotations=rotations, scale_modifier=scale_modifier, cov3D_precomp=cov3D_precomp,
+        viewmatrix=viewmatrix, projmatrix=projmatrix, cams=cams, H=H, W=W, sh=sh, degree=degree, campos=campos,
+        prefiltered=prefiltered, computer_pseudo_normal=computer_pseudo_normal, debug=False, capacity=capacity,
+        pinned=pinned, defer=False, antialiasing=antialiasing, filter_3d=filter_3d, ray_depth=ray_depth,
+        depth_stats=depth_stats)
     _views_capacity[key] = max(int(sum(rendered) * 1.25) + 4096, 4 * V * P + 4096)
     return (rendered,) + out
 
@@ -608,15 +614,16 @@ def rasterize_views_backward(background, means3D, features, colors, scales, rota
     gradients follow, never summed: dL_dviewmatrix [V,4,4], dL_dprojmatrix [V,4,4], dL_dcampos [V,3].  `surface` =
     (dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth), all [V,*,H,W] (a cotangent may be None), and
     `surface_work` are those of rasterize_gaussians_backward; each view uses its own principal point from `cams` (with
-    one view, cams[0]'s, entered as the call's cx, cy).  `geometry` and `appearance` are those of
-    rasterize_gaussians_backward, and `antialiasing` must be the forward's.  `absgrad=True`: dL_dmeans2D_abs [V,P,2]
-    is the last element, as in rasterize_gaussians_backward.  `filter_3d` and `opacities` are those of
-    rasterize_gaussians_backward, and `ray_depth` is that of rasterize_gaussians_backward.  `depth_stats`,
-    `dL_dout_depth2` and `dL_dout_median_depth` ([V,1,H,W]) are those of rasterize_gaussians_backward."""
-    grads, cam, extra = _backward(True, background, means3D, features, colors, scales, rotations, scale_modifier,
-                           cov3D_precomp, viewmatrix, projmatrix, cams, dL_dout_color, dL_dout_opacity, dL_dout_depth,
-                           dL_dout_feature, sh, degree, campos, geomBuffer, binningBuffer, imageBuffer,
-                           backward_geometry, False, None, cam_grads, surface, surface_work, cams[0][2:4], geometry,
-                           appearance, antialiasing, absgrad, filter_3d, opacities, ray_depth, depth_stats, dL_dout_depth2,
-                           dL_dout_median_depth)
+    one view, cams[0]'s, entered as the call's cx, cy).  With absgrad, dL_dmeans2D_abs [V,P,2] is the last element.
+    The modes: see the module notes."""
+    grads, cam, extra = _backward(
+        views=True, background=background, means3D=means3D, features=features, colors=colors, scales=scales,
+        rotations=rotations, scale_modifier=scale_modifier, cov3D_precomp=cov3D_precomp, viewmatrix=viewmatrix,
+        projmatrix=projmatrix, cams=cams, dL_dout_color=dL_dout_color, dL_dout_opacity=dL_dout_opacity,
+        dL_dout_depth=dL_dout_depth, dL_dout_feature=dL_dout_feature, sh=sh, degree=degree, campos=campos,
+        geomBuffer=geomBuffer, binningBuffer=binningBuffer, imageBuffer=imageBuffer,
+        backward_geometry=backward_geometry, debug=False, _out=None, cam_grads=cam_grads, surface=surface,
+        surface_work=surface_work, principal=cams[0][2:4], geometry=geometry, appearance=appearance,
+        antialiasing=antialiasing, absgrad=absgrad, filter_3d=filter_3d, opacities=opacities, ray_depth=ray_depth,
+        depth_stats=depth_stats, dL_dout_depth2=dL_dout_depth2, dL_dout_median_depth=dL_dout_median_depth)
     return grads + cam + extra

@@ -61,64 +61,77 @@ _ABSGRAD = False
 
 def set_absgrad(enabled: bool):
     """Process default of the absolute screen-space gradients (not part of the reference surface): with it on, every
-    `GaussianRasterizer`, `rasterize_gaussians` and `rasterize_views` call runs as with `absgrad=True`.  Together with
-    `densify.install(absgrad=True)` this gives the reference's unmodified training loop the AbsGS densification
-    statistic.  `set_absgrad(False)` restores the default (off)."""
+    `GaussianRasterizer`, `rasterize_gaussians` and `rasterize_views` call runs as with `absgrad=True` (see
+    rasterize_gaussians).  Together with `densify.install(absgrad=True)` this gives the reference's unmodified training
+    loop the AbsGS densification statistic.  `set_absgrad(False)` restores the default (off)."""
     global _ABSGRAD
     _ABSGRAD = bool(enabled)
 
 
-def _absgrad_on(absgrad):
-    """The call's absgrad mode: its keyword, or the process default (set_absgrad)."""
-    return bool(absgrad) or _ABSGRAD
-
-
 def set_ray_depth(enabled: bool):
-    """Process default of the ray-depth mode (not part of the reference surface).  After `set_ray_depth(True)` every
-    forward that does not ask otherwise runs as with `ray_depth=True`: `GaussianRasterizer`, `rasterize_gaussians` and
-    `rasterize_views` here, and `_C_raster.rasterize_gaussians` / `rasterize_views`, which the reference's own wrapper
-    (gaussian_renderer/r3dg_rasterization.py over dropin/r3dg_rasterization) calls.  The depth output, and so
-    surface_xyz and the pseudo-normal, then come from per-pixel depth planes instead of the Gaussians' centre depths,
-    and the reference's unmodified stage-1 loop trains its normals on the better pseudo-normal.  Each backward takes
-    its forward's mode from the geometry buffer.  `set_ray_depth(False)` restores the default (off)."""
+    """Process default of the ray-depth mode (not part of the reference surface; see rasterize_gaussians).  After
+    `set_ray_depth(True)` every forward that does not ask otherwise runs as with `ray_depth=True`: `GaussianRasterizer`,
+    `rasterize_gaussians` and `rasterize_views` here, and `_C_raster.rasterize_gaussians` / `rasterize_views`, which the
+    reference's own wrapper (gaussian_renderer/r3dg_rasterization.py over dropin/r3dg_rasterization) calls, so the
+    reference's unmodified stage-1 loop trains its normals on the better pseudo-normal.  Each backward takes its
+    forward's mode from the geometry buffer.  `set_ray_depth(False)` restores the default (off)."""
     _C.set_ray_depth(enabled)
 
 
-def _ray_depth_on(ray_depth):
-    """The call's ray-depth mode: its keyword, or the process default (set_ray_depth)."""
-    return bool(ray_depth) or _C.ray_depth_default()
+class _Modes(NamedTuple):
+    """The opt-in modes of one rasterizer call (each described in rasterize_gaussians), resolved once per call by
+    _modes.  A mode that is off adds no keyword to a library call: the call is exactly the call without that mode."""
+    surface_grads: bool
+    antialiasing: bool
+    filter_3d: object           # [P] fp32 CUDA tensor, or None
+    ray_depth: bool
+    depth_stats: bool
+    absgrad: bool
+
+    def forward_kw(self, rerun=False):
+        """The library forward's keywords.  The deferred-count re-run (`rerun`) passes `ray_depth` explicitly whenever
+        the process default could differ from the node's mode (the default may have changed since the forward)."""
+        kw = {}
+        if self.antialiasing:
+            kw["antialiasing"] = True
+        if self.filter_3d is not None:
+            kw["filter_3d"] = self.filter_3d
+        if self.ray_depth or (rerun and _C.ray_depth_default()):
+            kw["ray_depth"] = self.ray_depth
+        if self.depth_stats:
+            kw["depth_stats"] = True
+        return kw
+
+    def backward_kw(self, opacities, means2D_grad, g_stats):
+        """The library backward's keywords.  The filter takes the forward's `opacities` along; absgrad is asked for only
+        when `means2D_grad` (means2D needs a gradient and the backward runs its geometry half); the depth statistics
+        take the cotangents `g_stats` of depth2 and median_depth (None: zeros)."""
+        kw = {}
+        if self.antialiasing:
+            kw["antialiasing"] = True
+        if self.absgrad and means2D_grad:
+            kw["absgrad"] = True
+        if self.filter_3d is not None:
+            kw.update(filter_3d=self.filter_3d, opacities=opacities)
+        if self.ray_depth:
+            kw["ray_depth"] = True
+        if self.depth_stats:
+            g2, gm = (tuple(g_stats) + (None, None))[:2]
+            kw.update(depth_stats=True, dL_dout_depth2=g2, dL_dout_median_depth=gm)
+        return kw
 
 
-def _rd_kw(ray_depth):
-    """The keyword that turns on the library's ray-depth mode, only when it is on: an off call is the call without
-    the mode.  (A library backward without it takes the forward's mode from the geometry buffer.)"""
-    return {"ray_depth": True} if ray_depth else {}
-
-
-def _rerun_rd_kw(ray_depth):
-    """The deferred-count re-run's keyword: the node's mode, explicit whenever the process default could differ from
-    it (the default may have changed since the forward), and no keyword when the mode is not in use at all."""
-    return {"ray_depth": bool(ray_depth)} if ray_depth or _C.ray_depth_default() else {}
-
-
-def _ds_kw(depth_stats):
-    """The keyword that turns on the library's depth statistics, only when they are on: an off call is the call without
-    them."""
-    return {"depth_stats": True} if depth_stats else {}
-
-
-def _ds_bwd_kw(ctx, g_stats):
-    """The backward's depth-statistics keywords: the flag and the cotangents of depth2 and median_depth (None: zeros),
-    only when the node's forward had them on."""
-    if not getattr(ctx, "depth_stats", False):
-        return {}
-    g2, gm = (tuple(g_stats) + (None, None))[:2]
-    return {"depth_stats": True, "dL_dout_depth2": g2, "dL_dout_median_depth": gm}
-
-
-def _stats_outputs(ctx, out):
-    """The node's outputs: the reference's ten, then depth2 and median_depth when the depth statistics are on."""
-    return out[:10] + (tuple(out[13:15]) if ctx.depth_stats else ())
+def _modes(P, cov3Ds_precomp, computer_pseudo_normal, surface_grads, antialiasing, filter_3d, ray_depth, depth_stats,
+           absgrad):
+    """The call's mode record: the keywords, with the process defaults of absgrad and ray_depth (set_absgrad,
+    set_ray_depth).  Refuses a 3D filter the library would refuse, and surface gradients without the pseudo-normal pass
+    (both outputs are then zeros: there is nothing to differentiate)."""
+    _C._check_filter_3d(filter_3d, P, cov3Ds_precomp)
+    if surface_grads and not computer_pseudo_normal:
+        raise ValueError("surface_grads=True needs computer_pseudo_normal=True: without it the normal and surface_xyz "
+                         "outputs are zeros and have no gradient")
+    return _Modes(bool(surface_grads), bool(antialiasing), filter_3d, bool(ray_depth) or _C.ray_depth_default(),
+                  bool(depth_stats), bool(absgrad) or _ABSGRAD)
 
 
 def _set_absgrad(means2D, g_abs):
@@ -168,175 +181,138 @@ def _debug_call(debug, fn, args, dump, message, **kw):
         raise
 
 
-def _save_forward(ctx, out, surface_grads, *tensors):
-    """Keeps what the backward of a forward with outputs `out` needs: `tensors`, then with `surface_grads` the forward's
-    opacity and depth images (see _surface_cotangents), and the shapes of the four image outputs (_image_cotangents)."""
-    # cotangents of outputs the reference's backward ignores (num_contrib, normal, surface_xyz, weights, radii)
-    # stay None instead of being materialised as zero tensors (5 fill kernels per step); the four image
-    # cotangents are filled in by _image_cotangents when a loss does not touch one of them
-    ctx.set_materialize_grads(False)
-    ctx.out_shapes = tuple(t.shape for t in out[2:6])
-    ctx.surface_grads = surface_grads
-    ctx.save_for_backward(*tensors, *(out[3:5] if surface_grads else ()))
+# the node's tensor inputs; the settings, the mode record and the deferred-count decision follow them
+_INPUTS = ("means3D", "means2D", "features", "sh", "colors_precomp", "opacities", "scales", "rotations",
+           "cov3Ds_precomp", "viewmatrix", "projmatrix", "campos")
+_CAMERAS = _INPUTS[_INPUTS.index("viewmatrix"):]
+# the inputs whose gradients need the geometry half of the backward (the others are appearance)
+_GEOMETRY = tuple(n for n in _INPUTS if n not in ("features", "sh", "colors_precomp"))
+# what the node saves for its backward, followed by the forward's opacity and depth images with surface_grads; the
+# work buffers stay at positions 8-10, where introspection code (debug_intermediate callers) finds them
+_SAVED = ("colors_precomp", "means3D", "features", "scales", "rotations", "cov3Ds_precomp", "radii", "sh", "geomBuffer",
+          "binningBuffer", "imgBuffer", "opacities", "filter_3d", "viewmatrix", "projmatrix", "campos")
+# the inputs of the library backward's nine gradients, in its order (rasterize_points.cu:143-235); cameras follow
+_LIB_GRADS = ("means2D", "colors_precomp", "opacities", "means3D", "features", "cov3Ds_precomp", "sh", "scales",
+              "rotations")
 
 
-def _image_cotangents(ctx, device, *grads):
-    """The cotangents of the color, opacity, depth and feature outputs, zeros for those the loss does not touch."""
-    return tuple(torch.zeros(shape, dtype=torch.float32, device=device) if g is None else g
-                 for g, shape in zip(grads, ctx.out_shapes))
+def _forward_args(rs, x):
+    """The positional arguments of _C.rasterize_gaussians for the settings `rs` and the node's inputs `x` (by name)."""
+    return (rs.bg, x["means3D"], x["features"], x["colors_precomp"], x["opacities"], x["scales"], x["rotations"],
+            rs.scale_modifier, x["cov3Ds_precomp"], rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.cx, rs.cy,
+            rs.image_height, rs.image_width, x["sh"], rs.sh_degree, rs.campos, rs.prefiltered,
+            rs.computer_pseudo_normal, rs.debug)
 
 
-def _surface_cotangents(ctx, g_normal, g_surface_xyz):
-    """(dL_dout_normal, dL_dout_surface_xyz, out_opacity, out_depth) when the node differentiates the pseudo-normal and
-    surface-xyz outputs and the loss touches one of them; None otherwise."""
-    if not ctx.surface_grads or (g_normal is None and g_surface_xyz is None):
-        return None
-    return (g_normal, g_surface_xyz) + tuple(ctx.saved_tensors[-2:])
 
-
-def _input_grads(ctx, grads, cameras):
-    """The gradients of the node's inputs from the library's nine (and camera gradients, if computed).  Those of the
-    three inputs `cameras` (viewmatrix, projmatrix, campos) come in their shapes: None for those that do not need
-    one, and for all three when none was computed.  The last five inputs, the 3D filter (a buffer, as in
-    Mip-Splatting) and the antialiasing, ray-depth, depth-statistics and absgrad flags, get None."""
-    g_means2D, g_colors_precomp, g_opacities, g_means3D, g_features, g_cov3Ds, g_sh, g_scales, g_rotations = grads[:9]
-    cam = (None, None, None)
-    if grads[9:]:
-        cam = tuple(g.reshape(t.shape) if n else None for g, t, n in zip(grads[9:], cameras, ctx.needs_input_grad[11:14]))
-    return (g_means3D, g_means2D, g_features, g_sh, g_colors_precomp, g_opacities, g_scales, g_rotations, g_cov3Ds,
-            None, None) + cam + (None, None, None, None, None)
-
-
-# the inputs of both autograd nodes whose gradients need the geometry half of the backward: means3D, means2D, opacities,
-# scales, rotations, cov3Ds_precomp, viewmatrix, projmatrix, campos (features, sh and colors_precomp are appearance)
-_GEOMETRY_INPUTS = (0, 1, 5, 6, 7, 8, 11, 12, 13)
-
-
-def _backward_mode(ctx):
-    """Keyword arguments of the node's library backward: none (the full backward) when a geometry input needs a
-    gradient or a gradient exchange is installed (set_grad_exchange), otherwise the appearance-only backward for the
-    appearance inputs that need one.  Frozen geometry (means2D included) thus pays only for the gradients it uses."""
-    need = ctx.needs_input_grad
-    if _EXCHANGE is not None or any(need[i] for i in _GEOMETRY_INPUTS):
-        return {}
-    return {"geometry": False, "appearance": (need[2], need[4], need[3])}
-
-
-def _aa_kw(antialiasing):
-    """The keyword that turns on the library's antialiased mode, only when it is on: an off call is the call without
-    the mode."""
-    return {"antialiasing": True} if antialiasing else {}
-
-
-def _f3d_kw(filter_3d, opacities=None):
-    """The keywords that turn on the library's 3D filter, only when a filter is given; the backward also takes the
-    forward's opacities."""
-    if filter_3d is None:
-        return {}
-    return {"filter_3d": filter_3d} if opacities is None else {"filter_3d": filter_3d, "opacities": opacities}
-
-
-def _absgrad_kw(ctx, kw):
-    """The keyword that asks the library backward for dL_dmeans2D_abs: only when the node's absgrad mode is on, means2D
-    needs a gradient and the backward runs its geometry half (`kw` from _backward_mode)."""
-    return {"absgrad": True} if ctx.absgrad and ctx.needs_input_grad[1] and kw.get("geometry", True) else {}
-
-
-def _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
-    """The positional arguments of _C.rasterize_gaussians for the settings `rs`."""
-    return (rs.bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp,
-            rs.viewmatrix, rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.cx, rs.cy, rs.image_height, rs.image_width, sh,
-            rs.sh_degree, rs.campos, rs.prefiltered, rs.computer_pseudo_normal, rs.debug)
-
-
-class _RasterizeGaussians(torch.autograd.Function):
-    """Autograd node (reference :58-185).  Inputs/outputs are the reference's; cotangents of weights / n_contrib /
-    radii are ignored exactly as there (:123-124 vs :132-157), and so are those of normal / surface_xyz unless
-    `surface_grads` is set.  Unlike the reference, the settings' `viewmatrix`, `projmatrix` and `campos` are inputs of
-    the node as well (the same tensors, passed after the settings): they get gradients when they require them, and the
-    backward computes those only then."""
+class _Rasterize(torch.autograd.Function):
+    """Autograd node of rasterize_gaussians (reference :58-185) and rasterize_views.  One view: the settings and
+    cameras [4,4], [4,4], [3] of one view; V views: V settings and the stacked cameras [V,4,4], [V,4,4], [V,3].
+    Inputs/outputs are the reference's; cotangents of weights / n_contrib / radii are ignored exactly as there
+    (:123-124 vs :132-157), and so are those of normal / surface_xyz unless `surface_grads` is set.  Unlike the
+    reference, the cameras are inputs of the node as well: they get gradients when they require them, and the backward
+    computes those only then."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
-                cov3Ds_precomp, raster_settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing,
-                ray_depth, depth_stats, absgrad):
-        rs = raster_settings
-        out = _debug_call(rs.debug, _C.rasterize_gaussians,
-                          _forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales, rotations,
-                                        cov3Ds_precomp),
-                          "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
-                          _defer=not rs.debug and _DEFER_COUNT and _CALL_GRAD_MODE and any(ctx.needs_input_grad),
-                          **_aa_kw(antialiasing), **_f3d_kw(filter_3d), **_rd_kw(ray_depth), **_ds_kw(depth_stats))
-        ctx.raster_settings = rs
-        ctx.depth_stats = depth_stats
-        ctx.antialiasing = antialiasing
-        ctx.ray_depth = ray_depth
-        ctx.absgrad = absgrad
-        ctx.means2D = means2D if absgrad else None      # the caller's tensor object: the backward sets .absgrad on it
+    def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                viewmatrix, projmatrix, campos, settings, modes, defer):
+        x = dict(zip(_INPUTS, (means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations,
+                               cov3Ds_precomp, viewmatrix, projmatrix, campos)))
+        ctx.settings, ctx.modes = settings, modes
+        if viewmatrix.dim() == 3:           # V views: the stacked backgrounds and the camera table
+            rs = settings[0]
+            ctx.views = (torch.stack([s.bg for s in settings]), [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings])
+            out = _C.rasterize_views(ctx.views[0], means3D, features, colors_precomp, opacities, scales, rotations,
+                                     rs.scale_modifier, cov3Ds_precomp, viewmatrix, projmatrix, ctx.views[1],
+                                     rs.image_height, rs.image_width, sh, rs.sh_degree, campos, rs.prefiltered,
+                                     rs.computer_pseudo_normal, **modes.forward_kw())
+        else:
+            ctx.views = None
+            out = _debug_call(settings.debug, _C.rasterize_gaussians, _forward_args(settings, x), "snapshot_fw.dump",
+                              "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
+                              _defer=defer, **modes.forward_kw())
+            # one view: the backward takes the cameras from the settings (the same tensors); saving them (often views
+            # of a larger buffer) would only add host time to every step
+            x.update(dict.fromkeys(_CAMERAS))
         ctx.num_rendered = out[0]
-        _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp,
-                      out[9], sh, *out[10:13], opacities, filter_3d)
-        return _stats_outputs(ctx, out)
+        ctx.means2D = means2D if modes.absgrad else None      # the caller's tensor object: the backward sets .absgrad on it
+        # cotangents of outputs the reference's backward ignores (num_contrib, normal, surface_xyz, weights, radii)
+        # stay None instead of being materialised as zero tensors (5 fill kernels per step); the four image
+        # cotangents are filled in by the backward when a loss does not touch one of them
+        ctx.set_materialize_grads(False)
+        ctx.out_shapes = tuple(t.shape for t in out[2:6])
+        x.update(filter_3d=modes.filter_3d, radii=out[9], geomBuffer=out[10], binningBuffer=out[11], imgBuffer=out[12])
+        ctx.save_for_backward(*(x[n] for n in _SAVED), *(out[3:5] if modes.surface_grads else ()))
+        return out[:10] + (tuple(out[13:15]) if modes.depth_stats else ())
 
     @staticmethod
-    def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature,
-                 g_normal, g_surface_xyz, g_weights, g_radii, *g_stats):
-        rs = ctx.raster_settings
-        (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, radii, sh,
-         geomBuffer, binningBuffer, imgBuffer, opacities, filter_3d) = ctx.saved_tensors[:13]
-        g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
-                                                                   g_feature)
-
-        def bwd_args(geom, num_rendered, binning, img):
-            return (rs.bg, means3D, features, radii, colors_precomp, scales, rotations,
-                    rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
-                    rs.tanfovy, g_color, g_opacity, g_depth, g_feature, sh, rs.sh_degree, rs.campos,
-                    geom, num_rendered, binning, img, rs.backward_geometry, rs.debug)
+    def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature, g_normal, g_surface_xyz,
+                 g_weights, g_radii, *g_stats):
+        rs, modes = (ctx.settings if ctx.views is None else ctx.settings[0]), ctx.modes
+        t = dict(zip(_SAVED, ctx.saved_tensors))
+        if ctx.views is None:
+            t.update(viewmatrix=rs.viewmatrix, projmatrix=rs.projmatrix, campos=rs.campos)
+        need = dict(zip(_INPUTS, ctx.needs_input_grad))
+        images = tuple(torch.zeros(shape, dtype=torch.float32, device=t["means3D"].device) if g is None else g
+                       for g, shape in zip((g_color, g_opacity, g_depth, g_feature), ctx.out_shapes))
         ex = None
-        if _EXCHANGE is not None:
-            if rs.debug or sh.numel() == 0:
+        if _EXCHANGE is not None and ctx.views is None:
+            if rs.debug or t["sh"].numel() == 0:
                 raise RuntimeError("a gradient exchange is installed (set_grad_exchange) but this backward cannot take "
                                    "part in it (debug mode or no `shs` input): every rank must run the same collectives")
             ex = _EXCHANGE
-        kw = _backward_mode(ctx)
-        kw.update(_aa_kw(ctx.antialiasing))
-        kw.update(_absgrad_kw(ctx, kw))
-        kw.update(_f3d_kw(filter_3d, opacities))
-        kw.update(_rd_kw(ctx.ray_depth))
-        kw.update(_ds_bwd_kw(ctx, g_stats))
+        # the full backward when a geometry input needs a gradient or a gradient exchange is installed, otherwise the
+        # appearance-only backward for the appearance inputs that need one: frozen geometry (means2D included) thus
+        # pays only for the gradients it uses
+        geometry = _EXCHANGE is not None or any(need[n] for n in _GEOMETRY)
+        kw = {} if geometry else {"geometry": False,
+                                  "appearance": (need["features"], need["colors_precomp"], need["sh"])}
+        kw.update(modes.backward_kw(t["opacities"], need["means2D"] and geometry, g_stats))
         if ex is not None:
             kw["_out"] = {"sh_factor": ex[0].factor}
-        if any(ctx.needs_input_grad[11:14]):         # viewmatrix, projmatrix, campos
+        if any(need[n] for n in _CAMERAS):
             kw["cam_grads"] = True
         # (appearance-only: the surface outputs depend only on the geometry, their cotangents have nothing to reach)
-        surface = _surface_cotangents(ctx, g_normal, g_surface_xyz) if kw.get("geometry", True) else None
-        if surface is not None:
-            kw["surface"] = surface + (rs.cx, rs.cy)
-        grads = _debug_call(rs.debug, _C.rasterize_gaussians_backward,
-                            bwd_args(geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer), "snapshot_bw.dump",
-                            "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n", **kw)
+        surface = geometry and modes.surface_grads and (g_normal is not None or g_surface_xyz is not None)
+        if surface:
+            kw["surface"] = ((g_normal, g_surface_xyz) + ctx.saved_tensors[len(_SAVED):] +
+                             ((rs.cx, rs.cy) if ctx.views is None else ()))
+
+        def library_backward(num_rendered, geom, binning, img):
+            if ctx.views is not None:
+                return _C.rasterize_views_backward(
+                    ctx.views[0], t["means3D"], t["features"], t["colors_precomp"], t["scales"], t["rotations"],
+                    rs.scale_modifier, t["cov3Ds_precomp"], t["viewmatrix"], t["projmatrix"], ctx.views[1], *images,
+                    t["sh"], rs.sh_degree, t["campos"], geom, binning, img, rs.backward_geometry, **kw)
+            return _debug_call(rs.debug, _C.rasterize_gaussians_backward,
+                               (rs.bg, t["means3D"], t["features"], t["radii"], t["colors_precomp"], t["scales"],
+                                t["rotations"], rs.scale_modifier, t["cov3Ds_precomp"], t["viewmatrix"],
+                                t["projmatrix"], rs.tanfovx, rs.tanfovy, *images, t["sh"], rs.sh_degree, t["campos"],
+                                geom, num_rendered, binning, img, rs.backward_geometry, rs.debug),
+                               "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n",
+                               **kw)
+        grads = library_backward(ctx.num_rendered, t["geomBuffer"], t["binningBuffer"], t["imgBuffer"])
         if isinstance(ctx.num_rendered, _C.DeferredCount):
             ctx.num_rendered.resolve()          # after the backward kernels are in flight
             if ctx.num_rendered.overflowed:     # rare: re-run the forward with the exact size, differentiate that
                 warnings.warn(f"deferred rasterization overflowed its binning buffer ({int(ctx.num_rendered)} instances); "
                               "forward re-run inside backward (cotangents come from the truncated first attempt)")
-                out = _C.rasterize_gaussians(*_forward_args(rs, means3D, features, sh, colors_precomp, opacities, scales,
-                                                            rotations, cov3Ds_precomp),
-                                             _min_capacity=int(ctx.num_rendered) + 4096, **_aa_kw(ctx.antialiasing),
-                                             **_f3d_kw(filter_3d), **_rerun_rd_kw(ctx.ray_depth),
-                                             **_ds_kw(ctx.depth_stats))
-                if surface is not None:         # the adjoint of the re-run's own surface pass
+                out = _C.rasterize_gaussians(*_forward_args(rs, t),
+                                             _min_capacity=int(ctx.num_rendered) + 4096, **modes.forward_kw(rerun=True))
+                if surface:                     # the adjoint of the re-run's own surface pass
                     kw["surface"] = (g_normal, g_surface_xyz, out[3], out[4], rs.cx, rs.cy)
-                grads = _C.rasterize_gaussians_backward(*bwd_args(out[10], out[0], out[11], out[12]), **kw)
+                grads = library_backward(out[0], *out[10:13])
+        g = dict(zip(_LIB_GRADS, grads[:9]))
         if ex is not None:                      # SH gradient: gather the views' factors, rebuild the mean locally
             exchange, campos_all = ex
             exchange.gather_factors()
-            g_sh_avg = exchange.rebuild_sh(means3D, campos_all, rs.sh_degree)
-            grads = grads[:6] + (g_sh_avg,) + grads[7:]
+            g["sh"] = exchange.rebuild_sh(t["means3D"], campos_all, rs.sh_degree)
         if kw.get("absgrad"):
             _set_absgrad(ctx.means2D, grads[-1])
             grads = grads[:-1]
-        return _input_grads(ctx, grads, (rs.viewmatrix, rs.projmatrix, rs.campos))
+        # camera gradients come in the cameras' shapes: None for those that do not need one (or when none was computed)
+        g.update((n, c.reshape(t[n].shape) if need[n] else None) for n, c in zip(_CAMERAS, grads[9:]))
+        return tuple(g.get(n) for n in _INPUTS) + (None,) * (len(ctx.needs_input_grad) - len(_INPUTS))
 
 
 def _refuse_camera_grad_with_exchange(*cameras):
@@ -345,16 +321,6 @@ def _refuse_camera_grad_with_exchange(*cameras):
             isinstance(t, torch.Tensor) and t.requires_grad for t in cameras):
         raise RuntimeError("camera gradients (a viewmatrix, projmatrix or campos that requires grad) cannot be combined "
                            "with an installed gradient exchange (set_grad_exchange)")
-
-
-_CALL_GRAD_MODE = True      # grad mode of the caller (inside autograd.Function.forward it is always off)
-
-
-def _refuse_surface_grads_without_normals(surface_grads, computer_pseudo_normal):
-    """Without the pseudo-normal pass both outputs are zeros: there is nothing to differentiate."""
-    if surface_grads and not computer_pseudo_normal:
-        raise ValueError("surface_grads=True needs computer_pseudo_normal=True: without it the normal and surface_xyz "
-                         "outputs are zeros and have no gradient")
 
 
 def _inputs(means3D, shs, colors_precomp, scales, rotations, cov3D_precomp, features):
@@ -423,16 +389,16 @@ def rasterize_gaussians(means3D, means2D, features, sh, colors_precomp, opacitie
     the reference's `lambda_depth_var`, and opacity depth2 - depth^2 the L2 depth distortion of 2DGS and Mip-NeRF 360.
     Both have gradients (the median's through the selected entry's depth only).  Every other output is unchanged, bit
     for bit.  There is no process default."""
-    global _CALL_GRAD_MODE
     rs = raster_settings
-    _C._check_filter_3d(filter_3d, means3D.shape[0], cov3Ds_precomp)
-    _refuse_surface_grads_without_normals(surface_grads, rs.computer_pseudo_normal)
+    modes = _modes(means3D.shape[0], cov3Ds_precomp, rs.computer_pseudo_normal, surface_grads, antialiasing, filter_3d,
+                   ray_depth, depth_stats, absgrad)
     _refuse_camera_grad_with_exchange(rs.viewmatrix, rs.projmatrix, rs.campos)
-    _CALL_GRAD_MODE = torch.is_grad_enabled()
-    return _RasterizeGaussians.apply(means3D, means2D, features, sh, colors_precomp, opacities,
-                                     scales, rotations, cov3Ds_precomp, raster_settings, bool(surface_grads),
-                                     rs.viewmatrix, rs.projmatrix, rs.campos, filter_3d, bool(antialiasing),
-                                     _ray_depth_on(ray_depth), bool(depth_stats), _absgrad_on(absgrad))
+    inputs = (means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+              rs.viewmatrix, rs.projmatrix, rs.campos)
+    # decided here: inside the node's forward, grad mode is always off
+    defer = (not rs.debug and _DEFER_COUNT and torch.is_grad_enabled()
+             and any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs))
+    return _Rasterize.apply(*inputs, raster_settings, modes, defer)
 
 
 class GaussianRasterizer(nn.Module):
@@ -469,55 +435,6 @@ _VIEWS_SHARED = ("image_height", "image_width", "sh_degree", "scale_modifier", "
                  "computer_pseudo_normal")
 
 
-class _RasterizeViews(torch.autograd.Function):
-    """Autograd node of rasterize_views: V views of one set of Gaussians in one forward and one backward call."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, features, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, surface_grads, viewmatrix, projmatrix, campos, filter_3d, antialiasing, ray_depth, depth_stats,
-                absgrad):
-        rs = settings[0]
-        bg = torch.stack([s.bg for s in settings])
-        cams = [(s.tanfovx, s.tanfovy, s.cx, s.cy) for s in settings]
-        out = _C.rasterize_views(bg, means3D, features, colors_precomp, opacities, scales, rotations, rs.scale_modifier,
-                                 cov3Ds_precomp, viewmatrix, projmatrix, cams, rs.image_height, rs.image_width, sh,
-                                 rs.sh_degree, campos, rs.prefiltered, rs.computer_pseudo_normal, **_aa_kw(antialiasing),
-                                 **_f3d_kw(filter_3d), **_rd_kw(ray_depth), **_ds_kw(depth_stats))
-        ctx.meta = (rs, cams, antialiasing)
-        ctx.depth_stats = depth_stats
-        ctx.ray_depth = ray_depth
-        ctx.absgrad = absgrad
-        ctx.means2D = means2D if absgrad else None
-        _save_forward(ctx, out, surface_grads, colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh,
-                      bg, viewmatrix, projmatrix, campos, *out[10:13], filter_3d,
-                      opacities if filter_3d is not None else None)
-        return _stats_outputs(ctx, out)
-
-    @staticmethod
-    def backward(ctx, g_num_rendered, g_num_contrib, g_color, g_opacity, g_depth, g_feature, g_normal, g_surface_xyz,
-                 g_weights, g_radii, *g_stats):
-        rs, cams, antialiasing = ctx.meta
-        (colors_precomp, means3D, features, scales, rotations, cov3Ds_precomp, sh, bg, viewmatrix, projmatrix, campos,
-         geomBuffer, binningBuffer, imgBuffer, filter_3d, opacities) = ctx.saved_tensors[:16]
-        g_color, g_opacity, g_depth, g_feature = _image_cotangents(ctx, means3D.device, g_color, g_opacity, g_depth,
-                                                                   g_feature)
-        kw = _backward_mode(ctx)
-        kw.update(_absgrad_kw(ctx, kw))
-        kw.update(_f3d_kw(filter_3d, opacities))
-        kw.update(_rd_kw(ctx.ray_depth))
-        kw.update(_ds_bwd_kw(ctx, g_stats))
-        if kw.get("geometry", True):
-            kw.update(cam_grads=any(ctx.needs_input_grad[11:14]), surface=_surface_cotangents(ctx, g_normal, g_surface_xyz))
-        grads = _C.rasterize_views_backward(bg, means3D, features, colors_precomp, scales, rotations, rs.scale_modifier,
-                                            cov3Ds_precomp, viewmatrix, projmatrix, cams, g_color, g_opacity, g_depth,
-                                            g_feature, sh, rs.sh_degree, campos, geomBuffer, binningBuffer, imgBuffer,
-                                            rs.backward_geometry, **_aa_kw(antialiasing), **kw)
-        if kw.get("absgrad"):
-            _set_absgrad(ctx.means2D, grads[-1])
-            grads = grads[:-1]
-        return _input_grads(ctx, grads, (viewmatrix, projmatrix, campos))
-
-
 def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_precomp=None, scales=None,
                     rotations=None, cov3D_precomp=None, features=None, surface_grads=False, antialiasing=False,
                     absgrad=False, filter_3d=None, ray_depth=False, depth_stats=False):
@@ -533,10 +450,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     the images are [V,C,H,W], `weights` [V,P,1], `radii` [V,P] and `num_contrib` [V,H,W] (a view of the work buffer).
     Each view equals the one-view call with its settings.  The call always reads the counts back synchronously;
     `debug=True` and an installed gradient exchange (`set_grad_exchange`) are refused, and so are more than
-    `MAX_VIEWS` views or V·P >= 2^30 rows.  `surface_grads`, `antialiasing`, `absgrad`, `filter_3d` and `ray_depth` are
-    those of rasterize_gaussians and apply to every view (each view with its own depth planes); `means2D.absgrad` is
-    then [V,P,2], each view's own.  With `depth_stats=True`, depth2 and median_depth [V,1,H,W] follow the ten outputs,
-    as in rasterize_gaussians."""
+    `MAX_VIEWS` views or V·P >= 2^30 rows.  The modes are those of rasterize_gaussians and apply to every view (each
+    view with its own depth planes); `means2D.absgrad` is then [V,P,2], and depth2 and median_depth [V,1,H,W]."""
     settings = list(settings)
     V = len(settings)
     if V < 1:
@@ -547,7 +462,8 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
         vals = {getattr(s, name) for s in settings}
         if len(vals) != 1:
             raise ValueError(f"rasterize_views: the views disagree on {name} ({sorted(vals)}); it must be shared")
-    _refuse_surface_grads_without_normals(surface_grads, settings[0].computer_pseudo_normal)
+    modes = _modes(means3D.shape[0], cov3D_precomp, settings[0].computer_pseudo_normal, surface_grads, antialiasing,
+                   filter_3d, ray_depth, depth_stats, absgrad)
     if any(s.debug for s in settings):
         raise ValueError("rasterize_views does not support debug=True; render the views one by one to debug")
     if _EXCHANGE is not None:
@@ -558,20 +474,16 @@ def rasterize_views(means3D, means2D, opacities, *, settings, shs=None, colors_p
     P = means3D.shape[0]
     if V * P >= 1 << 30:
         raise ValueError(f"rasterize_views: V*P = {V * P} rows exceed the limit of 2^30")
-    _C._check_filter_3d(filter_3d, P, cov3D_precomp)
     if tuple(means2D.shape) != (V, P, 3):
         raise ValueError(f"rasterize_views: means2D must be [V,P,3] = {(V, P, 3)}, got {tuple(means2D.shape)}")
     for name, t in (("features", features), ("colors_precomp", colors_precomp)):
         if t.dim() == 3 and t.shape[0] != V:
             raise ValueError(f"rasterize_views: per-view {name} must have V = {V} rows, got {t.shape[0]}")
     # stacked here, outside the node, so that autograd routes each view's camera gradients to that view's tensors
-    viewmatrix = torch.stack([s.viewmatrix for s in settings])
-    projmatrix = torch.stack([s.projmatrix for s in settings])
-    campos = torch.stack([s.campos for s in settings])
-    return _RasterizeViews.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
-                                 cov3D_precomp, tuple(settings), bool(surface_grads), viewmatrix, projmatrix, campos,
-                                 filter_3d, bool(antialiasing), _ray_depth_on(ray_depth), bool(depth_stats),
-                                 _absgrad_on(absgrad))
+    cameras = (torch.stack([s.viewmatrix for s in settings]), torch.stack([s.projmatrix for s in settings]),
+               torch.stack([s.campos for s in settings]))
+    return _Rasterize.apply(means3D, means2D, features, shs, colors_precomp, opacities, scales, rotations,
+                            cov3D_precomp, *cameras, tuple(settings), modes, False)
 
 
 MAX_VIEWS = 64          # R3DG_MAX_VIEWS (include/r3dg_b200.h)

@@ -351,3 +351,54 @@ def adam_case():
         gs[1][::2] = 0.0
         return [t.numpy() for t in gs]
     return params, lrs, grads_for_step, {5: [(0, 1.0e-4)]}
+
+
+def fake_raster_library(monkeypatch, overflow=False):
+    """Replaces the four library functions behind rasterizer._C with stand-ins that record each call as (name, keyword
+    arguments) in the list returned, and give zero outputs and gradients of the right shapes (None for the geometry
+    gradients of an appearance-only backward).  With `overflow`, a deferred forward's count overflows its buffer, so
+    the backward re-runs the forward."""
+    import inspect
+    from relightable3dgaussian_b200 import _C_raster
+    from relightable3dgaussian_b200 import rasterizer as R
+
+    class Overflowed(_C_raster.DeferredCount):
+        def __init__(self):
+            self._value, self.overflowed = 10, True
+
+        def resolve(self):
+            return 10
+
+        __int__ = __index__ = resolve
+    calls = []
+
+    def stand_in(name):
+        sig = inspect.signature(getattr(_C_raster, name))
+
+        def call(*args, **kw):
+            calls.append((name, kw))
+            b = sig.bind(*args, **kw)
+            b.apply_defaults()
+            a = b.arguments
+            P, S = a["means3D"].shape[0], a["features"].shape[-1]
+            V = len(a["cams"]) if "views" in name else 1
+            lead = (V,) if "views" in name else ()
+            z = lambda *s: torch.zeros(*s)                                       # noqa: E731
+            if not name.endswith("backward"):
+                H, W = a["image_height"], a["image_width"]
+                count = [1] * V if lead else (Overflowed() if overflow and a["_defer"] else 1)
+                return ((count, z(lead + (H, W)).int()) + tuple(z(lead + (c, H, W)) for c in (3, 1, 1, S, 3, 3)) +
+                        (z(lead + (P, 1)), z(lead + (P,)).int()) + tuple(z(8).byte() for _ in range(3)) +
+                        ((z(lead + (1, H, W)), z(lead + (1, H, W))) if a["depth_stats"] else ()))
+            geo = a["geometry"]
+            M = a["sh"].shape[1] if a["sh"].numel() else 0
+            grads = (z(lead + (P, 3)) if geo else None, z(P, 3), z(P, 1) if geo else None, z(P, 3) if geo else None,
+                     z(tuple(a["features"].shape)), z(P, 6) if geo else None, z(P, M, 3), z(P, 3) if geo else None,
+                     z(P, 4) if geo else None)
+            if a["cam_grads"]:
+                grads += (z(lead + (4, 4)), z(lead + (4, 4)), z(lead + (3,)))
+            return grads + ((z(lead + (P, 2)) if geo else None,) if a["absgrad"] else ())
+        return call
+    for name in ("rasterize_gaussians", "rasterize_gaussians_backward", "rasterize_views", "rasterize_views_backward"):
+        monkeypatch.setattr(R._C, name, stand_in(name))
+    return calls

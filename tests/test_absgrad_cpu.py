@@ -10,6 +10,7 @@ import torch
 import absgrad64
 import raster64
 import densify_oracle as do
+from helpers import fake_raster_library
 from relightable3dgaussian_b200 import _C_raster, _lib, densify
 from relightable3dgaussian_b200 import rasterizer as R
 
@@ -128,10 +129,6 @@ def test_keyword_defaults_off(fn):
     assert inspect.signature(fn).parameters["absgrad"].default is False
 
 
-class _Stop(Exception):
-    pass
-
-
 def _settings():
     rs = R.GaussianRasterizationSettings(4, 5, 1.0, 1.0, 2.5, 2.0, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 3,
                                          torch.zeros(3), False, True, True, False)
@@ -142,44 +139,49 @@ def _settings():
     return rs, lv
 
 
-@pytest.mark.parametrize("how", ["off", "keyword", "process-default"])
-def test_nodes_take_the_mode(monkeypatch, how):
-    """The autograd nodes get the call's absgrad mode: the keyword, or set_absgrad's process default."""
-    seen = []
+def _backward_kw(calls):
+    return [kw for name, kw in calls if name.endswith("backward")]
 
-    def fake(*args):
-        seen.append(args[-1])
-        raise _Stop()
-    monkeypatch.setattr(R._RasterizeGaussians, "apply", fake)
-    monkeypatch.setattr(R._RasterizeViews, "apply", fake)
+
+def _render_one(rs, lv, means2D, **kw):
+    out = R.GaussianRasterizer(rs, **kw)(means3D=lv["means3D"], means2D=means2D, opacities=lv["opacities"],
+                                         shs=lv["shs"], scales=lv["scales"], rotations=lv["rotations"])
+    out[2].sum().backward()
+
+
+@pytest.mark.parametrize("how", ["off", "keyword", "process-default"])
+def test_calls_take_the_mode(monkeypatch, how):
+    """The autograd node gets the call's absgrad mode, the keyword or set_absgrad's process default, and hands it to
+    the library backward of one view and of V views."""
+    calls = fake_raster_library(monkeypatch)
     rs, lv = _settings()
     R.set_absgrad(how == "process-default")
     try:
         kw = {"absgrad": True} if how == "keyword" else {}
-        with pytest.raises(_Stop):
-            R.GaussianRasterizer(rs, **kw)(means3D=lv["means3D"], means2D=torch.zeros(7, 3), opacities=lv["opacities"],
-                                           shs=lv["shs"], scales=lv["scales"], rotations=lv["rotations"])
-        with pytest.raises(_Stop):
-            R.rasterize_views(lv["means3D"], torch.zeros(2, 7, 3), lv["opacities"], settings=[rs, rs], shs=lv["shs"],
-                              scales=lv["scales"], rotations=lv["rotations"], **kw)
+        _render_one(rs, lv, torch.zeros(7, 3, requires_grad=True), **kw)
+        out = R.rasterize_views(lv["means3D"], torch.zeros(2, 7, 3, requires_grad=True), lv["opacities"],
+                                settings=[rs, rs], shs=lv["shs"], scales=lv["scales"], rotations=lv["rotations"], **kw)
+        out[2].sum().backward()
     finally:
         R.set_absgrad(False)
-    assert seen == [how != "off"] * 2
-
-
-class _Ctx:
-    def __init__(self, absgrad, needs):
-        self.absgrad, self.needs_input_grad = absgrad, needs
+    assert [k.get("absgrad") for k in _backward_kw(calls)] == [True if how != "off" else None] * 2
 
 
 @pytest.mark.parametrize("absgrad, means2d, geometry, want", [
     (False, True, True, {}), (True, True, True, {"absgrad": True}),
     (True, False, True, {}),          # means2D needs no gradient: nothing computed, nothing set
-    (True, True, False, {})])         # (the appearance-only backward has no geometry half)
-def test_backward_asks_only_when_means2d_needs_a_gradient(absgrad, means2d, geometry, want):
-    needs = (True, means2d) + (False,) * 13
-    kw = {} if geometry else {"geometry": False}
-    assert R._absgrad_kw(_Ctx(absgrad, needs), kw) == want
+    (True, False, False, {})])        # (the appearance-only backward has no geometry half)
+def test_backward_asks_for_absgrad_only_when_means2d_needs_a_gradient(monkeypatch, absgrad, means2d, geometry, want):
+    calls = fake_raster_library(monkeypatch)
+    rs, lv = _settings()
+    lv["means3D"].requires_grad_(geometry)
+    lv["shs"].requires_grad_(True)
+    means2D = torch.zeros(7, 3, requires_grad=means2d)
+    _render_one(rs, lv, means2D, absgrad=absgrad)
+    (kw,) = _backward_kw(calls)
+    assert {k: v for k, v in kw.items() if k == "absgrad"} == want
+    assert kw.get("geometry", True) is geometry
+    assert (getattr(means2D, "absgrad", None) is not None) == bool(want)
 
 
 def test_attribute_accumulates_like_grad():
@@ -189,14 +191,18 @@ def test_attribute_accumulates_like_grad():
     assert torch.equal(t.absgrad, torch.full((3, 2), 3.0))
 
 
-def test_set_absgrad_round_trip():
-    assert R._ABSGRAD is False and R._absgrad_on(False) is False
+def test_set_absgrad_round_trips_through_the_backward(monkeypatch):
+    calls = fake_raster_library(monkeypatch)
+    rs, lv = _settings()
+    assert R._ABSGRAD is False
     R.set_absgrad(True)
     try:
-        assert R._absgrad_on(False) is True
+        _render_one(rs, lv, torch.zeros(7, 3, requires_grad=True))
     finally:
         R.set_absgrad(False)
-    assert R._absgrad_on(False) is False and R._absgrad_on(True) is True
+    _render_one(rs, lv, torch.zeros(7, 3, requires_grad=True))
+    _render_one(rs, lv, torch.zeros(7, 3, requires_grad=True), absgrad=True)
+    assert [k.get("absgrad") for k in _backward_kw(calls)] == [True, None, True]
 
 
 def _model():

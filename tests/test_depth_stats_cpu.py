@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import depthstats64 as ds64
+from helpers import fake_raster_library
 from relightable3dgaussian_b200 import _C_raster, _lib
 from relightable3dgaussian_b200 import rasterizer as R
 
@@ -197,72 +198,47 @@ def test_host_layer_passes_the_flag_to_the_forward(monkeypatch, on):
     assert [k.get("depth_stats") for k in seen] == ([True, True] if on else [None, None])
 
 
-def _ctx(depth_stats=True, geometry=True):
-    class Ctx:
-        needs_input_grad = (geometry, False, True) + (False,) * 16
-        antialiasing = False
-        ray_depth = False
-        absgrad = False
-        surface_grads = False
-        out_shapes = ((3, 4, 5), (1, 4, 5), (1, 4, 5), (0, 4, 5))
-        num_rendered = 1
-        raster_settings = _settings()[0]
-        saved_tensors = (torch.zeros(0),) * 13
-    c = Ctx()
-    c.depth_stats = depth_stats
-    return c
+def _render(rs, lv, geometry=True, **kw):
+    """A one-view forward with means3D (geometry) or only shs (appearance) requiring grad; returns its outputs."""
+    P = lv["means3D"].shape[0]
+    return R.GaussianRasterizer(rs, **kw)(means3D=lv["means3D"].requires_grad_(geometry), means2D=torch.zeros(P, 3),
+                                          opacities=lv["opacities"], shs=lv["shs"].requires_grad_(True),
+                                          scales=lv["scales"], rotations=lv["rotations"])
 
 
 @pytest.mark.parametrize("geometry", [True, False])
-def test_backward_gets_the_flag_and_the_cotangents(monkeypatch, geometry):
-    seen = []
-
-    def fake_bwd(*args, **kw):
-        seen.append(kw)
-        raise _Stop()
-    monkeypatch.setattr(R._C, "rasterize_gaussians_backward", fake_bwd)
+def test_library_backward_gets_the_flag_and_the_cotangents(monkeypatch, geometry):
+    calls = fake_raster_library(monkeypatch)
+    rs, lv = _settings()
+    out = _render(rs, lv, geometry, depth_stats=True)
     g2, gm = torch.ones(1, 4, 5), torch.full((1, 4, 5), 2.0)
-    with pytest.raises(_Stop):
-        R._RasterizeGaussians.backward(_ctx(geometry=geometry), *([None] * 10), g2, gm)
-    assert seen[0]["depth_stats"] is True
-    assert seen[0]["dL_dout_depth2"] is g2 and seen[0]["dL_dout_median_depth"] is gm
-    assert seen[0].get("geometry", True) is geometry
+    torch.autograd.backward([out[10], out[11]], [g2, gm])
+    name, kw = calls[-1]
+    assert name == "rasterize_gaussians_backward" and kw["depth_stats"] is True
+    assert kw["dL_dout_depth2"] is g2 and kw["dL_dout_median_depth"] is gm
+    assert kw.get("geometry", True) is geometry
     # flag off: the call is exactly the flag-off call
-    seen.clear()
-    with pytest.raises(_Stop):
-        R._RasterizeGaussians.backward(_ctx(depth_stats=False), *([None] * 10))
-    assert "depth_stats" not in seen[0] and "dL_dout_depth2" not in seen[0]
+    calls.clear()
+    _render(rs, lv, geometry)[2].sum().backward()
+    assert "depth_stats" not in calls[-1][1] and "dL_dout_depth2" not in calls[-1][1]
 
 
-def test_deferred_count_rerun_keeps_the_flag(monkeypatch):
+def test_deferred_count_rerun_through_backward_keeps_the_flag(monkeypatch):
     """The deferred-count repair re-runs the forward with the flag and differentiates the re-run's buffers."""
-    calls = []
-
-    class Overflowed(_C_raster.DeferredCount):
-        def __init__(self):
-            self._value, self.overflowed = 10, True
-
-        def resolve(self):
-            return 10
-
-        __int__ = __index__ = resolve
-
-    def fake_fwd(*args, **kw):
-        calls.append(("fwd", kw))
-        return (11,) + tuple(torch.zeros(1) for _ in range(14))
-
-    def fake_bwd(*args, **kw):
-        calls.append(("bwd", kw))
-        return tuple(torch.zeros(1) for _ in range(9))
-    monkeypatch.setattr(R._C, "rasterize_gaussians", fake_fwd)
-    monkeypatch.setattr(R._C, "rasterize_gaussians_backward", fake_bwd)
-    ctx = _ctx()
-    ctx.num_rendered = Overflowed()
+    calls = fake_raster_library(monkeypatch, overflow=True)
+    rs, lv = _settings()
+    R.set_deferred_count(True)
+    try:
+        out = _render(rs, lv, depth_stats=True)
+    finally:
+        R.set_deferred_count(False)
     with pytest.warns(UserWarning):
-        R._RasterizeGaussians.backward(ctx, *([None] * 10), torch.ones(1, 4, 5), None)
-    assert [c[0] for c in calls] == ["bwd", "fwd", "bwd"]
-    assert calls[1][1].get("depth_stats") is True
-    assert calls[2][1]["depth_stats"] is True and calls[2][1]["dL_dout_median_depth"] is None
+        out[10].sum().backward()
+    assert [n for n, _ in calls] == ["rasterize_gaussians", "rasterize_gaussians_backward", "rasterize_gaussians",
+                                     "rasterize_gaussians_backward"]
+    assert calls[0][1]["_defer"] is True and "_defer" not in calls[2][1]
+    assert calls[2][1].get("depth_stats") is True
+    assert calls[3][1]["depth_stats"] is True and calls[3][1]["dL_dout_median_depth"] is None
 
 
 def test_debug_snapshot_records_the_flag(monkeypatch, tmp_path):

@@ -10,6 +10,7 @@ import torch
 import aa_oracle
 import proj64
 import raydepth64
+from helpers import fake_raster_library
 from relightable3dgaussian_b200 import _C_raster, _lib, synth
 from relightable3dgaussian_b200 import rasterizer as R
 
@@ -205,14 +206,23 @@ def test_keyword_defaults_are_off():
         R.set_ray_depth(False)
 
 
-def test_set_ray_depth_round_trips():
-    assert R._ray_depth_on(False) is False
+def test_set_ray_depth_round_trips_through_the_forward(monkeypatch):
+    calls = fake_raster_library(monkeypatch)
+    rs, lv = _settings()
+    P = lv["means3D"].shape[0]
+
+    def render(**kw):
+        R.GaussianRasterizer(rs, **kw)(means3D=lv["means3D"], means2D=torch.zeros(P, 3), opacities=lv["opacities"],
+                                       shs=lv["shs"], scales=lv["scales"], rotations=lv["rotations"])
+    render()
     R.set_ray_depth(True)
     try:
-        assert R._ray_depth_on(False) is True
+        render()
     finally:
         R.set_ray_depth(False)
-    assert R._ray_depth_on(False) is False and R._ray_depth_on(True) is True
+    render()
+    render(ray_depth=True)
+    assert [kw.get("ray_depth") for _, kw in calls] == [None, True, None, True]
 
 
 class _Stop(Exception):
@@ -257,29 +267,19 @@ def test_host_layer_passes_the_flag(monkeypatch, how):
     assert [k.get("ray_depth") for k in seen] == ([None, None] if how == "off" else [True, True])
 
 
-def test_backward_gets_the_flag(monkeypatch):
+def test_library_backward_gets_the_flag(monkeypatch):
     """The autograd node hands the forward's flag to the library backward, also for the appearance-only backward (its
     work buffers have the mode's layout)."""
-    seen = []
-
-    def fake_bwd(*args, **kw):
-        seen.append(kw)
-        raise _Stop()
-    monkeypatch.setattr(R._C, "rasterize_gaussians_backward", fake_bwd)
-
-    class Ctx:
-        needs_input_grad = (False, False, True) + (False,) * 15
-        antialiasing = False
-        ray_depth = True
-        absgrad = False
-        surface_grads = False
-        out_shapes = ((3, 4, 5), (1, 4, 5), (1, 4, 5), (0, 4, 5))
-        num_rendered = 1
-        raster_settings = _settings()[0]
-        saved_tensors = (torch.zeros(0),) * 13
-    with pytest.raises(_Stop):
-        R._RasterizeGaussians.backward(Ctx(), None, None, None, None, None, None, None, None, None, None)
-    assert seen[0].get("ray_depth") is True and seen[0].get("geometry") is False
+    calls = fake_raster_library(monkeypatch)
+    rs, lv = _settings()
+    P = lv["means3D"].shape[0]
+    out = R.GaussianRasterizer(rs, ray_depth=True)(means3D=lv["means3D"], means2D=torch.zeros(P, 3),
+                                                   opacities=lv["opacities"], shs=lv["shs"].requires_grad_(True),
+                                                   scales=lv["scales"], rotations=lv["rotations"])
+    out[2].sum().backward()
+    name, kw = calls[-1]
+    assert name == "rasterize_gaussians_backward"
+    assert kw.get("ray_depth") is True and kw.get("geometry") is False
 
 
 def test_debug_snapshot_records_the_flag(monkeypatch, tmp_path):
