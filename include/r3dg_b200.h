@@ -332,7 +332,11 @@ int r3dg_sh_grad_from_factors(int P, int D, int M, int num_views, const float* m
  *       writes it back to all ranks with `multimem.st`; with dense_multicast == NULL it falls back to peer loads/stores.
  * The caller must order it between two cross-rank barriers (all ranks' backward kernels done before; all ranks'
  * exchange kernels done before anyone reads the dense section or overwrites a factor buffer).  n_dense: floats,
- * a multiple of 4, 16-byte aligned sections.  world <= 64. */
+ * a multiple of 4, 16-byte aligned sections.  world <= 64.  Slice r is float4s [r c, (r + 1) c) of the section, with
+ * c = ceil(n_dense / 4 / world), clipped to the section (empty for the last ranks when n_dense / 4 < world).
+ * R3DG_ERR_BAD_ARG before any launch: P < 0, D outside 0..3, M outside 1..16 or below (D + 1)^2, world outside 1..64,
+ * rank outside [0, world), n_dense negative or not a multiple of 4, a NULL means3D, campos, dL_dsh or factors[v]
+ * with P > 0, or a NULL dense[v] with n_dense > 0. */
 typedef struct r3dg_exchange_args {
     int P, D, M, world, rank;
     const float* means3D;          /* [P,3] (replicated) */

@@ -203,6 +203,7 @@ int r3dg_exchange_p2p(const r3dg_exchange_args* a, r3dg_stream_t stream) {
     if (a->world < 1 || a->world > SHX_MAX_VIEWS || a->rank < 0 || a->rank >= a->world) return R3DG_ERR_BAD_ARG;
     if (a->n_dense < 0 || (a->n_dense & 3)) return R3DG_ERR_BAD_ARG;
     if (a->P == 0 && a->n_dense == 0) return 0;
+    if (a->P > 0 && (!a->means3D || !a->campos || !a->dL_dsh)) return R3DG_ERR_BAD_ARG;
     ShxParams p = {};
     p.P = a->P; p.D = a->D; p.M = a->M; p.num_views = a->world; p.rank = a->rank;
     p.means3D = a->means3D; p.campos = a->campos; p.scale = 1.0f / (float)a->world; p.dL_dsh = a->dL_dsh;
