@@ -28,8 +28,10 @@ constexpr int FWD_NT = 256;
 constexpr int MAX_NODES = 1024;        // staged nodes per tile (48 KB of coefficients)
 constexpr int MAX_L = 16;              // 4 L (xy corner, z node) rows over the 32 lanes of the backward warp: R <= 2
 
-// Grid coordinate of pixel p on an axis of npix pixels and n nodes: (p + 0.5) (n - 1) / npix, correctly rounded (the
-// product is exact for the supported sizes).  In [0, n - 1] and monotone in p.
+// Grid coordinate of pixel p on an axis of npix pixels and n nodes: fl(fl((p + 0.5) (n - 1)) / npix), each step
+// correctly rounded.  The product is not always exact (e.g. npix = 100003, n = 1024), so the result can lie about an
+// fp32 ulp from the exact coordinate; every step is monotone, so it stays in [0, n - 1] and monotone in p, and all
+// tiles agree on each pixel's cell.
 __device__ __forceinline__ float pix_coord(int p, int n, int npix) {
     return div_(mul_((float)p + 0.5f, (float)(n - 1)), (float)npix);
 }
@@ -212,6 +214,9 @@ __global__ void __launch_bounds__(32) bilagrid_bwd_kernel(int H, int W, int GX, 
         for (int k = 0; k < 12; ++k) acc[j][k] = 0.0f;
     int cur_x = -1, cur_y = -1;                      // xy cell of the rows being accumulated (sub-grid relative)
     auto flush = [&]() {
+        // consecutive flushes of one pixel row share part entries across lanes (corner bx = 1 of cell X is corner
+        // bx = 0 of cell X + 1), so the previous flush's stores must be visible first
+        __syncwarp();
         if (cur_x < 0) return;
 #pragma unroll
         for (int j = 0; j < R; ++j) {

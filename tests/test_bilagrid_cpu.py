@@ -1,6 +1,7 @@
 """Bilateral-grid slice without a GPU: the fp64 numpy restatement (tests/bilagrid_oracle.py) against
-F.grid_sample + autograd in fp64, the grids' TV term against an explicit sum, and the argument checks of the C ABI and
-of bilagrid.slice, none of which may launch anything."""
+F.grid_sample + autograd in fp64, its fp32 fma and per-element scales, the grids' TV term against an explicit sum, the
+host's bound on each tile's staged nodes against the device's fp32 count, the workspace size, and the argument checks
+of the C ABI and of bilagrid.slice, none of which may launch anything."""
 import ctypes
 
 import numpy as np
@@ -125,6 +126,95 @@ def test_abi_rejects_bad_arguments_before_launching():
     # the smallest images gsplat's default grid fits, as the header states
     assert lib.r3dg_bilagrid_tmp_bytes(1, 1, 52, 52, 16, 16, 8) > 0
     assert lib.r3dg_bilagrid_tmp_bytes(1, 1, 51, 52, 16, 16, 8) == 0
+
+
+TS = 32                           # csrc/bilagrid.cu: tile edge in pixels
+
+
+def _host_bound(n, npix):
+    """max_tile_nodes: min(n, (int)((double)(TS - 1)(n - 1) / npix + 1e-3) + 3)."""
+    return np.minimum(n, (float(TS - 1) * (n - 1) / npix + 1e-3).astype(np.int64) + 3)
+
+
+def _device_counts(n, npix):
+    """tile_nodes' count for every tile of an axis of npix pixels ([len(n), tiles]) and n nodes ([len(n), 1]), in the
+    kernel's float32 arithmetic: pix_coord = fl(fl(fl(p + 0.5) (n - 1)) / npix), cell_of = min((int)c, n - 2)."""
+    t0 = np.arange(0, npix, TS)
+    t1 = np.minimum(t0 + TS, npix) - 1
+
+    def cell(p):
+        c = (p.astype(np.float32) + np.float32(0.5)) * (n - 1).astype(np.float32) / np.float32(npix)
+        return np.minimum(c.astype(np.int64), n - 2)
+    return cell(t1) + 2 - cell(t0)
+
+
+def test_no_tile_stages_more_nodes_than_the_host_sized():
+    """The host sizes the staged sub-grid, the shared memory, the workspace slab and the reduce's indexing with
+    max_tile_nodes; each tile's real count comes from fp32 coordinates on the device.  Over every n in [2, 1024] and
+    every axis length up to 1024 plus the usual training widths and the largest axis, the device count never exceeds
+    the host bound (and the tiles at the bound exist)."""
+    n = np.arange(2, 1025)[:, None]
+    at_bound = 0
+    for npix in list(range(1, 1025)) + [1080, 1200, 1216, 1440, 1600, 1920, 2160, 3840, 4096, 16384, 100003, 1 << 20]:
+        for lo in range(0, len(n), 128):              # [128, 32768] int64 at most per step
+            nn = n[lo:lo + 128]
+            cnt = _device_counts(nn, npix).max(axis=1)
+            host = _host_bound(nn[:, 0], npix)
+            bad = cnt > host
+            assert not bad.any(), (npix, nn[bad, 0][:5], cnt[bad][:5], host[bad][:5])
+            at_bound += int((cnt == host).sum())
+    assert at_bound > 0
+
+
+@pytest.mark.parametrize("G,N,H,W,GX,GY,L", [(1, 1, 20, 20, 64, 8, 2), (1, 1, 40, 40, 8, 8, 16),
+                                             (2, 3, 64, 80, 16, 16, 8), (4, 9, 48, 80, 10, 6, 8),
+                                             (3, 2, 33, 65, 33, 7, 4), (1, 1, 1, 100003, 1024, 2, 8),
+                                             (1, 1, 1080, 1920, 2, 2, 8), (5, 64, 24, 40, 6, 4, 5)])
+def test_workspace_is_one_host_sized_slab_per_tile(G, N, H, W, GX, GY, L):
+    """r3dg_bilagrid_tmp_bytes = align256(tiles_x tiles_y N nx ny L 12 floats) with the host bounds nx and ny; the
+    first two shapes stage exactly MAX_NODES = 1024 nodes, and one more node in x is refused (0 bytes)."""
+    lib = _lib.load()
+    nx, ny = (int(_host_bound(np.array(GX), W)), int(_host_bound(np.array(GY), H)))
+    slab = -(-W // TS) * -(-H // TS) * N * nx * ny * L * 48
+    assert lib.r3dg_bilagrid_tmp_bytes(G, N, H, W, GX, GY, L) == -(-slab // 256) * 256
+    if (H, W) in ((20, 20), (40, 40)):
+        assert nx * ny * L == 1024
+        assert lib.r3dg_bilagrid_tmp_bytes(G, N, H, W, GX + 1, GY, L) == 0
+
+
+def test_fma32_is_correctly_rounded():
+    """The oracle's fp32 fma (the kernel's luma) against exact rational arithmetic, including a sum that rounds to an
+    fp32 midpoint in fp64: 1 + 2^-23 + 2^-24 - 2^-54, where rounding through fp64 would give 1 + 2^-22."""
+    from fractions import Fraction
+    a, b, c = np.float32(1 + 2.0 ** -15), np.float32(2.0 ** -24 * (1 - 2.0 ** -15)), np.float32(1 + 2.0 ** -23)
+    assert np.float32(np.float64(a) * np.float64(b) + np.float64(c)) == np.float32(1 + 2.0 ** -22)
+    assert bo.fma32(a, b, c) == np.float32(1 + 2.0 ** -23)
+    rs = np.random.default_rng(0)
+    a, b = rs.standard_normal(2000).astype(np.float32), rs.standard_normal(2000).astype(np.float32)
+    c = (rs.standard_normal(2000) * 10.0 ** rs.integers(-9, 9, 2000)).astype(np.float32)
+    for x, y, z, got in zip(a, b, c, bo.fma32(a, b, c)):
+        exact = Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z))
+        lo, hi = np.nextafter(got, np.float32(-np.inf)), np.nextafter(got, np.float32(np.inf))
+        err = abs(Fraction(float(got)) - exact)
+        assert err <= abs(Fraction(float(lo)) - exact) and err <= abs(Fraction(float(hi)) - exact), (x, y, z)
+
+
+@pytest.mark.parametrize("coords", ["fp64", "fp32"])
+def test_scales_bound_their_values_and_vanish_where_nothing_contributes(coords):
+    """Each truth value is at most its scale (a sum of the magnitudes of its terms), the scales of an unused grid and of
+    nodes no pixel reaches are exactly 0, and the two coordinate choices agree to a few eps32 of the scale."""
+    ids, L = [2, 0, 2], 4
+    grids, rgb = bo.random_case(3, 3, 9, 40, L, 3, 30, seed=2, luma_lo=-0.3, luma_hi=1.3, noise=0.3)
+    dout = np.random.default_rng(2).standard_normal(rgb.shape)
+    out = bo.slice64(grids, rgb, ids, coords)
+    drgb, dgrids, _ = bo.grads64(grids, rgb, ids, dout, coords)
+    m_out, m_drgb, m_dgrids = bo.scales64(grids, rgb, ids, dout, coords)
+    for v, m in ((out, m_out), (drgb, m_drgb), (dgrids, m_dgrids)):
+        assert np.all(np.abs(v) <= m * (1 + 1e-12))
+    assert np.all(m_dgrids[1] == 0) and np.all(dgrids[1] == 0)
+    assert (m_dgrids[0] == 0).any() and np.all(dgrids[m_dgrids == 0] == 0)   # 30 x nodes over 40 px: some unreached
+    other = bo.slice64(grids, rgb, ids, "fp64" if coords == "fp32" else "fp32")
+    assert np.all(np.abs(other - out) <= 64 * 2.0 ** -24 * m_out)
 
 
 def test_slice_rejects_bad_ids_and_dtypes_on_the_host():
