@@ -674,6 +674,12 @@ typedef struct r3dg_shade_args {
     int V;
     int transform_per_view;            /* non-zero with V > 1: env_transform is [V,3,3]; forward only (the backward
                                         * returns R3DG_ERR_UNSUPPORTED) */
+    /* Prefiltered environment (PREFILTERED ENVIRONMENT below).  env_pyramid: NULL = the point lookup above, or the
+     * r3dg_env_pyramid_build output of `env`, whose env_h x env_w level 0 equals `env`: each incident sample then reads
+     * the env averaged over its own solid angle.  dL_denv_pyramid: backward workspace of r3dg_env_pyramid_floats floats,
+     * required (R3DG_ERR_BAD_ARG) whenever env_pyramid is set; dL_denv is still the complete gradient of `env`. */
+    const float* env_pyramid;
+    float* dL_denv_pyramid;
     /* Deterministic mode (torch.use_deterministic_algorithms(True)): non-zero (backward only) = sums that float atomics would make
      * depend on warp arrival order are accumulated in fixed point in `det_work` (see DETERMINISTIC MODE below);
      * det_work: device workspace of at least r3dg_shade_det_bytes(env_h, env_w) bytes, zeroed by the call.  0 = the default path (det_work unused). */
@@ -683,6 +689,51 @@ typedef struct r3dg_shade_args {
 
 int r3dg_render_equation_forward(const r3dg_shade_args* args, r3dg_stream_t stream);
 int r3dg_render_equation_backward(const r3dg_shade_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * PREFILTERED ENVIRONMENT (the shading step's filtered mode).  Each incident sample s of Gaussian g
+ * stands for a solid angle Omega = incident_areas[g,s] / N (2 pi / N in the reference), yet the point
+ * lookup reads one bilinear tap of the env.  With a 1024x512 or 2000x1000 HDR map and N = 64 a sample
+ * covers thousands of texels, and small bright sources alias.  The filtered mode reads a lat-long mip
+ * pyramid at the sample's footprint instead; directions, visibility and areas are unchanged.
+ *   Pyramid.  Level 0 is the activated env [He,We,3].  Level l+1 has ceil(H_l / 2) x ceil(W_l / 2)
+ *   texels, made while level l has at least 3 rows and 3 columns (at most 16 levels); an env with
+ *   fewer than 3 rows or columns has level 0 only, and the mode changes nothing for it.  Every level
+ *   is read on the grid of grid_sample(align_corners=True) at its own size: rows 0 and H-1 are the
+ *   poles, columns 0 and W-1 the same azimuth.  Row j stands for the latitude band
+ *   [(j - 1/2) dt, (j + 1/2) dt] clipped to [0, pi], dt = pi / (H-1), column i for the azimuth cell
+ *   [(i - 1/2) dp, (i + 1/2) dp] modulo 2 pi, dp = 2 pi / (W-1); a texel's weight is its cell's solid
+ *   angle, 2 sin(dt/2) dp sin(theta) inside and (1 - cos(dt/2)) dp at a pole (sin(theta) clamped).
+ *   A coarser texel is the mean of the finer level over its cell, each finer texel weighted by the
+ *   solid angle the two cells share (fp64 sums, one rounding to fp32); a pole row is the mean over
+ *   its whole cap, and column W-1 repeats column 0.  So a constant env gives that constant at every
+ *   level, the solid-angle-weighted mean is kept at every level, the seam columns are equal and each
+ *   pole row is constant.
+ *   Level of detail.  d = the sample direction after env_transform, theta = acos(d.z),
+ *   Omega0 = dt0 dp0 max(sin(theta), sin(dt0 / 2)) (level 0's texel solid angle),
+ *   lambda = log2(Omega / Omega0) / 2 clamped to [0, L-1], evaluated in fp32.  The lookup blends
+ *   levels floor(lambda) and floor(lambda) + 1 with weights 1 - f and f (f = the fraction), each with
+ *   the four bilinear taps of the point lookup at that level's size.  At lambda <= 0 the lookup is the
+ *   point lookup, its taps, arithmetic and bits.  Near the poles this isotropic footprint blurs
+ *   latitude more than needed (a texel is narrow in azimuth there); that is accepted.
+ *   Gradients.  lambda depends only on the baked direction and area and carries none; dL/denv is the
+ *   adjoint of the taps through the pyramid (the backward folds it in with 2 (L-1) gather launches and
+ *   no atomics); every other gradient keeps its form.  Deterministic mode accumulates every level in
+ *   fixed point: det_work needs r3dg_shade_filtered_det_bytes(env_h, env_w) bytes.
+ *   Composition: one view and several views (the filtered light is evaluated once per sample for all
+ *   views, per view with per-view transforms), both light kinds, every r3dg_tune shading variant
+ *   (same forward bits), the per-sample outputs (they hold the filtered light).
+ *   Cost: the pyramid is ~4/3 of the env; the backward workspace as much again.  The env-gradient
+ *   mode is picked from the texel count of all levels (a 16x32 env stays in shared memory).
+ * r3dg_env_pyramid_levels / _floats: L, and the floats of all levels (0 for a size <= 0).
+ * r3dg_env_pyramid_build: pyramid = every level of env, level after level (L - 1 launches and one
+ * copy); fixed order, no atomics (bitwise reproducible), no host synchronisation.  A NULL pointer or a
+ * size <= 0 returns R3DG_ERR_BAD_ARG before anything is launched.
+ * ------------------------------------------------------------------------------------------ */
+int r3dg_env_pyramid_levels(int env_h, int env_w);
+size_t r3dg_env_pyramid_floats(int env_h, int env_w);
+int r3dg_env_pyramid_build(const float* env, int env_h, int env_w, float* pyramid, r3dg_stream_t stream);
+size_t r3dg_shade_filtered_det_bytes(int env_h, int env_w);
 
 /* ------------------------------------------------------------------------------------------
  * DETERMINISTIC MODE.  With `deterministic` set in r3dg_raster_fwd_args, r3dg_raster_bwd_args or

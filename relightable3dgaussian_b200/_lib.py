@@ -71,7 +71,7 @@ class ShadeArgs(ctypes.Structure):
                                  "incident_lights", "local_incident_lights", "global_incident_lights",
                                  "dL_dpbr", "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color",
                                  "dL_droughness", "dL_dviewdirs", "dL_dincidents", "dL_denv")] +
-        [("V", c_int), ("transform_per_view", c_int)] +
+        [("V", c_int), ("transform_per_view", c_int), ("env_pyramid", c_void_p), ("dL_denv_pyramid", c_void_p)] +
         [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
@@ -162,6 +162,10 @@ SYMBOLS = [
     ("r3dg_unpremultiply_backward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_render_equation_forward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),
     ("r3dg_render_equation_backward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),
+    ("r3dg_env_pyramid_levels", c_int, [c_int, c_int]),
+    ("r3dg_env_pyramid_floats", c_size_t, [c_int, c_int]),
+    ("r3dg_env_pyramid_build", c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    ("r3dg_shade_filtered_det_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_pack_features_forward", c_int, [c_int, c_int, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p, c_void_p]),
     ("r3dg_pack_features_backward", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p,
                                             c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -23,6 +23,7 @@
 #include <type_traits>
 #include "common.cuh"
 #include "detacc.cuh"
+#include "envfilter.cuh"
 #include "kernels.h"
 
 namespace r3dg {
@@ -57,9 +58,41 @@ __device__ __forceinline__ void sh_basis3(float x, float y, float z, float* w) {
     w[15] = -0.5900435899266435f * x * (xx - 3.f * yy);
 }
 
-struct EnvTap { int idx[4]; float w[4]; };      // texel base offsets (float index of channel 0, or -1) + weights
+template <int K> struct EnvTaps { int idx[K]; float w[K]; };   // texel base offsets (float index of channel 0, or -1) + weights
+using EnvTap = EnvTaps<4>;
 
-// grid_sample(bilinear, zeros padding, align_corners=True) at the lat-long coordinates of dir d
+// the filtered mode's grid_sample coordinates of dir d in [0, 1]: u along the columns, v along the rows
+__device__ __forceinline__ void env_uv(float dx, float dy, float dz, float& u, float& v) {
+    const float phi = acosf(dz) - 1e-6f;
+    const float theta = atan2f(dy, dx);
+    const float qy = (phi / PI_F) * 2.0f - 1.0f;
+    const float qx = -theta / PI_F;
+    u = (qx + 1.0f) / 2.0f;
+    v = (qy + 1.0f) / 2.0f;
+}
+
+// the four bilinear taps of (u, v) on an He x We texture, into taps B .. B+3 of t
+template <int B, int K>
+__device__ __forceinline__ void fill_taps(float u, float v, int He, int We, EnvTaps<K>& t) {
+    const float ix = u * (float)(We - 1);
+    const float iy = v * (float)(He - 1);
+    const float fx = floorf(ix), fy = floorf(iy);
+    const int x0 = (int)fx, y0 = (int)fy;
+    const float ax = ix - fx, ay = iy - fy;        // == ix - ix_nw ; (ix_se - ix) == 1 - ax
+    const int xs[2] = {x0, x0 + 1}, ys[2] = {y0, y0 + 1};
+    const float wx[2] = {(fx + 1.0f) - ix, ax}, wy[2] = {(fy + 1.0f) - iy, ay};
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const bool in = xs[i] >= 0 && xs[i] < We && ys[j] >= 0 && ys[j] < He;
+            t.idx[B + 2 * j + i] = in ? (ys[j] * We + xs[i]) * 3 : -1;
+            t.w[B + 2 * j + i] = wx[i] * wy[j];
+        }
+}
+
+// grid_sample(bilinear, zeros padding, align_corners=True) at the lat-long coordinates of dir d (the point lookup; the
+// filtered mode's taps below repeat its arithmetic through env_uv and fill_taps)
 __device__ __forceinline__ EnvTap env_taps(float dx, float dy, float dz, int He, int We) {
     const float phi = acosf(dz) - 1e-6f;
     const float theta = atan2f(dy, dx);
@@ -81,6 +114,33 @@ __device__ __forceinline__ EnvTap env_taps(float dx, float dy, float dz, int He,
             t.idx[2 * j + i] = in ? (ys[j] * We + xs[i]) * 3 : -1;
             t.w[2 * j + i] = wx[i] * wy[j];
         }
+    return t;
+}
+
+// The filtered lookup (include/r3dg_b200.h, "PREFILTERED ENVIRONMENT"): the trilinear taps of d on the pyramid `lv`
+// for a sample of solid angle omega.  lambda = log2(omega / Omega0(theta)) / 2, clamped to [0, L-1], is evaluated in
+// fp32; at lambda <= 0 the taps are env_taps' four, weights and order unchanged (the upper four are absent).
+__device__ __forceinline__ EnvTaps<8> env_taps_filtered(float dx, float dy, float dz, const EnvLevels& lv, float omega) {
+    float u, v;
+    env_uv(dx, dy, dz, u, v);
+    const float st = sqrtf(fmaxf(1.0f - dz * dz, 0.0f));
+    const float lam = fminf(fmaxf(0.5f * log2f(omega / (lv.dtdp * fmaxf(st, lv.sin_half))), 0.0f), (float)(lv.L - 1));
+    const int l0 = (int)lam;
+    const float f = lam - (float)l0;
+    EnvTaps<8> t;
+    fill_taps<0>(u, v, lv.h[l0], lv.w[l0], t);
+    const int o0 = 3 * lv.off[l0];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { if (t.idx[q] >= 0) t.idx[q] += o0; t.w[q] *= 1.0f - f; }
+    if (f > 0.0f) {
+        fill_taps<4>(u, v, lv.h[l0 + 1], lv.w[l0 + 1], t);
+        const int o1 = 3 * lv.off[l0 + 1];
+#pragma unroll
+        for (int q = 4; q < 8; ++q) { if (t.idx[q] >= 0) t.idx[q] += o1; t.w[q] *= f; }
+    } else {
+#pragma unroll
+        for (int q = 4; q < 8; ++q) { t.idx[q] = -1; t.w[q] = 0.0f; }
+    }
     return t;
 }
 
@@ -151,13 +211,15 @@ __device__ __forceinline__ float fast_rcp(float x) {
 }
 #define INV_PI_F 0.318309873342514038f    // float32(1 / float32(np.pi))
 
-struct SampleEval {       // forward quantities of one (Gaussian, direction) pair
+template <bool FILT = false>
+struct SampleEvalT {      // forward quantities of one (Gaussian, direction) pair; FILT: the filtered mode's 8 env taps
     float local_raw[3], glob[3], ndi, fs;
     float w[16];
-    EnvTap taps;
+    EnvTaps<FILT ? 8 : 4> taps;
     // GGX intermediates for the backward
     float H[3], hn, NoL, NoV, NoH, VoH, NoL_r, NoV_r, NoH_r, VoH_r, p2, frac0, nom0, nom1, nom2, nom_r, nom;
 };
+using SampleEval = SampleEvalT<false>;
 
 // Each sample's evaluation comes in three parts, so that the view kernels can run the first two once for all views:
 // the environment light (depends on the env transform), the local SH light and n.w (depend on the Gaussian only),
@@ -182,10 +244,34 @@ __device__ __forceinline__ void eval_env(const float* T, const float* __restrict
     }
 }
 
+// the filtered mode's global light: env is the pyramid, omega the sample's solid angle
+template <bool SMEM_ENV>
+__device__ __forceinline__ void eval_env_filtered(const float* T, const float* __restrict__ env, const EnvLevels& lv, float omega,
+                                                  float dx, float dy, float dz, float vis, SampleEvalT<true>& e) {
+    float ex = dx, ey = dy, ez = dz;
+    if (T) { ex = 0.f + dx * T[0] + dy * T[1] + dz * T[2]; ey = 0.f + dx * T[3] + dy * T[4] + dz * T[5]; ez = 0.f + dx * T[6] + dy * T[7] + dz * T[8]; }
+    e.taps = env_taps_filtered(ex, ey, ez, lv, omega);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        float s = 0.f;
+#pragma unroll
+        for (int t = 0; t < 8; ++t) if (e.taps.idx[t] >= 0) s += (SMEM_ENV ? env[e.taps.idx[t] + c] : __ldg(env + e.taps.idx[t] + c)) * e.taps.w[t];
+        e.glob[c] = s * vis;
+    }
+}
+
+// the global light of either mode (omega = area / N: read by the filtered mode only)
+template <bool SMEM_ENV, bool FILT>
+__device__ __forceinline__ void eval_env_any(const float* T, const float* __restrict__ env, const ShadeArgs& a, const EnvLevels& lv,
+                                             float omega, float dx, float dy, float dz, float vis, SampleEvalT<FILT>& e) {
+    if constexpr (FILT) eval_env_filtered<SMEM_ENV>(T, env, lv, omega, dx, dy, dz, vis, e);
+    else eval_env<SMEM_ENV>(T, env, a.He, a.We, dx, dy, dz, vis, e);
+}
+
 // the local SH light (before its clamp) and n.w with the raw normal
-template <bool INC_SMEM>
+template <bool INC_SMEM, class E>
 __device__ __forceinline__ void eval_local(const GaussianOperands& o, const float* __restrict__ sinc, float dx, float dy, float dz,
-                                           SampleEval& e) {
+                                           E& e) {
     sh_basis3(dx, dy, dz, e.w);
     if (INC_SMEM) {
         float acc[3] = {0.f, 0.f, 0.f};
@@ -212,9 +298,9 @@ __device__ __forceinline__ void eval_local(const GaussianOperands& o, const floa
 
 // GGX_specular (neilf.py:374-406) for the view V with the flipped normal Ns (o: alpha^2 and k)
 // FAST: one-MUFU reciprocals (the backward kernels); the forward keeps IEEE divisions
-template <bool FAST>
+template <bool FAST, class E>
 __device__ __forceinline__ void eval_ggx(const float* V, const float* Ns, const GaussianOperands& o, float dx, float dy, float dz,
-                                         SampleEval& e) {
+                                         E& e) {
     const float ln = fmaxf(sqrtf(dx * dx + dy * dy + dz * dz), 1e-12f);
     float L0, L1, L2;
     if (FAST) { const float il = fast_rcp(ln); L0 = dx * il; L1 = dy * il; L2 = dz * il; }
@@ -240,10 +326,11 @@ __device__ __forceinline__ void eval_ggx(const float* V, const float* Ns, const 
     e.fs = FAST ? e.frac0 * o.a2 * fast_rcp(e.nom) : e.frac0 * o.a2 / e.nom;
 }
 
-template <bool SMEM_ENV, bool INC_SMEM, bool FAST = false>
-__device__ __forceinline__ void eval_sample(const ShadeArgs& a, const GaussianOperands& o, const float* __restrict__ env,
-                                            const float* __restrict__ sinc, float dx, float dy, float dz, float vis, SampleEval& e) {
-    eval_env<SMEM_ENV>(a.transform, env, a.He, a.We, dx, dy, dz, vis, e);
+template <bool SMEM_ENV, bool INC_SMEM, bool FAST, bool FILT>
+__device__ __forceinline__ void eval_sample(const ShadeArgs& a, const EnvLevels& lv, const GaussianOperands& o, const float* __restrict__ env,
+                                            const float* __restrict__ sinc, float dx, float dy, float dz, float vis, float omega,
+                                            SampleEvalT<FILT>& e) {
+    eval_env_any<SMEM_ENV>(a.transform, env, a, lv, omega, dx, dy, dz, vis, e);
     eval_local<INC_SMEM>(o, sinc, dx, dy, dz, e);
     eval_ggx<FAST>(o.V, o.Ns, o, dx, dy, dz, e);
 }
@@ -283,8 +370,8 @@ __device__ __forceinline__ void group_reduce_scatter(float (&v)[V], int sub) {
     }
 }
 
-template <bool SMEM_ENV, int G, int VAR>
-__global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? 6 : 1) shade_fwd_kernel(const ShadeArgs a) {
+template <bool SMEM_ENV, int G, int VAR, bool FILT>
+__global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? (FILT ? 5 : 6) : 1) shade_fwd_kernel(const ShadeArgs a, const EnvLevels lv) {
     extern __shared__ __align__(16) float s_fwd[];     // [incident slots (VAR 1)][env texture (SMEM_ENV)]
     constexpr int GPW = 32 / G;                    // Gaussians per warp
     constexpr int INC_FLOATS = VAR >= 1 ? SHADE_WARPS * GPW * SHADE_INC_STRIDE : 0;
@@ -293,7 +380,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? 6 : 1) shade_fwd_ker
     const int sub = lane & (G - 1), grp = lane / G;
     float* sinc = s_fwd + (warp * GPW + grp) * SHADE_INC_STRIDE;
     if (SMEM_ENV) {
-        for (int i = threadIdx.x; i < a.He * a.We * 3; i += SHADE_THREADS) s_env[i] = a.env[i];
+        for (int i = threadIdx.x; i < (FILT ? lv.total : a.He * a.We) * 3; i += SHADE_THREADS) s_env[i] = a.env[i];
         __syncthreads();
     }
     const float* env = SMEM_ENV ? s_env : a.env;
@@ -311,8 +398,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 1 ? 6 : 1) shade_fwd_ker
         for (int i = sub; i < a.N; i += G) {
             const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
             const float vis = a.visibility[row + i], area = a.areas[row + i];
-            SampleEval e;
-            eval_sample<SMEM_ENV, (VAR >= 1)>(a, o, env, sinc, dx, dy, dz, vis, e);
+            SampleEvalT<FILT> e;
+            eval_sample<SMEM_ENV, (VAR >= 1), false>(a, lv, o, env, sinc, dx, dy, dz, vis, area * invN, e);
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
                 const float loc = fmaxf(e.local_raw[c], 0.f);
@@ -388,19 +475,20 @@ struct EnvGrad {
     const float* env;                                // the texture the samples read (shared or global memory)
     float* genv;                                     // ENV_CAS / ENV_GLOBAL: where the taps are added
 
-    // bytes of `s_mem` the constructor lays out for an He x We texture (0 for the global-memory modes):
+    // bytes of `s_mem` the constructor lays out for a texture of nt texels (0 for the global-memory modes):
     // ENV_CAS: [env ne][grad ne]; ENV_TAG: [env ne (padded to 4)][per warp: float4 grad[nt]][per warp: tag[nt] padded to 16];
     // ENV_DET_SMEM: [env ne (padded to 2)][accumulator words 3 ne][flag words (ne + 15) / 16]
-    static __host__ __device__ size_t smem_bytes(int He, int We) {
-        const size_t nt = (size_t)He * We, ne = nt * 3;
+    static __host__ __device__ size_t smem_bytes(size_t nt) {
+        const size_t ne = nt * 3;
         if (ENV_MODE == ENV_CAS) return 2 * ne * sizeof(float);
         if (ENV_MODE == ENV_TAG) return ((ne + 3) & ~(size_t)3) * sizeof(float) + SHADE_WARPS * (nt * sizeof(float4) + ((nt + 15) & ~(size_t)15));
         if (ENV_MODE == ENV_DET_SMEM) return ((ne + 1) & ~(size_t)1) * sizeof(float) + 3 * ne * sizeof(uint64_t) + (ne + 15) / 16 * sizeof(uint32_t);
         return 0;
     }
 
-    __device__ __forceinline__ EnvGrad(const ShadeArgs& a, float* s_mem, int warp) {
-        nt = a.He * a.We; ne = nt * 3;
+    // texels: of the texture the samples read (He * We, or every level of the filtered mode's pyramid)
+    __device__ __forceinline__ EnvGrad(const ShadeArgs& a, float* s_mem, int warp, int texels) {
+        nt = texels; ne = nt * 3;
         s_env = s_mem;
         s_genv = s_mem + ne;
         const int ne4 = (ne + 3) & ~3, ntp = (nt + 15) & ~15;
@@ -426,11 +514,12 @@ struct EnvGrad {
     }
 
     // dG: the sample's light cotangent times its visibility (zero for an inactive lane); called by every lane of the warp
-    __device__ __forceinline__ void scatter(const ShadeArgs& a, const EnvTap& taps, const float* dG, int lane) {
+    template <int K>
+    __device__ __forceinline__ void scatter(const ShadeArgs& a, const EnvTaps<K>& taps, const float* dG, int lane) {
         if (ENV_MODE == ENV_TAG) {
             const bool any = dG[0] != 0.f || dG[1] != 0.f || dG[2] != 0.f;
 #pragma unroll
-            for (int t = 0; t < 4; ++t) {
+            for (int t = 0; t < K; ++t) {
                 const int texel = (any && taps.idx[t] >= 0) ? taps.idx[t] / 3 : -1;
                 warp_private_add(wgrad, wtag, texel, dG[0] * taps.w[t], dG[1] * taps.w[t], dG[2] * taps.w[t], lane);
             }
@@ -439,7 +528,7 @@ struct EnvGrad {
             for (int c = 0; c < 3; ++c)
                 if (dG[c] != 0.f) {
 #pragma unroll
-                    for (int t = 0; t < 4; ++t)
+                    for (int t = 0; t < K; ++t)
                         if (taps.idx[t] >= 0) {
                             if (ENV_MODE == ENV_DET_SMEM) det_add(s_dwords, s_dflags, ne, taps.idx[t] + c, dG[c] * taps.w[t], det_e, true);
                             else det_add(a.det, taps.idx[t] + c, dG[c] * taps.w[t], det_e);
@@ -450,7 +539,7 @@ struct EnvGrad {
             for (int c = 0; c < 3; ++c)
                 if (dG[c] != 0.f) {
 #pragma unroll
-                    for (int t = 0; t < 4; ++t) if (taps.idx[t] >= 0) atomicAdd(genv + taps.idx[t] + c, dG[c] * taps.w[t]);
+                    for (int t = 0; t < K; ++t) if (taps.idx[t] >= 0) atomicAdd(genv + taps.idx[t] + c, dG[c] * taps.w[t]);
                 }
         }
     }
@@ -497,7 +586,8 @@ __device__ __forceinline__ void accumulate_dinc(float4* acc4, const float* dLg, 
 }
 
 // GGX_specular backward for the view V (flipped normal Ns) from dfs = dL/dfs: adds to drough and to dV = dL/dV
-__device__ __forceinline__ void ggx_backward(const float* V, const float* Ns, const GaussianOperands& o, const SampleEval& e,
+template <class E>
+__device__ __forceinline__ void ggx_backward(const float* V, const float* Ns, const GaussianOperands& o, const E& e,
                                              float dfs, float& drough, float (&dV)[3]) {
     const float inom = fast_rcp(e.nom);
     const float dfrac = dfs * inom;
@@ -528,9 +618,11 @@ __device__ __forceinline__ void ggx_backward(const float* V, const float* Ns, co
 
 // resident CTAs the register allocation is pinned to: variant 1 -> 3 (<= 168 registers); variant 2 ->
 // 3 with the warp-private env copies (67 KB of shared memory per CTA) or the deterministic modes (their fixed-point
-// conversion spills at 102 registers), 5 otherwise (<= 102 registers)
-template <int ENV_MODE, int G, int VAR>
-__global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (ENV_MODE <= 1 ? 5 : 3)) shade_bwd_kernel(const ShadeArgs a) {
+// conversion spills at 102 registers), 5 otherwise (<= 102 registers; 4 in the filtered mode, whose 8 env taps spill
+// at 102)
+template <int ENV_MODE, int G, int VAR, bool FILT>
+__global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (ENV_MODE <= 1 ? (FILT ? 4 : 5) : 3))
+shade_bwd_kernel(const ShadeArgs a, const EnvLevels lv) {
     extern __shared__ __align__(16) float s_bwd[];    // [incident slots (VAR >= 1)][gradient accumulators (VAR 2)][env ...]
     constexpr bool SMEM_ENV = EnvGrad<ENV_MODE>::SMEM_ENV;
     constexpr int GPW = 32 / G;
@@ -543,7 +635,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
     constexpr int RQ = VP / G;                       // finished components per lane
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane & (G - 1), grp = lane / G;
-    EnvGrad<ENV_MODE> eg(a, s_mem, warp);
+    EnvGrad<ENV_MODE> eg(a, s_mem, warp, FILT ? lv.total : a.He * a.We);
     const float invN = 1.0f / (float)a.N;
     const int units = (a.P + GPW - 1) / GPW;
     for (int u = blockIdx.x * SHADE_WARPS + warp; u < units; u += gridDim.x * SHADE_WARPS) {
@@ -574,8 +666,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, VAR == 0 ? 1 : VAR == 1 ? 3 : (
             const int i = (i0 + sub) < a.N ? (i0 + sub) : a.N - 1;
             const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
             const float vis = a.visibility[row + i], area = a.areas[row + i];
-            SampleEval e;
-            eval_sample<SMEM_ENV, (VAR >= 1), true>(a, o, eg.env, sinc, dx, dy, dz, vis, e);
+            SampleEvalT<FILT> e;
+            eval_sample<SMEM_ENV, (VAR >= 1), true>(a, lv, o, eg.env, sinc, dx, dy, dz, vis, area * invN, e);
             float dfs = 0.f;
             float dG[3], dLg[3];
 #pragma unroll
@@ -672,8 +764,8 @@ struct ViewChunk {
 // per-lane partial sums of one view in the forward: pbr, specular, diffuse (+ mean lights, mean global with per-view transforms)
 __host__ __device__ inline int view_fwd_sums(bool per_view_means) { return per_view_means ? 15 : 9; }
 
-template <bool SMEM_ENV>
-__global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const ShadeArgs a, const ViewChunk vc) {
+template <bool SMEM_ENV, bool FILT>
+__global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const ShadeArgs a, const ViewChunk vc, const EnvLevels lv) {
     constexpr int G = 8, GPW = 32 / G;
     constexpr int INC_FLOATS = SHADE_WARPS * GPW * SHADE_INC_STRIDE;
     constexpr int SLOT_FLOATS = SHADE_WARPS * GPW * SHADE_VIEW_CHUNK * VIEW_FWD_SLOT;
@@ -687,7 +779,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const
     float* sinc = s_vfwd + (warp * GPW + grp) * SHADE_INC_STRIDE;
     float* slot = s_vfwd + INC_FLOATS + (warp * GPW + grp) * SHADE_VIEW_CHUNK * VIEW_FWD_SLOT;
     if (SMEM_ENV) {
-        for (int i = threadIdx.x; i < a.He * a.We * 3; i += SHADE_THREADS) s_env[i] = a.env[i];
+        for (int i = threadIdx.x; i < (FILT ? lv.total : a.He * a.We) * 3; i += SHADE_THREADS) s_env[i] = a.env[i];
         __syncthreads();
     }
     const float* env = SMEM_ENV ? s_env : a.env;
@@ -712,8 +804,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const
         for (int i = sub; i < a.N; i += G) {
             const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
             const float vis = a.visibility[row + i], area = a.areas[row + i];
-            SampleEval e;
-            if (!pvt) eval_env<SMEM_ENV>(a.transform, env, a.He, a.We, dx, dy, dz, vis, e);
+            SampleEvalT<FILT> e;
+            if (!pvt) eval_env_any<SMEM_ENV>(a.transform, env, a, lv, area * invN, dx, dy, dz, vis, e);
             eval_local<true>(o, sinc, dx, dy, dz, e);
             float loc[3];
 #pragma unroll
@@ -725,7 +817,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const
             mv += vis;
             for (int v = 0; v < vc.nv; ++v) {
                 const float* vs = slot + v * VIEW_FWD_SLOT;
-                if (pvt) eval_env<SMEM_ENV>(a.transform + 9 * (size_t)(vc.v0 + v), env, a.He, a.We, dx, dy, dz, vis, e);
+                if (pvt) eval_env_any<SMEM_ENV>(a.transform + 9 * (size_t)(vc.v0 + v), env, a, lv, area * invN, dx, dy, dz, vis, e);
                 eval_ggx<false>(vs, vs + 3, o, dx, dy, dz, e);
                 float* acc = s_acc + v * K * SHADE_THREADS + threadIdx.x;
 #pragma unroll
@@ -772,8 +864,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_fwd_kernel(const
 // loop sums dT = sum_v dL/dT_v; the SH-gradient contraction and the env scatter then run once on that sum, and dL/dbase
 // uses the summed dL/dpbr.  dL/dviewdirs stays per view.  `accumulate` adds the leaf gradients to those of the earlier
 // launches, in launch order (a fixed fold, so the deterministic mode stays reproducible).
-template <int ENV_MODE>
-__global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_bwd_kernel(const ShadeArgs a, const ViewChunk vc) {
+template <int ENV_MODE, bool FILT>
+__global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_bwd_kernel(const ShadeArgs a, const ViewChunk vc, const EnvLevels lv) {
     constexpr bool SMEM_ENV = EnvGrad<ENV_MODE>::SMEM_ENV;
     constexpr int G = 8, GPW = 32 / G, RQ = 48 / G;
     constexpr int INC_FLOATS = SHADE_WARPS * GPW * SHADE_INC_STRIDE;
@@ -788,7 +880,7 @@ __global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_bwd_kernel(const
     float4* acc4 = reinterpret_cast<float4*>(s_vbwd + INC_FLOATS) + threadIdx.x;
     float* slot = s_vbwd + INC_FLOATS + DINC_FLOATS + (warp * GPW + grp) * SHADE_VIEW_CHUNK * VIEW_BWD_SLOT;
     float* s_dv = s_vbwd + INC_FLOATS + DINC_FLOATS + SLOT_FLOATS + threadIdx.x;
-    EnvGrad<ENV_MODE> eg(a, s_vbwd + INC_FLOATS + DINC_FLOATS + SLOT_FLOATS + DV_FLOATS, warp);
+    EnvGrad<ENV_MODE> eg(a, s_vbwd + INC_FLOATS + DINC_FLOATS + SLOT_FLOATS + DV_FLOATS, warp, FILT ? lv.total : a.He * a.We);
     const float invN = 1.0f / (float)a.N;
     const int units = (a.P + GPW - 1) / GPW;
     for (int u = blockIdx.x * SHADE_WARPS + warp; u < units; u += gridDim.x * SHADE_WARPS) {
@@ -824,8 +916,8 @@ __global__ void __launch_bounds__(SHADE_THREADS, 3) shade_views_bwd_kernel(const
             const int i = (i0 + sub) < a.N ? (i0 + sub) : a.N - 1;
             const float dx = a.dirs[3 * (row + i)], dy = a.dirs[3 * (row + i) + 1], dz = a.dirs[3 * (row + i) + 2];
             const float vis = a.visibility[row + i], area = a.areas[row + i];
-            SampleEval e;
-            eval_env<SMEM_ENV>(a.transform, eg.env, a.He, a.We, dx, dy, dz, vis, e);
+            SampleEvalT<FILT> e;
+            eval_env_any<SMEM_ENV>(a.transform, eg.env, a, lv, area * invN, dx, dy, dz, vis, e);
             eval_local<true>(o, sinc, dx, dy, dz, e);
             float T[3], dT[3] = {0, 0, 0};
 #pragma unroll
@@ -942,47 +1034,51 @@ static int shade_launch(K kernel, const ShadeArgs& a, int units, int num_sms, si
 
 static size_t inc_slot_bytes(int G, int var) { return var >= 1 ? (size_t)SHADE_WARPS * (32 / G) * SHADE_INC_STRIDE * sizeof(float) : 0; }
 
-template <bool SMEM>
-static int launch_fwd(const ShadeArgs& a, int num_sms, size_t env_smem, cudaStream_t stream) {
+template <bool SMEM, bool FILT>
+static int launch_fwd(const ShadeArgs& a, const EnvLevels& lv, int num_sms, size_t env_smem, cudaStream_t stream) {
     const int G = knob(0);
     const int var = G == 8 ? knob(2) : 0;              // the shared-memory variants are built for the default group width
     const size_t smem = env_smem + inc_slot_bytes(G, var);
     const int units = (a.P + 32 / G - 1) / (32 / G);
-    if (G == 8) return var ? shade_launch(shade_fwd_kernel<SMEM, 8, 1>, a, units, num_sms, smem, stream)
-                           : shade_launch(shade_fwd_kernel<SMEM, 8, 0>, a, units, num_sms, smem, stream);
-    if (G == 16) return shade_launch(shade_fwd_kernel<SMEM, 16, 0>, a, units, num_sms, smem, stream);
-    return shade_launch(shade_fwd_kernel<SMEM, 32, 0>, a, units, num_sms, smem, stream);
+    if (G == 8) return var ? shade_launch(shade_fwd_kernel<SMEM, 8, 1, FILT>, a, units, num_sms, smem, stream, lv)
+                           : shade_launch(shade_fwd_kernel<SMEM, 8, 0, FILT>, a, units, num_sms, smem, stream, lv);
+    if (G == 16) return shade_launch(shade_fwd_kernel<SMEM, 16, 0, FILT>, a, units, num_sms, smem, stream, lv);
+    return shade_launch(shade_fwd_kernel<SMEM, 32, 0, FILT>, a, units, num_sms, smem, stream, lv);
 }
 
-int launch_shade_forward(ShadeArgs a, int num_sms, cudaStream_t stream) {
+// texels of the texture the kernels read: the env, or every level of the filtered mode's pyramid
+static size_t env_texels(const ShadeArgs& a, const EnvLevels& lv, bool filt) { return filt ? (size_t)lv.total : (size_t)a.He * a.We; }
+
+int launch_shade_forward(ShadeArgs a, const EnvLevels& lv, bool filt, int num_sms, cudaStream_t stream) {
     if (a.P <= 0) return 0;
-    const size_t env_bytes = (size_t)a.He * a.We * 3 * sizeof(float);
+    const size_t env_bytes = env_texels(a, lv, filt) * 3 * sizeof(float);
     const bool smem = env_bytes <= 40 * 1024;
     a.env_in_smem = smem;
-    return smem ? launch_fwd<true>(a, num_sms, env_bytes, stream) : launch_fwd<false>(a, num_sms, 0, stream);
+    if (filt) return smem ? launch_fwd<true, true>(a, lv, num_sms, env_bytes, stream) : launch_fwd<false, true>(a, lv, num_sms, 0, stream);
+    return smem ? launch_fwd<true, false>(a, lv, num_sms, env_bytes, stream) : launch_fwd<false, false>(a, lv, num_sms, 0, stream);
 }
 
-template <int MODE>
-static int launch_bwd(const ShadeArgs& a, int num_sms, size_t env_smem, cudaStream_t stream) {
+template <int MODE, bool FILT>
+static int launch_bwd(const ShadeArgs& a, const EnvLevels& lv, int num_sms, size_t env_smem, cudaStream_t stream) {
     const int G = knob(0);
     const int var = G == 8 ? knob(3) : 0;
     const size_t smem = env_smem + inc_slot_bytes(G, var) + (var == 2 ? (size_t)48 * SHADE_THREADS * sizeof(float) : 0);
     const int units = (a.P + 32 / G - 1) / (32 / G);
-    if (G == 8) return var == 2 ? shade_launch(shade_bwd_kernel<MODE, 8, 2>, a, units, num_sms, smem, stream)
-                     : var == 1 ? shade_launch(shade_bwd_kernel<MODE, 8, 1>, a, units, num_sms, smem, stream)
-                                : shade_launch(shade_bwd_kernel<MODE, 8, 0>, a, units, num_sms, smem, stream);
-    if (G == 16) return shade_launch(shade_bwd_kernel<MODE, 16, 0>, a, units, num_sms, smem, stream);
-    return shade_launch(shade_bwd_kernel<MODE, 32, 0>, a, units, num_sms, smem, stream);
+    if (G == 8) return var == 2 ? shade_launch(shade_bwd_kernel<MODE, 8, 2, FILT>, a, units, num_sms, smem, stream, lv)
+                     : var == 1 ? shade_launch(shade_bwd_kernel<MODE, 8, 1, FILT>, a, units, num_sms, smem, stream, lv)
+                                : shade_launch(shade_bwd_kernel<MODE, 8, 0, FILT>, a, units, num_sms, smem, stream, lv);
+    if (G == 16) return shade_launch(shade_bwd_kernel<MODE, 16, 0, FILT>, a, units, num_sms, smem, stream, lv);
+    return shade_launch(shade_bwd_kernel<MODE, 32, 0, FILT>, a, units, num_sms, smem, stream, lv);
 }
 
 template <int M> using EnvMode = std::integral_constant<int, M>;
 
-// Clears dL/denv (or the deterministic accumulators), picks the env-gradient mode from the texture size, the deterministic
-// flag and the highest mode allowed (`cap`), and calls run(EnvMode<mode>, args, env shared-memory bytes) unless P = 0;
-// the deterministic mode first reduces the scale of the V views' cotangents and then converts its accumulators into
-// dL/denv.
+// Clears dL/denv (or the deterministic accumulators), picks the env-gradient mode from the texture size (nt texels),
+// the deterministic flag and the highest mode allowed (`cap`), and calls run(EnvMode<mode>, args, env shared-memory
+// bytes) unless P = 0; the deterministic mode first reduces the scale of the V views' cotangents and then converts its
+// accumulators into dL/denv.
 template <typename Run>
-static int shade_backward(ShadeArgs a, int V, int cap, int num_sms, cudaStream_t stream, Run run) {
+static int shade_backward(ShadeArgs a, int V, int cap, size_t nt, int num_sms, cudaStream_t stream, Run run) {
     if (a.det.words) {
         R3DG_CUDA_TRY(cudaMemsetAsync(a.det.words, 0, det_bytes(a.det.n) + sizeof(uint32_t), stream));   // + the scale word
         int rc = 0;
@@ -990,7 +1086,7 @@ static int shade_backward(ShadeArgs a, int V, int cap, int num_sms, cudaStream_t
             const size_t n = (size_t)(V < 1 ? 1 : V) * a.P * 3;
             const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)4 * num_sms);
             det_scale_kernel<<<blocks, 256, 0, stream>>>(n, a.g_pbr, a.g_diffuse, a.g_specular, a.det_scale);
-            const size_t smem = EnvGrad<ENV_DET_SMEM>::smem_bytes(a.He, a.We);     // larger textures use ENV_DET_GLOBAL
+            const size_t smem = EnvGrad<ENV_DET_SMEM>::smem_bytes(nt);     // larger textures use ENV_DET_GLOBAL
             a.env_in_smem = smem <= 64 * 1024;
             rc = a.env_in_smem ? run(EnvMode<ENV_DET_SMEM>(), a, smem) : run(EnvMode<ENV_DET_GLOBAL>(), a, 0);
         }
@@ -999,28 +1095,30 @@ static int shade_backward(ShadeArgs a, int V, int cap, int num_sms, cudaStream_t
         R3DG_CUDA_TRY(cudaGetLastError());
         return 0;
     }
-    R3DG_CUDA_TRY(cudaMemsetAsync(a.d_env, 0, (size_t)a.He * a.We * 3 * sizeof(float), stream));
+    R3DG_CUDA_TRY(cudaMemsetAsync(a.d_env, 0, nt * 3 * sizeof(float), stream));
     if (a.P <= 0) return 0;
     // shared-memory cost of the env-gradient modes (kept within the 48 KB that need no opt-in on their own)
-    const size_t tag_bytes = EnvGrad<ENV_TAG>::smem_bytes(a.He, a.We), cas_bytes = EnvGrad<ENV_CAS>::smem_bytes(a.He, a.We);
+    const size_t tag_bytes = EnvGrad<ENV_TAG>::smem_bytes(nt), cas_bytes = EnvGrad<ENV_CAS>::smem_bytes(nt);
     if (cap >= ENV_TAG && tag_bytes <= 48 * 1024) { a.env_in_smem = 1; return run(EnvMode<ENV_TAG>(), a, tag_bytes); }
     if (cap >= ENV_CAS && cas_bytes <= 40 * 1024) { a.env_in_smem = 1; return run(EnvMode<ENV_CAS>(), a, cas_bytes); }
     a.env_in_smem = 0;
     return run(EnvMode<ENV_GLOBAL>(), a, 0);
 }
 
-int launch_shade_backward(ShadeArgs a, int num_sms, cudaStream_t stream) {
-    return shade_backward(a, 1, knob(1), num_sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
-        return launch_bwd<decltype(mode)::value>(x, num_sms, env_smem, stream);
+int launch_shade_backward(ShadeArgs a, const EnvLevels& lv, bool filt, int num_sms, cudaStream_t stream) {
+    return shade_backward(a, 1, knob(1), env_texels(a, lv, filt), num_sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
+        constexpr int M = decltype(mode)::value;
+        return filt ? launch_bwd<M, true>(x, lv, num_sms, env_smem, stream) : launch_bwd<M, false>(x, lv, num_sms, env_smem, stream);
     });
 }
 
 // ---- several views: one launch per SHADE_VIEW_CHUNK views ------------------------------------------
 static size_t view_slot_bytes(int slot_floats) { return (size_t)SHADE_WARPS * 4 * SHADE_VIEW_CHUNK * slot_floats * sizeof(float); }
 
-int launch_shade_views_forward(ShadeArgs a, int V, int per_view_transform, int num_sms, cudaStream_t stream) {
+int launch_shade_views_forward(ShadeArgs a, const EnvLevels& lv, bool filt, int V, int per_view_transform, int num_sms,
+                               cudaStream_t stream) {
     if (a.P <= 0) return 0;
-    const size_t env_bytes = (size_t)a.He * a.We * 3 * sizeof(float);
+    const size_t env_bytes = env_texels(a, lv, filt) * 3 * sizeof(float);
     const bool smem_env = env_bytes <= 40 * 1024;     // as the one-view forward
     a.env_in_smem = smem_env;
     const int K = view_fwd_sums(per_view_transform && a.mean_lights);
@@ -1029,16 +1127,18 @@ int launch_shade_views_forward(ShadeArgs a, int V, int per_view_transform, int n
     const int units = (a.P + 3) / 4;
     for (int v0 = 0; v0 < V; v0 += SHADE_VIEW_CHUNK) {
         const ViewChunk vc{v0, V - v0 < SHADE_VIEW_CHUNK ? V - v0 : SHADE_VIEW_CHUNK, per_view_transform, 0};
-        const int rc = smem_env ? shade_launch(shade_views_fwd_kernel<true>, a, units, num_sms, smem, stream, vc)
-                                : shade_launch(shade_views_fwd_kernel<false>, a, units, num_sms, smem, stream, vc);
+        const int rc = filt ? (smem_env ? shade_launch(shade_views_fwd_kernel<true, true>, a, units, num_sms, smem, stream, vc, lv)
+                                        : shade_launch(shade_views_fwd_kernel<false, true>, a, units, num_sms, smem, stream, vc, lv))
+                            : (smem_env ? shade_launch(shade_views_fwd_kernel<true, false>, a, units, num_sms, smem, stream, vc, lv)
+                                        : shade_launch(shade_views_fwd_kernel<false, false>, a, units, num_sms, smem, stream, vc, lv));
         if (rc) return rc;
     }
     return 0;
 }
 
 // the env-gradient mode as the one-view backward picks it at its default highest mode (the view kernels have no knobs)
-int launch_shade_views_backward(ShadeArgs a, int V, int num_sms, cudaStream_t stream) {
-    return shade_backward(a, V, ENV_CAS, num_sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
+int launch_shade_views_backward(ShadeArgs a, const EnvLevels& lv, bool filt, int V, int num_sms, cudaStream_t stream) {
+    return shade_backward(a, V, ENV_CAS, env_texels(a, lv, filt), num_sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
         constexpr int M = decltype(mode)::value;
         if constexpr (M == ENV_TAG) return (int)R3DG_ERR_UNSUPPORTED;     // above the cap: never selected
         else {
@@ -1046,7 +1146,8 @@ int launch_shade_views_backward(ShadeArgs a, int V, int num_sms, cudaStream_t st
                                 (size_t)3 * SHADE_VIEW_CHUNK * SHADE_THREADS * sizeof(float) + env_smem;
             for (int v0 = 0; v0 < V; v0 += SHADE_VIEW_CHUNK) {
                 const ViewChunk vc{v0, V - v0 < SHADE_VIEW_CHUNK ? V - v0 : SHADE_VIEW_CHUNK, 0, v0 > 0};
-                const int rc = shade_launch(shade_views_bwd_kernel<M>, x, (x.P + 3) / 4, num_sms, smem, stream, vc);
+                const int rc = filt ? shade_launch(shade_views_bwd_kernel<M, true>, x, (x.P + 3) / 4, num_sms, smem, stream, vc, lv)
+                                    : shade_launch(shade_views_bwd_kernel<M, false>, x, (x.P + 3) / 4, num_sms, smem, stream, vc, lv);
                 if (rc) return rc;
             }
             return 0;
@@ -1080,6 +1181,9 @@ static int fill_args(const r3dg_shade_args* s, ShadeArgs& a) {
     return 0;
 }
 
+// the filtered mode runs when a pyramid is given and the env has a coarser level; otherwise the call is the plain one
+static bool filtered(const r3dg_shade_args* s, const EnvLevels& lv) { return s->env_pyramid && lv.L > 1; }
+
 int r3dg_render_equation_forward(const r3dg_shade_args* s, r3dg_stream_t stream) {
     ShadeArgs a;
     int rc = fill_args(s, a);
@@ -1087,12 +1191,15 @@ int r3dg_render_equation_forward(const r3dg_shade_args* s, r3dg_stream_t stream)
     if (a.P > 0 && (!a.pbr || !a.diffuse || !a.specular)) return R3DG_ERR_BAD_ARG;
     if ((a.mean_lights != nullptr) != (a.mean_local != nullptr) || (a.mean_lights != nullptr) != (a.mean_global != nullptr)) return R3DG_ERR_BAD_ARG;
     if ((a.s_lights != nullptr) != (a.s_local != nullptr) || (a.s_lights != nullptr) != (a.s_global != nullptr)) return R3DG_ERR_BAD_ARG;
+    const EnvLevels lv = env_levels(a.He, a.We);
+    const bool filt = filtered(s, lv);
+    if (filt) a.env = s->env_pyramid;
     if (s->V > 1) {
         if (a.s_lights) return R3DG_ERR_UNSUPPORTED;               // no per-sample [V,P,N,3] outputs
         if (a.mean_lights && !a.mean_vis) return R3DG_ERR_BAD_ARG;
-        return launch_shade_views_forward(a, s->V, s->transform_per_view && a.transform, num_sms(), (cudaStream_t)stream);
+        return launch_shade_views_forward(a, lv, filt, s->V, s->transform_per_view && a.transform, num_sms(), (cudaStream_t)stream);
     }
-    return launch_shade_forward(a, num_sms(), (cudaStream_t)stream);
+    return launch_shade_forward(a, lv, filt, num_sms(), (cudaStream_t)stream);
 }
 
 int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream) {
@@ -1100,20 +1207,32 @@ int r3dg_render_equation_backward(const r3dg_shade_args* s, r3dg_stream_t stream
     int rc = fill_args(s, a);
     if (rc) return rc;
     if (!a.g_pbr || !a.d_base || !a.d_rough || !a.d_view || !a.d_incidents || !a.d_env) return R3DG_ERR_BAD_ARG;
+    if (s->env_pyramid && !s->dL_denv_pyramid) return R3DG_ERR_BAD_ARG;
     if (s->V > 1 && s->transform_per_view && a.transform) return R3DG_ERR_UNSUPPORTED;    // forward only
+    const EnvLevels lv = env_levels(a.He, a.We);
+    const bool filt = filtered(s, lv);
+    float* d_env = a.d_env;
+    if (filt) { a.env = s->env_pyramid; a.d_env = s->dL_denv_pyramid; }      // the kernels' gradient: every level
     if (s->deterministic) {
-        const size_t n = (size_t)a.He * a.We * 3;
-        if (!s->det_work || s->det_work_bytes < r3dg_shade_det_bytes(a.He, a.We)) return R3DG_ERR_BAD_ARG;
+        const size_t need = s->env_pyramid ? r3dg_shade_filtered_det_bytes(a.He, a.We) : r3dg_shade_det_bytes(a.He, a.We);
+        if (!s->det_work || s->det_work_bytes < need) return R3DG_ERR_BAD_ARG;
+        const size_t n = env_texels(a, lv, filt) * 3;
         a.det = det_acc(s->det_work, n);
         a.det_scale = (uint32_t*)((char*)s->det_work + det_bytes(n));
     }
-    return s->V > 1 ? launch_shade_views_backward(a, s->V, num_sms(), (cudaStream_t)stream)
-                    : launch_shade_backward(a, num_sms(), (cudaStream_t)stream);
+    const cudaStream_t st = (cudaStream_t)stream;
+    rc = s->V > 1 ? launch_shade_views_backward(a, lv, filt, s->V, num_sms(), st) : launch_shade_backward(a, lv, filt, num_sms(), st);
+    if (rc || !filt) return rc;
+    return launch_env_pyramid_adjoint(lv, a.d_env, d_env, st);               // dL/denv through the pyramid
 }
 
 // the accumulators and the call's scale word
 size_t r3dg_shade_det_bytes(int env_h, int env_w) {
     return env_h > 0 && env_w > 0 ? det_bytes((size_t)env_h * env_w * 3) + 256 : 0;
+}
+
+size_t r3dg_shade_filtered_det_bytes(int env_h, int env_w) {
+    return env_h > 0 && env_w > 0 ? det_bytes(r3dg_env_pyramid_floats(env_h, env_w)) + 256 : 0;
 }
 
 }  // extern "C"

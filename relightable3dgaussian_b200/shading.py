@@ -14,6 +14,12 @@ time, the backward accumulates the environment-map gradient in fixed point, so e
 bitwise reproducible (the reference's grid_sample backward raises under that flag).  The per-sample entries of extra_results
 (`incident_lights`, `local_incident_lights`, `global_incident_lights`) are materialised lazily on
 first access (eval only) and carry no gradient.
+
+Filtered environment lighting (opt-in: `env_filter=True`, or `set_env_filter(True)` for the process): each incident
+sample reads the environment averaged over its own solid angle from a lat-long mip pyramid instead of one bilinear
+tap (include/r3dg_b200.h, PREFILTERED ENVIRONMENT).  The pyramid is built from the activated env on every call, so
+the env gradient flows through it (and softplus); at footprints below a texel the lookup is the point lookup, bit for
+bit.
 """
 import ctypes
 
@@ -30,6 +36,34 @@ def _env_texture(light):
     if hasattr(light, "envmap"):
         return light.envmap, getattr(light, "transform", None)
     raise TypeError("direct_light_env_light must expose `get_env` (DirectLightMap) or `envmap` (EnvLight)")
+
+
+_ENV_FILTER = False      # process default of `env_filter` (set_env_filter)
+
+
+def set_env_filter(enabled):
+    """Process default of the filtered environment lookup for calls that pass env_filter=None (the reference's
+    unmodified callers after install()).  Off by default.  Returns the previous setting."""
+    global _ENV_FILTER
+    prev, _ENV_FILTER = _ENV_FILTER, bool(enabled)
+    return prev
+
+
+def _filter_on(env_filter):
+    return _ENV_FILTER if env_filter is None else bool(env_filter)
+
+
+def env_pyramid(env):
+    """The filtered mode's mip pyramid of the activated env [He,We,3] (all levels, level 0 = env, flattened), or None
+    when the env has no coarser level (fewer than 3 rows or columns): the mode then changes nothing."""
+    env = _lib.f32(env)
+    He, We = env.shape[0], env.shape[1]
+    lib = _lib.load()
+    if lib.r3dg_env_pyramid_levels(He, We) <= 1:
+        return None
+    pyr = torch.empty((lib.r3dg_env_pyramid_floats(He, We),), dtype=torch.float32, device=env.device)
+    _lib.call("r3dg_env_pyramid_build", env.device, env.data_ptr(), He, We, pyr.data_ptr(), what="env pyramid build")
+    return pyr
 
 
 def _args(P, N, He, We):
@@ -59,11 +93,14 @@ class _RenderEquation(torch.autograd.Function):
     """The shading step of one view (viewdirs [P,3], outputs [P,*]) or of V views (viewdirs [V,P,3], outputs [V,P,*])."""
 
     @staticmethod
-    def forward(ctx, base_color, roughness, viewdirs, incidents, env, normals, visibility, dirs, areas, transform, want_means):
+    def forward(ctx, base_color, roughness, viewdirs, incidents, env, normals, visibility, dirs, areas, transform, want_means,
+                env_filter=False):
         P = dirs.shape[0]
         lead = tuple(viewdirs.shape[:-2])
         f = dict(dtype=torch.float32, device=dirs.device)
         a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, visibility, dirs, areas), transform)
+        pyr = env_pyramid(ts[5]) if env_filter and P > 0 else None
+        a.env_pyramid = None if pyr is None else pyr.data_ptr()
         pbr, diffuse, specular = (torch.empty(lead + (P, 3), **f) for _ in range(3))
         a.pbr, a.diffuse_light, a.specular = pbr.data_ptr(), diffuse.data_ptr(), specular.data_ptr()
         means = []
@@ -73,7 +110,7 @@ class _RenderEquation(torch.autograd.Function):
         if P > 0:
             _lib.call("r3dg_render_equation_forward", dirs.device, ctypes.byref(a), what="rendering_equation")
         ctx.save_for_backward(*ts)
-        ctx.transform = tr
+        ctx.transform, ctx.pyramid = tr, pyr
         ctx.mark_non_differentiable(*means)
         return (pbr, diffuse, specular) + tuple(means)
 
@@ -89,15 +126,20 @@ class _RenderEquation(torch.autograd.Function):
         d_inc = torch.empty((P, 16, 3), **f)
         d_env = torch.empty(env.shape, **f)
         if P == 0:                      # nothing to shade: empty gradients (no device pointers to pass)
-            return d_base, d_rough, d_view, d_inc, d_env.zero_(), None, None, None, None, None, None
+            return d_base, d_rough, d_view, d_inc, d_env.zero_(), None, None, None, None, None, None, None
         gz = torch.zeros(viewdirs.shape, **f)
         g = [gz if t is None else _lib.f32(t) for t in (g_pbr, g_diffuse, g_specular)]
         a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = [t.data_ptr() for t in g]
         a.dL_dbase_color, a.dL_droughness, a.dL_dviewdirs = d_base.data_ptr(), d_rough.data_ptr(), d_view.data_ptr()
         a.dL_dincidents, a.dL_denv = d_inc.data_ptr(), d_env.data_ptr()
-        det_ws = _lib.det_workspace(a, _lib.load().r3dg_shade_det_bytes(env.shape[0], env.shape[1]), dev)
+        lib, pyr, g_pyr = _lib.load(), ctx.pyramid, None
+        if pyr is not None:             # the gradient of every pyramid level, folded into dL/denv by the call
+            a.env_pyramid, g_pyr = pyr.data_ptr(), torch.empty_like(pyr)
+            a.dL_denv_pyramid = g_pyr.data_ptr()
+        det_bytes = (lib.r3dg_shade_det_bytes if pyr is None else lib.r3dg_shade_filtered_det_bytes)(env.shape[0], env.shape[1])
+        det_ws = _lib.det_workspace(a, det_bytes, dev)
         _lib.call("r3dg_render_equation_backward", dev, ctypes.byref(a), what="rendering_equation backward")
-        return d_base, d_rough, d_view, d_inc, d_env, None, None, None, None, None, None
+        return d_base, d_rough, d_view, d_inc, d_env, None, None, None, None, None, None, None
 
 
 class _LazyExtras(dict):
@@ -135,18 +177,24 @@ class _LazyExtras(dict):
 
 
 def rendering_equation(base_color, roughness, normals, viewdirs, incidents, direct_light_env_light=None,
-                       visibility_precompute=None, incident_dirs_precompute=None, incident_areas_precompute=None):
-    """Drop-in for gaussian_renderer/neilf.py:339-371: returns (pbr [P,3], extra_results)."""
+                       visibility_precompute=None, incident_dirs_precompute=None, incident_areas_precompute=None,
+                       env_filter=None):
+    """Drop-in for gaussian_renderer/neilf.py:339-371: returns (pbr [P,3], extra_results).  env_filter: True reads the
+    environment filtered over each sample's footprint, False the point lookup, None the process default
+    (set_env_filter)."""
     if incidents.shape[1] != 16:
         raise RuntimeError("incidents must be degree-3 SH coefficients [P,16,3]")
     env, transform = _env_texture(direct_light_env_light)
     dirs, areas, vis = incident_dirs_precompute, incident_areas_precompute, visibility_precompute
+    filt = _filter_on(env_filter)
     pbr, diffuse, specular = _RenderEquation.apply(base_color, roughness, viewdirs, incidents, env, normals, vis, dirs,
-                                                   areas, transform, False)
+                                                   areas, transform, False, filt)
 
     def per_sample():
         a, ts, tr = _shade_args((base_color, roughness, normals, viewdirs, incidents, env, vis, dirs, areas), transform)
         P, N = dirs.shape[0], dirs.shape[1]
+        pyr = env_pyramid(ts[5]) if filt and P > 0 else None
+        a.env_pyramid = None if pyr is None else pyr.data_ptr()
         f = dict(dtype=torch.float32, device=dirs.device)
         outs = [torch.empty((P, N, 3), **f) for _ in range(3)]
         scratch = [torch.empty((P, 3), **f) for _ in range(3)]
@@ -167,7 +215,7 @@ _MEANS = ("mean_incident_lights", "mean_local_incident_lights", "mean_global_inc
 
 def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents, direct_light_env_light=None,
                              visibility_precompute=None, incident_dirs_precompute=None, incident_areas_precompute=None,
-                             means=False):
+                             means=False, env_filter=None):
     """`rendering_equation` for V view directions of the same Gaussians in one call: viewdirs [V,P,3], every other input
     as in `rendering_equation`.  The incident light of each sample is evaluated once for all views.
 
@@ -179,7 +227,9 @@ def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents
     An EnvLight `transform` may be [3,3] or [V,3,3] (one per view, forward only).  Gradients: viewdirs per view;
     base_color, roughness, incidents and the environment map summed over the views; none for normals and the baked
     tensors.  Refused before anything is launched: V outside 1..MAX_VIEWS, viewdirs not [V,P,3], incidents not [P,16,3],
-    a [V',3,3] transform with V' != V, and per-view transforms when autograd would need a backward."""
+    a [V',3,3] transform with V' != V, and per-view transforms when autograd would need a backward.  env_filter: as in
+    `rendering_equation`; the filtered light is evaluated once per sample for all views (per view with per-view
+    transforms)."""
     dirs, areas, vis = incident_dirs_precompute, incident_areas_precompute, visibility_precompute
     P = dirs.shape[0]
     if viewdirs.dim() != 3 or viewdirs.shape[1:] != (P, 3):
@@ -196,7 +246,7 @@ def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents
         if torch.is_grad_enabled() and any(t.requires_grad for t in (base_color, roughness, viewdirs, incidents, env)):
             raise ValueError("per-view transforms are forward-only: call under torch.no_grad() or with detached inputs")
     outs = _RenderEquation.apply(base_color, roughness, viewdirs, incidents, env, normals, vis, dirs, areas, transform,
-                                 bool(means))
+                                 bool(means), _filter_on(env_filter))
     pbr, diffuse, specular = outs[:3]
     extra = {"incident_dirs": dirs, "incident_visibility": vis, "diffuse_light": diffuse, "specular": specular}
     extra.update(zip(_MEANS, outs[3:]))
@@ -204,7 +254,8 @@ def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents
 
 
 def install(module=None):
-    """Rebind `rendering_equation` inside the reference's gaussian_renderer.neilf (or `module`)."""
+    """Rebind `rendering_equation` inside the reference's gaussian_renderer.neilf (or `module`).  Its callers pass no
+    env_filter, so set_env_filter decides their lookup."""
     if module is None:
         import gaussian_renderer.neilf as module
     module.rendering_equation = rendering_equation
