@@ -441,6 +441,40 @@ int r3dg_bvh_bake_visibility(int P, int first_slot, int count, int N, const int3
                              void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Ray-traced indirect light: what each Gaussian's incident rays see of the other Gaussians,
+ * and its least-squares fit into the incident-light SH `incidents` (DESIGN.md §4.25).
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_bvh_bake_radiance_tmp_bytes(int P);
+
+/* The radiance bake of a built tree: for every Gaussian g and sample i the ray of
+ * r3dg_bvh_bake_visibility (direction generated in the kernel from normals[g], origin
+ * mean_g + origin_offset * dir), with the same hit rule (opacity >= 1/255, not back-facing, peak
+ * t >= 0.01, alpha = opacity * exp(power)).  Hits are composited front to back in ascending
+ * (t, Gaussian index):  L += T * alpha * c,  T *= 1 - alpha,  until T < 1e-4.  The payload is the
+ * hit Gaussian's SH shs f32[P,M,3] of degree sh_degree (0..3, M >= (sh_degree+1)^2) in the
+ * rasterizer's colour convention c = max(sum_k Y_k(v) sh_k + 0.5, 0), v = normalize(mean_hit -
+ * origin).  Outputs, every element written: radiance f32[P,N,3], transmittance f32[P,N] (T when
+ * the ray stopped), num_hits i32[P,N] (hits composited; may be NULL).  The result is bitwise
+ * reproducible.  R3DG_ERR_BAD_ARG for a bad degree / M or a short tmp, R3DG_ERR_UNSUPPORTED for
+ * N beyond the bake's sample table (N * 12 > 32 KB, as r3dg_bvh_bake_visibility).
+ * tmp: r3dg_bvh_bake_radiance_tmp_bytes(P). */
+int r3dg_bvh_bake_radiance(int P, int N, const int32_t* nodes, const float* aabbs, const float* means3D,
+                           const float* covs3D, const float* opacities, const float* normals,
+                           const float* shs, int M, int sh_degree, float origin_offset, float* radiance,
+                           float* transmittance, int32_t* num_hits, void* tmp, size_t tmp_bytes,
+                           r3dg_stream_t stream);
+
+/* Per Gaussian g: c = argmin (1/N) sum_i |Y(w_i)^T c - L_i|^2 + ridge |c|^2 over SH of degree
+ * `degree` (0..3), with w_i the bake's N directions around normals[g] (regenerated, not read) and
+ * L_i = radiance[g,i] f32[P,N,3].  The model is the shading step's local light sum_k Y_k c_k (no
+ * +0.5).  out f32[P,(degree+1)^2,3] in the layout of `get_incidents()` (dc first).  Solved in
+ * fp64 (Gram matrix summed in sample order, Cholesky): deterministic.  ridge must be > 0: the
+ * samples cover one hemisphere only.  R3DG_ERR_BAD_ARG for a bad degree / ridge or N == 0 with
+ * P > 0, R3DG_ERR_UNSUPPORTED for N * 12 > 32 KB. */
+int r3dg_fit_incident_sh(int P, int N, const float* radiance, const float* normals, int degree, float ridge,
+                         float* out, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optional fused epilogue of the rasterizer call sites (SURVEY.md §8(f)2):
  *     feature / opacity.clamp_min(1e-5) * (num_contrib > 0)
  * (gaussian_renderer/neilf.py:135-137, render.py:106-108; 3 PyTorch kernels forward, ~6 backward).

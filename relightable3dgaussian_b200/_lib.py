@@ -158,6 +158,10 @@ SYMBOLS = [
     ("r3dg_sample_incident_dirs", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_bvh_bake_visibility", c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("r3dg_bvh_bake_radiance_tmp_bytes", c_size_t, [c_int]),
+    ("r3dg_bvh_bake_radiance", c_int, [c_int, c_int] + [c_void_p] * 7 + [c_int, c_int, c_float] + [c_void_p] * 4 +
+                                      [c_size_t, c_void_p]),
+    ("r3dg_fit_incident_sh", c_int, [c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     ("r3dg_unpremultiply_forward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_unpremultiply_backward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_render_equation_forward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),

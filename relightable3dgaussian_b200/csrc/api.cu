@@ -468,6 +468,26 @@ int r3dg_bvh_bake_visibility(int P, int first_slot, int count, int N, const int3
                            num_contributes, visibility, dirs, areas, tmp, tmp_bytes, num_sms(), (cudaStream_t)stream);
 }
 
+// ---- ray-traced indirect light ------------------------------------------------------------
+size_t r3dg_bvh_bake_radiance_tmp_bytes(int P) { return bvh_radiance_tmp_bytes(P); }
+
+int r3dg_bvh_bake_radiance(int P, int N, const int32_t* nodes, const float* aabbs, const float* means3D,
+                           const float* covs3D, const float* opacities, const float* normals, const float* shs, int M,
+                           int sh_degree, float origin_offset, float* radiance, float* transmittance, int32_t* num_hits,
+                           void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {
+    const int rc = launch_bvh_radiance(P, N, nodes, aabbs, means3D, covs3D, opacities, normals, shs, M, sh_degree, origin_offset,
+                                       radiance, transmittance, num_hits, tmp, tmp_bytes, (cudaStream_t)stream);
+    g_launches += (rc == 0 && P > 0 && N > 0) ? 2 : 0;
+    return rc;
+}
+
+int r3dg_fit_incident_sh(int P, int N, const float* radiance, const float* normals, int degree, float ridge, float* out,
+                         r3dg_stream_t stream) {
+    const int rc = launch_fit_incident_sh(P, N, radiance, normals, degree, ridge, out, (cudaStream_t)stream);
+    g_launches += (rc == 0 && P > 0) ? 1 : 0;
+    return rc;
+}
+
 int r3dg_unpremultiply_forward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
                                float* out, r3dg_stream_t stream) {
     if (S < 0 || HW < 0) return R3DG_ERR_BAD_ARG;

@@ -18,7 +18,7 @@
 //    early exit at T < 0.9 does not idle lanes.  Per ray the visiting order (far child pushed
 //    first) is the reference's, hence the product order of (1 - alpha) too.
 #include <cstdio>
-#include "common.cuh"
+#include "bvh.cuh"
 #include "kernels.h"
 
 namespace r3dg {
@@ -241,8 +241,7 @@ __global__ void __launch_bounds__(256) bvh_refit_kernel(int P, int32_t* nodes, f
 }
 
 // ---- trace ------------------------------------------------------------------------------------
-// packets: [NI] internal {l, r, lbox[6], rbox[6], pad[2]} then [P] leaf {mean3, cinv6, opacity, normal3, pad3}
-// child encoding: >= 0 internal node index; < 0 leaf slot  -(slot + 1)   (slot = Morton-order position)
+// packets: the layout of bvh.cuh (LeafRecord)
 __global__ void __launch_bounds__(256) bvh_pack_kernel(int P, const int32_t* __restrict__ nodes, const float* __restrict__ aabbs,
                                                        const float* __restrict__ means3D, const float* __restrict__ covs3D,
                                                        const float* __restrict__ opacities, const float* __restrict__ normals,
@@ -272,62 +271,6 @@ __global__ void __launch_bounds__(256) bvh_pack_kernel(int P, const int32_t* __r
     }
 }
 
-// Slab test of utility.cuh:35-82.  The reference divides (b - o) / d six times per box; here the three reciprocals
-// 1/d are formed ONCE per ray (IEEE, so zero components still give +-inf and 0 * inf = NaN exactly where the
-// reference's 0 / 0 does) and each slab distance is one multiply: ~12 instructions per box instead of ~60.  A product
-// by the rounded reciprocal can differ from the quotient in the last bit, which only matters when a ray grazes a box
-// exactly; the tests bound the resulting visibility flip rate against the reference's own kernels (<= 1e-3).
-__device__ __forceinline__ float ray_box_tmax(float b0, float b1, float b2, float b3, float b4, float b5,
-                                              float ox, float oy, float oz, float ix, float iy, float iz) {
-    float tmin = mul_(sub_(b0, ox), ix), tmax = mul_(sub_(b3, ox), ix);
-    if (tmin > tmax) { const float t = tmin; tmin = tmax; tmax = t; }
-    float tymin = mul_(sub_(b1, oy), iy), tymax = mul_(sub_(b4, oy), iy);
-    if (tymin > tymax) { const float t = tymin; tymin = tymax; tymax = t; }
-    if (tmin > tymax || tymin > tmax) return -1.0f;
-    if (tymin > tmin) tmin = tymin;
-    if (tymax < tmax) tmax = tymax;
-    float tzmin = mul_(sub_(b2, oz), iz), tzmax = mul_(sub_(b5, oz), iz);
-    if (tzmin > tzmax) { const float t = tzmin; tzmin = tzmax; tzmax = t; }
-    if (tmin > tzmax || tzmin > tmax) return -1.0f;
-    if (tzmax < tmax) tmax = tzmax;
-    return tmax;
-}
-
-// ---- incident-direction sampling (reference utils/graphics_utils.py:9-37 fibonacci_sphere_sampling with
-// random_rotate=False — the bake always samples deterministically, scene/gaussian_model.py:324 — and
-// utils/sh_utils.py:36-68 rotation_between_z), restated with torch's op-by-op fp32 rounding -------------
-// Canonical sample i of N (the [1,3,N] `z_samples` tensor of the reference): computed per CTA into shared
-// memory by whoever needs it; identical for every Gaussian.
-__device__ __forceinline__ float3 fib_sample(int i, int N) {
-    const float idx = (float)i;
-    // z = (1 - 2*idx/(2N-1)).clamp_min(sin(10 deg));  rad = sqrt(1 - z**2);  theta = delta*idx
-    const float z = fmaxf(sub_(1.0f, div_(mul_(2.0f, idx), (float)(2 * N - 1))), 0.17364817766693033f);
-    const float rad = sqrt_(sub_(1.0f, mul_(z, z)));
-    const float theta = mul_(2.399963229728653f, idx);          // pi * (3 - sqrt(5))
-    return make_float3(mul_(sinf(theta), rad), mul_(cosf(theta), rad), z);
-}
-// R(normal) @ sample, then F.normalize: the rotation taking +z to `normal` (Rodrigues from z; -I when n.z + 1 <= 0).
-// With v = (-n.y, n.x, 0) the reference's nine entries reduce exactly (x + 0 == x, -0 - x == -x in IEEE) to the ones below.
-__device__ __forceinline__ float3 rotate_from_z(float nx, float ny, float nz, float3 s) {
-    float r00, r01, r02, r10, r11, r12, r20, r21, r22;
-    const float zp1 = add_(nz, 1.0f);
-    if (zp1 > 0.0f) {
-        const float v1 = -ny, v2 = nx, c = fmaxf(zp1, 1e-7f);
-        const float v11 = mul_(v1, v1), v22 = mul_(v2, v2), v12 = mul_(v1, v2);
-        r00 = add_(1.0f, div_(-v22, c)); r01 = div_(v12, c);             r02 = v2;
-        r10 = div_(v12, c);             r11 = add_(1.0f, div_(-v11, c)); r12 = -v1;
-        r20 = -v2;                      r21 = v1;                        r22 = add_(1.0f, div_(sub_(-v22, v11), c));
-    } else {
-        r00 = r11 = r22 = -1.0f; r01 = r02 = r10 = r12 = r20 = r21 = 0.0f;
-    }
-    // the [P,3,3] @ [1,3,N] matmul: K = 3 accumulated in order (fp32 FMA chain, as cuBLAS sgemm does)
-    const float x = fma_(r02, s.z, fma_(r01, s.y, mul_(r00, s.x)));
-    const float y = fma_(r12, s.z, fma_(r11, s.y, mul_(r10, s.x)));
-    const float z = fma_(r22, s.z, fma_(r21, s.y, mul_(r20, s.x)));
-    const float nrm = fmaxf(sqrt_(fma_(z, z, fma_(y, y, mul_(x, x)))), 1e-12f);   // F.normalize eps
-    return make_float3(div_(x, nrm), div_(y, nrm), div_(z, nrm));
-}
-
 // phase != nullptr: random_rotate=True — theta_i += phase[g] * 2 * pi with phase = torch.rand(P) drawn by the caller
 __global__ void __launch_bounds__(256) sample_dirs_kernel(int P, int N, const float* __restrict__ normals,
                                                           const float* __restrict__ phase,
@@ -352,8 +295,6 @@ __global__ void __launch_bounds__(256) sample_dirs_kernel(int P, int N, const fl
 }
 
 #define TRACE_THREADS 128
-#define TRACE_STACK 64          // total per-ray stack capacity (the reference's local array is 64 too, trace.cuh)
-#define TRACE_STACK_SH 20       // entries kept in shared memory; deeper levels spill to a per-thread local array
 // BAKE = false: explicit rays (rays_o [num_rays / o_group, 3], rays_d [num_rays, 3]) — trace_bvh_opacity.
 // BAKE = true : the visibility bake: ray r = (leaf slot first_slot + r / N, sample r % N); the Gaussian is the
 //   slot's object (Morton order => neighbouring warps walk neighbouring subtrees), the origin its mean, the
@@ -551,6 +492,13 @@ int launch_bvh_trace(int P, long long num_rays, const int32_t* nodes, const floa
     return 0;
 }
 
+int launch_bvh_pack(int P, const int32_t* nodes, const float* aabbs, const float* means3D, const float* covs3D,
+                    const float* opacities, const float* normals, float4* packets, cudaStream_t stream) {
+    bvh_pack_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, nodes, aabbs, means3D, covs3D, opacities, normals, packets);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
 int launch_sample_dirs(int P, int N, const float* normals, const float* phase, float* dirs, float* areas, int num_sms, cudaStream_t stream) {
     if (P <= 0 || N <= 0) return 0;
     if ((size_t)N * sizeof(float3) > 48 * 1024) return R3DG_ERR_UNSUPPORTED;          // N <= 4096
@@ -568,7 +516,7 @@ int launch_bvh_bake(int P, int first_slot, int count, int N, const int32_t* node
                     size_t packets_bytes, int num_sms, cudaStream_t stream) {
     if (P <= 0 || count <= 0 || N <= 0) return 0;
     if (packets_bytes < bvh_packets_bytes(P) || first_slot < 0 || first_slot + count > P) return R3DG_ERR_BAD_ARG;
-    if ((size_t)N * sizeof(float3) > 32 * 1024) return R3DG_ERR_UNSUPPORTED;
+    if ((size_t)N * sizeof(float3) > BAKE_SAMPLE_SMEM) return R3DG_ERR_UNSUPPORTED;
     unsigned long long* counter = (unsigned long long*)packets_;
     float4* packets = (float4*)((char*)packets_ + 256);
     R3DG_CUDA_TRY(cudaMemsetAsync(counter, 0, 8, stream));

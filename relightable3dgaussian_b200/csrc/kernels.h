@@ -131,6 +131,16 @@ int launch_bvh_bake(int P, int first_slot, int count, int N, const int32_t* node
                     const float* covs3D, const float* opacities, const float* normals, float o_offset,
                     int32_t* num_contributes, float* visibility, float* dirs, float* areas, void* packets,
                     size_t packets_bytes, int num_sms, cudaStream_t stream);
+// the packed tree of bvh.cuh into `packets` (bvh_packets_bytes(P) - 256 bytes)
+int launch_bvh_pack(int P, const int32_t* nodes, const float* aabbs, const float* means3D, const float* covs3D,
+                    const float* opacities, const float* normals, float4* packets, cudaStream_t stream);
+size_t bvh_radiance_tmp_bytes(int P);
+int launch_bvh_radiance(int P, int N, const int32_t* nodes, const float* aabbs, const float* means3D, const float* covs3D,
+                        const float* opacities, const float* normals, const float* shs, int M, int sh_degree,
+                        float o_offset, float* radiance, float* transmittance, int32_t* num_hits, void* tmp,
+                        size_t tmp_bytes, cudaStream_t stream);
+int launch_fit_incident_sh(int P, int N, const float* radiance, const float* normals, int degree, float ridge, float* out,
+                           cudaStream_t stream);
 int launch_unpremultiply_forward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
                                  float* out, int num_sms, cudaStream_t stream);
 int launch_unpremultiply_backward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,

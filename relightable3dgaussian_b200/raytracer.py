@@ -11,6 +11,10 @@ Differences from the reference that are not observable in the results:
   * update_visibility is ONE launch over all Gaussians in Morton order instead of the reference's
     chunk loop (the chunks only bound the size of its [chunk,N,3] PyTorch temporaries); the
     `[P,N,3]` ray-origin / ray-direction inputs of the reference's trace call never exist.
+
+Beyond the reference: `RayTracer.bake_radiance` / `fit_incident_sh` / `update_incidents` compute each Gaussian's
+incident-light SH (`incidents`) from the scene itself — the bake's rays composited front to back through the
+other Gaussians (r3dg_bvh_bake_radiance), then a per-Gaussian ridge fit (r3dg_fit_incident_sh).
 """
 import torch
 
@@ -105,6 +109,63 @@ class RayTracer:
                       _lib.ptr(out.get("contribute")), out["visibility"].data_ptr(), _lib.ptr(out.get("incident_dirs")),
                       _lib.ptr(out.get("incident_areas")), tmp.data_ptr(), tmp.numel(), what="bake_visibility")
         return out
+
+    @torch.no_grad()
+    def bake_radiance(self, means3D, symm_inv, opacity, normals, shs, sh_degree, sample_num, want_hits=False):
+        """What each of the bake's rays (those of `bake_visibility`) sees of the other Gaussians, composited front to
+        back in ascending (t, Gaussian index) until T < 1e-4 (r3dg_bvh_bake_radiance).  The payload `shs` [P,M,3]
+        is coloured like the rasterizer does from the ray origin; a view-independent radiance L [P,3] goes in as
+        degree 0 with shs = ((L - 0.5) / C0)[:, None].  Returns dict(radiance [P,N,3], transmittance [P,N,1]
+        [, num_hits i32[P,N]])."""
+        P, N, deg = means3D.shape[0], int(sample_num), int(sh_degree)
+        dev = means3D.device
+        if not all(t.is_cuda for t in (means3D, symm_inv, opacity, normals, shs)):
+            raise RuntimeError("bake_radiance runs on the GPU only (no CPU path)")
+        sh = _lib.f32(shs)
+        if sh.dim() != 3 or sh.shape[0] != P or sh.shape[2] != 3:
+            raise ValueError(f"shs must be [P, M, 3] with P = {P}, got {tuple(sh.shape)}")
+        out = {"radiance": torch.empty((P, N, 3), dtype=torch.float32, device=dev),
+               "transmittance": torch.empty((P, N, 1), dtype=torch.float32, device=dev)}
+        if want_hits:
+            out["num_hits"] = torch.empty((P, N), dtype=torch.int32, device=dev)
+        m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(normals)
+        tmp = _lib.scratch(_lib.load().r3dg_bvh_bake_radiance_tmp_bytes(P), dev)
+        _lib.call("r3dg_bvh_bake_radiance", dev, P, N, self.tree.data_ptr(), self.aabb.data_ptr(), m.data_ptr(),
+                  ci.data_ptr(), op.data_ptr(), nr.data_ptr(), sh.data_ptr(), sh.shape[1], deg, 0.05,
+                  out["radiance"].data_ptr(), out["transmittance"].data_ptr(), _lib.ptr(out.get("num_hits")),
+                  tmp.data_ptr(), tmp.numel(), what="bake_radiance")
+        return out
+
+
+@torch.no_grad()
+def fit_incident_sh(radiance, normals, degree=3, ridge=1e-3):
+    """Per Gaussian, the SH c [(degree+1)^2, 3] minimising (1/N) sum_i |Y(w_i)^T c - L_i|^2 + ridge |c|^2 over the
+    bake's N directions w_i around its normal (r3dg_fit_incident_sh): the local incident light of the shading step,
+    in the layout of `get_incidents()` (dc first).  radiance [P,N,3] -> [P,(degree+1)^2,3]."""
+    L, n = _lib.f32(radiance), _lib.f32(normals).reshape(-1, 3)
+    if not (L.is_cuda and n.is_cuda):
+        raise RuntimeError("fit_incident_sh runs on the GPU only (no CPU path)")
+    if L.dim() != 3 or L.shape[2] != 3 or L.shape[0] != n.shape[0]:
+        raise ValueError(f"radiance must be [P, N, 3] matching normals [P, 3], got {tuple(L.shape)}")
+    P, N, deg = L.shape[0], L.shape[1], int(degree)
+    out = torch.empty((P, max(deg + 1, 0) ** 2, 3), dtype=torch.float32, device=L.device)
+    _lib.call("r3dg_fit_incident_sh", L.device, P, N, L.data_ptr(), n.data_ptr(), deg, float(ridge), out.data_ptr(),
+              what="fit_incident_sh")
+    return out
+
+
+@torch.no_grad()
+def update_incidents(xyz, scaling, rotation, inverse_covariance, opacity, normal, shs, sh_degree, sample_num,
+                     incident_degree=3, ridge=1e-3):
+    """The analogue of `update_visibility` for the local half of the incident light: bake what each Gaussian's N
+    incident rays see of the others (payload `shs` of degree `sh_degree`, see RayTracer.bake_radiance) and fit it
+    into incident SH of degree `incident_degree`.  Returns incidents [P,(incident_degree+1)^2,3], to be written into
+    `_incidents_dc` (coefficient 0) and `_incidents_rest` (the others)."""
+    if xyz.shape[0] == 0:                   # no tree to build; the fit of nothing is empty
+        return fit_incident_sh(torch.zeros((0, int(sample_num), 3), device=xyz.device), normal, incident_degree, ridge)
+    raytracer = RayTracer(xyz, scaling, rotation)
+    out = raytracer.bake_radiance(xyz, inverse_covariance, opacity, normal, shs, sh_degree, sample_num)
+    return fit_incident_sh(out["radiance"], normal, incident_degree, ridge)
 
 
 @torch.no_grad()
