@@ -933,9 +933,12 @@ int r3dg_bilagrid_backward(int G, int N, int H, int W, int GX, int GY, int L, co
  *   sampling location of D', D', p', n_c, d and H), the geometric term scattered into depth[n] at the four
  *   bilinear taps of q; masks, w, counts and the clamp's flat region carry none.  It recomputes the forward per
  *   pixel.  Default: float atomics into zeroed outputs (2 memsets + 1 launch).  deterministic != 0: fixed-point
- *   accumulators (detacc.cuh) in det_work of r3dg_multiview_det_bytes(V, H, W) (96 B per view pixel), bitwise
- *   reproducible (memset + 2 launches); a term beyond 2^47 times the largest |dL_dgeo[b]| / max(count, 1) or
- *   |dL_dphoto[b]| / max(count, 1) saturates to +-Inf.
+ *   accumulators (detacc.cuh) in det_work of r3dg_multiview_det_bytes(V, H, W) (96 B per view pixel and 256 B),
+ *   bitwise reproducible and independent of the pairs' order (memset + 3 launches: the backward runs twice, first
+ *   to measure the largest |term| of dL_ddepth and of dL_dnormal).  Each of the two has its own exponent: that of
+ *   the largest |dL_dgeo[b]| / max(count, 1) and |dL_dphoto[b]| / max(count, 1), raised until its largest term
+ *   fits the accumulator range 2^47, so a term the default mode writes as a finite float (e.g. a normal shorter
+ *   than 1e-12, whose gradient carries 1e12) is finite here too; the resolution is 2^-48 of the larger of the two.
  * R3DG_ERR_BAD_ARG for V, H or W <= 0, B outside 1..R3DG_MAX_VIEWS, a pair index outside [0, V), a
  * non-finite camera row or tan_fov <= 0, a negative or NaN threshold, a NULL pointer the call needs, or too small
  * a workspace; R3DG_ERR_UNSUPPORTED for H*W >= 2^31 or H > 1048560.  Nothing is launched on an error.

@@ -7,7 +7,8 @@
 //             fixed-order reduction that writes the per-pair losses and counts on the device;
 //   backward: ONE kernel that recomputes the forward per pixel (nothing per tap is saved) and adds dL/ddepth and
 //             dL/dnormal at the pixel and dL/ddepth of the neighbour at the four bilinear taps of the reprojected
-//             pixel: float atomics into zeroed outputs by default; in deterministic mode fixed-point accumulators
+//             pixel: float atomics into zeroed outputs by default; in deterministic mode a first launch of the same
+//             kernel that only measures the largest |term| of each gradient, then fixed-point accumulators
 //             (detacc.cuh) and ONE pass that reads them back, so repeated references and shared neighbours sum in an
 //             order-independent way.
 // Arithmetic is IEEE fp32: divisions and square roots are the correctly rounded forms (no fast-math intrinsics);
@@ -97,21 +98,25 @@ __device__ __forceinline__ float bilinear(const float* __restrict__ p, int H, in
     return w00 * v00 + w10 * v10 + w01 * v01 + w11 * v11;
 }
 
-// Gradient sink of the backward: float atomics into zeroed outputs, or fixed-point accumulators (deterministic mode).
+// Gradient sink of the backward: float atomics into zeroed outputs, or fixed-point accumulators (deterministic mode),
+// or (measure) the largest |term| of each class in this thread, to size the accumulators' exponents.
 // Accumulator layout: depth [V][H*W], then normal [V][3][H*W].
 struct Sink {
     float* dd;           // dL_ddepth  [V,H,W]
     float* dn;           // dL_dnormal [V,3,H,W]
     DetAcc acc;
-    int e;               // fixed-point class exponent
-    bool det;
+    int ed, en;          // fixed-point exponents of the depth and the normal class
+    bool det, measure;
     size_t VHW;
-    __device__ __forceinline__ void depth(size_t i, float x) const {
-        if (det) det_add(acc, i, x, e);
+    uint32_t md, mn;     // measure: the thread's largest |term| (float bits) of each class
+    __device__ __forceinline__ void depth(size_t i, float x) {
+        if (measure) md = max(md, det_abs_bits(x));
+        else if (det) det_add(acc, i, x, ed);
         else atomicAdd(dd + i, x);
     }
-    __device__ __forceinline__ void normal(size_t i, float x) const {
-        if (det) det_add(acc, VHW + i, x, e);
+    __device__ __forceinline__ void normal(size_t i, float x) {
+        if (measure) mn = max(mn, det_abs_bits(x));
+        else if (det) det_add(acc, VHW + i, x, en);
         else atomicAdd(dn + i, x);
     }
 };
@@ -122,7 +127,7 @@ template <bool BWD>
 __device__ __forceinline__ void mv_pixel(const MvParams& prm, const MvPair& pr, const MvCam& cam, int x, int y,
                                          const float* __restrict__ depth, const float* __restrict__ normal,
                                          const float* __restrict__ gray, const float* sgray, int lx, int ly,
-                                         double* acc, float sg, float sp, const Sink& sink) {
+                                         double* acc, float sg, float sp, Sink& sink) {
     const int H = prm.H, W = prm.W;
     const size_t HW = (size_t)H * W, o = (size_t)y * W + x;
     const float* dr = depth + (size_t)pr.r * HW;
@@ -323,7 +328,7 @@ __global__ void __launch_bounds__(NT) mv_fwd_kernel(const __grid_constant__ MvPa
     const int lx = threadIdx.x % TS, ly = threadIdx.x / TS;
     const int x = blockIdx.x * TS + lx, y = blockIdx.y * TS + ly;
     double acc[4] = {0.0, 0.0, 0.0, 0.0};
-    const Sink none = {};
+    Sink none = {};
     if (x < prm.W && y < prm.H)
         mv_pixel<false>(prm, prm.pair[blockIdx.z], cam, x, y, depth, normal, gray, sgray, lx, ly, acc, 0.f, 0.f, none);
     cta_partials<NT, 4>(acc, partial + 4 * (((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x));
@@ -363,16 +368,24 @@ __device__ __forceinline__ float pair_scale(const float* __restrict__ g, const i
     return __ldg(g + b) / (float)max(__ldg(counts + 2 * b + k), 1);
 }
 
-// The fixed-point class exponent: from the largest |sg|, |sp| over the pairs (every term is linear in one of them).
-// Computed by warp 0 of each CTA (every CTA gets the same value); the result lands in *e.
+// The fixed-point exponents of the depth and the normal class (e[0], e[1]).  Every term is linear in one of the
+// pairs' |sg|, |sp|, so the exponent starts from the largest of them.  A term can still be far larger than its
+// cotangent: a normal shorter than kNormEps carries 1 / kNormEps = 1e12 in its gradient, and Y.z, X'.z or |d| near
+// their 1e-6 thresholds divide.  So each class's exponent is raised until its largest |term|, measured by the
+// backward's first launch (tmax[0], tmax[1]), lies inside the accumulator range 2^R3DG_DET_RANGE_LOG2; it is unchanged
+// when the terms already fit.  Computed by warp 0 of each CTA (every CTA gets the same values).
 __device__ __forceinline__ void det_exponent(int B, const float* __restrict__ dgeo, const float* __restrict__ dphoto,
-                                             const int* __restrict__ counts, int* e) {
+                                             const int* __restrict__ counts, const uint32_t* __restrict__ tmax, int* e) {
     if (threadIdx.x < 32) {
         uint32_t mx = 0u;
         for (int b = threadIdx.x; b < B; b += 32)
             mx = max(mx, max(det_abs_bits(pair_scale(dgeo, counts, b, 0)), det_abs_bits(pair_scale(dphoto, counts, b, 1))));
         mx = __reduce_max_sync(0xffffffffu, mx);
-        if (threadIdx.x == 0) *e = det_scale_exp(mx);
+        if (threadIdx.x < 2) {
+            const int ec = det_scale_exp(mx);
+            const uint32_t t = tmax[threadIdx.x], tb = t >> 23;    // 0 < tb < 255: a finite, normal largest term
+            e[threadIdx.x] = (tb == 0u || tb >= 255u) ? ec : max(ec, det_scale_exp(t) - (R3DG_DET_RANGE_LOG2 - 1));
+        }
     }
 }
 
@@ -380,32 +393,36 @@ __global__ void __launch_bounds__(NT) mv_bwd_kernel(const __grid_constant__ MvPa
                                                     const float* __restrict__ normal, const float* __restrict__ gray,
                                                     const float* __restrict__ view, const float* __restrict__ dgeo,
                                                     const float* __restrict__ dphoto, const int* __restrict__ counts,
-                                                    const Sink sink_arg) {
+                                                    const Sink sink_arg, uint32_t* __restrict__ tmax) {
     __shared__ float sgray[ST * ST];
     __shared__ MvCam cam;
-    __shared__ int s_e;
-    if (sink_arg.det) det_exponent(prm.B, dgeo, dphoto, counts, &s_e);
+    __shared__ int s_e[2];
+    if (sink_arg.det) det_exponent(prm.B, dgeo, dphoto, counts, tmax, s_e);
     mv_setup(prm, gray, view, cam, sgray);
     Sink sink = sink_arg;
-    if (sink.det) sink.e = s_e;
+    if (sink.det) { sink.ed = s_e[0]; sink.en = s_e[1]; }
     const int b = blockIdx.z;
     const float sg = pair_scale(dgeo, counts, b, 0), sp = pair_scale(dphoto, counts, b, 1);
     const int lx = threadIdx.x % TS, ly = threadIdx.x / TS;
     const int x = blockIdx.x * TS + lx, y = blockIdx.y * TS + ly;
     if (x < prm.W && y < prm.H && (sg != 0.f || sp != 0.f))
         mv_pixel<true>(prm, prm.pair[b], cam, x, y, depth, normal, gray, sgray, lx, ly, nullptr, sg, sp, sink);
+    if (sink.measure) {                                       // every thread of the CTA gets here
+        det_max_bits(tmax, sink.md);
+        det_max_bits(tmax + 1, sink.mn);
+    }
 }
 
 // deterministic mode: the accumulators read back into dL_ddepth and dL_dnormal (every element written)
 __global__ void __launch_bounds__(256) mv_det_read_kernel(int B, size_t VHW, const float* __restrict__ dgeo,
                                                           const float* __restrict__ dphoto, const int* __restrict__ counts,
-                                                          DetAcc acc, float* __restrict__ dd, float* __restrict__ dn) {
-    __shared__ int s_e;
-    det_exponent(B, dgeo, dphoto, counts, &s_e);
+                                                          const uint32_t* __restrict__ tmax, DetAcc acc,
+                                                          float* __restrict__ dd, float* __restrict__ dn) {
+    __shared__ int s_e[2];
+    det_exponent(B, dgeo, dphoto, counts, tmax, s_e);
     __syncthreads();
-    const int e = s_e;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < 4 * VHW; i += (size_t)gridDim.x * blockDim.x) {
-        const float v = det_load(acc, i, e);
+        const float v = det_load(acc, i, i < VHW ? s_e[0] : s_e[1]);
         if (i < VHW) dd[i] = v;
         else dn[i - VHW] = v;
     }
@@ -456,7 +473,7 @@ size_t multiview_work_bytes(int B, int H, int W) {
 
 size_t multiview_det_bytes(int V, int H, int W) {
     if (V <= 0 || H <= 0 || W <= 0 || (long long)H * W >= (1LL << 31)) return 0;
-    return det_bytes((size_t)V * 4 * H * W);
+    return det_bytes((size_t)V * 4 * H * W) + 256;          // the accumulators, then the two largest-term words
 }
 
 int launch_multiview_forward(const r3dg_multiview_args* a, cudaStream_t stream) {
@@ -482,20 +499,29 @@ int launch_multiview_backward(const r3dg_multiview_args* a, cudaStream_t stream)
     sink.dn = a->dL_dnormal;
     sink.det = a->deterministic != 0;
     sink.VHW = VHW;
+    const dim3 grid = tile_grid(a->B, a->H, a->W);
+    uint32_t* tmax = nullptr;
     if (sink.det) {
         sink.acc = det_acc(a->det_work, 4 * VHW);
-        R3DG_CUDA_TRY(cudaMemsetAsync(a->det_work, 0, det_bytes(4 * VHW), stream));
+        tmax = (uint32_t*)((char*)a->det_work + det_bytes(4 * VHW));
+        R3DG_CUDA_TRY(cudaMemsetAsync(a->det_work, 0, det_bytes(4 * VHW) + 2 * sizeof(uint32_t), stream));
+        Sink measure = sink;
+        measure.det = false;
+        measure.measure = true;
+        mv_bwd_kernel<<<grid, NT, 0, stream>>>(prm, a->depth, a->normal, a->gray, a->viewmatrix, a->dL_dgeo,
+                                               a->dL_dphoto, a->counts, measure, tmax);
+        R3DG_CUDA_TRY(cudaGetLastError());
     } else {
         R3DG_CUDA_TRY(cudaMemsetAsync(a->dL_ddepth, 0, VHW * sizeof(float), stream));
         R3DG_CUDA_TRY(cudaMemsetAsync(a->dL_dnormal, 0, 3 * VHW * sizeof(float), stream));
     }
-    mv_bwd_kernel<<<tile_grid(a->B, a->H, a->W), NT, 0, stream>>>(prm, a->depth, a->normal, a->gray, a->viewmatrix,
-                                                                  a->dL_dgeo, a->dL_dphoto, a->counts, sink);
+    mv_bwd_kernel<<<grid, NT, 0, stream>>>(prm, a->depth, a->normal, a->gray, a->viewmatrix, a->dL_dgeo, a->dL_dphoto,
+                                           a->counts, sink, tmax);
     R3DG_CUDA_TRY(cudaGetLastError());
     if (sink.det) {
         const size_t n = 4 * VHW;
         const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 132 * 16);
-        mv_det_read_kernel<<<blocks, 256, 0, stream>>>(a->B, VHW, a->dL_dgeo, a->dL_dphoto, a->counts, sink.acc,
+        mv_det_read_kernel<<<blocks, 256, 0, stream>>>(a->B, VHW, a->dL_dgeo, a->dL_dphoto, a->counts, tmax, sink.acc,
                                                        a->dL_ddepth, a->dL_dnormal);
         R3DG_CUDA_TRY(cudaGetLastError());
     }

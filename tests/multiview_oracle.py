@@ -47,6 +47,32 @@ def bilinear(img, u, v):
     return bx * by * tap(ix, iy) + ax * by * tap(ix + 1, iy) + bx * ay * tap(ix, iy + 1) + ax * ay * tap(ix + 1, iy + 1)
 
 
+def _grid(c, extent):
+    """How far a sampling coordinate lies from the nearest grid line, in units of 2e-4 + 2e-6 |c| pixels (about 1700
+    fp32 ulps at |c| = 1 and 2 at |c| = 4096): the bilinear sample's derivative jumps at a grid line, and the kernel's
+    fp32 coordinate, through the reprojection or the plane homography, may lie on the other side when this is below
+    1.  On an axis one pixel long, q and the warped taps are exact integers in the scenes that test such images:
+    they are built with exact arithmetic (axis-aligned cameras, principal point 0, equal focal lengths), which fp32
+    reproduces, so an exact integer there counts as decided."""
+    c = c.detach()
+    d = (c - torch.round(c)).abs() / (2e-4 + 2e-6 * c.abs())
+    return torch.where((c == torch.round(c)) & (extent == 1), torch.full_like(d, float("inf")), d)
+
+
+def _taps_le0(img, u, v):
+    """How many of the bilinear taps of (u, v) that carry weight and lie in the image hold a value <= 0."""
+    H, W = img.shape
+    x0, y0 = torch.floor(u), torch.floor(v)
+    ax, ay = u - x0, v - y0
+    ix, iy = x0.long(), y0.long()
+    n = torch.zeros_like(ix)
+    for dx, dy, wt in ((0, 0, (1 - ax) * (1 - ay)), (1, 0, ax * (1 - ay)), (0, 1, (1 - ax) * ay), (1, 1, ax * ay)):
+        i, j = ix + dx, iy + dy
+        inb = (i >= 0) & (i < W) & (j >= 0) & (j < H) & (wt > 0)
+        n = n + (inb & (img[j.clamp(0, H - 1), i.clamp(0, W - 1)] <= 0)).long()
+    return n
+
+
 def _pair(depth_r, depth_n, normal_r, gray_r, gray_n, cam_r, cam_n, tau, dtype, w=None):
     """Per-pixel terms of one pair: dict of geo / photo contributions and masks, with the decision quantities."""
     H, W = depth_r.shape
@@ -60,7 +86,11 @@ def _pair(depth_r, depth_n, normal_r, gray_r, gray_n, cam_r, cam_n, tau, dtype, 
     ys, xs = torch.meshgrid(torch.arange(H, device=dev, dtype=dtype), torch.arange(W, device=dev, dtype=dtype),
                             indexing="ij")
     xs, ys = xs.reshape(-1), ys.reshape(-1)
-    D = depth_r.reshape(-1)
+    # a non-finite depth is never valid: +inf makes q (reference) or phi (neighbour tap) NaN, -inf fails D > 0.  They
+    # are replaced by 0 where they are read, so that no inf * 0 reaches the gradients of the valid pixels.
+    D_raw = depth_r.reshape(-1)
+    D = torch.where(torch.isfinite(D_raw), D_raw, torch.zeros_like(D_raw))
+    depth_nf = torch.where(torch.isfinite(depth_n), depth_n, torch.zeros_like(depth_n))
     u = torch.stack([(xs - cxr) / fxr, (ys - cyr) / fyr, torch.ones_like(xs)], -1)
     X = D[:, None] * u
     Y = X @ R.T + t
@@ -68,13 +98,18 @@ def _pair(depth_r, depth_n, normal_r, gray_r, gray_n, cam_r, cam_n, tau, dtype, 
     Yz = _safe(ok, Y[:, 2])
     qx, qy = fxn * (Y[:, 0] / Yz) + cxn, fyn * (Y[:, 1] / Yz) + cyn
     qmargin = torch.minimum(torch.minimum(qx, W - 1 - qx), torch.minimum(qy, H - 1 - qy))
+    q_raw = torch.stack([qx, qy], -1).detach()
     ok = ok & (qmargin >= 0)
     qx, qy = _safe(ok, qx, 0.0), _safe(ok, qy, 0.0)
-    Dn = bilinear(depth_n, qx, qy)
-    ok = ok & (Dn > 0)
+    Dn_raw = bilinear(depth_n.detach(), qx.detach(), qy.detach())
+    taps_le0 = _taps_le0(depth_n.detach(), qx.detach(), qy.detach())
+    ok_q = ok
+    Dn = bilinear(depth_nf, qx, qy)
+    ok = ok & (Dn_raw > 0) & torch.isfinite(Dn_raw)
     Dn = _safe(ok, Dn)
     un = torch.stack([(qx - cxn) / fxn, (qy - cyn) / fyn, torch.ones_like(qx)], -1)
     Xp = (Dn[:, None] * un - t) @ R
+    ok_dn = ok
     ok = ok & (Xp[:, 2] > MIN_Z)
     Xz = _safe(ok, Xp[:, 2])
     ex, ey = fxr * (Xp[:, 0] / Xz) + cxr - xs, fyr * (Xp[:, 1] / Xz) + cyr - ys
@@ -89,6 +124,7 @@ def _pair(depth_r, depth_n, normal_r, gray_r, gray_n, cam_r, cam_n, tau, dtype, 
     idx = geo.nonzero().squeeze(1)
     n_w = normal_r.reshape(3, -1).T[idx]
     n_c = F.normalize(n_w @ Rr.T, dim=-1)
+    nlen = (n_w @ Rr.T).detach().norm(dim=-1)
     Xg = X[idx]
     d = (n_c * Xg).sum(-1)
     pok = d.abs() > MIN_Z
@@ -102,15 +138,19 @@ def _pair(depth_r, depth_n, normal_r, gray_r, gray_n, cam_r, cam_n, tau, dtype, 
     ixl, iyl = px.long(), py.long()
     Sa = Sb = Saa = Sbb = Sab = 0
     hz_min = torch.full_like(d, float("inf"))
+    hz_border = torch.full_like(d, float("inf"))      # |h.z - MIN_Z| over the magnitude of h.z's terms
+    tap_grid = torch.full_like(d, float("inf"))       # the warped taps' least margin to a grid line (see _grid)
     for ky in range(-3, 4):
         for kx in range(-3, 4):
             P = torch.stack([px + kx, py + ky, torch.ones_like(px)], -1)
             h = (Hm @ P[:, :, None]).squeeze(-1)
             hz_min = torch.minimum(hz_min, h[:, 2].detach())
+            hz_border = torch.minimum(hz_border, ((h[:, 2] - MIN_Z).abs() / (Hm[:, 2].abs() * P.abs()).sum(-1)).detach())
             hok = h[:, 2] > MIN_Z
             pok = pok & hok
             hz = _safe(hok, h[:, 2])
             b = bilinear(gray_n, h[:, 0] / hz, h[:, 1] / hz)
+            tap_grid = torch.minimum(tap_grid, torch.minimum(_grid(h[:, 0] / hz, W), _grid(h[:, 1] / hz, H)))
             a = gpad[iyl + 3 + ky, ixl + 3 + kx]
             Sa, Sb, Saa, Sbb, Sab = Sa + a, Sb + b, Saa + a * a, Sbb + b * b, Sab + a * b
     ma, mb = Sa / 49, Sb / 49
@@ -127,9 +167,18 @@ def _pair(depth_r, depth_n, normal_r, gray_r, gray_n, cam_r, cam_n, tau, dtype, 
     ncc_m = inf.clone().index_put((idx,), (1 - ncc).detach().abs())
     d_full = inf.clone().index_put((idx,), d.detach().abs())
     hz_full = inf.clone().index_put((idx,), hz_min)
+    # the other decision quantities, NaN where the pixel never reaches them
+    nan = torch.full_like(phi, float("nan")).detach()
+    on_geo = lambda v: nan.clone().index_put((idx,), v.detach())
+    reached = lambda mask, v: torch.where(mask, v.detach(), nan)
     return {"geo_c": geo_c, "photo_c": photo_c, "geo": geo, "photo": photo_full, "phi": phi.detach(),
             "pre_geo": pre_geo, "w": w, "q": torch.stack([qx, qy], -1).detach(), "qmargin": qmargin.detach(),
-            "Dn": Dn.detach(), "c": c_full, "ncc_margin": ncc_m, "d": d_full, "hz": hz_full}
+            "Dn": Dn.detach(), "c": c_full, "ncc_margin": ncc_m, "d": d_full, "hz": hz_full,
+            "q_raw": q_raw, "D": D_raw.detach(), "Y2": reached(D > 0, Y[:, 2]), "Dn_raw": reached(ok_q, Dn_raw),
+            "taps_le0": torch.where(ok_q, taps_le0, torch.zeros_like(taps_le0)), "P2": reached(ok_dn, Xp[:, 2]),
+            "d_signed": on_geo(d), "va": on_geo(va), "vb": on_geo(vb), "ncc": on_geo(ncc), "nlen": on_geo(nlen),
+            "hz_border": on_geo(hz_border),
+            "q_grid": torch.minimum(_grid(q_raw[:, 0], W), _grid(q_raw[:, 1], H)), "tap_grid": on_geo(tap_grid)}
 
 
 def consistency(depth, normal, gray, cams, pairs, tau=1.0, counts=None, info=False, weights=None):
@@ -159,6 +208,30 @@ def borderline(e, tau, W, H, delta=5e-4):
     pre = e["pre_geo"]
     g = (e["qmargin"].abs() < delta) | (pre & ((e["phi"] - tau).abs() < delta)) | (pre & (e["Dn"].abs() < delta))
     p = e["geo"] & (((e["c"] - MAX_COST).abs() < delta) | (e["d"] < 1e-5) | (e["hz"] < 1e-5))
+    return g, p
+
+
+def borderline_edges(e, tau, W, H, delta=5e-4):
+    """borderline() for adversarial maps: the same phi, q and c margins, and the decisions whose fp32 evaluation is
+    ill-conditioned rather than merely close, each measured against the scale of its own terms: Y.z and X'.z near
+    MIN_Z against the depth (the reprojection divides by them), D' near 0 against the depth (a tap next to a hole),
+    |d| near MIN_Z against the depth, and h.z near MIN_Z against its terms."""
+    pre = e["pre_geo"]
+    D = torch.where(e["D"] > 0, e["D"], torch.zeros_like(e["D"]))
+    near = lambda v, at, bound: torch.nan_to_num((v - at).abs(), nan=float("inf")) < bound
+    q = e["q_raw"]
+    margin = e["qmargin"].abs()
+    for axis, extent in ((0, W), (1, H)):      # a one-pixel axis has both bounds at 0: exactly 0 there is decided
+        if extent == 1:
+            other = q[:, 1 - axis]
+            rest = torch.minimum(other, (H if axis == 0 else W) - 1 - other).abs()
+            margin = torch.where(q[:, axis] == 0, rest if (H if axis == 0 else W) > 1 else torch.full_like(rest, 1.0),
+                                 margin)
+    g = (margin < delta) | (pre & ((e["phi"] - tau).abs() < delta)) | near(e["Y2"], MIN_Z, 1e-3 * D) \
+        | near(e["P2"], MIN_Z, 1e-3 * e["Dn_raw"].abs()) | near(e["Dn_raw"], 0.0, delta * D)
+    nc = (e["nlen"] / 1e-12).clamp(max=1.0)                    # |n_c|
+    p = e["geo"] & (((e["c"] - MAX_COST).abs() < delta) | near(e["d"], MIN_Z, 1e-6 * D * nc)
+                    | near(e["hz_border"], 0.0, 1e-5))
     return g, p
 
 

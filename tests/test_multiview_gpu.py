@@ -7,89 +7,11 @@ import pytest
 import torch
 
 import multiview_oracle as mo
+from multiview_check import DEV, TAU, _kernel, _settings, check_against_oracle
 from relightable3dgaussian_b200 import _lib, multiview, synth
 from relightable3dgaussian_b200 import rasterizer as R
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda")
-TAU = 1.0
-
-
-def _settings(cams, W, H):
-    return [R.GaussianRasterizationSettings(H, W, c.tanfovx, c.tanfovy, c.cx, c.cy, torch.zeros(3, device=DEV), 1.0,
-                                            c.viewmatrix.float().to(DEV), torch.eye(4, device=DEV), 0,
-                                            torch.zeros(3, device=DEV), False, True, True, False) for c in cams]
-
-
-def _kernel(depth, normal, gray, settings, pairs, cot):
-    """(geo, photo, counts, dL/ddepth, dL/dnormal) of the fused loss for the loss sum(geo * cot[0] + photo * cot[1])."""
-    d, n = depth.detach().clone().requires_grad_(), normal.detach().clone().requires_grad_()
-    view, cams, idx, tau = multiview._prepare(d, n, gray, settings, pairs, TAU)
-    geo, photo, counts = multiview._Consistency.apply(d, n, gray, view, cams, idx, tau)
-    gd, gn = torch.autograd.grad((geo * cot[0]).sum() + (photo * cot[1]).sum(), [d, n])
-    return geo.detach(), photo.detach(), counts, gd, gn
-
-
-def _oracle(depth, normal, gray, cams, pairs, cot, counts, dtype):
-    d = depth.detach().to(dtype).requires_grad_()
-    n = normal.detach().to(dtype).requires_grad_()
-    geo, photo, info = mo.consistency(d, n, gray.to(dtype), cams, pairs, TAU, counts=counts, info=True)
-    gd, gn = torch.autograd.grad((geo * cot[0].to(dtype)).sum() + (photo * cot[1].to(dtype)).sum(), [d, n],
-                                 allow_unused=True)
-    gd = torch.zeros_like(d) if gd is None else gd
-    gn = torch.zeros_like(n) if gn is None else gn
-    return geo.detach(), photo.detach(), gd, gn, info
-
-
-def _rel(a, b, keep):
-    fin = lambda t: torch.isfinite(t).reshape(*keep.shape, -1).all(-1)
-    keep = keep & fin(a) & fin(b)
-    a, b = a.double()[keep], b.double()[keep]
-    return float((a - b).norm() / b.norm().clamp_min(1e-300))
-
-
-def check_against_oracle(depth, normal, gray, cams, pairs, seed=0, border_budget=1e-3):
-    """Kernel vs fp64 oracle within max(1e-6, 4 e_ref) (+ the share of pixels on a decision boundary for the losses),
-    e_ref the fp32 oracle's own error; gradient maps in relative L2 off the boundary pixels."""
-    V, _, H, W = depth.shape
-    settings = _settings(cams, W, H)
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    B = len(pairs)
-    cot = (torch.rand(B, device=DEV, generator=g) + 0.5, torch.rand(B, device=DEV, generator=g) + 0.5)
-    kg, kp, counts, kgd, kgn = _kernel(depth, normal, gray, settings, pairs, cot)
-    cl = counts.cpu().tolist()
-    tg, tp, tgd, tgn, info = _oracle(depth, normal, gray, cams, pairs, cot, cl, torch.float64)
-    fg, fp, fgd, fgn, _ = _oracle(depth, normal, gray, cams, pairs, cot, cl, torch.float32)
-    keep_d = torch.ones(V, H * W, dtype=torch.bool, device=DEV)
-    keep_n = torch.ones(V, H * W, dtype=torch.bool, device=DEV)
-    for b, ((r, n), e) in enumerate(zip(pairs, info)):
-        gb, pb = mo.borderline(e, TAU, W, H)
-        if r != n:          # for (v, v) every edge pixel reprojects onto the image bound by construction
-            assert int((gb | pb).sum()) <= border_budget * H * W, (b, int(gb.sum()), int(pb.sum()))
-        allow_g = int(gb.sum()) * TAU / max(cl[b][0], 1)
-        allow_p = int((gb | pb).sum()) * mo.MAX_COST / max(cl[b][1], 1)
-        for k, t, f, allow in ((kg[b], tg[b], fg[b], allow_g), (kp[b], tp[b], fp[b], allow_p)):
-            e_ref = abs(float(f) - float(t))
-            assert abs(float(k) - float(t)) <= max(1e-6, 4 * e_ref) + allow, (b, float(k), float(t), e_ref, allow)
-        bad = gb | pb
-        keep_d[r] &= ~bad
-        keep_n[r] &= ~bad
-        q = e["q"][bad]
-        x0, y0 = q[:, 0].floor().long().clamp(0, W - 1), q[:, 1].floor().long().clamp(0, H - 1)
-        for dx in (0, 1):
-            for dy in (0, 1):
-                keep_d[n, (y0 + dy).clamp(max=H - 1) * W + (x0 + dx).clamp(max=W - 1)] = False
-    kd, td, fd = kgd.reshape(V, -1), tgd.reshape(V, -1), fgd.reshape(V, -1)
-    # where the fp32 formulation overflows (e.g. unbounded depths off a rendered silhouette) it has no error to compare
-    keep_d &= torch.isfinite(fd)
-    keep_n &= torch.isfinite(fgn.reshape(V, 3, -1)).all(1)
-    rk, rf = _rel(kd, td, keep_d), _rel(fd, td, keep_d)
-    assert rk <= max(1e-6, 4 * rf), ("depth", rk, rf)
-    kn, tn, fn = (t.reshape(V, 3, -1).transpose(1, 2) for t in (kgn, tgn, fgn))
-    rk, rf = _rel(kn, tn, keep_n), _rel(fn, tn, keep_n)
-    assert rk <= max(1e-6, 4 * rf), ("normal", rk, rf)
-    assert torch.isfinite(kgd).all() and torch.isfinite(kgn).all()
-    return kg, kp, counts
 
 
 def _dev(*ts):
