@@ -475,6 +475,93 @@ int r3dg_fit_incident_sh(int P, int N, const float* radiance, const float* norma
                          float* out, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * LIGHTS: point and directional lights on top of the environment light (DESIGN.md §4.26).
+ * Two operations: the shadow transmittance of every (Gaussian, light) pair through a built tree,
+ * and the lights' shading terms, forward and backward, for one view or several.  The caller adds
+ * the terms to the shading step's pbr, diffuse_light and specular before packing the features.
+ *   Light set.  K lights, 0 <= K <= R3DG_MAX_LIGHTS.  kind i32[K] is a HOST array: 0 directional,
+ *   1 point.  vec f32[K,3]: a directional light's direction TOWARDS the light (any non-zero length,
+ *   normalised as F.normalize, eps 1e-12), a point light's position.  color f32[K,3]: a directional
+ *   light's irradiance at normal incidence, a point light's intensity (divided by the squared
+ *   distance).  vec and color are device arrays.
+ *   Per Gaussian g (mean m, raw normal n) and light j:
+ *     directional: l = vec_j / max(|vec_j|, 1e-12),  E = color_j
+ *     point:       w = vec_j - m,  l = w / max(|w|, 1e-12),  E = color_j / max(|w|^2, 1e-8)
+ *       (1e-8 = R2_MIN: a light at a Gaussian's centre stays finite; |w|^2 is ((w0 w0 + w1 w1) + w2 w2)
+ *       and l, like the ray origin below, is rounded op by op, so both operations see the same bits)
+ *     transport = E * T[g,j] * max(n . l, 0),  f_s = GGX_specular(V, l) of the shading step (its clamps,
+ *     normal flipped towards the view), and the outputs are the sums over j in index order:
+ *       diffuse_light = sum transport,  specular = sum f_s transport,
+ *       pbr = sum (base_color / pi + f_s) transport.
+ *   This is the shading step's one incident sample along l with area 1, visibility T, global light E
+ *   and zero local light: a directional light equals rendering_equation with N = 1, incident_dirs = l,
+ *   incident_areas = 1, visibility = T, zero incidents and a constant env E.
+ *   Shadow T[g,j]: the ray from o = m + 0.05 l (the bake's offset, rounded op by op) along l, with
+ *   t_max = +inf for a directional light and |vec_j - o| for a point light.  A Gaussian is a hit when
+ *   it satisfies the bake's rule (opacity >= 1/255, not back-facing, peak t >= 0.01, power <= 0), its
+ *   peak t < (1 - 1e-5) t_max (so a Gaussian whose peak is at the light, e.g. with the light at its
+ *   centre, is clearly not a hit rather than a tie), and the segment [0, t_max] meets its leaf box.  T is the product of
+ *   (1 - opacity exp(power)) over the hits in the bake's traversal order (far child pushed first),
+ *   stopped once T < 1e-4 (T as reached).  No 0.9 threshold: shadows are continuous.  T carries no
+ *   gradient.  A light at a Gaussian's centre gives l = 0 and t_max = 0 there: no hit, T = 1.
+ * ------------------------------------------------------------------------------------------ */
+#define R3DG_MAX_LIGHTS 32
+
+size_t r3dg_bvh_trace_lights_tmp_bytes(int P);
+
+/* T f32[P,K] (row at the Gaussian's index, every element written) of a tree built over the same
+ * Gaussians: means3D [P,3], covs3D the INVERSE covariances [P,6], opacities [P], normals [P,3].
+ * Bitwise reproducible.  R3DG_ERR_BAD_ARG before any launch for P < 0, K outside 0..R3DG_MAX_LIGHTS,
+ * a kind other than 0 or 1, a NULL pointer the call needs or a tmp smaller than
+ * r3dg_bvh_trace_lights_tmp_bytes(P).  P = 0 or K = 0 launches nothing. */
+int r3dg_bvh_trace_lights(int P, int K, const int32_t* kind, const float* vec, const int32_t* nodes,
+                          const float* aabbs, const float* means3D, const float* covs3D, const float* opacities,
+                          const float* normals, float* shadows, void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+
+/* The lights' shading terms.  1 <= V <= R3DG_MAX_VIEWS views share the Gaussians, lights and shadows:
+ * viewdirs, pbr, diffuse_light, specular, their cotangents and dL_dviewdirs are [V,P,3] (view-major),
+ * and each view's outputs equal a one-view call's bit for bit.
+ * Forward: writes pbr, diffuse_light and specular.  Backward: from dL_dpbr (required) and
+ * dL_ddiffuse_light, dL_dspecular (NULL = zero) writes every element of dL_dbase_color [P,3],
+ * dL_droughness [P], dL_dviewdirs [V,P,3], dL_dmeans3D [P,3] (through l and |w| of the point
+ * lights), dL_dvec [K,3] and dL_dcolor [K,3]; the per-Gaussian gradients of shared inputs are the
+ * sums of the per-view gradients in view order.  Normals, shadows and kind get none.  The light
+ * gradients are per-CTA partials in `work` (r3dg_shade_lights_work_bytes(P, K)) summed in block
+ * order: no float atomics, every output is bitwise reproducible.  R3DG_ERR_BAD_ARG before any launch
+ * for P < 0, K outside 0..R3DG_MAX_LIGHTS, a kind other than 0 or 1, V outside 1..R3DG_MAX_VIEWS, a
+ * NULL pointer the call needs or a short workspace.  P = 0 or K = 0 launches no kernel and zero-fills
+ * the outputs that exist. */
+struct r3dg_light_args {
+    int P, K, V;
+    const int32_t* kind;          /* HOST [K] */
+    const float* vec;             /* [K,3] */
+    const float* color;           /* [K,3] */
+    const float* means3D;         /* [P,3] */
+    const float* base_color;      /* [P,3] */
+    const float* roughness;       /* [P] */
+    const float* normals;         /* [P,3] */
+    const float* viewdirs;        /* [V,P,3] */
+    const float* shadows;         /* [P,K] */
+    float* pbr;                   /* forward: [V,P,3] */
+    float* diffuse_light;         /* forward: [V,P,3] */
+    float* specular;              /* forward: [V,P,3] */
+    const float* dL_dpbr;         /* backward: [V,P,3] */
+    const float* dL_ddiffuse_light;
+    const float* dL_dspecular;
+    float* dL_dbase_color;
+    float* dL_droughness;
+    float* dL_dviewdirs;
+    float* dL_dmeans3D;
+    float* dL_dvec;
+    float* dL_dcolor;
+    void* work;                   /* backward */
+    size_t work_bytes;
+};
+size_t r3dg_shade_lights_work_bytes(int P, int K);
+int r3dg_shade_lights_forward(const struct r3dg_light_args* args, r3dg_stream_t stream);
+int r3dg_shade_lights_backward(const struct r3dg_light_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optional fused epilogue of the rasterizer call sites (SURVEY.md §8(f)2):
  *     feature / opacity.clamp_min(1e-5) * (num_contrib > 0)
  * (gaussian_renderer/neilf.py:135-137, render.py:106-108; 3 PyTorch kernels forward, ~6 backward).

@@ -84,6 +84,15 @@ class MultiviewArgs(ctypes.Structure):
                 [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
+class LightArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("P", "K", "V")] +
+                [(n, c_void_p) for n in ("kind", "vec", "color", "means3D", "base_color", "roughness", "normals", "viewdirs",
+                                         "shadows", "pbr", "diffuse_light", "specular", "dL_dpbr", "dL_ddiffuse_light",
+                                         "dL_dspecular", "dL_dbase_color", "dL_droughness", "dL_dviewdirs", "dL_dmeans3D",
+                                         "dL_dvec", "dL_dcolor", "work")] +
+                [("work_bytes", c_size_t)])
+
+
 class TsdfIntegrateArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("NX", "NY", "NZ")] + [("origin", c_float * 3)] +
                 [(n, c_float) for n in ("voxel_size", "sdf_trunc", "depth_trunc")] +
@@ -162,6 +171,12 @@ SYMBOLS = [
     ("r3dg_bvh_bake_radiance", c_int, [c_int, c_int] + [c_void_p] * 7 + [c_int, c_int, c_float] + [c_void_p] * 4 +
                                       [c_size_t, c_void_p]),
     ("r3dg_fit_incident_sh", c_int, [c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p]),
+    ("r3dg_bvh_trace_lights_tmp_bytes", c_size_t, [c_int]),
+    ("r3dg_bvh_trace_lights", c_int, [c_int, c_int] + [c_void_p] * 9 + [c_void_p, c_size_t, c_void_p]),
+    ("r3dg_shade_lights_work_bytes", c_size_t, [c_int, c_int]),
+    # `const struct r3dg_light_args*`: pass ctypes.byref(LightArgs(...))
+    ("r3dg_shade_lights_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_shade_lights_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_unpremultiply_forward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_unpremultiply_backward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_render_equation_forward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),

@@ -488,6 +488,35 @@ int r3dg_fit_incident_sh(int P, int N, const float* radiance, const float* norma
     return rc;
 }
 
+// ---- point and directional lights (lights.py) -----------------------------------------------
+size_t r3dg_bvh_trace_lights_tmp_bytes(int P) { return bvh_lights_tmp_bytes(P); }
+
+int r3dg_bvh_trace_lights(int P, int K, const int32_t* kind, const float* vec, const int32_t* nodes, const float* aabbs,
+                          const float* means3D, const float* covs3D, const float* opacities, const float* normals,
+                          float* shadows, void* tmp, size_t tmp_bytes, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_bvh_lights(P, K, kind, vec, nodes, aabbs, means3D, covs3D, opacities, normals, shadows, tmp, tmp_bytes,
+                                     num_sms(), (cudaStream_t)stream, &launched);
+    g_launches += launched ? 2 : 0;                       // pack, trace
+    return rc;
+}
+
+size_t r3dg_shade_lights_work_bytes(int P, int K) { return shade_lights_work_bytes(P, K); }
+
+int r3dg_shade_lights_forward(const r3dg_light_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_shade_lights_forward(args, (cudaStream_t)stream, &launched);
+    g_launches += launched ? 1 : 0;
+    return rc;
+}
+
+int r3dg_shade_lights_backward(const r3dg_light_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_shade_lights_backward(args, (cudaStream_t)stream, &launched);
+    g_launches += launched ? 2 : 0;                       // Gaussians, fixed-order light reduction
+    return rc;
+}
+
 int r3dg_unpremultiply_forward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
                                float* out, r3dg_stream_t stream) {
     if (S < 0 || HW < 0) return R3DG_ERR_BAD_ARG;

@@ -1,5 +1,5 @@
-// Device pieces shared by the BVH traces of bvh.cu (visibility) and indirect.cu (radiance): the packed
-// tree layout, the incident-direction generator, the slab test and the split ray stack.
+// Device pieces shared by the BVH traces of bvh.cu (visibility), indirect.cu (radiance) and lights_trace.cu (shadows):
+// the packed tree layout, the incident-direction generator, the slab test, the hit rule and the split ray stack.
 #pragma once
 #include <cstdio>
 #include "common.cuh"
@@ -26,8 +26,11 @@ __device__ __forceinline__ LeafRecord load_leaf(const float4* __restrict__ p) {
 // by the rounded reciprocal can differ from the quotient in the last bit, which only matters when a ray grazes a box
 // exactly; the tests bound the resulting visibility flip rate against the reference's own kernels (<= 1e-3).
 // Returns the exit distance, or -1 for a miss; a child is visited when the result is > 0.
+// SEG (the light traces, lights_trace.cu): -1 also when the box is entered beyond tseg, so a result > 0 means the
+// segment [0, tseg] of the ray meets the box; with tseg = +inf it is the plain test.
+template <bool SEG = false>
 __device__ __forceinline__ float ray_box_tmax(float b0, float b1, float b2, float b3, float b4, float b5,
-                                              float ox, float oy, float oz, float ix, float iy, float iz) {
+                                              float ox, float oy, float oz, float ix, float iy, float iz, float tseg = 0.f) {
     float tmin = mul_(sub_(b0, ox), ix), tmax = mul_(sub_(b3, ox), ix);
     if (tmin > tmax) { const float t = tmin; tmin = tmax; tmax = t; }
     float tymin = mul_(sub_(b1, oy), iy), tymax = mul_(sub_(b4, oy), iy);
@@ -39,7 +42,30 @@ __device__ __forceinline__ float ray_box_tmax(float b0, float b1, float b2, floa
     if (tzmin > tzmax) { const float t = tzmin; tzmin = tzmax; tzmax = t; }
     if (tmin > tzmax || tzmin > tmax) return -1.0f;
     if (tzmax < tmax) tmax = tzmax;
+    if (SEG) {
+        if (tzmin > tmin) tmin = tzmin;
+        if (tmin > tseg) return -1.0f;
+    }
     return tmax;
+}
+
+// The visibility trace's hit rule for the Gaussian of leaf record `q` on ray (o, d): opacity >= 1/255, not
+// back-facing, peak t >= 0.01 and power <= 0.  Same arithmetic as bvh_trace_kernel, so the bakes and the light
+// traces see one hit set.
+__device__ __forceinline__ bool gaussian_hit(const LeafRecord& q, float ox, float oy, float oz, float dx, float dy, float dz,
+                                             float& t, float& power) {
+    if ((q.op < 1.f / 255.f) || (q.nx * dx + q.ny * dy + q.nz * dz > 0)) return false;
+    const float c0 = q.c0, c1 = q.c1, c2 = q.c2, c3 = q.c3, c4 = q.c4, c5 = q.c5;
+    const float m0 = q.mx - ox, m1 = q.my - oy, m2 = q.mz - oz;
+    const float t1 = c0 * m0 * dx + c1 * m0 * dy + c2 * m0 * dz + c1 * m1 * dx + c3 * m1 * dy + c4 * m1 * dz +
+                     c2 * m2 * dx + c4 * m2 * dy + c5 * m2 * dz;
+    const float t2 = c0 * dx * dx + c1 * dx * dy + c2 * dx * dz + c1 * dy * dx + c3 * dy * dy + c4 * dy * dz +
+                     c2 * dz * dx + c4 * dz * dy + c5 * dz * dz;
+    t = t1 / t2;
+    if (t < 0.01f) return false;
+    const float e0 = q.mx - (ox + t * dx), e1 = q.my - (oy + t * dy), e2 = q.mz - (oz + t * dz);
+    power = -0.5f * (e0 * e0 * c0 + e1 * e1 * c3 + e2 * e2 * c5 + 2 * e0 * e1 * c1 + 2 * e0 * e2 * c2 + 2 * e1 * e2 * c4);
+    return !(power > 0);
 }
 
 // ---- incident-direction sampling (reference utils/graphics_utils.py:9-37 fibonacci_sphere_sampling with

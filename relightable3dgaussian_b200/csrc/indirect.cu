@@ -23,24 +23,6 @@ namespace r3dg {
 #define RAD_K 16                // k-buffer entries per round
 #define RAD_T_MIN 1e-4f         // a ray stops once its transmittance falls below this
 
-// The visibility trace's hit rule for the Gaussian of leaf record `q` on ray (o, d): opacity >= 1/255, not
-// back-facing, peak t >= 0.01 and power <= 0.  Same arithmetic as bvh_trace_kernel, so both bakes see one hit set.
-__device__ __forceinline__ bool gaussian_hit(const LeafRecord& q, float ox, float oy, float oz, float dx, float dy, float dz,
-                                             float& t, float& power) {
-    if ((q.op < 1.f / 255.f) || (q.nx * dx + q.ny * dy + q.nz * dz > 0)) return false;
-    const float c0 = q.c0, c1 = q.c1, c2 = q.c2, c3 = q.c3, c4 = q.c4, c5 = q.c5;
-    const float m0 = q.mx - ox, m1 = q.my - oy, m2 = q.mz - oz;
-    const float t1 = c0 * m0 * dx + c1 * m0 * dy + c2 * m0 * dz + c1 * m1 * dx + c3 * m1 * dy + c4 * m1 * dz +
-                     c2 * m2 * dx + c4 * m2 * dy + c5 * m2 * dz;
-    const float t2 = c0 * dx * dx + c1 * dx * dy + c2 * dx * dz + c1 * dy * dx + c3 * dy * dy + c4 * dy * dz +
-                     c2 * dz * dx + c4 * dz * dy + c5 * dz * dz;
-    t = t1 / t2;
-    if (t < 0.01f) return false;
-    const float e0 = q.mx - (ox + t * dx), e1 = q.my - (oy + t * dy), e2 = q.mz - (oz + t * dz);
-    power = -0.5f * (e0 * e0 * c0 + e1 * e1 * c3 + e2 * e2 * c5 + 2 * e0 * e1 * c1 + 2 * e0 * e2 * c2 + 2 * e1 * e2 * c4);
-    return !(power > 0);
-}
-
 // Ray r = (leaf slot r / N, sample r % N): rays in Morton order, results at the Gaussian's own row g * N + i.
 __global__ void __launch_bounds__(RAD_THREADS) bvh_radiance_kernel(int P, int N, const float4* __restrict__ packets,
                                                                    const int32_t* __restrict__ nodes,

@@ -141,6 +141,15 @@ int launch_bvh_radiance(int P, int N, const int32_t* nodes, const float* aabbs, 
                         size_t tmp_bytes, cudaStream_t stream);
 int launch_fit_incident_sh(int P, int N, const float* radiance, const float* normals, int degree, float ridge, float* out,
                            cudaStream_t stream);
+// lights_trace.cu / lights.cu: point and directional lights; every launcher validates its arguments before launching
+// anything and sets *launched when its kernels ran
+size_t bvh_lights_tmp_bytes(int P);
+int launch_bvh_lights(int P, int K, const int32_t* kind, const float* vec, const int32_t* nodes, const float* aabbs,
+                      const float* means3D, const float* covs3D, const float* opacities, const float* normals, float* shadows,
+                      void* tmp, size_t tmp_bytes, int num_sms, cudaStream_t stream, bool* launched);
+size_t shade_lights_work_bytes(int P, int K);
+int launch_shade_lights_forward(const r3dg_light_args* a, cudaStream_t stream, bool* launched);
+int launch_shade_lights_backward(const r3dg_light_args* a, cudaStream_t stream, bool* launched);
 int launch_unpremultiply_forward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
                                  float* out, int num_sms, cudaStream_t stream);
 int launch_unpremultiply_backward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,

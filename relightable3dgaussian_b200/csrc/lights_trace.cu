@@ -1,0 +1,138 @@
+// Shadow transmittance of point and directional lights through the LBVH (include/r3dg_b200.h, LIGHTS; DESIGN.md
+// §4.26).  One ray per (Gaussian, light): the visibility bake's packed tree, persistent warps refilled from a global
+// ray counter, traversal order (far child pushed first), slab test and hit rule, compiled with the bake's flags so
+// that a directional light's T is the bake's product bit for bit wherever the bake keeps it (T >= 0.9).  Differences
+// from the bake: a subtree is skipped when the ray's segment [0, t_max] misses its box (exact, because a hit must also
+// meet its own leaf box within the segment), hits need peak t < (1 - 1e-5) t_max, and the ray stops at T < 1e-4 instead of 0.9.
+#include <cmath>
+#include "bvh.cuh"
+#include "kernels.h"
+#include "lights.cuh"
+
+namespace r3dg {
+
+#define LT_THREADS 128
+#define LIGHT_T_MIN 1e-4f           // a shadow ray stops once its transmittance falls below this
+// A hit's peak t must lie below (1 - 1e-5) t_max: a Gaussian whose peak is at the light (the light at its centre) is
+// then clearly not a hit, instead of a tie that fp32 rounding decides
+#define LIGHT_T_MAX_MARGIN (1.0f - 1e-5f)
+
+// Ray r = (leaf slot r / K, light r % K): neighbouring lanes start from neighbouring Gaussians (Morton order).
+__global__ void __launch_bounds__(LT_THREADS) bvh_lights_kernel(int P, int K, const uint32_t point_mask, const float* __restrict__ vec,
+                                                                const float4* __restrict__ packets,
+                                                                const int32_t* __restrict__ nodes, float* __restrict__ shadows,
+                                                                unsigned long long* counter) {
+    __shared__ int sStack[TRACE_STACK_SH][LT_THREADS];
+    __shared__ float sVec[3 * R3DG_MAX_LIGHTS];
+    const int tid = threadIdx.x, lane = tid & 31;
+    for (int i = tid; i < 3 * K; i += LT_THREADS) sVec[i] = vec[i];
+    __syncthreads();
+    const int NI = P - 1;
+    const long long num_rays = (long long)P * K;
+    SplitStack<LT_THREADS> st;
+    st.sh = sStack; st.tid = tid; st.sp = 0;
+    bool has_ray = false, exhausted = false;
+    long long out = 0;
+    float ox = 0, oy = 0, oz = 0, dx = 0, dy = 0, dz = 0, ix = 0, iy = 0, iz = 0, tseg = 0, thit = 0, T = 1.0f;
+    while (true) {
+        // ---- refill idle lanes from the global ray counter (warp-aggregated), as the bake does ----
+        const unsigned want = __ballot_sync(0xffffffffu, !has_ray && !exhausted);
+        if (want) {
+            const int leader = __ffs(want) - 1;
+            unsigned long long base = 0;
+            if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(want));
+            base = __shfl_sync(0xffffffffu, base, leader);
+            if (!has_ray && !exhausted) {
+                const long long ray = (long long)base + __popc(want & ((1u << lane) - 1u));
+                if (ray < num_rays) {
+                    const long long slot = ray / K;
+                    const int j = (int)(ray - slot * K);
+                    const LeafRecord self = load_leaf(packets + (size_t)(NI + slot) * 4);
+                    const int kind = (point_mask >> j) & 1;
+                    const LightDir ld = light_dir(kind, sVec + 3 * j, self.mx, self.my, self.mz);
+                    dx = ld.l[0]; dy = ld.l[1]; dz = ld.l[2];
+                    ox = add_(self.mx, mul_(dx, LIGHT_ORIGIN_OFFSET));
+                    oy = add_(self.my, mul_(dy, LIGHT_ORIGIN_OFFSET));
+                    oz = add_(self.mz, mul_(dz, LIGHT_ORIGIN_OFFSET));
+                    if (kind == 0) {
+                        tseg = INFINITY; thit = INFINITY;
+                    } else {
+                        const float e0 = sub_(sVec[3 * j], ox), e1 = sub_(sVec[3 * j + 1], oy), e2 = sub_(sVec[3 * j + 2], oz);
+                        tseg = sqrt_(add_(add_(mul_(e0, e0), mul_(e1, e1)), mul_(e2, e2)));
+                        thit = mul_(tseg, LIGHT_T_MAX_MARGIN);
+                    }
+                    out = (long long)nodes[(size_t)(NI + slot) * 5 + 3] * K + j;
+                    ix = div_(1.0f, dx); iy = div_(1.0f, dy); iz = div_(1.0f, dz);
+                    has_ray = true; T = 1.0f;
+                    st.sp = 0; st.push(NI == 0 ? -1 : 0);         // root (a lone leaf when P == 1)
+                } else {
+                    exhausted = true;
+                }
+            }
+        }
+        if (!__any_sync(0xffffffffu, has_ray)) break;
+        // ---- a bounded burst of traversal steps, ended early once 8+ lanes can be refilled (the bake's policy) ----
+#pragma unroll 1
+        for (int step = 0; step < 32; ++step) {
+            if (step > 0 && (step & 3) == 0 && __popc(__ballot_sync(0xffffffffu, !has_ray && !exhausted)) >= 8) break;
+            if (!has_ray) continue;
+            const int node = st.pop();
+            if (node >= 0) {
+                const float4* p = packets + (size_t)node * 4;
+                const float4 p0 = p[0], p1 = p[1], p2 = p[2], p3 = p[3];
+                const int l = __float_as_int(p0.x), r = __float_as_int(p0.y);
+                const float lmax = ray_box_tmax<true>(p0.z, p0.w, p1.x, p1.y, p1.z, p1.w, ox, oy, oz, ix, iy, iz, tseg);
+                const float rmax = ray_box_tmax<true>(p2.x, p2.y, p2.z, p2.w, p3.x, p3.y, ox, oy, oz, ix, iy, iz, tseg);
+                if (lmax > rmax) {                                    // far child first
+                    if (lmax > 0) st.push(l);
+                    if (rmax > 0) st.push(r);
+                } else {
+                    if (rmax > 0) st.push(r);
+                    if (lmax > 0) st.push(l);
+                }
+            } else {
+                const LeafRecord q = load_leaf(packets + (size_t)(NI - node - 1) * 4);   // leaf slot = -node - 1
+                float t, power;
+                if (gaussian_hit(q, ox, oy, oz, dx, dy, dz, t, power) && t < thit) {
+                    const float alpha = q.op * __expf(power);
+                    T *= 1 - alpha;
+                    if (T < LIGHT_T_MIN) {
+                        shadows[out] = T;
+                        has_ray = false;
+                    }
+                }
+            }
+            if (has_ray && st.sp == 0) {
+                shadows[out] = T;
+                has_ray = false;
+            }
+        }
+    }
+}
+
+// ---- host launcher ------------------------------------------------------------------------
+size_t bvh_lights_tmp_bytes(int P) { return bvh_packets_bytes(P); }
+
+int launch_bvh_lights(int P, int K, const int32_t* kind, const float* vec, const int32_t* nodes, const float* aabbs,
+                      const float* means3D, const float* covs3D, const float* opacities, const float* normals, float* shadows,
+                      void* tmp, size_t tmp_bytes, int num_sms, cudaStream_t stream, bool* launched) {
+    *launched = false;
+    if (P < 0 || !lights_valid(K, kind)) return R3DG_ERR_BAD_ARG;
+    if (P == 0 || K == 0) return 0;
+    if (!vec || !nodes || !aabbs || !means3D || !covs3D || !opacities || !normals || !shadows || !tmp) return R3DG_ERR_BAD_ARG;
+    if (tmp_bytes < bvh_lights_tmp_bytes(P)) return R3DG_ERR_BAD_ARG;
+    unsigned long long* counter = (unsigned long long*)tmp;
+    float4* packets = (float4*)((char*)tmp + 256);
+    R3DG_CUDA_TRY(cudaMemsetAsync(counter, 0, 8, stream));
+    const int rc = launch_bvh_pack(P, nodes, aabbs, means3D, covs3D, opacities, normals, packets, stream);
+    if (rc != 0) return rc;
+    const long long num_rays = (long long)P * K;
+    const long long want = (num_rays + LT_THREADS - 1) / LT_THREADS;
+    const int blocks = (int)(want < (long long)num_sms * 16 ? want : (long long)num_sms * 16);
+    bvh_lights_kernel<<<blocks, LT_THREADS, 0, stream>>>(P, K, point_mask(K, kind), vec, packets, nodes, shadows, counter);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    *launched = true;
+    return 0;
+}
+
+}  // namespace r3dg

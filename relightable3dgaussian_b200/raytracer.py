@@ -15,6 +15,7 @@ Differences from the reference that are not observable in the results:
 Beyond the reference: `RayTracer.bake_radiance` / `fit_incident_sh` / `update_incidents` compute each Gaussian's
 incident-light SH (`incidents`) from the scene itself — the bake's rays composited front to back through the
 other Gaussians (r3dg_bvh_bake_radiance), then a per-Gaussian ridge fit (r3dg_fit_incident_sh).
+`RayTracer.trace_lights` traces the shadows of point and directional lights (lights.py).
 """
 import torch
 
@@ -134,6 +135,25 @@ class RayTracer:
                   ci.data_ptr(), op.data_ptr(), nr.data_ptr(), sh.data_ptr(), sh.shape[1], deg, 0.05,
                   out["radiance"].data_ptr(), out["transmittance"].data_ptr(), _lib.ptr(out.get("num_hits")),
                   tmp.data_ptr(), tmp.numel(), what="bake_radiance")
+        return out
+
+    @torch.no_grad()
+    def trace_lights(self, means3D, symm_inv, opacity, normals, lights):
+        """Shadow transmittance T [P,K] of every (Gaussian, light) pair of `lights` (lights.Lights) through this tree
+        (r3dg_bvh_trace_lights): the ray from mean + 0.05 l towards the light, the bake's hit rule, hits only before
+        a point light, T multiplied until it falls below 1e-4.  No gradient.  A static light is traced once and its T
+        reused for every view."""
+        P, K = means3D.shape[0], len(lights)
+        dev = means3D.device
+        if not all(t.is_cuda for t in (means3D, symm_inv, opacity, normals, lights.vec)):
+            raise RuntimeError("trace_lights runs on the GPU only (no CPU path)")
+        kind, vec = lights.kind, _lib.f32(lights.vec)
+        out = torch.empty((P, K), dtype=torch.float32, device=dev)
+        m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(normals)
+        tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_lights_tmp_bytes(P), dev)
+        _lib.call("r3dg_bvh_trace_lights", dev, P, K, kind.data_ptr() if K else None, _lib.ptr(vec), self.tree.data_ptr(),
+                  self.aabb.data_ptr(), m.data_ptr(), ci.data_ptr(), op.data_ptr(), nr.data_ptr(), _lib.ptr(out),
+                  tmp.data_ptr(), tmp.numel(), what="trace_lights")
         return out
 
 
