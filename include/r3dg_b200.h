@@ -562,6 +562,75 @@ int r3dg_shade_lights_forward(const struct r3dg_light_args* args, r3dg_stream_t 
 int r3dg_shade_lights_backward(const struct r3dg_light_args* args, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * COMPOSE: similarity transforms of Gaussian models, K objects in one launch (DESIGN.md §4.27).
+ *   Objects are contiguous row ranges: offsets is a HOST int32[K+1] with 0 = o[0] <= ... <= o[K] = P
+ *   (empty ranges allowed), 1 <= K <= R3DG_MAX_OBJECTS.  Object k has quat[k] (w,x,y,z), normalised
+ *   by the call as build_rotation does (q^ = q / |q|), R = R(q^) in build_rotation's convention,
+ *   translation t[k] and scale s[k] > 0.  For each row p of object k, on the stored parameters:
+ *     xyz' = s R xyz + t,  normal' = R normal (not renormalised),  rotation' = q^ (x) rotation
+ *     (the reference's quaternion_multiply order, not renormalised),  scaling' = scaling + log s,
+ *     sh'_l = D^l(R) sh_l for every band l >= 1 of each SH "rest" tensor [P,(L+1)^2-1,C]
+ *   where D^l is defined by  sum_m Y_lm(d) c'_m = sum_m Y_lm(R^T d) c_m  for every unit d, Y the
+ *   rasterizer's real SH basis (extended to l = 4 as the reference's eval_sh).  Up to
+ *   R3DG_COMPOSE_MAX_SH rest tensors per call, each with its own L (0..4; 0 = no coefficients) and
+ *   C (1 or 3).  Scale does not enter the SH.  D is built per CTA in fp64 from a generated table
+ *   (csrc/sh_rotation_table.cuh) and applied in fp32.
+ * Forward: one launch.  Backward: one launch plus a fixed-order finish; writes every element of the
+ * per-row input gradients (dL_dxyz ... dL_dsh) and the per-object pose gradients dL_dR [K,9]
+ * (row-major, w.r.t. R(q^) through xyz, normal and the SH), dL_dquat [K,4] (w.r.t. q^ through
+ * q^ (x) rotation only; the caller chains both through q^ = q / |q|), dL_dtranslation [K,3] and
+ * dL_dscale [K] (through xyz and log s).  The pose gradients are per-CTA partials in `work`
+ * (r3dg_compose_work_bytes(P, K)) summed in a fixed order: no float atomics, every output is
+ * bitwise reproducible.  An object with no rows gets zero pose gradients.
+ * R3DG_ERR_BAD_ARG before any launch for P < 0, K outside 1..R3DG_MAX_OBJECTS, offsets that do not
+ * rise from 0 to P, n_sh outside 0..R3DG_COMPOSE_MAX_SH, L outside 0..4, C other than 1 or 3, a
+ * missing pointer the call needs or a short workspace.  P = 0 launches nothing (the backward
+ * zero-fills the pose gradients).
+ * ------------------------------------------------------------------------------------------ */
+#define R3DG_MAX_OBJECTS 64
+#define R3DG_COMPOSE_MAX_SH 3
+
+struct r3dg_compose_args {
+    int P, K;
+    const int32_t* offsets;       /* HOST [K+1] */
+    const float* quat;            /* [K,4] */
+    const float* translation;     /* [K,3] */
+    const float* scale;           /* [K] */
+    const float* xyz;             /* [P,3] */
+    const float* normal;          /* [P,3] */
+    const float* rotation;        /* [P,4] */
+    const float* scaling;         /* [P,3] log-scales */
+    int n_sh;
+    int sh_degree[3];
+    int sh_channels[3];
+    const float* sh[3];           /* [P,(L+1)^2-1,C] */
+    float* xyz_out;               /* forward */
+    float* normal_out;
+    float* rotation_out;
+    float* scaling_out;
+    float* sh_out[3];
+    const float* dL_dxyz_out;     /* backward: cotangents of the outputs */
+    const float* dL_dnormal_out;
+    const float* dL_drotation_out;
+    const float* dL_dscaling_out;
+    const float* dL_dsh_out[3];
+    float* dL_dxyz;               /* backward: gradients of the inputs */
+    float* dL_dnormal;
+    float* dL_drotation;
+    float* dL_dscaling;
+    float* dL_dsh[3];
+    float* dL_dR;                 /* [K,9] */
+    float* dL_dquat;              /* [K,4] */
+    float* dL_dtranslation;       /* [K,3] */
+    float* dL_dscale;             /* [K] */
+    void* work;                   /* backward */
+    size_t work_bytes;
+};
+size_t r3dg_compose_work_bytes(int P, int K);
+int r3dg_compose_forward(const struct r3dg_compose_args* args, r3dg_stream_t stream);
+int r3dg_compose_backward(const struct r3dg_compose_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Optional fused epilogue of the rasterizer call sites (SURVEY.md §8(f)2):
  *     feature / opacity.clamp_min(1e-5) * (num_contrib > 0)
  * (gaussian_renderer/neilf.py:135-137, render.py:106-108; 3 PyTorch kernels forward, ~6 backward).

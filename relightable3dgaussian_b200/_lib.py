@@ -93,6 +93,18 @@ class LightArgs(ctypes.Structure):
                 [("work_bytes", c_size_t)])
 
 
+class ComposeArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("P", "K")] +
+                [(n, c_void_p) for n in ("offsets", "quat", "translation", "scale", "xyz", "normal", "rotation", "scaling")] +
+                [("n_sh", c_int), ("sh_degree", c_int * 3), ("sh_channels", c_int * 3), ("sh", c_void_p * 3)] +
+                [(n, c_void_p) for n in ("xyz_out", "normal_out", "rotation_out", "scaling_out")] + [("sh_out", c_void_p * 3)] +
+                [(n, c_void_p) for n in ("dL_dxyz_out", "dL_dnormal_out", "dL_drotation_out", "dL_dscaling_out")] +
+                [("dL_dsh_out", c_void_p * 3)] +
+                [(n, c_void_p) for n in ("dL_dxyz", "dL_dnormal", "dL_drotation", "dL_dscaling")] + [("dL_dsh", c_void_p * 3)] +
+                [(n, c_void_p) for n in ("dL_dR", "dL_dquat", "dL_dtranslation", "dL_dscale", "work")] +
+                [("work_bytes", c_size_t)])
+
+
 class TsdfIntegrateArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("NX", "NY", "NZ")] + [("origin", c_float * 3)] +
                 [(n, c_float) for n in ("voxel_size", "sdf_trunc", "depth_trunc")] +
@@ -177,6 +189,10 @@ SYMBOLS = [
     # `const struct r3dg_light_args*`: pass ctypes.byref(LightArgs(...))
     ("r3dg_shade_lights_forward", c_int, [c_void_p, c_void_p]),
     ("r3dg_shade_lights_backward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_compose_work_bytes", c_size_t, [c_int, c_int]),
+    # `const struct r3dg_compose_args*`: pass ctypes.byref(ComposeArgs(...))
+    ("r3dg_compose_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_compose_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_unpremultiply_forward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_unpremultiply_backward", c_int, [c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("r3dg_render_equation_forward", c_int, [ctypes.POINTER(ShadeArgs), c_void_p]),

@@ -517,6 +517,23 @@ int r3dg_shade_lights_backward(const r3dg_light_args* args, r3dg_stream_t stream
     return rc;
 }
 
+// ---- similarity transforms of Gaussian models (compose.py) --------------------------------------
+size_t r3dg_compose_work_bytes(int P, int K) { return compose_work_bytes(P, K); }
+
+int r3dg_compose_forward(const r3dg_compose_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_compose_forward(args, (cudaStream_t)stream, &launched);
+    g_launches += launched ? 1 : 0;
+    return rc;
+}
+
+int r3dg_compose_backward(const r3dg_compose_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_compose_backward(args, (cudaStream_t)stream, &launched);
+    g_launches += launched ? 2 : 0;                       // rows, fixed-order pose reduction
+    return rc;
+}
+
 int r3dg_unpremultiply_forward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
                                float* out, r3dg_stream_t stream) {
     if (S < 0 || HW < 0) return R3DG_ERR_BAD_ARG;

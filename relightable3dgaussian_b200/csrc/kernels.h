@@ -150,6 +150,10 @@ int launch_bvh_lights(int P, int K, const int32_t* kind, const float* vec, const
 size_t shade_lights_work_bytes(int P, int K);
 int launch_shade_lights_forward(const r3dg_light_args* a, cudaStream_t stream, bool* launched);
 int launch_shade_lights_backward(const r3dg_light_args* a, cudaStream_t stream, bool* launched);
+// compose.cu: similarity transforms of Gaussian models; validates before launching, sets *launched when kernels ran
+size_t compose_work_bytes(int P, int K);
+int launch_compose_forward(const r3dg_compose_args* a, cudaStream_t stream, bool* launched);
+int launch_compose_backward(const r3dg_compose_args* a, cudaStream_t stream, bool* launched);
 int launch_unpremultiply_forward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
                                  float* out, int num_sms, cudaStream_t stream);
 int launch_unpremultiply_backward(int S, long long HW, const float* feature, const float* opacity, const int32_t* n_contrib,
