@@ -232,7 +232,11 @@ int r3dg_raster_forward(const r3dg_raster_fwd_args* a, r3dg_stream_t stream_) {
                             a->binning_bytes, b, V, a->ray_depth != 0, a->depth_stats != 0);
     if (rc != 0) return rc;
     if (a->deterministic && (!a->det_work || a->det_work_bytes < r3dg_raster_fwd_det_bytes(V * a->P))) return R3DG_ERR_BAD_ARG;
-    if (V > 1 && (b.gx > 65535 || b.gy > 65535 || b.tiles > 65535)) return R3DG_ERR_UNSUPPORTED;   // the binning's limits, before any launch
+    if (a->P > 0) {                                       // the binning's limits, before any launch
+        if ((rc = check_binning_limits(b)) != 0) return rc;
+    } else if (V > 1 && (b.gx > 65535 || b.gy > 65535 || b.tiles > 65535)) {
+        return R3DG_ERR_UNSUPPORTED;                      // (P == 0: only the tile order of several views runs)
+    }
     R3DG_CUDA_TRY(cudaMemsetAsync(b.header, 0, V * sizeof(GeomHeader), stream));
     auto mark = [](int i, cudaStream_t s) { prof_mark(true, i, s); };
     auto no_mark = [](int, cudaStream_t) {};

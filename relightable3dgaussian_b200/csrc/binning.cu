@@ -466,19 +466,32 @@ int launch_rebuild_keys(int T, const void* ranges, const uint32_t* point_list, c
     return 0;
 }
 
+// shared memory of bin_scatter: the per-tile array, the per-warp bitmaps, the per-position ids and block
+// rectangles + a staging area of up to 12 entries per Gaussian, as far as it fits (>= CH entries, since one tile
+// can receive every Gaussian of the chunk); a copy of the chunk's first slots per tile where that still leaves the
+// full staging area (up to 1080p tile counts), otherwise step 3 reads them from M.  A larger staging area is
+// slower at the headline: it spares the few heaviest chunks a second window but leaves less of the SM's
+// L1 / shared-memory split to L1.
+constexpr size_t kBinSmemMax = 220 * 1024;                // + ~5 KB static
+static size_t bin_tile_bytes(int T) { return (((size_t)T + 3) & ~(size_t)3) * 4; }
+static size_t bin_table_bytes(int T, int CH) {
+    return bin_tile_bytes(T) + (size_t)(BIN_SCATTER_THREADS / 32) * 2 * ((CH + 31) / 32) * 4 + (size_t)CH * 12;
+}
+
+int check_binning_limits(const RasterBuffers& b) {
+    const int CH = b.chunk_len;
+    if (b.gx > 65535 || b.gy > 65535 || b.tiles > 65535 || CH > 65536 ||
+        bin_table_bytes(b.tiles, CH) + (size_t)CH * 4 > kBinSmemMax) return R3DG_ERR_UNSUPPORTED;
+    return 0;
+}
+
 int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stream, stage_mark_fn mark,
                    int* num_rendered_host, void* count_ready_event) {
-    const int gx = b.gx, gy = b.gy, T = b.tiles, CH = b.chunk_len, chunks = b.chunks;
-    // shared memory of bin_scatter: the per-tile array, the per-warp bitmaps, the per-position ids and block
-    // rectangles + a staging area of up to 12 entries per Gaussian, as far as it fits (>= CH entries, since one tile
-    // can receive every Gaussian of the chunk); a copy of the chunk's first slots per tile where that still leaves the
-    // full staging area (up to 1080p tile counts), otherwise step 3 reads them from M.  A larger staging area is
-    // slower at the headline: it spares the few heaviest chunks a second window but leaves less of the SM's
-    // L1 / shared-memory split to L1.
-    const size_t smem_max = 220 * 1024;                   // + ~5 KB static
-    const size_t tile_bytes = (((size_t)T + 3) & ~(size_t)3) * 4;
-    size_t tbl_bytes = tile_bytes + (size_t)(BIN_SCATTER_THREADS / 32) * 2 * ((CH + 31) / 32) * 4 + (size_t)CH * 12;
-    if (gx > 65535 || gy > 65535 || T > 65535 || CH > 65536 || tbl_bytes + (size_t)CH * 4 > smem_max) return R3DG_ERR_UNSUPPORTED;
+    const int gx = b.gx, T = b.tiles, CH = b.chunk_len, chunks = b.chunks;
+    if (int rc = check_binning_limits(b)) return rc;
+    const size_t smem_max = kBinSmemMax;
+    const size_t tile_bytes = bin_tile_bytes(T);
+    size_t tbl_bytes = bin_table_bytes(T, CH);
     const size_t full_stage = std::min<size_t>((size_t)CH * 12, (size_t)BIN_MAX_LONG * BIN_LONG_RUN);
     const int starts_in_smem = tbl_bytes + tile_bytes + full_stage * 4 <= smem_max ? 1 : 0;
     if (starts_in_smem) tbl_bytes += tile_bytes;

@@ -70,6 +70,8 @@ int launch_sort(void* geom_header, char* buf, const SortLayout& sl, long long n,
 // tile_order, zeroed bwd_work.  launch_empty_binning: the same per-tile outputs for P == 0 (all lists empty).
 int launch_binning(int P, const RasterBuffers& b, int num_sms, cudaStream_t stream, stage_mark_fn mark,
                    int* num_rendered_host, void* count_ready_event);
+// R3DG_ERR_UNSUPPORTED when launch_binning cannot bin this tile grid / chunk length (launches nothing), else 0
+int check_binning_limits(const RasterBuffers& b);
 int launch_empty_binning(const RasterBuffers& b, cudaStream_t stream);
 // the compositors' tile order over all V * tiles tiles of the tall grid (and zeroed bwd_work), after every view's binning
 int launch_tile_order(const RasterBuffers& b, cudaStream_t stream);

@@ -94,8 +94,8 @@ def _axis_points(n, g, W, H, tanfovx, z, margin=0.9):
     return torch.stack([u[:, 0] * tanfovx * z, u[:, 1] * tanfovy * z, z], dim=1)
 
 
-def _edge_scene(name):
-    """-> (Scene-like dict of torch inputs, Camera, S).  See EDGE_CASES."""
+def _edge_scene(name, P=None):
+    """-> (Scene-like dict of torch inputs, Camera, S).  See EDGE_CASES.  `P` overrides the size of a depth case."""
     family, _, arg = name.partition("-")
     g = torch.Generator().manual_seed(sum(map(ord, name)))
     if family == "inside":                                  # camera inside a cube of random Gaussians
@@ -123,7 +123,7 @@ def _edge_scene(name):
         return dict(means3D=means, opacities=opac, shs=sc.shs, scales=scales, rotations=sc.rotations,
                     features=sc.features), synth.make_camera(1, 208, 144), S
     if family == "depth":                                   # depth-key bit patterns of every radix-sort plan
-        P, W, H = 6_500, 128, 96
+        P, W, H = P or 6_500, 128, 96
         cam = synth.make_axis_camera(W, H)
         z = {"equal": torch.full((P,), 2.0),
              "adjacent": torch.where(torch.rand(P, generator=g) < 0.5, torch.tensor(2.0),
@@ -199,9 +199,10 @@ EDGE_CASES = (["inside-x1", "inside-x0.6", "inside-x1.8", "needles", "opaque-S0"
               ["precomp"])
 
 
-def edge_case(name):
-    """Seeded inputs of one EDGE_CASES entry as numpy arrays: (oracle / run_ours keyword arguments, cotangents)."""
-    d, cam, S = _edge_scene(name)
+def edge_case(name, P=None):
+    """Seeded inputs of one EDGE_CASES entry as numpy arrays: (oracle / run_ours keyword arguments, cotangents).
+    `P` overrides the size of a depth case (the default is the fixture's)."""
+    d, cam, S = _edge_scene(name, P)
     bg = torch.tensor([0.0, 0.5, 1.0])
     kw = dict(means3D=d["means3D"], opacities=d["opacities"], viewmatrix=cam.viewmatrix, projmatrix=cam.projmatrix,
               campos=cam.campos, bg=bg, W=cam.image_width, H=cam.image_height, tan_fovx=cam.tanfovx,
