@@ -562,6 +562,109 @@ int r3dg_shade_lights_forward(const struct r3dg_light_args* args, r3dg_stream_t 
 int r3dg_shade_lights_backward(const struct r3dg_light_args* args, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * SHAPED LIGHTS: spot and rectangular area lights with soft shadows (DESIGN.md §4.28).
+ * The same two operations as LIGHTS (shadow trace, shading terms forward and backward) over a
+ * set of K lights, 0 <= K <= R3DG_MAX_LIGHTS, each a spot (kind 2) or a rect (kind 3).  kind i32[K]
+ * is a HOST array.  Device arrays, packed per light j:
+ *   pos f32[K,3]    spot: position;  rect: centre
+ *   a   f32[K,3]    spot: axis, the direction the light points (any non-zero length, normalised
+ *                   with eps 1e-12);  rect: half-edge vector u
+ *   b   f32[K,3]    rect: half-edge vector v;  unused by a spot
+ *   color f32[K,3]  spot: intensity;  rect: radiance
+ *   cone f32[K,2]   spot: (cos_inner, cos_outer);  unused by a rect
+ * Unused fields are not read (they may be NULL when no light of the set reads them) and get a zero
+ * gradient.  M (1..R3DG_MAX_RECT_SAMPLES) and the seed are per set.
+ *   Per Gaussian g (row index g, mean m, raw normal n) and light j:
+ *     spot:  w = pos - m,  l = w / max(|w|, 1e-12) (exactly a point light's l),
+ *            x = clamp((-l . a^ - cos_outer) / max(cos_inner - cos_outer, 1e-6), 0, 1),
+ *            E = color * x^2 (3 - 2x) / max(|w|^2, 1e-8);  one shadow ray, a point light's at pos.
+ *     rect:  a one-sided parallelogram y(s,t) = pos + s u + t v, s,t in [-1,1], emitting along
+ *            n_e = normalize(u x v), area A = 4 |u x v|.  M x M stratified samples (i,k),
+ *            sample index q = i M + k:  s = -1 + (2i + 2 xi1) / M,  t = -1 + (2k + 2 xi2) / M
+ *            (xi in [0,1) spans the whole stratum of width 2/M),
+ *            y_q = (pos + s u) + t v,  w_q = y_q - m,  l_q = w_q / max(|w_q|, 1e-12),
+ *            E_q = color * max(-n_e . l_q, 0) A / (M^2 max(|w_q|^2, 1e-8)).
+ *            A degenerate rect (u x v = 0) contributes 0 with finite gradients.
+ *     xi: h = lowbias32(lowbias32(lowbias32(seed) ^ g) ^ j) and xi1 = (lowbias32(h ^ 2q) >> 8) 2^-24,
+ *         xi2 = (lowbias32(h ^ (2q + 1)) >> 8) 2^-24, with lowbias32(x): x ^= x >> 16;
+ *         x *= 0x7feb352d; x ^= x >> 15; x *= 0x846ca68b; x ^= x >> 16 (u32 arithmetic).  g is
+ *         the Gaussian's row, so the trace and the shading see the same points.  s, t, y, w and l
+ *         are rounded op by op in that order (one IEEE op each), identically in both operations.
+ *   Rays: light j owns the columns [r_j, r_j + n_j) of the shadows T f32[P,R], n_j = 1 (spot) or
+ *   M^2 (rect, column r_j + q), R = sum n_j <= R3DG_MAX_SHAPED_RAYS.
+ *   Outputs, summed in light order, then sample order, with transport = E T max(n . l, 0) and f_s
+ *   the shading step's GGX along l (LIGHTS): diffuse_light = sum transport,
+ *   specular = sum f_s transport, pbr = sum (base_color / pi + f_s) transport.
+ *   Shadow T: the LIGHTS trace of a point light at the ray's target (pos, or y_q): origin
+ *   o = m + 0.05 l, t_max = |target - o|, the same hit rule, margin and T < 1e-4 stop.
+ *   Gradients are those of the estimator at fixed T and fixed (s,t): the rect's flow through y_q,
+ *   A and n_e.  Visibility-boundary terms (T's dependence on the light) are not included.
+ * ------------------------------------------------------------------------------------------ */
+#define R3DG_MAX_RECT_SAMPLES 8
+#define R3DG_MAX_SHAPED_RAYS 256
+
+/* The light set and the Gaussians of both operations.  Trace reads P, K, M, seed, kind, pos, a, b,
+ * means3D and normals.  Forward additionally reads V, color, cone, base_color, roughness,
+ * viewdirs [V,P,3] and shadows [P,R], and writes pbr, diffuse_light, specular [V,P,3].  Backward
+ * from dL_dpbr (required) and dL_ddiffuse_light, dL_dspecular (NULL = zero) writes every element of
+ * dL_dbase_color [P,3], dL_droughness [P], dL_dviewdirs [V,P,3], dL_dmeans3D [P,3], dL_dpos,
+ * dL_da, dL_db, dL_dcolor [K,3] and dL_dcone [K,2]; per-Gaussian gradients of shared inputs are
+ * the sums of the per-view gradients in view order, and each view's outputs equal a one-view
+ * call's bit for bit.  Normals, shadows, kind and seed get none.  The light gradients are per-CTA
+ * partials in `work` (r3dg_shade_shaped_lights_work_bytes(P, K)) summed in block order: no float
+ * atomics, every output is bitwise reproducible.  R3DG_ERR_BAD_ARG before any launch for P < 0,
+ * K outside 0..R3DG_MAX_LIGHTS, a kind other than 2 or 3, M outside 1..R3DG_MAX_RECT_SAMPLES,
+ * R > R3DG_MAX_SHAPED_RAYS, V outside 1..R3DG_MAX_VIEWS (shading), a NULL pointer the call needs or
+ * a short workspace.  P = 0 or K = 0 launches no kernel and zero-fills the outputs that exist. */
+struct r3dg_shaped_light_args {
+    int P, K, V, M;
+    uint32_t seed;
+    const int32_t* kind;          /* HOST [K] */
+    const float* pos;             /* [K,3] */
+    const float* a;               /* [K,3] */
+    const float* b;               /* [K,3] */
+    const float* color;           /* [K,3] */
+    const float* cone;            /* [K,2] */
+    const float* means3D;         /* [P,3] */
+    const float* base_color;      /* [P,3] */
+    const float* roughness;       /* [P] */
+    const float* normals;         /* [P,3] */
+    const float* viewdirs;        /* [V,P,3] */
+    const float* shadows;         /* [P,R] */
+    float* pbr;                   /* forward: [V,P,3] */
+    float* diffuse_light;         /* forward: [V,P,3] */
+    float* specular;              /* forward: [V,P,3] */
+    const float* dL_dpbr;         /* backward: [V,P,3] */
+    const float* dL_ddiffuse_light;
+    const float* dL_dspecular;
+    float* dL_dbase_color;
+    float* dL_droughness;
+    float* dL_dviewdirs;
+    float* dL_dmeans3D;
+    float* dL_dpos;
+    float* dL_da;
+    float* dL_db;
+    float* dL_dcolor;
+    float* dL_dcone;
+    void* work;                   /* backward */
+    size_t work_bytes;
+};
+
+/* R of a set (-1 for a bad set); the trace's tmp size */
+int r3dg_shaped_lights_num_rays(int K, const int32_t* kind, int M);
+size_t r3dg_bvh_trace_shaped_lights_tmp_bytes(int P);
+
+/* T f32[P,R] (row at the Gaussian's index, every element written) of a tree built over the same
+ * Gaussians (args->means3D), with covs3D the INVERSE covariances [P,6] and opacities [P]. */
+int r3dg_bvh_trace_shaped_lights(const struct r3dg_shaped_light_args* args, const int32_t* nodes, const float* aabbs,
+                                 const float* covs3D, const float* opacities, float* shadows, void* tmp,
+                                 size_t tmp_bytes, r3dg_stream_t stream);
+
+size_t r3dg_shade_shaped_lights_work_bytes(int P, int K);
+int r3dg_shade_shaped_lights_forward(const struct r3dg_shaped_light_args* args, r3dg_stream_t stream);
+int r3dg_shade_shaped_lights_backward(const struct r3dg_shaped_light_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * COMPOSE: similarity transforms of Gaussian models, K objects in one launch (DESIGN.md §4.27).
  *   Objects are contiguous row ranges: offsets is a HOST int32[K+1] with 0 = o[0] <= ... <= o[K] = P
  *   (empty ranges allowed), 1 <= K <= R3DG_MAX_OBJECTS.  Object k has quat[k] (w,x,y,z), normalised

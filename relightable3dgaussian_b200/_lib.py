@@ -93,6 +93,16 @@ class LightArgs(ctypes.Structure):
                 [("work_bytes", c_size_t)])
 
 
+class ShapedLightArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("P", "K", "V", "M")] + [("seed", ctypes.c_uint32)] +
+                [(n, c_void_p) for n in ("kind", "pos", "a", "b", "color", "cone", "means3D", "base_color", "roughness",
+                                         "normals", "viewdirs", "shadows", "pbr", "diffuse_light", "specular", "dL_dpbr",
+                                         "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color", "dL_droughness",
+                                         "dL_dviewdirs", "dL_dmeans3D", "dL_dpos", "dL_da", "dL_db", "dL_dcolor",
+                                         "dL_dcone", "work")] +
+                [("work_bytes", c_size_t)])
+
+
 class ComposeArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("P", "K")] +
                 [(n, c_void_p) for n in ("offsets", "quat", "translation", "scale", "xyz", "normal", "rotation", "scaling")] +
@@ -189,6 +199,13 @@ SYMBOLS = [
     # `const struct r3dg_light_args*`: pass ctypes.byref(LightArgs(...))
     ("r3dg_shade_lights_forward", c_int, [c_void_p, c_void_p]),
     ("r3dg_shade_lights_backward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_shaped_lights_num_rays", c_int, [c_int, c_void_p, c_int]),
+    ("r3dg_bvh_trace_shaped_lights_tmp_bytes", c_size_t, [c_int]),
+    # `const struct r3dg_shaped_light_args*`: pass ctypes.byref(ShapedLightArgs(...))
+    ("r3dg_bvh_trace_shaped_lights", c_int, [c_void_p] * 7 + [c_size_t, c_void_p]),
+    ("r3dg_shade_shaped_lights_work_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_shade_shaped_lights_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_shade_shaped_lights_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_compose_work_bytes", c_size_t, [c_int, c_int]),
     # `const struct r3dg_compose_args*`: pass ctypes.byref(ComposeArgs(...))
     ("r3dg_compose_forward", c_int, [c_void_p, c_void_p]),

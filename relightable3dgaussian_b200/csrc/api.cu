@@ -521,6 +521,37 @@ int r3dg_shade_lights_backward(const r3dg_light_args* args, r3dg_stream_t stream
     return rc;
 }
 
+// ---- spot and rect lights (lights.py, ShapedLights) ---------------------------------------------
+int r3dg_shaped_lights_num_rays(int K, const int32_t* kind, int M) { return shaped_num_rays(K, kind, M); }
+
+size_t r3dg_bvh_trace_shaped_lights_tmp_bytes(int P) { return bvh_lights_tmp_bytes(P); }
+
+int r3dg_bvh_trace_shaped_lights(const r3dg_shaped_light_args* args, const int32_t* nodes, const float* aabbs,
+                                 const float* covs3D, const float* opacities, float* shadows, void* tmp, size_t tmp_bytes,
+                                 r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_bvh_shaped_lights(args, nodes, aabbs, covs3D, opacities, shadows, tmp, tmp_bytes, num_sms(),
+                                            (cudaStream_t)stream, &launched);
+    g_launches += launched ? 2 : 0;                       // pack, trace
+    return rc;
+}
+
+size_t r3dg_shade_shaped_lights_work_bytes(int P, int K) { return shade_shaped_lights_work_bytes(P, K); }
+
+int r3dg_shade_shaped_lights_forward(const r3dg_shaped_light_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_shade_shaped_lights_forward(args, (cudaStream_t)stream, &launched);
+    g_launches += launched ? 1 : 0;
+    return rc;
+}
+
+int r3dg_shade_shaped_lights_backward(const r3dg_shaped_light_args* args, r3dg_stream_t stream) {
+    bool launched = false;
+    const int rc = launch_shade_shaped_lights_backward(args, (cudaStream_t)stream, &launched);
+    g_launches += launched ? 2 : 0;                       // Gaussians, per-light reduction
+    return rc;
+}
+
 // ---- similarity transforms of Gaussian models (compose.py) --------------------------------------
 size_t r3dg_compose_work_bytes(int P, int K) { return compose_work_bytes(P, K); }
 

@@ -152,6 +152,14 @@ int launch_bvh_lights(int P, int K, const int32_t* kind, const float* vec, const
 size_t shade_lights_work_bytes(int P, int K);
 int launch_shade_lights_forward(const r3dg_light_args* a, cudaStream_t stream, bool* launched);
 int launch_shade_lights_backward(const r3dg_light_args* a, cudaStream_t stream, bool* launched);
+// lights_trace.cu / lights.cu: spot and rect lights (SHAPED LIGHTS), validated the same way
+int shaped_num_rays(int K, const int32_t* kind, int M);
+int launch_bvh_shaped_lights(const r3dg_shaped_light_args* a, const int32_t* nodes, const float* aabbs, const float* covs3D,
+                             const float* opacities, float* shadows, void* tmp, size_t tmp_bytes, int num_sms,
+                             cudaStream_t stream, bool* launched);
+size_t shade_shaped_lights_work_bytes(int P, int K);
+int launch_shade_shaped_lights_forward(const r3dg_shaped_light_args* a, cudaStream_t stream, bool* launched);
+int launch_shade_shaped_lights_backward(const r3dg_shaped_light_args* a, cudaStream_t stream, bool* launched);
 // compose.cu: similarity transforms of Gaussian models; validates before launching, sets *launched when kernels ran
 size_t compose_work_bytes(int P, int K);
 int launch_compose_forward(const r3dg_compose_args* a, cudaStream_t stream, bool* launched);

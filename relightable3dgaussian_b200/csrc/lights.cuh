@@ -1,7 +1,8 @@
 // Point and directional lights (include/r3dg_b200.h, LIGHTS): the light geometry shared by the shadow trace
 // (lights_trace.cu) and the shading kernels (lights.cu).  Both must see the same direction l for a (Gaussian, light)
 // pair, but the two files are compiled with different contraction settings (the trace with the bake's, the shading
-// with the shading step's -fmad=false), so l is rounded op by op with explicit intrinsics.
+// with the shading step's -fmad=false), so l is rounded op by op with explicit intrinsics.  The spot and rect lights
+// (SHAPED LIGHTS) share their sample hash and sample points the same way.
 #pragma once
 #include "common.cuh"
 #include "kernels.h"
@@ -24,6 +25,55 @@ __device__ __forceinline__ LightDir light_dir(int kind, const float* vec, float 
     const float den = fmaxf(d.rn, LIGHT_EPS);
     d.l[0] = div_(d.w[0], den); d.l[1] = div_(d.w[1], den); d.l[2] = div_(d.w[2], den);
     return d;
+}
+
+// ---- spot and rect lights (SHAPED LIGHTS) ----
+#define LIGHT_SPOT 2
+#define LIGHT_RECT 3
+
+// lowbias32 (C. Wellons' integer hash): the sample hash of a rect light
+__host__ __device__ __forceinline__ uint32_t lowbias32(uint32_t x) {
+    x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
+    return x;
+}
+
+// the per-(set, Gaussian row, light) hash state; sample q's jitter is lowbias32(h ^ 2q) and lowbias32(h ^ (2q + 1))
+__device__ __forceinline__ uint32_t rect_hash(uint32_t seed, uint32_t g, uint32_t j) {
+    return lowbias32(lowbias32(lowbias32(seed) ^ g) ^ j);
+}
+
+__device__ __forceinline__ float hash_unit(uint32_t h) { return (float)(h >> 8) * (1.0f / 16777216.0f); }   // exact
+
+// Stratified sample q = i M + k of the rect (pos, u, v): s = -1 + (2i + 2 xi1) / M (stratum i of width 2/M, jittered
+// over all of it), t likewise, and y = (pos + s u) + t v, rounded op by op (2 xi and 2i + 2 xi are exact)
+__device__ __forceinline__ void rect_sample(const float* pos, const float* u, const float* v, int M, uint32_t h, int q,
+                                            float& s, float& t, float* y) {
+    const int i = q / M, k = q - (q / M) * M;
+    const float xi1 = hash_unit(lowbias32(h ^ (2u * (uint32_t)q))), xi2 = hash_unit(lowbias32(h ^ (2u * (uint32_t)q + 1u)));
+    const float fm = (float)M;
+    s = add_(-1.0f, div_(add_((float)(2 * i), mul_(2.0f, xi1)), fm));
+    t = add_(-1.0f, div_(add_((float)(2 * k), mul_(2.0f, xi2)), fm));
+#pragma unroll
+    for (int c = 0; c < 3; ++c) y[c] = add_(add_(pos[c], mul_(s, u[c])), mul_(t, v[c]));
+}
+
+// rays of a shaped light set (R of the header), -1 for a bad set: K out of range, a kind other than 2 or 3, M out of
+// range or R above R3DG_MAX_SHAPED_RAYS
+inline int shaped_rays(int K, const int32_t* kind, int M) {
+    if (K < 0 || K > R3DG_MAX_LIGHTS || (K > 0 && !kind) || M < 1 || M > R3DG_MAX_RECT_SAMPLES) return -1;
+    int R = 0;
+    for (int j = 0; j < K; ++j) {
+        if (kind[j] != LIGHT_SPOT && kind[j] != LIGHT_RECT) return -1;
+        R += kind[j] == LIGHT_SPOT ? 1 : M * M;
+    }
+    return R > R3DG_MAX_SHAPED_RAYS ? -1 : R;
+}
+
+// the host kind array as the kernels' argument: bit j set = light j is a rect
+inline uint32_t rect_mask(int K, const int32_t* kind) {
+    uint32_t m = 0u;
+    for (int j = 0; j < K; ++j) m |= (uint32_t)(kind[j] == LIGHT_RECT) << j;
+    return m;
 }
 
 // host-side checks shared by both operations: K in range and every kind 0 or 1

@@ -15,8 +15,11 @@ Differences from the reference that are not observable in the results:
 Beyond the reference: `RayTracer.bake_radiance` / `fit_incident_sh` / `update_incidents` compute each Gaussian's
 incident-light SH (`incidents`) from the scene itself — the bake's rays composited front to back through the
 other Gaussians (r3dg_bvh_bake_radiance), then a per-Gaussian ridge fit (r3dg_fit_incident_sh).
-`RayTracer.trace_lights` traces the shadows of point and directional lights (lights.py).
+`RayTracer.trace_lights` traces the shadows of point and directional lights (lights.py), `trace_shaped_lights` those
+of spot and rect lights.
 """
+import ctypes
+
 import torch
 
 from . import _C_bvh as _C
@@ -154,6 +157,28 @@ class RayTracer:
         _lib.call("r3dg_bvh_trace_lights", dev, P, K, kind.data_ptr() if K else None, _lib.ptr(vec), self.tree.data_ptr(),
                   self.aabb.data_ptr(), m.data_ptr(), ci.data_ptr(), op.data_ptr(), nr.data_ptr(), _lib.ptr(out),
                   tmp.data_ptr(), tmp.numel(), what="trace_lights")
+        return out
+
+    @torch.no_grad()
+    def trace_shaped_lights(self, means3D, symm_inv, opacity, normals, lights):
+        """Shadow transmittance T [P,R] of the spot and rect lights `lights` (lights.ShapedLights) through this tree
+        (r3dg_bvh_trace_shaped_lights): a spot's column is trace_lights' T of a point light at its position, a rect's
+        M^2 columns those of point lights at its hashed stratified samples (the points shade_shaped uses).  No
+        gradient.  A static light set is traced once and its T reused for every view."""
+        from .lights import _shaped_args
+        P, R = means3D.shape[0], lights.num_rays()
+        dev = means3D.device
+        if not all(t.is_cuda for t in (means3D, symm_inv, opacity, normals, lights.pos, lights.a, lights.b)):
+            raise RuntimeError("trace_shaped_lights runs on the GPU only (no CPU path)")
+        if means3D.shape != (P, 3) or normals.shape != (P, 3) or symm_inv.shape != (P, 6) or opacity.numel() != P:
+            raise ValueError("means3D and normals must be [P,3], symm_inv [P,6] and opacity [P]")
+        out = torch.empty((P, R), dtype=torch.float32, device=dev)
+        m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(normals)
+        ts = [_lib.f32(t) for t in (lights.pos, lights.a, lights.b, lights.color, lights.cone)] + [m, None, None, nr, None, None]
+        args = _shaped_args(P, 1, lights, ts)
+        tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_shaped_lights_tmp_bytes(P), dev)
+        _lib.call("r3dg_bvh_trace_shaped_lights", dev, ctypes.byref(args), self.tree.data_ptr(), self.aabb.data_ptr(),
+                  ci.data_ptr(), op.data_ptr(), _lib.ptr(out), tmp.data_ptr(), tmp.numel(), what="trace_shaped_lights")
         return out
 
 
