@@ -1029,6 +1029,81 @@ int r3dg_env_pyramid_build(const float* env, int env_h, int env_w, float* pyrami
 size_t r3dg_shade_filtered_det_bytes(int env_h, int env_w);
 
 /* ------------------------------------------------------------------------------------------
+ * PIXEL SHADING: the shading step's rendering equation at every pixel of rasterized material images
+ * (deferred shading, DESIGN.md §4.29), with each pixel's visibility traced through the BVH.
+ *   Layout: V views (1 <= V <= R3DG_MAX_VIEWS) of planar H x W images; view v's block of a [C,H,W] image
+ *   starts at v C H W.  Views share nothing but the env: each view's outputs equal a one-view call's.
+ *   Pixel p of view v is valid when mask is NULL or mask[v,p] != 0; invalid pixels are traced and shaded
+ *   not at all, and every output and gradient element of theirs is +0.
+ *   For a valid pixel: n^ = F.normalize(normal_p) op by op, n / max(sqrt((x*x + y*y) + z*z), 1e-12).
+ *   Directions d_i = rotate_from_z(n^, fib_sample(i, N)), i < N: bit for bit r3dg_sample_incident_dirs of
+ *   n^ without a phase; the area of every sample is 2 pi.
+ *   Trace (r3dg_bvh_trace_pixels): T[v,i,p] is what r3dg_bvh_trace_opacity returns for the ray with
+ *   origin points_p, direction d_i and origin_offset 0.05 through a tree built over the P Gaussians
+ *   (same hit rule, slab test and stop rule: T in {0} U [0.9, 1]).  Reads V, H, W, N, normal, points
+ *   and mask; writes T f32[V,N,H,W], every element.  No gradient.  Rays are numbered in 64 bits (V H W N
+ *   may exceed 2^31), the samples of a pixel adjacent and the pixels in 8 x 8 tiles.
+ *   Shading (r3dg_shade_pixels_forward / _backward): the shading step's formula (r3dg_shade_args) per
+ *   pixel, with viewdir = campos_v - points_p (one fp32 subtraction per component), the raw normal_p
+ *   for n.d and GGX, local light max(sum_k Y_k(d_i) inc_k, 0) (zero when incidents is NULL), global light
+ *   env(transform_v d_i) T[v,i,p] (the point lookup, or the filtered one at Omega = 2 pi / N with
+ *   env_pyramid), and pbr, diffuse_light, specular the means over the samples; mean_visibility = mean_i
+ *   T.  Each output equals r3dg_render_equation_forward of the pixel as a row (viewdirs, T and the
+ *   sampler's directions and areas) bit for bit.
+ *   Backward from dL_dpbr (required), dL_ddiffuse_light and dL_dspecular (NULL = zero) writes every
+ *   element of dL_dbase_color [V,3,H,W], dL_droughness [V,1,H,W], dL_dincidents [V,48,H,W] (with
+ *   incidents) and dL_denv [env_h,env_w,3] (summed over all views).  None to normal, points, campos or
+ *   T.  dL_denv follows r3dg_shade_args: the pyramid's dL_denv_pyramid workspace with env_pyramid, and
+ *   the deterministic mode's fixed-point sums in det_work (r3dg_shade_det_bytes, or
+ *   r3dg_shade_filtered_det_bytes with env_pyramid), anchored to the largest cotangent of the call.
+ *   Refusals before any launch: R3DG_ERR_BAD_ARG for V outside 1..R3DG_MAX_VIEWS, H, W, N, env_h or
+ *   env_w < 1, a NULL pointer the call needs, transform_per_view without env_transform, a missing
+ *   dL_denv_pyramid, a missing or short det_work, or a short tmp; R3DG_ERR_UNSUPPORTED for N beyond the
+ *   bake's sample table (N * 12 > 32 KB) or V H W > 2^31 - 1.
+ * ------------------------------------------------------------------------------------------ */
+struct r3dg_pixel_args {
+    int V, H, W, N;
+    int env_h, env_w;
+    const float* base_color;      /* [V,3,H,W] un-premultiplied */
+    const float* roughness;       /* [V,1,H,W] */
+    const float* normal;          /* [V,3,H,W] (no gradient) */
+    const float* points;          /* [V,3,H,W] world-space surface points */
+    const float* campos;          /* [V,3] camera centres */
+    const float* incidents;       /* [V,48,H,W] or NULL: channel 3k + c = SH coefficient k of colour c */
+    const uint8_t* mask;          /* [V,H,W] or NULL */
+    const float* env;             /* [env_h,env_w,3] ACTIVATED environment map */
+    const float* env_transform;   /* NULL, [3,3], or [V,3,3] with transform_per_view */
+    int transform_per_view;
+    const float* env_pyramid;     /* NULL or r3dg_env_pyramid_build of env */
+    float* dL_denv_pyramid;       /* backward with env_pyramid: r3dg_env_pyramid_floats floats of workspace */
+    const float* visibility;      /* T [V,N,H,W] */
+    float* pbr;                   /* forward: [V,3,H,W] */
+    float* diffuse_light;         /* forward: [V,3,H,W] */
+    float* specular;              /* forward: [V,3,H,W] */
+    float* mean_visibility;       /* forward: [V,1,H,W] */
+    const float* dL_dpbr;         /* backward: [V,3,H,W] */
+    const float* dL_ddiffuse_light;
+    const float* dL_dspecular;
+    float* dL_dbase_color;
+    float* dL_droughness;
+    float* dL_dincidents;
+    float* dL_denv;
+    int deterministic;
+    void* det_work;
+    size_t det_work_bytes;
+};
+
+size_t r3dg_bvh_trace_pixels_tmp_bytes(int P);
+/* T of the valid pixels through a tree built over P Gaussians (means3D [P,3], covs3D the INVERSE
+ * covariances [P,6], opacities [P], normals [P,3]); tmp: r3dg_bvh_trace_pixels_tmp_bytes(P).  P < 1:
+ * R3DG_ERR_BAD_ARG (there is no tree). */
+int r3dg_bvh_trace_pixels(const struct r3dg_pixel_args* args, int P, const int32_t* nodes, const float* aabbs,
+                          const float* means3D, const float* covs3D, const float* opacities, const float* normals,
+                          float* T, void* tmp, size_t tmp_bytes, r3dg_stream_t stream);
+int r3dg_shade_pixels_forward(const struct r3dg_pixel_args* args, r3dg_stream_t stream);
+int r3dg_shade_pixels_backward(const struct r3dg_pixel_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * DETERMINISTIC MODE.  With `deterministic` set in r3dg_raster_fwd_args, r3dg_raster_bwd_args or
  * r3dg_shade_args, the three sums that float atomics make depend on the order in which warps finish
  * are accumulated in fixed point instead (csrc/detacc.cuh): out_weights of the forward, the

@@ -103,6 +103,17 @@ class ShapedLightArgs(ctypes.Structure):
                 [("work_bytes", c_size_t)])
 
 
+class PixelArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("V", "H", "W", "N", "env_h", "env_w")] +
+                [(n, c_void_p) for n in ("base_color", "roughness", "normal", "points", "campos", "incidents", "mask", "env",
+                                         "env_transform")] +
+                [("transform_per_view", c_int)] +
+                [(n, c_void_p) for n in ("env_pyramid", "dL_denv_pyramid", "visibility", "pbr", "diffuse_light", "specular",
+                                         "mean_visibility", "dL_dpbr", "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color",
+                                         "dL_droughness", "dL_dincidents", "dL_denv")] +
+                [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+
+
 class ComposeArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("P", "K")] +
                 [(n, c_void_p) for n in ("offsets", "quat", "translation", "scale", "xyz", "normal", "rotation", "scaling")] +
@@ -206,6 +217,11 @@ SYMBOLS = [
     ("r3dg_shade_shaped_lights_work_bytes", c_size_t, [c_int, c_int]),
     ("r3dg_shade_shaped_lights_forward", c_int, [c_void_p, c_void_p]),
     ("r3dg_shade_shaped_lights_backward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_bvh_trace_pixels_tmp_bytes", c_size_t, [c_int]),
+    # `const struct r3dg_pixel_args*`: pass ctypes.byref(PixelArgs(...))
+    ("r3dg_bvh_trace_pixels", c_int, [c_void_p, c_int] + [c_void_p] * 8 + [c_size_t, c_void_p]),
+    ("r3dg_shade_pixels_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_shade_pixels_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_compose_work_bytes", c_size_t, [c_int, c_int]),
     # `const struct r3dg_compose_args*`: pass ctypes.byref(ComposeArgs(...))
     ("r3dg_compose_forward", c_int, [c_void_p, c_void_p]),

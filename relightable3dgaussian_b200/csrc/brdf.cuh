@@ -35,6 +35,13 @@ __device__ __forceinline__ void view_operands(const float* n, const float* viewd
     Ns[0] = N0 * sg; Ns[1] = N1 * sg; Ns[2] = N2 * sg;
 }
 
+// alpha^2 and k of the roughness o.rough
+__device__ __forceinline__ void roughness_operands(GaussianOperands& o) {
+    const float al = o.rough * o.rough;
+    o.a2 = al * al;
+    o.k = (al + 2.0f * o.rough + 1.0f) / 8.0f;
+}
+
 // the view-independent operands: material, raw normal, alpha^2 and k of the roughness (A: any argument record with
 // the base_color [P,3], roughness [P] and normals [P,3] pointers)
 template <class A>
@@ -42,9 +49,7 @@ __device__ __forceinline__ void load_material(const A& a, int g, GaussianOperand
 #pragma unroll
     for (int c = 0; c < 3; ++c) { o.base[c] = a.base_color[3 * (size_t)g + c]; o.n[c] = a.normals[3 * (size_t)g + c]; }
     o.rough = a.roughness[g];
-    const float al = o.rough * o.rough;
-    o.a2 = al * al;
-    o.k = (al + 2.0f * o.rough + 1.0f) / 8.0f;
+    roughness_operands(o);
 }
 
 // 1/x with one MUFU (<= 1 ulp), for the BACKWARD kernels only: their recomputed forward quantities and their gradient

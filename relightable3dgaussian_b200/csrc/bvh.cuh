@@ -102,6 +102,12 @@ __device__ __forceinline__ float3 rotate_from_z(float nx, float ny, float nz, fl
     const float nrm = fmaxf(sqrt_(fma_(z, z, fma_(y, y, mul_(x, x)))), 1e-12f);   // F.normalize eps
     return make_float3(div_(x, nrm), div_(y, nrm), div_(z, nrm));
 }
+// F.normalize(n) op by op: n / max(sqrt((x*x + y*y) + z*z), 1e-12).  The per-pixel trace and shading rotate the
+// samples to this unit normal (a rasterized normal is a blend, not unit length).
+__device__ __forceinline__ float3 unit_normal(float x, float y, float z) {
+    const float nn = fmaxf(sqrt_(add_(add_(mul_(x, x), mul_(y, y)), mul_(z, z))), 1e-12f);
+    return make_float3(div_(x, nn), div_(y, nn), div_(z, nn));
+}
 // The bake's sample table holds N float3 in dynamic shared memory; a larger N is refused (R3DG_ERR_UNSUPPORTED).
 #define BAKE_SAMPLE_SMEM (32 * 1024)
 

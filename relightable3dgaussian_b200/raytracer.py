@@ -16,7 +16,8 @@ Beyond the reference: `RayTracer.bake_radiance` / `fit_incident_sh` / `update_in
 incident-light SH (`incidents`) from the scene itself — the bake's rays composited front to back through the
 other Gaussians (r3dg_bvh_bake_radiance), then a per-Gaussian ridge fit (r3dg_fit_incident_sh).
 `RayTracer.trace_lights` traces the shadows of point and directional lights (lights.py), `trace_shaped_lights` those
-of spot and rect lights.
+of spot and rect lights.  `RayTracer.trace_pixels` traces the visibility of the per-pixel
+shading (shading.shade_pixels) from the surface points of rasterized G-buffer images.
 """
 import ctypes
 
@@ -180,6 +181,28 @@ class RayTracer:
         _lib.call("r3dg_bvh_trace_shaped_lights", dev, ctypes.byref(args), self.tree.data_ptr(), self.aabb.data_ptr(),
                   ci.data_ptr(), op.data_ptr(), _lib.ptr(out), tmp.data_ptr(), tmp.numel(), what="trace_shaped_lights")
         return out
+
+    @torch.no_grad()
+    def trace_pixels(self, points, normals, sample_num, means3D, symm_inv, opacity, gaussian_normals, mask=None):
+        """Visibility T [N,H,W] (or [V,N,H,W]) of the per-pixel shading (shading.shade_pixels) through this tree
+        (r3dg_bvh_trace_pixels): for every valid pixel of points / normals [3,H,W] (or [V,3,H,W]; world-space surface
+        points and the rasterized normals) and sample i, trace_visibility's T of the ray from the point along the
+        sampler's direction i around normalize(normal), bit for bit.  Pixels outside `mask` ([H,W] or [V,H,W], bool
+        or uint8) trace nothing and get 0.  No gradient.  A view is traced once and shaded under any number of envs."""
+        from .shading import pixel_args
+        P = means3D.shape[0]
+        if not all(t.is_cuda for t in (means3D, symm_inv, opacity, gaussian_normals)):
+            raise RuntimeError("trace_pixels runs on the GPU only (no CPU path)")
+        if means3D.shape != (P, 3) or gaussian_normals.shape != (P, 3) or symm_inv.shape != (P, 6) or opacity.numel() != P:
+            raise ValueError("means3D and gaussian_normals must be [P,3], symm_inv [P,6] and opacity [P]")
+        a, lead, keep = pixel_args(normals, points, sample_num, mask)
+        out = torch.empty((a.V, a.N, a.H, a.W), dtype=torch.float32, device=points.device)
+        m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(gaussian_normals)
+        tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_pixels_tmp_bytes(P), points.device)
+        _lib.call("r3dg_bvh_trace_pixels", points.device, ctypes.byref(a), P, self.tree.data_ptr(), self.aabb.data_ptr(),
+                  m.data_ptr(), ci.data_ptr(), op.data_ptr(), nr.data_ptr(), out.data_ptr(), tmp.data_ptr(), tmp.numel(),
+                  what="trace_pixels")
+        return out.reshape(lead[0] + out.shape[1:])
 
 
 @torch.no_grad()

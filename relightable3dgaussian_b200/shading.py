@@ -260,3 +260,130 @@ def install(module=None):
         import gaussian_renderer.neilf as module
     module.rendering_equation = rendering_equation
     return module
+
+
+# ---- per-pixel (deferred) shading ------------------------------------------------------------------------------------
+def _views(t, C, name, lead=None):
+    """A planar image `t` [C,H,W] (one view) or [V,C,H,W] as contiguous float32 [V,C,H,W], and (leading shape, H, W).
+    lead: the call's (leading shape, H, W) to match."""
+    if t.dim() not in (3, 4) or t.shape[-3] != C:
+        raise ValueError(f"{name} must be [{C},H,W] or [V,{C},H,W], got {tuple(t.shape)}")
+    shape = (tuple(t.shape[:-3]), t.shape[-2], t.shape[-1])
+    if lead is not None and shape != lead:
+        raise ValueError(f"{name} {tuple(t.shape)} does not match the images' views and size {lead}")
+    if not 1 <= (t.shape[0] if t.dim() == 4 else 1) <= MAX_VIEWS:
+        raise ValueError(f"per-pixel shading takes 1 to {MAX_VIEWS} views per call (got {t.shape[0]})")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor (per-pixel shading runs on the GPU only)")
+    x = _lib.f32(t)
+    return (x if x.dim() == 4 else x.unsqueeze(0)), shape
+
+
+def _mask(mask, lead):
+    """The optional validity mask [H,W] or [V,H,W] (bool or uint8) as contiguous uint8 [V,H,W]."""
+    if mask is None:
+        return None
+    if mask.dtype not in (torch.bool, torch.uint8) or tuple(mask.shape) != lead[0] + (lead[1], lead[2]):
+        raise ValueError(f"mask must be bool or uint8 {lead[0] + (lead[1], lead[2])}, got {mask.dtype} {tuple(mask.shape)}")
+    if not mask.is_cuda:
+        raise RuntimeError("mask must be a CUDA tensor (per-pixel shading runs on the GPU only)")
+    m = mask.detach().contiguous()
+    m = m.view(torch.uint8) if m.dtype == torch.bool else m
+    return m.reshape(-1, lead[1], lead[2])
+
+
+def pixel_args(normal, points, N, mask):
+    """PixelArgs with the views, size, samples, normal, points and mask of a per-pixel call, and the tensors it points
+    to (which must outlive the launch): (args, lead, [normal, points, mask]) with lead = (leading shape, H, W)."""
+    n, lead = _views(normal, 3, "normal")
+    p, _ = _views(points, 3, "points", lead)
+    m = _mask(mask, lead)
+    if not 1 <= int(N):
+        raise ValueError(f"sample_num must be >= 1 (got {N})")
+    a = _lib.PixelArgs()
+    a.V, a.H, a.W, a.N = n.shape[0], lead[1], lead[2], int(N)
+    a.normal, a.points, a.mask = n.data_ptr(), p.data_ptr(), _lib.ptr(m)
+    return a, lead, [n, p, m]
+
+
+class _ShadePixels(torch.autograd.Function):
+    """The per-pixel shading of V views: one node with gradients to base_color, roughness, incidents and env."""
+
+    @staticmethod
+    def forward(ctx, base_color, roughness, incidents, env, normal, points, campos, visibility, mask, transform, env_filter):
+        a, lead, keep = pixel_args(normal, points, visibility.shape[-3], mask)
+        V, H, W = a.V, a.H, a.W
+        b, _ = _views(base_color, 3, "base_color", lead)
+        r, _ = _views(roughness, 1, "roughness", lead)
+        vis, _ = _views(visibility, a.N, "visibility", lead)
+        inc = None if incidents is None else _views(incidents, 48, "incidents", lead)[0]
+        cp = _lib.f32(campos).reshape(-1, 3)
+        if cp.shape[0] != V or not cp.is_cuda:
+            raise ValueError(f"campos must be a CUDA [3] or [V,3] tensor with V = {V}, got {tuple(campos.shape)}")
+        e = _lib.f32(env)
+        tr = None if transform is None else _lib.f32(transform)
+        if tr is not None and tr.shape not in ((3, 3), (V, 3, 3)):
+            raise ValueError(f"the env transform must be [3,3] or [V,3,3] with V = {V}, got {tuple(tr.shape)}")
+        a.env_h, a.env_w = e.shape[0], e.shape[1]
+        a.base_color, a.roughness, a.campos, a.incidents, a.env = b.data_ptr(), r.data_ptr(), cp.data_ptr(), _lib.ptr(inc), e.data_ptr()
+        a.env_transform, a.transform_per_view = _lib.ptr(tr), int(tr is not None and tr.dim() == 3)
+        a.visibility = vis.data_ptr()
+        pyr = env_pyramid(e) if env_filter else None
+        a.env_pyramid = _lib.ptr(pyr)
+        f = dict(dtype=torch.float32, device=b.device)
+        pbr, diffuse, specular = (torch.empty((V, 3, H, W), **f) for _ in range(3))
+        mean_vis = torch.empty((V, 1, H, W), **f)
+        a.pbr, a.diffuse_light, a.specular, a.mean_visibility = (t.data_ptr() for t in (pbr, diffuse, specular, mean_vis))
+        _lib.call("r3dg_shade_pixels_forward", b.device, ctypes.byref(a), what="shade_pixels")
+        ctx.save_for_backward(b, r, inc, e, vis, cp, tr, pyr, *keep[:2])
+        ctx.mask, ctx.lead = keep[2], lead
+        ctx.mark_non_differentiable(mean_vis)
+        shape = lambda t: t.reshape(lead[0] + t.shape[1:])
+        return shape(pbr), shape(diffuse), shape(specular), shape(mean_vis)
+
+    @staticmethod
+    def backward(ctx, g_pbr, g_diffuse, g_specular, _):
+        b, r, inc, e, vis, cp, tr, pyr, n, p = ctx.saved_tensors
+        V, H, W = b.shape[0], b.shape[2], b.shape[3]
+        a = _lib.PixelArgs()
+        a.V, a.H, a.W, a.N, a.env_h, a.env_w = V, H, W, vis.shape[1], e.shape[0], e.shape[1]
+        a.base_color, a.roughness, a.normal, a.points, a.campos = (t.data_ptr() for t in (b, r, n, p, cp))
+        a.incidents, a.mask, a.env, a.visibility = _lib.ptr(inc), _lib.ptr(ctx.mask), e.data_ptr(), vis.data_ptr()
+        a.env_transform, a.transform_per_view = _lib.ptr(tr), int(tr is not None and tr.dim() == 3)
+        dev = b.device
+        f = dict(dtype=torch.float32, device=dev)
+        g = [None if t is None else _lib.f32(t).reshape(V, 3, H, W) for t in (g_pbr, g_diffuse, g_specular)]
+        if g[0] is None:
+            g[0] = torch.zeros((V, 3, H, W), **f)
+        a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = (_lib.ptr(t) for t in g)
+        d_base, d_rough, d_env = torch.empty_like(b), torch.empty_like(r), torch.empty_like(e)
+        d_inc = None if inc is None else torch.empty_like(inc)
+        a.dL_dbase_color, a.dL_droughness, a.dL_dincidents, a.dL_denv = d_base.data_ptr(), d_rough.data_ptr(), _lib.ptr(d_inc), d_env.data_ptr()
+        lib, g_pyr = _lib.load(), None
+        if pyr is not None:
+            a.env_pyramid, g_pyr = pyr.data_ptr(), torch.empty_like(pyr)
+            a.dL_denv_pyramid = g_pyr.data_ptr()
+        det_bytes = (lib.r3dg_shade_det_bytes if pyr is None else lib.r3dg_shade_filtered_det_bytes)(e.shape[0], e.shape[1])
+        det_ws = _lib.det_workspace(a, det_bytes, dev)
+        _lib.call("r3dg_shade_pixels_backward", dev, ctypes.byref(a), what="shade_pixels backward")
+        shape = lambda t: None if t is None else t.reshape(ctx.lead[0] + t.shape[1:])
+        return shape(d_base), shape(d_rough), shape(d_inc), d_env, None, None, None, None, None, None, None
+
+
+def shade_pixels(base_color, roughness, normal, points, campos, visibility, direct_light_env_light, incidents=None,
+                 mask=None, env_filter=None):
+    """The shading step at every pixel of rasterized material images (deferred shading; include/r3dg_b200.h, PIXEL
+    SHADING).  One view: base_color [3,H,W], roughness [1,H,W], normal [3,H,W] (un-premultiplied material channels),
+    points [3,H,W] world-space surface points, campos [3], visibility [N,H,W] from RayTracer.trace_pixels, optional
+    incidents [48,H,W] (channel 3k + c = SH coefficient k of colour c) and mask [H,W] (bool or uint8).  V views: a
+    leading V on every image, campos [V,3], and an EnvLight transform of [3,3] or [V,3,3].
+
+    Per valid pixel: the N samples of the sampler around normalize(normal) (area 2 pi), viewdir = campos - points,
+    and the formula of `rendering_equation`, so each output equals that function on the pixel as a row bit for bit.
+    Returns dict(pbr, diffuse_light, specular [.., 3,H,W], visibility [.., 1,H,W] = mean_i T); masked pixels are 0.
+    Gradients: base_color, roughness, incidents and the environment map; none for normal, points, campos or the
+    visibility.  env_filter: as in `rendering_equation` (None: set_env_filter's default)."""
+    env, transform = _env_texture(direct_light_env_light)
+    pbr, diffuse, specular, vis = _ShadePixels.apply(base_color, roughness, incidents, env, normal, points, campos, visibility,
+                                                     mask, transform, _filter_on(env_filter))
+    return {"pbr": pbr, "diffuse_light": diffuse, "specular": specular, "visibility": vis}
