@@ -1104,6 +1104,85 @@ int r3dg_shade_pixels_forward(const struct r3dg_pixel_args* args, r3dg_stream_t 
 int r3dg_shade_pixels_backward(const struct r3dg_pixel_args* args, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * PIXEL LIGHTS: the shadows and shading terms of a LIGHTS or a SHAPED LIGHTS set at every pixel of
+ * the PIXEL SHADING layout (DESIGN.md §4.30), so a highlight or a shadow edge varies inside one
+ * Gaussian's footprint.  The caller adds the terms to r3dg_shade_pixels_forward's outputs.
+ *   Light set.  K lights, 0 <= K <= R3DG_MAX_LIGHTS, kind i32[K] a HOST array, all of one family:
+ *   {0 directional, 1 point} (LIGHTS, R = K shadow columns) or {2 spot, 3 rect} (SHAPED LIGHTS, M and
+ *   seed as there, R = sum n_j <= R3DG_MAX_SHAPED_RAYS columns in the same order).  pos [K,3] is a
+ *   LIGHTS set's vec; a, b and cone are read only by a SHAPED LIGHTS set, as there.  M must lie in
+ *   1..R3DG_MAX_RECT_SAMPLES for either family.
+ *   Layout: V views (1 <= V <= R3DG_MAX_VIEWS) of planar H x W images, as PIXEL SHADING; pixel p = y W + x
+ *   of view v is valid when mask is NULL or mask[v,p] != 0.
+ *   A valid pixel is a Gaussian row of LIGHTS / SHAPED LIGHTS with: mean m = points_p, raw normal
+ *   normal_p, viewdir = campos_v - points_p (one fp32 subtraction per component), shadows T[v,:,p] and
+ *   row index p for the rect hash (the same for every view, so each view equals a one-view call).
+ *   Trace (r3dg_bvh_trace_pixel_lights): T[v,c,p] is the LIGHTS trace of column c's ray from m = points_p
+ *   (origin m + 0.05 l, t_max +inf for a directional light and |target - o| otherwise, the same hit
+ *   rule, margin and T < 1e-4 stop) through a tree built over P Gaussians; a spot's column is a point
+ *   light's ray.  Reads V, H, W, K, M, seed, kind, pos, a, b, points and mask; writes T f32[V,R,H,W],
+ *   every element (0 for invalid pixels, which trace nothing).  Rays are numbered in 64 bits, a
+ *   pixel's columns adjacent and the pixels in 8 x 8 tiles.  No gradient.
+ *   Shading (r3dg_shade_pixel_lights_forward / _backward): pbr, diffuse_light and specular [V,3,H,W]
+ *   are the LIGHTS / SHAPED LIGHTS outputs of the pixel as a row, bit for bit; 0 for invalid pixels.
+ *   Backward from dL_dpbr (required), dL_ddiffuse_light and dL_dspecular (NULL = zero) writes every
+ *   element of dL_dbase_color [V,3,H,W] and dL_droughness [V,1,H,W] (0 for invalid pixels), and the
+ *   light gradients summed over the valid pixels of every view: dL_dpos and dL_dcolor [K,3] for a
+ *   LIGHTS set; dL_dpos, dL_da, dL_db, dL_dcolor [K,3] and dL_dcone [K,2] for a SHAPED LIGHTS set.
+ *   None to normal, points, campos or T.  The light gradients are per-CTA partials in `work`
+ *   (r3dg_shade_pixel_lights_work_bytes(V, H, W, K)) summed in block order over a grid that depends
+ *   on V H W only: no float atomics, every output is bitwise reproducible.
+ *   Refusals before any launch: R3DG_ERR_BAD_ARG for V outside 1..R3DG_MAX_VIEWS, H or W < 1, K outside
+ *   0..R3DG_MAX_LIGHTS, a kind outside 0..3 or a set that mixes the two families, M outside
+ *   1..R3DG_MAX_RECT_SAMPLES, R > R3DG_MAX_SHAPED_RAYS, a NULL pointer the call needs, a short tmp or
+ *   workspace, or P < 1 (trace); R3DG_ERR_UNSUPPORTED for V H W > 2^31 - 1.  K = 0 launches no kernel
+ *   and zero-fills the outputs that exist.
+ * ------------------------------------------------------------------------------------------ */
+struct r3dg_pixel_light_args {
+    int V, H, W, K, M;
+    uint32_t seed;
+    const int32_t* kind;          /* HOST [K] */
+    const float* pos;             /* [K,3]: vec for kinds 0 and 1 */
+    const float* a;               /* [K,3] (spot, rect) */
+    const float* b;               /* [K,3] (rect) */
+    const float* color;           /* [K,3] */
+    const float* cone;            /* [K,2] (spot) */
+    const float* base_color;      /* [V,3,H,W] un-premultiplied */
+    const float* roughness;       /* [V,1,H,W] */
+    const float* normal;          /* [V,3,H,W] (no gradient) */
+    const float* points;          /* [V,3,H,W] world-space surface points */
+    const float* campos;          /* [V,3] camera centres */
+    const uint8_t* mask;          /* [V,H,W] or NULL */
+    const float* shadows;         /* T [V,R,H,W] */
+    float* pbr;                   /* forward: [V,3,H,W] */
+    float* diffuse_light;         /* forward: [V,3,H,W] */
+    float* specular;              /* forward: [V,3,H,W] */
+    const float* dL_dpbr;         /* backward: [V,3,H,W] */
+    const float* dL_ddiffuse_light;
+    const float* dL_dspecular;
+    float* dL_dbase_color;        /* [V,3,H,W] */
+    float* dL_droughness;         /* [V,1,H,W] */
+    float* dL_dpos;               /* [K,3] */
+    float* dL_da;                 /* [K,3] (SHAPED LIGHTS) */
+    float* dL_db;                 /* [K,3] (SHAPED LIGHTS) */
+    float* dL_dcolor;             /* [K,3] */
+    float* dL_dcone;              /* [K,2] (SHAPED LIGHTS) */
+    void* work;                   /* backward */
+    size_t work_bytes;
+};
+
+size_t r3dg_bvh_trace_pixel_lights_tmp_bytes(int P);
+/* T of every pixel through a tree built over P Gaussians (means3D [P,3], covs3D the INVERSE
+ * covariances [P,6], opacities [P], normals [P,3]); tmp: r3dg_bvh_trace_pixel_lights_tmp_bytes(P). */
+int r3dg_bvh_trace_pixel_lights(const struct r3dg_pixel_light_args* args, int P, const int32_t* nodes,
+                                const float* aabbs, const float* means3D, const float* covs3D,
+                                const float* opacities, const float* normals, float* T, void* tmp,
+                                size_t tmp_bytes, r3dg_stream_t stream);
+size_t r3dg_shade_pixel_lights_work_bytes(int V, int H, int W, int K);
+int r3dg_shade_pixel_lights_forward(const struct r3dg_pixel_light_args* args, r3dg_stream_t stream);
+int r3dg_shade_pixel_lights_backward(const struct r3dg_pixel_light_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * DETERMINISTIC MODE.  With `deterministic` set in r3dg_raster_fwd_args, r3dg_raster_bwd_args or
  * r3dg_shade_args, the three sums that float atomics make depend on the order in which warps finish
  * are accumulated in fixed point instead (csrc/detacc.cuh): out_weights of the forward, the

@@ -114,6 +114,15 @@ class PixelArgs(ctypes.Structure):
                 [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
 
 
+class PixelLightArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("V", "H", "W", "K", "M")] + [("seed", ctypes.c_uint32)] +
+                [(n, c_void_p) for n in ("kind", "pos", "a", "b", "color", "cone", "base_color", "roughness", "normal", "points",
+                                         "campos", "mask", "shadows", "pbr", "diffuse_light", "specular", "dL_dpbr",
+                                         "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color", "dL_droughness", "dL_dpos",
+                                         "dL_da", "dL_db", "dL_dcolor", "dL_dcone", "work")] +
+                [("work_bytes", c_size_t)])
+
+
 class ComposeArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("P", "K")] +
                 [(n, c_void_p) for n in ("offsets", "quat", "translation", "scale", "xyz", "normal", "rotation", "scaling")] +
@@ -222,6 +231,12 @@ SYMBOLS = [
     ("r3dg_bvh_trace_pixels", c_int, [c_void_p, c_int] + [c_void_p] * 8 + [c_size_t, c_void_p]),
     ("r3dg_shade_pixels_forward", c_int, [c_void_p, c_void_p]),
     ("r3dg_shade_pixels_backward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_bvh_trace_pixel_lights_tmp_bytes", c_size_t, [c_int]),
+    # `const struct r3dg_pixel_light_args*`: pass ctypes.byref(PixelLightArgs(...))
+    ("r3dg_bvh_trace_pixel_lights", c_int, [c_void_p, c_int] + [c_void_p] * 8 + [c_size_t, c_void_p]),
+    ("r3dg_shade_pixel_lights_work_bytes", c_size_t, [c_int, c_int, c_int, c_int]),
+    ("r3dg_shade_pixel_lights_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_shade_pixel_lights_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_compose_work_bytes", c_size_t, [c_int, c_int]),
     # `const struct r3dg_compose_args*`: pass ctypes.byref(ComposeArgs(...))
     ("r3dg_compose_forward", c_int, [c_void_p, c_void_p]),

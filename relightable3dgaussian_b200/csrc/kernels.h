@@ -160,6 +160,11 @@ int launch_bvh_shaped_lights(const r3dg_shaped_light_args* a, const int32_t* nod
 size_t shade_shaped_lights_work_bytes(int P, int K);
 int launch_shade_shaped_lights_forward(const r3dg_shaped_light_args* a, cudaStream_t stream, bool* launched);
 int launch_shade_shaped_lights_backward(const r3dg_shaped_light_args* a, cudaStream_t stream, bool* launched);
+// lights.cu: the backward's light-gradient sums over `blocks` CTA partials, in block order: [blocks][K][6] into dvec and
+// dcolor (LIGHTS), or [blocks][K][SL_SLOTS] into a's light gradients (SHAPED LIGHTS; reads a.K, a.a and a.b)
+int launch_lights_reduce(int K, int blocks, const float* partial, float* dvec, float* dcolor, cudaStream_t stream);
+int launch_shaped_reduce(const r3dg_shaped_light_args& a, uint32_t rect_mask, int blocks, const float* partial,
+                         cudaStream_t stream);
 // compose.cu: similarity transforms of Gaussian models; validates before launching, sets *launched when kernels ran
 size_t compose_work_bytes(int P, int K);
 int launch_compose_forward(const r3dg_compose_args* a, cudaStream_t stream, bool* launched);

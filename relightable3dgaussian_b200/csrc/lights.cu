@@ -11,38 +11,12 @@
 //    the warp's shared-memory row, the warps' rows summed in warp order into the CTA's partial [K,6], and the
 //    partials summed in block order by lights_reduce_kernel.  The grid depends on P only, so every output is
 //    bitwise reproducible.
-#include "brdf.cuh"
 #include "kernels.h"
-#include "lights.cuh"
+#include "lights_eval.cuh"
 
 namespace r3dg {
 
-#define LS_THREADS 128
-#define LS_WARPS (LS_THREADS / 32)
-
 static int lights_blocks(int P) { return (P + LS_THREADS - 1) / LS_THREADS; }
-
-// The K lights in shared memory
-struct LightSmem { float vec[3 * R3DG_MAX_LIGHTS], color[3 * R3DG_MAX_LIGHTS]; };
-
-__device__ __forceinline__ void stage_lights(const r3dg_light_args& a, LightSmem& s) {
-    for (int i = threadIdx.x; i < 3 * a.K; i += LS_THREADS) { s.vec[i] = a.vec[i]; s.color[i] = a.color[i]; }
-    __syncthreads();
-}
-
-// The light's term before GGX: l, E and max(n . l, 0) (ndr: n . l before the clamp)
-struct LightTerm { LightDir d; float E[3], r2c, ndr, ndi; };
-
-__device__ __forceinline__ LightTerm light_term(int kind, const LightSmem& s, int j, const GaussianOperands& o, const float* m) {
-    LightTerm t;
-    t.d = light_dir(kind, s.vec + 3 * j, m[0], m[1], m[2]);
-    t.r2c = fmaxf(t.d.r2, LIGHT_R2_MIN);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) t.E[c] = kind == 0 ? s.color[3 * j + c] : s.color[3 * j + c] / t.r2c;
-    t.ndr = o.n[0] * t.d.l[0] + o.n[1] * t.d.l[1] + o.n[2] * t.d.l[2];        // the shading step's n . w
-    t.ndi = fmaxf(t.ndr, 0.f);
-    return t;
-}
 
 __global__ void __launch_bounds__(LS_THREADS) lights_fwd_kernel(const r3dg_light_args a, const uint32_t point_mask) {
     __shared__ LightSmem s;
@@ -72,20 +46,6 @@ __global__ void __launch_bounds__(LS_THREADS) lights_fwd_kernel(const r3dg_light
 #pragma unroll
         for (int c = 0; c < 3; ++c) { a.pbr[3 * row + c] = pbr[c]; a.specular[3 * row + c] = spec[c]; a.diffuse_light[3 * row + c] = diff[c]; }
     }
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// dL/dw of l = w / max(|w|, eps) (F.normalize: the norm's gradient is cut below eps)
-__device__ __forceinline__ void normalize_backward(const LightDir& d, const float* dl, float* dw) {
-    const float den = fmaxf(d.rn, LIGHT_EPS);
-    const float ldl = d.rn >= LIGHT_EPS ? d.l[0] * dl[0] + d.l[1] * dl[1] + d.l[2] * dl[2] : 0.f;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) dw[c] = (dl[c] - d.l[c] * ldl) / den;
 }
 
 // partial: [gridDim.x][K][6] = (dL/dvec, dL/dcolor) of each light summed over the CTA's Gaussians and the views
@@ -204,6 +164,12 @@ __global__ void __launch_bounds__(LS_THREADS) lights_reduce_kernel(int K, int bl
 }
 
 // ---- host launchers -----------------------------------------------------------------------
+int launch_lights_reduce(int K, int blocks, const float* partial, float* dvec, float* dcolor, cudaStream_t stream) {
+    lights_reduce_kernel<<<(6 * K + LS_WARPS - 1) / LS_WARPS, LS_THREADS, 0, stream>>>(K, blocks, partial, dvec, dcolor);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
 size_t shade_lights_work_bytes(int P, int K) {
     return P <= 0 || K <= 0 ? 0 : (size_t)lights_blocks(P) * 6 * K * sizeof(float);
 }
@@ -258,9 +224,9 @@ int launch_shade_lights_backward(const r3dg_light_args* a, cudaStream_t stream, 
     const int blocks = lights_blocks(a->P);
     float* partial = (float*)a->work;
     lights_bwd_kernel<<<blocks, LS_THREADS, 0, stream>>>(*a, point_mask(a->K, a->kind), partial);
-    lights_reduce_kernel<<<(6 * a->K + LS_WARPS - 1) / LS_WARPS, LS_THREADS, 0, stream>>>(a->K, blocks, partial, a->dL_dvec,
-                                                                                         a->dL_dcolor);
     R3DG_CUDA_TRY(cudaGetLastError());
+    const int rc = launch_lights_reduce(a->K, blocks, partial, a->dL_dvec, a->dL_dcolor, stream);
+    if (rc != 0) return rc;
     *launched = true;
     return 0;
 }
@@ -268,82 +234,9 @@ int launch_shade_lights_backward(const r3dg_light_args* a, cudaStream_t stream, 
 // ==== spot and rect lights (SHAPED LIGHTS; DESIGN.md §4.28) ==================================================
 // The same layout as above: one thread per Gaussian, views outer, lights then samples inner, so every view's sums run
 // in one-view order.  A rect sample's point y_q is rect_sample's (lights.cuh), bit for bit the trace's.  The backward
-// accumulates each light's gradient over its samples in registers, as 16 intermediate values per light (SL_SLOTS),
-// sums them over the warp and the CTA as lights_bwd_kernel does, and shaped_reduce_kernel sums the CTAs in block order
-// and applies the light-level chain rule once (axis normalisation, u x v, n_e and A).
-#define SL_SLOTS 16
-// slots: 0-2 dL/dpos (= dL/dy summed), 3-5 dL/du through y (rect) or dL/da^ (spot), 6-8 dL/dv through y (rect) or
-// dL/dcos_inner, dL/dcos_outer (spot, 6 and 7), 9-11 dL/dcolor, 12-14 dL/dn_e and 15 dL/dA (rect)
-
-struct ShapedSmem {
-    float L[9 * R3DG_MAX_LIGHTS];              // pos, a (axis or u), b (v)
-    float color[3 * R3DG_MAX_LIGHTS];
-    float dir[3 * R3DG_MAX_LIGHTS];            // rect: n_e;  spot: a^
-    float sc[R3DG_MAX_LIGHTS];                 // rect: A;  spot: max(cos_inner - cos_outer, 1e-6)
-    float co[R3DG_MAX_LIGHTS];                 // spot: cos_outer
-    float live[R3DG_MAX_LIGHTS];               // spot: 1 where cos_inner - cos_outer >= 1e-6 (the clamp passes its gradient)
-};
-
-__device__ __forceinline__ void stage_shaped(const r3dg_shaped_light_args& a, uint32_t rect_mask, ShapedSmem& s) {
-    for (int i = threadIdx.x; i < 3 * a.K; i += LS_THREADS) {
-        const int j = i / 3, c = i - 3 * j;
-        const bool rect = (rect_mask >> j) & 1;
-        s.L[9 * j + c] = a.pos[i];
-        s.L[9 * j + 3 + c] = a.a[i];
-        s.L[9 * j + 6 + c] = rect ? a.b[i] : 0.f;
-        s.color[i] = a.color[i];
-    }
-    __syncthreads();
-    for (int j = threadIdx.x; j < a.K; j += LS_THREADS) {
-        const float* u = s.L + 9 * j + 3;
-        if ((rect_mask >> j) & 1) {
-            const float* v = s.L + 9 * j + 6;
-            const float c0 = u[1] * v[2] - u[2] * v[1], c1 = u[2] * v[0] - u[0] * v[2], c2 = u[0] * v[1] - u[1] * v[0];
-            const float cn = sqrtf(c0 * c0 + c1 * c1 + c2 * c2), den = fmaxf(cn, LIGHT_EPS);
-            s.dir[3 * j] = c0 / den; s.dir[3 * j + 1] = c1 / den; s.dir[3 * j + 2] = c2 / den;
-            s.sc[j] = 4.0f * cn;
-            s.co[j] = 0.f; s.live[j] = 0.f;
-        } else {
-            const float an = fmaxf(sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]), LIGHT_EPS);
-            s.dir[3 * j] = u[0] / an; s.dir[3 * j + 1] = u[1] / an; s.dir[3 * j + 2] = u[2] / an;
-            const float ci = a.cone[2 * j], co = a.cone[2 * j + 1];
-            s.sc[j] = fmaxf(ci - co, 1e-6f);
-            s.co[j] = co; s.live[j] = ci - co >= 1e-6f ? 1.f : 0.f;
-        }
-    }
-    __syncthreads();
-}
-
-// One ray of a shaped light at the Gaussian: l, w and the scalar weight of E = color * wgt, with its operands
-struct ShapedTerm {
-    LightDir d;
-    float st[2];          // rect: (s, t)
-    float r2c, ce_r, xr, x, wgt, ndr, ndi;
-};
-
-__device__ __forceinline__ void shaped_term(bool rect, const ShapedSmem& s, int j, int M, uint32_t h, int q,
-                                            const GaussianOperands& o, const float* m, ShapedTerm& t) {
-    const float* L = s.L + 9 * j;
-    const float* dir = s.dir + 3 * j;
-    float y[3];
-    if (rect) rect_sample(L, L + 3, L + 6, M, h, q, t.st[0], t.st[1], y);
-    else { y[0] = L[0]; y[1] = L[1]; y[2] = L[2]; t.st[0] = t.st[1] = 0.f; }
-    t.d = light_dir(1, y, m[0], m[1], m[2]);
-    t.r2c = fmaxf(t.d.r2, LIGHT_R2_MIN);
-    const float dl = dir[0] * t.d.l[0] + dir[1] * t.d.l[1] + dir[2] * t.d.l[2];
-    if (rect) {
-        t.ce_r = -dl;
-        t.xr = t.x = 0.f;
-        t.wgt = s.sc[j] * fmaxf(t.ce_r, 0.f) / ((float)(M * M) * t.r2c);
-    } else {
-        t.ce_r = 0.f;
-        t.xr = (-dl - s.co[j]) / s.sc[j];
-        t.x = fminf(fmaxf(t.xr, 0.f), 1.f);
-        t.wgt = t.x * t.x * (3.0f - 2.0f * t.x) / t.r2c;
-    }
-    t.ndr = o.n[0] * t.d.l[0] + o.n[1] * t.d.l[1] + o.n[2] * t.d.l[2];
-    t.ndi = fmaxf(t.ndr, 0.f);
-}
+// accumulates each light's gradient over its samples in registers (SL_SLOTS, lights_eval.cuh), sums them over the warp
+// and the CTA as lights_bwd_kernel does, and shaped_reduce_kernel sums the CTAs in block order and applies the
+// light-level chain rule once (axis normalisation, u x v, n_e and A).
 
 __global__ void __launch_bounds__(LS_THREADS) shaped_fwd_kernel(const r3dg_shaped_light_args a, const uint32_t rect_mask, const int R) {
     __shared__ ShapedSmem s;
@@ -510,14 +403,6 @@ __global__ void __launch_bounds__(LS_THREADS) shaped_bwd_kernel(const r3dg_shape
     }
 }
 
-// dL/dx of n = x / max(|x|, eps) for the cotangent dn (F.normalize: the norm's gradient is cut below eps)
-__device__ __forceinline__ void normalize3_backward(const float* x, const float* dn, float* dx) {
-    const float xn = sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]), den = fmaxf(xn, LIGHT_EPS);
-    const float ndn = xn >= LIGHT_EPS ? (x[0] * dn[0] + x[1] * dn[1] + x[2] * dn[2]) / den : 0.f;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) dx[c] = (dn[c] - x[c] / den * ndn) / den;
-}
-
 // One CTA per light: warp k sums slot k over the CTA partials in block order (lane-strided, then a fixed butterfly),
 // then one thread applies the light-level chain rule and writes the light's gradients
 __global__ void __launch_bounds__(32 * SL_SLOTS) shaped_reduce_kernel(const r3dg_shaped_light_args a, const uint32_t rect_mask,
@@ -555,6 +440,13 @@ __global__ void __launch_bounds__(32 * SL_SLOTS) shaped_reduce_kernel(const r3dg
 }
 
 // ---- shaped-light host launchers --------------------------------------------------------------
+int launch_shaped_reduce(const r3dg_shaped_light_args& a, uint32_t rect_mask, int blocks, const float* partial,
+                         cudaStream_t stream) {
+    shaped_reduce_kernel<<<a.K, 32 * SL_SLOTS, 0, stream>>>(a, rect_mask, blocks, partial);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
 size_t shade_shaped_lights_work_bytes(int P, int K) {
     return P <= 0 || K <= 0 ? 0 : (size_t)lights_blocks(P) * SL_SLOTS * K * sizeof(float);
 }
@@ -622,8 +514,9 @@ int launch_shade_shaped_lights_backward(const r3dg_shaped_light_args* a, cudaStr
     const uint32_t rm = rect_mask(a->K, a->kind);
     float* partial = (float*)a->work;
     shaped_bwd_kernel<<<blocks, LS_THREADS, 0, stream>>>(*a, rm, R, partial);
-    shaped_reduce_kernel<<<a->K, 32 * SL_SLOTS, 0, stream>>>(*a, rm, blocks, partial);
     R3DG_CUDA_TRY(cudaGetLastError());
+    const int rc = launch_shaped_reduce(*a, rm, blocks, partial, stream);
+    if (rc != 0) return rc;
     *launched = true;
     return 0;
 }

@@ -91,4 +91,33 @@ inline uint32_t point_mask(int K, const int32_t* kind) {
     return m;
 }
 
+// ---- per-pixel lights (PIXEL LIGHTS) ----
+// The set of a per-pixel light call: its R and the kernels' light masks
+struct PixelLightSet {
+    int R;
+    bool shaped;                     // spots and rects (else directional and point lights)
+    uint32_t dir_mask, point_mask, rect_mask;
+};
+
+// The checks the trace and the shading share, before any launch: 0 and the set, or the call's R3DG_ERR_* code.
+// `shading`: also the light fields only the shading reads.
+inline int pixel_light_set(const r3dg_pixel_light_args* a, bool shading, PixelLightSet& ls) {
+    if (!a || a->V < 1 || a->V > R3DG_MAX_VIEWS || a->H < 1 || a->W < 1 || a->M < 1 || a->M > R3DG_MAX_RECT_SAMPLES)
+        return R3DG_ERR_BAD_ARG;
+    if (a->K < 0 || a->K > R3DG_MAX_LIGHTS || (a->K > 0 && !a->kind)) return R3DG_ERR_BAD_ARG;
+    ls.shaped = a->K > 0 && (a->kind[0] == LIGHT_SPOT || a->kind[0] == LIGHT_RECT);
+    ls.R = ls.shaped ? shaped_rays(a->K, a->kind, a->M) : (lights_valid(a->K, a->kind) ? a->K : -1);
+    if (ls.R < 0) return R3DG_ERR_BAD_ARG;                 // a kind outside 0..3, mixed families, or R too large
+    const uint32_t all = a->K == 32 ? 0xffffffffu : (1u << a->K) - 1u;
+    ls.rect_mask = ls.shaped ? rect_mask(a->K, a->kind) : 0u;
+    ls.point_mask = ls.shaped ? 0u : point_mask(a->K, a->kind);
+    ls.dir_mask = ls.shaped ? 0u : all & ~ls.point_mask;
+    if (!a->points) return R3DG_ERR_BAD_ARG;
+    if (a->K > 0 && (!a->pos || (ls.rect_mask && (!a->a || !a->b)))) return R3DG_ERR_BAD_ARG;
+    if (shading && a->K > 0 && (!a->color || (ls.shaped && (!a->a || ((all & ~ls.rect_mask) && !a->cone)))))
+        return R3DG_ERR_BAD_ARG;
+    if ((long long)a->V * a->H * a->W > 0x7fffffffLL) return R3DG_ERR_UNSUPPORTED;
+    return 0;
+}
+
 }  // namespace r3dg

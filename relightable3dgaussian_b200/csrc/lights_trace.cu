@@ -5,7 +5,8 @@
 // from the bake: a subtree is skipped when the ray's segment [0, t_max] misses its box (exact, because a hit must also
 // meet its own leaf box within the segment), hits need peak t < (1 - 1e-5) t_max, and the ray stops at T < 1e-4 instead of 0.9.
 // Spot and rect lights (SHAPED LIGHTS; DESIGN.md §4.28) trace the same point-light rays towards a spot's position or
-// a rect's hashed stratified samples, in bvh_shaped_lights_kernel.
+// a rect's hashed stratified samples, in bvh_shaped_lights_kernel.  The per-pixel lights (PIXEL LIGHTS; DESIGN.md
+// §4.30) trace the same rays from every valid pixel's surface point, in bvh_pixel_lights_kernel.
 #include <cmath>
 #include "bvh.cuh"
 #include "kernels.h"
@@ -18,10 +19,13 @@ namespace r3dg {
 // A hit's peak t must lie below (1 - 1e-5) t_max: a Gaussian whose peak is at the light (the light at its centre) is
 // then clearly not a hit, instead of a tie that fp32 rounding decides
 #define LIGHT_T_MAX_MARGIN (1.0f - 1e-5f)
+#define PL_TILE 8                   // pixels are numbered in PL_TILE x PL_TILE tiles, as pixel_trace.cu's PT_TILE
 
 // The shaped lights' persistent trace loop: bvh_lights_kernel's loop (kept as written there, so that its SASS is
 // unchanged) with the ray setup as a parameter.  `setup(ray, ...)` starts ray `ray` of the launch: its
-// direction d, origin o, segment tseg, hit bound thit and output index out (S: a ray source, inlined).
+// direction d, origin o, segment tseg, hit bound thit and output index out (S: a ray source, inlined).  A source
+// with S::kDeclines may return false for a ray it does not trace (a masked pixel's, whose T it writes, or one outside
+// the image); such rays hold no lane: the refill repeats until every lane has a ray or the rays are exhausted.
 template <class S>
 __device__ __forceinline__ void trace_shadow_rays(const S& setup, long long num_rays, int NI, const float4* __restrict__ packets,
                                                   float* __restrict__ shadows, unsigned long long* counter,
@@ -34,23 +38,27 @@ __device__ __forceinline__ void trace_shadow_rays(const S& setup, long long num_
     float ox = 0, oy = 0, oz = 0, dx = 0, dy = 0, dz = 0, ix = 0, iy = 0, iz = 0, tseg = 0, thit = 0, T = 1.0f;
     while (true) {
         // ---- refill idle lanes from the global ray counter (warp-aggregated), as the bake does ----
-        const unsigned want = __ballot_sync(0xffffffffu, !has_ray && !exhausted);
-        if (want) {
-            const int leader = __ffs(want) - 1;
-            unsigned long long base = 0;
-            if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(want));
-            base = __shfl_sync(0xffffffffu, base, leader);
-            if (!has_ray && !exhausted) {
-                const long long ray = (long long)base + __popc(want & ((1u << lane) - 1u));
-                if (ray < num_rays) {
-                    setup(ray, ox, oy, oz, dx, dy, dz, tseg, thit, out);
-                    ix = div_(1.0f, dx); iy = div_(1.0f, dy); iz = div_(1.0f, dz);
-                    has_ray = true; T = 1.0f;
-                    st.sp = 0; st.push(NI == 0 ? -1 : 0);         // root (a lone leaf when P == 1)
-                } else {
-                    exhausted = true;
+        while (true) {
+            const unsigned want = __ballot_sync(0xffffffffu, !has_ray && !exhausted);
+            if (want) {
+                const int leader = __ffs(want) - 1;
+                unsigned long long base = 0;
+                if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(want));
+                base = __shfl_sync(0xffffffffu, base, leader);
+                if (!has_ray && !exhausted) {
+                    const long long ray = (long long)base + __popc(want & ((1u << lane) - 1u));
+                    if (ray < num_rays) {
+                        if (setup(ray, ox, oy, oz, dx, dy, dz, tseg, thit, out)) {
+                            ix = div_(1.0f, dx); iy = div_(1.0f, dy); iz = div_(1.0f, dz);
+                            has_ray = true; T = 1.0f;
+                            st.sp = 0; st.push(NI == 0 ? -1 : 0);         // root (a lone leaf when P == 1)
+                        }
+                    } else {
+                        exhausted = true;
+                    }
                 }
             }
+            if (!S::kDeclines || !want) break;
         }
         if (!__any_sync(0xffffffffu, has_ray)) break;
         // ---- a bounded burst of traversal steps, ended early once 8+ lanes can be refilled (the bake's policy) ----
@@ -199,44 +207,11 @@ __global__ void __launch_bounds__(LT_THREADS) bvh_lights_kernel(int P, int K, co
     }
 }
 
-// Spot and rect lights.  Ray r = (leaf slot r / R, column r % R); column c belongs to light sRay[c] >> 8 (its sample
-// sRay[c] & 255).  A spot's ray is a point light's at pos, a rect sample's the same towards its y_q.
-struct ShapedRays {
-    int NI, R, M;
-    uint32_t rect_mask, seed;
-    const float* sL;                 // [K][9]: pos, u (or the axis), v
-    const uint16_t* sRay;
-    const float4* packets;
-    const int32_t* nodes;
-    __device__ __forceinline__ void operator()(long long ray, float& ox, float& oy, float& oz, float& dx, float& dy, float& dz,
-                                               float& tseg, float& thit, long long& out) const {
-        const long long slot = ray / R;
-        const int col = (int)(ray - slot * R);
-        const LeafRecord self = load_leaf(packets + (size_t)(NI + slot) * 4);
-        const int g = nodes[(size_t)(NI + slot) * 5 + 3];
-        const int j = sRay[col] >> 8, q = sRay[col] & 255;
-        const float* L = sL + 9 * j;
-        float y[3];
-        if ((rect_mask >> j) & 1) {
-            float s, t;
-            rect_sample(L, L + 3, L + 6, M, rect_hash(seed, (uint32_t)g, (uint32_t)j), q, s, t, y);
-        } else {
-            y[0] = L[0]; y[1] = L[1]; y[2] = L[2];
-        }
-        ray_to_point(y, self.mx, self.my, self.mz, ox, oy, oz, dx, dy, dz, tseg, thit);
-        out = (long long)g * R + col;
-    }
-};
-
-__global__ void __launch_bounds__(LT_THREADS) bvh_shaped_lights_kernel(int P, int K, int R, int M, uint32_t rect_mask, uint32_t seed,
-                                                                       const float* __restrict__ pos, const float* __restrict__ a,
-                                                                       const float* __restrict__ b,
-                                                                       const float4* __restrict__ packets,
-                                                                       const int32_t* __restrict__ nodes,
-                                                                       float* __restrict__ shadows, unsigned long long* counter) {
-    __shared__ int sStack[TRACE_STACK_SH][LT_THREADS];
-    __shared__ float sL[9 * R3DG_MAX_LIGHTS];
-    __shared__ uint16_t sRay[R3DG_MAX_SHAPED_RAYS];
+// The lights' ray targets in shared memory: sL [K][9] = pos, and u, v of a rect; column c of a Gaussian or pixel
+// belongs to light sRay[c] >> 8 (its sample sRay[c] & 255), 1 column per light and M^2 per rect, in light order
+__device__ __forceinline__ void stage_light_rays(int K, int M, uint32_t rect_mask, const float* __restrict__ pos,
+                                                 const float* __restrict__ a, const float* __restrict__ b, float* sL,
+                                                 uint16_t* sRay) {
     const int tid = threadIdx.x;
     for (int i = tid; i < 3 * K; i += LT_THREADS) {
         const int j = i / 3, c = i - 3 * j;
@@ -253,9 +228,114 @@ __global__ void __launch_bounds__(LT_THREADS) bvh_shaped_lights_kernel(int P, in
         }
     }
     __syncthreads();
+}
+
+// Spot and rect lights.  Ray r = (leaf slot r / R, column r % R); column c belongs to light sRay[c] >> 8 (its sample
+// sRay[c] & 255).  A spot's ray is a point light's at pos, a rect sample's the same towards its y_q.
+struct ShapedRays {
+    static constexpr bool kDeclines = false;
+    int NI, R, M;
+    uint32_t rect_mask, seed;
+    const float* sL;                 // [K][9]: pos, u (or the axis), v
+    const uint16_t* sRay;
+    const float4* packets;
+    const int32_t* nodes;
+    __device__ __forceinline__ bool operator()(long long ray, float& ox, float& oy, float& oz, float& dx, float& dy, float& dz,
+                                               float& tseg, float& thit, long long& out) const {
+        const long long slot = ray / R;
+        const int col = (int)(ray - slot * R);
+        const LeafRecord self = load_leaf(packets + (size_t)(NI + slot) * 4);
+        const int g = nodes[(size_t)(NI + slot) * 5 + 3];
+        const int j = sRay[col] >> 8, q = sRay[col] & 255;
+        const float* L = sL + 9 * j;
+        float y[3];
+        if ((rect_mask >> j) & 1) {
+            float s, t;
+            rect_sample(L, L + 3, L + 6, M, rect_hash(seed, (uint32_t)g, (uint32_t)j), q, s, t, y);
+        } else {
+            y[0] = L[0]; y[1] = L[1]; y[2] = L[2];
+        }
+        ray_to_point(y, self.mx, self.my, self.mz, ox, oy, oz, dx, dy, dz, tseg, thit);
+        out = (long long)g * R + col;
+        return true;
+    }
+};
+
+__global__ void __launch_bounds__(LT_THREADS) bvh_shaped_lights_kernel(int P, int K, int R, int M, uint32_t rect_mask, uint32_t seed,
+                                                                       const float* __restrict__ pos, const float* __restrict__ a,
+                                                                       const float* __restrict__ b,
+                                                                       const float4* __restrict__ packets,
+                                                                       const int32_t* __restrict__ nodes,
+                                                                       float* __restrict__ shadows, unsigned long long* counter) {
+    __shared__ int sStack[TRACE_STACK_SH][LT_THREADS];
+    __shared__ float sL[9 * R3DG_MAX_LIGHTS];
+    __shared__ uint16_t sRay[R3DG_MAX_SHAPED_RAYS];
+    stage_light_rays(K, M, rect_mask, pos, a, b, sL, sRay);
     const int NI = P - 1;
     const ShapedRays setup{NI, R, M, rect_mask, seed, sL, sRay, packets, nodes};
     trace_shadow_rays(setup, (long long)P * R, NI, packets, shadows, counter, sStack);
+}
+
+// Per-pixel lights (PIXEL LIGHTS).  Ray r = (cell r / R, column r % R); cell c of view v = c / cells is pixel (c % 64)
+// of tile (c % cells) / 64, tiles in rows of tiles_x (pixel_trace.cu's numbering).  Column c is a directional light's
+// ray (dir_mask), a rect sample's towards y_q with the pixel's index p in the hash, or a point light's or spot's
+// towards pos.  Output T[v,c,p].
+struct PixelLightRays {
+    static constexpr bool kDeclines = true;
+    int R, M, W, H, tiles_x;
+    uint32_t dir_mask, rect_mask, seed;
+    long long cells;                 // PT_TILE^2 * tiles per view
+    const float* sL;
+    const uint16_t* sRay;
+    const float* points;             // [V,3,H,W]
+    const uint8_t* mask;             // [V,H,W] or NULL
+    float* T;
+    __device__ __forceinline__ bool operator()(long long ray, float& ox, float& oy, float& oz, float& dx, float& dy, float& dz,
+                                               float& tseg, float& thit, long long& out) const {
+        const long long cell = ray / R;
+        const int col = (int)(ray - cell * R);
+        const long long v = cell / cells;
+        const long long c = cell - v * cells;
+        const long long tile = c / (PL_TILE * PL_TILE);
+        const int w = (int)(c - tile * (PL_TILE * PL_TILE));
+        const int px = (int)(tile % tiles_x) * PL_TILE + w % PL_TILE, py = (int)(tile / tiles_x) * PL_TILE + w / PL_TILE;
+        if (px >= W || py >= H) return false;
+        const size_t HW = (size_t)H * W, p = (size_t)py * W + px;
+        out = ((long long)v * R + col) * (long long)HW + (long long)p;
+        if (mask && !mask[v * HW + p]) { T[out] = 0.0f; return false; }
+        const float* pb = points + 3 * v * HW + p;
+        const float mx = pb[0], my = pb[HW], mz = pb[2 * HW];
+        const int j = sRay[col] >> 8, q = sRay[col] & 255;
+        const float* L = sL + 9 * j;
+        if ((dir_mask >> j) & 1) {                       // bvh_lights_kernel's directional ray
+            const LightDir ld = light_dir(0, L, mx, my, mz);
+            dx = ld.l[0]; dy = ld.l[1]; dz = ld.l[2];
+            ox = add_(mx, mul_(dx, LIGHT_ORIGIN_OFFSET));
+            oy = add_(my, mul_(dy, LIGHT_ORIGIN_OFFSET));
+            oz = add_(mz, mul_(dz, LIGHT_ORIGIN_OFFSET));
+            tseg = INFINITY; thit = INFINITY;
+        } else if ((rect_mask >> j) & 1) {
+            float s, t, y[3];
+            rect_sample(L, L + 3, L + 6, M, rect_hash(seed, (uint32_t)p, (uint32_t)j), q, s, t, y);
+            ray_to_point(y, mx, my, mz, ox, oy, oz, dx, dy, dz, tseg, thit);
+        } else {
+            ray_to_point(L, mx, my, mz, ox, oy, oz, dx, dy, dz, tseg, thit);
+        }
+        return true;
+    }
+};
+
+__global__ void __launch_bounds__(LT_THREADS) bvh_pixel_lights_kernel(int P, int K, long long num_rays, PixelLightRays rays,
+                                                                      const float* __restrict__ pos, const float* __restrict__ a,
+                                                                      const float* __restrict__ b,
+                                                                      const float4* __restrict__ packets,
+                                                                      unsigned long long* counter) {
+    __shared__ int sStack[TRACE_STACK_SH][LT_THREADS];
+    __shared__ float sL[9 * R3DG_MAX_LIGHTS];
+    __shared__ uint16_t sRay[R3DG_MAX_SHAPED_RAYS];
+    stage_light_rays(K, rays.M, rays.rect_mask, pos, a, b, sL, sRay);
+    rays.sL = sL; rays.sRay = sRay;
+    trace_shadow_rays(rays, num_rays, P - 1, packets, rays.T, counter, sStack);
 }
 
 // ---- host launcher ------------------------------------------------------------------------
@@ -314,3 +394,37 @@ int launch_bvh_shaped_lights(const r3dg_shaped_light_args* a, const int32_t* nod
 }
 
 }  // namespace r3dg
+
+using namespace r3dg;
+extern "C" {
+
+size_t r3dg_bvh_trace_pixel_lights_tmp_bytes(int P) { return bvh_lights_tmp_bytes(P); }
+
+int r3dg_bvh_trace_pixel_lights(const r3dg_pixel_light_args* a, int P, const int32_t* nodes, const float* aabbs,
+                                const float* means3D, const float* covs3D, const float* opacities, const float* normals,
+                                float* T, void* tmp, size_t tmp_bytes, r3dg_stream_t stream_) {
+    PixelLightSet ls;
+    const int err = pixel_light_set(a, false, ls);
+    if (err != 0) return err;
+    if (P < 1 || !nodes || !aabbs || !means3D || !covs3D || !opacities || !normals || !T || !tmp) return R3DG_ERR_BAD_ARG;
+    if (tmp_bytes < bvh_lights_tmp_bytes(P)) return R3DG_ERR_BAD_ARG;
+    if (a->K == 0) return 0;                             // T [V,0,H,W] is empty
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    unsigned long long* counter = (unsigned long long*)tmp;
+    float4* packets = (float4*)((char*)tmp + 256);
+    R3DG_CUDA_TRY(cudaMemsetAsync(counter, 0, 8, stream));
+    const int rc = launch_bvh_pack(P, nodes, aabbs, means3D, covs3D, opacities, normals, packets, stream);
+    if (rc != 0) return rc;
+    const int tiles_x = (a->W + PL_TILE - 1) / PL_TILE, tiles_y = (a->H + PL_TILE - 1) / PL_TILE;
+    const long long cells = (long long)tiles_x * tiles_y * PL_TILE * PL_TILE;
+    const PixelLightRays rays{ls.R, a->M, a->W, a->H, tiles_x, ls.dir_mask, ls.rect_mask, a->seed, cells, nullptr, nullptr,
+                              a->points, a->mask, T};
+    const long long num_rays = (long long)a->V * cells * ls.R;
+    const long long want = (num_rays + LT_THREADS - 1) / LT_THREADS;
+    const int blocks = (int)(want < (long long)num_sms() * 16 ? want : (long long)num_sms() * 16);
+    bvh_pixel_lights_kernel<<<blocks, LT_THREADS, 0, stream>>>(P, a->K, num_rays, rays, a->pos, a->a, a->b, packets, counter);
+    R3DG_CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+}  // extern "C"

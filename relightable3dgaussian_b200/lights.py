@@ -14,6 +14,10 @@ vec and color.  Normals and shadows get none, as in the shading step.  Every out
 
 `ShapedLights` holds spot and rectangular area lights (SHAPED LIGHTS): `RayTracer.trace_shaped_lights` traces their
 shadows T [P,R] (one ray per spot, M x M stratified rays per rect), `shade_shaped` their terms, in the same conventions.
+
+Either set also shades every pixel of the per-pixel shading's G-buffer (PIXEL LIGHTS): `RayTracer.trace_pixel_lights`
+traces T [R,H,W] from each pixel's surface point, and `shade_pixels` returns terms to add to `shading.shade_pixels`'
+outputs.
 """
 import ctypes
 
@@ -287,3 +291,108 @@ def shade_shaped(base_color, roughness, normals, viewdirs, means3D, lights, shad
     if one:
         pbr, diffuse, specular = pbr[0], diffuse[0], specular[0]
     return pbr, {"diffuse_light": diffuse, "specular": specular}
+
+
+# ---- per-pixel lights --------------------------------------------------------------------------------------------
+def _fields(lights):
+    """The set's differentiable fields in the PIXEL LIGHTS order: (vec, color) of a Lights set, (pos, a, b, color,
+    cone) of a ShapedLights set."""
+    return (lights.vec, lights.color) if isinstance(lights, Lights) else (lights.pos, lights.a, lights.b, lights.color,
+                                                                          lights.cone)
+
+
+def num_rays(lights):
+    """R: the shadow columns of a Lights set (one per light) or a ShapedLights set (lights.num_rays())."""
+    return len(lights) if isinstance(lights, Lights) else lights.num_rays()
+
+
+def pixel_light_args(lights, points, mask):
+    """PixelLightArgs with the set, views, size, points and mask of a per-pixel light call, and the tensors it points to
+    (which must outlive the launch): (args, lead, keep) with lead = (leading shape, H, W)."""
+    from .shading import _mask, _views
+    if not isinstance(lights, (Lights, ShapedLights)):
+        raise TypeError(f"lights must be a Lights or a ShapedLights set (got {type(lights).__name__})")
+    p, lead = _views(points, 3, "points")
+    m = _mask(mask, lead)
+    fs = [_lib.f32(t) for t in _fields(lights)]
+    if not all(t.is_cuda for t in fs):
+        raise RuntimeError("per-pixel lights run on the GPU only (the light set must be on the GPU)")
+    a = _lib.PixelLightArgs()
+    a.V, a.H, a.W, a.K = p.shape[0], lead[1], lead[2], len(lights)
+    a.kind = lights.kind.data_ptr() if len(lights) > 0 else None
+    a.points, a.mask = p.data_ptr(), _lib.ptr(m)
+    if isinstance(lights, Lights):
+        a.M, a.seed = 1, 0
+        a.pos, a.color = [_lib.ptr(t) for t in fs]
+    else:
+        a.M, a.seed = lights.M, lights.seed
+        a.pos, a.a, a.b, a.color, a.cone = [_lib.ptr(t) for t in fs]
+    return a, lead, [p, m] + fs
+
+
+class _ShadePixelLights(torch.autograd.Function):
+    """The per-pixel light terms of V views: one node with gradients to base_color, roughness and the light fields."""
+
+    @staticmethod
+    def forward(ctx, base_color, roughness, normal, points, campos, shadows, mask, lights, *fields):
+        from .shading import _views
+        a, lead, keep = pixel_light_args(lights, points, mask)
+        V, H, W = a.V, a.H, a.W
+        b, _ = _views(base_color, 3, "base_color", lead)
+        r, _ = _views(roughness, 1, "roughness", lead)
+        n, _ = _views(normal, 3, "normal", lead)
+        T, _ = _views(shadows, num_rays(lights), "shadows", lead)
+        cp = _lib.f32(campos).reshape(-1, 3)
+        if cp.shape[0] != V or not cp.is_cuda:
+            raise ValueError(f"campos must be a CUDA [3] or [V,3] tensor with V = {V}, got {tuple(campos.shape)}")
+        a.base_color, a.roughness, a.normal, a.campos, a.shadows = (t.data_ptr() for t in (b, r, n, cp, T))
+        f = dict(dtype=torch.float32, device=b.device)
+        outs = [torch.empty((V, 3, H, W), **f) for _ in range(3)]
+        a.pbr, a.diffuse_light, a.specular = (t.data_ptr() for t in outs)
+        _lib.call("r3dg_shade_pixel_lights_forward", b.device, ctypes.byref(a), what="shade_pixels (lights)")
+        ctx.save_for_backward(b, r, n, cp, T)
+        ctx.keep, ctx.lights, ctx.lead = keep, lights, lead
+        return tuple(t.reshape(lead[0] + t.shape[1:]) for t in outs)
+
+    @staticmethod
+    def backward(ctx, g_pbr, g_diffuse, g_specular):
+        b, r, n, cp, T = ctx.saved_tensors
+        lights = ctx.lights
+        a, lead, keep = pixel_light_args(lights, ctx.keep[0], None)
+        a.mask = _lib.ptr(ctx.keep[1])
+        V, H, W, K = a.V, a.H, a.W, len(lights)
+        a.base_color, a.roughness, a.normal, a.campos, a.shadows = (t.data_ptr() for t in (b, r, n, cp, T))
+        dev = b.device
+        f = dict(dtype=torch.float32, device=dev)
+        g = [None if t is None else _lib.f32(t).reshape(V, 3, H, W) for t in (g_pbr, g_diffuse, g_specular)]
+        if g[0] is None:
+            g[0] = torch.zeros((V, 3, H, W), **f)
+        a.dL_dpbr, a.dL_ddiffuse_light, a.dL_dspecular = (_lib.ptr(t) for t in g)
+        d_base, d_rough = torch.empty_like(b), torch.empty_like(r)
+        d_fields = [torch.empty((K, t.shape[1]), **f) for t in _fields(lights)]
+        a.dL_dbase_color, a.dL_droughness = d_base.data_ptr(), d_rough.data_ptr()
+        if isinstance(lights, Lights):
+            a.dL_dpos, a.dL_dcolor = (_lib.ptr(t) for t in d_fields)
+        else:
+            a.dL_dpos, a.dL_da, a.dL_db, a.dL_dcolor, a.dL_dcone = (_lib.ptr(t) for t in d_fields)
+        work = _lib.scratch(_lib.load().r3dg_shade_pixel_lights_work_bytes(V, H, W, K), dev)
+        a.work, a.work_bytes = _lib.ptr(work), work.numel()
+        _lib.call("r3dg_shade_pixel_lights_backward", dev, ctypes.byref(a), what="shade_pixels (lights) backward")
+        shape = lambda t: t.reshape(ctx.lead[0] + t.shape[1:])
+        return (shape(d_base), shape(d_rough), None, None, None, None, None, None, *d_fields)
+
+
+def shade_pixels(base_color, roughness, normal, points, campos, lights, shadows, mask=None):
+    """The terms of `lights` (Lights or ShapedLights) at every pixel of the per-pixel shading's G-buffer (include/
+    r3dg_b200.h, PIXEL LIGHTS).  One view: base_color [3,H,W], roughness [1,H,W], normal [3,H,W], points [3,H,W],
+    campos [3], shadows T [R,H,W] from RayTracer.trace_pixel_lights and an optional mask [H,W] (bool or uint8).  V views
+    (1 <= V <= MAX_VIEWS): a leading V on every image and campos [V,3].
+
+    Each valid pixel is `shade` / `shade_shaped` of one row (mean = its point, the raw normal, viewdir = campos -
+    point, row index y W + x for the rect samples), bit for bit.  Returns dict(pbr, diffuse_light, specular), each
+    [.., 3,H,W], to add to shading.shade_pixels' outputs; masked pixels are 0.  Gradients: base_color, roughness and the
+    light fields (vec, color, or pos, a, b, color, cone), summed over pixels and views; none for normal, points, campos
+    or the shadows.  Every output is bitwise reproducible.  Inputs are checked before anything is launched."""
+    pbr, diffuse, specular = _ShadePixelLights.apply(base_color, roughness, normal, points, campos, shadows, mask, lights,
+                                                     *_fields(lights))
+    return {"pbr": pbr, "diffuse_light": diffuse, "specular": specular}

@@ -204,6 +204,29 @@ class RayTracer:
                   what="trace_pixels")
         return out.reshape(lead[0] + out.shape[1:])
 
+    @torch.no_grad()
+    def trace_pixel_lights(self, points, lights, means3D, symm_inv, opacity, gaussian_normals, mask=None):
+        """Shadow transmittance T [R,H,W] (or [V,R,H,W]) of `lights` (lights.Lights, R = K, or lights.ShapedLights,
+        R = num_rays(), trace_shaped_lights' column order) at every valid pixel of points [3,H,W] (or [V,3,H,W];
+        world-space surface points) through this tree (r3dg_bvh_trace_pixel_lights): column c is trace_lights' /
+        trace_shaped_lights' ray of a Gaussian whose mean is the pixel's point, a rect's samples hashed with the
+        pixel's index y W + x (the points lights.shade_pixels uses).  Pixels outside `mask` ([H,W] or [V,H,W]) trace
+        nothing and get 0.  No gradient.  A light placement is traced once per view."""
+        from .lights import num_rays, pixel_light_args
+        P = means3D.shape[0]
+        if not all(t.is_cuda for t in (means3D, symm_inv, opacity, gaussian_normals)):
+            raise RuntimeError("trace_pixel_lights runs on the GPU only (no CPU path)")
+        if means3D.shape != (P, 3) or gaussian_normals.shape != (P, 3) or symm_inv.shape != (P, 6) or opacity.numel() != P:
+            raise ValueError("means3D and gaussian_normals must be [P,3], symm_inv [P,6] and opacity [P]")
+        a, lead, keep = pixel_light_args(lights, points, mask)
+        out = torch.empty((a.V, num_rays(lights), a.H, a.W), dtype=torch.float32, device=points.device)
+        m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(gaussian_normals)
+        tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_pixel_lights_tmp_bytes(P), points.device)
+        _lib.call("r3dg_bvh_trace_pixel_lights", points.device, ctypes.byref(a), P, self.tree.data_ptr(), self.aabb.data_ptr(),
+                  m.data_ptr(), ci.data_ptr(), op.data_ptr(), nr.data_ptr(), out.data_ptr(), tmp.data_ptr(), tmp.numel(),
+                  what="trace_pixel_lights")
+        return out.reshape(lead[0] + out.shape[1:])
+
 
 @torch.no_grad()
 def fit_incident_sh(radiance, normals, degree=3, ridge=1e-3):
