@@ -1029,6 +1029,58 @@ int r3dg_env_pyramid_build(const float* env, int env_h, int env_w, float* pyrami
 size_t r3dg_shade_filtered_det_bytes(int env_h, int env_w);
 
 /* ------------------------------------------------------------------------------------------
+ * IMPORTANCE SAMPLING of the environment light (DESIGN.md §4.31).  The bake's Fibonacci directions ignore where
+ * the light is and where the BRDF points; under an HDR map with a small bright source their estimate does not
+ * converge to the rendering equation.  This sampler draws each shading point's N directions from three strategies
+ * and weights them by the multi-sample balance heuristic, so the shading step's unchanged estimator
+ * mean_i (f_d + f_s) L_i area_i (n.d_i)+ becomes an unbiased estimate of the integral.
+ *   Env table (r3dg_env_sampler_build, from the ACTIVATED env [He,We,3], He, We >= 2), on the cells of the
+ *   PREFILTERED ENVIRONMENT stencil: row j is the band [(j - 1/2) dt, (j + 1/2) dt] clipped to [0, pi],
+ *   dt = pi / (He-1); column i < We-1 the azimuth cell [(i - 1/2) dp, (i + 1/2) dp] modulo 2 pi, dp = 2 pi / (We-1)
+ *   (columns 0 and We-1 are one azimuth).  Cell weight = max(lum, 0) over the texel's 3 x 3 neighbourhood (wrapped
+ *   in azimuth, clamped in latitude; lum = 0.2126 R + 0.7152 G + 0.0722 B, a non-finite lum counts as 0) times the
+ *   cell's solid angle; all weights 0: the solid angles (uniform on the sphere).  The table holds the row CDF, each
+ *   row's column CDF (fp64 sums in a fixed order, rounded once to fp32: bitwise reproducible, no atomics) and each
+ *   cell's pdf per steradian, P(row) P(column | row) / solid angle from those rounded CDFs.  3 launches.
+ *   Strategies.  Samples i < n_env are env samples, then n_ggx GGX samples, then n_cos = N - n_env - n_ggx >= 1
+ *   cosine samples.  Sample k of a strategy s with n_s samples at shading point q (Gaussian row g, or pixel y W + x)
+ *   uses h = lowbias32(lowbias32(lowbias32(seed) ^ q) ^ s) (s = 0 env, 1 ggx, 2 cos), h1 = lowbias32(h ^ 0),
+ *   h2 = lowbias32(h ^ 1), u1 = (((2^32 k) / n_s + h1) mod 2^32 >> 8) 2^-24, u2 = ((k 0x9E3779B9 + h2) mod 2^32 >> 8)
+ *   2^-24 (integer division; a rank-1 lattice rotated per point).
+ *     env: row j by the row CDF (the largest j with cdf[j] <= u1), column i by row j's column CDF, remainders t1,
+ *       t2; cos theta = cos lo_j + t1 (cos hi_j - cos lo_j), formed from the table's 1 - cos (rows j <= (He-1)/2) or
+ *       1 + cos (the others) of the band edges, so sin theta keeps its precision at the poles; azimuth
+ *       pi - (i - 1/2 + t2) dp (the lookup's column
+ *       coordinate i - 1/2 + t2); the env-space direction is mapped to the world by T^T (T = env_transform, which
+ *       must be orthonormal: the lookup reads T d).  pdf: that of the cell T d falls in.
+ *     ggx: around Ns = n^ sign(n^.V^) (V^ = normalize(viewdir)), a2 = max(r^4, 1e-7): cos^2 theta_h =
+ *       (1 - u1) / (1 + (a2 - 1) u1) (sin^2 theta_h = a2 u1 / (1 + (a2 - 1) u1)), azimuth 2 pi u2, h rotated to Ns
+ *       by rotate_from_z, l = 2 (V^.h) h - V^.
+ *       pdf(l) = D(h) (Ns.h) / (4 V^.h) with h = normalize(V^ + l), D = a2 / (pi ((Ns.h)^2 (a2 - 1) + 1)^2); 0 when
+ *       Ns.h <= 0 or V^.h <= 0.  A sample whose own h has V^.h <= 0 gets area 0.  The BRDF is unchanged.
+ *     cos: (sqrt(u1) cos 2 pi u2, sqrt(u1) sin 2 pi u2, sqrt(1 - u1)) rotated to n^ = F.normalize(normal) by
+ *       rotate_from_z; pdf (n^.l)+ / pi.  It covers every direction where the integrand can be non-zero, so the
+ *       estimator is unbiased for any env, filter and table.
+ *   area_i = N / ((n_env p_env(d_i) + n_ggx p_ggx(d_i)) + n_cos p_cos(d_i)) (fp32), 0 when that denominator is not a
+ *   positive finite number.  The env filter's footprint is area_i / N.  Directions and areas carry no gradient; with
+ *   the pdf held fixed, sum_i df/p_i is an unbiased estimate of the gradient of the integral.  Every operation of
+ *   the sampler is rounded on its own, so any kernel that reproduces it gets the same bits.
+ * r3dg_env_sampler_floats: the table's floats, 0 for env_h or env_w < 2.
+ * r3dg_env_sampler_build: R3DG_ERR_BAD_ARG for a NULL pointer or env_h, env_w < 2, R3DG_ERR_UNSUPPORTED for more
+ * than 2^31 / 3 texels, before any launch.
+ * r3dg_sample_importance_dirs: dirs f32[P,N,3] and areas f32[P,N] of Gaussian rows g (q = g) from normals [P,3],
+ * viewdirs [P,3] and roughness [P] (read only when n_ggx > 0), a table and env_transform ([3,3] or NULL; the
+ * transform the shading step will use).  R3DG_ERR_BAD_ARG before any launch for P < 0, N < 1, n_env or n_ggx < 0,
+ * n_cos < 1, n_ggx > 0 without viewdirs or roughness, seed >= 2^32, or (P > 0) a NULL normals, table, dirs or
+ * areas.  One launch (none for P = 0).
+ * ------------------------------------------------------------------------------------------ */
+size_t r3dg_env_sampler_floats(int env_h, int env_w);
+int r3dg_env_sampler_build(const float* env, int env_h, int env_w, float* table, r3dg_stream_t stream);
+int r3dg_sample_importance_dirs(int P, int N, const float* normals, const float* viewdirs, const float* roughness,
+                                const float* table, const float* env_transform, int n_env, int n_ggx,
+                                unsigned long long seed, float* dirs, float* areas, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * PIXEL SHADING: the shading step's rendering equation at every pixel of rasterized material images
  * (deferred shading, DESIGN.md §4.29), with each pixel's visibility traced through the BVH.
  *   Layout: V views (1 <= V <= R3DG_MAX_VIEWS) of planar H x W images; view v's block of a [C,H,W] image
@@ -1091,6 +1143,18 @@ struct r3dg_pixel_args {
     int deterministic;
     void* det_work;
     size_t det_work_bytes;
+    /* Importance sampling (IMPORTANCE SAMPLING above).  sampler_table NULL: the Fibonacci directions above, unchanged.
+     * Otherwise sample i of pixel p = y W + x (q = p in every view) is the sampler's, with n_env env samples drawn under
+     * sampler_transform ([3,3] or NULL; the transform the table's samples follow, which may differ from the shading's
+     * env_transform), n_ggx GGX samples (they read roughness and campos; the trace reads them too) and
+     * N - n_env - n_ggx >= 1 cosine samples: the trace traces those directions, and the shading uses them with their
+     * areas (the filtered env's footprint is area_i / N).  mean_visibility is then mean_i T over the importance-sampled
+     * directions.  T must come from r3dg_bvh_trace_pixels with the same sampler fields.  Refused (R3DG_ERR_BAD_ARG):
+     * n_env or n_ggx < 0, n_cos < 1, n_ggx > 0 without roughness or campos (trace). */
+    const float* sampler_table;
+    int n_env, n_ggx;
+    uint32_t seed;
+    const float* sampler_transform;
 };
 
 size_t r3dg_bvh_trace_pixels_tmp_bytes(int P);

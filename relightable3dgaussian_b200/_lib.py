@@ -111,7 +111,9 @@ class PixelArgs(ctypes.Structure):
                 [(n, c_void_p) for n in ("env_pyramid", "dL_denv_pyramid", "visibility", "pbr", "diffuse_light", "specular",
                                          "mean_visibility", "dL_dpbr", "dL_ddiffuse_light", "dL_dspecular", "dL_dbase_color",
                                          "dL_droughness", "dL_dincidents", "dL_denv")] +
-                [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)])
+                [("deterministic", c_int), ("det_work", c_void_p), ("det_work_bytes", c_size_t)] +
+                [("sampler_table", c_void_p), ("n_env", c_int), ("n_ggx", c_int), ("seed", ctypes.c_uint32),
+                 ("sampler_transform", c_void_p)])
 
 
 class PixelLightArgs(ctypes.Structure):
@@ -249,6 +251,10 @@ SYMBOLS = [
     ("r3dg_env_pyramid_floats", c_size_t, [c_int, c_int]),
     ("r3dg_env_pyramid_build", c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     ("r3dg_shade_filtered_det_bytes", c_size_t, [c_int, c_int]),
+    ("r3dg_env_sampler_floats", c_size_t, [c_int, c_int]),
+    ("r3dg_env_sampler_build", c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    ("r3dg_sample_importance_dirs", c_int, [c_int, c_int] + [c_void_p] * 5 + [c_int, c_int, ctypes.c_ulonglong] +
+                                           [c_void_p, c_void_p, c_void_p]),
     ("r3dg_pack_features_forward", c_int, [c_int, c_int, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p, c_void_p]),
     ("r3dg_pack_features_backward", c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(PackSrc), c_void_p,
                                             c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -11,6 +11,7 @@
 // forward output equals the per-Gaussian kernel's on the pixel as a row, bit for bit.  A group of masked pixels does
 // no sample work and writes zeros.
 #include "bvh.cuh"
+#include "importance.cuh"
 #include "shading_eval.cuh"
 
 namespace r3dg {
@@ -70,17 +71,32 @@ __device__ __forceinline__ const float* view_transform(const ShadeArgs& a, const
     return a.transform && pv.per_view_transform ? a.transform + 9 * (size_t)v : a.transform;
 }
 
-template <bool SMEM_ENV, bool FILT>
+// the importance sampler's GGX frame of pixel vq (read only with GGX samples)
+__device__ __forceinline__ GgxFrame pixel_ggx_frame(const ShadeArgs& a, const PixelView& pv, const ImportanceSampler& smp, int v,
+                                                    size_t q, const GaussianOperands& o, float3 nh) {
+    GgxFrame f{};
+    if (smp.n_ggx > 0) {
+        const size_t HW = (size_t)a.P;
+        f = ggx_frame(nh, sub_(pv.campos[3 * v], pv.points[3 * v * HW + q]), sub_(pv.campos[3 * v + 1], pv.points[(3 * v + 1) * HW + q]),
+                      sub_(pv.campos[3 * v + 2], pv.points[(3 * v + 2) * HW + q]), o.rough);
+    }
+    return f;
+}
+
+// IS: the importance sampler's directions and areas (include/r3dg_b200.h, IMPORTANCE SAMPLING) instead of the canonical
+// sample table's with area 2 pi; the same sums in the same order
+template <bool SMEM_ENV, bool FILT, bool IS>
 __global__ void __launch_bounds__(SHADE_THREADS, FILT ? 5 : 6) pixel_shade_fwd_kernel(const ShadeArgs a, const PixelView pv,
-                                                                                      const EnvLevels lv) {
+                                                                                      const EnvLevels lv, ImportanceSampler smp) {
     extern __shared__ __align__(16) float s_pfwd[];     // [incident slots][sample table][env texture (SMEM_ENV)]
     constexpr int INC_FLOATS = SHADE_WARPS * PIX_GPW * SHADE_INC_STRIDE;
     float3* s_smp = reinterpret_cast<float3*>(s_pfwd + INC_FLOATS);
-    float* s_env = s_pfwd + INC_FLOATS + sample_table_floats(a.N);
+    float* s_env = s_pfwd + INC_FLOATS + (IS ? 0 : sample_table_floats(a.N));
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane & (PIX_G - 1), grp = lane / PIX_G;
     float* sinc = s_pfwd + (warp * PIX_GPW + grp) * SHADE_INC_STRIDE;
-    for (int i = threadIdx.x; i < a.N; i += SHADE_THREADS) s_smp[i] = fib_sample(i, a.N);
+    if constexpr (IS) smp.t = EnvTable(smp.table);
+    else for (int i = threadIdx.x; i < a.N; i += SHADE_THREADS) s_smp[i] = fib_sample(i, a.N);
     if (SMEM_ENV)
         for (int i = threadIdx.x; i < (FILT ? lv.total : a.He * a.We) * 3; i += SHADE_THREADS) s_env[i] = a.env[i];
     __syncthreads();
@@ -103,18 +119,23 @@ __global__ void __launch_bounds__(SHADE_THREADS, FILT ? 5 : 6) pixel_shade_fwd_k
         const float* vis_row = a.visibility + (size_t)v * a.N * HW + q;
         float pbr[3] = {0, 0, 0}, spec[3] = {0, 0, 0}, diff[3] = {0, 0, 0}, mv = 0;
         if (live) {
+            GgxFrame f{};
+            if constexpr (IS) f = pixel_ggx_frame(a, pv, smp, v, q, o, nh);
             for (int i = sub; i < a.N; i += PIX_G) {
-                const float3 d = rotate_from_z(nh.x, nh.y, nh.z, s_smp[i]);
+                float3 d;
+                float ar = PIX_AREA;
+                if constexpr (IS) d = importance_sample(smp, (uint32_t)q, i, nh, f, ar);
+                else d = rotate_from_z(nh.x, nh.y, nh.z, s_smp[i]);
                 const float vis = vis_row[(size_t)i * HW];
                 SampleEvalT<FILT> e;
-                eval_env_any<SMEM_ENV>(tr, env, a, lv, PIX_AREA * invN, d.x, d.y, d.z, vis, e);
+                eval_env_any<SMEM_ENV>(tr, env, a, lv, ar * invN, d.x, d.y, d.z, vis, e);
                 pixel_local(a, o, sinc, d, e);
                 eval_ggx<false>(o.V, o.Ns, o, d.x, d.y, d.z, e);
 #pragma unroll
                 for (int c = 0; c < 3; ++c) {                 // the per-Gaussian forward's expressions
                     const float loc = fmaxf(e.local_raw[c], 0.f);
                     const float Lc = loc + e.glob[c];
-                    const float T = Lc * PIX_AREA * e.ndi;
+                    const float T = Lc * ar * e.ndi;
                     const float fd = o.base[c] / PI_F;
                     pbr[c] += (fd + e.fs) * T; spec[c] += e.fs * T; diff[c] += T;
                 }
@@ -142,9 +163,9 @@ __global__ void __launch_bounds__(SHADE_THREADS, FILT ? 5 : 6) pixel_shade_fwd_k
 // inside the sample loop, so masked groups skip it).  3 resident CTAs (<= 168 registers): at 4 (128) every
 // mode but the deterministic ones spills a few words.  dL/dbase, dL/droughness and dL/dincidents are written per pixel
 // (zeros for masked ones), dL/denv is accumulated over every view.
-template <int ENV_MODE, bool FILT>
+template <int ENV_MODE, bool FILT, bool IS>
 __global__ void __launch_bounds__(SHADE_THREADS, 3)
-pixel_shade_bwd_kernel(const ShadeArgs a, const PixelView pv, const EnvLevels lv) {
+pixel_shade_bwd_kernel(const ShadeArgs a, const PixelView pv, const EnvLevels lv, ImportanceSampler smp) {
     static_assert(ENV_MODE != ENV_TAG, "the tagged mode's collectives need a warp-uniform sample loop");
     // [incident slots][SH-gradient accumulators][sample table][env ...]
     extern __shared__ __align__(16) float s_pbwd[];
@@ -157,8 +178,9 @@ pixel_shade_bwd_kernel(const ShadeArgs a, const PixelView pv, const EnvLevels lv
     float* sinc = s_pbwd + (warp * PIX_GPW + grp) * SHADE_INC_STRIDE;
     float4* acc4 = reinterpret_cast<float4*>(s_pbwd + INC_FLOATS) + threadIdx.x;
     float3* s_smp = reinterpret_cast<float3*>(s_pbwd + INC_FLOATS + DINC_FLOATS);
-    for (int i = threadIdx.x; i < a.N; i += SHADE_THREADS) s_smp[i] = fib_sample(i, a.N);
-    EnvGrad<ENV_MODE> eg(a, s_pbwd + INC_FLOATS + DINC_FLOATS + sample_table_floats(a.N), warp, FILT ? lv.total : a.He * a.We);
+    if constexpr (IS) smp.t = EnvTable(smp.table);
+    else for (int i = threadIdx.x; i < a.N; i += SHADE_THREADS) s_smp[i] = fib_sample(i, a.N);
+    EnvGrad<ENV_MODE> eg(a, s_pbwd + INC_FLOATS + DINC_FLOATS + (IS ? 0 : sample_table_floats(a.N)), warp, FILT ? lv.total : a.He * a.We);
     __syncthreads();                                     // the sample table (EnvGrad syncs only in its shared-memory modes)
     const float invN = 1.0f / (float)a.N;
     const size_t HW = (size_t)a.P, total = (size_t)pv.V * HW;
@@ -188,11 +210,16 @@ pixel_shade_bwd_kernel(const ShadeArgs a, const PixelView pv, const EnvLevels lv
 #pragma unroll
         for (int k = 0; k < 12; ++k) acc4[k * SHADE_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (live) {
+            GgxFrame f{};
+            if constexpr (IS) f = pixel_ggx_frame(a, pv, smp, v, q, o, nh);
             for (int i = sub; i < a.N; i += PIX_G) {
-                const float3 d = rotate_from_z(nh.x, nh.y, nh.z, s_smp[i]);
+                float3 d;
+                float ar = PIX_AREA;
+                if constexpr (IS) d = importance_sample(smp, (uint32_t)q, i, nh, f, ar);
+                else d = rotate_from_z(nh.x, nh.y, nh.z, s_smp[i]);
                 const float vis = vis_row[(size_t)i * HW];
                 SampleEvalT<FILT> e;
-                eval_env_any<SMEM_ENV>(tr, eg.env, a, lv, PIX_AREA * invN, d.x, d.y, d.z, vis, e);
+                eval_env_any<SMEM_ENV>(tr, eg.env, a, lv, ar * invN, d.x, d.y, d.z, vis, e);
                 pixel_local(a, o, sinc, d, e);
                 eval_ggx<true>(o.V, o.Ns, o, d.x, d.y, d.z, e);
                 float dfs = 0.f;
@@ -200,11 +227,11 @@ pixel_shade_bwd_kernel(const ShadeArgs a, const PixelView pv, const EnvLevels lv
 #pragma unroll
                 for (int c = 0; c < 3; ++c) {                 // the per-Gaussian backward's expressions
                     const float loc = fmaxf(e.local_raw[c], 0.f);
-                    const float T = (loc + e.glob[c]) * PIX_AREA * e.ndi;
+                    const float T = (loc + e.glob[c]) * ar * e.ndi;
                     const float fd = o.base[c] * INV_PI_F;
                     const float dT = gp[c] * (fd + e.fs) + gs[c] * e.fs + gd[c];
                     dbase[c] += gp[c] * T * INV_PI_F; dfs += (gp[c] + gs[c]) * T;
-                    const float dL = dT * PIX_AREA * e.ndi;
+                    const float dL = dT * ar * e.ndi;
                     dLg[c] = e.local_raw[c] >= 0.f ? dL : 0.f;      // clamp_min(0) passes the gradient at equality
                     dG[c] = dL * vis;                                // -> env texels (grid_sample backward)
                 }
@@ -237,35 +264,43 @@ pixel_shade_bwd_kernel(const ShadeArgs a, const PixelView pv, const EnvLevels lv
     eg.flush(a);
 }
 
-static size_t pixel_fixed_bytes(int N) {
-    return (size_t)SHADE_WARPS * PIX_GPW * SHADE_INC_STRIDE * sizeof(float) + (size_t)sample_table_floats(N) * sizeof(float);
+static size_t pixel_fixed_bytes(int N, bool is) {
+    return (size_t)SHADE_WARPS * PIX_GPW * SHADE_INC_STRIDE * sizeof(float) + (is ? 0 : (size_t)sample_table_floats(N) * sizeof(float));
 }
 
 static int pixel_units(const PixelView& pv, const ShadeArgs& a) { return (int)(((size_t)pv.V * a.P + PIX_GPW - 1) / PIX_GPW); }
 
-static int launch_pixel_forward(ShadeArgs a, const PixelView& pv, const EnvLevels& lv, bool filt, cudaStream_t stream) {
+static int launch_pixel_forward(ShadeArgs a, const PixelView& pv, const EnvLevels& lv, bool filt, const ImportanceSampler& smp,
+                                cudaStream_t stream) {
     const size_t env_bytes = env_texels(a, lv, filt) * 3 * sizeof(float);
     const bool smem_env = env_bytes <= 40 * 1024;       // as the per-Gaussian forward
     a.env_in_smem = smem_env;
-    const size_t smem = pixel_fixed_bytes(a.N) + (smem_env ? env_bytes : 0);
+    const bool is = smp.table != nullptr;
+    const size_t smem = pixel_fixed_bytes(a.N, is) + (smem_env ? env_bytes : 0);
     const int units = pixel_units(pv, a), sms = num_sms();
-    if (filt) return smem_env ? shade_launch(pixel_shade_fwd_kernel<true, true>, a, units, sms, smem, stream, pv, lv)
-                              : shade_launch(pixel_shade_fwd_kernel<false, true>, a, units, sms, smem, stream, pv, lv);
-    return smem_env ? shade_launch(pixel_shade_fwd_kernel<true, false>, a, units, sms, smem, stream, pv, lv)
-                    : shade_launch(pixel_shade_fwd_kernel<false, false>, a, units, sms, smem, stream, pv, lv);
+    const auto go = [&](auto k) { return shade_launch(k, a, units, sms, smem, stream, pv, lv, smp); };
+    if (is) {
+        if (filt) return smem_env ? go(pixel_shade_fwd_kernel<true, true, true>) : go(pixel_shade_fwd_kernel<false, true, true>);
+        return smem_env ? go(pixel_shade_fwd_kernel<true, false, true>) : go(pixel_shade_fwd_kernel<false, false, true>);
+    }
+    if (filt) return smem_env ? go(pixel_shade_fwd_kernel<true, true, false>) : go(pixel_shade_fwd_kernel<false, true, false>);
+    return smem_env ? go(pixel_shade_fwd_kernel<true, false, false>) : go(pixel_shade_fwd_kernel<false, false, false>);
 }
 
 // the env-gradient mode as the per-Gaussian backward picks it at its default highest mode
-static int launch_pixel_backward(ShadeArgs a, const PixelView& pv, const EnvLevels& lv, bool filt, cudaStream_t stream) {
+static int launch_pixel_backward(ShadeArgs a, const PixelView& pv, const EnvLevels& lv, bool filt, const ImportanceSampler& smp,
+                                 cudaStream_t stream) {
     const int sms = num_sms();
     return shade_backward(a, pv.V, ENV_CAS, env_texels(a, lv, filt), sms, stream, [&](auto mode, const ShadeArgs& x, size_t env_smem) {
         constexpr int M = decltype(mode)::value;
         if constexpr (M == ENV_TAG) return (int)R3DG_ERR_UNSUPPORTED;     // above the cap: never selected
         else {
-            const size_t smem = pixel_fixed_bytes(x.N) + (size_t)48 * SHADE_THREADS * sizeof(float) + env_smem;
+            const bool is = smp.table != nullptr;
+            const size_t smem = pixel_fixed_bytes(x.N, is) + (size_t)48 * SHADE_THREADS * sizeof(float) + env_smem;
             const int units = pixel_units(pv, x);
-            return filt ? shade_launch(pixel_shade_bwd_kernel<M, true>, x, units, sms, smem, stream, pv, lv)
-                        : shade_launch(pixel_shade_bwd_kernel<M, false>, x, units, sms, smem, stream, pv, lv);
+            const auto go = [&](auto k) { return shade_launch(k, x, units, sms, smem, stream, pv, lv, smp); };
+            if (is) return filt ? go(pixel_shade_bwd_kernel<M, true, true>) : go(pixel_shade_bwd_kernel<M, false, true>);
+            return filt ? go(pixel_shade_bwd_kernel<M, true, false>) : go(pixel_shade_bwd_kernel<M, false, false>);
         }
     });
 }
@@ -277,7 +312,7 @@ using namespace r3dg;
 extern "C" {
 
 // the shared checks of both directions; ShadeArgs and PixelView of the call
-static int pixel_args(const r3dg_pixel_args* s, ShadeArgs& a, PixelView& pv) {
+static int pixel_args(const r3dg_pixel_args* s, ShadeArgs& a, PixelView& pv, ImportanceSampler& smp) {
     if (!s || s->V < 1 || s->V > R3DG_MAX_VIEWS || s->H < 1 || s->W < 1 || s->N < 1 || s->env_h < 1 || s->env_w < 1)
         return R3DG_ERR_BAD_ARG;
     if (!s->base_color || !s->roughness || !s->normal || !s->points || !s->campos || !s->env || !s->visibility)
@@ -285,6 +320,12 @@ static int pixel_args(const r3dg_pixel_args* s, ShadeArgs& a, PixelView& pv) {
     if (s->transform_per_view && !s->env_transform) return R3DG_ERR_BAD_ARG;
     if ((size_t)s->N * sizeof(float3) > BAKE_SAMPLE_SMEM) return R3DG_ERR_UNSUPPORTED;
     if ((long long)s->V * s->H * s->W > 0x7fffffffLL) return R3DG_ERR_UNSUPPORTED;
+    if (s->sampler_table && (s->n_env < 0 || s->n_ggx < 0 || (long long)s->N - s->n_env - s->n_ggx < 1)) return R3DG_ERR_BAD_ARG;
+    smp = ImportanceSampler{};
+    if (s->sampler_table) {
+        smp.table = s->sampler_table; smp.T = s->sampler_transform;
+        smp.N = s->N; smp.n_env = s->n_env; smp.n_ggx = s->n_ggx; smp.seed = s->seed;
+    }
     a = ShadeArgs{};
     a.P = s->H * s->W; a.N = s->N; a.He = s->env_h; a.We = s->env_w;
     a.base_color = s->base_color; a.roughness = s->roughness; a.normals = s->normal; a.incidents = s->incidents;
@@ -300,19 +341,21 @@ static int pixel_args(const r3dg_pixel_args* s, ShadeArgs& a, PixelView& pv) {
 int r3dg_shade_pixels_forward(const r3dg_pixel_args* s, r3dg_stream_t stream) {
     ShadeArgs a;
     PixelView pv;
-    const int rc = pixel_args(s, a, pv);
+    ImportanceSampler smp;
+    const int rc = pixel_args(s, a, pv, smp);
     if (rc) return rc;
     if (!a.pbr || !a.diffuse || !a.specular || !a.mean_vis) return R3DG_ERR_BAD_ARG;
     const EnvLevels lv = env_levels(a.He, a.We);
     const bool filt = s->env_pyramid && lv.L > 1;
     if (filt) a.env = s->env_pyramid;
-    return launch_pixel_forward(a, pv, lv, filt, (cudaStream_t)stream);
+    return launch_pixel_forward(a, pv, lv, filt, smp, (cudaStream_t)stream);
 }
 
 int r3dg_shade_pixels_backward(const r3dg_pixel_args* s, r3dg_stream_t stream) {
     ShadeArgs a;
     PixelView pv;
-    int rc = pixel_args(s, a, pv);
+    ImportanceSampler smp;
+    int rc = pixel_args(s, a, pv, smp);
     if (rc) return rc;
     if (!a.g_pbr || !a.d_base || !a.d_rough || !a.d_env || (a.incidents && !a.d_incidents)) return R3DG_ERR_BAD_ARG;
     if (s->env_pyramid && !s->dL_denv_pyramid) return R3DG_ERR_BAD_ARG;
@@ -328,7 +371,7 @@ int r3dg_shade_pixels_backward(const r3dg_pixel_args* s, r3dg_stream_t stream) {
         a.det_scale = (uint32_t*)((char*)s->det_work + det_bytes(n));
     }
     const cudaStream_t st = (cudaStream_t)stream;
-    rc = launch_pixel_backward(a, pv, lv, filt, st);
+    rc = launch_pixel_backward(a, pv, lv, filt, smp, st);
     if (rc || !filt) return rc;
     return launch_env_pyramid_adjoint(lv, a.d_env, d_env, st);               // dL/denv through the pyramid
 }

@@ -3,6 +3,7 @@
 // sample i) is the one r3dg_bvh_trace_opacity traces for origin points_p, direction rotate_from_z(n^, fib_sample(i, N))
 // and origin offset 0.05, so T is the same bits.  Compiled with the bake's flags (bvh.cu).
 #include "bvh.cuh"
+#include "importance.cuh"
 #include "kernels.h"
 
 namespace r3dg {
@@ -116,6 +117,52 @@ struct PixelRays {
     }
 };
 
+// The same rays along the importance sampler's directions (include/r3dg_b200.h, IMPORTANCE SAMPLING): sample i of
+// pixel p = y W + x is importance_sample(q = p), with the GGX frame of viewdir campos_v - point_p and the pixel's
+// roughness when the sampler has GGX samples.
+struct ImportancePixelRays {
+    int N, W, H, tiles_x;
+    long long cells;
+    const float *normal, *points, *roughness, *campos;   // roughness [V,1,H,W], campos [V,3]: read when n_ggx > 0
+    const uint8_t* mask;
+    ImportanceSampler s;
+    float* T;
+    __device__ __forceinline__ bool operator()(long long ray, float& ox, float& oy, float& oz, float& dx, float& dy, float& dz,
+                                               long long& out) const {
+        const long long cell = ray / N;
+        const int i = (int)(ray - cell * N);
+        const long long v = cell / cells;
+        const long long c = cell - v * cells;
+        const long long tile = c / (PT_TILE * PT_TILE);
+        const int w = (int)(c - tile * (PT_TILE * PT_TILE));
+        const int px = (int)(tile % tiles_x) * PT_TILE + w % PT_TILE, py = (int)(tile / tiles_x) * PT_TILE + w / PT_TILE;
+        if (px >= W || py >= H) return false;
+        const size_t HW = (size_t)H * W, p = (size_t)py * W + px;
+        out = ((long long)v * N + i) * (long long)HW + (long long)p;
+        if (mask && !mask[v * HW + p]) { T[out] = 0.0f; return false; }
+        const float* nb = normal + 3 * v * HW + p;
+        const float3 n = unit_normal(nb[0], nb[HW], nb[2 * HW]);
+        const float* pb = points + 3 * v * HW + p;
+        GgxFrame f{};
+        if (s.n_ggx > 0)
+            f = ggx_frame(n, sub_(campos[3 * v], pb[0]), sub_(campos[3 * v + 1], pb[HW]), sub_(campos[3 * v + 2], pb[2 * HW]),
+                          roughness[v * HW + p]);
+        float area;
+        const float3 d = importance_sample(s, (uint32_t)p, i, n, f, area);
+        dx = d.x; dy = d.y; dz = d.z;
+        ox = add_(pb[0], mul_(dx, PT_ORIGIN_OFFSET)); oy = add_(pb[HW], mul_(dy, PT_ORIGIN_OFFSET)); oz = add_(pb[2 * HW], mul_(dz, PT_ORIGIN_OFFSET));
+        return true;
+    }
+};
+
+__global__ void __launch_bounds__(PT_THREADS) bvh_pixel_importance_kernel(int P, long long num_rays, ImportancePixelRays rays,
+                                                                          const float* __restrict__ table,
+                                                                          const float4* __restrict__ packets, unsigned long long* counter) {
+    __shared__ int sStack[TRACE_STACK_SH][PT_THREADS];
+    rays.s.t = EnvTable(table);
+    trace_opacity_rays(rays, num_rays, P - 1, packets, rays.T, counter, sStack);
+}
+
 __global__ void __launch_bounds__(PT_THREADS) bvh_pixel_trace_kernel(int P, long long num_rays, PixelRays rays,
                                                                      const float4* __restrict__ packets, unsigned long long* counter) {
     __shared__ int sStack[TRACE_STACK_SH][PT_THREADS];
@@ -148,13 +195,22 @@ int r3dg_bvh_trace_pixels(const r3dg_pixel_args* a, int P, const int32_t* nodes,
     R3DG_CUDA_TRY(cudaMemsetAsync(counter, 0, 8, stream));
     const int rc = launch_bvh_pack(P, nodes, aabbs, means3D, covs3D, opacities, normals, packets, stream);
     if (rc != 0) return rc;
+    if (a->sampler_table && (a->n_env < 0 || a->n_ggx < 0 || (long long)a->N - a->n_env - a->n_ggx < 1)) return R3DG_ERR_BAD_ARG;
+    if (a->sampler_table && a->n_ggx > 0 && (!a->roughness || !a->campos)) return R3DG_ERR_BAD_ARG;
     const int tiles_x = (a->W + PT_TILE - 1) / PT_TILE, tiles_y = (a->H + PT_TILE - 1) / PT_TILE;
     const PixelRays rays{a->N, a->W, a->H, tiles_x, (long long)tiles_x * tiles_y * PT_TILE * PT_TILE, a->normal, a->points,
                          a->mask, nullptr, T};
     const long long num_rays = (long long)a->V * rays.cells * a->N;
     const long long want = (num_rays + PT_THREADS - 1) / PT_THREADS;
     const int blocks = (int)(want < (long long)num_sms() * 16 ? want : (long long)num_sms() * 16);
-    bvh_pixel_trace_kernel<<<blocks, PT_THREADS, (size_t)a->N * sizeof(float3), stream>>>(P, num_rays, rays, packets, counter);
+    if (a->sampler_table) {
+        ImportancePixelRays ir{a->N, a->W, a->H, tiles_x, rays.cells, a->normal, a->points, a->roughness, a->campos, a->mask,
+                               ImportanceSampler{}, T};
+        ir.s.T = a->sampler_transform; ir.s.N = a->N; ir.s.n_env = a->n_env; ir.s.n_ggx = a->n_ggx; ir.s.seed = a->seed;
+        bvh_pixel_importance_kernel<<<blocks, PT_THREADS, 0, stream>>>(P, num_rays, ir, a->sampler_table, packets, counter);
+    } else {
+        bvh_pixel_trace_kernel<<<blocks, PT_THREADS, (size_t)a->N * sizeof(float3), stream>>>(P, num_rays, rays, packets, counter);
+    }
     R3DG_CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -116,6 +116,21 @@ class RayTracer:
         return out
 
     @torch.no_grad()
+    def bake_importance(self, means3D, symm_inv, opacity, normals, sampler, sample_num, viewdirs=None, roughness=None):
+        """The visibility bake along importance-sampled directions (shading.EnvSampler): shading.importance_sample's
+        directions and areas for every Gaussian, then trace_visibility's T of the rays from each mean + 0.05 d
+        (r3dg_bvh_trace_opacity, the bake's hit rule).  Returns dict(visibility [P,N,1], incident_dirs [P,N,3],
+        incident_areas [P,N,1]) in bake_visibility's shapes, for `rendering_equation` under the sampler's light."""
+        from .shading import importance_sample
+        dirs, areas = importance_sample(normals, sampler, sample_num, viewdirs, roughness)
+        P, N = dirs.shape[0], dirs.shape[1]
+        if P == 0:
+            return {"visibility": torch.empty((0, N, 1), dtype=torch.float32, device=dirs.device), "incident_dirs": dirs,
+                    "incident_areas": areas}
+        _, opa = _C._trace(self.tree, self.aabb, _lib.f32(means3D), N, 0.05, dirs, means3D, symm_inv, opacity, normals)
+        return {"visibility": opa.unsqueeze(-1), "incident_dirs": dirs, "incident_areas": areas}
+
+    @torch.no_grad()
     def bake_radiance(self, means3D, symm_inv, opacity, normals, shs, sh_degree, sample_num, want_hits=False):
         """What each of the bake's rays (those of `bake_visibility`) sees of the other Gaussians, composited front to
         back in ascending (t, Gaussian index) until T < 1e-4 (r3dg_bvh_bake_radiance).  The payload `shs` [P,M,3]
@@ -183,12 +198,16 @@ class RayTracer:
         return out
 
     @torch.no_grad()
-    def trace_pixels(self, points, normals, sample_num, means3D, symm_inv, opacity, gaussian_normals, mask=None):
+    def trace_pixels(self, points, normals, sample_num, means3D, symm_inv, opacity, gaussian_normals, mask=None, sampler=None,
+                     roughness=None, campos=None):
         """Visibility T [N,H,W] (or [V,N,H,W]) of the per-pixel shading (shading.shade_pixels) through this tree
         (r3dg_bvh_trace_pixels): for every valid pixel of points / normals [3,H,W] (or [V,3,H,W]; world-space surface
         points and the rasterized normals) and sample i, trace_visibility's T of the ray from the point along the
         sampler's direction i around normalize(normal), bit for bit.  Pixels outside `mask` ([H,W] or [V,H,W], bool
-        or uint8) trace nothing and get 0.  No gradient.  A view is traced once and shaded under any number of envs."""
+        or uint8) trace nothing and get 0.  No gradient.  A view is traced once and shaded under any number of envs.
+        sampler: a shading.EnvSampler; the directions are then its directions of pixel p = y W + x as row p (those of
+        importance_sample), and roughness [1,H,W] / [V,1,H,W] and campos [3] / [V,3] are required when its mix has GGX
+        samples.  Shade the result with shading.shade_pixels(..., sampler=) and the same sampler."""
         from .shading import pixel_args
         P = means3D.shape[0]
         if not all(t.is_cuda for t in (means3D, symm_inv, opacity, gaussian_normals)):
@@ -196,6 +215,18 @@ class RayTracer:
         if means3D.shape != (P, 3) or gaussian_normals.shape != (P, 3) or symm_inv.shape != (P, 6) or opacity.numel() != P:
             raise ValueError("means3D and gaussian_normals must be [P,3], symm_inv [P,6] and opacity [P]")
         a, lead, keep = pixel_args(normals, points, sample_num, mask)
+        if sampler is not None:
+            if sampler.table.device != points.device:
+                raise ValueError(f"the sampler is on {sampler.table.device}, the images on {points.device}")
+            if sampler.fill(a, a.N) > 0:
+                if roughness is None or campos is None:
+                    raise ValueError("a sampler with GGX samples needs roughness and campos")
+                r = _lib.f32(roughness).reshape(a.V, 1, a.H, a.W)
+                cp = _lib.f32(campos).reshape(a.V, 3)
+                if r.device != points.device or cp.device != points.device:
+                    raise ValueError(f"roughness and campos must be on the images' device {points.device}")
+                a.roughness, a.campos = r.data_ptr(), cp.data_ptr()
+                keep += [r, cp]
         out = torch.empty((a.V, a.N, a.H, a.W), dtype=torch.float32, device=points.device)
         m, ci, op, nr = _lib.f32(means3D), _lib.f32(symm_inv), _lib.f32(opacity), _lib.f32(gaussian_normals)
         tmp = _lib.scratch(_lib.load().r3dg_bvh_trace_pixels_tmp_bytes(P), points.device)

@@ -215,7 +215,7 @@ _MEANS = ("mean_incident_lights", "mean_local_incident_lights", "mean_global_inc
 
 def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents, direct_light_env_light=None,
                              visibility_precompute=None, incident_dirs_precompute=None, incident_areas_precompute=None,
-                             means=False, env_filter=None):
+                             means=False, env_filter=None, sampler=None):
     """`rendering_equation` for V view directions of the same Gaussians in one call: viewdirs [V,P,3], every other input
     as in `rendering_equation`.  The incident light of each sample is evaluated once for all views.
 
@@ -229,9 +229,19 @@ def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents
     tensors.  Refused before anything is launched: V outside 1..MAX_VIEWS, viewdirs not [V,P,3], incidents not [P,16,3],
     a [V',3,3] transform with V' != V, and per-view transforms when autograd would need a backward.  env_filter: as in
     `rendering_equation`; the filtered light is evaluated once per sample for all views (per view with per-view
-    transforms)."""
+    transforms).  sampler: the EnvSampler the directions and areas came from (importance_sample or
+    RayTracer.bake_importance); the views share them, so it is refused when its mix has GGX samples (they depend on
+    the view) or with per-view transforms (the env samples follow one transform)."""
     dirs, areas, vis = incident_dirs_precompute, incident_areas_precompute, visibility_precompute
     P = dirs.shape[0]
+    if sampler is not None:
+        transform = _env_texture(direct_light_env_light)[1]
+        if sampler.counts(dirs.shape[1])[1] > 0:
+            raise ValueError("rendering_equation_views shares its directions over the views: a sampler with GGX "
+                             "samples (per-view directions) is refused; use mix=(m_env, 0, m_cos)")
+        if transform is not None and transform.dim() == 3:
+            raise ValueError("a sampler follows one env transform: per-view transforms are refused")
+        sampler.check_light(direct_light_env_light, "rendering_equation_views")
     if viewdirs.dim() != 3 or viewdirs.shape[1:] != (P, 3):
         raise ValueError(f"viewdirs must be [V,P,3] with P = {P} (got {tuple(viewdirs.shape)})")
     V = viewdirs.shape[0]
@@ -251,6 +261,99 @@ def rendering_equation_views(base_color, roughness, normals, viewdirs, incidents
     extra = {"incident_dirs": dirs, "incident_visibility": vis, "diffuse_light": diffuse, "specular": specular}
     extra.update(zip(_MEANS, outs[3:]))
     return pbr, extra
+
+
+class EnvSampler:
+    """The importance sampler of an environment light (include/r3dg_b200.h, IMPORTANCE SAMPLING): a table built once
+    from the detached activated env, the EnvLight transform it samples under, the strategy mix (env, GGX, cosine) and
+    the seed.  Refused on the host: a mix that is negative or does not sum to 1, an env with fewer than 2 rows or
+    columns, a transform that is not one orthonormal [3,3] (to 1e-4), a seed outside [0, 2^32).  The table follows
+    the env as it was at construction; rebuilding it after an env update is the caller's choice."""
+
+    def __init__(self, direct_light_env_light, mix=(0.5, 0.25, 0.25), seed=0):
+        env, transform = _env_texture(direct_light_env_light)
+        mix = tuple(float(m) for m in mix)
+        if len(mix) != 3 or not all(m >= 0 for m in mix) or abs(sum(mix) - 1.0) > 1e-6:
+            raise ValueError(f"mix must be three non-negative weights (env, ggx, cos) summing to 1, got {mix}")
+        if not 0 <= int(seed) < 2 ** 32:
+            raise ValueError(f"seed must be in [0, 2^32), got {seed}")
+        env = _lib.f32(env)
+        if env.dim() != 3 or env.shape[2] != 3 or env.shape[0] < 2 or env.shape[1] < 2:
+            raise ValueError(f"the env must be [He,We,3] with He, We >= 2, got {tuple(env.shape)}")
+        tr = None
+        if transform is not None:
+            tr = _lib.f32(transform)
+            if tr.device != env.device:
+                raise ValueError(f"the env transform must be on the env's device {env.device}, got {tr.device}")
+            if tr.shape != (3, 3):
+                raise ValueError(f"the sampler takes one [3,3] env transform, got {tuple(tr.shape)}")
+            err = float((tr.double() @ tr.double().T - torch.eye(3, dtype=torch.float64, device=tr.device)).abs().max())
+            if not err <= 1e-4:
+                raise ValueError(f"the env transform must be orthonormal to 1e-4 (|T T^T - I| = {err:.3g})")
+        if not env.is_cuda:
+            raise RuntimeError("EnvSampler builds its table on the GPU only (no CPU path)")
+        He, We = env.shape[0], env.shape[1]
+        lib = _lib.load()
+        self.table = torch.empty((lib.r3dg_env_sampler_floats(He, We),), dtype=torch.float32, device=env.device)
+        _lib.call("r3dg_env_sampler_build", env.device, env.data_ptr(), He, We, self.table.data_ptr(), what="env sampler build")
+        self.transform, self.mix, self.seed, self.env_shape = tr, mix, int(seed), (He, We)
+
+    def counts(self, N):
+        """(n_env, n_ggx, n_cos) of N samples: n_env = floor(N m_e + 1/2), n_env + n_ggx = floor(N (m_e + m_g) + 1/2).
+        Refuses a split without a cosine sample (the cosine lobe is what keeps the estimator unbiased)."""
+        N = int(N)
+        n_env = int(N * self.mix[0] + 0.5)
+        n_eg = int(N * (self.mix[0] + self.mix[1]) + 0.5)
+        if N - n_eg < 1:
+            raise ValueError(f"mix {self.mix} leaves no cosine sample of N = {N}: at least one is required")
+        return n_env, n_eg - n_env, N - n_eg
+
+    def check_light(self, direct_light_env_light, what):
+        """Refuse a light whose env size or (one [3,3]) transform differs from the sampler's: its areas would be wrong."""
+        env, transform = _env_texture(direct_light_env_light)
+        if tuple(env.shape[:2]) != self.env_shape:
+            raise ValueError(f"{what}: the light's env is {tuple(env.shape[:2])}, the sampler's {self.env_shape}")
+        if transform is not None and transform.dim() == 3:
+            return
+        same = (transform is None) == (self.transform is None) and (
+            transform is None or torch.equal(_lib.f32(transform).to(self.transform.device), self.transform))
+        if not same:
+            raise ValueError(f"{what}: the light's env transform is not the one the sampler was built with")
+
+    def fill(self, args, N):
+        """Enter the sampler into a PixelArgs record for N samples per pixel."""
+        n_env, n_ggx, _ = self.counts(N)
+        args.sampler_table, args.n_env, args.n_ggx, args.seed = self.table.data_ptr(), n_env, n_ggx, self.seed
+        args.sampler_transform = _lib.ptr(self.transform)
+        return n_ggx
+
+
+def importance_sample(normals, sampler, N, viewdirs=None, roughness=None):
+    """N importance-sampled incident directions per Gaussian row (r3dg_sample_importance_dirs): (dirs [P,N,3],
+    areas [P,N,1]), the `incident_dirs_precompute` / `incident_areas_precompute` of `rendering_equation` shaded under
+    the sampler's light.  normals [P,3]; viewdirs [P,3] and roughness [P,1] are required when the mix has GGX samples.
+    Row g's numbers are hashed with g.  No gradient."""
+    n = _lib.f32(normals).reshape(-1, 3)
+    P = n.shape[0]
+    n_env, n_ggx, _ = sampler.counts(N)
+    if n_ggx > 0 and (viewdirs is None or roughness is None):
+        raise ValueError("GGX samples need viewdirs and roughness")
+    if not n.is_cuda:
+        raise RuntimeError("importance_sample runs on the GPU only (no CPU path)")
+    if n.device != sampler.table.device:
+        raise ValueError(f"normals are on {n.device}, the sampler on {sampler.table.device}")
+    v = None if n_ggx == 0 else _lib.f32(viewdirs).reshape(-1, 3)
+    r = None if n_ggx == 0 else _lib.f32(roughness).reshape(-1)
+    if v is not None and (v.shape[0] != P or r.shape[0] != P):
+        raise ValueError(f"viewdirs and roughness must hold P = {P} rows")
+    if v is not None and (v.device != n.device or r.device != n.device):
+        raise ValueError(f"viewdirs and roughness must be on the normals' device {n.device}")
+    f = dict(dtype=torch.float32, device=n.device)
+    dirs, areas = torch.empty((P, int(N), 3), **f), torch.empty((P, int(N), 1), **f)
+    _lib.call("r3dg_sample_importance_dirs", n.device, P, int(N), _lib.ptr(n), _lib.ptr(v), _lib.ptr(r),
+              sampler.table.data_ptr(), _lib.ptr(sampler.transform), n_env, n_ggx, sampler.seed, _lib.ptr(dirs),
+              _lib.ptr(areas), what="importance_sample")
+    return dirs, areas
 
 
 def install(module=None):
@@ -310,8 +413,13 @@ class _ShadePixels(torch.autograd.Function):
     """The per-pixel shading of V views: one node with gradients to base_color, roughness, incidents and env."""
 
     @staticmethod
-    def forward(ctx, base_color, roughness, incidents, env, normal, points, campos, visibility, mask, transform, env_filter):
+    def forward(ctx, base_color, roughness, incidents, env, normal, points, campos, visibility, mask, transform, env_filter,
+                sampler=None):
         a, lead, keep = pixel_args(normal, points, visibility.shape[-3], mask)
+        if sampler is not None:
+            if sampler.table.device != normal.device:
+                raise ValueError(f"the sampler is on {sampler.table.device}, the images on {normal.device}")
+            sampler.fill(a, a.N)
         V, H, W = a.V, a.H, a.W
         b, _ = _views(base_color, 3, "base_color", lead)
         r, _ = _views(roughness, 1, "roughness", lead)
@@ -336,7 +444,7 @@ class _ShadePixels(torch.autograd.Function):
         a.pbr, a.diffuse_light, a.specular, a.mean_visibility = (t.data_ptr() for t in (pbr, diffuse, specular, mean_vis))
         _lib.call("r3dg_shade_pixels_forward", b.device, ctypes.byref(a), what="shade_pixels")
         ctx.save_for_backward(b, r, inc, e, vis, cp, tr, pyr, *keep[:2])
-        ctx.mask, ctx.lead = keep[2], lead
+        ctx.mask, ctx.lead, ctx.sampler = keep[2], lead, sampler
         ctx.mark_non_differentiable(mean_vis)
         shape = lambda t: t.reshape(lead[0] + t.shape[1:])
         return shape(pbr), shape(diffuse), shape(specular), shape(mean_vis)
@@ -350,6 +458,8 @@ class _ShadePixels(torch.autograd.Function):
         a.base_color, a.roughness, a.normal, a.points, a.campos = (t.data_ptr() for t in (b, r, n, p, cp))
         a.incidents, a.mask, a.env, a.visibility = _lib.ptr(inc), _lib.ptr(ctx.mask), e.data_ptr(), vis.data_ptr()
         a.env_transform, a.transform_per_view = _lib.ptr(tr), int(tr is not None and tr.dim() == 3)
+        if ctx.sampler is not None:
+            ctx.sampler.fill(a, a.N)
         dev = b.device
         f = dict(dtype=torch.float32, device=dev)
         g = [None if t is None else _lib.f32(t).reshape(V, 3, H, W) for t in (g_pbr, g_diffuse, g_specular)]
@@ -367,11 +477,11 @@ class _ShadePixels(torch.autograd.Function):
         det_ws = _lib.det_workspace(a, det_bytes, dev)
         _lib.call("r3dg_shade_pixels_backward", dev, ctypes.byref(a), what="shade_pixels backward")
         shape = lambda t: None if t is None else t.reshape(ctx.lead[0] + t.shape[1:])
-        return shape(d_base), shape(d_rough), shape(d_inc), d_env, None, None, None, None, None, None, None
+        return shape(d_base), shape(d_rough), shape(d_inc), d_env, None, None, None, None, None, None, None, None
 
 
 def shade_pixels(base_color, roughness, normal, points, campos, visibility, direct_light_env_light, incidents=None,
-                 mask=None, env_filter=None):
+                 mask=None, env_filter=None, sampler=None):
     """The shading step at every pixel of rasterized material images (deferred shading; include/r3dg_b200.h, PIXEL
     SHADING).  One view: base_color [3,H,W], roughness [1,H,W], normal [3,H,W] (un-premultiplied material channels),
     points [3,H,W] world-space surface points, campos [3], visibility [N,H,W] from RayTracer.trace_pixels, optional
@@ -382,8 +492,15 @@ def shade_pixels(base_color, roughness, normal, points, campos, visibility, dire
     and the formula of `rendering_equation`, so each output equals that function on the pixel as a row bit for bit.
     Returns dict(pbr, diffuse_light, specular [.., 3,H,W], visibility [.., 1,H,W] = mean_i T); masked pixels are 0.
     Gradients: base_color, roughness, incidents and the environment map; none for normal, points, campos or the
-    visibility.  env_filter: as in `rendering_equation` (None: set_env_filter's default)."""
+    visibility.  env_filter: as in `rendering_equation` (None: set_env_filter's default).
+
+    sampler: a shading.EnvSampler of this light (same env size and transform; a per-view transform is allowed, the env
+    samples then follow the sampler's).  The N samples of pixel p = y W + x are the sampler's directions of row p with
+    their areas (importance_sample of the pixels as rows), and `visibility` must be RayTracer.trace_pixels' T traced
+    with the same sampler: this call cannot tell.  The returned visibility is then mean_i T over those directions."""
     env, transform = _env_texture(direct_light_env_light)
+    if sampler is not None:
+        sampler.check_light(direct_light_env_light, "shade_pixels")
     pbr, diffuse, specular, vis = _ShadePixels.apply(base_color, roughness, incidents, env, normal, points, campos, visibility,
-                                                     mask, transform, _filter_on(env_filter))
+                                                     mask, transform, _filter_on(env_filter), sampler)
     return {"pbr": pbr, "diffuse_light": diffuse, "specular": specular, "visibility": vis}
