@@ -1247,6 +1247,63 @@ int r3dg_shade_pixel_lights_forward(const struct r3dg_pixel_light_args* args, r3
 int r3dg_shade_pixel_lights_backward(const struct r3dg_pixel_light_args* args, r3dg_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * DENOISE: a cross-bilateral a-trous wavelet filter (Dammertz et al. 2010, the spatial filter of SVGF) over
+ * planar images of the PIXEL SHADING layout (DESIGN.md §4.32), for per-pixel shading at few samples.  Its
+ * edge-stopping weights come from the G-buffer guides only, never from the signal, so the filter is linear
+ * in the image, y = A(guides) x, and the backward is the exact transpose A^T g.
+ *   Inputs: x f32[V,C,H,W], 1 <= C <= R3DG_DENOISE_MAX_CHANNELS, 1 <= V <= R3DG_MAX_VIEWS; guides of the same
+ *   views and size: normal [V,3,H,W] (un-premultiplied, any length), points [V,3,H,W] (world-space surface
+ *   points), mask u8[V,H,W] or NULL (pixel p of view v is valid when mask is NULL or mask[v,p] != 0) and
+ *   features [V,F,H,W], 0 <= F <= R3DG_DENOISE_MAX_FEATURES (NULL when F = 0).
+ *   Unit normal: n^ = n / max(sqrt((x*x + y*y) + z*z), 1e-12) (F.normalize; a zero normal stays zero).
+ *   Pass k = 0 .. L-1, 1 <= L <= R3DG_DENOISE_MAX_PASSES, step s = 2^k, y_0 = x, y_L = y:
+ *     y_{k+1}(p) = sum_o w(p, p + s o) y_k(p + s o) / W_k(p),  W_k(p) = sum_o w(p, p + s o),  o in {-2..2}^2
+ *   (taps in row-major order of o).  For q = p + s o != p:
+ *     w(p,q) = h(o_x) h(o_y) w_n w_x w_f,  h = (1, 4, 6, 4, 1) / 16,
+ *     w_n = min(max(n^_p . n^_q, 0), 1)^sigma_normal,
+ *     w_x = exp(-t / sigma_plane),  t = |n^_p . (x_q - x_p)| / |x_q - x_p|  (t = 0 when x_q = x_p): the sine of the
+ *           offset's angle out of p's tangent plane, free of world and image scale, near 1 across a depth step,
+ *     w_f = exp(-|f_p - f_q|^2 / sigma_features^2);
+ *   the centre tap (o = 0) weighs exactly h(0)^2 = 9/64, so W_k(p) > 0 on every valid pixel.  Taps outside the
+ *   image or on invalid pixels weigh 0 and are not read.  Invalid pixels output 0, get gradient 0, and their
+ *   values of x (and of the guides) change no output bit.  The kernels evaluate w_n w_x w_f as one
+ *   exp2(sigma_normal log2 c - (t / sigma_plane + |df|^2 / sigma_features^2) log2 e), without FMA contraction.
+ *   Backward (the transpose): with g_L = dL_dy and g^ = g_{k+1} / W_k (the forward's 1 / W_k, kept in `work`),
+ *     g_k(q) = sum_o w(q - s o, q) g^(q - s o),  dL_dx = g_0,
+ *   each weight recomputed by the forward's function from the same records, so bit for bit the forward's: a
+ *   gather with no atomics, bitwise reproducible.  No gradient to the guides.
+ *   Work (r3dg_denoise_work_bytes): the forward packs each pixel's unit normal, validity, point and features
+ *   once into float4 records (2 + ceil((F - 1) / 4) planes), stores 1 / W_k of every pass and ping-pongs
+ *   through one [V,C,H,W] image; the backward reads the records and 1 / W_k a forward with the same V, H, W,
+ *   C, F and L left in `work`, and uses the same image.  x must not alias y, nor dL_dy alias dL_dx.
+ *   Launches: forward 1 + L, backward L.  Each view's outputs equal a one-view call's bit for bit.
+ *   Refusals before any launch: R3DG_ERR_BAD_ARG for V outside 1..R3DG_MAX_VIEWS, H or W < 1, C, F or L out of
+ *   range, a sigma <= 0 or not finite, a NULL pointer the call needs, or a missing or short work;
+ *   R3DG_ERR_UNSUPPORTED for V H W max(C, F) >= 2^31 (the kernels index in 32 bits).
+ * ------------------------------------------------------------------------------------------ */
+#define R3DG_DENOISE_MAX_CHANNELS 8
+#define R3DG_DENOISE_MAX_FEATURES 8
+#define R3DG_DENOISE_MAX_PASSES 6
+struct r3dg_denoise_args {
+    int V, H, W, C, F, L;
+    float sigma_normal, sigma_plane, sigma_features;
+    const float* normal;          /* forward: [V,3,H,W] (no gradient) */
+    const float* points;          /* forward: [V,3,H,W] world-space surface points */
+    const uint8_t* mask;          /* forward: [V,H,W] or NULL */
+    const float* features;        /* forward: [V,F,H,W], NULL when F = 0 */
+    const float* x;               /* forward: [V,C,H,W] */
+    float* y;                     /* forward: [V,C,H,W] */
+    const float* dL_dy;           /* backward: [V,C,H,W] */
+    float* dL_dx;                 /* backward: [V,C,H,W] */
+    void* work;                   /* r3dg_denoise_work_bytes; the backward reads what the forward wrote */
+    size_t work_bytes;
+};
+
+size_t r3dg_denoise_work_bytes(int V, int H, int W, int C, int F, int L);
+int r3dg_denoise_forward(const struct r3dg_denoise_args* args, r3dg_stream_t stream);
+int r3dg_denoise_backward(const struct r3dg_denoise_args* args, r3dg_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * DETERMINISTIC MODE.  With `deterministic` set in r3dg_raster_fwd_args, r3dg_raster_bwd_args or
  * r3dg_shade_args, the three sums that float atomics make depend on the order in which warps finish
  * are accumulated in fixed point instead (csrc/detacc.cuh): out_weights of the forward, the

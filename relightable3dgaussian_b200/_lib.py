@@ -125,6 +125,13 @@ class PixelLightArgs(ctypes.Structure):
                 [("work_bytes", c_size_t)])
 
 
+class DenoiseArgs(ctypes.Structure):
+    _fields_ = ([(n, c_int) for n in ("V", "H", "W", "C", "F", "L")] +
+                [(n, c_float) for n in ("sigma_normal", "sigma_plane", "sigma_features")] +
+                [(n, c_void_p) for n in ("normal", "points", "mask", "features", "x", "y", "dL_dy", "dL_dx", "work")] +
+                [("work_bytes", c_size_t)])
+
+
 class ComposeArgs(ctypes.Structure):
     _fields_ = ([(n, c_int) for n in ("P", "K")] +
                 [(n, c_void_p) for n in ("offsets", "quat", "translation", "scale", "xyz", "normal", "rotation", "scaling")] +
@@ -239,6 +246,10 @@ SYMBOLS = [
     ("r3dg_shade_pixel_lights_work_bytes", c_size_t, [c_int, c_int, c_int, c_int]),
     ("r3dg_shade_pixel_lights_forward", c_int, [c_void_p, c_void_p]),
     ("r3dg_shade_pixel_lights_backward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_denoise_work_bytes", c_size_t, [c_int] * 6),
+    # `const struct r3dg_denoise_args*`: pass ctypes.byref(DenoiseArgs(...))
+    ("r3dg_denoise_forward", c_int, [c_void_p, c_void_p]),
+    ("r3dg_denoise_backward", c_int, [c_void_p, c_void_p]),
     ("r3dg_compose_work_bytes", c_size_t, [c_int, c_int]),
     # `const struct r3dg_compose_args*`: pass ctypes.byref(ComposeArgs(...))
     ("r3dg_compose_forward", c_int, [c_void_p, c_void_p]),

@@ -18,11 +18,12 @@ FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
 # shading.cu (and pixel_shading.cu, lights.cu and pixel_lights.cu, which share its per-sample and GGX code in shading_eval.cuh and brdf.cuh) mirrors a chain of separate PyTorch elementwise kernels (each op rounded on its own);
 # without FMA contraction the fused kernel reproduces that rounding instead of a differently
 # (if slightly better) rounded result of an ill-conditioned GGX denominator.
+# denoise.cu: the backward recomputes each of the forward's weights, and must round it alike in another kernel.
 # adam.cu: flush-to-zero arithmetic.  Real gradients span the whole fp32 range (g^2 of a barely visible Gaussian is a
 # denormal); IEEE sqrt / division take a slow subroutine for denormal operands, and one such lane stalls its warp.
 # With -ftz the results are unchanged for every normal number (torch's own CUDA kernels are compiled the same way).
 PER_FILE_FLAGS = {"shading.cu": ["-fmad=false"], "pixel_shading.cu": ["-fmad=false"], "lights.cu": ["-fmad=false"],
-                  "pixel_lights.cu": ["-fmad=false"], "adam.cu": ["-ftz=true"]}
+                  "pixel_lights.cu": ["-fmad=false"], "denoise.cu": ["-fmad=false"], "adam.cu": ["-ftz=true"]}
 
 
 def sources():
